@@ -2,7 +2,7 @@
 """bench.py -- BASELINE.json's metric: scan-pairs/s (overlap + yaw) of the 1-query-vs-N-candidate
 loop-closure search at 64x900, on synthetic KITTI-shaped data.
 
-  python bench.py --gpus N --steps K --warmup W            # this repo's B200 path
+  python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (H100, sm_90a)
   python bench.py --impl reference --steps K --warmup W    # the CPU port of the reference, host cores
   (N > 1: python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...)
 
@@ -21,9 +21,12 @@ The same JSON line carries the other BASELINE configs as extra objects (each mea
   "bank4541"       config 4  4541-volume bank SHARDED over the N ranks (strong scaling)
   "all_pairs"      config 5  rows of the 4541 x 4541 ordered pair matrix + streamed raw-cloud encode
   "range_proj"               batched projection + normals (Mpts/s, GB/s against the measured HBM peak)
-`roofline` = k_delta_conv1_tc (the dominant kernel) against the measured bf16 tensor peaks (burst and
-sustained); `cpu_baseline` = the oracle port of the reference graph on a bounded sample, whose float64
+`roofline` = k_delta_conv1_mma (the dominant kernel) against the fp16 tensor peak (MEASURED_PEAKS.json when
+present, else the H100 SXM data sheet); `cpu_baseline` = the oracle port of the reference graph on a bounded sample, whose float64
 twin also spot-checks the timed GPU output in-run (`parity_check`).
+--dump-outputs DIR writes what the timed path returned in its last step (rank 0's overlaps and yaws of the
+1101 candidates) as DIR/overlap.npy (float32) and DIR/yaw.npy (float64), for output-for-output comparisons
+of two builds: every input is generated from fixed seeds.
 """
 import argparse
 import json
@@ -50,6 +53,7 @@ FLOP_LEG_C4 = 2 * 866611072
 FLOP_LEG_C25 = 2 * 1201519072
 METRIC = 'scan-pairs/sec (overlap+yaw) at 64x900'
 WORKLOAD = '1 query x 1101 candidates per GPU, geo-only 64x900 (BASELINE config 2)'
+CALIB_PAIRS = 16                  # oracle pairs that set the Dense rescale
 LOGIT_SPREAD = 1.5                # the Dense layer is rescaled so that the bank's logits have this std (parity_check)
 
 
@@ -63,6 +67,7 @@ def parse():
   ap.add_argument('--cpu-pairs', type=int, default=8, help='pairs per step in the CPU sample')
   ap.add_argument('--transport', default='auto', choices=['auto', 'symm', 'collective'])
   ap.add_argument('--no-extras', action='store_true', help='only the headline config (fast)')
+  ap.add_argument('--dump-outputs', metavar='DIR', help='write the last timed step\'s outputs as DIR/<name>.npy')
   return ap.parse_args()
 
 
@@ -73,11 +78,12 @@ def peaks():
       d = json.load(f)
     return {'burst': d.get('bf16_tflops'), 'sustained': d.get('bf16_tflops_sustained'), 'hbm': d.get('hbm_gbs'),
             'source': 'measured (MEASURED_PEAKS.json)'}
-  return {'burst': 1590.0, 'sustained': 1400.0, 'hbm': 6650.0, 'source': 'fallback (B200_PROFILING.md)'}
+  return {'burst': 989.0, 'sustained': 989.0, 'hbm': 3350.0,
+          'source': 'H100 SXM data sheet (dense fp16 / bf16, 700 W), not measured'}
 
 
 class ClockSampler(threading.Thread):
-  """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+  """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
 
   def __init__(self, index=0):
     super().__init__(daemon=True)
@@ -170,6 +176,12 @@ def cpu_extrapolate(samples, n_pairs):
                            't_step_1101_s': t_step}
 
 
+def synth_bank_rows(rank, n):
+  """The first n rows of rank `rank`'s bank as built by main() (n <= N_SRC_SCANS: roll 0), on the host."""
+  from overlapnet_b200 import synth
+  return synth.feature_volumes(1000 * rank + 7, N_SRC_SCANS)[:n, 0]
+
+
 def synth_bank_np(n, seed=7):
   from overlapnet_b200 import synth
   return synth.feature_volumes(seed, n)[:, 0]
@@ -206,7 +218,7 @@ def run_reference(args):
   }))
 
 
-# ---- the B200 path ---------------------------------------------------------------------------------------
+# ---- the GPU path ----------------------------------------------------------------------------------------
 def rolled_bank(eng, fv_src, n, dev):
   src = torch.arange(n, device=dev) % fv_src.shape[0]
   roll = (torch.arange(n, device=dev) // fv_src.shape[0]) * 7
@@ -264,24 +276,20 @@ def main():
                max_batch_pairs=N_CAND)
   eng.load_weights(w)
 
-  # ---- candidate bank of this rank: 32 synthetic scans encoded by the product path, yaw-rolled to 1101
+  # ---- candidate bank of this rank: 32 seeded synthetic feature volumes, yaw-rolled to 1101.  Every input
+  # (bank, query clouds, weights) comes from fixed seeds and host code, so two builds run the same problem.
   clouds = [synth.kitti_like_cloud(1000 * rank + s) for s in range(N_SRC_SCANS)]
-  cloud_batch = eng.upload_clouds(clouds)
-  fv_src = eng.leg(eng.preprocess(cloud_batch))
+  cloud_batch = eng.upload_clouds(clouds)                     # the streamed-encode and projection extras
+  fv_src = torch.from_numpy(synth.feature_volumes(1000 * rank + 7, N_SRC_SCANS)[:, 0]).to(dev)
   bank = rolled_bank(eng, fv_src, N_CAND, dev)
   # query clouds: a fresh scan per step (pinned host copies for the e2e leg); the same on every rank
   n_q = 4
   q_np = [synth.kitti_like_cloud(50000 + s) for s in range(n_q)]
   q_host = [torch.from_numpy(q).pin_memory() for q in q_np]
   q_dev = [eng.upload_clouds([q]) for q in q_np]
-  # Dense layer rescaled from a first pass of the product path (logit spread 1.5 over this bank)
-  ov0, _, _ = eng.heads_1vsN(bank, eng.leg(eng.preprocess(q_dev[0]))[0], n_cand=N_CAND)
-  eng.check()
-  ov0 = ov0.cpu().numpy()
-  if world > 1:                                             # every rank must run the same weights
-    t0 = torch.from_numpy(ov0).to(dev)
-    dist.broadcast(t0, 0)
-    ov0 = t0.cpu().numpy()
+  # Dense layer rescaled by the float64 oracle (logit spread 1.5 over rank 0's first candidates and query 0):
+  # the same weights for every build and every rank
+  ov0 = cpu_sample(w, synth_bank_rows(0, CALIB_PAIRS), q_np[0], CALIB_PAIRS, dtype=torch.float64)['ov']
   w = spread_dense(w, ov0)
   eng.load_weights(w)
   eng.bank_prepare(bank)          # the candidate bank is static: keep its tensor-core operand copies resident
@@ -335,6 +343,10 @@ def main():
   gpu_ov = last['res'][0][:N_CAND].cpu().numpy() if rank == 0 else None     # rank 0's own shard of the last timed step
   gpu_yaw = last['res'][1][:N_CAND].cpu().numpy() if rank == 0 else None
   last_q = (args.steps - 1) % n_q if args.steps else 0
+  if rank == 0 and args.dump_outputs:
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    np.save(os.path.join(args.dump_outputs, 'overlap.npy'), gpu_ov.astype(np.float32))
+    np.save(os.path.join(args.dump_outputs, 'yaw.npy'), gpu_yaw.astype(np.float64))
   # ---- timed region 2: end to end through the host-buffer entry point
   ms_e2e = timed(step_e2e, args.steps, args.warmup)
   clocks = sampler.stop() if sampler else None
@@ -375,12 +387,6 @@ def main():
               'overlap_range_checked': [float(chk['ov'].min()), float(chk['ov'].max())],
               'checker': 'oracle float64 on the first %d candidates of the last timed step (query scan %d)'
                          % (args.cpu_pairs, last_q)}
-    traffic = None
-    tp = os.path.join(ROOT, 'profiles', 'r2_delta_traffic.json')
-    if os.path.exists(tp) and args.precision == 'f16_tc':
-      with open(tp) as f:
-        tj = json.load(f)
-      traffic = (tj['dram_bytes_read'] + tj['dram_bytes_write']) * N_CAND / tj['pairs_per_launch']
     line = {
         'metric': METRIC, 'value': value, 'unit': 'pairs/s', 'n_gpus': world, 'steps': args.steps,
         'warmup': args.warmup, 'ms_per_step': ms / args.steps, 'higher_is_better': True, 'scaling': 'weak',
@@ -389,19 +395,19 @@ def main():
                    'l2': 'inputs larger than L2: the fp32 candidate bank is 203 MB per step',
                    'parallelism': 'bank sharded x%d; transport: %s' % (world, transport),
                    'precision': args.precision,
-                   'weights': 'seeded Glorot (no pretrained weights offline), Dense rescaled to logit spread %.1f' % LOGIT_SPREAD},
+                   'weights': 'seeded Glorot (no pretrained weights offline), Dense rescaled to logit spread %.1f by the float64 '
+                              'oracle' % LOGIT_SPREAD},
         'gpu_launches': int(launches),
         'e2e': {'value': e2e, 'unit': 'pairs/s', 'ms_per_step': ms_e2e / args.steps,
                 'h2d_bytes_per_step': int(q_host[0].numel() * 4),
                 'd2h_bytes_per_step': int(N_CAND * 8 * world)},
-        'roofline': {'kernel': 'k_delta_conv1_tc' if args.precision == 'f16_tc' else 'k_simt_gemm<DeltaOperand>',
+        'roofline': {'kernel': 'k_delta_conv1_mma' if args.precision == 'f16_tc' else 'k_simt_gemm<DeltaOperand>',
                      'bound': 'tensor', 'achieved': ach, 'peak': pk['burst'], 'unit': 'TFLOP/s',
                      'frac': (ach / pk['burst']) if ach else None,
                      'frac_burst': (ach / pk['burst']) if ach else None,
                      'frac_sustained': (ach / pk['sustained']) if ach else None,
                      'peak_burst': pk['burst'], 'peak_sustained': pk['sustained'],
-                     'peak_note': 'the kernel is timed inside a ~60 ms region at full clock: the burst peak applies',
-                     'traffic': traffic, 'peak_source': pk['source'],
+                     'peak_source': pk['source'],
                      'flop_per_launch': N_CAND * FLOP_DELTA_CONV1, 'avg_launch_ms': k_ms / max(k_n, 1),
                      'share_of_step': shares},
         'whole_path_tflops': pairs * FLOP_PAIR / 1e12 / (ms * 1e-3),
@@ -439,15 +445,15 @@ def measure_extras(args, eng, w, dev, rank, world, local, timed, q_dev, q_host, 
       eng.heads(fv, li, ri)
     eng.bank_release(None)
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    for i in range(5):
+    for i in range(args.warmup):
       one_pair(i)
     torch.cuda.synchronize()
     a.record()
-    for i in range(50):
+    for i in range(args.steps):
       one_pair(i)
     b.record()
     torch.cuda.synchronize()
-    ms1 = a.elapsed_time(b) / 50
+    ms1 = a.elapsed_time(b) / args.steps
     # same work replayed from a CUDA graph (launch-bound chain of ~40 small kernels)
     ms1_graph = None
     try:
@@ -461,11 +467,11 @@ def measure_extras(args, eng, w, dev, rank, world, local, timed, q_dev, q_host, 
           one_pair(0)
       torch.cuda.synchronize()
       a.record()
-      for i in range(50):
+      for i in range(args.steps):
         g.replay()
       b.record()
       torch.cuda.synchronize()
-      ms1_graph = a.elapsed_time(b) / 50
+      ms1_graph = a.elapsed_time(b) / args.steps
     except Exception as e:                                   # capture is an optimisation, never a requirement
       ms1_graph = None
       out['latency_1pair_graph_error'] = repr(e)[:200]
@@ -482,23 +488,23 @@ def measure_extras(args, eng, w, dev, rank, world, local, timed, q_dev, q_host, 
     eng.profile_enable(True)
     for k in ('project_scatter', 'project_gather'):
       eng.profile_read(k)
-    for i in range(3):
+    for i in range(args.warmup):
       proj(i)
     for k in ('project_scatter', 'project_gather'):
       eng.profile_read(k)
-    for i in range(10):
+    for i in range(args.steps):
       proj(i)
     ps, pg = eng.profile_read('project_scatter'), eng.profile_read('project_gather')
     eng.profile_enable(False)
     n_scans = cloud_batch.n
     npts = int(cloud_batch.offsets_host[-1])
-    ms_p = (ps[0] + pg[0]) / 10
+    ms_p = (ps[0] + pg[0]) / args.steps
     byts = npts * 16 + n_scans * 64 * 900 * 16
     out['range_proj'] = {'scans_per_launch': n_scans, 'points': npts, 'ms_per_launch': ms_p,
                          'mpts_per_s': npts / (ms_p * 1e-3) / 1e6, 'algorithmic_bytes': byts,
                          'gb_per_s': byts / (ms_p * 1e-3) / 1e9, 'hbm_peak_gb_per_s': pk['hbm'],
                          'frac_of_hbm_peak': byts / (ms_p * 1e-3) / 1e9 / pk['hbm'],
-                         'kernels_ms': {'scatter': ps[0] / 10, 'gather_normals_pack': pg[0] / 10},
+                         'kernels_ms': {'scatter': ps[0] / args.steps, 'gather_normals_pack': pg[0] / args.steps},
                          'note': 'fused projection + normals + channel packing of %d clouds in one launch pair; '
                                  'bytes = 16 B/point read once + 16 B/pixel written once (SURVEY 8d)' % n_scans}
 
@@ -510,16 +516,16 @@ def measure_extras(args, eng, w, dev, rank, world, local, timed, q_dev, q_host, 
       eng25.load_weights(make_weights(25))
       x_small = torch.from_numpy(synth.range_like_images(5, 8, 25)).to(dev)
       x25 = x_small.repeat(32, 1, 1, 1)                      # 256 scans, 1.47 GB of NHWC input (> L2)
-      for i in range(2):
+      for i in range(args.warmup):
         eng25.leg(x25)
       torch.cuda.synchronize()
       a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
       a.record()
-      for i in range(5):
+      for i in range(args.steps):
         eng25.leg(x25)
       b.record()
       torch.cuda.synchronize()
-      ms3 = a.elapsed_time(b) / 5
+      ms3 = a.elapsed_time(b) / args.steps
       tf = 256 * FLOP_LEG_C25 / 1e12 / (ms3 * 1e-3)
       out['leg_batch256'] = {'workload': 'BASELINE config 3: 4-cue C=25 64x900 input, batch-256 leg encode',
                              'ms_per_batch': ms3, 'scans_per_s': 256 / (ms3 * 1e-3), 'tflops': tf,
@@ -550,8 +556,8 @@ def measure_extras(args, eng, w, dev, rank, world, local, timed, q_dev, q_host, 
       eng.heads_1vsN(big, qfv, n_cand=N_BANK4)
     else:
       ss4.query(qfv)
-  k4 = max(3, min(10, args.steps))
-  ms4 = timed(step4, k4, 2)
+  k4 = args.steps
+  ms4 = timed(step4, k4, args.warmup)
   eng.check()
   if rank == 0:
     out['bank4541'] = {'workload': 'BASELINE config 4: 1 query x 4541-volume bank sharded over %d GPU(s), shard sizes %s '
@@ -569,7 +575,7 @@ def measure_extras(args, eng, w, dev, rank, world, local, timed, q_dev, q_host, 
   def encode32(i):
     stage.copy_(host_clouds, non_blocking=True)
     eng.leg(eng.preprocess(CloudBatch(stage, offs_dev, offs_host)))
-  ms_enc = timed(encode32, 5, 2) / 5
+  ms_enc = timed(encode32, args.steps, args.warmup) / args.steps
   # (b) rows of the ordered pair matrix: every rank holds the whole bank (one all_gather in a real run;
   #     here the shards are re-generated locally) and scores ROWS rows against all 4541 volumes
   eng.bank_release(None)
@@ -582,7 +588,7 @@ def measure_extras(args, eng, w, dev, rank, world, local, timed, q_dev, q_host, 
 
   def rows_step(i):
     eng.heads_rows_vs_bank(full, r_lo, r_lo + rows)
-  ms_rows = timed(rows_step, 3, 1) / 3
+  ms_rows = timed(rows_step, args.steps, args.warmup) / args.steps
   eng.check()
   t_ag = None
   lo, hi = shard_range(N_BANK4, rank, world)
@@ -594,7 +600,7 @@ def measure_extras(args, eng, w, dev, rank, world, local, timed, q_dev, q_host, 
 
     def ag(i):
       dist.all_gather(parts, pad)
-    t_ag = timed(ag, 3, 1) / 3
+    t_ag = timed(ag, args.steps, args.warmup) / args.steps
     del parts, pad, shard
   if rank == 0:
     per_rank_rows = (N_BANK4 + world - 1) // world

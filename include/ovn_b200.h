@@ -1,5 +1,5 @@
 /*
- * ovn_b200.h -- C ABI of the Blackwell-native OverlapNet inference hot path (libovn_b200.so).
+ * ovn_b200.h -- C ABI of the Hopper-native (sm_90a) OverlapNet inference hot path (libovn_b200.so).
  *
  * The reference (PRBonn/OverlapNet) has no FFI / plugin interface: its boundary is the Python
  * class `Infer` (src/two_heads/infer.py:22-265) plus the NumPy preprocessing functions
@@ -38,14 +38,14 @@ typedef enum ovn_status {
   OVN_ERR_BAD_CONFIG = -2,     /* unsupported model wiring (config/network.yml:64-82) */
   OVN_ERR_WEIGHTS = -3,        /* unknown layer name / wrong shape / weights not finalised */
   OVN_ERR_CUDA = -4,           /* a CUDA runtime call failed; see ovn_last_error */
-  OVN_ERR_NO_DEVICE = -5,      /* no sm_100 device: the library has NO CPU fallback */
+  OVN_ERR_NO_DEVICE = -5,      /* no sm_90 device: the library has NO CPU fallback */
   OVN_ERR_CAPACITY = -6        /* batch larger than the workspace reserved at ovn_create */
 } ovn_status;
 
 /* Arithmetic of the network kernels. */
 typedef enum ovn_precision {
   OVN_PREC_FP32 = 0,           /* fp32 SIMT kernels (verification path) */
-  OVN_PREC_F16_TC = 1          /* fp16 operands, fp32 accumulate in TMEM, tcgen05 tensor cores */
+  OVN_PREC_F16_TC = 1          /* fp16 (hi/lo split) operands, fp32 accumulate, tensor cores */
 } ovn_precision;
 
 /*
@@ -218,7 +218,7 @@ int ovn_peer_wait(ovn_handle* h, const int32_t* d_flags, int32_t n, int32_t skip
 /* ---- feature centre of the tensor-core delta head ------------------------------------------------
  * DeltaLayer only sees |l - r| (generateNet.py:59), which is invariant to a common per-channel offset:
  * the fp16 operand copies of the volumes are stored as fp16(x - mu[c]), which shrinks their rounding
- * error (measured: 3x on leg outputs, profiles/r2_precision_budget.txt).  mu is calibrated automatically
+ * error (3x on leg outputs in a float64 emulation of the rounding, tools/precision_study.py).  mu is calibrated automatically
  * on the first volume the handle sees (first ovn_bank_prepare row, else the first RIGHT volume) and
  * then frozen until ovn_finalize_weights; ovn_set_feature_center(h, mu[128]) fixes it explicitly
  * (NULL = back to automatic; not allowed while a bank is resident).  No effect for precision fp32. */

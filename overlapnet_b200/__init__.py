@@ -1,4 +1,4 @@
-"""overlapnet_b200 -- Blackwell-native (sm_100a) OverlapNet inference hot path.
+"""overlapnet_b200 -- Hopper-native (sm_90a) OverlapNet inference hot path.
 
 Public surface mirrors the reference (PRBonn/OverlapNet):
   Infer                         src/two_heads/infer.py:22

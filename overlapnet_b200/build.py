@@ -1,4 +1,4 @@
-"""In-tree build of libovn_b200.so (nvcc, sm_100a only).  The built .so is git-ignored but ships
+"""In-tree build of libovn_b200.so (nvcc, sm_90a only).  The built .so is git-ignored but ships
 with the repo snapshot to the GPU box; nothing is JIT-compiled at import time."""
 import os
 import subprocess
@@ -8,10 +8,9 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libovn_b200.so')
-PROBE = os.path.join(HERE, 'umma_probe')
 SOURCES = ['api.cu', 'projection.cu', 'gt_overlap.cu', 'network_fp32.cu', 'network_tc.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
-              '-Xcompiler', '-fPIC'] + os.environ.get('OVN_NVCC_EXTRA', '').split()      # e.g. -DOVN_K4_ROT=0 for A/B timing
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
+              '-Xcompiler', '-fPIC'] + os.environ.get('OVN_NVCC_EXTRA', '').split()
 
 
 def _newer(target, deps):
@@ -22,7 +21,7 @@ def _newer(target, deps):
 
 
 def build(force=False, verbose=False):
-  """Compile every CUDA source for sm_100a into overlapnet_b200/libovn_b200.so."""
+  """Compile every CUDA source for sm_90a into overlapnet_b200/libovn_b200.so."""
   nvcc = os.environ.get('NVCC', 'nvcc')
   srcs = [os.path.join(CSRC, s) for s in SOURCES]
   deps = srcs + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(('.cuh', '.h'))]
@@ -45,11 +44,6 @@ def build(force=False, verbose=False):
     with ThreadPoolExecutor(max_workers=len(srcs)) as ex:
       objs = list(ex.map(compile_one, srcs))
     subprocess.check_call([nvcc] + NVCC_FLAGS + ['-shared', '-o', LIB] + objs)
-  # standalone known-answer / rate probes of the tcgen05 building blocks (tools, not linked into the library)
-  for name in ('umma_probe', 'cta2_probe', 'ss_rate_probe'):
-    probe_src, probe_bin = os.path.join(CSRC, name + '.cu'), os.path.join(HERE, name)
-    if os.path.exists(probe_src) and (force or _newer(probe_bin, [probe_src] + deps)):
-      subprocess.check_call([nvcc] + NVCC_FLAGS + ['-o', probe_bin, probe_src])
   return LIB
 
 

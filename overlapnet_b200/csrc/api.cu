@@ -1,6 +1,6 @@
 // api.cu -- the C ABI declared in include/ovn_b200.h: handle lifetime, weights, stage dispatch
 // and the host-buffer convenience entry points.  No CPU fallback exists anywhere in this library:
-// without an sm_100 device ovn_create fails with OVN_ERR_NO_DEVICE.
+// without an sm_90 (Hopper) device ovn_create fails with OVN_ERR_NO_DEVICE.
 #include "common.cuh"
 #include <math.h>
 #include <string.h>
@@ -86,7 +86,7 @@ int check_device_error(ovn_handle* h, cudaStream_t s) {
   if (e == kErrRowNotPrepared)
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "resident bank: an indexed row was never passed to ovn_bank_prepare");
   if (e == 950) OVN_SET_ERR(h, OVN_ERR_CUDA, "ovn_peer_wait timed out: a peer rank never signalled");
-  OVN_SET_ERR(h, OVN_ERR_CUDA, "tensor-core pipeline barrier timed out (code %d); outputs of the call are poisoned (NaN / INT32_MIN)", e);
+  OVN_SET_ERR(h, OVN_ERR_CUDA, "tensor-core pipeline failed (code %d: barrier time-out or injected fault); outputs of the call are poisoned (NaN / INT32_MIN)", e);
 }
 
 }  // namespace ovn
@@ -164,8 +164,8 @@ int ovn_create(const ovn_config* cfg, ovn_handle** out) {
   CREATE_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   CREATE_CUDA(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10)
-    CREATE_FAIL(OVN_ERR_NO_DEVICE, "ovn_create: device %d is sm_%d%d; this build targets sm_100a only", dev,
+  if (prop.major != 9 || prop.minor != 0)
+    CREATE_FAIL(OVN_ERR_NO_DEVICE, "ovn_create: device %d is sm_%d%d; this build targets sm_90a only", dev,
                 prop.major, prop.minor);
   h = new ovn_handle();
   h->cfg = *cfg;

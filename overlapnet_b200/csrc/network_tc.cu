@@ -1,78 +1,44 @@
-// network_tc.cu -- tensor-core (tcgen05 / TMEM / bulk-async-copy) path of the two heads.
+// network_tc.cu -- tensor-core path (precision f16_tc) of the leg and the two heads, for Hopper (sm_90a).
 //
-// Replaces: DeltaLayer + c_conv1 (generateNet.py:15-61,96-100)      -> k_delta_conv1_tc
-//           c_conv2 (+ReLU) (generateNet.py:102-105)                -> k_conv2_sw_tc
-//           c_conv3 (+ReLU), Flatten + Dense(1, sigmoid) (:107-114) -> k_conv3_pair_tc (CTA pairs; k_conv3_resident_tc = the
-//                                                                      single-CTA A/B twin) + k_dense_finalize
-//           NormalizedCorrelation2D + argmax (:117-143, infer.py)   -> k_corr_tc + k_corr_finalize
-//           leg Conv2D stack (generateNet.py:149-230)               -> k_leg_layer1_small + k_leg_resident_tc (1-2 scans);
-//                                                                      batched: k_input_to_parity_planes (layer-1 input
-//                                                                      as even / odd column planes) + k_leg_batched_tc for
-//                                                                      every layer (hi | lo weights stacked along N)
+// Replaces: DeltaLayer + c_conv1 (generateNet.py:15-61,96-100)      -> k_delta_conv1_wgmma
+//           c_conv2 (+ReLU) (generateNet.py:102-105)                -> k_conv2_mma
+//           c_conv3 (+ReLU), Flatten + Dense(1, sigmoid) (:107-114) -> k_conv3_mma + k_dense_finalize
+//           NormalizedCorrelation2D + argmax (:117-143, infer.py)   -> k_corr_mma + k_corr_finalize
+//           leg Conv2D stack (generateNet.py:149-230)               -> layer 1: k_leg_layer1_small (1-2 scans) /
+//                                                                      k_leg_layer1_direct (batches), SIMT fp32;
+//                                                                      layers 2..: k_leg_mma
 //
-// k_delta_conv1_tc (the kernel that decides scan-pairs/s; 83 % of the FLOPs of a pair)
-//   GEMM view per pair:  o1[(i, jb), o] = sum_{dj<15, c<128} |L[i,c] - R[15 jb + dj, c]| W1[dj, c, o]
-//   M = 360 x 24, N = 64, K = 1920.  The A operand (66 MB per pair in the reference) is never
-//   materialised: 12 producer warps synthesise |l - r| as packed fp16 straight into TENSOR MEMORY
-//   (tcgen05.st), one warp's elected lane issues tcgen05.mma in TS mode (A from TMEM, B = W1
-//   slice from shared memory), accumulators (3 row tiles x 64 fp32 columns) live in TMEM.
-//   Mapping: TMEM lane = LEFT row i (3 tiles: i0 = 0, 128, 256); a thread keeps its three LEFT
-//   rows' current 32 channels in registers and reads the RIGHT row by broadcast LDS, so each
-//   synthesised element costs ~1 ALU instruction.  W1 (245 KB fp16) is streamed in 24 KB groups
-//   (cp.async.bulk + mbarrier) through a ring recycled by tcgen05.commit.
-//   Roofline: tensor pipe (co-limited by operand synthesis, DESIGN.md section 4).
-//
-// SS-mode GEMM kernels: operands in shared memory either as C8-interleaved planes
-//   [channel/8][row][8] (16-byte core-matrix rows at uniform pitch, SWIZZLE_NONE descriptors; a row
-//   shift of the descriptor start address is a convolution tap) or as SWIZZLE_128B tiles
-//   [128 rows][64 K] (k_conv2_sw_tc: o1 is written by k_delta_conv1_tc already in that image).
+// Every GEMM runs on warp-level tensor-core MMAs (mma.sync m16n8k16, fp16 operands, fp32 accumulators)
+// whose fragments are loaded straight from the packed operand layouts below (8 consecutive K values per
+// 16-byte chunk).  k_delta_conv1_wgmma (83 % of the FLOPs of a pair) synthesises its A operand |l - r| in
+// registers, so the 66 MB delta tensor of a pair (the reference's DeltaLayer output) is never materialised.
+// Operands that must be fp32-grade are split into hi + lo fp16 halves (x = hi + lo exactly to 2^-22).
 #include "common.cuh"
-#include "umma.cuh"
+#include "hopper.cuh"
 
 #include <cuda_fp16.h>
+#include <stddef.h>
 #include <stdlib.h>
 
-using namespace umma;
-
 namespace ovn {
+
+using namespace hopper;
 
 constexpr int WF = 360;                 // leg_output_width (the TC path is specialised to the
 constexpr int CF = 128;                 //   reference geometry: 360 x 128 volumes, conv1size 15)
 constexpr int S15 = 15;
 constexpr int NB = 24;                  // 360 / 15
 constexpr int PAIR_ROWS = NB * NB;      // 576 rows of c_conv2 output per pair
-constexpr long long kWaitCycles = 1ll << 28;
-constexpr int K4_PITCH = CF + 8;        // fp16 row pitch of L / R for k_delta_conv1_tc: 272 B => conflict-free LDS.128 across rows
-
-constexpr int kLegPartTiles = 320;       // (output tile, split) slots of the leg's split-K workspace
+constexpr int K4_PITCH = CF + 8;        // fp16 row pitch of the L / R operand copies of k_delta_conv1_wgmma
 
 struct TcState {
   __half* w1p = nullptr;        // [60 steps][4][64][8]
   __half* w2p = nullptr;        // [15 di][hi, lo][128 n][64 o] SWIZZLE_128B tiles (W2 = hi + lo in fp16)
   __half* w3p = nullptr;        // [2 halves][36 slabs][4][128][8]
   float* b2eff = nullptr;       // c_conv2 bias + the c_conv1 bias pushed through W2 (both layers are linear)
-  // tensor-core leg (layers 2..): packed weights + copy tables per layer, ping-pong activation planes
-  __half* wres[kMaxLegLayers] = {};      // [cout/64][kh*kw*3][C_in/8][64][8] (latency-mode kernel)
-  // batched kernel: per tap the hi and lo halves of the weights stacked along N, [cout/64][kh*kw][C_in/8/c8u][c8u][2 n_mma][8]
-  // with rows [0, n_mma) = hi, [n_mma, 2 n_mma) = lo: x*w ~= xh*[wh; wl] (one MMA, N = 2 n_mma) + xl*wh (N = n_mma)
-  __half* wstk[kMaxLegLayers] = {};
-  int stk_c8u[kMaxLegLayers] = {};
-  // layers with 128 output channels: all of them in one CTA (n_mma = 128, 256 stacked rows), so that the
-  // activation window is read once instead of once per 64-channel half
-  __half* wstkw[kMaxLegLayers] = {};
-  int stkw_c8u[kMaxLegLayers] = {};
-  bool leg_wide = true;
+  // tensor-core leg (layers 2..): packed weights per layer, ping-pong activation planes
+  __half* wres[kMaxLegLayers] = {};      // [cout/64][kh*kw*3 slabs (tap, term)][C_in/8][64][8]; term 0, 1 = hi, 2 = lo
   __half* actp[2] = {nullptr, nullptr};
-  // layer 1 on tensor cores (batched encode): the stride-2 columns are de-interleaved into even / odd planes, which
-  // turns the 5 x 15 stride-(2,2) conv over C channels into a 5 x 8 stride-(2,1) conv over 2C channels
-  // Narrow inputs (C <= 8) additionally fold the kh kernel rows into K (channel' = (dh * 2 + parity) * C + c, one
-  // plane set per OUTPUT row): K = 16 per MMA would otherwise be half padding.
-  __half* in_planes = nullptr;          // [max_batch_scans][rows][hi,lo][l1_c8in][ceil(W/2)][8]; rows = H (l1_fold = 1) or H_out
-  int l1_c8in = 0;                      // (l1_fold * 2C rounded up to a multiple of 16) / 8
-  int l1_fold = 1;                      // kernel rows folded into the channel dimension (1 or kh)
-  bool l1_tc = false;
-  float* leg_part = nullptr;     // split-K partial tiles of the latency-mode leg: [kLegPartTiles][128 x 64] fp32
-  int* leg_counters = nullptr;   // [kLegPartTiles * 4] arrival counters (always left at zero)
   __half* l16 = nullptr;        // [max_pairs][360][128]
   __half* r16 = nullptr;        // [max_pairs][360][128] (pair mode) / [1][360][128] (query mode)
   __half* o1 = nullptr;         // [rows_pad/128][15 di][128][64]: SWIZZLE_128B A tiles of c_conv2 (o1_chunk_offset)
@@ -80,7 +46,7 @@ struct TcState {
   float* partial = nullptr;     // [rows_pad][2]
   __half* lc = nullptr;         // correlation operands: [max_pairs][3 tiles][2 k-halves][hi,lo][8][128][8]
   __half* rc = nullptr;         // [max_pairs or 1][2 n-halves][hi,lo][16][192][8]
-  float* corr_part = nullptr;   // [max_pairs][2][360]
+  float* corr_part = nullptr;   // [max_pairs][C6_IBLK row blocks][360]
   // resident bank (ovn_bank_prepare): operand copies of the LEFT volumes, indexed by bank row
   const float* pb_key = nullptr;
   int64_t pb_cap = 0, pb_rows = 0;      // capacity / rows [0, pb_rows) prepared
@@ -147,39 +113,10 @@ k_channel_mean(const float* __restrict__ bank, const int32_t* __restrict__ idx, 
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// k_delta_conv1_tc
-// ------------------------------------------------------------------------------------------------
-#ifndef OVN_K4_GROUPS
-#define OVN_K4_GROUPS 3
-#endif
-constexpr int K4_GROUPS = OVN_K4_GROUPS; // producer groups of 4 warps (one per TMEM lane quarter); group g owns steps with step % K4_GROUPS == g
-constexpr int K4_PROD_WARPS = 4 * K4_GROUPS;
-constexpr int K4_THREADS = (8 + K4_PROD_WARPS) * 32;
-#ifndef OVN_K4_ROT
-#define OVN_K4_ROT 0
-#endif
-// OVN_K4_ROT = 1 (round-2 experiment, correct but SLOWER, kept as a build switch): FOUR accumulator tiles used
-// round-robin by the three row tiles of consecutive units (unit u, tile t -> physical tile (3u + t) mod 4), paid for
-// with one A ring slot (5 x 48 columns instead of 6).  The first tile of the next unit is then always free and the
-// second is the one the epilogue pulled first, which removes the issuer's ~1000 clk wait per unit for the
-// single-buffered accumulators -- but the shallower A ring costs more in steady state: measured on one box,
-// back to back, 2.06-2.08 ms against 1.91-1.98 ms (tools/gpu_r2_ab.sh, profiles/r2_k4_rot_ab.txt).
-constexpr int K4_DTILES = OVN_K4_ROT ? 4 : 3;
-constexpr int K4_STAGES = OVN_K4_ROT ? 5 : 6;   // A ring: TMEM column slots
-constexpr int K4_BGROUPS = 3;           // B ring: 3 groups of 6 consecutive W1 slices (24 KB, one bulk copy, one barrier each;
-                                        //   4 groups measured no faster, and the 24 KB pay for the epilogue staging)
-constexpr int K4_BSLOTS = K4_BGROUPS * K4_STAGES;
-constexpr int K4_TILES = 3;
-constexpr int K4_ACOL0 = K4_DTILES * 64; // TMEM columns: D = [0, 64 * K4_DTILES), A stages behind it (48 columns each)
-static_assert(K4_DTILES * 64 + K4_STAGES * 48 <= 512 && 60 % K4_STAGES == 0 && (60 / K4_STAGES) % 2 == 0, "k_delta_conv1_tc TMEM / ring layout");
-constexpr int K4_STAGE_COLS = 48;
-constexpr int K4_STEPS = 60;            // 4 channel chunks x 15 dj per jb
-constexpr int K4_BSLICE = 4096;         // bytes of W1 per step: [4 k8][64 o][8]
-constexpr int K4_RWIN_BYTES = S15 * K4_PITCH * 2;   // the 15 RIGHT rows one jb touches
+constexpr int K4_STEPS = 60;            // W1 slices: 4 channel chunks x 15 dj
 
-// o1 layout ("SWIZZLE_128B tiles"): the A operand of c_conv2, stored as the shared-memory image its
-// MMAs read, so that c_conv2 loads a [128 rows x 64 K] tile with ONE 16 KB bulk copy:
+// o1 layout ("SWIZZLE_128B tiles", kept from the bulk-copy design: [128 rows x 64 K] tiles whose 16-byte
+// chunks are XOR-swizzled by the row):
 //   row m = pair*576 + jb*24 + ib (i = ib*15 + di), K = di*64 + o
 //   o1[(m / 128) * 15 + di][m % 128][chunk (o/8) ^ (m & 7)][o % 8]
 __host__ __device__ __forceinline__ size_t o1_chunk_offset(int64_t m, int di, int c8) {
@@ -187,1344 +124,24 @@ __host__ __device__ __forceinline__ size_t o1_chunk_offset(int64_t m, int di, in
   return ((size_t)((m >> 7) * S15 + di) * 128 + r) * 64 + (size_t)((c8 ^ (r & 7)) * 8);
 }
 
-struct K4Smem {
-  __half L[WF * K4_PITCH];
-  __half Rw[2][S15 * K4_PITCH];         // double-buffered RIGHT-row window (streamed per jb)
-  __half B[K4_BSLOTS][K4_BSLICE / 2];
-  __half Bc[2 * 64 * 8];                // constant K16 x N64 B slice: row k = 0 holds -mu_o1[o], the rest is zero
-  uint8_t epi[K4_TILES][4][32 * 128];   // [tile][epilogue warp]: 32 fp16 output rows staged for the transposed store
-  uint64_t a_full[K4_STAGES], a_empty[K4_STAGES], b_full[K4_BGROUPS], b_empty[K4_BGROUPS];
-  uint64_t d_full, d_empty[K4_DTILES], l_full, l_empty, rw_full[2], rw_empty[2];
-  uint32_t tmem_base;
-};
-
-static_assert(sizeof(K4Smem) <= 232448, "k_delta_conv1_tc shared memory");
-constexpr int K4_ONES_COL = K4_ACOL0 + K4_STAGES * K4_STAGE_COLS;     // 8 TMEM columns: A operand "1 at k = 0"
-static_assert(K4_ONES_COL + 8 <= 512, "k_delta_conv1_tc TMEM layout");
-
-// Development aid (tools/k4_trace.py): a build with -DOVN_K4_TRACE records clock64() timestamps of
-// CTA 0's roles for one jb.  Compiled out of the product library.
-#ifdef OVN_K4_TRACE
-__device__ long long g_k4_trace[8][64][4];
-#define K4_TR(cond, role, step, ev, val) do { if ((cond) && blockIdx.x == 0) g_k4_trace[role][step][ev] = (val); } while (0)
-#else
-#define K4_TR(cond, role, step, ev, val) do { } while (0)
-#endif
-
-#define TC_WAIT(bar, parity, code)                       \
-  if (!mbar_wait((bar), (parity), kWaitCycles)) {        \
-    atomicExch(err, (code));                             \
-    goto done;                                           \
-  }
-
-// Work unit = (pair, jb): one 360 x 64 block of o1.  Every CTA takes a contiguous range of the
-// n_pairs*24 units (1101 pairs on 148 SMs is 7.44 pairs per SM: whole pairs would leave 7 % idle).
-//
-// Measured on B200 (profiles/r1_*): (1) with W1 slices sharing the 6-deep A ring the kernel was
-// bound by the L2 -> shared round trip of a slice (slot turnaround ~4000 clk), so the W1 ring is
-// separate and 24 deep; (2) that only fits next to the LEFT volume if the RIGHT volume is not
-// resident: a jb touches just 15 RIGHT rows, which are streamed as a 4 KB double-buffered window;
-// (3) a producer warp's LDS -> ALU -> tcgen05.st -> wait::st -> arrive chain runs at IPC ~0.2, so
-// 12 producer warps in three groups work on interleaved steps; (4) the clock64 trace
-// (profiles/r1_k4_trace*.log) showed the issuer at the tensor rate (250 clk per step) in steady
-// state, but stalled ~5000 clk per jb behind the epilogue, whose stores were one 16 B piece per
-// lane per line (32 LSU transactions per instruction): the epilogue now transposes through shared
-// memory and stores whole 128 B lines, and hands the accumulator back tile by tile.
-__global__ void __launch_bounds__(K4_THREADS, 1)
-k_delta_conv1_tc(const __half* __restrict__ L16, const int32_t* __restrict__ l_idx, const __half* __restrict__ R16,
-                 int r_per_pair, const __half* __restrict__ W1p, const float* __restrict__ mu_o1, __half* __restrict__ o1,
-                 int n_pairs, int* __restrict__ err) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  K4Smem& S = *reinterpret_cast<K4Smem*>(smem_raw);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int64_t n_units = (int64_t)n_pairs * NB;
-  const int u_begin = (int)(n_units * blockIdx.x / gridDim.x), u_end = (int)(n_units * (blockIdx.x + 1) / gridDim.x);
-
-  if (tid == 0) {
-    for (int s = 0; s < K4_STAGES; ++s) { mbar_init(&S.a_full[s], 4); mbar_init(&S.a_empty[s], 1); }
-    for (int s = 0; s < K4_BGROUPS; ++s) { mbar_init(&S.b_full[s], 1); mbar_init(&S.b_empty[s], 1); }
-    mbar_init(&S.d_full, 1);
-    for (int t = 0; t < K4_DTILES; ++t) mbar_init(&S.d_empty[t], 4);
-    mbar_init(&S.l_full, 1); mbar_init(&S.l_empty, K4_PROD_WARPS);
-    for (int b = 0; b < 2; ++b) { mbar_init(&S.rw_full[b], 1); mbar_init(&S.rw_empty[b], K4_PROD_WARPS); }
-    mbar_fence_init();
-  }
-  if (warp == 2) tmem_alloc(&S.tmem_base, 512);
-  // The o1 centre is subtracted BY THE TENSOR CORE: the first MMA of every accumulator tile of a unit is
-  // D = ones(k = 0) x Bc with Bc[0][o] = -mu_o1[o] (fp16; k_o1_channel_mean rounds mu_o1 to fp16 so that the
-  // bias fold downstream uses exactly the subtracted value).  Doing it in the epilogue (64 FADD + 16 LDS per
-  // row tile in front of the next tile's tcgen05.ld) cost 3 % of this kernel (profiles/r2_k4_center_ab.txt).
-  if (tid >= 64 && tid < 128) {
-    const int o = tid - 64;
-    const __half neg = __float2half_rn(-mu_o1[o]);
-    uint4 z = make_uint4(0u, 0u, 0u, 0u), f = z;
-    f.x = (uint32_t)__half_as_ushort(neg);
-    *reinterpret_cast<uint4*>(&S.Bc[(0 * 64 + o) * 8]) = f;        // k = 0..7 of channel o
-    *reinterpret_cast<uint4*>(&S.Bc[(1 * 64 + o) * 8]) = z;        // k = 8..15
-  }
-  fence_proxy_async();
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = S.tmem_base;
-  if (warp >= 4 && warp < 8) {             // the constant A operand: every lane (row) holds 1.0 at k = 0
-    const uint32_t ones[8] = {0x00003c00u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-    tmem_st_x8(tmem + ((uint32_t)((warp & 3) * 32) << 16) + K4_ONES_COL, ones);
-    tmem_st_wait();
-  }
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  constexpr uint32_t VOL_BYTES = WF * K4_PITCH * 2;
-
-  if (warp == 0) {
-    // ===================== loader A: W1 through the deep ring, 6 consecutive slices per copy ====
-    if (lane == 0) {
-      uint32_t bg = 0, bph = 0;
-      for (int u = u_begin; u < u_end; ++u) {
-        for (int o = 0; o < K4_STEPS / K4_STAGES; ++o) {
-          TC_WAIT(&S.b_empty[bg], bph ^ 1, 102);
-          mbar_arrive_expect_tx(&S.b_full[bg], K4_STAGES * K4_BSLICE);
-          bulk_g2s(S.B[bg * K4_STAGES], W1p + (size_t)o * K4_STAGES * (K4_BSLICE / 2), K4_STAGES * K4_BSLICE, &S.b_full[bg]);
-          if (++bg == K4_BGROUPS) { bg = 0; bph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 3) {
-    // ===================== loader B: LEFT volume per pair, RIGHT row window per jb ==============
-    if (lane == 0) {
-      uint32_t pi = 0, ui = 0;
-      int p = u_begin / NB, jb = u_begin - p * NB;
-      for (int u = u_begin; u < u_end; ++u, ++ui) {
-        if (u == u_begin || jb == 0) {
-          TC_WAIT(&S.l_empty, (pi & 1) ^ 1, 101);
-          mbar_arrive_expect_tx(&S.l_full, VOL_BYTES);
-          bulk_g2s(S.L, L16 + (size_t)(l_idx ? l_idx[p] : p) * WF * K4_PITCH, VOL_BYTES, &S.l_full);
-          ++pi;
-        }
-        const __half* Rp = R16 + (r_per_pair ? (size_t)p * WF * K4_PITCH : 0);
-        const uint32_t b = ui & 1;
-        TC_WAIT(&S.rw_empty[b], ((ui >> 1) & 1) ^ 1, 103);
-        mbar_arrive_expect_tx(&S.rw_full[b], K4_RWIN_BYTES);
-        bulk_g2s(S.Rw[b], Rp + (size_t)jb * S15 * K4_PITCH, K4_RWIN_BYTES, &S.rw_full[b]);
-        if (++jb == NB) { jb = 0; ++p; }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer ==========================================================
-    // Warp-uniform loop (addresses / descriptors stay in uniform registers), one elected lane
-    // issues.  The A ring is unrolled (60 steps = 10 x 6 slots: slot offsets are immediates and the
-    // phase is the parity of the outer counter); the B group is a running counter.
-    {
-      const uint32_t idesc = make_idesc_f16(128, 64);
-      const uint64_t bdesc0 = make_desc_kmajor_noswizzle(smem_u32(S.B[0]), 1024, 128);
-      const uint64_t bdesc_c = make_desc_kmajor_noswizzle(smem_u32(S.Bc), 1024, 128);
-      const uint32_t bd_hi = (uint32_t)(bdesc0 >> 32), bd_lo = (uint32_t)bdesc0;
-      const bool leader = elect_one() != 0;
-      // An mbarrier probe costs ~90 clk even when the phase is already complete, and this warp is the
-      // pacemaker: every barrier it needs (A slot of the next step, W1 group and first A slot of the
-      // next 6-step group) is probed with a non-blocking test_wait one step BEFORE it is needed, so the
-      // probe latency hides behind the MMAs being issued; only a failed probe falls back to a wait.
-      const uint32_t a_full0 = smem_u32(&S.a_full[0]), b_full0 = smem_u32(&S.b_full[0]);
-      uint32_t ui = 0, bg = 0, bph = 0;
-      uint32_t dcnt[K4_DTILES] = {};        // how often each physical accumulator tile has been handed to a unit so far
-      bool ready = false, bready = false;
-      for (int u = u_begin; u < u_end; ++u, ++ui) {
-        // physical accumulator tile of this unit's row tile t
-        uint32_t pt[K4_TILES];
-#pragma unroll
-        for (int t = 0; t < K4_TILES; ++t) pt[t] = OVN_K4_ROT ? ((3u * ui + t) & 3u) : (uint32_t)t;
-#pragma unroll 1
-        for (uint32_t o = 0; o < K4_STEPS / K4_STAGES; ++o) {
-          const uint32_t ph = o & 1;            // (step / 6) & 1: 10 groups per unit
-          if (!bready) { if (!mbar_wait_addr(b_full0 + bg * 8, bph, kWaitCycles)) { atomicExch(err, 203); goto done; } }
-          const uint32_t b_lo = bd_lo + ((bg * K4_STAGES * K4_BSLICE) >> 4);
-          const uint32_t nbg = (bg + 1 == K4_BGROUPS) ? 0 : bg + 1, nbph = (bg + 1 == K4_BGROUPS) ? bph ^ 1 : bph;
-#pragma unroll
-          for (int sg = 0; sg < K4_STAGES; ++sg) {
-            K4_TR(leader && u == u_begin + 2, 0, o * 6 + sg, 0, clock64());
-            K4_TR(leader && u == u_begin + 2, 0, o * 6 + sg, 3, (long long)ready);
-            if (!ready) { if (!mbar_wait_addr(a_full0 + sg * 8, ph, kWaitCycles)) { atomicExch(err, 202); goto done; } }
-            K4_TR(leader && u == u_begin + 2, 0, o * 6 + sg, 1, clock64());
-            // non-blocking probes ahead
-            if (sg + 1 < K4_STAGES) ready = mbar_test_addr(a_full0 + (sg + 1) * 8, ph);
-            else ready = mbar_test_addr(a_full0, ph ^ 1);
-            if (sg == K4_STAGES - 2) bready = mbar_test_addr(b_full0 + nbg * 8, nbph);
-            fence_after_sync();
-            if (sg == 0 && o == 0) {
-              // D is single-buffered (TMEM is full): the first step of a unit is issued tile by tile,
-              // each tile as soon as the epilogue has pulled that tile of the previous unit into
-              // registers.  (Running the first six steps tile-major was measured slower: the producers
-              // have only just been given the six slots back and tile 0 then waits for slot 5.)
-#pragma unroll
-              for (int t = 0; t < K4_TILES; ++t) {
-                // the epilogue has pulled the previous contents of this physical tile (its k-th release, k = dcnt - 1)
-#pragma unroll
-                for (int p = 0; p < K4_DTILES; ++p) {
-                  if (pt[t] == (uint32_t)p) {
-                    TC_WAIT(&S.d_empty[p], (dcnt[p] & 1) ^ 1, 201);
-                    ++dcnt[p];
-                  }
-                }
-                fence_after_sync();
-                if (leader) {
-                  mma_ts(tmem + pt[t] * 64, tmem + K4_ONES_COL, bdesc_c, idesc, 0);          // D = -mu_o1 (overwrites)
-#pragma unroll
-                  for (int kk = 0; kk < 2; ++kk) {
-                    const uint64_t bd = ((uint64_t)bd_hi << 32) | (uint64_t)(b_lo + ((kk * 2048) >> 4));
-                    mma_ts(tmem + pt[t] * 64, tmem + K4_ACOL0 + t * 16 + kk * 8, bd, idesc, 1);
-                  }
-                }
-                __syncwarp();
-              }
-              if (leader) commit(&S.a_empty[0]);
-              K4_TR(leader && u == u_begin + 2, 0, 0, 2, clock64());
-              __syncwarp();
-              continue;
-            }
-            if (leader) {
-              // consecutive MMAs go to different accumulator tiles
-#pragma unroll
-              for (int kk = 0; kk < 2; ++kk) {
-                const uint64_t bd = ((uint64_t)bd_hi << 32) | (uint64_t)(b_lo + ((sg * K4_BSLICE + kk * 2048) >> 4));
-#pragma unroll
-                for (int t = 0; t < K4_TILES; ++t) {
-                  mma_ts(tmem + pt[t] * 64, tmem + K4_ACOL0 + sg * K4_STAGE_COLS + t * 16 + kk * 8, bd, idesc, 1);
-                }
-              }
-              commit(&S.a_empty[sg]);
-              if (sg == K4_STAGES - 1) commit(&S.b_empty[bg]);
-            }
-            K4_TR(leader && u == u_begin + 2, 0, o * 6 + sg, 2, clock64());
-            __syncwarp();
-          }
-          bg = nbg; bph = nbph;
-        }
-        if (leader) commit(&S.d_full);
-        __syncwarp();
-      }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ===================== epilogue: D (TMEM) -> fp16 -> o1 tiles ================================
-    // Lane = output row i.  A row is 64 channels = one 128 B line of o1; written lane-per-row the 8
-    // STG.128 of a warp would each touch 32 lines.  The warp transposes its 32 rows through shared
-    // memory instead, so that 8 lanes cover one line and an instruction stores 4 whole lines.
-    // (Measured alternatives: one 128 B bulk shared->global copy per lane is slower -- the copy
-    // engine takes ~18 clk per small copy; STG itself tops out near 32 B/clk/SM.)
-    const int q = warp & 3;
-    uint32_t ui = 0;
-    int p = u_begin / NB, jb = u_begin - p * NB;
-    for (int u = u_begin; u < u_end; ++u, ++ui) {
-      K4_TR(q == 0 && lane == 0 && u == u_begin + 1, 4, 0, 0, clock64());
-      TC_WAIT(&S.d_full, ui & 1, 301);
-      fence_after_sync();
-      K4_TR(q == 0 && lane == 0 && u == u_begin + 1, 4, 0, 1, clock64());
-      const int64_t m0 = (int64_t)p * PAIR_ROWS + jb * NB;
-      // pass 1: pull the three accumulator tiles out of TMEM as fast as possible (the MMA issuer is
-      // waiting for them): tcgen05.ld -> release -> fp16 -> staging buffer t (row = lane, 16-byte
-      // chunks XOR-swizzled by the row so that both passes are bank-conflict free without padding)
-#pragma unroll 1
-      for (int t = 0; t < K4_TILES; ++t) {
-        uint32_t v0[32], v1[32];
-        const uint32_t ptile = OVN_K4_ROT ? ((3u * ui + (uint32_t)t) & 3u) : (uint32_t)t;   // physical accumulator tile
-        K4_TR(q == 0 && lane == 0 && u == u_begin + 1, 4, 1 + t, 1, clock64());
-        tmem_ld_x32(tmem + ((uint32_t)(q * 32) << 16) + ptile * 64, v0);
-        tmem_ld_x32(tmem + ((uint32_t)(q * 32) << 16) + ptile * 64 + 32, v1);
-        tmem_ld_wait();
-        fence_before_sync();                 // this tile is in registers: hand it back to the MMA issuer
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&S.d_empty[ptile]);
-        K4_TR(q == 0 && lane == 0 && u == u_begin + 1, 4, 1 + t, 0, clock64());
-        // (the c_conv1 bias is folded into the c_conv2 bias at pack time: both layers are linear)
-        uint8_t* row = S.epi[t][q] + lane * 128;
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-#pragma unroll
-          for (int h8 = 0; h8 < 4; ++h8) {
-            uint32_t pk[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const uint32_t a = c ? v1[h8 * 8 + 2 * j] : v0[h8 * 8 + 2 * j];
-              const uint32_t b = c ? v1[h8 * 8 + 2 * j + 1] : v0[h8 * 8 + 2 * j + 1];
-              __half2 hh = __floats2half2_rn(__uint_as_float(a), __uint_as_float(b));   // (the centre is already subtracted)
-              pk[j] = *reinterpret_cast<uint32_t*>(&hh);
-            }
-            *reinterpret_cast<uint4*>(row + (((c * 4 + h8) ^ (lane & 7)) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          }
-        }
-        K4_TR(q == 0 && lane == 0 && u == u_begin + 1, 4, 1 + t, 3, clock64());
-      }
-      __syncwarp();
-      // pass 2 (overlaps the MMAs of the next unit): transposed stores, 8 lanes per 128 B line.
-      // lane -> (row rr0 + 4k, chunk c8); (ib, di) advance incrementally, the address is counted in
-      // 16-byte chunks: (((m >> 7) * 15 + di) << 10) | ((m & 127) << 3) | (c8 ^ (m & 7)), m0 % 8 == 0
-#pragma unroll 1
-      for (int t = 0; t < K4_TILES; ++t) {
-        const int c8 = lane & 7, rr0 = lane >> 3;
-        int i = t * 128 + q * 32 + rr0;
-        int ib = i / S15, di = i - ib * S15;
-        const uint8_t* src = S.epi[t][q] + rr0 * 128;
-        uint4* const o1c = reinterpret_cast<uint4*>(o1);
-        // branch-free and batched (all loads, then all stores): one warp per scheduler has nothing
-        // else to hide the LDS -> address -> STG chain behind
-        uint4 v[8];
-        size_t chunk[8];
-        bool ok[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          v[k] = *reinterpret_cast<const uint4*>(src + k * 512 + ((c8 ^ ((rr0 + 4 * k) & 7)) << 4));
-          const int64_t m = m0 + ib;
-          chunk[k] = ((size_t)((m >> 7) * S15 + di) << 10) | (size_t)(((int)m & 127) << 3) | (size_t)(c8 ^ (ib & 7));
-          ok[k] = i < WF;
-          i += 4; di += 4;
-          if (di >= S15) { di -= S15; ++ib; }
-        }
-#pragma unroll
-        for (int k = 0; k < 8; ++k)     // predicated (not branched) stores keep the eight chains independent
-          asm volatile("{ .reg .pred p; setp.ne.u32 p, %5, 0; @p st.global.v4.b32 [%0], {%1, %2, %3, %4}; }"
-                       :: "l"(o1c + chunk[k]), "r"(v[k].x), "r"(v[k].y), "r"(v[k].z), "r"(v[k].w), "r"((uint32_t)ok[k]) : "memory");
-        K4_TR(q == 0 && lane == 0 && u == u_begin + 1, 4, 1 + t, 2, clock64());
-      }
-      __syncwarp();                          // staging buffers are rewritten by the next unit's pass 1
-      if (++jb == NB) { jb = 0; ++p; }
-    }
-  } else if (warp >= 8) {
-    // ===================== producers: |l - r| -> TMEM ==========================================
-    // 12 warps = 3 groups x 4 TMEM lane quarters.  A thread owns LEFT rows q*32+lane (+128, +256);
-    // all 32 channels of the current chunk live in registers (48), the RIGHT row comes by broadcast
-    // LDS.128 from the per-jb window.  Group g produces the steps with step % 3 == g (15 and 60 are
-    // multiples of 3: dj = g, g+3, ...) into ring slots g, g+3: per synthesised element this costs
-    // 1 ALU instruction + ~0.3 of loop / barrier overhead, and a group has three MMA stage-times
-    // to hide its LDS -> ALU -> tcgen05.st -> wait::st -> arrive chain.
-    const int pw = warp - 8, q = pw & 3, grp = pw >> 2;
-    const int row0 = q * 32 + lane;
-    const uint32_t lane_addr = tmem + ((uint32_t)(q * 32) << 16) + K4_ACOL0;
-    const uint32_t a_empty0 = smem_u32(&S.a_empty[0]), a_full0 = smem_u32(&S.a_full[0]);
-    uint32_t pi = 0, ui = 0;
-    bool slot_free = true;                  // result of the probe issued one step ahead (the first steps find fresh slots)
-    int jb = u_begin % NB;
-    for (int u = u_begin; u < u_end; ++u, ++ui) {
-      if (u == u_begin || jb == 0) { TC_WAIT(&S.l_full, pi & 1, 402); ++pi; }
-      const uint32_t wb = ui & 1;
-      TC_WAIT(&S.rw_full[wb], (ui >> 1) & 1, 404);
-      int st = grp;                         // step within the unit: slot = st % 6, phase = (st / 6) & 1 (10 ring turns per unit)
-#pragma unroll 1
-      for (int cc = 0; cc < 4; ++cc) {
-        const int ch = cc * 32;
-        uint32_t Lr[K4_TILES][16];
-#pragma unroll
-        for (int t = 0; t < K4_TILES; ++t) {
-          const int i = t * 128 + row0;
-#pragma unroll
-          for (int v4 = 0; v4 < 4; ++v4) {
-            uint4 a = make_uint4(0u, 0u, 0u, 0u);
-            if (i < WF) a = *reinterpret_cast<const uint4*>(&S.L[i * K4_PITCH + ch + v4 * 8]);
-            Lr[t][v4 * 4 + 0] = a.x; Lr[t][v4 * 4 + 1] = a.y; Lr[t][v4 * 4 + 2] = a.z; Lr[t][v4 * 4 + 3] = a.w;
-          }
-        }
-#pragma unroll 1
-        for (; st < (cc + 1) * S15; st += K4_GROUPS) {
-          const int dj = st - cc * S15;
-          const uint32_t sg = (uint32_t)st % K4_STAGES, ph = ((uint32_t)st / K4_STAGES) & 1;
-          const __half* rrow = &S.Rw[wb][dj * K4_PITCH + ch];
-          K4_TR(q == 0 && lane == 0 && u == u_begin + 2 && grp < 3, 1 + grp, st, 0, clock64());
-          if (!slot_free) { if (!mbar_wait_addr(a_empty0 + sg * 8, ph ^ 1, kWaitCycles)) { atomicExch(err, 403); goto done; } }
-          K4_TR(q == 0 && lane == 0 && u == u_begin + 2 && grp < 3, 1 + grp, st, 1, clock64());
-          {
-            // probe the slot of this group's NEXT step now; the ~90 clk answer is consumed next iteration
-            const uint32_t s1 = (uint32_t)st + K4_GROUPS, sg1 = s1 % K4_STAGES, ph1 = (s1 / K4_STAGES) & 1;
-            slot_free = mbar_test_addr(a_empty0 + sg1 * 8, ph1 ^ 1);
-          }
-          fence_after_sync();
-#pragma unroll
-          for (int hk = 0; hk < 2; ++hk) {          // two 16-channel halves: keeps the live set of r at 8 registers
-            const uint4 ra = *reinterpret_cast<const uint4*>(rrow + hk * 16);        // broadcast LDS
-            const uint4 rb = *reinterpret_cast<const uint4*>(rrow + hk * 16 + 8);
-            const uint32_t rw[8] = {ra.x, ra.y, ra.z, ra.w, rb.x, rb.y, rb.z, rb.w};
-#pragma unroll
-            for (int t = 0; t < K4_TILES; ++t) {
-              uint32_t o[8];
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                // |l - r|: subtract on the FMA pipe, clear both sign bits on the ALU pipe (LOP3)
-                const __half2 d = __hsub2(*reinterpret_cast<const __half2*>(&Lr[t][hk * 8 + j]),
-                                          *reinterpret_cast<const __half2*>(&rw[j]));
-                o[j] = *reinterpret_cast<const uint32_t*>(&d) & 0x7fff7fffu;
-              }
-              tmem_st_x8(lane_addr + sg * K4_STAGE_COLS + t * 16 + hk * 8, o);
-            }
-            K4_TR(q == 0 && lane == 0 && u == u_begin + 2 && grp < 3 && hk == 0, 5 + grp, st, 0, clock64());
-          }
-          K4_TR(q == 0 && lane == 0 && u == u_begin + 2 && grp < 3, 1 + grp, st, 2, clock64());
-          tmem_st_wait();
-          K4_TR(q == 0 && lane == 0 && u == u_begin + 2 && grp < 3, 5 + grp, st, 1, clock64());
-          fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_addr(a_full0 + sg * 8);
-          K4_TR(q == 0 && lane == 0 && u == u_begin + 2 && grp < 3, 1 + grp, st, 3, clock64());
-        }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&S.rw_empty[wb]);
-      const bool last_of_pair = (jb == NB - 1) || (u == u_end - 1);
-      if (last_of_pair) { __syncwarp(); if (lane == 0) mbar_arrive(&S.l_empty); }
-      if (++jb == NB) jb = 0;
-    }
-  }
-done:
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem, 512);
-}
-
-constexpr int G_THREADS = 256;
-
-// ------------------------------------------------------------------------------------------------
-// k_conv2_sw_tc -- c_conv2 (15x1 stride 15, 64 -> 128, ReLU) as a GEMM  [M x 960] x [960 x 128].
-// k_delta_conv1_tc leaves o1 as ready-made SWIZZLE_128B operand tiles (o1_chunk_offset), so a
-// K step of 64 (= one di) is three 16 KB bulk copies: two A row tiles and the W2 tile they share.
-// Rows are (pair, jb, ib); the ReLU'd result goes to the x3 planes c_conv3 reads.
-// ------------------------------------------------------------------------------------------------
-constexpr int C2_STAGES = 3, C2_TILE_BYTES = 128 * 128;
-
-struct C2Smem {
-  uint8_t st[C2_STAGES][4][C2_TILE_BYTES];     // [A tile 0][A tile 1][W2 hi tile][W2 lo tile]
-  float bias[128], mu[128];
-  uint64_t full[C2_STAGES], empty[C2_STAGES], d_full[2], d_empty[2];
-  uint32_t tmem_base;
-};
-
-// W2 is applied as hi + lo (two MMAs per K16 step and row tile): the kernel streams 1.2 GB of o1 and
-// is HBM-bound, so the second MMA is nearly free, and the fp16 rounding of W2 was the largest single
-// term of the logit error budget after the feature volumes (DESIGN.md section 2).
-// (Round 2: a CTA-pair version of this kernel -- one row tile and half of the W2 tiles per CTA, cta_group::2 --
-// was built and measured bit-identical but SLOWER, 0.256 vs 0.236 ms: the kernel is bound by the 1.2 GB o1
-// stream from HBM, and the pair's extra barrier hop costs more than the cheaper operand fetch saves.)
-// `fault` != 0 is the test hook of ovn_debug_inject_fault: the loader never arrives, every consumer
-// runs into its bounded barrier wait and the error flag is raised (tests/test_gpu_errors.py).
-__global__ void __launch_bounds__(G_THREADS, 1)
-k_conv2_sw_tc(const __half* __restrict__ o1, const __half* __restrict__ W2s, const float* __restrict__ bias2,
-              const float* __restrict__ mu_x3, __half* __restrict__ x3, int64_t out_pitch, int64_t M, int n_iter, int fault,
-              int* __restrict__ err) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  C2Smem& S = *reinterpret_cast<C2Smem*>(smem_raw);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    for (int s = 0; s < C2_STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&S.d_full[b], 1); mbar_init(&S.d_empty[b], 4); }
-    mbar_fence_init();
-  }
-  if (tid < 128) { S.bias[tid] = bias2[tid]; S.mu[tid] = mu_x3[tid]; }
-  if (warp == 2) tmem_alloc(&S.tmem_base, 512);
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = S.tmem_base;
-
-  if (warp == 0) {
-    if (lane == 0 && !fault) {
-      uint32_t s = 0, ph = 0;
-      for (int it = blockIdx.x; it < n_iter; it += gridDim.x) {
-        for (int di = 0; di < S15; ++di) {
-          TC_WAIT(&S.empty[s], ph ^ 1, 501);
-          mbar_arrive_expect_tx(&S.full[s], 4 * C2_TILE_BYTES);
-          bulk_g2s(S.st[s][0], o1 + ((size_t)(2 * it) * S15 + di) * (C2_TILE_BYTES / 2), C2_TILE_BYTES, &S.full[s]);
-          bulk_g2s(S.st[s][1], o1 + ((size_t)(2 * it + 1) * S15 + di) * (C2_TILE_BYTES / 2), C2_TILE_BYTES, &S.full[s]);
-          bulk_g2s(S.st[s][2], W2s + (size_t)di * C2_TILE_BYTES, 2 * C2_TILE_BYTES, &S.full[s]);   // hi + lo tiles are adjacent
-          if (++s == C2_STAGES) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    const uint32_t idesc = make_idesc_f16(128, 128);
-    const bool leader = elect_one() != 0;
-    const uint64_t d0 = make_desc_kmajor_sw128(smem_u32(S.st[0][0]), 0);
-    const uint32_t d_hi = (uint32_t)(d0 >> 32), d_lo = (uint32_t)d0;
-    uint32_t s = 0, ph = 0, li = 0;
-    for (int it = blockIdx.x; it < n_iter; it += gridDim.x, ++li) {
-      const uint32_t buf = li & 1;
-      TC_WAIT(&S.d_empty[buf], ((li >> 1) & 1) ^ 1, 502);
-      fence_after_sync();
-#pragma unroll 1
-      for (int di = 0; di < S15; ++di) {
-        TC_WAIT(&S.full[s], ph, 503);
-        fence_after_sync();
-        if (leader) {
-          const uint32_t base = d_lo + ((s * 4 * C2_TILE_BYTES) >> 4);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {            // 16 K values = 32 B inside the 128 B swizzle row
-            const uint64_t bh = ((uint64_t)d_hi << 32) | (uint64_t)(base + ((2 * C2_TILE_BYTES + kk * 32) >> 4));
-            const uint64_t bl = ((uint64_t)d_hi << 32) | (uint64_t)(base + ((3 * C2_TILE_BYTES + kk * 32) >> 4));
-#pragma unroll
-            for (int t = 0; t < 2; ++t) {
-              const uint64_t ad = ((uint64_t)d_hi << 32) | (uint64_t)(base + ((t * C2_TILE_BYTES + kk * 32) >> 4));
-              mma_ss(tmem + buf * 256 + t * 128, ad, bh, idesc, (di | kk) != 0);
-              mma_ss(tmem + buf * 256 + t * 128, ad, bl, idesc, 1);
-            }
-          }
-          commit(&S.empty[s]);
-        }
-        __syncwarp();
-        if (++s == C2_STAGES) { s = 0; ph ^= 1; }
-      }
-      if (leader) commit(&S.d_full[buf]);
-      __syncwarp();
-    }
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    uint32_t li = 0;
-    for (int it = blockIdx.x; it < n_iter; it += gridDim.x, ++li) {
-      const uint32_t buf = li & 1;
-      TC_WAIT(&S.d_full[buf], (li >> 1) & 1, 504);
-      fence_after_sync();
-#pragma unroll 1
-      for (int t = 0; t < 2; ++t) {
-        const int64_t m = ((int64_t)(2 * it + t) * 128) + q * 32 + lane;
-#pragma unroll 1
-        for (int c0 = 0; c0 < 128; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld_x32(tmem + ((uint32_t)(q * 32) << 16) + buf * 256 + t * 128 + c0, v);
-          tmem_ld_wait();
-          if (t == 1 && c0 == 96) {                    // both tiles of this buffer are in registers / stored
-            fence_before_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&S.d_empty[buf]);
-          }
-          if (m < M) {
-#pragma unroll
-            for (int j8 = 0; j8 < 4; ++j8) {
-              uint32_t pk[4];
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const int c = c0 + j8 * 8 + 2 * j;
-                __half2 hh = __floats2half2_rn(fmaxf(__uint_as_float(v[j8 * 8 + 2 * j]) + S.bias[c], 0.f) - S.mu[c],
-                                               fmaxf(__uint_as_float(v[j8 * 8 + 2 * j + 1]) + S.bias[c + 1], 0.f) - S.mu[c + 1]);
-                pk[j] = *reinterpret_cast<uint32_t*>(&hh);
-              }
-              *reinterpret_cast<uint4*>(x3 + ((size_t)(c0 / 8 + j8) * out_pitch + m) * 8) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            }
-          }
-        }
-      }
-    }
-  }
-done:
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem, 512);
-}
-
-// ------------------------------------------------------------------------------------------------
-// k_conv3_resident_tc -- c_conv3 (3x3, 128 -> 256, ReLU) + Flatten + Dense partial sums.
-// The streamed GEMM re-read the activation tile for each of the 9 taps and both N halves (3.6 GB of
-// L2 traffic per 1101 pairs: L2-bound).  Here the 16 activation planes of a 256-row group (+64 halo
-// rows) are loaded ONCE (80 KB) and the 3x3 window is applied by the UMMA descriptor itself: the tap
-// at row shift a*24 + b is a start-address offset in the SWIZZLE_NONE layout (16-byte rows at uniform
-// pitch -- probe mode 2).  Only the weights (8 KB per slab) are streamed.
-// Persistent: a CTA walks row groups; per group two work items (the two 128-channel halves) share
-// the window.  Windows and accumulators (2 tiles x 128 columns per item) are double-buffered, so
-// the window load of the next group and the Dense epilogue of the previous item overlap the MMAs
-// (the one-shot version spent a third of its time in the un-overlapped load and epilogue).
-// ------------------------------------------------------------------------------------------------
-constexpr int C3_ROWS = 256, C3_WIN = 320, C3_PLANES = 16, C3_SLABS = 36, C3_STAGES = 4;
-constexpr int C3_PLANE_BYTES = C3_WIN * 16;             // 5120
-constexpr int C3_WIN_BYTES = C3_PLANES * C3_PLANE_BYTES;   // 81920
-constexpr int C3_B_BYTES = 4 * 128 * 16;                // 8192
-
-struct C3Smem {
-  uint8_t A[2][C3_WIN_BYTES];
-  uint8_t B[C3_STAGES][C3_B_BYTES];
-  float bias[256];
-  uint64_t a_full[2], a_empty[2], full[C3_STAGES], empty[C3_STAGES], d_full[2], d_empty[2];
-  uint32_t tmem_base;
-};
-
-__global__ void __launch_bounds__(G_THREADS, 1)
-k_conv3_resident_tc(const __half* __restrict__ X3, int64_t a_pitch, const __half* __restrict__ Bp,
-                    const float* __restrict__ bias, int64_t M, int n_groups, const float* __restrict__ wd,
-                    float* __restrict__ partial, int* __restrict__ err) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  C3Smem& S = *reinterpret_cast<C3Smem*>(smem_raw);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&S.a_full[b], 1); mbar_init(&S.a_empty[b], 1);
-      mbar_init(&S.d_full[b], 1); mbar_init(&S.d_empty[b], 4);
-    }
-    for (int s = 0; s < C3_STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], 1); }
-    mbar_fence_init();
-  }
-  S.bias[tid] = bias[tid];                 // G_THREADS == 256 output channels
-  if (warp == 2) tmem_alloc(&S.tmem_base, 512);
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = S.tmem_base;
-
-  if (warp == 0) {
-    // ---- loader: window of group g, then the weight slabs of its two items; the window of the
-    // next group is requested after the first item's slabs so that it lands during the second item
-    if (lane == 0) {
-      uint32_t s = 0, ph = 0, gi = 0;
-      auto load_window = [&](int g, uint32_t k) -> bool {
-        const uint32_t ab = k & 1;
-        if (!mbar_wait(&S.a_empty[ab], ((k >> 1) & 1) ^ 1, kWaitCycles)) return false;
-        mbar_arrive_expect_tx(&S.a_full[ab], C3_WIN_BYTES);
-        for (int pl = 0; pl < C3_PLANES; ++pl)
-          bulk_g2s(S.A[ab] + pl * C3_PLANE_BYTES, X3 + ((size_t)pl * a_pitch + (size_t)g * C3_ROWS) * 8, C3_PLANE_BYTES, &S.a_full[ab]);
-        return true;
-      };
-      if ((int)blockIdx.x < n_groups) { if (!load_window(blockIdx.x, 0)) { atomicExch(err, 700); goto done; } }
-      for (int g = blockIdx.x; g < n_groups; g += gridDim.x, ++gi) {
-        for (int nh = 0; nh < 2; ++nh) {
-          for (int sl = 0; sl < C3_SLABS; ++sl) {
-            TC_WAIT(&S.empty[s], ph ^ 1, 701);
-            mbar_arrive_expect_tx(&S.full[s], C3_B_BYTES);
-            bulk_g2s(S.B[s], Bp + ((size_t)nh * C3_SLABS + sl) * (C3_B_BYTES / 2), C3_B_BYTES, &S.full[s]);
-            if (++s == C3_STAGES) { s = 0; ph ^= 1; }
-          }
-          if (nh == 0 && g + (int)gridDim.x < n_groups) {
-            if (!load_window(g + gridDim.x, gi + 1)) { atomicExch(err, 700); goto done; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    const uint32_t idesc = make_idesc_f16(128, 128);
-    const bool leader = elect_one() != 0;
-    const uint64_t ad0 = make_desc_kmajor_noswizzle(smem_u32(S.A[0]), C3_PLANE_BYTES, 128);
-    const uint64_t bd0 = make_desc_kmajor_noswizzle(smem_u32(S.B[0]), 128 * 16, 128);
-    const uint32_t ad_hi = (uint32_t)(ad0 >> 32), ad_lo = (uint32_t)ad0;
-    const uint32_t bd_hi = (uint32_t)(bd0 >> 32), bd_lo = (uint32_t)bd0;
-    uint32_t sg = 0, ph = 0, gi = 0, item = 0;
-    for (int g = blockIdx.x; g < n_groups; g += gridDim.x, ++gi) {
-      const uint32_t ab = gi & 1;
-      TC_WAIT(&S.a_full[ab], (gi >> 1) & 1, 702);
-      for (int nh = 0; nh < 2; ++nh, ++item) {
-        const uint32_t db = item & 1;
-        TC_WAIT(&S.d_empty[db], ((item >> 1) & 1) ^ 1, 705);
-        fence_after_sync();
-#pragma unroll 1
-        for (int tap = 0; tap < 9; ++tap) {
-          const uint32_t shift = (tap / 3) * NB + (tap % 3);                // rows
-#pragma unroll 1
-          for (int gq = 0; gq < 4; ++gq) {                                  // slab = (tap, 32-channel group)
-            TC_WAIT(&S.full[sg], ph, 703);
-            fence_after_sync();
-            if (leader) {
-              const uint32_t b_off = (sg * C3_B_BYTES) >> 4;
-#pragma unroll
-              for (int kk = 0; kk < 2; ++kk) {
-                const uint64_t bd = ((uint64_t)bd_hi << 32) | (uint64_t)(bd_lo + b_off + ((kk * 2 * (128 * 16)) >> 4));
-                const uint32_t a_k = ad_lo + ((ab * C3_WIN_BYTES + (gq * 4 + kk * 2) * C3_PLANE_BYTES + shift * 16) >> 4);
-#pragma unroll
-                for (int t = 0; t < 2; ++t) {
-                  const uint64_t ad = ((uint64_t)ad_hi << 32) | (uint64_t)(a_k + ((t * 128 * 16) >> 4));
-                  mma_ss(tmem + db * 256 + t * 128, ad, bd, idesc, (tap | gq | kk) != 0);
-                }
-              }
-              commit(&S.empty[sg]);
-            }
-            __syncwarp();
-            if (++sg == C3_STAGES) { sg = 0; ph ^= 1; }
-          }
-        }
-        if (leader) {
-          commit(&S.d_full[db]);
-          if (nh == 1) commit(&S.a_empty[ab]);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    uint32_t item = 0;
-    for (int g = blockIdx.x; g < n_groups; g += gridDim.x) {
-      for (int nh = 0; nh < 2; ++nh, ++item) {
-        const uint32_t db = item & 1;
-        TC_WAIT(&S.d_full[db], (item >> 1) & 1, 704);
-        fence_after_sync();
-#pragma unroll 1
-        for (int t = 0; t < 2; ++t) {
-          const int64_t r = (int64_t)g * C3_ROWS + t * 128 + q * 32 + lane;
-          const int rem = (int)(r % PAIR_ROWS);
-          const int yy = rem / NB, xx = rem - yy * NB;
-          const bool valid = (r < M) && (yy < NB - 2) && (xx < NB - 2);
-          // rows are (pair, jb, ib): yy = jb, xx = ib; Flatten order of the reference is (ib, jb, channel)
-          const float* wrow = wd + ((size_t)(valid ? (xx * (NB - 2) + yy) : 0) * 256 + nh * 128);
-          float acc = 0.f;
-#pragma unroll 1
-          for (int c0 = 0; c0 < 128; c0 += 32) {
-            uint32_t v[32];
-            tmem_ld_x32(tmem + ((uint32_t)(q * 32) << 16) + db * 256 + t * 128 + c0, v);
-            float4 w[8];
-#pragma unroll
-            for (int j4 = 0; j4 < 8; ++j4) w[j4] = __ldg(reinterpret_cast<const float4*>(wrow + c0) + j4);
-            tmem_ld_wait();
-            if (t == 1 && c0 == 96) {          // the last accumulator columns of this item are in registers
-              fence_before_sync();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(&S.d_empty[db]);
-            }
-            const float* bs = S.bias + nh * 128 + c0;
-#pragma unroll
-            for (int j4 = 0; j4 < 8; ++j4) {
-              acc = fmaf(fmaxf(__uint_as_float(v[j4 * 4 + 0]) + bs[j4 * 4 + 0], 0.f), w[j4].x, acc);
-              acc = fmaf(fmaxf(__uint_as_float(v[j4 * 4 + 1]) + bs[j4 * 4 + 1], 0.f), w[j4].y, acc);
-              acc = fmaf(fmaxf(__uint_as_float(v[j4 * 4 + 2]) + bs[j4 * 4 + 2], 0.f), w[j4].z, acc);
-              acc = fmaf(fmaxf(__uint_as_float(v[j4 * 4 + 3]) + bs[j4 * 4 + 3], 0.f), w[j4].w, acc);
-            }
-          }
-          if (r < M) partial[r * 2 + nh] = valid ? acc : 0.f;
-        }
-      }
-    }
-  }
-done:
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem, 512);
-}
-
-// ------------------------------------------------------------------------------------------------
-// k_conv3_pair_tc -- c_conv3 on CTA PAIRS (tcgen05 cta_group::2), round 2.
-// The single-CTA kernel above is bound by the shared-memory operand fetch of SS-mode MMAs (N = 128:
-// 111.8 clk per MMA against 64 ideal, profiles/r1_mma_rate_probe.txt; ncu: tensor pipe 64 % active).
-// A pair of CTAs on one TPC computes one M = 256 x N = 256 tile: each CTA holds the activation window of
-// its own 128 rows and only HALF of every weight slab (128 of the 256 output channels), so per MMA a CTA
-// fetches 4 KB + 4 KB for twice the work of the old 4 KB + 4 KB MMA; measured rate 133 clk per
-// M256 N256 K16 MMA = 0.96 of ideal (csrc/cta2_probe.cu, profiles/r2_cta2_probe.txt).  All 256 output
-// channels are produced at once (no second pass over the window), the L2 -> shared weight traffic per row
-// is unchanged.  Protocol: only the leader CTA (cluster rank 0) issues MMAs; tcgen05.commit multicasts
-// "slot free" / "accumulator full" to both CTAs' barriers; the peer's warp 1 relays "my operands have
-// landed" to the leader's barriers (remote mbarrier arrive); the peer's epilogue warps release the
-// accumulator on the leader's barrier.  Same MMA order as the single-CTA kernel: bit-identical results.
-// ------------------------------------------------------------------------------------------------
-constexpr int P3_ROWS = 128, P3_WIN = 192, P3_STAGES = 4;
-constexpr int P3_PLANE_BYTES = P3_WIN * 16;                 // 3072
-constexpr int P3_WIN_BYTES = C3_PLANES * P3_PLANE_BYTES;   // 49152
-constexpr int P3_B_BYTES = 4 * 4 * 128 * 16;                // one ring stage = this CTA's half of the FOUR K32 x N256 slabs of a tap
-                                                            //   (8 MMAs per barrier round trip: with one slab per stage the issuer's two ~90 clk
-                                                            //    barrier probes per 2 MMAs kept the tensor pipe half idle, 0.32 ms -- no gain)
-
-struct P3Smem {
-  uint8_t A[2][P3_WIN_BYTES];
-  uint8_t B[P3_STAGES][P3_B_BYTES];
-  float bias[256];
-  uint64_t a_full[2], a_empty[2], full[P3_STAGES], empty[P3_STAGES], d_full[2], d_empty[2];
-  uint64_t peer_a_full[2], peer_full[P3_STAGES];            // used on the leader: the peer's operands have landed
-  uint32_t tmem_base;
-};
-
-__global__ void __launch_bounds__(G_THREADS, 1)
-k_conv3_pair_tc(const __half* __restrict__ X3, int64_t a_pitch, const __half* __restrict__ Bp,
-                const float* __restrict__ bias, int64_t M, int n_groups, const float* __restrict__ wd,
-                float* __restrict__ partial, int* __restrict__ err) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  P3Smem& S = *reinterpret_cast<P3Smem*>(smem_raw);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int cl = blockIdx.x >> 1, n_cl = gridDim.x >> 1;
-  if (tid == 0) {
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&S.a_full[b], 1); mbar_init(&S.a_empty[b], 1); mbar_init(&S.peer_a_full[b], 1);
-      mbar_init(&S.d_full[b], 1); mbar_init(&S.d_empty[b], 8);        // 4 epilogue warps of each CTA
-    }
-    for (int s = 0; s < P3_STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], 1); mbar_init(&S.peer_full[s], 1); }
-    mbar_fence_init();
-  }
-  S.bias[tid] = bias[tid];                 // G_THREADS == 256 output channels
-  if (warp == 2) tmem_alloc_cta2(&S.tmem_base, 512);
-  fence_before_sync();
-  __syncthreads();
-  cluster_sync_all();                      // both CTAs' barriers are initialised before anyone signals them
-  fence_after_sync();
-  const uint32_t tmem = S.tmem_base;
-
-  if (warp == 0) {
-    // ---- loader (both CTAs): own window of group g, then own half of the 36 weight slabs
-    if (lane == 0) {
-      uint32_t s = 0, ph = 0, gi = 0;
-      auto load_window = [&](int g, uint32_t k) -> bool {
-        const uint32_t ab = k & 1;
-        if (!mbar_wait(&S.a_empty[ab], ((k >> 1) & 1) ^ 1, kWaitCycles)) return false;
-        mbar_arrive_expect_tx(&S.a_full[ab], P3_WIN_BYTES);
-        const size_t row0 = (size_t)g * 256 + (size_t)rank * P3_ROWS;
-        for (int pl = 0; pl < C3_PLANES; ++pl)
-          bulk_g2s(S.A[ab] + pl * P3_PLANE_BYTES, X3 + ((size_t)pl * a_pitch + row0) * 8, P3_PLANE_BYTES, &S.a_full[ab]);
-        return true;
-      };
-      if (cl < n_groups) { if (!load_window(cl, 0)) { atomicExch(err, 720); goto done; } }
-      for (int g = cl; g < n_groups; g += n_cl, ++gi) {
-        for (int tap = 0; tap < 9; ++tap) {
-          TC_WAIT(&S.empty[s], ph ^ 1, 721);
-          mbar_arrive_expect_tx(&S.full[s], P3_B_BYTES);
-          bulk_g2s(S.B[s], Bp + ((size_t)rank * C3_SLABS + tap * 4) * (P3_B_BYTES / 8), P3_B_BYTES, &S.full[s]);   // w3p: [half][slab][4][128][8]
-          if (++s == P3_STAGES) { s = 0; ph ^= 1; }
-          if (tap == 4 && g + n_cl < n_groups) {
-            if (!load_window(g + n_cl, gi + 1)) { atomicExch(err, 720); goto done; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1 && rank == 1) {
-    // ---- relay (peer CTA): tell the leader when this CTA's window / weight halves have landed
-    if (lane == 0) {
-      uint32_t sg = 0, ph = 0, gi = 0;
-      const uint32_t r_a_full = mapa_shared(smem_u32(&S.peer_a_full[0]), 0), r_full = mapa_shared(smem_u32(&S.peer_full[0]), 0);
-      for (int g = cl; g < n_groups; g += n_cl, ++gi) {
-        const uint32_t ab = gi & 1;
-        TC_WAIT(&S.a_full[ab], (gi >> 1) & 1, 722);
-        mbar_arrive_remote(r_a_full + ab * 8);
-        for (int tap = 0; tap < 9; ++tap) {
-          TC_WAIT(&S.full[sg], ph, 723);
-          mbar_arrive_remote(r_full + sg * 8);
-          if (++sg == P3_STAGES) { sg = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ---- MMA issuer (leader CTA only)
-    const uint32_t idesc = make_idesc_f16(256, 256);
-    const bool leader = elect_one() != 0;
-    const uint64_t ad0 = make_desc_kmajor_noswizzle(smem_u32(S.A[0]), P3_PLANE_BYTES, 128);
-    const uint64_t bd0 = make_desc_kmajor_noswizzle(smem_u32(S.B[0]), 128 * 16, 128);
-    const uint32_t ad_hi = (uint32_t)(ad0 >> 32), ad_lo = (uint32_t)ad0;
-    const uint32_t bd_hi = (uint32_t)(bd0 >> 32), bd_lo = (uint32_t)bd0;
-    uint32_t sg = 0, ph = 0, gi = 0;
-    for (int g = cl; g < n_groups; g += n_cl, ++gi) {
-      const uint32_t ab = gi & 1, db = gi & 1;
-      TC_WAIT(&S.a_full[ab], (gi >> 1) & 1, 724);
-      TC_WAIT(&S.peer_a_full[ab], (gi >> 1) & 1, 725);
-      TC_WAIT(&S.d_empty[db], ((gi >> 1) & 1) ^ 1, 726);
-      fence_after_sync();
-#pragma unroll 1
-      for (int tap = 0; tap < 9; ++tap) {
-        const uint32_t shift = (tap / 3) * NB + (tap % 3);                // rows
-        TC_WAIT(&S.full[sg], ph, 727);
-        TC_WAIT(&S.peer_full[sg], ph, 728);
-        fence_after_sync();
-        if (leader) {
-#pragma unroll
-          for (int gq = 0; gq < 4; ++gq) {                                // slab = (tap, 32-channel group)
-            const uint32_t b_off = (sg * P3_B_BYTES + gq * (4 * 128 * 16)) >> 4;
-#pragma unroll
-            for (int kk = 0; kk < 2; ++kk) {
-              const uint64_t bd = ((uint64_t)bd_hi << 32) | (uint64_t)(bd_lo + b_off + ((kk * 2 * (128 * 16)) >> 4));
-              const uint64_t ad = ((uint64_t)ad_hi << 32) |
-                                  (uint64_t)(ad_lo + ((ab * P3_WIN_BYTES + (gq * 4 + kk * 2) * P3_PLANE_BYTES + shift * 16) >> 4));
-              mma_ss_cta2(tmem + db * 256, ad, bd, idesc, (tap | gq | kk) != 0);
-            }
-          }
-          commit_cta2(&S.empty[sg]);
-        }
-        __syncwarp();
-        if (++sg == P3_STAGES) { sg = 0; ph ^= 1; }
-      }
-      if (leader) {
-        commit_cta2(&S.d_full[db]);
-        commit_cta2(&S.a_empty[ab]);
-      }
-      __syncwarp();
-    }
-  } else if (warp >= 4) {
-    // ---- epilogue (both CTAs, own 128 rows x all 256 channels): bias + ReLU -> Dense partial sums
-    const int q = warp & 3;
-    uint32_t gi = 0;
-    const uint32_t r_d_empty = mapa_shared(smem_u32(&S.d_empty[0]), 0);
-    for (int g = cl; g < n_groups; g += n_cl, ++gi) {
-      const uint32_t db = gi & 1;
-      TC_WAIT(&S.d_full[db], (gi >> 1) & 1, 729);
-      fence_after_sync();
-      const int64_t r = (int64_t)g * 256 + (int64_t)rank * P3_ROWS + q * 32 + lane;
-      const int rem = (int)(r % PAIR_ROWS);
-      const int yy = rem / NB, xx = rem - yy * NB;
-      const bool valid = (r < M) && (yy < NB - 2) && (xx < NB - 2);
-      // rows are (pair, jb, ib): yy = jb, xx = ib; Flatten order of the reference is (ib, jb, channel)
-      const float* wrow = wd + (size_t)(valid ? (xx * (NB - 2) + yy) : 0) * 256;
-#pragma unroll 1
-      for (int nh = 0; nh < 2; ++nh) {
-        float acc = 0.f;
-#pragma unroll 1
-        for (int c0 = 0; c0 < 128; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld_x32(tmem + ((uint32_t)(q * 32) << 16) + db * 256 + nh * 128 + c0, v);
-          float4 w[8];
-#pragma unroll
-          for (int j4 = 0; j4 < 8; ++j4) w[j4] = __ldg(reinterpret_cast<const float4*>(wrow + nh * 128 + c0) + j4);
-          tmem_ld_wait();
-          if (nh == 1 && c0 == 96) {          // the last accumulator columns of this group are in registers
-            fence_before_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_remote(r_d_empty + db * 8);      // the leader's barrier (also for the leader itself)
-          }
-          const float* bs = S.bias + nh * 128 + c0;
-#pragma unroll
-          for (int j4 = 0; j4 < 8; ++j4) {
-            acc = fmaf(fmaxf(__uint_as_float(v[j4 * 4 + 0]) + bs[j4 * 4 + 0], 0.f), w[j4].x, acc);
-            acc = fmaf(fmaxf(__uint_as_float(v[j4 * 4 + 1]) + bs[j4 * 4 + 1], 0.f), w[j4].y, acc);
-            acc = fmaf(fmaxf(__uint_as_float(v[j4 * 4 + 2]) + bs[j4 * 4 + 2], 0.f), w[j4].z, acc);
-            acc = fmaf(fmaxf(__uint_as_float(v[j4 * 4 + 3]) + bs[j4 * 4 + 3], 0.f), w[j4].w, acc);
-          }
-        }
-        if (r < M) partial[r * 2 + nh] = valid ? acc : 0.f;
-      }
-    }
-  }
-done:
-  fence_before_sync();
-  __syncthreads();
-  cluster_sync_all();                      // the leader's MMAs read the peer's shared memory until the very end
-  if (warp == 2) tmem_dealloc_cta2(tmem, 512);
-}
-
-// ------------------------------------------------------------------------------------------------
-// k_leg_resident_tc -- one leg layer in latency mode (single query scan).
-// Measured (profiles/r1_ncu_summary): the streamed GEMM needs 5 small bulk copies per K slab and a
-// CTA cannot get more than ~1 bulk copy per ~150 clk through, so a 108-slab layer took 45 us at 9 %
-// tensor activity.  Here the activation window of the CTA's 128 output pixels (kh input rows x
-// [hi, lo] x C_in/8 planes x (128 + kw - 1) pixels, <= 108 KB) is loaded once and every (dh, dw) tap
-// is a descriptor offset into it; only the weights move: one copy per (tap, split term) of
-// C_in x 64 x 2 B.  Three-term hi/lo split product as in the streamed leg (fp32-grade accuracy).
-// ------------------------------------------------------------------------------------------------
-constexpr int LR_WIN = 144;                       // 128 + max(kw) - 1 = 142, rounded to a multiple of 8
-constexpr int LR_A_MAX = 48 * LR_WIN * 16;        // 110 592 B (s_conv3a: 3 rows x 2 x 8 planes)
-constexpr int LR_B_MAX = 16 * 64 * 16;            // 16 384 B  (C_in = 128)
-constexpr int LR_STAGES = 5;
-
-struct LRSmem {
-  uint8_t A[LR_A_MAX];
-  uint8_t B[LR_STAGES][LR_B_MAX];
-  float bias[64];
-  uint64_t a_full, full[LR_STAGES], empty[LR_STAGES], d_full;
-  uint32_t tmem_base;
-};
-
 struct LegArgs {
   const __half* A; int64_t a_pitch;
   int runs_per_img, in_img_planes, in_run_planes;
   int kh, kw, c8in;
-  const __half* Bp;           // [cout/64][kh*kw*3][c8in][64][8]   (k_leg_batched_tc: stacked layout, see TcState::wstk)
-  int c8u;                    // k_leg_batched_tc: C_in/8 chunks per streamed weight unit
+  const __half* Bp;           // [cout/64][kh*kw*3][c8in][64][8]
   const float* bias; int n_valid;
   int64_t M;                  // output pixels per run
   __half* out_planes; int64_t out_pitch; int out_run_planes;   // EPI 4
   float* out_f32;                                               // EPI 3
-  int n_split;                // split-K: blockIdx.z = nh * n_split + split; each split takes a slab range
-  float* part;                // [tile][split][16 col4][128 rows] float4 partial accumulators (n_split > 1)
-  int* counters;              // [tile][4 lane quarters] arrival counters, left at zero
 };
 
-template <int EPI>
-__global__ void __launch_bounds__(G_THREADS, 1)
-k_leg_resident_tc(LegArgs g, int* __restrict__ err) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  LRSmem& S = *reinterpret_cast<LRSmem*>(smem_raw);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int64_t row0 = (int64_t)blockIdx.x * 128;
-  const int y = blockIdx.y, nh = blockIdx.z / g.n_split, split = blockIdx.z % g.n_split;
-  const int64_t in_base = (int64_t)(y / g.runs_per_img) * g.in_img_planes + (int64_t)(y % g.runs_per_img) * g.in_run_planes;
-  const int n_planes = g.kh * 2 * g.c8in;
-  const int n_slabs = g.kh * g.kw * 3;
-  // A single scan gives a layer only 8-56 output tiles, each a serial chain of up to 432 MMAs: the K
-  // loop is split over CTAs (slab ranges) and the last CTA to arrive sums the partials in split order.
-  const int sl0 = (int)((int64_t)n_slabs * split / g.n_split), sl1 = (int)((int64_t)n_slabs * (split + 1) / g.n_split);
-  const uint32_t b_bytes = (uint32_t)g.c8in * 64 * 16;
-  const int grp = (int)(LR_B_MAX / b_bytes) > 0 ? (int)(LR_B_MAX / b_bytes) : 1;      // slabs per ring stage
-
-  if (tid == 0) {
-    mbar_init(&S.a_full, 1);
-    for (int s = 0; s < LR_STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], 1); }
-    mbar_init(&S.d_full, 1);
-    mbar_fence_init();
-  }
-  if (tid < 64) S.bias[tid] = (nh * 64 + tid < g.n_valid) ? g.bias[nh * 64 + tid] : 0.f;
-  if (warp == 2) tmem_alloc(&S.tmem_base, 64);
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = S.tmem_base;
-  // Programmatic dependent launch: the layers of a single-scan leg are ~10 us kernels in a chain, so
-  // the next layer may start its prologue (barriers, TMEM, weight copies) while this one finishes.
-  // Only the activation window (and everything downstream of it) waits for the previous layer.
-  pdl_launch_dependents();
-
-  if (warp == 0) {
-    // weights of the first ring stages do not depend on the previous layer
-    uint32_t s = 0, ph = 0;
-    int sl = sl0;
-    for (; sl < sl1 && s < LR_STAGES; sl += grp) {
-      const int cnt = (sl1 - sl < grp) ? sl1 - sl : grp;
-      if (lane == 0) {
-        mbar_arrive_expect_tx(&S.full[s], (uint32_t)cnt * b_bytes);
-        bulk_g2s(S.B[s], g.Bp + ((size_t)nh * n_slabs + sl) * (b_bytes / 2), (uint32_t)cnt * b_bytes, &S.full[s]);
-      }
-      ++s;
-    }
-    if (s == LR_STAGES) { s = 0; ph = 1; }
-    pdl_wait();
-    // activation window: one copy per plane, issued by the lanes in parallel
-    if (lane == 0) mbar_arrive_expect_tx(&S.a_full, (uint32_t)n_planes * LR_WIN * 16);
-    __syncwarp();
-    for (int pl = lane; pl < n_planes; pl += 32)
-      bulk_g2s(S.A + (size_t)pl * LR_WIN * 16, g.A + ((size_t)(in_base + pl) * g.a_pitch + row0) * 8, LR_WIN * 16, &S.a_full);
-    // weights: consecutive (dh, dw, term) slabs are contiguous in memory, so a ring stage takes as
-    // many of them as fit (a 2 KB slab per copy made s_conv2 a chain of 135 copy round trips)
-    for (; sl < sl1; sl += grp) {
-      const int cnt = (sl1 - sl < grp) ? sl1 - sl : grp;
-      TC_WAIT(&S.empty[s], ph ^ 1, 801);
-      if (lane == 0) {
-        mbar_arrive_expect_tx(&S.full[s], (uint32_t)cnt * b_bytes);
-        bulk_g2s(S.B[s], g.Bp + ((size_t)nh * n_slabs + sl) * (b_bytes / 2), (uint32_t)cnt * b_bytes, &S.full[s]);
-      }
-      __syncwarp();
-      if (++s == LR_STAGES) { s = 0; ph ^= 1; }
-    }
-  } else if (warp == 1) {
-    const uint32_t idesc = make_idesc_f16(128, 64);
-    const bool leader = elect_one() != 0;
-    const uint64_t ad0 = make_desc_kmajor_noswizzle(smem_u32(S.A), LR_WIN * 16, 128);
-    const uint64_t bd0 = make_desc_kmajor_noswizzle(smem_u32(S.B[0]), 64 * 16, 128);
-    const uint32_t ad_hi = (uint32_t)(ad0 >> 32), ad_lo = (uint32_t)ad0;
-    const uint32_t bd_hi = (uint32_t)(bd0 >> 32), bd_lo = (uint32_t)bd0;
-    TC_WAIT(&S.a_full, 0, 802);
-    uint32_t sg = 0, ph = 0, first = 1;
-    int term = sl0 % 3, dw = (sl0 / 3) % g.kw, dh = sl0 / (3 * g.kw);   // slab = (dh, dw, term); x*w ~= xh*wh + xl*wh + xh*wl
-#pragma unroll 1
-    for (int sl = sl0; sl < sl1; sl += grp) {
-      const int cnt = (sl1 - sl < grp) ? sl1 - sl : grp;
-      TC_WAIT(&S.full[sg], ph, 803);
-      fence_after_sync();
-      for (int j = 0; j < cnt; ++j) {
-        if (leader) {
-          const uint32_t kind = (term == 1) ? 1u : 0u;
-          const uint32_t a_k = ad_lo + ((((dh * 2 + kind) * g.c8in) * (LR_WIN * 16) + dw * 16) >> 4);
-          const uint32_t b_k = bd_lo + ((sg * LR_B_MAX + j * b_bytes) >> 4);
-          for (int c16 = 0; c16 < g.c8in / 2; ++c16) {
-            const uint64_t ad = ((uint64_t)ad_hi << 32) | (uint64_t)(a_k + ((c16 * 2 * (LR_WIN * 16)) >> 4));
-            const uint64_t bd = ((uint64_t)bd_hi << 32) | (uint64_t)(b_k + ((c16 * 2 * (64 * 16)) >> 4));
-            mma_ss(tmem, ad, bd, idesc, first ? 0u : 1u);
-            first = 0;
-          }
-        }
-        first = 0;
-        if (++term == 3) { term = 0; if (++dw == g.kw) { dw = 0; ++dh; } }
-      }
-      if (leader) commit(&S.empty[sg]);
-      __syncwarp();
-      if (++sg == LR_STAGES) { sg = 0; ph ^= 1; }
-    }
-    if (leader) commit(&S.d_full);
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    pdl_wait();                               // the split-K workspace and the output planes belong to the previous layer until now
-    TC_WAIT(&S.d_full, 0, 804);
-    fence_after_sync();
-    const int64_t r = row0 + q * 32 + lane;
-    const int nz = gridDim.z / g.n_split;
-    const int tile_id = (int)((blockIdx.y * gridDim.x + blockIdx.x) * nz + nh);
-    const float4* parts = reinterpret_cast<const float4*>(g.part) + (size_t)tile_id * g.n_split * 16 * 128 + q * 32 + lane;
-    bool emit = true;
-    if (g.n_split > 1) {
-      float4* mine = reinterpret_cast<float4*>(g.part) + ((size_t)tile_id * g.n_split + split) * 16 * 128 + q * 32 + lane;
-#pragma unroll 1
-      for (int c0 = 0; c0 < 64; c0 += 16) {
-        uint32_t v[16];
-        tmem_ld_x16(tmem + ((uint32_t)(q * 32) << 16) + c0, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4)
-          mine[((c0 >> 2) + j4) * 128] = make_float4(__uint_as_float(v[j4 * 4 + 0]), __uint_as_float(v[j4 * 4 + 1]),
-                                                     __uint_as_float(v[j4 * 4 + 2]), __uint_as_float(v[j4 * 4 + 3]));
-      }
-      __threadfence();
-      __syncwarp();
-      int prev = 0;
-      if (lane == 0) prev = atomicAdd(g.counters + tile_id * 4 + q, 1);
-      prev = __shfl_sync(0xffffffffu, prev, 0);
-      emit = (prev == g.n_split - 1);            // this warp's rows are complete in every split
-      if (emit) {
-        __threadfence();
-        if (lane == 0) g.counters[tile_id * 4 + q] = 0;
-      }
-    }
-    if (emit) {
-#pragma unroll 1
-    for (int c0 = 0; c0 < 64; c0 += 16) {
-      float v[16];
-      if (g.n_split > 1) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = 0.f;
-        for (int sp = 0; sp < g.n_split; ++sp) {     // fixed order: bit-reproducible
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            const float4 t = __ldcg(parts + ((size_t)sp * 16 + (c0 >> 2) + j4) * 128);
-            v[j4 * 4 + 0] += t.x; v[j4 * 4 + 1] += t.y; v[j4 * 4 + 2] += t.z; v[j4 * 4 + 3] += t.w;
-          }
-        }
-      } else {
-        uint32_t u[16];
-        tmem_ld_x16(tmem + ((uint32_t)(q * 32) << 16) + c0, u);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(u[j]);
-      }
-      if (r < g.M && nh * 64 + c0 < g.n_valid) {
-        if (EPI == 4) {
-#pragma unroll
-          for (int h8 = 0; h8 < 2; ++h8) {
-            uint32_t phh[4], pll[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const int n = c0 + h8 * 8 + 2 * j;
-              const float a = fmaxf(v[h8 * 8 + 2 * j] + S.bias[n], 0.f);
-              const float b = fmaxf(v[h8 * 8 + 2 * j + 1] + S.bias[n + 1], 0.f);
-              const __half2 hi = __floats2half2_rn(a, b);
-              const float2 hf = __half22float2(hi);
-              const __half2 lo = __floats2half2_rn(a - hf.x, b - hf.y);
-              phh[j] = *reinterpret_cast<const uint32_t*>(&hi);
-              pll[j] = *reinterpret_cast<const uint32_t*>(&lo);
-            }
-            const int c8 = nh * 8 + (c0 >> 3) + h8;
-            const int64_t plane = (int64_t)y * g.out_run_planes + c8;
-            *reinterpret_cast<uint4*>(g.out_planes + ((size_t)plane * g.out_pitch + r) * 8) = make_uint4(phh[0], phh[1], phh[2], phh[3]);
-            *reinterpret_cast<uint4*>(g.out_planes + ((size_t)(plane + g.out_run_planes / 2) * g.out_pitch + r) * 8) =
-                make_uint4(pll[0], pll[1], pll[2], pll[3]);
-          }
-        } else {
-          float* dst = g.out_f32 + ((size_t)y * g.M + r) * g.n_valid + nh * 64 + c0;
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            float4 o;
-            o.x = fmaxf(v[j4 * 4 + 0] + S.bias[c0 + j4 * 4 + 0], 0.f);
-            o.y = fmaxf(v[j4 * 4 + 1] + S.bias[c0 + j4 * 4 + 1], 0.f);
-            o.z = fmaxf(v[j4 * 4 + 2] + S.bias[c0 + j4 * 4 + 2], 0.f);
-            o.w = fmaxf(v[j4 * 4 + 3] + S.bias[c0 + j4 * 4 + 3], 0.f);
-            reinterpret_cast<float4*>(dst)[j4] = o;
-          }
-        }
-      }
-    }
-    }
-  }
-done:
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem, 64);
-}
-
-// ------------------------------------------------------------------------------------------------
-// k_leg_batched_tc -- one leg layer for a BATCH of scans (throughput mode).
-// The streamed GEMM (k_gemm_stream_tc) re-read the activation rows from L2 for every (dh, dw, term) tap:
-// 103 MB of L2 -> shared traffic per scan, 5.9 TB/s at 17.5 us/scan -- L2-bandwidth bound (profiles/
-// r2_leg_batched.txt).  Here, as in the latency-mode kernel, the activation window of the CTA's output
-// pixels is loaded ONCE and every tap is a descriptor offset; a CTA owns TILES consecutive 128-pixel
-// tiles so that each streamed weight slab is used TILES times (27 MB of L2 traffic per scan).
-// No split-K: a batch gives every layer enough tiles to fill the GPU.
-// ------------------------------------------------------------------------------------------------
-constexpr int LB_A_MAX = 139264;                  // 2 x 2 x 8 planes x 272 px x 16 B (s_conv4 with two tiles)
-
-constexpr int LB_A_FAT = 188416;                  // layer 1 with 25 input channels: 5 x 2 x 8 planes x 144 px x 16 B (+ slack)
-
-template <int STAGES, int A_MAX>
-struct LBSmemT {
-  uint8_t A[A_MAX];
-  uint8_t B[STAGES][LR_B_MAX];
-  float bias[128];
-  uint64_t a_full, full[STAGES], empty[STAGES], d_full;
-  uint32_t tmem_base;
-};
-using LBSmem = LBSmemT<LR_STAGES, LB_A_MAX>;
-using LBSmemFat = LBSmemT<2, LB_A_FAT>;          // a fat window leaves room for a 2-stage weight ring only
-
-template <int EPI, int TILES, int STAGES = LR_STAGES, int A_MAX = LB_A_MAX>
-__global__ void __launch_bounds__(G_THREADS, 1)
-k_leg_batched_tc(LegArgs g, int n_mma, int* __restrict__ err) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  using Smem = LBSmemT<STAGES, A_MAX>;
-  Smem& S = *reinterpret_cast<Smem*>(smem_raw);
-  constexpr int WIN = TILES * 128 + 16;             // pixels per window plane (kw <= 15)
-  // per tile: accumulator columns [0, n_mma) and [n_mma, 2 n_mma), summed by the epilogue (n_mma = 128: TILES <= 2)
-  const uint32_t tcol = n_mma > 64 ? 256u : 128u;
-  const uint32_t TMEM_COLS = TILES * tcol;
-  const int n_cols = n_mma > 64 ? 128 : 64;         // output channels of this CTA
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int64_t row0 = (int64_t)blockIdx.x * (TILES * 128);
-  const int y = blockIdx.y, nh = blockIdx.z;
-  const int64_t in_base = (int64_t)(y / g.runs_per_img) * g.in_img_planes + (int64_t)(y % g.runs_per_img) * g.in_run_planes;
-  const int n_planes = g.kh * 2 * g.c8in;
-  const int R = 2 * n_mma;                          // stacked weight rows per unit: [hi | lo]
-  const int kc_n = g.c8in / g.c8u;
-  const int n_slabs = g.kh * g.kw * kc_n;           // streamed weight units: (dh, dw, C_in chunk)
-  const uint32_t b_bytes = (uint32_t)g.c8u * R * 16;
-  const int grp = (int)(LR_B_MAX / b_bytes) > 0 ? (int)(LR_B_MAX / b_bytes) : 1;      // units per ring stage
-  int nt = (int)((g.M - row0 + 127) / 128);         // tiles of this CTA that hold valid pixels
-  if (nt > TILES) nt = TILES;
-
-  if (tid == 0) {
-    mbar_init(&S.a_full, 1);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], 1); }
-    mbar_init(&S.d_full, 1);
-    mbar_fence_init();
-  }
-  if (tid < 128) S.bias[tid] = (nh * 64 + tid < g.n_valid) ? g.bias[nh * 64 + tid] : 0.f;
-  if (warp == 2) tmem_alloc(&S.tmem_base, TMEM_COLS);
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = S.tmem_base;
-
-  if (warp == 0) {
-    if (lane == 0) mbar_arrive_expect_tx(&S.a_full, (uint32_t)n_planes * WIN * 16);
-    __syncwarp();
-    for (int pl = lane; pl < n_planes; pl += 32)
-      bulk_g2s(S.A + (size_t)pl * WIN * 16, g.A + ((size_t)(in_base + pl) * g.a_pitch + row0) * 8, WIN * 16, &S.a_full);
-    uint32_t s = 0, ph = 0;
-    for (int sl = 0; sl < n_slabs; sl += grp) {
-      const int cnt = (n_slabs - sl < grp) ? n_slabs - sl : grp;
-      TC_WAIT(&S.empty[s], ph ^ 1, 811);
-      if (lane == 0) {
-        mbar_arrive_expect_tx(&S.full[s], (uint32_t)cnt * b_bytes);
-        bulk_g2s(S.B[s], g.Bp + ((size_t)nh * n_slabs + sl) * (b_bytes / 2), (uint32_t)cnt * b_bytes, &S.full[s]);
-      }
-      __syncwarp();
-      if (++s == STAGES) { s = 0; ph ^= 1; }
-    }
-  } else if (warp == 1) {
-    const uint32_t idesc2 = make_idesc_f16(128, R), idesc1 = make_idesc_f16(128, n_mma);
-    const bool leader = elect_one() != 0;
-    const uint64_t ad0 = make_desc_kmajor_noswizzle(smem_u32(S.A), WIN * 16, 128);
-    const uint64_t bd0 = make_desc_kmajor_noswizzle(smem_u32(S.B[0]), R * 16, 128);
-    const uint32_t ad_hi = (uint32_t)(ad0 >> 32), ad_lo = (uint32_t)ad0;
-    const uint32_t bd_hi = (uint32_t)(bd0 >> 32), bd_lo = (uint32_t)bd0;
-    const uint32_t lo_off = (uint32_t)((g.c8in * (WIN * 16)) >> 4);    // hi planes -> lo planes of the same input row
-    TC_WAIT(&S.a_full, 0, 812);
-    uint32_t sg = 0, ph = 0, first = 1;
-    int kc = 0, dw = 0, dh = 0;                     // unit = (dh, dw, kc)
-#pragma unroll 1
-    for (int sl = 0; sl < n_slabs; sl += grp) {
-      const int cnt = (n_slabs - sl < grp) ? n_slabs - sl : grp;
-      TC_WAIT(&S.full[sg], ph, 813);
-      fence_after_sync();
-      for (int j = 0; j < cnt; ++j) {
-        if (leader) {
-          const uint32_t a_k = ad_lo + ((((dh * 2) * g.c8in + kc * g.c8u) * (WIN * 16) + dw * 16) >> 4);
-          const uint32_t b_k = bd_lo + ((sg * LR_B_MAX + j * b_bytes) >> 4);
-          for (int c16 = 0; c16 < g.c8u / 2; ++c16) {
-            const uint64_t bd = ((uint64_t)bd_hi << 32) | (uint64_t)(b_k + ((c16 * 2 * (R * 16)) >> 4));
-            const uint32_t a_c = a_k + ((c16 * 2 * (WIN * 16)) >> 4);
-#pragma unroll
-            for (int t = 0; t < TILES; ++t) {
-              if (t < nt) {
-                const uint64_t adh = ((uint64_t)ad_hi << 32) | (uint64_t)(a_c + ((t * 128 * 16) >> 4));
-                const uint64_t adl = ((uint64_t)ad_hi << 32) | (uint64_t)(a_c + lo_off + ((t * 128 * 16) >> 4));
-                mma_ss(tmem + t * tcol, adh, bd, idesc2, first ? 0u : 1u);     // xh * [wh | wl] -> columns [0, 2 n_mma)
-                mma_ss(tmem + t * tcol, adl, bd, idesc1, 1u);                  // xl * wh        -> columns [0, n_mma)
-              }
-            }
-            first = 0;
-          }
-        }
-        first = 0;
-        if (++kc == kc_n) { kc = 0; if (++dw == g.kw) { dw = 0; ++dh; } }
-      }
-      if (leader) commit(&S.empty[sg]);
-      __syncwarp();
-      if (++sg == STAGES) { sg = 0; ph ^= 1; }
-    }
-    if (leader) commit(&S.d_full);
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    TC_WAIT(&S.d_full, 0, 814);
-    fence_after_sync();
-#pragma unroll 1
-    for (int t = 0; t < nt; ++t) {
-      const int64_t r = row0 + t * 128 + q * 32 + lane;
-#pragma unroll 1
-      for (int c0 = 0; c0 < n_cols; c0 += 16) {
-        if (nh * 64 + c0 >= g.n_valid) break;         // warp-uniform
-        uint32_t u[16], u2[16];
-        tmem_ld_x16(tmem + ((uint32_t)(q * 32) << 16) + t * tcol + c0, u);
-        tmem_ld_x16(tmem + ((uint32_t)(q * 32) << 16) + t * tcol + n_mma + c0, u2);
-        tmem_ld_wait();
-        if (r < g.M) {
-          float v[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(u[j]) + __uint_as_float(u2[j]);
-          if (EPI == 4) {
-#pragma unroll
-            for (int h8 = 0; h8 < 2; ++h8) {
-              uint32_t phh[4], pll[4];
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const int n = c0 + h8 * 8 + 2 * j;
-                const float a = fmaxf(v[h8 * 8 + 2 * j] + S.bias[n], 0.f);
-                const float b = fmaxf(v[h8 * 8 + 2 * j + 1] + S.bias[n + 1], 0.f);
-                const __half2 hi = __floats2half2_rn(a, b);
-                const float2 hf = __half22float2(hi);
-                const __half2 lo = __floats2half2_rn(a - hf.x, b - hf.y);
-                phh[j] = *reinterpret_cast<const uint32_t*>(&hi);
-                pll[j] = *reinterpret_cast<const uint32_t*>(&lo);
-              }
-              const int c8 = nh * 8 + (c0 >> 3) + h8;
-              const int64_t plane = (int64_t)y * g.out_run_planes + c8;
-              *reinterpret_cast<uint4*>(g.out_planes + ((size_t)plane * g.out_pitch + r) * 8) = make_uint4(phh[0], phh[1], phh[2], phh[3]);
-              *reinterpret_cast<uint4*>(g.out_planes + ((size_t)(plane + g.out_run_planes / 2) * g.out_pitch + r) * 8) =
-                  make_uint4(pll[0], pll[1], pll[2], pll[3]);
-            }
-          } else {
-            float* dst = g.out_f32 + ((size_t)y * g.M + r) * g.n_valid + nh * 64 + c0;
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              float4 o;
-              o.x = fmaxf(v[j4 * 4 + 0] + S.bias[c0 + j4 * 4 + 0], 0.f);
-              o.y = fmaxf(v[j4 * 4 + 1] + S.bias[c0 + j4 * 4 + 1], 0.f);
-              o.z = fmaxf(v[j4 * 4 + 2] + S.bias[c0 + j4 * 4 + 2], 0.f);
-              o.w = fmaxf(v[j4 * 4 + 3] + S.bias[c0 + j4 * 4 + 3], 0.f);
-              reinterpret_cast<float4*>(dst)[j4] = o;
-            }
-          }
-        }
-      }
-    }
-  }
-done:
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem, TMEM_COLS);
-}
-
-// ------------------------------------------------------------------------------------------------
-// Correlation (yaw) head on tensor cores.
-//   G = L R^T (360 x 360, K = 128), corr[k] = sum_j G[(k + j + 180) mod 360, j]
-//   (RangePadding2D.py:34 + NormalizedCorrelation2D.py:96-109), yaw = 180 - argmax (infer.py:158).
-// fp16 alone (10-bit mantissa) is not enough to keep the argmax of a flat correlation curve, so the
-// operands are split hi/lo (x = hi + lo exactly to 2^-22) and G = Lhi Rhi + Llo Rhi + Lhi Rlo is
-// accumulated in fp32 in TMEM: three tcgen05.mma per K16 step, fp32-grade result, still < 5 % of
-// c_conv1's tensor time.  One CTA owns one half of R's rows (N = 192, zero-padded past 360) for all
-// of its pairs; L arrives as 32 KB stages (row tile x K half, hi+lo) through a 3-deep bulk-copy
-// ring.  The diagonal sums never touch memory: eight epilogue warps read 32-row x 32-column chunks of a
-// finished 128 x 192 tile from TMEM and sum along the diagonals with two lane reduce-scatters whose send
-// register absorbs the per-lane rotation (see the epilogue below); partial bins live in shared memory.
-// ------------------------------------------------------------------------------------------------
-constexpr int C6_THREADS = 384;            // warps 0-2: loader, MMA issuer, TMEM owner; warps 4-11: epilogue (2 per TMEM lane quarter)
-constexpr int C6_STAGES = 3;
 constexpr int C6_STAGE_BYTES = 32768;            // [hi,lo][8 planes][128 rows][8] fp16
 constexpr int C6_R_BYTES = 98304;                // [hi,lo][16 planes][192 rows][8] fp16
 constexpr int C6_VOL_L_BYTES = 6 * C6_STAGE_BYTES;
 constexpr int C6_VOL_R_BYTES = 2 * C6_R_BYTES;
 
-struct C6Smem {
-  uint8_t R[C6_R_BYTES];
-  uint8_t A[C6_STAGES][C6_STAGE_BYTES];
-  float corr[8][WF];
-  uint64_t full[C6_STAGES], empty[C6_STAGES], d_full[2], d_empty[2], r_full, r_empty, epi;
-  uint32_t tmem_base;
-};
 
-// fp32 volumes -> hi/lo fp16 split in the stage layout of k_corr_tc (zero rows past 360)
+// fp32 volumes -> hi/lo fp16 split in the operand layout of k_corr_mma (zero rows past 360)
 __global__ void __launch_bounds__(256)
 k_pack_corr_L(const float* __restrict__ bank, const int32_t* __restrict__ idx, int n, __half* __restrict__ out) {
   // one thread per (pair, tile, khalf, plane j, row): 8 channels
@@ -1593,186 +210,466 @@ k_pack_corr_R(const float* __restrict__ bank, const int32_t* __restrict__ idx, i
   *reinterpret_cast<uint4*>(base + (C6_R_BYTES / 4) + ((size_t)pl * 192 + row) * 8) = *reinterpret_cast<const uint4*>(lo);
 }
 
-__device__ __forceinline__ int wrap360(int x) {
-  x %= WF;
-  return x < 0 ? x + WF : x;
+// ------------------------------------------------------------------------------------------------
+// Warp-level tensor-core building blocks (mma.sync m16n8k16, f16 x f16 -> f32).
+// Fragment ownership (PTX ISA, "Matrix fragments for mma.m16n8k16"): g = lane / 4, t = lane % 4;
+//   A (16 x 16, row-major): a0 = (g, 2t..2t+1), a1 = (g + 8, 2t..), a2 = (g, 2t + 8..), a3 = (g + 8, 2t + 8..)
+//   B (16 x 8, K-major):    b0 = (k = 2t..2t+1, n = g), b1 = (k = 2t + 8.., n = g)
+//   D (16 x 8):             d0, d1 = (g, 2t..2t+1), d2, d3 = (g + 8, 2t..2t+1)
+// Every operand below is stored with 8 consecutive K values (16 bytes) contiguous, so each fragment
+// register is one aligned 32-bit load.  A block is 4 warps; a warp owns 16 output rows.
+// ------------------------------------------------------------------------------------------------
+constexpr int MMA_THREADS = 128;
+constexpr int MMA_ROWS = 64;                       // output rows per block (4 warps x 16)
+
+__device__ __forceinline__ void mma16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                         uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
-__global__ void __launch_bounds__(C6_THREADS, 1)
-k_corr_tc(const __half* __restrict__ Lc, const int32_t* __restrict__ l_idx, const __half* __restrict__ Rc,
-          int r_per_pair, int n_pairs,
-          float* __restrict__ corr_part, int* __restrict__ err) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  C6Smem& S = *reinterpret_cast<C6Smem*>(smem_raw);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int h = blockIdx.x & 1;
-  const int cta = blockIdx.x >> 1, n_cta = gridDim.x >> 1;
+__device__ __forceinline__ uint32_t ld_h2(const __half* p) { return __ldg(reinterpret_cast<const unsigned int*>(p)); }
 
+// |a - b| of two packed fp16 pairs: subtract, then clear both sign bits
+__device__ __forceinline__ uint32_t absdiff_h2(uint32_t a, uint32_t b) {
+  const __half2 d = __hsub2(*reinterpret_cast<const __half2*>(&a), *reinterpret_cast<const __half2*>(&b));
+  return *reinterpret_cast<const uint32_t*>(&d) & 0x7fff7fffu;
+}
+
+__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+// ------------------------------------------------------------------------------------------------
+// k_delta_conv1_wgmma -- DeltaLayer + c_conv1 without the delta tensor (83 % of the FLOPs of a pair).
+//   GEMM per work unit (pair, jb):  o1[i, o] = sum_{dj < 15, c < 128} |L[i, c] - R[15 jb + dj, c]| W1[dj, c, o] - mu_o1[o]
+//   M = 360 LEFT rows (6 row tiles of 64, rows past 360 masked), N = 64, K = 1920 (60 W1 slices of 32 channels).
+// Warp specialisation: warp 12 is the producer (one lane issues bulk copies): the LEFT volume of the current
+// pair (98 KB, once per pair), the 15 RIGHT rows of a unit (double-buffered) and W1 in groups of 6 slices
+// (24 KB) through a 4-deep ring, each buffer guarded by a full / empty mbarrier pair.  Warpgroups 0-2 are
+// the consumers: warpgroup w owns row tiles w and w + 3 (2 x 32 fp32 accumulators per thread).  The A
+// operand |l - r| is synthesised in registers from the LEFT rows (kept in registers for a 32-channel chunk)
+// and the broadcast RIGHT row, and multiplied by wgmma in register-A mode against the W1 slice in shared
+// memory: the 66 MB delta tensor of a pair is never written.  The accumulators start at the fp16-rounded
+// -mu_o1 (the centre that k_fold_bias2 pushes through c_conv2).  Output: fp16 o1 tiles.
+// Persistent: each CTA takes a contiguous range of the n_pairs * 24 units.
+// ------------------------------------------------------------------------------------------------
+constexpr int K4_WG = 3;                               // consumer warpgroups
+constexpr int K4_THREADS = K4_WG * 128 + 32;           // + the producer warp
+constexpr int K4_GROUP = 6;                            // W1 slices per bulk copy
+constexpr int K4_NGROUPS = K4_STEPS / K4_GROUP;        // 10 per unit
+constexpr int K4_RING = 4;
+constexpr int K4_BSLICE = 4096;                        // bytes of W1 per slice: [4 k8][64 o][8]
+constexpr uint32_t K4_VOL_BYTES = WF * K4_PITCH * 2;
+constexpr uint32_t K4_RWIN_BYTES = S15 * K4_PITCH * 2;
+constexpr long long kWaitCycles = 1ll << 28;
+
+struct K4Smem {
+  __half L[WF * K4_PITCH];
+  __half Rw[2][S15 * K4_PITCH];
+  __half B[K4_RING][K4_GROUP * K4_BSLICE / 2];
+  uint64_t full[K4_RING], empty[K4_RING], l_full, l_empty, rw_full[2], rw_empty[2];
+};
+static_assert(sizeof(K4Smem) <= 232448, "k_delta_conv1_wgmma shared memory");
+static_assert(offsetof(K4Smem, B) % 16 == 0 && offsetof(K4Smem, Rw) % 16 == 0, "bulk-copy alignment");
+
+#define K4_WAIT(bar, parity, code)                         \
+  if (!mbar_wait((bar), (parity), kWaitCycles)) {          \
+    atomicExch(err, (code));                               \
+    goto done;                                             \
+  }
+
+__global__ void __launch_bounds__(K4_THREADS, 1)
+k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ l_idx, const __half* __restrict__ R16,
+                    int r_per_pair, const __half* __restrict__ W1p, const float* __restrict__ mu_o1,
+                    __half* __restrict__ o1, int n_pairs, int* __restrict__ err) {
+  extern __shared__ __align__(128) uint8_t smem_raw[];
+  K4Smem& S = *reinterpret_cast<K4Smem*>(smem_raw);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int64_t n_units = (int64_t)n_pairs * NB;
+  const int u_begin = (int)(n_units * blockIdx.x / gridDim.x), u_end = (int)(n_units * (blockIdx.x + 1) / gridDim.x);
+  constexpr uint32_t kConsumerWarps = K4_WG * 4;
   if (tid == 0) {
-    for (int s = 0; s < C6_STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&S.d_full[b], 1); mbar_init(&S.d_empty[b], 8); }
-    mbar_init(&S.r_full, 1); mbar_init(&S.r_empty, 1); mbar_init(&S.epi, 8);
+    for (int s = 0; s < K4_RING; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], kConsumerWarps); }
+    mbar_init(&S.l_full, 1); mbar_init(&S.l_empty, kConsumerWarps);
+    for (int b = 0; b < 2; ++b) { mbar_init(&S.rw_full[b], 1); mbar_init(&S.rw_empty[b], kConsumerWarps); }
     mbar_fence_init();
   }
-  if (warp == 2) tmem_alloc(&S.tmem_base, 512);
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = S.tmem_base;
 
-  if (warp == 0) {
+  if (warp == K4_WG * 4) {
+    // ===================== producer ==========================================================
     if (lane == 0) {
-      if (!r_per_pair) {
-        mbar_arrive_expect_tx(&S.r_full, C6_R_BYTES);
-        bulk_g2s(S.R, reinterpret_cast<const uint8_t*>(Rc) + (size_t)h * C6_R_BYTES, C6_R_BYTES, &S.r_full);
-      }
-      uint32_t it = 0, pi = 0;
-      for (int p = cta; p < n_pairs; p += n_cta, ++pi) {
-        if (r_per_pair) {
-          TC_WAIT(&S.r_empty, (pi & 1) ^ 1, 601);
-          mbar_arrive_expect_tx(&S.r_full, C6_R_BYTES);
-          bulk_g2s(S.R, reinterpret_cast<const uint8_t*>(Rc) + (size_t)p * C6_VOL_R_BYTES + (size_t)h * C6_R_BYTES,
-                   C6_R_BYTES, &S.r_full);
+      uint32_t pi = 0, gi = 0, ui = 0;
+      for (int u = u_begin; u < u_end; ++u, ++ui) {
+        const int p = u / NB, jb = u - p * NB;
+        if (u == u_begin || jb == 0) {
+          K4_WAIT(&S.l_empty, (pi & 1) ^ 1, 101);
+          mbar_arrive_expect_tx(&S.l_full, K4_VOL_BYTES);
+          bulk_g2s(S.L, L16 + (size_t)(l_idx ? l_idx[p] : p) * WF * K4_PITCH, K4_VOL_BYTES, &S.l_full);
+          ++pi;
         }
-        const int64_t lrow = l_idx ? l_idx[p] : p;
-        for (int st = 0; st < 6; ++st, ++it) {
-          const uint32_t s = it % C6_STAGES, ph = (it / C6_STAGES) & 1;
-          TC_WAIT(&S.empty[s], ph ^ 1, 602);
-          mbar_arrive_expect_tx(&S.full[s], C6_STAGE_BYTES);
-          bulk_g2s(S.A[s], reinterpret_cast<const uint8_t*>(Lc) + (size_t)lrow * C6_VOL_L_BYTES + (size_t)st * C6_STAGE_BYTES,
-                   C6_STAGE_BYTES, &S.full[s]);
+        const uint32_t b = ui & 1;
+        K4_WAIT(&S.rw_empty[b], ((ui >> 1) & 1) ^ 1, 103);
+        mbar_arrive_expect_tx(&S.rw_full[b], K4_RWIN_BYTES);
+        bulk_g2s(S.Rw[b], R16 + (r_per_pair ? (size_t)p * WF * K4_PITCH : 0) + (size_t)jb * S15 * K4_PITCH, K4_RWIN_BYTES,
+                 &S.rw_full[b]);
+        for (int grp = 0; grp < K4_NGROUPS; ++grp, ++gi) {
+          const uint32_t s = gi % K4_RING, ph = (gi / K4_RING) & 1;
+          K4_WAIT(&S.empty[s], ph ^ 1, 102);
+          mbar_arrive_expect_tx(&S.full[s], K4_GROUP * K4_BSLICE);
+          bulk_g2s(S.B[s], W1p + (size_t)grp * K4_GROUP * (K4_BSLICE / 2), K4_GROUP * K4_BSLICE, &S.full[s]);
         }
-      }
-    }
-  } else if (warp == 1) {
-    {
-      const uint32_t idesc = make_idesc_f16(128, 192);
-      const bool leader = elect_one() != 0;
-      const uint64_t ad0 = make_desc_kmajor_noswizzle(smem_u32(S.A[0]), 2048, 128);
-      const uint64_t bd0 = make_desc_kmajor_noswizzle(smem_u32(S.R), 3072, 128);
-      const uint32_t ad_hi = (uint32_t)(ad0 >> 32), ad_lo = (uint32_t)ad0;
-      const uint32_t bd_hi = (uint32_t)(bd0 >> 32), bd_lo = (uint32_t)bd0;
-      uint32_t sg = 0, ph = 0, tileit = 0, pi = 0;
-      if (!r_per_pair) { TC_WAIT(&S.r_full, 0, 603); }
-      for (int p = cta; p < n_pairs; p += n_cta, ++pi) {
-        if (r_per_pair) { TC_WAIT(&S.r_full, pi & 1, 604); }
-        for (int t = 0; t < 3; ++t, ++tileit) {
-          const uint32_t buf = tileit & 1;
-          TC_WAIT(&S.d_empty[buf], ((tileit >> 1) & 1) ^ 1, 605);
-          fence_after_sync();
-#pragma unroll
-          for (int kh = 0; kh < 2; ++kh) {
-            TC_WAIT(&S.full[sg], ph, 606);
-            fence_after_sync();
-            if (leader) {
-              const uint32_t a_off = (sg * C6_STAGE_BYTES) >> 4;
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) {
-                const uint64_t a_hi = ((uint64_t)ad_hi << 32) | (uint64_t)(ad_lo + a_off + ((kk * 2 * 2048) >> 4));
-                const uint64_t a_lo = ((uint64_t)ad_hi << 32) | (uint64_t)(ad_lo + a_off + ((16384 + kk * 2 * 2048) >> 4));
-                const uint64_t b_hi = ((uint64_t)bd_hi << 32) | (uint64_t)(bd_lo + (((kh * 8 + kk * 2) * 3072) >> 4));
-                const uint64_t b_lo = ((uint64_t)bd_hi << 32) | (uint64_t)(bd_lo + ((49152 + (kh * 8 + kk * 2) * 3072) >> 4));
-                mma_ss(tmem + buf * 192, a_hi, b_hi, idesc, (kh | kk) != 0);
-                mma_ss(tmem + buf * 192, a_lo, b_hi, idesc, 1);
-                mma_ss(tmem + buf * 192, a_hi, b_lo, idesc, 1);
-              }
-              commit(&S.empty[sg]);
-            }
-            __syncwarp();
-            if (++sg == C6_STAGES) { sg = 0; ph ^= 1; }
-          }
-          if (leader) commit(&S.d_full[buf]);
-          __syncwarp();
-        }
-        if (r_per_pair && leader) commit(&S.r_empty);
-        __syncwarp();
       }
     }
-  } else if (warp >= 4) {
-    // ---- epilogue: corr[(i - j - 180) mod 360] += G[i][j], i.e. sums along the diagonals of the tile.
-    // Lane l holds row i0 + l, registers v[cc] the columns j0 + cc of a 32-column chunk; element
-    // (l, cc) lies on diagonal d = l - cc.  A first version walked the columns with a rotating
-    // accumulator (two dependent shuffles per column: 60 clk x 192 columns per tile, 3x the MMA time).
-    // Now: two masked reduce-scatters over the lanes (31 shuffles each, all independent within a stage)
-    // whose send register depends on the lane bit, which absorbs the per-lane rotation that lines
-    // the diagonals up: lane m ends with the sums of diagonals m and m - 32; then one shared-memory
-    // add per lane and chunk, the m - 32 part carried into the next chunk.
-    const int q = warp & 3, half = (warp - 4) >> 2;        // this warp's chunks: half*3 .. half*3 + 2
-    float* my = S.corr[warp - 4];
-    uint32_t tileit = 0, rz = 0;      // rz: rendezvous count of the 8 epilogue warps (bounded mbarrier, never bar.sync)
-    for (int p = cta; p < n_pairs; p += n_cta) {
-      for (int k = lane; k < WF; k += 32) my[k] = 0.f;
-      __syncwarp();
-      for (int t = 0; t < 3; ++t, ++tileit) {
-        const uint32_t buf = tileit & 1;
-        TC_WAIT(&S.d_full[buf], (tileit >> 1) & 1, 607);
-        fence_after_sync();
-        float carry = 0.f;
-        int b0 = 0;
+  } else {
+    // ===================== consumers ==========================================================
+    const int wg = warp >> 2, wi = warp & 3, g = lane >> 2, t = lane & 3;
+    int rows[2][2];                         // [tile][a / b]: this thread's fragment rows
+#pragma unroll
+    for (int tt = 0; tt < 2; ++tt) {
+      const int r = (wg + 3 * tt) * 64 + wi * 16 + g;
+      rows[tt][0] = r;
+      rows[tt][1] = r + 8;
+    }
+    float mu0[8], mu1[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      mu0[j] = __half2float(__float2half_rn(-mu_o1[j * 8 + 2 * t]));
+      mu1[j] = __half2float(__float2half_rn(-mu_o1[j * 8 + 2 * t + 1]));
+    }
+    const uint32_t b_base = smem_u32(S.B[0]);
+    uint32_t pi = 0, gi = 0, ui = 0;
+    for (int u = u_begin; u < u_end; ++u, ++ui) {
+      const int p = u / NB, jb = u - p * NB;
+      if (u == u_begin || jb == 0) { K4_WAIT(&S.l_full, pi & 1, 402); ++pi; }
+      const uint32_t wb = ui & 1;
+      K4_WAIT(&S.rw_full[wb], (ui >> 1) & 1, 404);
+      float acc[2][32];
+#pragma unroll
+      for (int tt = 0; tt < 2; ++tt)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          acc[tt][4 * j + 0] = mu0[j]; acc[tt][4 * j + 1] = mu1[j];
+          acc[tt][4 * j + 2] = mu0[j]; acc[tt][4 * j + 3] = mu1[j];
+        }
+      int st = 0;
 #pragma unroll 1
-        for (int c3 = 0; c3 < 3; ++c3) {
-          const int ch = half * 3 + c3;
-          uint32_t v[32];
-          tmem_ld_x32(tmem + ((uint32_t)(q * 32) << 16) + buf * 192 + ch * 32, v);
-          tmem_ld_wait();
-          if (c3 == 2) {                     // this warp's part of the tile is in registers: release the buffer
-            fence_before_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&S.d_empty[buf]);
-          }
-          // (1) split every column by the sign of its diagonal: register t holds column t, which lies
-          //     on diagonal lane - t (class m = (lane - t) mod 32): x if t <= lane, y (diagonal m - 32) else
-          float x[32], y[32];
+      for (int cc = 0; cc < 4; ++cc) {
+        // this thread's LEFT values of the 32-channel chunk: [tile][row a / b][kk][lo / hi 8]
+        uint32_t Lr[2][2][2][2];
 #pragma unroll
-          for (int t2 = 0; t2 < 32; ++t2) {
-            const bool ge = lane >= t2;
-            const float f = __uint_as_float(v[t2]);
-            x[t2] = ge ? f : 0.f;
-            y[t2] = ge ? 0.f : f;
-          }
-          // (2) reduce-scatter over the lanes, low bit first.  Before stage b a lane holds the classes
-          //     with (lane - m) % 2^b == 0 in registers t = (lane - m) mod 32; it keeps those with bit b
-          //     of t clear and hands the others to lane ^ 2^b, in whose frame they sit at t +- 2^b: the
-          //     lane-dependent rotation is absorbed into which static register each lane sends.
+        for (int tt = 0; tt < 2; ++tt)
 #pragma unroll
-          for (int b = 0; b < 5; ++b) {
-            const int o = 1 << b;
-            const bool up = (lane & o) != 0;
+          for (int h = 0; h < 2; ++h) {
+            const int r = rows[tt][h] < WF ? rows[tt][h] : WF - 1;
+            const __half* lp = S.L + r * K4_PITCH + cc * 32 + 2 * t;
 #pragma unroll
-            for (int tp = 0; tp < 32; tp += 2 * o) {
-              const float sx = up ? x[(tp + o) & 31] : x[(tp - o) & 31];
-              const float sy = up ? y[(tp + o) & 31] : y[(tp - o) & 31];
-              x[tp] += __shfl_xor_sync(0xffffffffu, sx, o);
-              y[tp] += __shfl_xor_sync(0xffffffffu, sy, o);
+            for (int kk = 0; kk < 2; ++kk) {
+              Lr[tt][h][kk][0] = *reinterpret_cast<const uint32_t*>(lp + kk * 16);
+              Lr[tt][h][kk][1] = *reinterpret_cast<const uint32_t*>(lp + kk * 16 + 8);
             }
           }
-          // (3) bin of (lane 0, column 0 of the chunk), before wrap
-          b0 = t * 128 + q * 32 - h * 192 - ch * 32 - 180;
-          my[wrap360(b0 + lane)] += x[0] + carry;
-          carry = y[0];
+#pragma unroll 1
+        for (int dj = 0; dj < S15; ++dj, ++st) {
+          const int sl = st % K4_GROUP;
+          const uint32_t s = gi % K4_RING;
+          if (sl == 0) K4_WAIT(&S.full[s], (gi / K4_RING) & 1, 202);
+          const __half* rp = S.Rw[wb] + dj * K4_PITCH + cc * 32 + 2 * t;
+          uint32_t A[2][2][4];                // [tile][kk]
+#pragma unroll
+          for (int kk = 0; kk < 2; ++kk) {
+            const uint32_t r0 = *reinterpret_cast<const uint32_t*>(rp + kk * 16);
+            const uint32_t r1 = *reinterpret_cast<const uint32_t*>(rp + kk * 16 + 8);
+#pragma unroll
+            for (int tt = 0; tt < 2; ++tt) {
+              A[tt][kk][0] = absdiff_h2(Lr[tt][0][kk][0], r0);
+              A[tt][kk][1] = absdiff_h2(Lr[tt][1][kk][0], r0);
+              A[tt][kk][2] = absdiff_h2(Lr[tt][0][kk][1], r1);
+              A[tt][kk][3] = absdiff_h2(Lr[tt][1][kk][1], r1);
+            }
+          }
+          const uint32_t slice = b_base + s * (K4_GROUP * K4_BSLICE) + sl * K4_BSLICE;
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < 2; ++kk) {
+            // the K16 step covers W1 chunks k8 = 2 kk, 2 kk + 1: LBO = 1024 B between them, SBO = 128 B per 8 outputs
+            const uint64_t bd = desc_kmajor_noswizzle(slice + kk * 2048, 1024, 128);
+#pragma unroll
+            for (int tt = 0; tt < 2; ++tt) wgmma_m64n64k16_rs(acc[tt], A[tt][kk], bd);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();                    // A registers and the W1 slot are free again
+          if (sl == K4_GROUP - 1) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&S.empty[s]);
+            ++gi;
+          }
         }
-        my[wrap360(b0 - 32 + lane)] += carry;
-        __syncwarp();                        // the next tile's bins belong to other lanes
       }
-      // combine the eight warps' private arrays in a fixed order (bit-reproducible)
       __syncwarp();
-      if (lane == 0) mbar_arrive(&S.epi);
-      TC_WAIT(&S.epi, rz & 1, 608);
-      ++rz;
-      for (int k = tid - 128; k < WF; k += 256)
-        corr_part[((size_t)p * 2 + h) * WF + k] =
-            (((S.corr[0][k] + S.corr[1][k]) + (S.corr[2][k] + S.corr[3][k])) +
-             ((S.corr[4][k] + S.corr[5][k]) + (S.corr[6][k] + S.corr[7][k])));
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&S.epi);
-      TC_WAIT(&S.epi, rz & 1, 609);
-      ++rz;
+      if (lane == 0) mbar_arrive(&S.rw_empty[wb]);
+      if (jb == NB - 1 || u == u_end - 1) { if (lane == 0) mbar_arrive(&S.l_empty); }
+      const int64_t mrow = (int64_t)p * PAIR_ROWS + jb * NB;
+#pragma unroll
+      for (int tt = 0; tt < 2; ++tt)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int i = rows[tt][h];
+          if (i >= WF) continue;
+          const int ibk = i / S15, di = i - ibk * S15;
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<uint32_t*>(o1 + o1_chunk_offset(mrow + ibk, di, j) + 2 * t) =
+                pack_h2(acc[tt][4 * j + 2 * h], acc[tt][4 * j + 2 * h + 1]);
+        }
     }
   }
 done:
-  fence_before_sync();
+  return;
+}
+
+// ------------------------------------------------------------------------------------------------
+// k_conv2_mma -- c_conv2 (15x1 stride 15, 64 -> 128, ReLU) as a GEMM [M x 960] x [960 x 128], W2 applied as
+// hi + lo (two MMAs per K16 step: the fp16 rounding of W2 was the largest term of the logit error budget
+// after the feature volumes).  A = the o1 tiles k_delta_conv1_wgmma wrote; output = the centred fp16 x3 planes.
+// `fault` != 0 is the test hook of ovn_debug_inject_fault: the kernel computes nothing and raises the
+// pipeline-failure flag, so that the finalize kernels poison the outputs of the call.
+// grid = (ceil(M / 64), 2 halves of 64 output channels)
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(MMA_THREADS)
+k_conv2_mma(const __half* __restrict__ o1, const __half* __restrict__ W2s, const float* __restrict__ bias2,
+            const float* __restrict__ mu_x3, __half* __restrict__ x3, int64_t out_pitch, int64_t M, int fault,
+            int* __restrict__ err) {
+  if (fault) {
+    if (threadIdx.x == 0 && blockIdx.x == 0 && blockIdx.y == 0) atomicExch(err, 501);
+    return;
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int64_t m0 = (int64_t)blockIdx.x * MMA_ROWS + warp * 16;
+  if (m0 >= M) return;
+  const int64_t ma = m0 + g, mb = m0 + g + 8;
+  const int nb0 = blockIdx.y * 64;
+  float acc[8][4] = {};
+#pragma unroll 1
+  for (int di = 0; di < S15; ++di) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const int c8 = kk * 2;
+      const uint32_t a0 = ld_h2(o1 + o1_chunk_offset(ma, di, c8) + 2 * t), a1 = ld_h2(o1 + o1_chunk_offset(mb, di, c8) + 2 * t);
+      const uint32_t a2 = ld_h2(o1 + o1_chunk_offset(ma, di, c8 + 1) + 2 * t), a3 = ld_h2(o1 + o1_chunk_offset(mb, di, c8 + 1) + 2 * t);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int n = nb0 + j * 8 + g;
+        const __half* Bh = W2s + ((size_t)(di * 2) * 128 + n) * 64 + 2 * t;     // [di][hi, lo][n][chunk ^ (n & 7)][8]
+        const int s0 = (c8 ^ (n & 7)) << 3, s1 = ((c8 + 1) ^ (n & 7)) << 3;
+        mma16816(acc[j], a0, a1, a2, a3, ld_h2(Bh + s0), ld_h2(Bh + s1));
+        mma16816(acc[j], a0, a1, a2, a3, ld_h2(Bh + 128 * 64 + s0), ld_h2(Bh + 128 * 64 + s1));
+      }
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t m = h ? mb : ma;
+    if (m >= M) continue;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int n = nb0 + j * 8 + 2 * t;
+      const float a = fmaxf(acc[j][2 * h] + __ldg(bias2 + n), 0.f) - __ldg(mu_x3 + n);
+      const float b = fmaxf(acc[j][2 * h + 1] + __ldg(bias2 + n + 1), 0.f) - __ldg(mu_x3 + n + 1);
+      *reinterpret_cast<uint32_t*>(x3 + ((size_t)(n >> 3) * out_pitch + m) * 8 + (n & 7)) = pack_h2(a, b);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// k_conv3_mma -- c_conv3 (3x3, 128 -> 256, ReLU) + Flatten + the Dense(1) partial sum of each row.
+// Rows are (pair, jb, ib) in the x3 planes; the 3x3 tap (dy, dx) reads row r + dy * 24 + dx.
+// partial[r][nh] = sum over the 128 channels of half nh of relu(conv + b3eff) * w_dense (0 for the
+// rows a valid convolution does not produce).
+// grid = (ceil(M / 64), 2 halves of 128 output channels)
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(MMA_THREADS)
+k_conv3_mma(const __half* __restrict__ X3, int64_t a_pitch, const __half* __restrict__ Bp, const float* __restrict__ bias,
+            int64_t M, const float* __restrict__ wd, float* __restrict__ partial) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int64_t r0 = (int64_t)blockIdx.x * MMA_ROWS + warp * 16;
+  if (r0 >= M) return;
+  const int nh = blockIdx.y;
+  float acc[16][4] = {};
+#pragma unroll 1
+  for (int tap = 0; tap < 9; ++tap) {
+    const int64_t shift = (tap / 3) * NB + (tap % 3);
+    const __half* Aa = X3 + (r0 + g + shift) * 8 + 2 * t;
+    const __half* Ab = Aa + 8 * 8;
+#pragma unroll 1
+    for (int c16 = 0; c16 < 8; ++c16) {
+      const size_t p0 = (size_t)(2 * c16) * a_pitch * 8, p1 = p0 + (size_t)a_pitch * 8;
+      const uint32_t a0 = ld_h2(Aa + p0), a1 = ld_h2(Ab + p0), a2 = ld_h2(Aa + p1), a3 = ld_h2(Ab + p1);
+      // [nh][slab = tap * 4 + c / 32][(c / 8) % 4][n][8]
+      const __half* B = Bp + (((size_t)(nh * 36 + tap * 4 + (c16 >> 1)) * 4 + (c16 & 1) * 2) * 128 + g) * 8 + 2 * t;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) mma16816(acc[j], a0, a1, a2, a3, ld_h2(B + j * 64), ld_h2(B + 128 * 8 + j * 64));
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t r = r0 + g + 8 * h;
+    const int rem = (int)(r % PAIR_ROWS);
+    const int yy = rem / NB, xx = rem - yy * NB;
+    const bool valid = (r < M) && (yy < NB - 2) && (xx < NB - 2);
+    // rows are (pair, jb, ib): yy = jb, xx = ib; Flatten order of the reference is (ib, jb, channel)
+    const float* wrow = wd + (size_t)(valid ? (xx * (NB - 2) + yy) : 0) * 256 + nh * 128;
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int n = j * 8 + 2 * t;
+      s = fmaf(fmaxf(acc[j][2 * h] + __ldg(bias + nh * 128 + n), 0.f), __ldg(wrow + n), s);
+      s = fmaf(fmaxf(acc[j][2 * h + 1] + __ldg(bias + nh * 128 + n + 1), 0.f), __ldg(wrow + n + 1), s);
+    }
+    s += __shfl_xor_sync(0xffffffffu, s, 1);
+    s += __shfl_xor_sync(0xffffffffu, s, 2);
+    if (t == 0 && r < M) partial[r * 2 + nh] = valid ? s : 0.f;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// k_corr_mma -- correlation (yaw) head.  G = L R^T (360 x 360, K = 128) from hi / lo fp16 operands
+// (G = Lhi Rhi + Llo Rhi + Lhi Rlo: fp32-grade, fp16 alone does not keep the argmax of a flat curve),
+// corr[k] = sum_j G[(k + j + 180) mod 360, j].  A block owns 64 rows of G of one pair: the warps write
+// their 16 x 360 strips to shared memory, then every bin sums the block's 64 diagonal terms in a fixed
+// order into corr_part[pair][row block][k] (no atomics: results are bit-reproducible).
+// grid = (n_pairs, C6_IBLK)
+// ------------------------------------------------------------------------------------------------
+constexpr int C6_IBLK = 6;                          // 6 x 64 = 384 >= 360 rows (the packed L is zero past 360)
+constexpr int C6_GPITCH = WF + 1;
+constexpr size_t C6_SMEM = (size_t)MMA_ROWS * C6_GPITCH * sizeof(float);
+
+__global__ void __launch_bounds__(MMA_THREADS)
+k_corr_mma(const __half* __restrict__ Lc, const int32_t* __restrict__ l_idx, const __half* __restrict__ Rc, int r_per_pair,
+           float* __restrict__ corr_part) {
+  extern __shared__ float Gs[];                      // [64][C6_GPITCH]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int p = blockIdx.x, i0 = blockIdx.y * MMA_ROWS;
+  const __half* lp = Lc + (size_t)(l_idx ? l_idx[p] : p) * (C6_VOL_L_BYTES / 2);
+  const __half* rp = Rc + (r_per_pair ? (size_t)p * (C6_VOL_R_BYTES / 2) : 0);
+  // L: [row / 128][c / 64][hi, lo][(c / 8) % 8][row % 128][8];  R: [row / 192][hi, lo][c / 8][row % 192][8]
+  const int ia = i0 + warp * 16 + g, ib = ia + 8;
+  const __half* La = lp + (size_t)((ia >> 7) * 2) * (C6_STAGE_BYTES / 2) + (ia & 127) * 8 + 2 * t;
+  const __half* Lb = lp + (size_t)((ib >> 7) * 2) * (C6_STAGE_BYTES / 2) + (ib & 127) * 8 + 2 * t;
+  for (int j0 = 0; j0 < 2 * 192; j0 += 64) {
+    float acc[8][4] = {};
+#pragma unroll 1
+    for (int c16 = 0; c16 < 8; ++c16) {
+      const size_t lo_k = (size_t)(c16 >> 2) * (C6_STAGE_BYTES / 2) + (size_t)((c16 & 3) * 2) * 128 * 8;
+      uint32_t ah[4], al[4];
+      ah[0] = ld_h2(La + lo_k); ah[1] = ld_h2(Lb + lo_k);
+      ah[2] = ld_h2(La + lo_k + 128 * 8); ah[3] = ld_h2(Lb + lo_k + 128 * 8);
+      al[0] = ld_h2(La + lo_k + C6_STAGE_BYTES / 4); al[1] = ld_h2(Lb + lo_k + C6_STAGE_BYTES / 4);
+      al[2] = ld_h2(La + lo_k + C6_STAGE_BYTES / 4 + 128 * 8); al[3] = ld_h2(Lb + lo_k + C6_STAGE_BYTES / 4 + 128 * 8);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int n = j0 + j * 8 + g;
+        const __half* B = rp + (size_t)(n / 192) * (C6_R_BYTES / 2) + ((size_t)(2 * c16) * 192 + n % 192) * 8 + 2 * t;
+        const uint32_t bh0 = ld_h2(B), bh1 = ld_h2(B + 192 * 8);
+        const uint32_t bl0 = ld_h2(B + C6_R_BYTES / 4), bl1 = ld_h2(B + C6_R_BYTES / 4 + 192 * 8);
+        mma16816(acc[j], ah[0], ah[1], ah[2], ah[3], bh0, bh1);
+        mma16816(acc[j], al[0], al[1], al[2], al[3], bh0, bh1);
+        mma16816(acc[j], ah[0], ah[1], ah[2], ah[3], bl0, bl1);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int n = j0 + j * 8 + 2 * t;
+      float* ra = Gs + (warp * 16 + g) * C6_GPITCH;
+      float* rb = ra + 8 * C6_GPITCH;
+      if (n < WF) { ra[n] = acc[j][0]; rb[n] = acc[j][2]; }
+      if (n + 1 < WF) { ra[n + 1] = acc[j][1]; rb[n + 1] = acc[j][3]; }
+    }
+  }
   __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem, 512);
+  for (int k = threadIdx.x; k < WF; k += MMA_THREADS) {
+    float s = 0.f;
+    // row i pairs with column j = (i - k - 180) mod 360
+    int jj = (i0 - k - WF / 2) % WF;
+    if (jj < 0) jj += WF;
+    for (int ii = 0; ii < MMA_ROWS && i0 + ii < WF; ++ii) {
+      s += Gs[ii * C6_GPITCH + jj];
+      if (++jj == WF) jj = 0;
+    }
+    corr_part[((size_t)p * C6_IBLK + blockIdx.y) * WF + k] = s;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// k_leg_mma -- one leg layer (2..) on the hi / lo fp16 C8-interleaved activation planes:
+//   out[y, px, n] = relu(bias[n] + sum_{dh, dw, c} x[y * sh + dh, px + dw, c] W[dh, dw, c, n]),
+//   x * w ~= xh wh + xl wh + xh wl  (three MMAs per K16 step, fp32-grade).
+// EPI 4: output as the next layer's hi / lo planes; EPI 3 (last layer): fp32 feature volume.
+// grid = (n_img * h_out, ceil(M / 64), cout / 64)
+// ------------------------------------------------------------------------------------------------
+template <int EPI>
+__global__ void __launch_bounds__(MMA_THREADS)
+k_leg_mma(LegArgs g) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, gq = lane >> 2, t = lane & 3;
+  const int64_t px0 = (int64_t)blockIdx.y * MMA_ROWS + warp * 16;
+  if (px0 >= g.M) return;
+  const int y = blockIdx.x, z = blockIdx.z;
+  const int64_t in_base = (int64_t)(y / g.runs_per_img) * g.in_img_planes + (int64_t)(y % g.runs_per_img) * g.in_run_planes;
+  const int64_t pa = px0 + gq < g.M ? px0 + gq : g.M - 1, pb = px0 + gq + 8 < g.M ? px0 + gq + 8 : g.M - 1;
+  const int n_slabs = g.kh * g.kw * 3;
+  const size_t plane = (size_t)g.a_pitch * 8;
+  float acc[8][4] = {};
+#pragma unroll 1
+  for (int dh = 0; dh < g.kh; ++dh) {
+#pragma unroll 1
+    for (int dw = 0; dw < g.kw; ++dw) {
+      const __half* Ah = g.A + (size_t)(in_base + (int64_t)dh * 2 * g.c8in) * plane + (size_t)dw * 8 + 2 * t;
+      const __half* Al = Ah + (size_t)g.c8in * plane;
+      // [z][slab = (dh * kw + dw) * 3 + term][c8][64][8]; term 0 = hi, term 2 = lo
+      const __half* Bh = g.Bp + ((size_t)(z * n_slabs + (dh * g.kw + dw) * 3) * g.c8in * 64 + gq) * 8 + 2 * t;
+      const __half* Bl = Bh + (size_t)2 * g.c8in * 64 * 8;
+#pragma unroll 1
+      for (int c8 = 0; c8 < g.c8in; c8 += 2) {
+        const size_t o0 = (size_t)c8 * plane, o1 = o0 + plane;
+        const uint32_t h0 = ld_h2(Ah + o0 + pa * 8), h1 = ld_h2(Ah + o0 + pb * 8), h2 = ld_h2(Ah + o1 + pa * 8), h3 = ld_h2(Ah + o1 + pb * 8);
+        const uint32_t l0 = ld_h2(Al + o0 + pa * 8), l1 = ld_h2(Al + o0 + pb * 8), l2 = ld_h2(Al + o1 + pa * 8), l3 = ld_h2(Al + o1 + pb * 8);
+        const size_t bo = (size_t)c8 * 64 * 8;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const uint32_t wh0 = ld_h2(Bh + bo + j * 64), wh1 = ld_h2(Bh + bo + 64 * 8 + j * 64);
+          const uint32_t wl0 = ld_h2(Bl + bo + j * 64), wl1 = ld_h2(Bl + bo + 64 * 8 + j * 64);
+          mma16816(acc[j], h0, h1, h2, h3, wh0, wh1);
+          mma16816(acc[j], l0, l1, l2, l3, wh0, wh1);
+          mma16816(acc[j], h0, h1, h2, h3, wl0, wl1);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t px = px0 + gq + 8 * h;
+    if (px >= g.M) continue;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int n = z * 64 + j * 8 + 2 * t;
+      if (n >= g.n_valid) continue;
+      const float a = fmaxf(acc[j][2 * h] + __ldg(g.bias + n), 0.f);
+      const float b = fmaxf(acc[j][2 * h + 1] + __ldg(g.bias + n + 1), 0.f);
+      if (EPI == 4) {
+        const __half2 hi = __floats2half2_rn(a, b);
+        const float2 hf = __half22float2(hi);
+        const int64_t pl = (int64_t)y * g.out_run_planes + (n >> 3);
+        *reinterpret_cast<__half2*>(g.out_planes + ((size_t)pl * g.out_pitch + px) * 8 + (n & 7)) = hi;
+        *reinterpret_cast<uint32_t*>(g.out_planes + ((size_t)(pl + g.out_run_planes / 2) * g.out_pitch + px) * 8 + (n & 7)) =
+            pack_h2(a - hf.x, b - hf.y);
+      } else {
+        *reinterpret_cast<float2*>(g.out_f32 + ((size_t)y * g.M + px) * g.n_valid + n) = make_float2(a, b);
+      }
+    }
+  }
 }
 
 __global__ void __launch_bounds__(384)
@@ -1781,7 +678,8 @@ k_corr_finalize(const float* __restrict__ part, float* __restrict__ corr_out, in
   __shared__ float s_corr[WF];
   const int p = blockIdx.x;
   for (int k = threadIdx.x; k < WF; k += blockDim.x) {
-    const float c = part[((size_t)p * 2) * WF + k] + part[((size_t)p * 2 + 1) * WF + k];
+    float c = 0.f;
+    for (int b = 0; b < C6_IBLK; ++b) c += part[((size_t)p * C6_IBLK + b) * WF + k];
     s_corr[k] = c;
     if (corr_out) corr_out[(size_t)p * WF + k] = c;
   }
@@ -1791,7 +689,7 @@ k_corr_finalize(const float* __restrict__ part, float* __restrict__ corr_out, in
     float bv = s_corr[0];
     for (int k = 1; k < WF; ++k)
       if (s_corr[k] > bv) { bv = s_corr[k]; best = k; }
-    // a raised error flag (barrier time-out, bad index) poisons the result: garbage never looks valid
+    // a raised error flag (pipeline failure, bad index) poisons the result: garbage never looks valid
     yaw[p] = (*err != 0) ? INT32_MIN : WF / 2 - best;
   }
 }
@@ -1810,7 +708,7 @@ k_o1_channel_mean(const __half* __restrict__ o1, int64_t M, float* __restrict__ 
   if (g == 0) {
     float t = 0.f;
     for (int k = 0; k < 16; ++k) t += part[k][o];
-    mu[o] = __half2float(__float2half_rn(t / (float)(M * S15)));   // fp16: k_delta_conv1_tc subtracts it as an MMA operand
+    mu[o] = __half2float(__float2half_rn(t / (float)(M * S15)));   // fp16: k_delta_conv1_wgmma starts its accumulators at -mu_o1
   }
 }
 
@@ -1845,7 +743,7 @@ k_fold_bias2(const float* __restrict__ b2base, const float* __restrict__ mu_o1, 
 // computes  sum (x3 - mu) W3_f16 + sum mu W3_f32 = sum x3 W3_f32 - sum (x3 - mu) dW3,  i.e. the fp16
 // rounding of W3 only acts on the centred fluctuation of x3.  Without this its effect was a nearly
 // pair-independent logit offset (a static perturbation times a non-negative input of stable mean):
-// the largest single term of the error budget on the Infer parity test (profiles/r2_precision_budget.txt).
+// the largest single term of the error budget on the Infer parity test (float64 emulation, tools/precision_study.py).
 __global__ void __launch_bounds__(256)
 k_fold_bias3(const float* __restrict__ b3, const float* __restrict__ mu_x3, const float* __restrict__ W3,
              float* __restrict__ b3eff) {
@@ -1880,7 +778,7 @@ k_dense_finalize(const float* __restrict__ partial, const float* __restrict__ bd
 // and N = 16: as a 64x64-tiled SIMT GEMM this took 61 us of a 245 us single-scan leg.  One thread
 // per TWO adjacent output pixels x all 16 output channels: the 16 weights of a (tap, channel) are read
 // once from shared memory (4 broadcast LDS.128) and feed 32 FFMAs -- the first version (one pixel x 8
-// channels per thread: 8 LDS per 32 FFMA) was bound by the load/store unit (profiles/r2_leg_batched.txt).
+// channels per thread: 8 LDS per 32 FFMA) was bound by the load/store unit.
 template <bool CIN4>
 __global__ void __launch_bounds__(512)
 k_leg_layer1_direct(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
@@ -1967,7 +865,7 @@ k_leg_layer1_small(const float* __restrict__ x, const float* __restrict__ w, con
                     int n, int H_in, int W_in, int cin, int kh, int kw, int sh, int sw, int H_out, int W_out, int cout,
                     int relu, __half* __restrict__ out) {
   // latency-mode variant (1-2 scans): one thread per (pixel, 8 output channels) -- four times the threads of
-  // k_leg_layer1_direct, which matters when a single scan has to fill 148 SMs
+  // k_leg_layer1_direct, which matters when a single scan has to fill every SM
   extern __shared__ __align__(16) float w_s[];              // [kh*kw*cin][cout]
   for (int i = threadIdx.x; i < kh * kw * cin * cout; i += blockDim.x) w_s[i] = w[i];
   __syncthreads();
@@ -2024,44 +922,6 @@ k_leg_layer1_small(const float* __restrict__ x, const float* __restrict__ w, con
   *reinterpret_cast<uint4*>(out + ((size_t)(plane_hi + C8) * W_out + xo) * 8) = *reinterpret_cast<const uint4*>(lo);
 }
 
-// fp32 NHWC [n][H][W][C] -> hi/lo fp16 planes [n][rows][hi,lo][c8in][ceil(W/2)][8], the input of the tensor-core
-// layer 1 (see TcState::in_planes).  channel' = (f * 2 + parity) * C + c with parity = column & 1 and f the folded
-// kernel row: fold = 1: rows = H, plane row r is input row r; fold = kh: rows = H_out, plane row r holds input
-// rows r * sh + f.
-__global__ void __launch_bounds__(256)
-k_input_to_parity_planes(const float* __restrict__ x, int64_t total, int H, int W, int C, int c8in, int Wh, int rows,
-                         int fold, int sh, __half* __restrict__ out) {
-  // thread = (img * rows + row, w', c8) with c8 fastest: the threads of one pixel pair read its 2C contiguous floats,
-  // a warp writes whole 32 B sectors of each plane
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int c8 = (int)(i % c8in);
-  const int64_t pw = i / c8in;
-  const int wp = (int)(pw % Wh);
-  const int r = (int)(pw / Wh);                                            // img * rows + row fits 32 bits
-  const int img = r / rows, row = r - img * rows;
-  const int n_ch = fold * 2 * C;
-  int ch = c8 * 8;
-  int f = ch / (2 * C), rem = ch - f * 2 * C;
-  int parity = rem / C, c = rem - parity * C;
-  __half hi[8], lo[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e, ++ch) {
-    float v = 0.f;
-    if (ch < n_ch) {
-      const int w = 2 * wp + parity;
-      const int in_row = (fold == 1) ? row : row * sh + f;
-      if (w < W && in_row < H) v = __ldg(x + (((int64_t)img * H + in_row) * W + w) * C + c);
-    }
-    hi[e] = __float2half_rn(v);
-    lo[e] = __float2half_rn(v - __half2float(hi[e]));
-    if (++c == C) { c = 0; if (++parity == 2) { parity = 0; ++f; } }
-  }
-  const int64_t plane_hi = (int64_t)r * (2 * c8in) + c8;
-  *reinterpret_cast<uint4*>(out + ((size_t)plane_hi * Wh + wp) * 8) = *reinterpret_cast<const uint4*>(hi);
-  *reinterpret_cast<uint4*>(out + ((size_t)(plane_hi + c8in) * Wh + wp) * 8) = *reinterpret_cast<const uint4*>(lo);
-}
-
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
@@ -2078,14 +938,9 @@ void tc_free(ovn_handle* h) {
   for (void* b : bufs) if (b) cudaFree(b);
   for (int l = 0; l < kMaxLegLayers; ++l) {
     if (t->wres[l]) cudaFree(t->wres[l]);
-    if (t->wstk[l]) cudaFree(t->wstk[l]);
-    if (t->wstkw[l]) cudaFree(t->wstkw[l]);
   }
   if (t->pb_l16) cudaFree(t->pb_l16);
   if (t->pb_lc) cudaFree(t->pb_lc);
-  if (t->leg_part) cudaFree(t->leg_part);
-  if (t->leg_counters) cudaFree(t->leg_counters);
-  if (t->in_planes) cudaFree(t->in_planes);
   if (t->actp[0]) cudaFree(t->actp[0]);
   if (t->actp[1]) cudaFree(t->actp[1]);
   delete t;
@@ -2148,7 +1003,7 @@ int tc_pack_weights(ovn_handle* h) {
                     __float2half(w3.kernel[(((size_t)dx * 3 + dy) * 128 + c) * 256 + nh * 128 + n]);
               }
       }
-  // k_delta_conv1_tc stores o1 without the c_conv1 bias; its image under c_conv2 is a constant per channel
+  // k_delta_conv1_wgmma stores o1 without the c_conv1 bias; its image under c_conv2 is a constant per channel
   std::vector<float> b2e(128);
   {
     const LayerWeights& wb1 = h->host_w["c_conv1"];
@@ -2170,7 +1025,7 @@ int tc_pack_weights(ovn_handle* h) {
   if ((rc = upload_vec(h, &t->w1p, p1)) != OVN_OK) return rc;
   if ((rc = upload_vec(h, &t->w2p, p2)) != OVN_OK) return rc;
   if ((rc = upload_vec(h, &t->w3p, p3)) != OVN_OK) return rc;
-  // ---- leg layers 2.. : resident-activation layout of the weights.  Three-term split product
+  // ---- leg layers 2.. : weights as (tap, term) slabs.  Three-term split product
   // x*w ~= xh*wh + xl*wh + xh*wl  (x = xh + xl, w = wh + wl in fp16): slab = (dh, dw, term)
   size_t max_planes_bytes = 0;
   for (int l = 0; l < h->n_leg; ++l) {
@@ -2178,14 +1033,14 @@ int tc_pack_weights(ovn_handle* h) {
     const size_t out_bytes = (size_t)L.h_out * 2 * (L.cout / 8) * L.w_out * 16;   // hi + lo planes
     if (out_bytes > max_planes_bytes) max_planes_bytes = out_bytes;
     if (l == 0) continue;
-    if (L.cin % 16 != 0 || L.cout % 8 != 0 || L.sw != 1 || L.kw > 16)
+    if (L.cin % 16 != 0 || L.cout % 8 != 0 || L.sw != 1)
       OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "tensor-core leg: layer %s shape not supported", L.name);
     const LayerWeights& w = h->host_w[L.name];
     const int c8in = L.cin / 8;
     const int nz = (L.cout + 63) / 64;
     int rc2;
     {
-      // resident-activation layout: slab = (dh, dw, term), rows = all C_in/8 chunks, 64 output channels
+      // slab = (dh, dw, term), rows = all C_in/8 chunks, 64 output channels
       const int nsl = L.kh * L.kw * 3;
       std::vector<__half> br((size_t)nz * nsl * c8in * 64 * 8, __float2half(0.f));
       for (int z = 0; z < nz; ++z)
@@ -2204,120 +1059,12 @@ int tc_pack_weights(ovn_handle* h) {
             }
       if ((rc2 = upload_vec(h, &t->wres[l], br)) != OVN_OK) return rc2;
     }
-    {
-      // batched kernel: hi | lo stacked along N (TcState::wstk)
-      const int n_mma = L.cout >= 64 ? 64 : ((L.cout + 15) / 16) * 16, R = 2 * n_mma;
-      int c8u = c8in;
-      while (c8u > 2 && (size_t)c8u * R * 16 > (size_t)LR_B_MAX) c8u /= 2;
-      if (c8in % c8u != 0 || c8u % 2 != 0 || (size_t)c8u * R * 16 > (size_t)LR_B_MAX)
-        OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "tensor-core leg: layer %s weight unit does not fit the ring", L.name);
-      const int kc_n = c8in / c8u, taps = L.kh * L.kw;
-      std::vector<__half> bs((size_t)nz * taps * c8in * R * 8, __float2half(0.f));
-      for (int z = 0; z < nz; ++z)
-        for (int tap = 0; tap < taps; ++tap)
-          for (int c8 = 0; c8 < c8in; ++c8)
-            for (int n = 0; n < n_mma && z * 64 + n < L.cout; ++n)
-              for (int k = 0; k < 8; ++k) {
-                const float wf = w.kernel[((size_t)tap * L.cin + c8 * 8 + k) * L.cout + z * 64 + n];
-                const __half wh = __float2half(wf);
-                const __half wl = __float2half(wf - __half2float(wh));
-                const size_t unit = ((size_t)z * taps + tap) * kc_n + c8 / c8u;
-                const size_t base = (unit * c8u + c8 % c8u) * R;
-                bs[(base + n) * 8 + k] = wh;
-                bs[(base + n_mma + n) * 8 + k] = wl;
-              }
-      if ((rc2 = upload_vec(h, &t->wstk[l], bs)) != OVN_OK) return rc2;
-      t->stk_c8u[l] = c8u;
-    }
-    if (L.cout == 128) {
-      const int n_mma = 128, R = 256, taps = L.kh * L.kw;
-      int c8u = c8in;
-      while (c8u > 2 && (size_t)c8u * R * 16 > (size_t)LR_B_MAX) c8u /= 2;
-      if (c8in % c8u == 0 && c8u % 2 == 0 && (size_t)c8u * R * 16 <= (size_t)LR_B_MAX) {
-        const int kc_n = c8in / c8u;
-        std::vector<__half> bs((size_t)taps * c8in * R * 8, __float2half(0.f));
-        for (int tap = 0; tap < taps; ++tap)
-          for (int c8 = 0; c8 < c8in; ++c8)
-            for (int n = 0; n < n_mma; ++n)
-              for (int k = 0; k < 8; ++k) {
-                const float wf = w.kernel[((size_t)tap * L.cin + c8 * 8 + k) * L.cout + n];
-                const __half wh = __float2half(wf);
-                const __half wl = __float2half(wf - __half2float(wh));
-                const size_t unit = (size_t)tap * kc_n + c8 / c8u;
-                const size_t base = (unit * c8u + c8 % c8u) * R;
-                bs[(base + n) * 8 + k] = wh;
-                bs[(base + n_mma + n) * 8 + k] = wl;
-              }
-        if ((rc2 = upload_vec(h, &t->wstkw[l], bs)) != OVN_OK) return rc2;
-        t->stkw_c8u[l] = c8u;
-      }
-    }
-  }
-  {
-    const char* e = getenv("OVN_LEG_WIDE");                      // measurement switch: 0 = 64-channel halves in two CTAs
-    t->leg_wide = !(e && e[0] == '0');
-  }
-  {
-    // ---- layer 1 on tensor cores: W'[dh'][j][(f * 2 + parity) * C + c][n] = W[dh][2j + parity][c][n]  (kw' = ceil(kw / 2);
-    // fold = 1: dh = dh', f = 0;  fold = kh: dh = f, dh' = 0)
-    const ConvSpec& L = h->leg[0];
-    // measured (batch 64, us/scan, whole leg), OVN_L1_TC = 0 (SIMT) / 1 (column planes) / 2 (column planes + folded rows):
-    // C = 25: 49.1 / 24.4 / -;  C = 4: 12.2 / 13.2 / 11.7;  C = 5: 14.2 / - / 12.6   (profiles/r2_leg_stacked.txt)
-    const char* l1_env = getenv("OVN_L1_TC");
-    const int mode = l1_env ? (l1_env[0] - '0') : (L.cin > 8 ? 1 : 2);
-    const int fold = (mode == 2) ? L.kh : 1;
-    const int khp = L.kh / fold;
-    const int c8in = (((fold * 2 * L.cin + 7) / 8) + 1) & ~1;
-    const int kwp = (L.kw + 1) / 2;
-    const int n_mma = 16, R = 2 * n_mma;
-    int c8u = 0;
-    for (int cand = c8in; cand >= 2; cand -= 2)
-      if (c8in % cand == 0 && (size_t)cand * R * 16 <= (size_t)LR_B_MAX) { c8u = cand; break; }
-    t->l1_tc = (mode == 1 || mode == 2) && L.sw == 2 && L.cout == 16 && kwp <= 16 && c8u > 0 &&
-               (size_t)khp * 2 * c8in * (128 + 16) * 16 <= (size_t)LB_A_FAT;
-    if (t->l1_tc) {
-      const LayerWeights& w = h->host_w[L.name];
-      const int taps = khp * kwp;
-      const int kc_n = c8in / c8u;
-      std::vector<__half> bs((size_t)taps * c8in * R * 8, __float2half(0.f));
-      for (int dhp = 0; dhp < khp; ++dhp)
-        for (int j = 0; j < kwp; ++j)
-          for (int c8 = 0; c8 < c8in; ++c8)
-            for (int n = 0; n < L.cout; ++n)
-              for (int k = 0; k < 8; ++k) {
-                const int ch = c8 * 8 + k;
-                if (ch >= fold * 2 * L.cin) continue;
-                const int f = ch / (2 * L.cin), rem = ch - f * 2 * L.cin;
-                const int parity = rem / L.cin, c = rem - parity * L.cin, dw = 2 * j + parity;
-                const int dh = (fold == 1) ? dhp : f;
-                if (dw >= L.kw) continue;
-                const float wf = w.kernel[(((size_t)dh * L.kw + dw) * L.cin + c) * L.cout + n];
-                const __half wh = __float2half(wf);
-                const __half wl = __float2half(wf - __half2float(wh));
-                const size_t unit = (size_t)(dhp * kwp + j) * kc_n + c8 / c8u;
-                const size_t base = (unit * c8u + c8 % c8u) * R;
-                bs[(base + n) * 8 + k] = wh;
-                bs[(base + n_mma + n) * 8 + k] = wl;
-              }
-      int rc2;
-      if ((rc2 = upload_vec(h, &t->wstk[0], bs)) != OVN_OK) return rc2;
-      t->stk_c8u[0] = c8u;
-      t->l1_c8in = c8in;
-      t->l1_fold = fold;
-      const int rows = (fold == 1) ? L.h_in : L.h_out;
-      const size_t bytes = (size_t)h->cfg.max_batch_scans * rows * 2 * c8in * ((L.w_in + 1) / 2) * 16 + 32768;
-      OVN_CUDA(h, cudaMalloc(&t->in_planes, bytes));
-      OVN_CUDA(h, cudaMemset(t->in_planes, 0, bytes));
-    }
   }
   for (int b = 0; b < 2; ++b) {
     const size_t bytes = max_planes_bytes * h->cfg.max_batch_scans + 32768;   // + tile overrun slack
     OVN_CUDA(h, cudaMalloc(&t->actp[b], bytes));
     OVN_CUDA(h, cudaMemset(t->actp[b], 0, bytes));
   }
-  OVN_CUDA(h, cudaMalloc(&t->leg_part, (size_t)kLegPartTiles * 128 * 64 * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->leg_counters, (size_t)kLegPartTiles * 4 * sizeof(int)));
-  OVN_CUDA(h, cudaMemset(t->leg_counters, 0, (size_t)kLegPartTiles * 4 * sizeof(int)));
   const int64_t maxp = h->cfg.max_batch_pairs;
   t->rows_pad = ((maxp * PAIR_ROWS + 1024 + 255) / 256) * 256;   // tile overrun (512) + window shift (50) slack; whole c_conv2 tile pairs
   OVN_CUDA(h, cudaMalloc(&t->l16, (size_t)maxp * WF * K4_PITCH * sizeof(__half)));
@@ -2329,24 +1076,15 @@ int tc_pack_weights(ovn_handle* h) {
   OVN_CUDA(h, cudaMalloc(&t->partial, (size_t)t->rows_pad * 2 * sizeof(float)));
   OVN_CUDA(h, cudaMalloc(&t->lc, (size_t)maxp * C6_VOL_L_BYTES));
   OVN_CUDA(h, cudaMalloc(&t->rc, (size_t)maxp * C6_VOL_R_BYTES));
-  OVN_CUDA(h, cudaMalloc(&t->corr_part, (size_t)maxp * 2 * WF * sizeof(float)));
-  OVN_CUDA(h, cudaFuncSetAttribute(k_corr_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(C6Smem)));
+  OVN_CUDA(h, cudaMalloc(&t->corr_part, (size_t)maxp * C6_IBLK * WF * sizeof(float)));
+  OVN_CUDA(h, cudaFuncSetAttribute(k_delta_conv1_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K4Smem)));
+  OVN_CUDA(h, cudaFuncSetAttribute(k_corr_mma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C6_SMEM));
   OVN_CUDA(h, cudaMalloc(&t->mu, CF * sizeof(float)));
   OVN_CUDA(h, cudaMemset(t->mu, 0, CF * sizeof(float)));
   OVN_CUDA(h, cudaMemset(t->o1, 0, (size_t)120 * t->rows_pad * 8 * sizeof(__half)));
   OVN_CUDA(h, cudaMemset(t->x3, 0, (size_t)16 * t->rows_pad * 8 * sizeof(__half)));
-  OVN_CUDA(h, cudaFuncSetAttribute(k_delta_conv1_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K4Smem)));
-  OVN_CUDA(h, cudaFuncSetAttribute(k_conv2_sw_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(C2Smem)));
-  OVN_CUDA(h, cudaFuncSetAttribute(k_conv3_resident_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(C3Smem)));
-  OVN_CUDA(h, cudaFuncSetAttribute(k_conv3_pair_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(P3Smem)));
   OVN_CUDA(h, cudaFuncSetAttribute(k_leg_layer1_small<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   OVN_CUDA(h, cudaFuncSetAttribute(k_leg_layer1_small<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  OVN_CUDA(h, cudaFuncSetAttribute(k_leg_resident_tc<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LRSmem)));
-  OVN_CUDA(h, cudaFuncSetAttribute(k_leg_resident_tc<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LRSmem)));
-#define OVN_LB_ATTR(E, T) OVN_CUDA(h, cudaFuncSetAttribute(k_leg_batched_tc<E, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LBSmem)))
-  OVN_LB_ATTR(3, 1); OVN_LB_ATTR(3, 2); OVN_LB_ATTR(3, 4); OVN_LB_ATTR(4, 1); OVN_LB_ATTR(4, 2); OVN_LB_ATTR(4, 4);
-#undef OVN_LB_ATTR
-  OVN_CUDA(h, cudaFuncSetAttribute(k_leg_batched_tc<4, 1, 2, LB_A_FAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LBSmemFat)));
   return OVN_OK;
 }
 
@@ -2374,9 +1112,8 @@ k_nhwc_to_planes(const float* __restrict__ x, int64_t total_chunks, int H, int W
 }
 
 int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cudaStream_t s) {
-  // layer 1 (C_in = 4..25, stride (2,2), N = 16) runs on the direct SIMT kernel and writes hi/lo fp16
-  // C8-interleaved planes; layers 2.. run on tcgen05 with the activation window resident in shared
-  // memory (kw taps = descriptor row offsets, kh taps = the input rows' planes).
+  // layer 1 (C_in = 4..25, stride (2,2), N = 16: K = 16 per MMA would be mostly padding) runs on the
+  // direct SIMT kernels and writes hi/lo fp16 C8-interleaved planes; layers 2.. run on k_leg_mma.
   TcState* t = h->tc;
   if (!t) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "tensor-core weights not packed");
   prof_mark(h, PROF_LEG, s);
@@ -2385,31 +1122,7 @@ int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cuda
     const int64_t chunks = (int64_t)n * L.h_out * (L.cout / 8) * L.w_out;
     const size_t w_bytes = (size_t)L.kw * L.cin * L.cout * sizeof(float);        // one kernel row of taps
     const size_t w_all = w_bytes * L.kh;
-    if (n > 2 && t->l1_tc) {
-      // batched encode: layer 1 on tensor cores through even / odd column planes (kernel rows folded into K for narrow inputs)
-      const int c8in = t->l1_c8in, Wh = (L.w_in + 1) / 2, kwp = (L.kw + 1) / 2, fold = t->l1_fold;
-      const int rows = (fold == 1) ? L.h_in : L.h_out, khp = L.kh / fold;
-      const int64_t total = (int64_t)n * rows * c8in * Wh;
-      if ((int64_t)n * rows > 0x7fffffffll) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "tensor-core leg: batch too large for the plane prepass");
-      k_input_to_parity_planes<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(d_input, total, L.h_in, L.w_in, L.cin, c8in, Wh,
-                                                                           rows, fold, L.sh, t->in_planes);
-      OVN_LAUNCH_CHECK(h);
-      LegArgs la = {};
-      la.A = t->in_planes; la.a_pitch = Wh; la.runs_per_img = L.h_out; la.in_img_planes = rows * 2 * c8in;
-      la.in_run_planes = ((fold == 1) ? L.sh : 1) * 2 * c8in; la.kh = khp; la.kw = kwp; la.c8in = c8in; la.Bp = t->wstk[0];
-      la.c8u = t->stk_c8u[0];
-      la.bias = h->d_b[0]; la.n_valid = L.cout; la.M = L.w_out; la.out_planes = t->actp[0]; la.out_pitch = L.w_out;
-      la.out_run_planes = 2 * (L.cout / 8); la.out_f32 = nullptr; la.n_split = 1;
-      const size_t per_px = (size_t)khp * 2 * c8in * 16;
-      int T = 0;
-      for (int cand = 4; cand >= 1; cand >>= 1)
-        if (per_px * (cand * 128 + 16) <= (size_t)LB_A_MAX && (cand == 1 || (cand / 2) * 128 < L.w_out)) { T = cand; break; }
-      const dim3 grid((unsigned)((L.w_out + (T ? T : 1) * 128 - 1) / ((T ? T : 1) * 128)), (unsigned)(n * L.h_out), 1);
-      if (T == 4) k_leg_batched_tc<4, 4><<<grid, G_THREADS, sizeof(LBSmem), s>>>(la, 16, h->d_err);
-      else if (T == 2) k_leg_batched_tc<4, 2><<<grid, G_THREADS, sizeof(LBSmem), s>>>(la, 16, h->d_err);
-      else if (T == 1) k_leg_batched_tc<4, 1><<<grid, G_THREADS, sizeof(LBSmem), s>>>(la, 16, h->d_err);
-      else k_leg_batched_tc<4, 1, 2, LB_A_FAT><<<grid, G_THREADS, sizeof(LBSmemFat), s>>>(la, 16, h->d_err);
-    } else if (n <= 2 && w_all <= 200 * 1024 && L.cout % 8 == 0) {
+    if (n <= 2 && w_all <= 200 * 1024 && L.cout % 8 == 0) {
       const unsigned grid = (unsigned)((chunks + 255) / 256);
       if (L.cin == 4)
         k_leg_layer1_small<true><<<grid, 256, w_all, s>>>(d_input, h->d_w[0], h->d_b[0], n, L.h_in, L.w_in, L.cin, L.kh, L.kw,
@@ -2438,72 +1151,16 @@ int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cuda
   for (int l = 1; l < h->n_leg; ++l) {
     const ConvSpec& L = h->leg[l];
     const bool last = (l == h->n_leg - 1);
-    // latency mode (1-2 scans): one 128-pixel tile and one 64-channel slice per CTA, K split over CTAs;
-    // throughput mode (batched encode): TILES tiles per CTA share every streamed weight slab
-    const int tiles_x = (L.w_out + 127) / 128, nz = (L.cout + 63) / 64;
-    const int base_ctas = tiles_x * n * L.h_out * nz;
-    const bool latency = base_ctas * 2 <= h->sm_count;
+    const int nz = (L.cout + 63) / 64;
     if (last && (L.cout != 128 || L.h_out != 1)) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "tensor-core leg: unexpected last layer");
     LegArgs la = {};
     la.A = t->actp[cur]; la.a_pitch = L.w_in; la.runs_per_img = L.h_out; la.in_img_planes = L.h_in * 2 * (L.cin / 8);
     la.in_run_planes = L.sh * 2 * (L.cin / 8); la.kh = L.kh; la.kw = L.kw; la.c8in = L.cin / 8; la.Bp = t->wres[l];
     la.bias = h->d_b[l]; la.n_valid = L.cout; la.M = L.w_out; la.out_planes = t->actp[cur ^ 1]; la.out_pitch = L.w_out;
     la.out_run_planes = 2 * (L.cout / 8); la.out_f32 = d_fv;
-    la.n_split = 1; la.part = t->leg_part; la.counters = t->leg_counters;
-    if (latency) {
-      dim3 grid((unsigned)tiles_x, (unsigned)(n * L.h_out), (unsigned)nz);
-      // split-K so that a layer's CTAs roughly fill the GPU
-      const int n_slabs_l = L.kh * L.kw * 3;
-      // measured (single scan, whole leg): >= 1 / 2 / 3 / 4 / 6 / 9 / 18 slabs per split ->
-      // 0.196 / 0.165 / 0.151 / 0.144 / 0.138 / 0.152 / 0.154 ms; filling the GPU twice over is worse
-      constexpr int kMinSlabsPerSplit = 6;
-      int n_split = h->sm_count / base_ctas;
-      if (n_split > n_slabs_l / kMinSlabsPerSplit) n_split = n_slabs_l / kMinSlabsPerSplit;
-      if (n_split > kLegPartTiles / base_ctas) n_split = kLegPartTiles / base_ctas;
-      if (n_split < 1) n_split = 1;
-      la.n_split = n_split;
-      grid.z *= n_split;
-      cudaLaunchConfig_t lc = {};
-      lc.gridDim = grid; lc.blockDim = dim3(G_THREADS); lc.dynamicSmemBytes = sizeof(LRSmem); lc.stream = s;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[0].val.programmaticStreamSerializationAllowed = 1;
-      lc.attrs = attr; lc.numAttrs = 1;
-      if (last) OVN_CUDA(h, cudaLaunchKernelEx(&lc, k_leg_resident_tc<3>, la, h->d_err));
-      else OVN_CUDA(h, cudaLaunchKernelEx(&lc, k_leg_resident_tc<4>, la, h->d_err));
-    } else {
-      const bool wide = t->leg_wide && L.cout == 128 && t->wstkw[l] != nullptr;
-      const int nzb = wide ? 1 : nz;
-      int T = 1;
-      if (wide) {
-        // 256 accumulator columns per tile: at most two tiles; fewest (waves x tiles), ties to the larger tile count
-        long best = -1;
-        for (int cand = 2; cand >= 1; --cand) {
-          const size_t win_bytes = (size_t)L.kh * 2 * (L.cin / 8) * (cand * 128 + 16) * 16;
-          if (win_bytes > (size_t)LB_A_MAX) continue;
-          const int ctas = ((L.w_out + cand * 128 - 1) / (cand * 128)) * n * L.h_out;
-          const long cost = (long)((ctas + h->sm_count - 1) / h->sm_count) * cand;
-          if (best < 0 || cost < best) { best = cost; T = cand; }
-        }
-      } else {
-        // largest tile count whose activation window fits and that still gives every SM a CTA
-        for (int cand = 4; cand >= 2; cand >>= 1) {
-          const size_t win_bytes = (size_t)L.kh * 2 * (L.cin / 8) * (cand * 128 + 16) * 16;
-          const int ctas = ((L.w_out + cand * 128 - 1) / (cand * 128)) * n * L.h_out * nz;
-          if (win_bytes <= (size_t)LB_A_MAX && ctas >= h->sm_count) { T = cand; break; }
-        }
-      }
-      if ((size_t)L.kh * 2 * (L.cin / 8) * (128 + 16) * 16 > (size_t)LB_A_MAX)
-        OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "tensor-core leg: layer %s window does not fit shared memory", L.name);
-      const dim3 grid((unsigned)((L.w_out + T * 128 - 1) / (T * 128)), (unsigned)(n * L.h_out), (unsigned)nzb);
-      int n_mma = wide ? 128 : (L.cout >= 64 ? 64 : ((L.cout + 15) / 16) * 16);   // MMA N (multiple of 16 for M = 128)
-      la.Bp = wide ? t->wstkw[l] : t->wstk[l];
-      la.c8u = wide ? t->stkw_c8u[l] : t->stk_c8u[l];
-#define OVN_LEG_BATCHED(E, TT) k_leg_batched_tc<E, TT><<<grid, G_THREADS, sizeof(LBSmem), s>>>(la, n_mma, h->d_err)
-      if (last) { if (T == 4) OVN_LEG_BATCHED(3, 4); else if (T == 2) OVN_LEG_BATCHED(3, 2); else OVN_LEG_BATCHED(3, 1); }
-      else { if (T == 4) OVN_LEG_BATCHED(4, 4); else if (T == 2) OVN_LEG_BATCHED(4, 2); else OVN_LEG_BATCHED(4, 1); }
-#undef OVN_LEG_BATCHED
-    }
+    const dim3 grid((unsigned)(n * L.h_out), (unsigned)((L.w_out + MMA_ROWS - 1) / MMA_ROWS), (unsigned)nz);
+    if (last) k_leg_mma<3><<<grid, MMA_THREADS, 0, s>>>(la);
+    else k_leg_mma<4><<<grid, MMA_THREADS, 0, s>>>(la);
     OVN_LAUNCH_CHECK(h);
     cur ^= 1;
   }
@@ -2578,18 +1235,17 @@ static int calibrate_all(ovn_handle* h, const float* d_vols, const int32_t* d_id
   k_gather_rows_f16<<<(unsigned)((per + 255) / 256), 256, 0, s>>>(d_vols, d_idx, 1, t->mu, WF / 2, t->r16);
   OVN_LAUNCH_CHECK(h);
   const int64_t Mc = PAIR_ROWS;
-  const int n_it_c = (int)((Mc + 255) / 256);
   const int g4c = NB < h->sm_count ? NB : h->sm_count;
-  k_delta_conv1_tc<<<g4c, K4_THREADS, sizeof(K4Smem), s>>>(t->l16, nullptr, t->r16, 0, t->w1p, t->mu_o1, t->o1, 1, h->d_err);
+  const dim3 g2c((unsigned)((Mc + MMA_ROWS - 1) / MMA_ROWS), 2);
+  k_delta_conv1_wgmma<<<g4c, K4_THREADS, sizeof(K4Smem), s>>>(t->l16, nullptr, t->r16, 0, t->w1p, t->mu_o1, t->o1, 1, h->d_err);
   OVN_LAUNCH_CHECK(h);
   k_o1_channel_mean<<<1, 1024, 0, s>>>(t->o1, Mc, t->mu_o1);
   OVN_LAUNCH_CHECK(h);
   k_fold_bias2<<<1, 128, 0, s>>>(t->b2base, t->mu_o1, h->d_w[base + 1], t->b2eff);
   OVN_LAUNCH_CHECK(h);
-  k_delta_conv1_tc<<<g4c, K4_THREADS, sizeof(K4Smem), s>>>(t->l16, nullptr, t->r16, 0, t->w1p, t->mu_o1, t->o1, 1, h->d_err);
+  k_delta_conv1_wgmma<<<g4c, K4_THREADS, sizeof(K4Smem), s>>>(t->l16, nullptr, t->r16, 0, t->w1p, t->mu_o1, t->o1, 1, h->d_err);
   OVN_LAUNCH_CHECK(h);
-  k_conv2_sw_tc<<<n_it_c, G_THREADS, sizeof(C2Smem), s>>>(t->o1, t->w2p, t->b2eff, t->mu_x3, t->x3, t->rows_pad, Mc, n_it_c, 0,
-                                                       h->d_err);
+  k_conv2_mma<<<g2c, MMA_THREADS, 0, s>>>(t->o1, t->w2p, t->b2eff, t->mu_x3, t->x3, t->rows_pad, Mc, 0, h->d_err);
   OVN_LAUNCH_CHECK(h);
   k_x3_channel_mean<<<1, 1024, 0, s>>>(t->x3, t->rows_pad, Mc, t->mu_x3);
   OVN_LAUNCH_CHECK(h);
@@ -2656,7 +1312,7 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
     k_gather_rows_f16<<<(unsigned)((per + 255) / 256), 256, 0, s>>>(d_query, nullptr, 1, t->mu, 0, t->r16);
     OVN_LAUNCH_CHECK(h);
   }
-  const bool inject_fault = getenv("OVN_DEBUG_FAULT") != nullptr;            // tests/test_gpu_errors.py
+  const bool inject_fault = getenv("OVN_DEBUG_FAULT") != nullptr;            // error-path test hook
   for (int p0 = 0; p0 < n; p0 += maxp) {
     const int np = (n - p0 < maxp) ? n - p0 : maxp;
     const int32_t* left = d_left + p0;
@@ -2679,37 +1335,23 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
       k_gather_rows_f16<<<(unsigned)((np * per + 255) / 256), 256, 0, s>>>(d_bank, right, np, t->mu, 0, t->r16);
       OVN_LAUNCH_CHECK(h);
     }
+    const int64_t M = (int64_t)np * PAIR_ROWS;
+    const unsigned row_blocks = (unsigned)((M + MMA_ROWS - 1) / MMA_ROWS);
+    prof_mark(h, PROF_DELTA, s);
     const int64_t units = (int64_t)np * NB;
     const int grid4 = units < h->sm_count ? (int)units : h->sm_count;
-    const int64_t M = (int64_t)np * PAIR_ROWS;
-    const int n_iter2 = (int)((M + 255) / 256);
-    const int grid2 = n_iter2 < h->sm_count ? n_iter2 : h->sm_count;
-    prof_mark(h, PROF_DELTA, s);
-    k_delta_conv1_tc<<<grid4, K4_THREADS, sizeof(K4Smem), s>>>(l16, lidx, t->r16, d_query ? 0 : 1, t->w1p, t->mu_o1, t->o1, np, h->d_err);
+    k_delta_conv1_wgmma<<<grid4, K4_THREADS, sizeof(K4Smem), s>>>(l16, lidx, t->r16, d_query ? 0 : 1, t->w1p, t->mu_o1, t->o1,
+                                                                 np, h->d_err);
     prof_mark(h, PROF_DELTA, s);
     OVN_LAUNCH_CHECK(h);
     prof_mark(h, PROF_CONV2, s);
-    k_conv2_sw_tc<<<grid2, G_THREADS, sizeof(C2Smem), s>>>(
-        t->o1, t->w2p, t->b2eff, t->mu_x3, t->x3, t->rows_pad, M, n_iter2, inject_fault ? 1 : 0, h->d_err);
+    k_conv2_mma<<<dim3(row_blocks, 2), MMA_THREADS, 0, s>>>(t->o1, t->w2p, t->b2eff, t->mu_x3, t->x3, t->rows_pad, M,
+                                                          inject_fault ? 1 : 0, h->d_err);
     prof_mark(h, PROF_CONV2, s);
     OVN_LAUNCH_CHECK(h);
     prof_mark(h, PROF_CONV3, s);
-    if (getenv("OVN_CONV3_1CTA") != nullptr) {                 // the single-CTA kernel (A/B tests: bit-identical results)
-      k_conv3_resident_tc<<<grid2, G_THREADS, sizeof(C3Smem), s>>>(
-          t->x3, t->rows_pad, t->w3p, t->b3eff, M, n_iter2, h->d_w[base + 3], t->partial, h->d_err);
-    } else {
-      int n_cl = h->sm_count / 2;
-      if (n_cl > n_iter2) n_cl = n_iter2;
-      cudaLaunchConfig_t lc = {};
-      lc.gridDim = dim3((unsigned)(2 * n_cl)); lc.blockDim = dim3(G_THREADS); lc.dynamicSmemBytes = sizeof(P3Smem); lc.stream = s;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-      lc.attrs = attr; lc.numAttrs = 1;
-      OVN_CUDA(h, cudaLaunchKernelEx(&lc, k_conv3_pair_tc, (const __half*)t->x3, (int64_t)t->rows_pad, (const __half*)t->w3p,
-                                     (const float*)t->b3eff, (int64_t)M, (int)n_iter2, (const float*)h->d_w[base + 3],
-                                     t->partial, h->d_err));
-    }
+    k_conv3_mma<<<dim3(row_blocks, 2), MMA_THREADS, 0, s>>>(t->x3, t->rows_pad, t->w3p, t->b3eff, M, h->d_w[base + 3],
+                                                          t->partial);
     prof_mark(h, PROF_CONV3, s);
     OVN_LAUNCH_CHECK(h);
     k_dense_finalize<<<np, 256, 0, s>>>(t->partial, h->d_b[base + 3], PAIR_ROWS, d_overlap + p0, h->d_err);
@@ -2730,11 +1372,8 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
         k_pack_corr_R<<<(unsigned)((np * perR + 255) / 256), 256, 0, s>>>(d_bank, right, np, t->rc);
         OVN_LAUNCH_CHECK(h);
       }
-      int g6 = h->sm_count / 2;
-      if (g6 > np) g6 = np;
-      if (g6 < 1) g6 = 1;
       prof_mark(h, PROF_CORR, s);
-      k_corr_tc<<<2 * g6, C6_THREADS, sizeof(C6Smem), s>>>(lc, lidx, t->rc, d_query ? 0 : 1, np, t->corr_part, h->d_err);
+      k_corr_mma<<<dim3((unsigned)np, C6_IBLK), MMA_THREADS, C6_SMEM, s>>>(lc, lidx, t->rc, d_query ? 0 : 1, t->corr_part);
       prof_mark(h, PROF_CORR, s);
       OVN_LAUNCH_CHECK(h);
       k_corr_finalize<<<np, 384, 0, s>>>(t->corr_part, d_corr ? d_corr + (int64_t)p0 * WF : nullptr, d_yaw + p0, h->d_err);
@@ -2747,9 +1386,3 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
 }
 
 }  // namespace ovn
-
-#ifdef OVN_K4_TRACE
-extern "C" int ovn_debug_k4_trace(long long* out_host, long long n_bytes) {
-  return (int)cudaMemcpyFromSymbol(out_host, ovn::g_k4_trace, (size_t)n_bytes);
-}
-#endif

@@ -126,7 +126,7 @@ k_project_scatter(const float4* __restrict__ pts, const int64_t* __restrict__ of
       // image -- floor(t) IS the reference's bin.  Otherwise (0.2 % of the points) the float64 function is
       // rounded once and pushed through the exact pipeline.  The first version ran the exact pipeline on
       // both ends of an error bracket for every point: 4 correctly rounded divisions, 295 instructions per
-      // point, issue-bound (profiles/r1_ncu_summary_v3.txt).
+      // point, issue-bound.
       // ---- yaw bin (utils.py:86,90,94,98-100)
       int bx;
       {

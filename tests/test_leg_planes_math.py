@@ -1,85 +1,18 @@
-"""The algebra behind the tensor-core layer 1 of the batched leg (overlapnet_b200/csrc/network_tc.cu:
-k_input_to_parity_planes + the `wstk[0]` packing in tc_pack_weights), restated in NumPy and checked on the
-CPU against the oracle's first layer (generateNet.py:161-164: 5 x 15 kernel, strides (2, 2), valid).
-
-  even / odd column planes   P[r, w', parity * C + c]            = x[r, 2 w' + parity, c]
-  folded kernel rows         P[y, w', (f * 2 + parity) * C + c]  = x[2 y + f, 2 w' + parity, c]
-
-turn the stride-(2, 2) convolution into a stride-(2, 1) / stride-(1, 1) one with kw' = ceil(15 / 2) = 8 column taps
-(the tap that would be column 15 has zero weights).  The same index formulas are used by the CUDA kernels; the GPU
-tests (tests/test_gpu_network.py::test_batched_leg_*) check those against the float64 oracle end to end.
-"""
+"""The three-term hi/lo product the tensor-core path uses for the leg layers and the correlation head
+(overlapnet_b200/csrc/network_tc.cu: k_leg_mma, k_corr_mma), restated in NumPy: x * w ~= x_hi w_hi + x_hi w_lo
++ x_lo w_hi with fp16 halves and fp32-grade accumulation."""
 import numpy as np
-import pytest
-
-from oracle import network as N
-
-MODEL = {'additional_unsymmetric_layer3a': True, 'strides_layer1': [2, 2]}
-
-
-def planes_and_weights(x, kernel, fold):
-  """x: (H, W, C) float64, kernel: (kh, kw, C, cout).  Returns planes (rows, Wh, K') and the packed weights
-  (kh', kw', K', cout) exactly as the device code lays them out (K' zero-padded to a multiple of 16)."""
-  H, W, C = x.shape
-  kh, kw, _, cout = kernel.shape
-  sh = 2
-  h_out = (H - kh) // sh + 1
-  Wh, kwp = (W + 1) // 2, (kw + 1) // 2
-  f_n = kh if fold else 1
-  rows = h_out if fold else H
-  kp = ((f_n * 2 * C + 15) // 16) * 16
-  planes = np.zeros((rows, Wh, kp))
-  wp = np.zeros((kh // f_n, kwp, kp, cout))
-  for ch in range(f_n * 2 * C):
-    f, rem = divmod(ch, 2 * C)
-    parity, c = divmod(rem, C)
-    for r in range(rows):
-      in_row = r * sh + f if fold else r
-      cols = x[in_row, parity::2, c]
-      planes[r, :len(cols), ch] = cols
-    for dhp in range(kh // f_n):
-      dh = f if fold else dhp
-      for j in range(kwp):
-        dw = 2 * j + parity
-        if dw < kw:
-          wp[dhp, j, ch] = kernel[dh, dw, c]
-  return planes, wp, h_out
-
-
-def conv_planes(planes, wp, h_out, w_out, fold, bias):
-  khp, kwp = wp.shape[:2]
-  out = np.zeros((h_out, w_out, wp.shape[3]))
-  for y in range(h_out):
-    for dhp in range(khp):
-      row = y if fold else 2 * y + dhp
-      for j in range(kwp):
-        out[y] += planes[row, j:j + w_out] @ wp[dhp, j]
-  return np.maximum(out + bias, 0.0)
-
-
-@pytest.mark.parametrize('channels', [4, 5, 25])
-@pytest.mark.parametrize('fold', [False, True])
-def test_column_planes_reproduce_layer1(channels, fold):
-  rng = np.random.default_rng(channels)
-  x = rng.normal(size=(1, 64, 900, channels))
-  w = N.glorot_weights(channels, MODEL, seed=1)
-  kernel, bias = [np.asarray(a, dtype=np.float64) for a in w['s_conv1']]
-  ref = N.leg_forward(x, w, MODEL, return_all=True)[0][0]                 # (30, 443, 16) float64
-  planes, wp, h_out = planes_and_weights(x[0], kernel, fold)
-  got = conv_planes(planes, wp, h_out, ref.shape[1], fold, bias)
-  assert got.shape == ref.shape
-  assert np.abs(got - ref).max() <= 1e-12 * max(1.0, np.abs(ref).max())
 
 
 def test_hi_lo_stacked_product_is_fp32_grade():
-  """x*w ~= x_hi*[w_hi | w_lo] + x_lo*w_hi with fp16 halves and fp32 accumulation: the term left out (x_lo*w_lo)
-  is below 2^-22 relative."""
+  """x*w ~= x_hi*w_hi + x_hi*w_lo + x_lo*w_hi with fp16 halves and fp32 accumulation: the term left out
+  (x_lo*w_lo) is below 2^-22 relative."""
   rng = np.random.default_rng(0)
   x = rng.normal(size=(512, 240)).astype(np.float32)
   w = rng.normal(size=(240, 16)).astype(np.float32)
   xh = x.astype(np.float16); xl = (x - xh.astype(np.float32)).astype(np.float16)
   wh = w.astype(np.float16); wl = (w - wh.astype(np.float32)).astype(np.float16)
-  stacked = xh.astype(np.float64) @ np.concatenate([wh, wl], axis=1).astype(np.float64)     # one MMA, N = 2 n
-  got = stacked[:, :16] + stacked[:, 16:] + xl.astype(np.float64) @ wh.astype(np.float64)
+  f = lambda a: a.astype(np.float64)
+  got = f(xh) @ f(wh) + f(xh) @ f(wl) + f(xl) @ f(wh)
   ref = x.astype(np.float64) @ w.astype(np.float64)
   assert np.abs(got - ref).max() / np.abs(ref).max() < 2e-6

@@ -9,11 +9,7 @@ from overlapnet_b200.engine import Engine
 sys.path.insert(0, ROOT)
 import bench
 
-def run(channels, use, batch, total, l1_tc=None, wide=None):
-  if wide is None: os.environ.pop('OVN_LEG_WIDE', None)
-  else: os.environ['OVN_LEG_WIDE'] = wide
-  if l1_tc is None: os.environ.pop('OVN_L1_TC', None)
-  else: os.environ['OVN_L1_TC'] = l1_tc
+def run(channels, use, batch, total):
   eng = Engine(use=use, model=bench.MODEL, precision='f16_tc', max_batch_scans=batch, max_batch_pairs=1)
   eng.load_weights(bench.make_weights(channels))
   x = torch.from_numpy(synth.range_like_images(5, 8, channels)).to(eng.device).repeat(total // 8, 1, 1, 1)
@@ -25,14 +21,13 @@ def run(channels, use, batch, total, l1_tc=None, wide=None):
   b.record(); torch.cuda.synchronize()
   ms = a.elapsed_time(b) / 5
   flop = {4: bench.FLOP_LEG_C4, 25: bench.FLOP_LEG_C25}.get(channels, bench.FLOP_LEG_C4)
-  print('C=%d batch=%d total=%d l1_tc=%s wide=%s: %.3f ms  %.2f us/scan  %.1f TFLOP/s algorithmic (x3 issued)' %
-        (channels, batch, total, l1_tc, wide, ms, ms * 1e3 / total, total * flop / 1e12 / (ms * 1e-3)))
+  print('C=%d batch=%d total=%d: %.3f ms  %.2f us/scan  %.1f TFLOP/s algorithmic (x3 issued)' %
+        (channels, batch, total, ms, ms * 1e3 / total, total * flop / 1e12 / (ms * 1e-3)))
   eng.close()
 
 if __name__ == '__main__':
   sem = {'use_intensity': True, 'use_class_probabilities': True}
-  for mode in (sys.argv[1:] or ['0', '1', '2']):
-    run(4, {}, 64, 256, l1_tc=mode)
+  run(4, {}, 64, 256)
   run(4, {}, 256, 256)
   run(5, {'use_intensity': True}, 64, 256)
   run(25, sem, 64, 256)
