@@ -1,5 +1,6 @@
 // hopper.cuh -- hand-written PTX wrappers for the Hopper (sm_90a) building blocks used by network_tc.cu:
-// wgmma (warpgroup MMA, A from registers, B from shared memory), mbarrier, cp.async.bulk (TMA engine, 1-D).
+// wgmma (warpgroup MMA; B from shared memory, A from registers or shared memory), mbarrier, cp.async.bulk
+// (TMA engine, 1-D).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -42,12 +43,17 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
 }
 
 // ---- wgmma ------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, K-major operand without swizzle: 8 x 16-byte core matrices,
-//   element (row r, k) at start + (r / 8) * SBO + (r % 8) * 16 + (k / 8) * LBO + (k % 8) * 2   (16-bit types)
-//   bits [0,14) start >> 4, [16,30) LBO >> 4, [32,46) SBO >> 4, [62,64) layout (0 = no swizzle)
-__device__ __forceinline__ uint64_t desc_kmajor_noswizzle(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
+// Shared-memory matrix descriptor of a K-major operand (16-bit types):
+//   bits [0,14) start >> 4, [16,30) LBO >> 4, [32,46) SBO >> 4, [62,64) layout
+// kNoSwizzle: 8 x 16-byte core matrices, 16-byte aligned,
+//   element (row r, k) at start + (r / 8) * SBO + (r % 8) * 16 + (k / 8) * LBO + (k % 8) * 2
+// kSwizzle128B: rows of 128 bytes (64 K values) whose 16-byte chunk c is stored at c ^ (r % 8), 8-row atoms of
+//   1024 bytes (SBO = 1024, LBO unused), tile on a 1024-byte boundary; the K16 step k of a 64-wide tile starts
+//   at tile + 32 k bytes (the hardware applies the XOR to the final address).
+constexpr uint32_t kNoSwizzle = 0, kSwizzle128B = 1;
+__device__ __forceinline__ uint64_t desc_kmajor(uint32_t smem_addr, uint32_t lbo, uint32_t sbo, uint32_t layout) {
   return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo >> 4) & 0x3FFF) << 32);
+         ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) | ((uint64_t)layout << 62);
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -63,6 +69,18 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1)
+      : "memory");
+}
+
+// D[64 x 128] (fp32, registers) += A[64 x 16] * B[16 x 128], both fp16 K-major in shared memory.  Executed by all
+// 128 threads of a warpgroup.  D fragment: d[4 j + {0, 1}] = (row 16 w + g, col 8 j + 2 t + {0, 1}),
+// d[4 j + {2, 3}] = row + 8, j < 16.
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(1)
       : "memory");
 }
 

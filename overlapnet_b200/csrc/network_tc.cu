@@ -1,17 +1,19 @@
 // network_tc.cu -- tensor-core path (precision f16_tc) of the leg and the two heads, for Hopper (sm_90a).
 //
 // Replaces: DeltaLayer + c_conv1 (generateNet.py:15-61,96-100)      -> k_delta_conv1_wgmma
-//           c_conv2 (+ReLU) (generateNet.py:102-105)                -> k_conv2_mma
-//           c_conv3 (+ReLU), Flatten + Dense(1, sigmoid) (:107-114) -> k_conv3_mma + k_dense_finalize
+//           c_conv2 (+ReLU) (generateNet.py:102-105)                -> k_conv2_wgmma
+//           c_conv3 (+ReLU), Flatten + Dense(1, sigmoid) (:107-114) -> k_conv3_wgmma + k_dense_finalize
 //           NormalizedCorrelation2D + argmax (:117-143, infer.py)   -> k_corr_mma + k_corr_finalize
 //           leg Conv2D stack (generateNet.py:149-230)               -> layer 1: k_leg_layer1_small (1-2 scans) /
 //                                                                      k_leg_layer1_direct (batches), SIMT fp32;
 //                                                                      layers 2..: k_leg_mma
 //
-// Every GEMM runs on warp-level tensor-core MMAs (mma.sync m16n8k16, fp16 operands, fp32 accumulators)
-// whose fragments are loaded straight from the packed operand layouts below (8 consecutive K values per
-// 16-byte chunk).  k_delta_conv1_wgmma (83 % of the FLOPs of a pair) synthesises its A operand |l - r| in
-// registers, so the 66 MB delta tensor of a pair (the reference's DeltaLayer output) is never materialised.
+// Every GEMM runs on tensor cores (fp16 operands, fp32 accumulators) and reads packed operand layouts (8
+// consecutive K values per 16-byte chunk).  The delta head is three persistent, warp-specialised wgmma kernels
+// fed by bulk copies through mbarrier rings: k_delta_conv1_wgmma (83 % of the FLOPs of a pair) synthesises its
+// A operand |l - r| in registers, so the 66 MB delta tensor of a pair (the reference's DeltaLayer output) is
+// never materialised; k_conv2_wgmma and k_conv3_wgmma take both operands from shared memory.  The correlation
+// head and the leg are warp-level mma.sync m16n8k16 kernels whose fragments are loaded straight from global.
 // Operands that must be fp32-grade are split into hi + lo fp16 halves (x = hi + lo exactly to 2^-22).
 #include "common.cuh"
 #include "hopper.cuh"
@@ -275,7 +277,8 @@ struct K4Smem {
 static_assert(sizeof(K4Smem) <= 232448, "k_delta_conv1_wgmma shared memory");
 static_assert(offsetof(K4Smem, B) % 16 == 0 && offsetof(K4Smem, Rw) % 16 == 0, "bulk-copy alignment");
 
-#define K4_WAIT(bar, parity, code)                         \
+// bounded wait of a pipeline stage: on time-out raise `code` and leave the kernel (label `done`)
+#define PIPE_WAIT(bar, parity, code)                       \
   if (!mbar_wait((bar), (parity), kWaitCycles)) {          \
     atomicExch(err, (code));                               \
     goto done;                                             \
@@ -306,19 +309,19 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
       for (int u = u_begin; u < u_end; ++u, ++ui) {
         const int p = u / NB, jb = u - p * NB;
         if (u == u_begin || jb == 0) {
-          K4_WAIT(&S.l_empty, (pi & 1) ^ 1, 101);
+          PIPE_WAIT(&S.l_empty, (pi & 1) ^ 1, 101);
           mbar_arrive_expect_tx(&S.l_full, K4_VOL_BYTES);
           bulk_g2s(S.L, L16 + (size_t)(l_idx ? l_idx[p] : p) * WF * K4_PITCH, K4_VOL_BYTES, &S.l_full);
           ++pi;
         }
         const uint32_t b = ui & 1;
-        K4_WAIT(&S.rw_empty[b], ((ui >> 1) & 1) ^ 1, 103);
+        PIPE_WAIT(&S.rw_empty[b], ((ui >> 1) & 1) ^ 1, 103);
         mbar_arrive_expect_tx(&S.rw_full[b], K4_RWIN_BYTES);
         bulk_g2s(S.Rw[b], R16 + (r_per_pair ? (size_t)p * WF * K4_PITCH : 0) + (size_t)jb * S15 * K4_PITCH, K4_RWIN_BYTES,
                  &S.rw_full[b]);
         for (int grp = 0; grp < K4_NGROUPS; ++grp, ++gi) {
           const uint32_t s = gi % K4_RING, ph = (gi / K4_RING) & 1;
-          K4_WAIT(&S.empty[s], ph ^ 1, 102);
+          PIPE_WAIT(&S.empty[s], ph ^ 1, 102);
           mbar_arrive_expect_tx(&S.full[s], K4_GROUP * K4_BSLICE);
           bulk_g2s(S.B[s], W1p + (size_t)grp * K4_GROUP * (K4_BSLICE / 2), K4_GROUP * K4_BSLICE, &S.full[s]);
         }
@@ -344,9 +347,9 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
     uint32_t pi = 0, gi = 0, ui = 0;
     for (int u = u_begin; u < u_end; ++u, ++ui) {
       const int p = u / NB, jb = u - p * NB;
-      if (u == u_begin || jb == 0) { K4_WAIT(&S.l_full, pi & 1, 402); ++pi; }
+      if (u == u_begin || jb == 0) { PIPE_WAIT(&S.l_full, pi & 1, 402); ++pi; }
       const uint32_t wb = ui & 1;
-      K4_WAIT(&S.rw_full[wb], (ui >> 1) & 1, 404);
+      PIPE_WAIT(&S.rw_full[wb], (ui >> 1) & 1, 404);
       float acc[2][32];
 #pragma unroll
       for (int tt = 0; tt < 2; ++tt)
@@ -376,7 +379,7 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
         for (int dj = 0; dj < S15; ++dj, ++st) {
           const int sl = st % K4_GROUP;
           const uint32_t s = gi % K4_RING;
-          if (sl == 0) K4_WAIT(&S.full[s], (gi / K4_RING) & 1, 202);
+          if (sl == 0) PIPE_WAIT(&S.full[s], (gi / K4_RING) & 1, 202);
           const __half* rp = S.Rw[wb] + dj * K4_PITCH + cc * 32 + 2 * t;
           uint32_t A[2][2][4];                // [tile][kk]
 #pragma unroll
@@ -396,7 +399,7 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
 #pragma unroll
           for (int kk = 0; kk < 2; ++kk) {
             // the K16 step covers W1 chunks k8 = 2 kk, 2 kk + 1: LBO = 1024 B between them, SBO = 128 B per 8 outputs
-            const uint64_t bd = desc_kmajor_noswizzle(slice + kk * 2048, 1024, 128);
+            const uint64_t bd = desc_kmajor(slice + kk * 2048, 1024, 128, kNoSwizzle);
 #pragma unroll
             for (int tt = 0; tt < 2; ++tt) wgmma_m64n64k16_rs(acc[tt], A[tt][kk], bd);
           }
@@ -431,108 +434,287 @@ done:
   return;
 }
 
+// Wait of a consumer with wgmma groups in flight: leaving the loop there would make the compiler wait for them
+// on a divergent path, which serialises every wgmma of the kernel.  A time-out raises `code`, later waits are
+// skipped, and the consumer leaves (`if (failed) goto done`) once its groups are retired.
+#define INFLIGHT_WAIT(bar, parity, code)                                      \
+  if (!failed && !mbar_wait((bar), (parity), kWaitCycles)) {                  \
+    atomicExch(err, (code));                                                  \
+    failed = true;                                                            \
+  }
+
 // ------------------------------------------------------------------------------------------------
-// k_conv2_mma -- c_conv2 (15x1 stride 15, 64 -> 128, ReLU) as a GEMM [M x 960] x [960 x 128], W2 applied as
-// hi + lo (two MMAs per K16 step: the fp16 rounding of W2 was the largest term of the logit error budget
-// after the feature volumes).  A = the o1 tiles k_delta_conv1_wgmma wrote; output = the centred fp16 x3 planes.
+// k_conv2_wgmma -- c_conv2 (15x1 stride 15, 64 -> 128, ReLU) as a GEMM [M x 960] x [960 x 128], W2 applied as
+// hi + lo (two MMAs per K16 step into the same accumulators: the fp16 rounding of W2 was the largest term of
+// the logit error budget after the feature volumes).  A = the o1 tiles k_delta_conv1_wgmma wrote; output = the
+// centred fp16 x3 planes.
+// Persistent and warp-specialised: a CTA walks a contiguous range of 256-row tiles.  Warp 8 is the producer
+// (one lane): per di it bulk-copies the two 16 KB o1 tiles of the 256 rows and the 32 KB W2 hi + lo tiles of
+// that di into a 3-deep ring (full / empty mbarrier pairs).  Warpgroups 0 and 1 own 128 rows each (2 x m64n128
+// fp32 accumulators) and multiply straight out of the SWIZZLE_128B tiles (wgmma, both operands in shared
+// memory), one commit group per di with the previous di's group still in flight.  256 rows per tile because
+// W2 hi + lo (480 KB) is re-read from L2 for every tile: at 128 rows that traffic would be twice the o1 read.
 // `fault` != 0 is the test hook of ovn_debug_inject_fault: the kernel computes nothing and raises the
 // pipeline-failure flag, so that the finalize kernels poison the outputs of the call.
-// grid = (ceil(M / 64), 2 halves of 64 output channels)
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(MMA_THREADS)
-k_conv2_mma(const __half* __restrict__ o1, const __half* __restrict__ W2s, const float* __restrict__ bias2,
-            const float* __restrict__ mu_x3, __half* __restrict__ x3, int64_t out_pitch, int64_t M, int fault,
-            int* __restrict__ err) {
+constexpr int TC_WG = 2;                               // consumer warpgroups of k_conv2_wgmma / k_conv3_wgmma
+constexpr int TC_THREADS = TC_WG * 128 + 32;           // + the producer warp
+constexpr int TC_ROWS = TC_WG * 128;                   // output rows per tile
+constexpr uint32_t C2_TILE = 128 * 64 * 2;             // bytes of one SWIZZLE_128B tile: 128 rows x 64 fp16
+constexpr int C2_RING = 3;
+
+struct C2Smem {
+  __half A[C2_RING][TC_WG][C2_TILE / 2];               // o1 of one di: rows [r0, r0 + 128), [r0 + 128, r0 + 256)
+  __half B[C2_RING][2][C2_TILE / 2];                   // W2 of that di: hi, lo
+  uint64_t full[C2_RING], empty[C2_RING];
+};
+constexpr size_t C2_SMEM = sizeof(C2Smem) + 1024;      // + the round-up of the base to a 1024-byte swizzle atom
+static_assert(C2_SMEM <= 232448, "k_conv2_wgmma shared memory");
+static_assert(offsetof(C2Smem, B) % 1024 == 0 && C2_TILE % 1024 == 0, "SWIZZLE_128B tiles on 1024-byte boundaries");
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
+k_conv2_wgmma(const __half* __restrict__ o1, const __half* __restrict__ W2s, const float* __restrict__ bias2,
+              const float* __restrict__ mu_x3, __half* __restrict__ x3, int64_t out_pitch, int64_t M, int fault,
+              int* __restrict__ err) {
   if (fault) {
-    if (threadIdx.x == 0 && blockIdx.x == 0 && blockIdx.y == 0) atomicExch(err, 501);
+    if (threadIdx.x == 0 && blockIdx.x == 0) atomicExch(err, 501);
     return;
   }
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const int64_t m0 = (int64_t)blockIdx.x * MMA_ROWS + warp * 16;
-  if (m0 >= M) return;
-  const int64_t ma = m0 + g, mb = m0 + g + 8;
-  const int nb0 = blockIdx.y * 64;
-  float acc[8][4] = {};
+  extern __shared__ __align__(128) uint8_t smem_raw[];
+  C2Smem& S = *reinterpret_cast<C2Smem*>(smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023));
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int64_t n_tiles = (M + TC_ROWS - 1) / TC_ROWS;
+  const int64_t t_begin = n_tiles * blockIdx.x / gridDim.x, t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
+  constexpr uint32_t kConsumerWarps = TC_WG * 4;
+  if (tid == 0) {
+    for (int s = 0; s < C2_RING; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], kConsumerWarps); }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp == TC_WG * 4) {
+    // ===================== producer ==========================================================
+    if (lane == 0) {
+      uint32_t gi = 0;
+      for (int64_t tile = t_begin; tile < t_end; ++tile)
+        for (int di = 0; di < S15; ++di, ++gi) {
+          const uint32_t s = gi % C2_RING;
+          PIPE_WAIT(&S.empty[s], ((gi / C2_RING) & 1) ^ 1, 111);
+          mbar_arrive_expect_tx(&S.full[s], 4 * C2_TILE);
+          for (int h = 0; h < TC_WG; ++h)      // o1 tile (m / 128, di) of the rows m = 256 tile + 128 h + [0, 128)
+            bulk_g2s(S.A[s][h], o1 + ((size_t)(tile * TC_WG + h) * S15 + di) * (C2_TILE / 2), C2_TILE, &S.full[s]);
+          bulk_g2s(S.B[s], W2s + (size_t)di * C2_TILE, 2 * C2_TILE, &S.full[s]);
+        }
+    }
+  } else {
+    // ===================== consumers ==========================================================
+    const int wg = warp >> 2, wi = warp & 3, g = lane >> 2, t = lane & 3;
+    uint32_t gi = 0;
+    bool failed = false;
+    for (int64_t tile = t_begin; tile < t_end; ++tile) {
+      float acc[2][64];                       // [m64 sub-tile][D fragment]
+#pragma unroll
+      for (int sub = 0; sub < 2; ++sub)
+#pragma unroll
+        for (int e = 0; e < 64; ++e) acc[sub][e] = 0.f;
 #pragma unroll 1
-  for (int di = 0; di < S15; ++di) {
+      for (int di = 0; di < S15; ++di, ++gi) {
+        const uint32_t s = gi % C2_RING;
+        INFLIGHT_WAIT(&S.full[s], (gi / C2_RING) & 1, 211);
+        const uint32_t a_base = smem_u32(S.A[s][wg]), b_base = smem_u32(S.B[s][0]);
+        wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      const int c8 = kk * 2;
-      const uint32_t a0 = ld_h2(o1 + o1_chunk_offset(ma, di, c8) + 2 * t), a1 = ld_h2(o1 + o1_chunk_offset(mb, di, c8) + 2 * t);
-      const uint32_t a2 = ld_h2(o1 + o1_chunk_offset(ma, di, c8 + 1) + 2 * t), a3 = ld_h2(o1 + o1_chunk_offset(mb, di, c8 + 1) + 2 * t);
+        for (int kk = 0; kk < 4; ++kk)
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int n = nb0 + j * 8 + g;
-        const __half* Bh = W2s + ((size_t)(di * 2) * 128 + n) * 64 + 2 * t;     // [di][hi, lo][n][chunk ^ (n & 7)][8]
-        const int s0 = (c8 ^ (n & 7)) << 3, s1 = ((c8 + 1) ^ (n & 7)) << 3;
-        mma16816(acc[j], a0, a1, a2, a3, ld_h2(Bh + s0), ld_h2(Bh + s1));
-        mma16816(acc[j], a0, a1, a2, a3, ld_h2(Bh + 128 * 64 + s0), ld_h2(Bh + 128 * 64 + s1));
+          for (int part = 0; part < 2; ++part) {  // W2 hi, then lo
+            const uint64_t bd = desc_kmajor(b_base + part * C2_TILE + kk * 32, 16, 1024, kSwizzle128B);
+#pragma unroll
+            for (int sub = 0; sub < 2; ++sub)     // rows 64 sub + [0, 64) of this warpgroup: 8 KB into the tile
+              wgmma_m64n128k16_ss(acc[sub], desc_kmajor(a_base + sub * (C2_TILE / 2) + kk * 32, 16, 1024, kSwizzle128B), bd);
+          }
+        wgmma_commit();
+        wgmma_wait<1>();                      // the previous di's group is done: its stage can be refilled
+        if (di > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&S.empty[(gi - 1) % C2_RING]);
+        }
       }
+      wgmma_wait<0>();
+      if (failed) goto done;
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&S.empty[(gi - 1) % C2_RING]);
+      // b2eff, ReLU, minus the x3 centre, fp16 into the C8-interleaved planes (rows past M are not stored)
+#pragma unroll
+      for (int sub = 0; sub < 2; ++sub)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int64_t m = tile * TC_ROWS + wg * 128 + sub * 64 + wi * 16 + g + 8 * h;
+          if (m >= M) continue;
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const int n = j * 8 + 2 * t;
+            const float a = fmaxf(acc[sub][4 * j + 2 * h] + __ldg(bias2 + n), 0.f) - __ldg(mu_x3 + n);
+            const float b = fmaxf(acc[sub][4 * j + 2 * h + 1] + __ldg(bias2 + n + 1), 0.f) - __ldg(mu_x3 + n + 1);
+            *reinterpret_cast<uint32_t*>(x3 + ((size_t)j * out_pitch + m) * 8 + 2 * t) = pack_h2(a, b);
+          }
+        }
     }
   }
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int64_t m = h ? mb : ma;
-    if (m >= M) continue;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int n = nb0 + j * 8 + 2 * t;
-      const float a = fmaxf(acc[j][2 * h] + __ldg(bias2 + n), 0.f) - __ldg(mu_x3 + n);
-      const float b = fmaxf(acc[j][2 * h + 1] + __ldg(bias2 + n + 1), 0.f) - __ldg(mu_x3 + n + 1);
-      *reinterpret_cast<uint32_t*>(x3 + ((size_t)(n >> 3) * out_pitch + m) * 8 + (n & 7)) = pack_h2(a, b);
-    }
-  }
+done:
+  return;
 }
 
 // ------------------------------------------------------------------------------------------------
-// k_conv3_mma -- c_conv3 (3x3, 128 -> 256, ReLU) + Flatten + the Dense(1) partial sum of each row.
-// Rows are (pair, jb, ib) in the x3 planes; the 3x3 tap (dy, dx) reads row r + dy * 24 + dx.
+// k_conv3_wgmma -- c_conv3 (3x3, 128 -> 256, ReLU) + Flatten + the Dense(1) partial sum of each row.
+// Rows are (pair, jb, ib) in the x3 planes; the 3x3 tap (a, b) reads row r + a * 24 + b (implicit im2col).
 // partial[r][nh] = sum over the 128 channels of half nh of relu(conv + b3eff) * w_dense (0 for the
 // rows a valid convolution does not produce).
-// grid = (ceil(M / 64), 2 halves of 128 output channels)
+// Persistent and warp-specialised; a tile is 256 output rows x one half nh of the output channels, and the
+// two halves of a row block are consecutive tiles of one CTA (the second finds its x3 rows in L2).  Warp 8 is
+// the producer (one lane): the 16 x3 planes of rows [r0, r0 + 306), one 4.9 KB bulk copy per plane (78 KB,
+// double-buffered and issued a tile ahead), and W3 half nh in stages of two (tap, 32-channel) slabs (16 KB)
+// through a 4-deep ring.  The x3 planes are the no-swizzle K-major layout a descriptor reads (8 rows x 16 B
+// core matrices, LBO = plane pitch, SBO = 128 B), so all 9 taps read the same stage from a start address
+// shifted by a * 24 + b rows.  Warpgroups 0 and 1 own 128 rows each (2 x m64n128 fp32 accumulators).
+// 256 rows per tile because W3 half nh (288 KB) is re-read from L2 for every tile.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(MMA_THREADS)
-k_conv3_mma(const __half* __restrict__ X3, int64_t a_pitch, const __half* __restrict__ Bp, const float* __restrict__ bias,
-            int64_t M, const float* __restrict__ wd, float* __restrict__ partial) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const int64_t r0 = (int64_t)blockIdx.x * MMA_ROWS + warp * 16;
-  if (r0 >= M) return;
-  const int nh = blockIdx.y;
-  float acc[16][4] = {};
-#pragma unroll 1
-  for (int tap = 0; tap < 9; ++tap) {
-    const int64_t shift = (tap / 3) * NB + (tap % 3);
-    const __half* Aa = X3 + (r0 + g + shift) * 8 + 2 * t;
-    const __half* Ab = Aa + 8 * 8;
-#pragma unroll 1
-    for (int c16 = 0; c16 < 8; ++c16) {
-      const size_t p0 = (size_t)(2 * c16) * a_pitch * 8, p1 = p0 + (size_t)a_pitch * 8;
-      const uint32_t a0 = ld_h2(Aa + p0), a1 = ld_h2(Ab + p0), a2 = ld_h2(Aa + p1), a3 = ld_h2(Ab + p1);
-      // [nh][slab = tap * 4 + c / 32][(c / 8) % 4][n][8]
-      const __half* B = Bp + (((size_t)(nh * 36 + tap * 4 + (c16 >> 1)) * 4 + (c16 & 1) * 2) * 128 + g) * 8 + 2 * t;
+constexpr int C3_AROWS = TC_ROWS + 2 * NB + 2;         // + the reach of the 3x3 window
+constexpr uint32_t C3_PLANE = C3_AROWS * 16;           // bytes of one x3 plane in shared memory
+constexpr uint32_t C3_SLAB = 4 * 128 * 16;             // W3 slab (tap, 32 channels) x 128 outputs: [4 k8][128 n][8]
+constexpr int C3_GROUP = 2;                            // slabs per ring stage
+constexpr int C3_NSTAGES = 36 / C3_GROUP;              // ring stages per tile
+constexpr int C3_RING = 4;
+
+struct C3Smem {
+  __half A[2][16 * C3_PLANE / 2];                      // [buffer][plane c / 8][row][8]
+  __half B[C3_RING][C3_GROUP * C3_SLAB / 2];
+  uint64_t full[C3_RING], empty[C3_RING], a_full[2], a_empty[2];
+};
+static_assert(sizeof(C3Smem) <= 232448, "k_conv3_wgmma shared memory");
+static_assert(offsetof(C3Smem, B) % 16 == 0 && C3_PLANE % 16 == 0, "bulk-copy alignment");
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
+k_conv3_wgmma(const __half* __restrict__ X3, int64_t a_pitch, const __half* __restrict__ W3p, const float* __restrict__ bias,
+              int64_t M, const float* __restrict__ wd, float* __restrict__ partial, int* __restrict__ err) {
+  extern __shared__ __align__(128) uint8_t smem_raw[];
+  C3Smem& S = *reinterpret_cast<C3Smem*>(smem_raw);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int64_t n_tiles = 2 * ((M + TC_ROWS - 1) / TC_ROWS);     // tile = 2 * row block + nh
+  const int64_t t_begin = n_tiles * blockIdx.x / gridDim.x, t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
+  constexpr uint32_t kConsumerWarps = TC_WG * 4;
+  if (tid == 0) {
+    for (int s = 0; s < C3_RING; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], kConsumerWarps); }
+    for (int b = 0; b < 2; ++b) { mbar_init(&S.a_full[b], 1); mbar_init(&S.a_empty[b], kConsumerWarps); }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp == TC_WG * 4) {
+    // ===================== producer ==========================================================
+    if (lane == 0) {
+      const uint32_t nt = (uint32_t)(t_end - t_begin);
+      uint32_t ai = 0, gi = 0;                // tiles whose x3 rows were issued, W3 stages issued
+      for (uint32_t ti = 0; ti < nt; ++ti) {
+        const int nh = (int)((t_begin + ti) & 1);
+        for (int st = 0; st < C3_NSTAGES; ++st, ++gi) {
+          // x3 rows of this tile (must go now) and of the next one (as soon as its buffer is free, i.e. once
+          // the tile before this one is done), so that they load while this tile computes
+          while (ai < nt && ai <= ti + 1) {
+            const uint32_t b = ai & 1, par = ((ai >> 1) & 1) ^ 1;
+            if (ai > ti) {
+              if (!mbar_try_wait(&S.a_empty[b], par)) break;
+            } else {
+              PIPE_WAIT(&S.a_empty[b], par, 121);
+            }
+            const int64_t r0 = ((t_begin + ai) >> 1) * TC_ROWS;
+            mbar_arrive_expect_tx(&S.a_full[b], 16 * C3_PLANE);
+            for (int pl = 0; pl < 16; ++pl)
+              bulk_g2s(S.A[b] + pl * (C3_PLANE / 2), X3 + ((size_t)pl * a_pitch + r0) * 8, C3_PLANE, &S.a_full[b]);
+            ++ai;
+          }
+          const uint32_t s = gi % C3_RING;
+          PIPE_WAIT(&S.empty[s], ((gi / C3_RING) & 1) ^ 1, 122);
+          mbar_arrive_expect_tx(&S.full[s], C3_GROUP * C3_SLAB);
+          bulk_g2s(S.B[s], W3p + ((size_t)nh * 36 + st * C3_GROUP) * (C3_SLAB / 2), C3_GROUP * C3_SLAB, &S.full[s]);
+        }
+      }
+    }
+  } else {
+    // ===================== consumers ==========================================================
+    const int wg = warp >> 2, wi = warp & 3, g = lane >> 2, t = lane & 3;
+    const uint32_t b_base = smem_u32(S.B[0]);
+    uint32_t gi = 0;
+    bool failed = false;
+    for (int64_t tile = t_begin; tile < t_end; ++tile) {
+      const uint32_t ti = (uint32_t)(tile - t_begin), ab = ti & 1;
+      const int nh = (int)(tile & 1);
+      const int64_t r0 = (tile >> 1) * TC_ROWS;
+      PIPE_WAIT(&S.a_full[ab], (ti >> 1) & 1, 221);
+      const uint32_t a_rows = smem_u32(S.A[ab]) + wg * 128 * 16;
+      float acc[2][64];                       // [m64 sub-tile][D fragment]
 #pragma unroll
-      for (int j = 0; j < 16; ++j) mma16816(acc[j], a0, a1, a2, a3, ld_h2(B + j * 64), ld_h2(B + 128 * 8 + j * 64));
+      for (int sub = 0; sub < 2; ++sub)
+#pragma unroll
+        for (int e = 0; e < 64; ++e) acc[sub][e] = 0.f;
+#pragma unroll 1
+      for (int st = 0; st < C3_NSTAGES; ++st, ++gi) {
+        const uint32_t s = gi % C3_RING;
+        INFLIGHT_WAIT(&S.full[s], (gi / C3_RING) & 1, 222);
+        wgmma_fence();
+#pragma unroll
+        for (int sl = 0; sl < C3_GROUP; ++sl) {
+          // slab = tap * 4 + c / 32; the x3 image is stored transposed, tap = a * 3 + b shifts by a * 24 + b rows
+          const int slab = st * C3_GROUP + sl, tap = slab >> 2, c32 = slab & 3;
+          const uint32_t a_tap = a_rows + ((tap / 3) * NB + tap % 3) * 16;
+          const uint32_t slab_addr = b_base + s * (C3_GROUP * C3_SLAB) + sl * C3_SLAB;
+#pragma unroll
+          for (int kk = 0; kk < 2; ++kk) {    // K16 step = planes 2 c16, 2 c16 + 1 = W3 k8 chunks 2 kk, 2 kk + 1
+            const int c16 = c32 * 2 + kk;
+            const uint64_t bd = desc_kmajor(slab_addr + kk * 4096, 2048, 128, kNoSwizzle);
+#pragma unroll
+            for (int sub = 0; sub < 2; ++sub)
+              wgmma_m64n128k16_ss(acc[sub], desc_kmajor(a_tap + 2 * c16 * C3_PLANE + sub * 64 * 16, C3_PLANE, 128, kNoSwizzle), bd);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                      // the previous stage's group is done: its slot can be refilled
+        if (st > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&S.empty[(gi - 1) % C3_RING]);
+        }
+      }
+      wgmma_wait<0>();
+      if (failed) goto done;
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&S.empty[(gi - 1) % C3_RING]);
+        mbar_arrive(&S.a_empty[ab]);
+      }
+#pragma unroll
+      for (int sub = 0; sub < 2; ++sub)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int64_t r = r0 + wg * 128 + sub * 64 + wi * 16 + g + 8 * h;
+          const int rem = (int)(r % PAIR_ROWS);
+          const int yy = rem / NB, xx = rem - yy * NB;
+          const bool valid = (r < M) && (yy < NB - 2) && (xx < NB - 2);
+          // rows are (pair, jb, ib): yy = jb, xx = ib; Flatten order of the reference is (ib, jb, channel)
+          const float* wrow = wd + (size_t)(valid ? (xx * (NB - 2) + yy) : 0) * 256 + nh * 128;
+          float sum = 0.f;
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const int n = j * 8 + 2 * t;
+            sum = fmaf(fmaxf(acc[sub][4 * j + 2 * h] + __ldg(bias + nh * 128 + n), 0.f), __ldg(wrow + n), sum);
+            sum = fmaf(fmaxf(acc[sub][4 * j + 2 * h + 1] + __ldg(bias + nh * 128 + n + 1), 0.f), __ldg(wrow + n + 1), sum);
+          }
+          sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+          sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+          if (t == 0 && r < M) partial[r * 2 + nh] = valid ? sum : 0.f;
+        }
     }
   }
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int64_t r = r0 + g + 8 * h;
-    const int rem = (int)(r % PAIR_ROWS);
-    const int yy = rem / NB, xx = rem - yy * NB;
-    const bool valid = (r < M) && (yy < NB - 2) && (xx < NB - 2);
-    // rows are (pair, jb, ib): yy = jb, xx = ib; Flatten order of the reference is (ib, jb, channel)
-    const float* wrow = wd + (size_t)(valid ? (xx * (NB - 2) + yy) : 0) * 256 + nh * 128;
-    float s = 0.f;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int n = j * 8 + 2 * t;
-      s = fmaf(fmaxf(acc[j][2 * h] + __ldg(bias + nh * 128 + n), 0.f), __ldg(wrow + n), s);
-      s = fmaf(fmaxf(acc[j][2 * h + 1] + __ldg(bias + nh * 128 + n + 1), 0.f), __ldg(wrow + n + 1), s);
-    }
-    s += __shfl_xor_sync(0xffffffffu, s, 1);
-    s += __shfl_xor_sync(0xffffffffu, s, 2);
-    if (t == 0 && r < M) partial[r * 2 + nh] = valid ? s : 0.f;
-  }
+done:
+  return;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1066,7 +1248,8 @@ int tc_pack_weights(ovn_handle* h) {
     OVN_CUDA(h, cudaMemset(t->actp[b], 0, bytes));
   }
   const int64_t maxp = h->cfg.max_batch_pairs;
-  t->rows_pad = ((maxp * PAIR_ROWS + 1024 + 255) / 256) * 256;   // tile overrun (512) + window shift (50) slack; whole c_conv2 tile pairs
+  // + slack for the last 256-row tile of c_conv2 / c_conv3 (255 rows) and c_conv3's window (50 rows); whole tiles
+  t->rows_pad = ((maxp * PAIR_ROWS + 1024 + 255) / 256) * 256;
   OVN_CUDA(h, cudaMalloc(&t->l16, (size_t)maxp * WF * K4_PITCH * sizeof(__half)));
   OVN_CUDA(h, cudaMalloc(&t->r16, (size_t)maxp * WF * K4_PITCH * sizeof(__half)));
   OVN_CUDA(h, cudaMemset(t->l16, 0, (size_t)maxp * WF * K4_PITCH * sizeof(__half)));
@@ -1078,6 +1261,8 @@ int tc_pack_weights(ovn_handle* h) {
   OVN_CUDA(h, cudaMalloc(&t->rc, (size_t)maxp * C6_VOL_R_BYTES));
   OVN_CUDA(h, cudaMalloc(&t->corr_part, (size_t)maxp * C6_IBLK * WF * sizeof(float)));
   OVN_CUDA(h, cudaFuncSetAttribute(k_delta_conv1_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K4Smem)));
+  OVN_CUDA(h, cudaFuncSetAttribute(k_conv2_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM));
+  OVN_CUDA(h, cudaFuncSetAttribute(k_conv3_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(C3Smem)));
   OVN_CUDA(h, cudaFuncSetAttribute(k_corr_mma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C6_SMEM));
   OVN_CUDA(h, cudaMalloc(&t->mu, CF * sizeof(float)));
   OVN_CUDA(h, cudaMemset(t->mu, 0, CF * sizeof(float)));
@@ -1236,7 +1421,7 @@ static int calibrate_all(ovn_handle* h, const float* d_vols, const int32_t* d_id
   OVN_LAUNCH_CHECK(h);
   const int64_t Mc = PAIR_ROWS;
   const int g4c = NB < h->sm_count ? NB : h->sm_count;
-  const dim3 g2c((unsigned)((Mc + MMA_ROWS - 1) / MMA_ROWS), 2);
+  const int64_t tiles_c = (Mc + TC_ROWS - 1) / TC_ROWS;
   k_delta_conv1_wgmma<<<g4c, K4_THREADS, sizeof(K4Smem), s>>>(t->l16, nullptr, t->r16, 0, t->w1p, t->mu_o1, t->o1, 1, h->d_err);
   OVN_LAUNCH_CHECK(h);
   k_o1_channel_mean<<<1, 1024, 0, s>>>(t->o1, Mc, t->mu_o1);
@@ -1245,7 +1430,8 @@ static int calibrate_all(ovn_handle* h, const float* d_vols, const int32_t* d_id
   OVN_LAUNCH_CHECK(h);
   k_delta_conv1_wgmma<<<g4c, K4_THREADS, sizeof(K4Smem), s>>>(t->l16, nullptr, t->r16, 0, t->w1p, t->mu_o1, t->o1, 1, h->d_err);
   OVN_LAUNCH_CHECK(h);
-  k_conv2_mma<<<g2c, MMA_THREADS, 0, s>>>(t->o1, t->w2p, t->b2eff, t->mu_x3, t->x3, t->rows_pad, Mc, 0, h->d_err);
+  k_conv2_wgmma<<<(unsigned)tiles_c, TC_THREADS, C2_SMEM, s>>>(t->o1, t->w2p, t->b2eff, t->mu_x3, t->x3, t->rows_pad, Mc, 0,
+                                                              h->d_err);
   OVN_LAUNCH_CHECK(h);
   k_x3_channel_mean<<<1, 1024, 0, s>>>(t->x3, t->rows_pad, Mc, t->mu_x3);
   OVN_LAUNCH_CHECK(h);
@@ -1336,7 +1522,9 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
       OVN_LAUNCH_CHECK(h);
     }
     const int64_t M = (int64_t)np * PAIR_ROWS;
-    const unsigned row_blocks = (unsigned)((M + MMA_ROWS - 1) / MMA_ROWS);
+    const int64_t tiles = (M + TC_ROWS - 1) / TC_ROWS;                 // 256-row tiles of c_conv2 / c_conv3
+    const int grid2 = tiles < h->sm_count ? (int)tiles : h->sm_count;
+    const int grid3 = 2 * tiles < h->sm_count ? (int)(2 * tiles) : h->sm_count;
     prof_mark(h, PROF_DELTA, s);
     const int64_t units = (int64_t)np * NB;
     const int grid4 = units < h->sm_count ? (int)units : h->sm_count;
@@ -1345,13 +1533,13 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
     prof_mark(h, PROF_DELTA, s);
     OVN_LAUNCH_CHECK(h);
     prof_mark(h, PROF_CONV2, s);
-    k_conv2_mma<<<dim3(row_blocks, 2), MMA_THREADS, 0, s>>>(t->o1, t->w2p, t->b2eff, t->mu_x3, t->x3, t->rows_pad, M,
-                                                          inject_fault ? 1 : 0, h->d_err);
+    k_conv2_wgmma<<<grid2, TC_THREADS, C2_SMEM, s>>>(t->o1, t->w2p, t->b2eff, t->mu_x3, t->x3, t->rows_pad, M,
+                                                     inject_fault ? 1 : 0, h->d_err);
     prof_mark(h, PROF_CONV2, s);
     OVN_LAUNCH_CHECK(h);
     prof_mark(h, PROF_CONV3, s);
-    k_conv3_mma<<<dim3(row_blocks, 2), MMA_THREADS, 0, s>>>(t->x3, t->rows_pad, t->w3p, t->b3eff, M, h->d_w[base + 3],
-                                                          t->partial);
+    k_conv3_wgmma<<<grid3, TC_THREADS, sizeof(C3Smem), s>>>(t->x3, t->rows_pad, t->w3p, t->b3eff, M, h->d_w[base + 3],
+                                                            t->partial, h->d_err);
     prof_mark(h, PROF_CONV3, s);
     OVN_LAUNCH_CHECK(h);
     k_dense_finalize<<<np, 256, 0, s>>>(t->partial, h->d_b[base + 3], PAIR_ROWS, d_overlap + p0, h->d_err);
