@@ -192,6 +192,33 @@ int ovn_bank_prepare(ovn_handle* h, const float* d_bank, int64_t bank_capacity, 
                      void* stream);
 int ovn_bank_release(ovn_handle* h, const float* d_bank);
 
+/* ---- training of the overlap head with a frozen leg (training.py; legsType 360OutputkLegsFixed,
+ * generateNet.py:222-324) ------------------------------------------------------------------------
+ * c_conv1..3 and overlap_output are trained, the leg is never touched.  fp32 arithmetic; every reduction
+ * runs in a fixed order, so identical calls give bit-identical weights.  The gradient, Adagrad-accumulator
+ * and activation buffers are allocated when a handle first trains (sized by max_batch_pairs).
+ * Losses (training.py:71-92,255-257): L = 5 L_ov + L_or,
+ *   L_ov = mean_p sigmoid((|overlap_p - gt_overlap_p| + 0.25) * 24 - 12),
+ *   L_or = mean_p mean_k weighted_cross_entropy_with_logits(t_pk, corr_pk, pos_weight = 360),
+ *   t_pk = 1 iff k == gt_orientation_p and gt_overlap_p > min_overlap_for_angle
+ *   (ImagePairOverlapOrientationSequence.py:118-121).  With a frozen leg L_or has no gradient. */
+/* fp32 handles only (OVN_ERR_BAD_CONFIG otherwise); n_pairs <= max_batch_pairs (OVN_ERR_CAPACITY).
+ * Forward of both heads + losses + backward of the overlap head for LEFT = bank[left], RIGHT = bank[right].
+ * Synchronous: h_loss[3] = {total, overlap, orientation}.  Leaves the batch gradients in the handle.
+ * An index outside the bank returns OVN_ERR_INVALID_ARG and leaves no usable gradients. */
+int ovn_head_gradients(ovn_handle* h, const float* d_bank, int64_t bank_size,
+                       const int32_t* d_left_idx, const int32_t* d_right_idx, int32_t n_pairs,
+                       const float* d_gt_overlap, const int32_t* d_gt_orientation,
+                       float min_overlap_for_angle, float* h_loss, void* stream);
+/* Adagrad update of c_conv1..3 / overlap_output from the last valid gradients (Keras 2.1.5:
+ * a += g^2; w -= lr g / (sqrt(a) + 1e-7), accumulators start at 0); refuses (INVALID_ARG) when there are
+ * none.  ovn_finalize_weights resets the accumulators. */
+int ovn_head_adagrad_step(ovn_handle* h, float learning_rate, void* stream);
+/* Current weights / last gradients of a layer, Keras layout, host buffers (same shapes as ovn_set_weights).
+ * Both synchronise the device.  ovn_get_gradients applies to the head layers only. */
+int ovn_get_weights(ovn_handle* h, const char* layer_name, float* h_kernel, float* h_bias);
+int ovn_get_gradients(ovn_handle* h, const char* layer_name, float* h_kernel, float* h_bias);
+
 /* ---- deferred device errors ------------------------------------------------------------------
  * The device-pointer entry points never synchronise, so two classes of error can only be detected on
  * the device: an index outside [0, bank_size) (or, for a resident bank, a row that was never

@@ -241,7 +241,7 @@ int ovn_create(const ovn_config* cfg, ovn_handle** out) {
   CREATE_CUDA(cudaMalloc(&h->d_err, sizeof(int)));
   CREATE_CUDA(cudaMemset(h->d_err, 0, sizeof(int)));
   CREATE_CUDA(cudaEventCreateWithFlags(&h->ev_bank, cudaEventDisableTiming));
-  // pinned staging of the host entry points: [err int, pad][offsets 2 x i64][cand idx][overlap][yaw]
+  // pinned staging of the host entry points: [err int, pad][offsets 2 x i64][3 training losses, pad][cand idx][overlap][yaw]
   h->cap_pinned = 64 + (int64_t)c.max_batch_pairs * 12;
   CREATE_CUDA(cudaHostAlloc(&h->h_pinned, (size_t)h->cap_pinned, cudaHostAllocDefault));
   CREATE_CUDA(cudaMalloc(&h->d_logit, (size_t)c.max_batch_pairs * sizeof(float)));
@@ -261,6 +261,7 @@ int ovn_destroy(ovn_handle* h) {
   if (!h) return OVN_OK;
   DeviceGuard guard(h);
   tc_free(h);
+  train_free(h);
   for (auto& p : h->d_w) if (p) cudaFree(p);
   for (auto& p : h->d_b) if (p) cudaFree(p);
   for (auto& p : h->d_w16) if (p) cudaFree(p);
@@ -387,7 +388,59 @@ int ovn_finalize_weights(ovn_handle* h) {
     int rc = tc_pack_weights(h);
     if (rc != OVN_OK) return rc;
   }
+  if (h->train) {                        // new weights: Adagrad starts over, old gradients are stale
+    OVN_CUDA(h, cudaMemset(h->train->accum, 0, (size_t)h->train->n_param * sizeof(float)));
+    h->train->grads_valid = false;
+  }
   h->weights_ready = true;
+  return OVN_OK;
+}
+
+// kernel / bias sizes and weight slot of a layer; dense = overlap_output
+static int layer_slot(const ovn_handle* h, const char* name, int64_t* n_kernel, int64_t* n_bias, bool* head) {
+  if (strcmp(name, "overlap_output") == 0) {
+    *n_kernel = h->dense_in; *n_bias = 1; *head = true;
+    return kMaxLegLayers + 3;
+  }
+  int slot = -1;
+  const ConvSpec* L = find_layer(h, name, &slot);
+  if (!L) return -1;
+  *n_kernel = (int64_t)L->kh * L->kw * L->cin * L->cout;
+  *n_bias = L->cout;
+  *head = slot >= kMaxLegLayers;
+  return slot;
+}
+
+int ovn_get_weights(ovn_handle* h, const char* name, float* h_kernel, float* h_bias) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  if (!name || !h_kernel || !h_bias) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_get_weights: NULL argument");
+  if (!h->weights_ready) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "ovn_get_weights: weights not finalised");
+  int64_t nk, nb;
+  bool head;
+  const int slot = layer_slot(h, name, &nk, &nb, &head);
+  if (slot < 0) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "ovn_get_weights: unknown layer name '%s'", name);
+  OVN_CUDA(h, cudaDeviceSynchronize());            // weights may be updated by work queued on any stream
+  OVN_CUDA(h, cudaMemcpy(h_kernel, h->d_w[slot], nk * sizeof(float), cudaMemcpyDeviceToHost));
+  OVN_CUDA(h, cudaMemcpy(h_bias, h->d_b[slot], nb * sizeof(float), cudaMemcpyDeviceToHost));
+  return OVN_OK;
+}
+
+int ovn_get_gradients(ovn_handle* h, const char* name, float* h_kernel, float* h_bias) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  if (!name || !h_kernel || !h_bias) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_get_gradients: NULL argument");
+  int64_t nk, nb;
+  bool head;
+  const int slot = layer_slot(h, name, &nk, &nb, &head);
+  if (slot < 0 || !head)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_get_gradients: '%s' is not a layer of the overlap head", name);
+  if (!h->train || !h->train->grads_valid)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_get_gradients: no valid gradients (call ovn_head_gradients first)");
+  const float* g = h->train->grad + h->train->off[slot - kMaxLegLayers];
+  OVN_CUDA(h, cudaDeviceSynchronize());
+  OVN_CUDA(h, cudaMemcpy(h_kernel, g, nk * sizeof(float), cudaMemcpyDeviceToHost));
+  OVN_CUDA(h, cudaMemcpy(h_bias, g + nk, nb * sizeof(float), cudaMemcpyDeviceToHost));
   return OVN_OK;
 }
 
@@ -567,6 +620,53 @@ int ovn_heads_rows_vs_bank(ovn_handle* h, const float* d_bank, int64_t bank_size
     if (rc != OVN_OK) return rc;
   }
   return OVN_OK;
+}
+
+// ---- training of the overlap head (frozen leg) ----------------------------------------------------
+int ovn_head_gradients(ovn_handle* h, const float* d_bank, int64_t bank_size, const int32_t* d_left_idx,
+                       const int32_t* d_right_idx, int32_t n_pairs, const float* d_gt_overlap,
+                       const int32_t* d_gt_orientation, float min_overlap_for_angle, float* h_loss, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_head_gradients: %s", h->net_error.c_str());
+  if (h->cfg.precision != OVN_PREC_FP32)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_head_gradients: training needs a precision fp32 handle");
+  if (!h->weights_ready) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "ovn_head_gradients: weights not finalised");
+  REQUIRE(h, n_pairs > 0 && bank_size > 0, "n_pairs and bank_size must be positive");
+  REQUIRE(h, d_bank && d_left_idx && d_right_idx && d_gt_overlap && d_gt_orientation && h_loss, "NULL pointer");
+  const int maxp = h->cfg.max_batch_pairs;
+  if (n_pairs > maxp)
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "ovn_head_gradients: n_pairs=%d exceeds max_batch_pairs=%d", n_pairs, maxp);
+  if (!h->train) {
+    int rc = train_alloc(h);
+    if (rc != OVN_OK) return rc;
+  }
+  h->train->grads_valid = false;
+  cudaStream_t s = (cudaStream_t)stream;
+  int32_t* l = h->d_idx_san;
+  int32_t* r = h->d_idx_san + maxp;
+  int rc = sanitize_indices(h, d_left_idx, n_pairs, bank_size, kErrBadIndex, l, s);
+  if (rc == OVN_OK) rc = sanitize_indices(h, d_right_idx, n_pairs, bank_size, kErrBadIndex, r, s);
+  if (rc == OVN_OK)
+    rc = head_gradients_fp32(h, d_bank, l, r, n_pairs, d_gt_overlap, d_gt_orientation, min_overlap_for_angle, s);
+  if (rc != OVN_OK) return rc;
+  float* p_loss = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(h->h_pinned) + 48);
+  OVN_CUDA(h, cudaMemcpyAsync(p_loss, h->train->loss, 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  rc = check_device_error(h, s);            // synchronises s; a bad index -> OVN_ERR_INVALID_ARG
+  if (rc != OVN_OK) return rc;
+  memcpy(h_loss, p_loss, 3 * sizeof(float));
+  h->train->grads_valid = true;
+  return OVN_OK;
+}
+
+int ovn_head_adagrad_step(ovn_handle* h, float learning_rate, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  if (h->cfg.precision != OVN_PREC_FP32)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_head_adagrad_step: training needs a precision fp32 handle");
+  if (!h->train || !h->train->grads_valid)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_head_adagrad_step: no valid gradients (call ovn_head_gradients first)");
+  return head_adagrad_fp32(h, learning_rate, (cudaStream_t)stream);
 }
 
 int ovn_bank_prepare(ovn_handle* h, const float* d_bank, int64_t bank_capacity, int64_t first, int64_t count,

@@ -32,7 +32,29 @@ struct LayerWeights {
 
 }  // namespace ovn
 
-namespace ovn { struct TcState; }
+namespace ovn {
+struct TcState;
+
+// Training of the overlap head (fp32 handles; allocated when a handle first trains, sized by max_batch_pairs).
+// Gradients and Adagrad accumulators of c_conv1..3 / overlap_output: per layer [K + 1][N] floats at off[l]
+// (the kernel in Keras layout, then the bias).
+struct TrainState {
+  float* x4 = nullptr;          // [max_batch_pairs][dense_in] c_conv3 output, then dL/d(its pre-activation)
+  float* dx3 = nullptr;         // [max_batch_pairs][24][24][128] dL/dx3, then dL/d(pre-activation of c_conv2)
+  float* corr = nullptr;        // [max_batch_pairs][Wf] orientation logits
+  float* overlap = nullptr;     // [max_batch_pairs]
+  float* dz = nullptr;          // [max_batch_pairs] dL/d(Dense logit)
+  int32_t* yaw = nullptr;       // [max_batch_pairs]
+  float* w3t = nullptr;         // c_conv3 kernel with in / out swapped
+  float* part = nullptr;        // split-K partials of the weight gradients
+  float* grad = nullptr;        // [n_param]
+  float* accum = nullptr;       // [n_param] Adagrad accumulators
+  float* loss = nullptr;        // [3] total, overlap, orientation
+  int64_t off[4] = {};
+  int64_t n_param = 0;
+  bool grads_valid = false;     // the last ovn_head_gradients succeeded
+};
+}  // namespace ovn
 
 struct ovn_handle {
   ovn_config cfg;
@@ -89,6 +111,7 @@ struct ovn_handle {
   bool profiling = false;
   std::vector<cudaEvent_t> prof_ev[ovn::kProfKinds];   // start/stop pairs, in launch order
   ovn::TcState* tc = nullptr;              // tensor-core path state (network_tc.cu)
+  ovn::TrainState* train = nullptr;        // overlap-head training state (network_fp32.cu), NULL until first used
 };
 
 #define OVN_SET_ERR(h, code, ...)                                 \
@@ -167,6 +190,14 @@ int leg_layer_fp32(ovn_handle* h, int l, const float* x, float* y, int n, cudaSt
 int heads_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query,
                        const int32_t* d_left, const int32_t* d_right, int n, float* d_overlap,
                        int32_t* d_yaw, float* d_corr, cudaStream_t s);
+
+// training of the overlap head (network_fp32.cu)
+int train_alloc(ovn_handle* h);
+void train_free(ovn_handle* h);
+int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left, const int32_t* right, int np,
+                        const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
+                        cudaStream_t s);
+int head_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s);
 
 int corr_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* left,
                       const int32_t* right, int np, int32_t* d_yaw, float* d_corr, cudaStream_t s);

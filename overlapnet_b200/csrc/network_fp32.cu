@@ -80,6 +80,96 @@ struct GramOperand {
   __device__ __forceinline__ int col_off2(int) const { return 0; }
 };
 
+// ---- operands of the overlap-head backward (training) ----
+// Weight gradient of a valid NHWC conv, as the transposed im2col:  A[k, m] = X[img, ho*sh + dh, wo*sw + dw, c],
+// k = (dh, dw, c) < Kc, m = (img, ho, wo).  Row k = Kc is all ones, so that the same product also yields
+// the bias gradient (the column sums of dY) as row Kc of the [Kc + 1][N] result.
+struct ConvWgradOperand {
+  const float* X;
+  int H, W, C, kw, sh, sw, Ho, Wo, Kc;
+  __device__ __forceinline__ int64_t row_base(int k, int) const {           // offset of tap (dh, dw, c)
+    if (k >= Kc) return 0;
+    const int rowlen = kw * C;
+    const int dh = k / rowlen;
+    return (int64_t)dh * W * C + (k - dh * rowlen);
+  }
+  __device__ __forceinline__ int64_t row_base2(int k, int) const { return k >= Kc; }   // 1: the ones row
+  __device__ __forceinline__ int col_off(int m) const { return m; }
+  __device__ __forceinline__ int col_off2(int) const { return 0; }
+  __device__ __forceinline__ float load(int64_t rb, int m, int64_t ones, int) const {
+    if (ones) return 1.f;
+    const int wo = m % Wo;
+    const int t = m / Wo;
+    const int ho = t % Ho;
+    const int img = t / Ho;
+    return __ldg(X + (((int64_t)img * H + (int64_t)ho * sh) * W + (int64_t)wo * sw) * C + rb);
+  }
+};
+
+// Weight gradient of c_conv1, with the |l - r| operand synthesised like DeltaOperand (never materialised):
+//   A[k, m] = | L[s*ho + dh, c] - R[s*jb + dj, c] |,  k = (dj, c) < Kc,  m = (((p*nho + ho)*nb + jb)*s + dh)
+// m runs over the rows of the c_conv1 output in the order in which the c_conv2 input gradient is stored
+// ([p][ho][jb][dh][o], see head_gradients_fp32).  Row Kc is all ones (bias gradient).
+struct DeltaWgradOperand {
+  const float* bank;
+  const int32_t* left;
+  const int32_t* right;
+  int Wf, Cf, s, nb, nho, Kc;
+  __device__ __forceinline__ int64_t row_base(int k, int) const { return k < Kc ? k % Cf : 0; }       // c
+  __device__ __forceinline__ int64_t row_base2(int k, int) const { return k < Kc ? k / Cf : -1; }     // dj, -1: ones
+  __device__ __forceinline__ int col_off(int m) const { return m; }
+  __device__ __forceinline__ int col_off2(int) const { return 0; }
+  __device__ __forceinline__ float load(int64_t c, int m, int64_t dj, int) const {
+    if (dj < 0) return 1.f;
+    const int dh = m % s;
+    int t = m / s;
+    const int jb = t % nb;
+    t /= nb;
+    const int ho = t % nho;
+    const int p = t / nho;
+    const float l = __ldg(bank + ((int64_t)left[p] * Wf + ho * s + dh) * Cf + c);
+    const float r = __ldg(bank + ((int64_t)right[p] * Wf + s * jb + dj) * Cf + c);
+    return fabsf(l - r);
+  }
+};
+
+// Input gradient of a stride-1 valid conv (the transposed conv):  A[m, k] = dY[img, h - dh, w - dw, n],
+// zero outside dY;  m = (img, h, w) over the [H][W] input, k = (dh, dw, n).  B = the kernel with its
+// in / out axes swapped, [(dh, dw, n)][c].
+struct ConvDgradOperand {
+  const float* dY;            // [img][Ho][Wo][Cout]
+  int Ho, Wo, Cout, kw, H, W;
+  __device__ __forceinline__ int64_t row_base(int m, int) const {
+    const int w = m % W;
+    const int t = m / W;
+    const int hh = t % H;
+    const int img = t / H;
+    return (((int64_t)img * Ho + hh) * Wo + w) * Cout;
+  }
+  __device__ __forceinline__ int64_t row_base2(int m, int) const {
+    const int t = m / W;
+    return ((int64_t)(t % H) << 16) | (m % W);
+  }
+  __device__ __forceinline__ int col_off(int k) const {
+    const int rowlen = kw * Cout;
+    const int dh = k / rowlen;
+    const int r = k - dh * rowlen;
+    const int dw = r / Cout;
+    return -(dh * Wo + dw) * Cout + (r - dw * Cout);
+  }
+  __device__ __forceinline__ int col_off2(int k) const {
+    const int rowlen = kw * Cout;
+    const int dh = k / rowlen;
+    return (dh << 16) | ((k - dh * rowlen) / Cout);
+  }
+  __device__ __forceinline__ float load(int64_t rb, int co, int64_t hw, int tap) const {
+    const int y = (int)(hw >> 16) - (tap >> 16);
+    const int x = (int)(hw & 0xffff) - (tap & 0xffff);
+    if (y < 0 || y >= Ho || x < 0 || x >= Wo) return 0.f;
+    return __ldg(dY + rb + co);
+  }
+};
+
 struct BOperand {
   const float* B;             // weights [K][N] (b_nk = 0) or per-batch [N][K] (b_nk = 1)
   const float* query;         // b_nk: RIGHT volume = query for every z when non-null
@@ -88,28 +178,34 @@ struct BOperand {
   int b_nk;
 };
 
-// C[m, n] = act(sum_k A[m,k] * B[k,n] + bias[n]);  C row-major [z][M][N]
+// C[m, n] = act(sum_k A[m,k] * B[k,n] + bias[n]);  C row-major [z][M][N].
+// kchunk == 0: z = blockIdx.z is the batch index of the operands.  kchunk > 0 (split-K): every z works on
+// the same product and sums only k in [z*kchunk, (z+1)*kchunk); C[z] is that slice's partial, which
+// k_splitk_reduce adds up in a fixed order (no atomics, so results are bit-reproducible).
 template <class AOp>
 __global__ void __launch_bounds__(256)
 k_simt_gemm(AOp a, BOperand bop, const float* __restrict__ bias, float* __restrict__ C, int M, int N, int K,
-            int relu) {
+            int relu, int kchunk) {
   __shared__ float As[BK][BM + 4];
   __shared__ float Bs[BK][BN + 4];
   __shared__ int64_t s_rb[BM];
   __shared__ int64_t s_rb2[BM];
   const int tid = threadIdx.x;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN, z = blockIdx.z;
+  const int zb = kchunk ? 0 : z;
+  const int kbeg = kchunk ? z * kchunk : 0;
+  const int kend = kchunk ? min(K, kbeg + kchunk) : K;
   if (tid < BM) {
     const int m = m0 + tid;
-    s_rb[tid] = m < M ? a.row_base(m, z) : -1;
-    s_rb2[tid] = m < M ? a.row_base2(m, z) : 0;
+    s_rb[tid] = m < M ? a.row_base(m, zb) : -1;
+    s_rb2[tid] = m < M ? a.row_base2(m, zb) : 0;
   }
   const float* Bz = bop.B;
-  if (bop.b_nk) Bz = bop.query ? bop.query : bop.B + (int64_t)bop.right[z] * bop.vol_stride;
+  if (bop.b_nk) Bz = bop.query ? bop.query : bop.B + (int64_t)bop.right[zb] * bop.vol_stride;
   __syncthreads();
   const int ty = tid / 16, tx = tid % 16;
   float acc[4][4] = {};
-  for (int k0 = 0; k0 < K; k0 += BK) {
+  for (int k0 = kbeg; k0 < kend; k0 += BK) {
     // A tile: 64 x 16 elements, consecutive threads -> consecutive k (contiguous in memory)
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -117,7 +213,7 @@ k_simt_gemm(AOp a, BOperand bop, const float* __restrict__ bias, float* __restri
       const int kk = e % BK, mm = e / BK;
       const int k = k0 + kk;
       float v = 0.f;
-      if (k < K && s_rb[mm] >= 0) v = a.load(s_rb[mm], a.col_off(k), s_rb2[mm], a.col_off2(k));
+      if (k < kend && s_rb[mm] >= 0) v = a.load(s_rb[mm], a.col_off(k), s_rb2[mm], a.col_off2(k));
       As[kk][mm] = v;
     }
 #pragma unroll
@@ -126,11 +222,11 @@ k_simt_gemm(AOp a, BOperand bop, const float* __restrict__ bias, float* __restri
       float v = 0.f;
       if (!bop.b_nk) {
         const int nn = e % BN, kk = e / BN;
-        if (k0 + kk < K && n0 + nn < N) v = __ldg(Bz + (int64_t)(k0 + kk) * N + n0 + nn);
+        if (k0 + kk < kend && n0 + nn < N) v = __ldg(Bz + (int64_t)(k0 + kk) * N + n0 + nn);
         Bs[kk][nn] = v;
       } else {
         const int kk = e % BK, nn = e / BK;
-        if (k0 + kk < K && n0 + nn < N) v = __ldg(Bz + (int64_t)(n0 + nn) * K + k0 + kk);
+        if (k0 + kk < kend && n0 + nn < N) v = __ldg(Bz + (int64_t)(n0 + nn) * K + k0 + kk);
         Bs[kk][nn] = v;
       }
     }
@@ -166,9 +262,9 @@ k_simt_gemm(AOp a, BOperand bop, const float* __restrict__ bias, float* __restri
 
 template <class AOp>
 static int launch_gemm(ovn_handle* h, const AOp& a, const BOperand& b, const float* bias, float* C, int M,
-                       int N, int K, int batch, int relu, cudaStream_t s) {
+                       int N, int K, int batch, int relu, cudaStream_t s, int kchunk = 0) {
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM, batch);
-  k_simt_gemm<AOp><<<grid, 256, 0, s>>>(a, b, bias, C, M, N, K, relu);
+  k_simt_gemm<AOp><<<grid, 256, 0, s>>>(a, b, bias, C, M, N, K, relu, kchunk);
   OVN_LAUNCH_CHECK(h);
   return OVN_OK;
 }
@@ -261,52 +357,319 @@ int corr_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, 
   return OVN_OK;
 }
 
+// overlap head of np <= max_batch_pairs pairs: c_conv1 -> h->d_o1, c_conv2 -> h->d_o2, c_conv3 -> d_o3
+// (which may alias d_o1: o1 is dead after c_conv2), Dense + sigmoid -> d_overlap
+static int overlap_head_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* left,
+                             const int32_t* right, int np, float* d_o3, float* d_overlap, cudaStream_t s) {
+  const int Wf = h->cfg.leg_output_width, Cf = kFeatC, sz = h->cfg.conv1size;
+  const int base = kMaxLegLayers;   // weight slots of c_conv1..3, overlap_output
+  // c_conv1 (linear) on the implicit delta image
+  {
+    DeltaOperand a{d_bank, d_query, left, right, Wf, Cf, sz, h->o1_w};
+    BOperand b{h->d_w[base + 0], nullptr, nullptr, 0, 0};
+    prof_mark(h, PROF_DELTA, s);
+    int rc = launch_gemm(h, a, b, h->d_b[base + 0], h->d_o1, np * h->o1_h * h->o1_w, h->head[0].cout,
+                         sz * Cf, 1, 0, s);
+    prof_mark(h, PROF_DELTA, s);
+    if (rc != OVN_OK) return rc;
+  }
+  // c_conv2 (relu): (15,1) stride (15,1) over [p][360][24][64]
+  {
+    const ConvSpec& L = h->head[1];
+    ConvOperand a{h->d_o1, L.h_in, L.w_in, L.cin, L.kw, L.sh, L.sw, L.h_out, L.w_out};
+    BOperand b{h->d_w[base + 1], nullptr, nullptr, 0, 0};
+    int rc = launch_gemm(h, a, b, h->d_b[base + 1], h->d_o2, np * L.h_out * L.w_out, L.cout,
+                         L.kh * L.kw * L.cin, 1, 1, s);
+    if (rc != OVN_OK) return rc;
+  }
+  // c_conv3 (relu) 3x3
+  {
+    const ConvSpec& L = h->head[2];
+    ConvOperand a{h->d_o2, L.h_in, L.w_in, L.cin, L.kw, L.sh, L.sw, L.h_out, L.w_out};
+    BOperand b{h->d_w[base + 2], nullptr, nullptr, 0, 0};
+    int rc = launch_gemm(h, a, b, h->d_b[base + 2], d_o3, np * L.h_out * L.w_out, L.cout,
+                         L.kh * L.kw * L.cin, 1, 1, s);
+    if (rc != OVN_OK) return rc;
+  }
+  k_dense_sigmoid<<<np, 256, 0, s>>>(d_o3, h->d_w[base + 3], h->d_b[base + 3], h->dense_in, d_overlap);
+  OVN_LAUNCH_CHECK(h);
+  return OVN_OK;
+}
+
 int heads_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* d_left,
                        const int32_t* d_right, int n, float* d_overlap, int32_t* d_yaw, float* d_corr,
                        cudaStream_t s) {
-  const int Wf = h->cfg.leg_output_width, Cf = kFeatC, sz = h->cfg.conv1size;
-  const int base = kMaxLegLayers;   // weight slots of c_conv1..3, overlap_output
+  const int Wf = h->cfg.leg_output_width;
   const int maxp = h->cfg.max_batch_pairs;
   for (int p0 = 0; p0 < n; p0 += maxp) {
     const int np = (n - p0 < maxp) ? n - p0 : maxp;
     const int32_t* left = d_left + p0;
     const int32_t* right = d_right ? d_right + p0 : nullptr;
-    // c_conv1 (linear) on the implicit delta image
-    {
-      DeltaOperand a{d_bank, d_query, left, right, Wf, Cf, sz, h->o1_w};
-      BOperand b{h->d_w[base + 0], nullptr, nullptr, 0, 0};
-      prof_mark(h, PROF_DELTA, s);
-      int rc = launch_gemm(h, a, b, h->d_b[base + 0], h->d_o1, np * h->o1_h * h->o1_w, h->head[0].cout,
-                           sz * Cf, 1, 0, s);
-      prof_mark(h, PROF_DELTA, s);
-      if (rc != OVN_OK) return rc;
-    }
-    // c_conv2 (relu): (15,1) stride (15,1) over [p][360][24][64]
-    {
-      const ConvSpec& L = h->head[1];
-      ConvOperand a{h->d_o1, L.h_in, L.w_in, L.cin, L.kw, L.sh, L.sw, L.h_out, L.w_out};
-      BOperand b{h->d_w[base + 1], nullptr, nullptr, 0, 0};
-      int rc = launch_gemm(h, a, b, h->d_b[base + 1], h->d_o2, np * L.h_out * L.w_out, L.cout,
-                           L.kh * L.kw * L.cin, 1, 1, s);
-      if (rc != OVN_OK) return rc;
-    }
-    // c_conv3 (relu) 3x3 -> reuse d_o1 as the o3 buffer (o1 is dead after c_conv2)
-    float* d_o3 = h->d_o1;
-    {
-      const ConvSpec& L = h->head[2];
-      ConvOperand a{h->d_o2, L.h_in, L.w_in, L.cin, L.kw, L.sh, L.sw, L.h_out, L.w_out};
-      BOperand b{h->d_w[base + 2], nullptr, nullptr, 0, 0};
-      int rc = launch_gemm(h, a, b, h->d_b[base + 2], d_o3, np * L.h_out * L.w_out, L.cout,
-                           L.kh * L.kw * L.cin, 1, 1, s);
-      if (rc != OVN_OK) return rc;
-    }
-    k_dense_sigmoid<<<np, 256, 0, s>>>(d_o3, h->d_w[base + 3], h->d_b[base + 3], h->dense_in, d_overlap + p0);
+    // the o3 buffer is d_o1 (o1 is dead after c_conv2)
+    int rc = overlap_head_fp32(h, d_bank, d_query, left, right, np, h->d_o1, d_overlap + p0, s);
+    if (rc != OVN_OK) return rc;
+    rc = corr_forward_fp32(h, d_bank, d_query, left, right, np, d_yaw + p0,
+                           d_corr ? d_corr + (int64_t)p0 * Wf : nullptr, s);
+    if (rc != OVN_OK) return rc;
+  }
+  return OVN_OK;
+}
+
+// ---- training of the overlap head with a frozen leg -------------------------------------------
+// 360OutputkLegsFixed (generateNet.py:222-324): the leg is frozen, c_conv1..3 and overlap_output are
+// trained.  All arithmetic is fp32, every reduction runs in a fixed order (split-K partials + a fixed-order
+// reduction, no floating-point atomics), so two identical runs give bit-identical weights.
+
+constexpr int kMaxSplit = 32;          // split-K slices of a weight-gradient product
+constexpr int kSplitBlocks = 528;      // target CTAs of a split-K launch (4 per SM of a 132-SM H100)
+
+// Losses of training.py:71-92,255-257 and dL/dz of the Dense logit.  One block: fixed summation order.
+//   L_ov = mean_p sigmoid(u_p),  u_p = (|yhat_p - y_p| + 0.25) * 24 - 12
+//   L_or = mean_p mean_k wce(t_pk, corr_pk, pos_weight = Wf),  t_pk = [k == gt_or_p and gt_ov_p > min_ov]
+//          (targets of ImagePairOverlapOrientationSequence.py:118-121; the stable form of
+//          tf.nn.weighted_cross_entropy_with_logits, the logits are raw correlation sums)
+//   L = 5 L_ov + L_or;  dL/dyhat_p = 5 sigmoid'(u_p) * 24 * sign(yhat_p - y_p) / B  (sign(0) = 0, TF's abs)
+//   dz_p = dL/dyhat_p * yhat_p (1 - yhat_p);  the Dense bias gradient = sum_p dz_p.
+__global__ void __launch_bounds__(256)
+k_train_loss(const float* __restrict__ ov, const float* __restrict__ corr, const float* __restrict__ gt_ov,
+             const int32_t* __restrict__ gt_or, int np, int Wf, float min_ov, float* __restrict__ dz,
+             float* __restrict__ g_bias_dense, float* __restrict__ loss) {
+  __shared__ double r_ov[256], r_or[256];
+  const int t = threadIdx.x;
+  double a = 0.0, b = 0.0;
+  for (int p = t; p < np; p += 256) {
+    const float y = ov[p], d = y - gt_ov[p];
+    const float u = (fabsf(d) + 0.25f) * 24.f - 12.f;
+    const float sg = 1.f / (1.f + expf(-u));
+    a += sg;
+    const float sgn = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);
+    dz[p] = 5.f * sg * (1.f - sg) * 24.f * sgn / (float)np * (y * (1.f - y));
+  }
+  const float q = (float)Wf;
+  for (int e = t; e < np * Wf; e += 256) {
+    const int p = e / Wf, k = e - p * Wf;
+    const float x = corr[e];
+    const float z = (k == gt_or[p] && gt_ov[p] > min_ov) ? 1.f : 0.f;
+    b += (1.f - z) * x + (1.f + (q - 1.f) * z) * (log1pf(expf(-fabsf(x))) + fmaxf(-x, 0.f));
+  }
+  r_ov[t] = a;
+  r_or[t] = b;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (t < o) { r_ov[t] += r_ov[t + o]; r_or[t] += r_or[t + o]; }
+    __syncthreads();
+  }
+  if (t == 0) {
+    const double l_ov = r_ov[0] / np, l_or = r_or[0] / ((double)np * Wf);
+    loss[0] = (float)(5.0 * l_ov + l_or);
+    loss[1] = (float)l_ov;
+    loss[2] = (float)l_or;
+    float g = 0.f;
+    for (int p = 0; p < np; ++p) g += dz[p];
+    *g_bias_dense = g;
+  }
+}
+
+// Dense backward: g_wd[i] = sum_p dz_p * x4[p, i] (pairs in order); then x4 is overwritten with
+// dL/d(pre-activation of c_conv3) = dz_p * wd[i] where x4 > 0 (ReLU), 0 elsewhere.
+__global__ void __launch_bounds__(256)
+k_dense_backward(float* __restrict__ x4, const float* __restrict__ wd, const float* __restrict__ dz, int np,
+                 int n_in, float* __restrict__ g_wd) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_in) return;
+  const float w = __ldg(wd + i);
+  float g = 0.f;
+  for (int p = 0; p < np; ++p) {
+    float* x = x4 + (int64_t)p * n_in + i;
+    const float v = *x;
+    const float d = __ldg(dz + p);
+    g = fmaf(d, v, g);
+    *x = v > 0.f ? d * w : 0.f;
+  }
+  g_wd[i] = g;
+}
+
+// d <- d where x > 0, else 0 (gradient through a ReLU whose output is x)
+__global__ void k_relu_grad(float* __restrict__ d, const float* __restrict__ x, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && !(x[i] > 0.f)) d[i] = 0.f;
+}
+
+// conv kernel [taps][cin][cout] -> [taps][cout][cin] (the B operand of the input gradient)
+__global__ void k_swap_io(const float* __restrict__ w, float* __restrict__ wt, int taps, int cin, int cout) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)taps * cin * cout) return;
+  const int n = (int)(i % cout);
+  const int64_t r = i / cout;
+  const int c = (int)(r % cin);
+  const int tap = (int)(r / cin);
+  wt[((int64_t)tap * cout + n) * cin + c] = w[i];
+}
+
+// out[i] = sum_{z < nsplit} part[z][i], z in order
+__global__ void k_splitk_reduce(const float* __restrict__ part, int nsplit, int64_t count, float* __restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  float v = 0.f;
+  for (int z = 0; z < nsplit; ++z) v += part[(int64_t)z * count + i];
+  out[i] = v;
+}
+
+// Adagrad as Keras 2.1.5 does it: a += g^2;  w -= lr * g / (sqrt(a) + 1e-7)
+__global__ void k_adagrad(float* __restrict__ w, const float* __restrict__ g, float* __restrict__ a, int64_t n,
+                          float lr) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float gi = g[i];
+  const float ai = a[i] + gi * gi;
+  a[i] = ai;
+  w[i] -= lr * gi / (sqrtf(ai) + 1e-7f);
+}
+
+static unsigned blocks_for(int64_t n) { return (unsigned)((n + 255) / 256); }
+
+// rows K and columns N of the gradient of head layer l (c_conv1..3, overlap_output); the gradient
+// buffer holds [K + 1][N] per layer: the kernel in Keras layout, then the bias
+static void head_dims(const ovn_handle* h, int l, int* K, int* N) {
+  if (l < 3) { const ConvSpec& L = h->head[l]; *K = L.kh * L.kw * L.cin; *N = L.cout; }
+  else { *K = h->dense_in; *N = 1; }
+}
+
+static int train_alloc_buffers(ovn_handle* h, TrainState* t) {
+  const int64_t maxp = h->cfg.max_batch_pairs, Wf = h->cfg.leg_output_width;
+  const ConvSpec& L3 = h->head[2];
+  int64_t total = 0, max_part = 0;
+  for (int l = 0; l < 4; ++l) {
+    int K, N;
+    head_dims(h, l, &K, &N);
+    t->off[l] = total;
+    total += (int64_t)(K + 1) * N;
+    if (l < 3 && (int64_t)(K + 1) * N > max_part) max_part = (int64_t)(K + 1) * N;
+  }
+  t->n_param = total;
+  OVN_CUDA(h, cudaMalloc(&t->x4, (size_t)maxp * h->dense_in * sizeof(float)));
+  OVN_CUDA(h, cudaMalloc(&t->dx3, (size_t)maxp * L3.h_in * L3.w_in * L3.cin * sizeof(float)));
+  OVN_CUDA(h, cudaMalloc(&t->corr, (size_t)maxp * Wf * sizeof(float)));
+  OVN_CUDA(h, cudaMalloc(&t->overlap, (size_t)maxp * sizeof(float)));
+  OVN_CUDA(h, cudaMalloc(&t->dz, (size_t)maxp * sizeof(float)));
+  OVN_CUDA(h, cudaMalloc(&t->yaw, (size_t)maxp * sizeof(int32_t)));
+  OVN_CUDA(h, cudaMalloc(&t->w3t, (size_t)L3.kh * L3.kw * L3.cin * L3.cout * sizeof(float)));
+  OVN_CUDA(h, cudaMalloc(&t->part, (size_t)kMaxSplit * max_part * sizeof(float)));
+  OVN_CUDA(h, cudaMalloc(&t->grad, (size_t)total * sizeof(float)));
+  OVN_CUDA(h, cudaMalloc(&t->accum, (size_t)total * sizeof(float)));
+  OVN_CUDA(h, cudaMalloc(&t->loss, 4 * sizeof(float)));
+  OVN_CUDA(h, cudaMemset(t->accum, 0, (size_t)total * sizeof(float)));
+  return OVN_OK;
+}
+
+int train_alloc(ovn_handle* h) {
+  h->train = new TrainState();
+  const int rc = train_alloc_buffers(h, h->train);
+  if (rc != OVN_OK) train_free(h);
+  return rc;
+}
+
+void train_free(ovn_handle* h) {
+  TrainState* t = h->train;
+  if (!t) return;
+  void* bufs[] = {t->x4, t->dx3, t->corr, t->overlap, t->dz, t->yaw, t->w3t, t->part, t->grad, t->accum, t->loss};
+  for (void* b : bufs) if (b) cudaFree(b);
+  delete t;
+  h->train = nullptr;
+}
+
+// [Kc + 1][N] weight + bias gradient = A^T dY summed over Kred rows, split over K in fixed slices
+template <class AOp>
+static int wgrad_gemm(ovn_handle* h, const AOp& a, const float* dY, int Kc, int N, int Kred, float* grad,
+                      cudaStream_t s) {
+  const int M = Kc + 1;
+  const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+  int nsplit = (kSplitBlocks + tiles - 1) / tiles;
+  if (nsplit > kMaxSplit) nsplit = kMaxSplit;
+  int kchunk = (Kred + nsplit - 1) / nsplit;
+  kchunk = (kchunk + BK - 1) / BK * BK;
+  nsplit = (Kred + kchunk - 1) / kchunk;
+  BOperand b{dY, nullptr, nullptr, 0, 0};
+  int rc = launch_gemm(h, a, b, nullptr, h->train->part, M, N, Kred, nsplit, 0, s, kchunk);
+  if (rc != OVN_OK) return rc;
+  k_splitk_reduce<<<blocks_for((int64_t)M * N), 256, 0, s>>>(h->train->part, nsplit, (int64_t)M * N, grad);
+  OVN_LAUNCH_CHECK(h);
+  return OVN_OK;
+}
+
+// Forward of both heads, the losses and the backward of the overlap head for np <= max_batch_pairs pairs
+// (indices already bounds-checked).  Activations kept for the backward: o1 (h->d_o1), x3 = c_conv2 output
+// (h->d_o2), x4 = c_conv3 output (train->x4).  Each buffer is reused for a gradient once it is dead:
+// x4 -> dL/d(pre-act c_conv3), o1 -> dL/do1.  The losses are left in train->loss.
+int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left, const int32_t* right, int np,
+                        const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
+                        cudaStream_t s) {
+  TrainState& t = *h->train;
+  const int Wf = h->cfg.leg_output_width, Cf = kFeatC, sz = h->cfg.conv1size;
+  const int base = kMaxLegLayers;
+  const ConvSpec& L1 = h->head[0];
+  const ConvSpec& L2 = h->head[1];
+  const ConvSpec& L3 = h->head[2];
+  int K[4], N[4];
+  for (int l = 0; l < 4; ++l) head_dims(h, l, &K[l], &N[l]);
+  int rc = overlap_head_fp32(h, d_bank, nullptr, left, right, np, t.x4, t.overlap, s);
+  if (rc == OVN_OK) rc = corr_forward_fp32(h, d_bank, nullptr, left, right, np, t.yaw, t.corr, s);
+  if (rc != OVN_OK) return rc;
+  k_train_loss<<<1, 256, 0, s>>>(t.overlap, t.corr, d_gt_overlap, d_gt_orientation, np, Wf, min_overlap, t.dz,
+                                 t.grad + t.off[3] + K[3], t.loss);
+  OVN_LAUNCH_CHECK(h);
+  // overlap_output (Dense): dWd, and x4 becomes dL/d(pre-activation of c_conv3)
+  k_dense_backward<<<blocks_for(h->dense_in), 256, 0, s>>>(t.x4, h->d_w[base + 3], t.dz, np, h->dense_in,
+                                                           t.grad + t.off[3]);
+  OVN_LAUNCH_CHECK(h);
+  // c_conv3: dW3 = patches(x3)^T dpre3 (+ db3), then dx3 = transposed 3x3 conv of dpre3, masked by x3 > 0
+  {
+    ConvWgradOperand a{h->d_o2, L3.h_in, L3.w_in, L3.cin, L3.kw, L3.sh, L3.sw, L3.h_out, L3.w_out, K[2]};
+    rc = wgrad_gemm(h, a, t.x4, K[2], N[2], np * L3.h_out * L3.w_out, t.grad + t.off[2], s);
+    if (rc != OVN_OK) return rc;
+    k_swap_io<<<blocks_for((int64_t)K[2] * N[2]), 256, 0, s>>>(h->d_w[base + 2], t.w3t, L3.kh * L3.kw, L3.cin,
+                                                               L3.cout);
     OVN_LAUNCH_CHECK(h);
-    {
-      int rc = corr_forward_fp32(h, d_bank, d_query, left, right, np, d_yaw + p0,
-                                 d_corr ? d_corr + (int64_t)p0 * Wf : nullptr, s);
-      if (rc != OVN_OK) return rc;
-    }
+    ConvDgradOperand d{t.x4, L3.h_out, L3.w_out, L3.cout, L3.kw, L3.h_in, L3.w_in};
+    BOperand b{t.w3t, nullptr, nullptr, 0, 0};
+    rc = launch_gemm(h, d, b, nullptr, t.dx3, np * L3.h_in * L3.w_in, L3.cin, L3.kh * L3.kw * L3.cout, 1, 0, s);
+    if (rc != OVN_OK) return rc;
+    const int64_t n3 = (int64_t)np * L3.h_in * L3.w_in * L3.cin;
+    k_relu_grad<<<blocks_for(n3), 256, 0, s>>>(t.dx3, h->d_o2, n3);
+    OVN_LAUNCH_CHECK(h);
+  }
+  // c_conv2: dW2 = patches(o1)^T dpre2 (+ db2); do1 = dpre2 W2^T.  Stride = kernel, so every o1 row belongs to
+  // exactly one output pixel: do1 is stored per output pixel, [p][ho][wo][dh][c], over the dead o1
+  {
+    ConvWgradOperand a{h->d_o1, L2.h_in, L2.w_in, L2.cin, L2.kw, L2.sh, L2.sw, L2.h_out, L2.w_out, K[1]};
+    rc = wgrad_gemm(h, a, t.dx3, K[1], N[1], np * L2.h_out * L2.w_out, t.grad + t.off[1], s);
+    if (rc != OVN_OK) return rc;
+    ConvOperand g{t.dx3, L2.h_out, L2.w_out, L2.cout, 1, 1, 1, L2.h_out, L2.w_out};
+    BOperand w2t{h->d_w[base + 1], h->d_w[base + 1], nullptr, 0, 1};     // W2 read as [(dh, c)][n]
+    rc = launch_gemm(h, g, w2t, nullptr, h->d_o1, np * L2.h_out * L2.w_out, K[1], L2.cout, 1, 0, s);
+    if (rc != OVN_OK) return rc;
+  }
+  // c_conv1 (linear): dW1[dj, c, o] = sum |L[i, c] - R[15 jb + dj, c]| do1[i, jb, o], db1 = sum do1
+  {
+    DeltaWgradOperand a{d_bank, left, right, Wf, Cf, sz, h->o1_w, L2.h_out, K[0]};
+    rc = wgrad_gemm(h, a, h->d_o1, K[0], N[0], np * L1.h_out * L1.w_out, t.grad + t.off[0], s);
+    if (rc != OVN_OK) return rc;
+  }
+  return OVN_OK;
+}
+
+int head_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s) {
+  TrainState& t = *h->train;
+  for (int l = 0; l < 4; ++l) {
+    int K, N;
+    head_dims(h, l, &K, &N);
+    const int64_t nk = (int64_t)K * N;
+    float* g = t.grad + t.off[l];
+    float* a = t.accum + t.off[l];
+    k_adagrad<<<blocks_for(nk), 256, 0, s>>>(h->d_w[kMaxLegLayers + l], g, a, nk, lr);
+    OVN_LAUNCH_CHECK(h);
+    k_adagrad<<<blocks_for(N), 256, 0, s>>>(h->d_b[kMaxLegLayers + l], g + nk, a + nk, N, lr);
+    OVN_LAUNCH_CHECK(h);
   }
   return OVN_OK;
 }

@@ -10,9 +10,11 @@ import numpy as np
 import torch
 
 from . import _cabi
+from . import weights as _weights
 from ._cabi import OvnConfig, OvnError, check, lib
 
 FEAT_C = 128
+HEAD_LAYERS = ('c_conv1', 'c_conv2', 'c_conv3', 'overlap_output')
 
 
 def _ptr(t):
@@ -59,6 +61,7 @@ class Engine:
     cfg.max_batch_scans = int(max_batch_scans)
     cfg.max_batch_pairs = int(max_batch_pairs)
     self.cfg = cfg
+    self.model = model
     self.precision = precision
     self.H, self.W = proj_H, proj_W
     self._h = C.c_void_p(0)
@@ -304,6 +307,52 @@ class Engine:
 
   def bank_release(self, bank=None):
     check(self._h, lib().ovn_bank_release(self._h, _ptr(bank)), 'ovn_bank_release')
+
+  # ---- training of the overlap head with a frozen leg (fp32 handles) -------------------------------
+  def head_gradients(self, bank, left_idx, right_idx, gt_overlap, gt_orientation, min_overlap_for_angle=0.7):
+    """ovn_head_gradients: forward of both heads for LEFT = bank[left_idx], RIGHT = bank[right_idx], the
+    losses of training.py and the backward of the overlap head.  Synchronous; returns the losses
+    (total, overlap, orientation) and keeps the batch gradients in the handle."""
+    n = left_idx.numel()
+    dev = self.device
+    li = left_idx.to(device=dev, dtype=torch.int32).contiguous()
+    ri = right_idx.to(device=dev, dtype=torch.int32).contiguous()
+    gov = torch.as_tensor(gt_overlap).to(device=dev, dtype=torch.float32).contiguous()
+    gor = torch.as_tensor(gt_orientation).to(device=dev, dtype=torch.int32).contiguous()
+    assert ri.numel() == n and gov.numel() == n and gor.numel() == n
+    loss = np.zeros(3, np.float32)
+    check(self._h, lib().ovn_head_gradients(self._h, _ptr(bank), int(bank.shape[0]), _ptr(li), _ptr(ri), n, _ptr(gov),
+                                           _ptr(gor), float(min_overlap_for_angle), loss.ctypes.data_as(C.c_void_p),
+                                           self._stream()), 'ovn_head_gradients')
+    return tuple(float(v) for v in loss)
+
+  def adagrad_step(self, lr):
+    """ovn_head_adagrad_step: Adagrad update of the head weights from the last gradients."""
+    check(self._h, lib().ovn_head_adagrad_step(self._h, float(lr), self._stream()), 'ovn_head_adagrad_step')
+
+  def _layer_shapes(self):
+    return _weights.layer_shapes(self.C, self.model, self.H, self.W)
+
+  def _read_layers(self, fn, names, what):
+    shapes = self._layer_shapes()
+    out = {}
+    for name in names:
+      ks, bs = shapes[name]
+      k = np.empty(ks, np.float32)
+      b = np.empty(bs, np.float32)
+      check(self._h, fn(self._h, name.encode(), k.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p)),
+            '%s(%s)' % (what, name))
+      out[name] = (k, b)
+    return out
+
+  def get_weights(self, names=None):
+    """Current weights {layer name: (kernel, bias)} in Keras layouts (every layer when names is None)."""
+    names = list(self._layer_shapes()) if names is None else list(names)
+    return self._read_layers(lib().ovn_get_weights, names, 'ovn_get_weights')
+
+  def get_gradients(self, names=HEAD_LAYERS):
+    """Gradients of the last head_gradients call {layer name: (kernel, bias)}, head layers only."""
+    return self._read_layers(lib().ovn_get_gradients, names, 'ovn_get_gradients')
 
   # ---- host-buffer entry points (synchronous) ------------------------------------------------
   def encode_clouds_host(self, clouds):

@@ -1,0 +1,219 @@
+"""The body of the reference's ``src/two_heads/training.py`` on the GPU path, for the
+``360OutputkLegsFixed`` configuration (generateNet.py:222-324): the leg is frozen and the four layers of
+the overlap head (c_conv1..3, overlap_output) are trained with Adagrad on the losses of training.py:71-92.
+
+Every distinct scan is encoded once by the frozen leg into a feature bank that stays on the GPU; a training
+step is then the heads' forward plus the overlap head's backward (``ovn_head_gradients``) and an Adagrad
+update (``ovn_head_adagrad_step``).  The orientation loss has no gradient with a frozen leg, but it is
+computed and logged as part of the total loss like training.py does.
+
+  python -m overlapnet_b200.training config.yml
+
+Not supported (an Exception says so): a trainable leg (legsType 360OutputkLegs), ``rotate_training_data``
+(it would re-encode the rolled RIGHT image for every pair of every epoch) and TensorBoard output.
+"""
+import logging
+import os
+import sys
+
+import numpy as np
+import torch
+
+from . import evaluate
+from . import weights as _weights
+from .config import load_config
+
+logger = logging.getLogger('overlapnet_b200.training')
+
+OVERLAP_THRESHOLDS = (0.3, 0.4, 0.5, 0.6, 0.7, 0.8, 0.9)          # training.py:398
+
+
+def learning_rate(epoch, initial_lr=1e-3, alpha=0.99):
+  """learning_rate_schedule (training.py:47-57): epoch 0 uses 0.1 lr, then lr alpha^(epoch-1)."""
+  if epoch < 1:
+    return initial_lr * 0.1
+  return initial_lr * np.power(alpha, epoch - 1.0)
+
+
+def check_config(config):
+  """Refuse the configurations this driver cannot train."""
+  model = config['model']
+  legs = model.get('legsType')
+  if legs == '360OutputkLegs':
+    raise Exception('legsType 360OutputkLegs trains the leg, which needs the backward of the leg '
+                    'convolutions and of |l - r|; only 360OutputkLegsFixed (frozen leg) is supported')
+  if legs != '360OutputkLegsFixed':
+    raise Exception('legsType %r is not supported for training; use 360OutputkLegsFixed' % (legs,))
+  if config.get('rotate_training_data', 0) != 0:
+    raise Exception('rotate_training_data != 0 is not supported: with a frozen leg it would re-encode the '
+                    'rolled RIGHT image of every pair in every epoch')
+  if config.get('tensorboard', False):
+    raise Exception('TensorBoard output is not supported')
+
+
+def npz_files(config):
+  """training.py:124-134: per-sequence train / validation sets, or two single files."""
+  root = config.get('data_root_folder', '')
+  if 'training_seqs' in config:
+    seqs = str(config['training_seqs']).split()
+    return ([os.path.join(root, s, 'ground_truth/train_set.npz') for s in seqs],
+            [os.path.join(root, s, 'ground_truth/validation_set.npz') for s in seqs])
+  return [config['traindata_npzfile']], [config['validationdata_npzfile']]
+
+
+def orientation_rms(overlap, argmax, gt_orientation, width):
+  """training.py:398-415: yaw RMS over the pairs whose predicted overlap exceeds each threshold
+  (NaN when no pair does)."""
+  out = {}
+  for thr in OVERLAP_THRESHOLDS:
+    sel = overlap > thr
+    a = np.abs(argmax[sel] - gt_orientation[sel])
+    d = np.minimum(a, width - a)
+    out[thr] = float(np.sqrt(np.mean(d * d))) if d.size else float('nan')
+  return out
+
+
+def _encode_bank(infer, keys):
+  """Feature volumes of the distinct (dir, scan) keys with the frozen leg, through Infer's cue loader
+  (one sequence directory at a time).  Returns the bank [n, Wf, 128] and {key: row}."""
+  rows, parts, n = {}, [], 0
+  for d in sorted({k[0] for k in keys}):
+    names = sorted(k[1] for k in keys if k[0] == d)
+    infer.seq = d
+    parts.append(infer._create_feature_volumes_device(names))
+    for i, name in enumerate(names):
+      rows[(d, name)] = n + i
+    n += len(names)
+  return torch.cat(parts).contiguous(), rows
+
+
+def save_weights(path, weights):
+  """The full model (leg + head) in the .npz container, written through a file object so that the
+  name stays exactly ``path`` (np.savez appends .npz to a path)."""
+  with open(path, 'wb') as f:
+    _weights.save_npz(f, weights)
+
+
+def train(config, device=None):
+  """Run the training of training.py for a loaded YAML dict.  Returns a dict with the per-epoch
+  losses, the batch losses, the validation statistics and the weight file name."""
+  from .infer import Infer
+  check_config(config)
+  model = config['model']
+  root = config.get('data_root_folder', '')
+  imgpath = config.get('imgpath', root)
+  out_dir = os.path.join(config['experiments_path'], config['testname'])
+  os.makedirs(out_dir, exist_ok=True)
+  handler = logging.FileHandler(os.path.join(out_dir, 'training.log'), mode='w')      # training.py:204-208
+  handler.setFormatter(logging.Formatter(fmt='%(asctime)s %(message)s', datefmt='%H:%M:%S'))
+  logger.addHandler(handler)
+  if logger.level == logging.NOTSET or logger.level > logging.INFO:
+    logger.setLevel(logging.INFO)
+  try:
+    return _train(config, model, imgpath, out_dir, device, Infer)
+  finally:
+    logger.removeHandler(handler)
+    handler.close()
+
+
+def _train(config, model, imgpath, out_dir, device, Infer):
+  weights_filename = os.path.join(out_dir, model['modelType'] + '_' + config['testname'] + '.weight')
+  initial_lr = float(config['learning_rate'])
+  lr_alpha = float(config.get('lr_alpha', 0.99))
+  batch_size = int(config['batch_size'])
+  no_batches_in_epoch = int(config['no_batches_in_epoch'])
+  no_epochs = int(config['no_epochs'])
+  no_test_pairs = int(config['no_test_pairs'])
+  min_overlap_for_angle = float(config.get('min_overlap_for_angle', 0.7))
+
+  train_files, val_files = npz_files(config)
+  logger.info('load training data ...')
+  t_f1, t_f2, t_d1, t_d2, t_ov, t_or = evaluate.load_overlap_npz(train_files)
+  n = min(len(t_ov), batch_size * no_batches_in_epoch)                                # training.py:275-286
+  t_f1, t_f2, t_d1, t_d2, t_ov, t_or = t_f1[:n], t_f2[:n], t_d1[:n], t_d2[:n], t_ov[:n], t_or[:n]
+  logger.info('load validation data ...')
+  v_f1, v_f2, v_d1, v_d2, v_ov, v_or = evaluate.load_overlap_npz(val_files, shuffle=False)
+  n_val = min(len(v_ov), no_test_pairs)                                                 # training.py:291-300
+  v_f1, v_f2, v_d1, v_d2, v_ov, v_or = v_f1[:n_val], v_f2[:n_val], v_d1[:n_val], v_d2[:n_val], v_ov[:n_val], v_or[:n_val]
+
+  cfg = dict(config)
+  for key, default in (('use_depth', True), ('use_normals', True), ('use_class_probabilities', False),
+                       ('use_class_probabilities_pca', False), ('use_intensity', False)):
+    cfg.setdefault(key, default)                                                        # training.py:137-160
+  cfg['data_root_folder'] = imgpath
+  cfg['infer_seqs'] = ''
+  cfg['model'] = dict(model)
+  cfg['model']['inputShape'] = list(model['inputShape'])
+  infer = Infer(cfg, precision='fp32', device=device, max_batch_pairs=batch_size)
+  eng = infer._engine
+  width = infer.network_output_size
+  if len(cfg['pretrained_weightsfilename']) > 0:
+    logger.info('Load old weights from %s', cfg['pretrained_weightsfilename'])
+
+  keys = set(zip(t_d1, t_f1)) | set(zip(t_d2, t_f2)) | set(zip(v_d1, v_f1)) | set(zip(v_d2, v_f2))
+  logger.info('Encoding %d scans with the frozen leg ...', len(keys))
+  bank, rows = _encode_bank(infer, keys)
+  dev = eng.device
+  t_left = torch.tensor([rows[k] for k in zip(t_d1, t_f1)], dtype=torch.int32, device=dev)
+  t_right = torch.tensor([rows[k] for k in zip(t_d2, t_f2)], dtype=torch.int32, device=dev)
+  t_ov_d = torch.as_tensor(np.asarray(t_ov, np.float32), device=dev)
+  t_or_d = torch.as_tensor(np.asarray(t_or).astype(np.int32), device=dev)
+  v_left = torch.tensor([rows[k] for k in zip(v_d1, v_f1)], dtype=torch.int32, device=dev)
+  v_right = torch.tensor([rows[k] for k in zip(v_d2, v_f2)], dtype=torch.int32, device=dev)
+
+  n_batches = int(np.ceil(n / float(batch_size)))                  # len() of the Keras Sequence
+  logger.info('Training loop, saving weights to %s', weights_filename)
+  logger.info('  batch size is           : %d', batch_size)
+  logger.info('  number of training pairs: %d', n)
+  logger.info('  number of test pairs    : %d', n_val)
+  logger.info('  NO rotation of training data')
+  history = {'epoch_loss': [], 'batch_losses': [], 'validation': [], 'weights_filename': weights_filename}
+  for epoch in range(no_epochs):
+    lr = learning_rate(epoch, initial_lr, lr_alpha)
+    losses, sizes = [], []
+    for b in np.random.permutation(n_batches):                     # Keras reshuffles a Sequence's batches
+      s0, s1 = b * batch_size, min(n, (b + 1) * batch_size)
+      loss = eng.head_gradients(bank, t_left[s0:s1], t_right[s0:s1], t_ov_d[s0:s1], t_or_d[s0:s1],
+                                min_overlap_for_angle)
+      eng.adagrad_step(lr)
+      losses.append(loss)
+      sizes.append(s1 - s0)
+      logger.info('  epoch %d batch %d: loss %.6f (overlap %.6f, orientation %.6f)', epoch + 1, len(losses),
+                  loss[0], loss[1], loss[2])
+    epoch_loss = float(np.average([l[0] for l in losses], weights=sizes))
+    history['epoch_loss'].append(epoch_loss)
+    history['batch_losses'].append([l[0] for l in losses])
+
+    logger.info('                  saving model weights ...')                          # training.py:346-349
+    save_weights(weights_filename, eng.get_weights())
+
+    logger.info('  Evaluation on test data ...')                                       # training.py:352-415
+    ov, yaw, _ = eng.heads(bank, v_left, v_right)
+    eng.check()
+    overlap = ov.cpu().numpy().astype(np.float64)
+    argmax = width // 2 - yaw.cpu().numpy().astype(np.int64)
+    diffs = np.abs(overlap - v_ov)
+    stats = {'mean': float(np.mean(diffs)), 'max': float(np.max(diffs)),
+             'rms': float(np.sqrt(np.mean(diffs * diffs))), 'learning_rate': float(lr),
+             'orientation_rms': orientation_rms(overlap, argmax, np.asarray(v_or, np.float64), width)}
+    history['validation'].append(stats)
+    logger.info('  Evaluation on test data results: ')
+    logger.info('           Evaluation: mean overlap difference:   %f', stats['mean'])
+    logger.info('           Evaluation: max  overlap difference:   %f', stats['max'])
+    logger.info('           Evaluation: RMS  overlap error        : %f', stats['rms'])
+    for thr, rms in stats['orientation_rms'].items():
+      logger.info('           Evaluation: orientation RMS (overlap > %.1f): %f', thr, rms)
+    logger.info('iteration %d, batch/epoch loss: %.9f  /  %.9f', epoch + 1, losses[-1][0], epoch_loss)
+  return history
+
+
+def main(argv=None):
+  argv = sys.argv[1:] if argv is None else argv
+  logging.basicConfig(format='%(message)s', level=logging.INFO)
+  configfilename = argv[0] if argv else 'network.yml'                                  # training.py:102-104
+  logger.info('Using configuration file %s.', configfilename)
+  train(load_config(configfilename))
+
+
+if __name__ == '__main__':
+  main()
