@@ -36,6 +36,11 @@ __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, long l
   return true;
 }
 
+// barrier `id` (1..15) among the `count` threads (a multiple of 32) that reach it, e.g. one warpgroup
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" :: "r"(id), "r"(count) : "memory");
+}
+
 // ---- bulk async copy global -> shared, completes on an mbarrier (bytes and addresses multiples of 16)
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"

@@ -3,17 +3,19 @@
 // Replaces: DeltaLayer + c_conv1 (generateNet.py:15-61,96-100)      -> k_delta_conv1_wgmma
 //           c_conv2 (+ReLU) (generateNet.py:102-105)                -> k_conv2_wgmma
 //           c_conv3 (+ReLU), Flatten + Dense(1, sigmoid) (:107-114) -> k_conv3_wgmma + k_dense_finalize
-//           NormalizedCorrelation2D + argmax (:117-143, infer.py)   -> k_corr_mma + k_corr_finalize
+//           NormalizedCorrelation2D + argmax (:117-143, infer.py)   -> k_corr_wgmma + k_corr_finalize
 //           leg Conv2D stack (generateNet.py:149-230)               -> layer 1: k_leg_layer1_small (1-2 scans) /
 //                                                                      k_leg_layer1_direct (batches), SIMT fp32;
-//                                                                      layers 2..: k_leg_mma
+//                                                                      layers 2..: k_leg_mma (+ k_leg_splitk_reduce,
+//                                                                      1-2 scans)
 //
 // Every GEMM runs on tensor cores (fp16 operands, fp32 accumulators) and reads packed operand layouts (8
 // consecutive K values per 16-byte chunk).  The delta head is three persistent, warp-specialised wgmma kernels
 // fed by bulk copies through mbarrier rings: k_delta_conv1_wgmma (83 % of the FLOPs of a pair) synthesises its
 // A operand |l - r| in registers, so the 66 MB delta tensor of a pair (the reference's DeltaLayer output) is
 // never materialised; k_conv2_wgmma and k_conv3_wgmma take both operands from shared memory.  The correlation
-// head and the leg are warp-level mma.sync m16n8k16 kernels whose fragments are loaded straight from global.
+// head k_corr_wgmma is built the same way.  The leg is a warp-level mma.sync m16n8k16 kernel whose fragments are
+// loaded straight from global; a single scan splits its K over more CTAs.
 // Operands that must be fp32-grade are split into hi + lo fp16 halves (x = hi + lo exactly to 2^-22).
 #include "common.cuh"
 #include "hopper.cuh"
@@ -41,14 +43,15 @@ struct TcState {
   // tensor-core leg (layers 2..): packed weights per layer, ping-pong activation planes
   __half* wres[kMaxLegLayers] = {};      // [cout/64][kh*kw*3 slabs (tap, term)][C_in/8][64][8]; term 0, 1 = hi, 2 = lo
   __half* actp[2] = {nullptr, nullptr};
+  float* leg_part = nullptr;    // K-slice sums of the single-scan leg: [n_split][rows][w_out][cout] fp32
   __half* l16 = nullptr;        // [max_pairs][360][128]
   __half* r16 = nullptr;        // [max_pairs][360][128] (pair mode) / [1][360][128] (query mode)
   __half* o1 = nullptr;         // [rows_pad/128][15 di][128][64]: SWIZZLE_128B A tiles of c_conv2 (o1_chunk_offset)
   __half* x3 = nullptr;         // [16 planes][rows_pad][8], row = pair*576 + jb*24 + ib
   float* partial = nullptr;     // [rows_pad][2]
-  __half* lc = nullptr;         // correlation operands: [max_pairs][3 tiles][2 k-halves][hi,lo][8][128][8]
-  __half* rc = nullptr;         // [max_pairs or 1][2 n-halves][hi,lo][16][192][8]
-  float* corr_part = nullptr;   // [max_pairs][C6_IBLK row blocks][360]
+  __half* lc = nullptr;         // correlation operands: [max_pairs][6 tiles][hi,lo][16][64][8]
+  __half* rc = nullptr;         // [max_pairs or 1][3 thirds][hi,lo][16][128][8]
+  float* corr_part = nullptr;   // [max_pairs][6 LEFT tiles][3 RIGHT thirds][360]
   // resident bank (ovn_bank_prepare): operand copies of the LEFT volumes, indexed by bank row
   const float* pb_key = nullptr;
   int64_t pb_cap = 0, pb_rows = 0;      // capacity / rows [0, pb_rows) prepared
@@ -135,62 +138,31 @@ struct LegArgs {
   int64_t M;                  // output pixels per run
   __half* out_planes; int64_t out_pitch; int out_run_planes;   // EPI 4
   float* out_f32;                                               // EPI 3
+  int n_split; float* part;                                     // K slices; EPI 5: [n_split][rows][M][n_valid] fp32
 };
 
-constexpr int C6_STAGE_BYTES = 32768;            // [hi,lo][8 planes][128 rows][8] fp16
-constexpr int C6_R_BYTES = 98304;                // [hi,lo][16 planes][192 rows][8] fp16
-constexpr int C6_VOL_L_BYTES = 6 * C6_STAGE_BYTES;
-constexpr int C6_VOL_R_BYTES = 2 * C6_R_BYTES;
+// Correlation operands (k_corr_wgmma): a volume is cut into row tiles of TR rows (64 for LEFT, 128 for RIGHT),
+// each tile one contiguous [hi, lo][16 planes = c / 8][TR rows][8] block of fp16, zero rows past 360: the
+// no-swizzle K-major layout a wgmma descriptor reads (LBO = plane pitch, SBO = 128 B).
+constexpr int C6_LROWS = 64, C6_RROWS = 128;
+constexpr int C6_LT = 6, C6_RT = 3;                    // LEFT tiles, RIGHT thirds (6 x 64 = 3 x 128 = 384 >= 360)
+constexpr int C6_L_BYTES = 2 * 16 * C6_LROWS * 16;     // 32 KB
+constexpr int C6_R_BYTES = 2 * 16 * C6_RROWS * 16;     // 64 KB
+constexpr int C6_VOL_L_BYTES = C6_LT * C6_L_BYTES;
+constexpr int C6_VOL_R_BYTES = C6_RT * C6_R_BYTES;
 
-
-// fp32 volumes -> hi/lo fp16 split in the operand layout of k_corr_mma (zero rows past 360)
+// fp32 volumes -> hi/lo fp16 split in the tiled operand layout above; one thread per (volume, plane, row)
+template <int TR, int NT>
 __global__ void __launch_bounds__(256)
-k_pack_corr_L(const float* __restrict__ bank, const int32_t* __restrict__ idx, int n, __half* __restrict__ out) {
-  // one thread per (pair, tile, khalf, plane j, row): 8 channels
+k_pack_corr(const float* __restrict__ bank, const int32_t* __restrict__ idx, int n, __half* __restrict__ out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t per = 3 * 2 * 8 * 128;
+  const int64_t per = 16 * NT * TR;
   if (i >= (int64_t)n * per) return;
   const int p = (int)(i / per);
   int r = (int)(i % per);
-  const int row = r % 128; r /= 128;
-  const int j = r % 8; r /= 8;
-  const int kh = r % 2; r /= 2;
-  const int t = r;
-  const int vrow = t * 128 + row;
-  const int c = kh * 64 + j * 8;
-  float v[8];
-  if (vrow < WF) {
-    const int64_t src = (idx ? idx[p] : p);
-    const float4 a = __ldg(reinterpret_cast<const float4*>(bank + (src * WF + vrow) * CF + c));
-    const float4 b = __ldg(reinterpret_cast<const float4*>(bank + (src * WF + vrow) * CF + c + 4));
-    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-  } else {
-#pragma unroll
-    for (int e = 0; e < 8; ++e) v[e] = 0.f;
-  }
-  __half hi[8], lo[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    hi[e] = __float2half_rn(v[e]);
-    lo[e] = __float2half_rn(v[e] - __half2float(hi[e]));
-  }
-  __half* base = out + (size_t)p * (C6_VOL_L_BYTES / 2) + (size_t)(t * 2 + kh) * (C6_STAGE_BYTES / 2);
-  *reinterpret_cast<uint4*>(base + ((size_t)j * 128 + row) * 8) = *reinterpret_cast<const uint4*>(hi);
-  *reinterpret_cast<uint4*>(base + (C6_STAGE_BYTES / 4) + ((size_t)j * 128 + row) * 8) = *reinterpret_cast<const uint4*>(lo);
-}
-
-__global__ void __launch_bounds__(256)
-k_pack_corr_R(const float* __restrict__ bank, const int32_t* __restrict__ idx, int n, __half* __restrict__ out) {
-  // one thread per (pair, nhalf, plane, row): 8 channels
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t per = 2 * 16 * 192;
-  if (i >= (int64_t)n * per) return;
-  const int p = (int)(i / per);
-  int r = (int)(i % per);
-  const int row = r % 192; r /= 192;
-  const int pl = r % 16; r /= 16;
-  const int h = r;
-  const int vrow = h * 192 + row;
+  const int vrow = r % (NT * TR); r /= NT * TR;
+  const int pl = r;
+  const int tile = vrow / TR, row = vrow % TR;
   float v[8];
   if (vrow < WF) {
     const int64_t src = (idx ? idx[p] : p);
@@ -207,9 +179,9 @@ k_pack_corr_R(const float* __restrict__ bank, const int32_t* __restrict__ idx, i
     hi[e] = __float2half_rn(v[e]);
     lo[e] = __float2half_rn(v[e] - __half2float(hi[e]));
   }
-  __half* base = out + (size_t)p * (C6_VOL_R_BYTES / 2) + (size_t)h * (C6_R_BYTES / 2);
-  *reinterpret_cast<uint4*>(base + ((size_t)pl * 192 + row) * 8) = *reinterpret_cast<const uint4*>(hi);
-  *reinterpret_cast<uint4*>(base + (C6_R_BYTES / 4) + ((size_t)pl * 192 + row) * 8) = *reinterpret_cast<const uint4*>(lo);
+  __half* base = out + ((size_t)p * NT + tile) * (2 * 16 * TR * 8);
+  *reinterpret_cast<uint4*>(base + ((size_t)pl * TR + row) * 8) = *reinterpret_cast<const uint4*>(hi);
+  *reinterpret_cast<uint4*>(base + ((size_t)(16 + pl) * TR + row) * 8) = *reinterpret_cast<const uint4*>(lo);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -718,79 +690,153 @@ done:
 }
 
 // ------------------------------------------------------------------------------------------------
-// k_corr_mma -- correlation (yaw) head.  G = L R^T (360 x 360, K = 128) from hi / lo fp16 operands
+// k_corr_wgmma -- correlation (yaw) head.  G = L R^T (360 x 360, K = 128) from hi / lo fp16 operands
 // (G = Lhi Rhi + Llo Rhi + Lhi Rlo: fp32-grade, fp16 alone does not keep the argmax of a flat curve),
-// corr[k] = sum_j G[(k + j + 180) mod 360, j].  A block owns 64 rows of G of one pair: the warps write
-// their 16 x 360 strips to shared memory, then every bin sums the block's 64 diagonal terms in a fixed
-// order into corr_part[pair][row block][k] (no atomics: results are bit-reproducible).
-// grid = (n_pairs, C6_IBLK)
+// corr[k] = sum_j G[(k + j + 180) mod 360, j]: row i meets column j in bin k = (i - j - 180) mod 360.
+// A work unit is one 64-row LEFT tile a of a pair against one 128-row RIGHT third q (m64 x n128, K = 128).
+// Persistent and warp-specialised: CTA b serves the third q = b % 3 and walks a contiguous range of the
+// n_pairs * 6 (pair, a) units; the CTAs 3c, 3c + 1, 3c + 2 walk the same range at the same pace, so a LEFT
+// tile is read from HBM once and served to the other two thirds from L2.  Warp 8 is the producer (one lane):
+// the RIGHT third (64 KB, once per CTA in query mode, once per pair in pair mode) and the LEFT tiles (32 KB,
+// hi + lo) through a 3-deep ring.  Consumer warpgroups 0 and 1 take alternate units: 24 wgmma.m64n128k16
+// (K16 steps in order, each as Lhi Rhi, Llo Rhi, Lhi Rlo), then the 64 x 128 block of G goes to the
+// warpgroup's own shared-memory buffer and each of its 191 diagonals is summed in a fixed order into
+// corr_part[pair][a][q][k] (the 169 bins the block does not reach are 0), while the other warpgroup
+// multiplies.  k_corr_finalize adds the 18 partial curves of a pair in a fixed order: no atomics, results
+// are bit-reproducible, and query mode gives the bits of pair mode.
 // ------------------------------------------------------------------------------------------------
-constexpr int C6_IBLK = 6;                          // 6 x 64 = 384 >= 360 rows (the packed L is zero past 360)
-constexpr int C6_GPITCH = WF + 1;
-constexpr size_t C6_SMEM = (size_t)MMA_ROWS * C6_GPITCH * sizeof(float);
+constexpr int C6_PARTS = C6_LT * C6_RT;                // partial curves per pair
+constexpr int C6_WG = 2;
+constexpr int C6_THREADS = C6_WG * 128 + 32;
+constexpr int C6_RING = 3;
+constexpr int C6_GPITCH = 132;                         // fp32 row pitch of a staged G block
 
-__global__ void __launch_bounds__(MMA_THREADS)
-k_corr_mma(const __half* __restrict__ Lc, const int32_t* __restrict__ l_idx, const __half* __restrict__ Rc, int r_per_pair,
-           float* __restrict__ corr_part) {
-  extern __shared__ float Gs[];                      // [64][C6_GPITCH]
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const int p = blockIdx.x, i0 = blockIdx.y * MMA_ROWS;
-  const __half* lp = Lc + (size_t)(l_idx ? l_idx[p] : p) * (C6_VOL_L_BYTES / 2);
-  const __half* rp = Rc + (r_per_pair ? (size_t)p * (C6_VOL_R_BYTES / 2) : 0);
-  // L: [row / 128][c / 64][hi, lo][(c / 8) % 8][row % 128][8];  R: [row / 192][hi, lo][c / 8][row % 192][8]
-  const int ia = i0 + warp * 16 + g, ib = ia + 8;
-  const __half* La = lp + (size_t)((ia >> 7) * 2) * (C6_STAGE_BYTES / 2) + (ia & 127) * 8 + 2 * t;
-  const __half* Lb = lp + (size_t)((ib >> 7) * 2) * (C6_STAGE_BYTES / 2) + (ib & 127) * 8 + 2 * t;
-  for (int j0 = 0; j0 < 2 * 192; j0 += 64) {
-    float acc[8][4] = {};
-#pragma unroll 1
-    for (int c16 = 0; c16 < 8; ++c16) {
-      const size_t lo_k = (size_t)(c16 >> 2) * (C6_STAGE_BYTES / 2) + (size_t)((c16 & 3) * 2) * 128 * 8;
-      uint32_t ah[4], al[4];
-      ah[0] = ld_h2(La + lo_k); ah[1] = ld_h2(Lb + lo_k);
-      ah[2] = ld_h2(La + lo_k + 128 * 8); ah[3] = ld_h2(Lb + lo_k + 128 * 8);
-      al[0] = ld_h2(La + lo_k + C6_STAGE_BYTES / 4); al[1] = ld_h2(Lb + lo_k + C6_STAGE_BYTES / 4);
-      al[2] = ld_h2(La + lo_k + C6_STAGE_BYTES / 4 + 128 * 8); al[3] = ld_h2(Lb + lo_k + C6_STAGE_BYTES / 4 + 128 * 8);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int n = j0 + j * 8 + g;
-        const __half* B = rp + (size_t)(n / 192) * (C6_R_BYTES / 2) + ((size_t)(2 * c16) * 192 + n % 192) * 8 + 2 * t;
-        const uint32_t bh0 = ld_h2(B), bh1 = ld_h2(B + 192 * 8);
-        const uint32_t bl0 = ld_h2(B + C6_R_BYTES / 4), bl1 = ld_h2(B + C6_R_BYTES / 4 + 192 * 8);
-        mma16816(acc[j], ah[0], ah[1], ah[2], ah[3], bh0, bh1);
-        mma16816(acc[j], al[0], al[1], al[2], al[3], bh0, bh1);
-        mma16816(acc[j], ah[0], ah[1], ah[2], ah[3], bl0, bl1);
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int n = j0 + j * 8 + 2 * t;
-      float* ra = Gs + (warp * 16 + g) * C6_GPITCH;
-      float* rb = ra + 8 * C6_GPITCH;
-      if (n < WF) { ra[n] = acc[j][0]; rb[n] = acc[j][2]; }
-      if (n + 1 < WF) { ra[n + 1] = acc[j][1]; rb[n + 1] = acc[j][3]; }
-    }
+struct C6Smem {
+  __half R[C6_R_BYTES / 2];
+  __half L[C6_RING][C6_L_BYTES / 2];
+  float G[C6_WG][C6_LROWS * C6_GPITCH];
+  uint64_t full[C6_RING], empty[C6_RING], r_full, r_empty;
+};
+static_assert(sizeof(C6Smem) <= 232448, "k_corr_wgmma shared memory");
+static_assert(offsetof(C6Smem, L) % 16 == 0, "bulk-copy alignment");
+
+__global__ void __launch_bounds__(C6_THREADS, 1)
+k_corr_wgmma(const __half* __restrict__ Lc, const int32_t* __restrict__ l_idx, const __half* __restrict__ Rc,
+             int r_per_pair, int n_pairs, float* __restrict__ corr_part, int* __restrict__ err) {
+  extern __shared__ __align__(128) uint8_t smem_raw[];
+  C6Smem& S = *reinterpret_cast<C6Smem*>(smem_raw);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int q = blockIdx.x % C6_RT, c = blockIdx.x / C6_RT, nc = gridDim.x / C6_RT;
+  const int64_t n_units = (int64_t)n_pairs * C6_LT;
+  const int u_begin = (int)(n_units * c / nc), u_end = (int)(n_units * (c + 1) / nc);
+  if (tid == 0) {
+    for (int s = 0; s < C6_RING; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], 4); }  // one warpgroup per unit
+    mbar_init(&S.r_full, 1); mbar_init(&S.r_empty, C6_WG * 4);
+    mbar_fence_init();
   }
   __syncthreads();
-  for (int k = threadIdx.x; k < WF; k += MMA_THREADS) {
-    float s = 0.f;
-    // row i pairs with column j = (i - k - 180) mod 360
-    int jj = (i0 - k - WF / 2) % WF;
-    if (jj < 0) jj += WF;
-    for (int ii = 0; ii < MMA_ROWS && i0 + ii < WF; ++ii) {
-      s += Gs[ii * C6_GPITCH + jj];
-      if (++jj == WF) jj = 0;
+
+  if (warp == C6_WG * 4) {
+    // ===================== producer ==========================================================
+    if (lane == 0) {
+      uint32_t ri = 0;
+      int key = -1;                           // pair whose RIGHT third is loaded (0 in query mode)
+      for (int u = u_begin, ui = 0; u < u_end; ++u, ++ui) {
+        const int p = u / C6_LT, a = u - p * C6_LT;
+        if ((r_per_pair ? p : 0) != key) {
+          key = r_per_pair ? p : 0;
+          PIPE_WAIT(&S.r_empty, (ri & 1) ^ 1, 131);
+          mbar_arrive_expect_tx(&S.r_full, C6_R_BYTES);
+          bulk_g2s(S.R, Rc + ((size_t)key * C6_RT + q) * (C6_R_BYTES / 2), C6_R_BYTES, &S.r_full);
+          ++ri;
+        }
+        const uint32_t s = ui % C6_RING;
+        PIPE_WAIT(&S.empty[s], ((ui / C6_RING) & 1) ^ 1, 132);
+        mbar_arrive_expect_tx(&S.full[s], C6_L_BYTES);
+        bulk_g2s(S.L[s], Lc + ((size_t)(l_idx ? l_idx[p] : p) * C6_LT + a) * (C6_L_BYTES / 2), C6_L_BYTES, &S.full[s]);
+      }
     }
-    corr_part[((size_t)p * C6_IBLK + blockIdx.y) * WF + k] = s;
+  } else {
+    // ===================== consumers ==========================================================
+    // A time-out raises the error and skips the later waits, but the warp keeps to the named barriers of its
+    // warpgroup (the outputs of the call are poisoned by the flag).
+    const int wg = warp >> 2, wi = warp & 3, g = lane >> 2, t = lane & 3, tw = tid & 127;
+    float* Gw = S.G[wg];
+    const uint32_t r_base = smem_u32(S.R);
+    uint32_t ri = 0;
+    int key = -1;
+    bool failed = false;
+    for (int u = u_begin, ui = 0; u < u_end; ++u, ++ui) {
+      const int p = u / C6_LT, a = u - p * C6_LT;
+      if ((r_per_pair ? p : 0) != key) {      // both warpgroups follow every change of the RIGHT third
+        if (key >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&S.r_empty); }
+        key = r_per_pair ? p : 0;
+        INFLIGHT_WAIT(&S.r_full, ri & 1, 231);
+        ++ri;
+      }
+      if ((ui & 1) != wg) continue;
+      const uint32_t s = ui % C6_RING;
+      INFLIGHT_WAIT(&S.full[s], (ui / C6_RING) & 1, 232);
+      const uint32_t l_base = smem_u32(S.L[s]);
+      float acc[64];
+#pragma unroll
+      for (int e = 0; e < 64; ++e) acc[e] = 0.f;
+      wgmma_fence();
+#pragma unroll
+      for (int c16 = 0; c16 < 8; ++c16) {
+        // K16 step = planes 2 c16, 2 c16 + 1: LBO = plane pitch, SBO = 8 rows x 16 B
+        const uint64_t ah = desc_kmajor(l_base + c16 * 2 * C6_LROWS * 16, C6_LROWS * 16, 128, kNoSwizzle);
+        const uint64_t al = desc_kmajor(l_base + C6_L_BYTES / 2 + c16 * 2 * C6_LROWS * 16, C6_LROWS * 16, 128, kNoSwizzle);
+        const uint64_t bh = desc_kmajor(r_base + c16 * 2 * C6_RROWS * 16, C6_RROWS * 16, 128, kNoSwizzle);
+        const uint64_t bl = desc_kmajor(r_base + C6_R_BYTES / 2 + c16 * 2 * C6_RROWS * 16, C6_RROWS * 16, 128, kNoSwizzle);
+        wgmma_m64n128k16_ss(acc, ah, bh);
+        wgmma_m64n128k16_ss(acc, al, bh);
+        wgmma_m64n128k16_ss(acc, ah, bl);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&S.empty[s]);
+      named_bar_sync(1 + wg, 128);            // this warpgroup's previous diagonal sums have read Gw
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        float* r0 = Gw + (wi * 16 + g) * C6_GPITCH + j * 8 + 2 * t;
+        *reinterpret_cast<float2*>(r0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(r0 + 8 * C6_GPITCH) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      named_bar_sync(1 + wg, 128);
+      const int i_lim = min(C6_LROWS, WF - a * C6_LROWS), j_lim = min(C6_RROWS, WF - q * C6_RROWS);
+      float* out = corr_part + ((size_t)p * C6_PARTS + a * C6_RT + q) * WF;
+      for (int d = tw; d < WF; d += 128) {
+        // diagonal i - j = d - 127 of the block: d < 191 covers all of them, the other bins get 0
+        const int dd = d - (C6_RROWS - 1);
+        float sum = 0.f;
+        if (d < C6_LROWS + C6_RROWS - 1) {
+#pragma unroll 8
+          for (int ii = 0; ii < C6_LROWS; ++ii) {
+            const int jj = ii - dd;
+            if (ii < i_lim && jj >= 0 && jj < j_lim) sum += Gw[ii * C6_GPITCH + jj];
+          }
+        }
+        int k = (a * C6_LROWS - q * C6_RROWS + dd - WF / 2) % WF;
+        if (k < 0) k += WF;
+        out[k] = sum;
+      }
+    }
   }
+done:
+  return;
 }
 
 // ------------------------------------------------------------------------------------------------
 // k_leg_mma -- one leg layer (2..) on the hi / lo fp16 C8-interleaved activation planes:
 //   out[y, px, n] = relu(bias[n] + sum_{dh, dw, c} x[y * sh + dh, px + dw, c] W[dh, dw, c, n]),
 //   x * w ~= xh wh + xl wh + xh wl  (three MMAs per K16 step, fp32-grade).
-// EPI 4: output as the next layer's hi / lo planes; EPI 3 (last layer): fp32 feature volume.
-// grid = (n_img * h_out, ceil(M / 64), cout / 64)
+// EPI 4: output as the next layer's hi / lo planes; EPI 3 (last layer): fp32 feature volume; EPI 5: the fp32
+// sum over K slice `slice` of the layer (no bias), combined by k_leg_splitk_reduce.
+// K is walked as (tap = dh * kw + dw, c8) in that order; slice s of n_split takes the iterations
+// [it * s / n_split, it * (s + 1) / n_split) of that walk.
+// grid = (n_img * h_out, ceil(M / 64), n_split * cout / 64), blockIdx.z = slice * nz + z
 // ------------------------------------------------------------------------------------------------
 template <int EPI>
 __global__ void __launch_bounds__(MMA_THREADS)
@@ -798,23 +844,27 @@ k_leg_mma(LegArgs g) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, gq = lane >> 2, t = lane & 3;
   const int64_t px0 = (int64_t)blockIdx.y * MMA_ROWS + warp * 16;
   if (px0 >= g.M) return;
-  const int y = blockIdx.x, z = blockIdx.z;
+  const int nz = (g.n_valid + 63) / 64;
+  const int y = blockIdx.x, z = blockIdx.z % nz, slice = blockIdx.z / nz;
   const int64_t in_base = (int64_t)(y / g.runs_per_img) * g.in_img_planes + (int64_t)(y % g.runs_per_img) * g.in_run_planes;
   const int64_t pa = px0 + gq < g.M ? px0 + gq : g.M - 1, pb = px0 + gq + 8 < g.M ? px0 + gq + 8 : g.M - 1;
   const int n_slabs = g.kh * g.kw * 3;
   const size_t plane = (size_t)g.a_pitch * 8;
+  const int per_tap = g.c8in / 2, n_it = g.kh * g.kw * per_tap;
+  const int it0 = n_it * slice / g.n_split, it1 = n_it * (slice + 1) / g.n_split;
   float acc[8][4] = {};
 #pragma unroll 1
-  for (int dh = 0; dh < g.kh; ++dh) {
-#pragma unroll 1
-    for (int dw = 0; dw < g.kw; ++dw) {
+  for (int it = it0; it < it1;) {
+    const int tap = it / per_tap, dh = tap / g.kw, dw = tap - dh * g.kw;
+    const int c8_end = (tap + 1) * per_tap < it1 ? g.c8in : (it1 - tap * per_tap) * 2;
+    {
       const __half* Ah = g.A + (size_t)(in_base + (int64_t)dh * 2 * g.c8in) * plane + (size_t)dw * 8 + 2 * t;
       const __half* Al = Ah + (size_t)g.c8in * plane;
       // [z][slab = (dh * kw + dw) * 3 + term][c8][64][8]; term 0 = hi, term 2 = lo
       const __half* Bh = g.Bp + ((size_t)(z * n_slabs + (dh * g.kw + dw) * 3) * g.c8in * 64 + gq) * 8 + 2 * t;
       const __half* Bl = Bh + (size_t)2 * g.c8in * 64 * 8;
 #pragma unroll 1
-      for (int c8 = 0; c8 < g.c8in; c8 += 2) {
+      for (int c8 = (it - tap * per_tap) * 2; c8 < c8_end; c8 += 2) {
         const size_t o0 = (size_t)c8 * plane, o1 = o0 + plane;
         const uint32_t h0 = ld_h2(Ah + o0 + pa * 8), h1 = ld_h2(Ah + o0 + pb * 8), h2 = ld_h2(Ah + o1 + pa * 8), h3 = ld_h2(Ah + o1 + pb * 8);
         const uint32_t l0 = ld_h2(Al + o0 + pa * 8), l1 = ld_h2(Al + o0 + pb * 8), l2 = ld_h2(Al + o1 + pa * 8), l3 = ld_h2(Al + o1 + pb * 8);
@@ -829,6 +879,7 @@ k_leg_mma(LegArgs g) {
         }
       }
     }
+    it = tap * per_tap + c8_end / 2;
   }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -838,6 +889,11 @@ k_leg_mma(LegArgs g) {
     for (int j = 0; j < 8; ++j) {
       const int n = z * 64 + j * 8 + 2 * t;
       if (n >= g.n_valid) continue;
+      if (EPI == 5) {         // [slice][y][px][n_valid]
+        *reinterpret_cast<float2*>(g.part + (((size_t)slice * gridDim.x + y) * g.M + px) * g.n_valid + n) =
+            make_float2(acc[j][2 * h], acc[j][2 * h + 1]);
+        continue;
+      }
       const float a = fmaxf(acc[j][2 * h] + __ldg(g.bias + n), 0.f);
       const float b = fmaxf(acc[j][2 * h + 1] + __ldg(g.bias + n + 1), 0.f);
       if (EPI == 4) {
@@ -854,6 +910,44 @@ k_leg_mma(LegArgs g) {
   }
 }
 
+// Single-scan leg: adds the n_split fp32 K-slice sums of k_leg_mma<5> in slice order, then bias, ReLU and the
+// output of EPI (4: hi / lo planes, 3: fp32 volume).  One thread per (row y, pixel, 8 channels).
+template <int EPI>
+__global__ void __launch_bounds__(256)
+k_leg_splitk_reduce(LegArgs g, int rows) {
+  const int c8n = g.n_valid / 8;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)rows * g.M * c8n) return;
+  const int c8 = (int)(i % c8n);
+  const int64_t px = (i / c8n) % g.M, y = i / c8n / g.M;
+  const int64_t slice_stride = (int64_t)rows * g.M * g.n_valid;
+  const float* src = g.part + (y * g.M + px) * g.n_valid + c8 * 8;
+  float v[8] = {};
+  for (int sl = 0; sl < g.n_split; ++sl) {
+    const float4 a = __ldg(reinterpret_cast<const float4*>(src + sl * slice_stride));
+    const float4 b = __ldg(reinterpret_cast<const float4*>(src + sl * slice_stride + 4));
+    v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w; v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
+  }
+#pragma unroll
+  for (int e = 0; e < 8; ++e) v[e] = fmaxf(v[e] + __ldg(g.bias + c8 * 8 + e), 0.f);
+  if (EPI == 4) {
+    __half hi[8], lo[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      hi[e] = __float2half_rn(v[e]);
+      lo[e] = __float2half_rn(v[e] - __half2float(hi[e]));
+    }
+    const int64_t pl = y * g.out_run_planes + c8;
+    *reinterpret_cast<uint4*>(g.out_planes + ((size_t)pl * g.out_pitch + px) * 8) = *reinterpret_cast<const uint4*>(hi);
+    *reinterpret_cast<uint4*>(g.out_planes + ((size_t)(pl + g.out_run_planes / 2) * g.out_pitch + px) * 8) =
+        *reinterpret_cast<const uint4*>(lo);
+  } else {
+    float* dst = g.out_f32 + (y * g.M + px) * g.n_valid + c8 * 8;
+    *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+    *reinterpret_cast<float4*>(dst + 4) = make_float4(v[4], v[5], v[6], v[7]);
+  }
+}
+
 __global__ void __launch_bounds__(384)
 k_corr_finalize(const float* __restrict__ part, float* __restrict__ corr_out, int32_t* __restrict__ yaw,
                 const int* __restrict__ err) {
@@ -861,7 +955,7 @@ k_corr_finalize(const float* __restrict__ part, float* __restrict__ corr_out, in
   const int p = blockIdx.x;
   for (int k = threadIdx.x; k < WF; k += blockDim.x) {
     float c = 0.f;
-    for (int b = 0; b < C6_IBLK; ++b) c += part[((size_t)p * C6_IBLK + b) * WF + k];
+    for (int b = 0; b < C6_PARTS; ++b) c += part[((size_t)p * C6_PARTS + b) * WF + k];
     s_corr[k] = c;
     if (corr_out) corr_out[(size_t)p * WF + k] = c;
   }
@@ -1125,6 +1219,7 @@ void tc_free(ovn_handle* h) {
   if (t->pb_lc) cudaFree(t->pb_lc);
   if (t->actp[0]) cudaFree(t->actp[0]);
   if (t->actp[1]) cudaFree(t->actp[1]);
+  if (t->leg_part) cudaFree(t->leg_part);
   delete t;
   h->tc = nullptr;
 }
@@ -1134,6 +1229,19 @@ static int upload_vec(ovn_handle* h, T** dst, const std::vector<T>& v) {
   OVN_CUDA(h, cudaMalloc(dst, v.size() * sizeof(T)));
   OVN_CUDA(h, cudaMemcpy(*dst, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
   return OVN_OK;
+}
+
+// K slices of a leg layer (2..) for n scans.  A single scan gives layers 3.. only 14-42 output tiles of 64 pixels
+// x 64 channels for 132 SMs, each a chain of up to 144 K iterations whose loads miss a cold L2; n <= 2 (the
+// threshold of k_leg_layer1_small) splits K into slices of >= 4 iterations, up to about 4 CTAs per SM.
+// Batches fill the GPU with tiles and keep one slice (no partial round trip).
+static int leg_split(const ovn_handle* h, const ConvSpec& L, int n) {
+  if (n > 2) return 1;
+  const int64_t tiles = (int64_t)n * L.h_out * ((L.w_out + MMA_ROWS - 1) / MMA_ROWS) * ((L.cout + 63) / 64);
+  const int64_t n_it = (int64_t)L.kh * L.kw * (L.cin / 16);
+  int64_t sp = (4 * h->sm_count + tiles - 1) / tiles;
+  if (sp > n_it / 4) sp = n_it / 4;
+  return sp < 1 ? 1 : (int)sp;
 }
 
 int tc_pack_weights(ovn_handle* h) {
@@ -1242,6 +1350,15 @@ int tc_pack_weights(ovn_handle* h) {
       if ((rc2 = upload_vec(h, &t->wres[l], br)) != OVN_OK) return rc2;
     }
   }
+  size_t part_bytes = 0;
+  for (int l = 1; l < h->n_leg; ++l)
+    for (int n = 1; n <= 2 && n <= h->cfg.max_batch_scans; ++n) {
+      const ConvSpec& L = h->leg[l];
+      const int sp = leg_split(h, L, n);
+      const size_t b = sp > 1 ? (size_t)sp * n * L.h_out * L.w_out * L.cout * sizeof(float) : 0;
+      if (b > part_bytes) part_bytes = b;
+    }
+  if (part_bytes) OVN_CUDA(h, cudaMalloc(&t->leg_part, part_bytes));
   for (int b = 0; b < 2; ++b) {
     const size_t bytes = max_planes_bytes * h->cfg.max_batch_scans + 32768;   // + tile overrun slack
     OVN_CUDA(h, cudaMalloc(&t->actp[b], bytes));
@@ -1259,11 +1376,11 @@ int tc_pack_weights(ovn_handle* h) {
   OVN_CUDA(h, cudaMalloc(&t->partial, (size_t)t->rows_pad * 2 * sizeof(float)));
   OVN_CUDA(h, cudaMalloc(&t->lc, (size_t)maxp * C6_VOL_L_BYTES));
   OVN_CUDA(h, cudaMalloc(&t->rc, (size_t)maxp * C6_VOL_R_BYTES));
-  OVN_CUDA(h, cudaMalloc(&t->corr_part, (size_t)maxp * C6_IBLK * WF * sizeof(float)));
+  OVN_CUDA(h, cudaMalloc(&t->corr_part, (size_t)maxp * C6_PARTS * WF * sizeof(float)));
   OVN_CUDA(h, cudaFuncSetAttribute(k_delta_conv1_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K4Smem)));
   OVN_CUDA(h, cudaFuncSetAttribute(k_conv2_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM));
   OVN_CUDA(h, cudaFuncSetAttribute(k_conv3_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(C3Smem)));
-  OVN_CUDA(h, cudaFuncSetAttribute(k_corr_mma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C6_SMEM));
+  OVN_CUDA(h, cudaFuncSetAttribute(k_corr_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(C6Smem)));
   OVN_CUDA(h, cudaMalloc(&t->mu, CF * sizeof(float)));
   OVN_CUDA(h, cudaMemset(t->mu, 0, CF * sizeof(float)));
   OVN_CUDA(h, cudaMemset(t->o1, 0, (size_t)120 * t->rows_pad * 8 * sizeof(__half)));
@@ -1343,9 +1460,19 @@ int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cuda
     la.in_run_planes = L.sh * 2 * (L.cin / 8); la.kh = L.kh; la.kw = L.kw; la.c8in = L.cin / 8; la.Bp = t->wres[l];
     la.bias = h->d_b[l]; la.n_valid = L.cout; la.M = L.w_out; la.out_planes = t->actp[cur ^ 1]; la.out_pitch = L.w_out;
     la.out_run_planes = 2 * (L.cout / 8); la.out_f32 = d_fv;
-    const dim3 grid((unsigned)(n * L.h_out), (unsigned)((L.w_out + MMA_ROWS - 1) / MMA_ROWS), (unsigned)nz);
-    if (last) k_leg_mma<3><<<grid, MMA_THREADS, 0, s>>>(la);
-    else k_leg_mma<4><<<grid, MMA_THREADS, 0, s>>>(la);
+    la.n_split = leg_split(h, L, n); la.part = t->leg_part;
+    const dim3 grid((unsigned)(n * L.h_out), (unsigned)((L.w_out + MMA_ROWS - 1) / MMA_ROWS), (unsigned)(nz * la.n_split));
+    if (la.n_split > 1) {
+      k_leg_mma<5><<<grid, MMA_THREADS, 0, s>>>(la);
+      OVN_LAUNCH_CHECK(h);
+      const int64_t work = (int64_t)n * L.h_out * L.w_out * (L.cout / 8);
+      if (last) k_leg_splitk_reduce<3><<<(unsigned)((work + 255) / 256), 256, 0, s>>>(la, n * L.h_out);
+      else k_leg_splitk_reduce<4><<<(unsigned)((work + 255) / 256), 256, 0, s>>>(la, n * L.h_out);
+    } else if (last) {
+      k_leg_mma<3><<<grid, MMA_THREADS, 0, s>>>(la);
+    } else {
+      k_leg_mma<4><<<grid, MMA_THREADS, 0, s>>>(la);
+    }
     OVN_LAUNCH_CHECK(h);
     cur ^= 1;
   }
@@ -1382,7 +1509,7 @@ int tc_bank_prepare(ovn_handle* h, const float* d_bank, int64_t capacity, int64_
   }
   if (first > t->pb_rows) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_bank_prepare: rows [%lld, %lld) were never prepared",
                                       (long long)t->pb_rows, (long long)first);
-  const int64_t per = (int64_t)WF * CF / 4, perL = 3 * 2 * 8 * 128;
+  const int64_t per = (int64_t)WF * CF / 4, perL = 16 * C6_LT * C6_LROWS;
   const float* src = d_bank + (size_t)first * WF * CF;
   if (!t->mu_set) {                     // first bank row seen by this handle: calibrate the centres on it
     int rc = calibrate_all(h, src, nullptr, false, s);
@@ -1391,7 +1518,7 @@ int tc_bank_prepare(ovn_handle* h, const float* d_bank, int64_t capacity, int64_
   k_gather_rows_f16<<<(unsigned)((count * per + 255) / 256), 256, 0, s>>>(src, nullptr, (int)count, t->mu, 0,
                                                                          t->pb_l16 + (size_t)first * WF * K4_PITCH);
   OVN_LAUNCH_CHECK(h);
-  k_pack_corr_L<<<(unsigned)((count * perL + 255) / 256), 256, 0, s>>>(src, nullptr, (int)count,
+  k_pack_corr<C6_LROWS, C6_LT><<<(unsigned)((count * perL + 255) / 256), 256, 0, s>>>(src, nullptr, (int)count,
                                                                       t->pb_lc + (size_t)first * (C6_VOL_L_BYTES / 2));
   OVN_LAUNCH_CHECK(h);
   if (first + count > t->pb_rows) t->pb_rows = first + count;
@@ -1546,22 +1673,24 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
     OVN_LAUNCH_CHECK(h);
     // correlation head (tensor cores, hi/lo split operands)
     {
-      const int64_t perL = 3 * 2 * 8 * 128, perR = 2 * 16 * 192;
+      const int64_t perL = 16 * C6_LT * C6_LROWS, perR = 16 * C6_RT * C6_RROWS;
       if (!resident) {
-        k_pack_corr_L<<<(unsigned)((np * perL + 255) / 256), 256, 0, s>>>(d_bank, left, np, t->lc);
+        k_pack_corr<C6_LROWS, C6_LT><<<(unsigned)((np * perL + 255) / 256), 256, 0, s>>>(d_bank, left, np, t->lc);
         OVN_LAUNCH_CHECK(h);
       }
       if (d_query) {
         if (p0 == 0) {
-          k_pack_corr_R<<<(unsigned)((perR + 255) / 256), 256, 0, s>>>(d_query, nullptr, 1, t->rc);
+          k_pack_corr<C6_RROWS, C6_RT><<<(unsigned)((perR + 255) / 256), 256, 0, s>>>(d_query, nullptr, 1, t->rc);
           OVN_LAUNCH_CHECK(h);
         }
       } else {
-        k_pack_corr_R<<<(unsigned)((np * perR + 255) / 256), 256, 0, s>>>(d_bank, right, np, t->rc);
+        k_pack_corr<C6_RROWS, C6_RT><<<(unsigned)((np * perR + 255) / 256), 256, 0, s>>>(d_bank, right, np, t->rc);
         OVN_LAUNCH_CHECK(h);
       }
       prof_mark(h, PROF_CORR, s);
-      k_corr_mma<<<dim3((unsigned)np, C6_IBLK), MMA_THREADS, C6_SMEM, s>>>(lc, lidx, t->rc, d_query ? 0 : 1, t->corr_part);
+      const int64_t units = (int64_t)np * C6_LT;
+      const int nc = units < h->sm_count / C6_RT ? (int)units : h->sm_count / C6_RT;
+      k_corr_wgmma<<<nc * C6_RT, C6_THREADS, sizeof(C6Smem), s>>>(lc, lidx, t->rc, d_query ? 0 : 1, np, t->corr_part, h->d_err);
       prof_mark(h, PROF_CORR, s);
       OVN_LAUNCH_CHECK(h);
       k_corr_finalize<<<np, 384, 0, s>>>(t->corr_part, d_corr ? d_corr + (int64_t)p0 * WF : nullptr, d_yaw + p0, h->d_err);
