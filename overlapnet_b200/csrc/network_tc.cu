@@ -33,7 +33,7 @@ constexpr int CF = 128;                 //   reference geometry: 360 x 128 volum
 constexpr int S15 = 15;
 constexpr int NB = 24;                  // 360 / 15
 constexpr int PAIR_ROWS = NB * NB;      // 576 rows of c_conv2 output per pair
-constexpr int K4_PITCH = CF + 8;        // fp16 row pitch of the L / R operand copies of k_delta_conv1_wgmma
+constexpr int K4_PITCH = CF;            // fp16 row pitch of the L / R operand copies of k_delta_conv1_wgmma (k4_pos)
 
 struct TcState {
   __half* w1p = nullptr;        // [60 steps][4][64][8]
@@ -77,6 +77,15 @@ struct TcState {
 // ------------------------------------------------------------------------------------------------
 // fp32 feature volumes -> fp16 rows gathered by index (the tensor-core operands)
 // ------------------------------------------------------------------------------------------------
+// Storage order of a row of these copies (what k_delta_conv1_wgmma reads; the logical K order is unchanged).  Lane
+// t of an A fragment needs the channel pairs 2t, 2t + 8, 2t + 16 and 2t + 24 of a 32-channel chunk: they are stored
+// adjacent, 16 bytes at t * 16 of the chunk, so a fragment row is one 128-bit shared load.  Chunk cc of row r sits at
+// chunk position cc ^ (r & 1): the two rows of a quarter-warp's load then fall in different halves of the banks.
+__host__ __device__ __forceinline__ int k4_pos(int r, int c) {
+  const int k = c & 31;
+  return (((c >> 5) ^ (r & 1)) << 5) + ((k & 7) >> 1) * 8 + (k >> 3) * 2 + (k & 1);
+}
+
 __global__ void __launch_bounds__(256)
 k_gather_rows_f16(const float* __restrict__ bank, const int32_t* __restrict__ idx, int n, const float* __restrict__ mu,
                   int row_shift, __half* __restrict__ out) {
@@ -86,16 +95,15 @@ k_gather_rows_f16(const float* __restrict__ bank, const int32_t* __restrict__ id
   const int p = (int)(i / per);
   const int64_t e = i % per;
   const int64_t row = idx ? idx[p] : p;
-  const int64_t r = e / (CF / 4), c4 = e % (CF / 4);           // padded row pitch (K4_PITCH halves)
+  const int r = (int)(e / (CF / 4)), c4 = (int)(e % (CF / 4));
   int64_t rs = r + row_shift;                                   // circular row shift (calibration pair only)
   if (rs >= WF) rs -= WF;
   const float4 v = __ldg(reinterpret_cast<const float4*>(bank + (row * WF + rs) * CF) + c4);
   const float4 m = __ldg(reinterpret_cast<const float4*>(mu) + c4);
   __half2 a = __floats2half2_rn(v.x - m.x, v.y - m.y), b = __floats2half2_rn(v.z - m.z, v.w - m.w);
-  uint2 o;
-  o.x = *reinterpret_cast<uint32_t*>(&a);
-  o.y = *reinterpret_cast<uint32_t*>(&b);
-  reinterpret_cast<uint2*>(out + ((int64_t)p * WF + r) * K4_PITCH)[c4] = o;
+  __half* o = out + ((int64_t)p * WF + r) * K4_PITCH;
+  *reinterpret_cast<uint32_t*>(o + k4_pos(r, 4 * c4)) = *reinterpret_cast<uint32_t*>(&a);
+  *reinterpret_cast<uint32_t*>(o + k4_pos(r, 4 * c4 + 2)) = *reinterpret_cast<uint32_t*>(&b);
 }
 
 // Per-channel mean over the rows of n volumes (bank rows idx[0..n) or 0..n-1), rounded to fp16:
@@ -221,19 +229,22 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 //   GEMM per work unit (pair, jb):  o1[i, o] = sum_{dj < 15, c < 128} |L[i, c] - R[15 jb + dj, c]| W1[dj, c, o] - mu_o1[o]
 //   M = 360 LEFT rows (6 row tiles of 64, rows past 360 masked), N = 64, K = 1920 (60 W1 slices of 32 channels).
 // Warp specialisation: warp 12 is the producer (one lane issues bulk copies): the LEFT volume of the current
-// pair (98 KB, once per pair), the 15 RIGHT rows of a unit (double-buffered) and W1 in groups of 6 slices
-// (24 KB) through a 4-deep ring, each buffer guarded by a full / empty mbarrier pair.  Warpgroups 0-2 are
+// pair (90 KB, once per pair), the 15 RIGHT rows of a unit (double-buffered) and W1 in groups of 5 slices
+// (20 KB) through a 4-deep ring, each buffer guarded by a full / empty mbarrier pair.  Warpgroups 0-2 are
 // the consumers: warpgroup w owns row tiles w and w + 3 (2 x 32 fp32 accumulators per thread).  The A
 // operand |l - r| is synthesised in registers from the LEFT rows (kept in registers for a 32-channel chunk)
 // and the broadcast RIGHT row, and multiplied by wgmma in register-A mode against the W1 slice in shared
-// memory: the 66 MB delta tensor of a pair is never written.  The accumulators start at the fp16-rounded
-// -mu_o1 (the centre that k_fold_bias2 pushes through c_conv2).  Output: fp16 o1 tiles.
+// memory: the 66 MB delta tensor of a pair is never written.  A group of 5 slices never straddles a 32-channel
+// chunk (15 dj each), so the slice loop is unrolled straight-line code whose W1 descriptors and RIGHT rows are
+// fixed offsets from bases computed once per group; a RIGHT row is one 128-bit load (k4_pos).  The accumulators
+// start at the fp16-rounded -mu_o1 (the centre that k_fold_bias2 pushes through c_conv2).  Output: fp16 o1 tiles.
 // Persistent: each CTA takes a contiguous range of the n_pairs * 24 units.
 // ------------------------------------------------------------------------------------------------
 constexpr int K4_WG = 3;                               // consumer warpgroups
 constexpr int K4_THREADS = K4_WG * 128 + 32;           // + the producer warp
-constexpr int K4_GROUP = 6;                            // W1 slices per bulk copy
-constexpr int K4_NGROUPS = K4_STEPS / K4_GROUP;        // 10 per unit
+constexpr int K4_GROUP = 5;                            // W1 slices per bulk copy (divides the 15 dj of a chunk)
+constexpr int K4_NGROUPS = K4_STEPS / K4_GROUP;        // 12 per unit
+static_assert(S15 % K4_GROUP == 0, "a W1 group within one 32-channel chunk");
 constexpr int K4_RING = 4;
 constexpr int K4_BSLICE = 4096;                        // bytes of W1 per slice: [4 k8][64 o][8]
 constexpr uint32_t K4_VOL_BYTES = WF * K4_PITCH * 2;
@@ -309,12 +320,6 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
       rows[tt][0] = r;
       rows[tt][1] = r + 8;
     }
-    float mu0[8], mu1[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      mu0[j] = __half2float(__float2half_rn(-mu_o1[j * 8 + 2 * t]));
-      mu1[j] = __half2float(__float2half_rn(-mu_o1[j * 8 + 2 * t + 1]));
-    }
     const uint32_t b_base = smem_u32(S.B[0]);
     uint32_t pi = 0, gi = 0, ui = 0;
     for (int u = u_begin; u < u_end; ++u, ++ui) {
@@ -324,69 +329,74 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
       PIPE_WAIT(&S.rw_full[wb], (ui >> 1) & 1, 404);
       float acc[2][32];
 #pragma unroll
-      for (int tt = 0; tt < 2; ++tt)
+      for (int j = 0; j < 8; ++j) {             // read per unit rather than held in 16 registers across the loop
+        const float m0 = __half2float(__float2half_rn(-__ldg(mu_o1 + j * 8 + 2 * t)));
+        const float m1 = __half2float(__float2half_rn(-__ldg(mu_o1 + j * 8 + 2 * t + 1)));
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          acc[tt][4 * j + 0] = mu0[j]; acc[tt][4 * j + 1] = mu1[j];
-          acc[tt][4 * j + 2] = mu0[j]; acc[tt][4 * j + 3] = mu1[j];
-        }
-      int st = 0;
-#pragma unroll 1
-      for (int cc = 0; cc < 4; ++cc) {
-        // this thread's LEFT values of the 32-channel chunk: [tile][row a / b][kk][lo / hi 8]
-        uint32_t Lr[2][2][2][2];
-#pragma unroll
-        for (int tt = 0; tt < 2; ++tt)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = rows[tt][h] < WF ? rows[tt][h] : WF - 1;
-            const __half* lp = S.L + r * K4_PITCH + cc * 32 + 2 * t;
-#pragma unroll
-            for (int kk = 0; kk < 2; ++kk) {
-              Lr[tt][h][kk][0] = *reinterpret_cast<const uint32_t*>(lp + kk * 16);
-              Lr[tt][h][kk][1] = *reinterpret_cast<const uint32_t*>(lp + kk * 16 + 8);
-            }
-          }
-#pragma unroll 1
-        for (int dj = 0; dj < S15; ++dj, ++st) {
-          const int sl = st % K4_GROUP;
-          const uint32_t s = gi % K4_RING;
-          if (sl == 0) PIPE_WAIT(&S.full[s], (gi / K4_RING) & 1, 202);
-          const __half* rp = S.Rw[wb] + dj * K4_PITCH + cc * 32 + 2 * t;
-          uint32_t A[2][2][4];                // [tile][kk]
-#pragma unroll
-          for (int kk = 0; kk < 2; ++kk) {
-            const uint32_t r0 = *reinterpret_cast<const uint32_t*>(rp + kk * 16);
-            const uint32_t r1 = *reinterpret_cast<const uint32_t*>(rp + kk * 16 + 8);
-#pragma unroll
-            for (int tt = 0; tt < 2; ++tt) {
-              A[tt][kk][0] = absdiff_h2(Lr[tt][0][kk][0], r0);
-              A[tt][kk][1] = absdiff_h2(Lr[tt][1][kk][0], r0);
-              A[tt][kk][2] = absdiff_h2(Lr[tt][0][kk][1], r1);
-              A[tt][kk][3] = absdiff_h2(Lr[tt][1][kk][1], r1);
-            }
-          }
-          const uint32_t slice = b_base + s * (K4_GROUP * K4_BSLICE) + sl * K4_BSLICE;
-          wgmma_fence();
-#pragma unroll
-          for (int kk = 0; kk < 2; ++kk) {
-            // the K16 step covers W1 chunks k8 = 2 kk, 2 kk + 1: LBO = 1024 B between them, SBO = 128 B per 8 outputs
-            const uint64_t bd = desc_kmajor(slice + kk * 2048, 1024, 128, kNoSwizzle);
-#pragma unroll
-            for (int tt = 0; tt < 2; ++tt) wgmma_m64n64k16_rs(acc[tt], A[tt][kk], bd);
-          }
-          wgmma_commit();
-          wgmma_wait<0>();                    // A registers and the W1 slot are free again
-          if (sl == K4_GROUP - 1) {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&S.empty[s]);
-            ++gi;
-          }
+        for (int tt = 0; tt < 2; ++tt) {
+          acc[tt][4 * j + 0] = m0; acc[tt][4 * j + 1] = m1;
+          acc[tt][4 * j + 2] = m0; acc[tt][4 * j + 3] = m1;
         }
       }
+      uint32_t Lr[2][2][4];                   // LEFT values of the chunk: [tile][row a / b][kk0 lo, hi, kk1 lo, hi]
+#pragma unroll 1
+      for (int grp = 0; grp < K4_NGROUPS; ++grp, ++gi) {
+        const int cc = grp / 3, dj0 = (grp - 3 * cc) * K4_GROUP;
+        if (dj0 == 0) {
+#pragma unroll
+          for (int tt = 0; tt < 2; ++tt)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int r = rows[tt][h] < WF ? rows[tt][h] : WF - 1;
+              const uint4 v = *reinterpret_cast<const uint4*>(S.L + r * K4_PITCH + ((cc ^ (r & 1)) << 5) + 8 * t);
+              Lr[tt][h][0] = v.x; Lr[tt][h][1] = v.y; Lr[tt][h][2] = v.z; Lr[tt][h][3] = v.w;
+            }
+        }
+        const uint32_t s = gi % K4_RING;
+        // slice sl of the stage, K16 step kk: W1 chunks k8 = 2 kk, 2 kk + 1 (LBO = 1024 B between them, SBO = 128 B
+        // per 8 outputs) at sl * 4096 + kk * 2048 bytes, i.e. (sl * 4096 + kk * 2048) >> 4 in the descriptor
+        const uint64_t bdesc = desc_kmajor(b_base + s * (K4_GROUP * K4_BSLICE), 1024, 128, kNoSwizzle);
+        // RIGHT row dj0 + sl of the window is row 15 jb + dj0 + sl of the volume: its chunks are swapped when odd
+        const int par = (jb + dj0) & 1;
+        const __half* rw = S.Rw[wb] + dj0 * K4_PITCH + 8 * t;
+        const __half* rp[2] = {rw + ((cc ^ par) << 5), rw + ((cc ^ par ^ 1) << 5)};
+        uint4 rv = *reinterpret_cast<const uint4*>(rp[0]);
+        PIPE_WAIT(&S.full[s], (gi / K4_RING) & 1, 202);
+#pragma unroll
+        for (int sl = 0; sl < K4_GROUP; ++sl) {
+          uint32_t A[2][2][4];                // [tile][kk]
+#pragma unroll
+          for (int tt = 0; tt < 2; ++tt) {
+            A[tt][0][0] = absdiff_h2(Lr[tt][0][0], rv.x);
+            A[tt][0][1] = absdiff_h2(Lr[tt][1][0], rv.x);
+            A[tt][0][2] = absdiff_h2(Lr[tt][0][1], rv.y);
+            A[tt][0][3] = absdiff_h2(Lr[tt][1][1], rv.y);
+            A[tt][1][0] = absdiff_h2(Lr[tt][0][2], rv.z);
+            A[tt][1][1] = absdiff_h2(Lr[tt][1][2], rv.z);
+            A[tt][1][2] = absdiff_h2(Lr[tt][0][3], rv.w);
+            A[tt][1][3] = absdiff_h2(Lr[tt][1][3], rv.w);
+          }
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+            for (int tt = 0; tt < 2; ++tt)
+              wgmma_m64n64k16_rs(acc[tt], A[tt][kk], bdesc + ((sl * K4_BSLICE + kk * 2048) >> 4));
+          wgmma_commit();
+          // the next RIGHT row loads while the MMAs run.  They are waited for at once and the three warpgroups supply
+          // the overlap: a second A register set for wait_group 1 spills at the 128-register cap of 13 warps, and
+          // the spill-light per-K16 form of it was slower (DESIGN §4)
+          if (sl + 1 < K4_GROUP) rv = *reinterpret_cast<const uint4*>(rp[(sl + 1) & 1] + (sl + 1) * K4_PITCH);
+          wgmma_wait<0>();
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&S.empty[s]);
+      }
       __syncwarp();
-      if (lane == 0) mbar_arrive(&S.rw_empty[wb]);
-      if (jb == NB - 1 || u == u_end - 1) { if (lane == 0) mbar_arrive(&S.l_empty); }
+      if (lane == 0) {
+        mbar_arrive(&S.rw_empty[wb]);
+        if (jb == NB - 1 || u == u_end - 1) mbar_arrive(&S.l_empty);
+      }
       const int64_t mrow = (int64_t)p * PAIR_ROWS + jb * NB;
 #pragma unroll
       for (int tt = 0; tt < 2; ++tt)
