@@ -145,6 +145,29 @@ int ovn_gt_overlap_count(ovn_handle* h, const float* d_ref_ranges /* [n][H][W] *
                          const float* d_cur_range /* [H][W] */, int32_t n_scans,
                          int32_t* d_counts /* [n_scans + 1] */, void* stream);
 
+/* ---- ground truth for every frame pair (demo4_gen_gt_files.py over a whole sequence) -------------
+ * The clouds stay resident on the device.  d_radius[b] = max ||p|| of scan b in float64 (0 if empty);
+ * compute it once per upload for ovn_gt_pairs_count. */
+int ovn_gt_scan_radius(ovn_handle* h, const float* d_points, const int64_t* d_offsets /* [n+1] */,
+                       int32_t n_scans, double* d_radius /* [n] */, void* stream);
+
+/* d_counts[f * ld_counts + r] = what ovn_gt_range_batch(reference scan r, d_pose_ref[r], d_pose_cur_inv[f])
+ * followed by ovn_gt_overlap_count(..., d_cur_range[f]) gives, bit for bit, for every current frame f < n_cur
+ * and reference scan r < n_ref.  Reference scan r is the points [h_offsets[r], h_offsets[r+1]) of d_points
+ * (the offsets are read on the host).  d_cur_range [n_cur][H][W]: the frames' untransformed images
+ * (ovn_gt_range_batch without poses).  Frames x references are processed in tiles of tile_cur x tile_ref
+ * pairs (<= 0: defaults sized so that the tile's key images stay in L2; more than 32 x 64 is
+ * OVN_ERR_CAPACITY); the counts do not depend on the tiling.  A pair whose every point provably lies at or
+ * beyond max_range (||t_rel|| - s(R_rel) d_radius[r] - eps >= max_range, DESIGN.md section 4) is skipped with
+ * count 0; *d_n_pruned (device, may be NULL) receives their number.  max_range < 0 selects the handle's.
+ * The key-image workspace is allocated by the first call. */
+int ovn_gt_pairs_count(ovn_handle* h, const float* d_points, const int64_t* h_offsets /* [n_ref+1], host */,
+                       int32_t n_ref, const double* d_pose_ref /* [n_ref][16] */, const double* d_radius /* [n_ref] */,
+                       const float* d_cur_range /* [n_cur][H][W] */, const double* d_pose_cur_inv /* [n_cur][16] */,
+                       int32_t n_cur, float max_range, int32_t tile_cur, int32_t tile_ref,
+                       int32_t* d_counts /* [n_cur][ld_counts] */, int64_t ld_counts, int64_t* d_n_pruned,
+                       void* stream);
+
 /* ---- stage 1d: fused raw cloud -> packed network input ------------------------------------- */
 /* Projection + normals + channel packing (ImagePairOverlapOrientationSequence.py:130-207) in one
  * pass; d_probs may be NULL when n_prob_channels == 0.  d_input: [n][H][W][C] float32. */

@@ -4,6 +4,8 @@ Public surface mirrors the reference (PRBonn/OverlapNet):
   Infer                         src/two_heads/infer.py:22
   range_projection, gen_normal_map, gen_*_data   src/utils/utils.py, src/utils/gen_*_data.py
   com_overlap_yaw               src/utils/com_overlap_yaw.py:10
+  normalize_data, split_train_val   src/utils/normalize_data.py, src/utils/split_train_val.py
+  overlap_yaw_all_pairs         com_overlap_yaw for every frame of a sequence at once
 Everything computes through hand-written CUDA kernels behind the C ABI in include/ovn_b200.h;
 there is no CPU fallback.
 """
@@ -22,7 +24,11 @@ def __getattr__(name):
               'gen_intensity_data', 'gen_semantic_data'):
     from . import preprocess
     return getattr(preprocess, name)
-  if name in ('com_overlap_yaw', 'load_poses', 'load_calib', 'euler_angles_from_rotation_matrix'):
+  if name in ('com_overlap_yaw', 'load_poses', 'load_calib', 'euler_angles_from_rotation_matrix',
+              'overlap_yaw_all_pairs', 'all_pairs_rows'):
     from . import gt
     return getattr(gt, name)
+  if name in ('normalize_data', 'split_train_val'):
+    from . import gt_files
+    return getattr(gt_files, name)
   raise AttributeError(name)

@@ -267,7 +267,7 @@ int ovn_destroy(ovn_handle* h) {
   for (auto& p : h->d_w16) if (p) cudaFree(p);
   void* bufs[] = {h->d_keys, h->d_valid_words, h->d_word_prefix, h->d_scan_tmp, h->d_act[0], h->d_act[1],
                   h->d_input, h->d_o1, h->d_o2, h->d_logit, h->d_G, h->d_idx_tmp, h->d_query_fv,
-                  h->d_stage_points, h->d_stage_offsets, h->d_idx_san, h->d_err};
+                  h->d_stage_points, h->d_stage_offsets, h->d_idx_san, h->d_err, h->d_pair_keys, h->d_pair_prune};
   for (void* b : bufs) if (b) cudaFree(b);
   if (h->h_pinned) cudaFreeHost(h->h_pinned);
   if (h->ev_bank) cudaEventDestroy(h->ev_bank);
@@ -496,6 +496,32 @@ int ovn_gt_overlap_count(ovn_handle* h, const float* d_ref_ranges, const float* 
   REQUIRE(h, n_scans >= 0, "negative size");
   REQUIRE(h, d_cur_range && d_counts && (n_scans == 0 || d_ref_ranges), "NULL pointer");
   return gt_overlap_count(h, d_ref_ranges, d_cur_range, n_scans, d_counts, (cudaStream_t)stream);
+}
+
+int ovn_gt_scan_radius(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int32_t n_scans,
+                       double* d_radius, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, n_scans >= 0, "negative size");
+  REQUIRE(h, n_scans == 0 || (d_points && d_offsets && d_radius), "NULL pointer");
+  return gt_scan_radius(h, d_points, d_offsets, n_scans, d_radius, (cudaStream_t)stream);
+}
+
+int ovn_gt_pairs_count(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int32_t n_ref,
+                       const double* d_pose_ref, const double* d_radius, const float* d_cur_range,
+                       const double* d_pose_cur_inv, int32_t n_cur, float max_range, int32_t tile_cur,
+                       int32_t tile_ref, int32_t* d_counts, int64_t ld_counts, int64_t* d_n_pruned, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, n_ref >= 0 && n_cur >= 0, "negative size");
+  REQUIRE(h, ld_counts >= n_ref, "ld_counts < n_ref");
+  REQUIRE(h, n_cur == 0 || d_counts, "NULL pointer");
+  REQUIRE(h, n_cur == 0 || n_ref == 0 || (d_points && h_offsets && d_pose_ref && d_radius && d_cur_range && d_pose_cur_inv),
+          "NULL pointer");
+  for (int32_t i = 0; i < n_ref && n_cur > 0; ++i)
+    REQUIRE(h, h_offsets[i] >= 0 && h_offsets[i] <= h_offsets[i + 1], "h_offsets must be non-negative and non-decreasing");
+  return gt_pairs_count(h, d_points, h_offsets, n_ref, d_pose_ref, d_radius, d_cur_range, d_pose_cur_inv, n_cur,
+                        max_range, tile_cur, tile_ref, d_counts, ld_counts, d_n_pruned, (cudaStream_t)stream);
 }
 
 int ovn_preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int32_t n_scans,

@@ -85,6 +85,10 @@ struct ovn_handle {
 
   // workspaces
   unsigned long long* d_keys = nullptr;      // [max_batch_scans][H*W] atomic-min keys
+  unsigned long long* d_pair_keys = nullptr; // ovn_gt_pairs_count: [tile_cur][tile_ref][H*W] keys, allocated on first use
+  size_t cap_pair_keys = 0;
+  uint8_t* d_pair_prune = nullptr;           // ovn_gt_pairs_count: pruned-pair counter + [n_cur][n_ref] flags
+  size_t cap_pair_prune = 0;
   uint32_t* d_valid_words = nullptr;         // validity bitmask, 1 bit per point
   uint32_t* d_word_prefix = nullptr;         // exclusive prefix of popcounts
   uint32_t* d_scan_tmp = nullptr;
@@ -182,6 +186,12 @@ int gt_range_batch(ovn_handle* h, const float* d_points, const int64_t* d_offset
                    const double* d_pose_ref, const double* d_pose_cur_inv, float max_range, float* d_range,
                    cudaStream_t s);
 int gt_overlap_count(ovn_handle* h, const float* d_ref, const float* d_cur, int n_scans, int32_t* d_counts, cudaStream_t s);
+int gt_scan_radius(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans, double* d_radius,
+                   cudaStream_t s);
+int gt_pairs_count(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int n_ref, const double* d_pose_ref,
+                   const double* d_radius, const float* d_cur_range, const double* d_pose_cur_inv, int n_cur,
+                   float max_range, int tile_cur, int tile_ref, int32_t* d_counts, int64_t ld_counts,
+                   int64_t* d_n_pruned, cudaStream_t s);
 int pack_input(ovn_handle* h, const float* d_depth, const float* d_normal, const float* d_prob,
                const float* d_intensity, int n_scans, float* d_input, cudaStream_t s);
 

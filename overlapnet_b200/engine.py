@@ -210,6 +210,33 @@ class Engine:
                                              self._stream()), 'ovn_gt_overlap_count')
     return counts
 
+  def gt_scan_radius(self, batch):
+    """ovn_gt_scan_radius: float64 [n] = max ||p|| of each scan of a CloudBatch (0 for an empty scan)."""
+    out = torch.empty((batch.n,), dtype=torch.float64, device=self.device)
+    check(self._h, lib().ovn_gt_scan_radius(self._h, _ptr(batch.points), _ptr(batch.offsets), batch.n, _ptr(out),
+                                           self._stream()), 'ovn_gt_scan_radius')
+    return out
+
+  def gt_pairs_count(self, batch, pose_ref, radius, cur_ranges, pose_cur_inv, counts=None, n_pruned=None,
+                     max_range=-1.0, tile_cur=0, tile_ref=0):
+    """ovn_gt_pairs_count: int32 [n_cur, n_ref] ground-truth counts of every (current frame, reference scan)
+    pair, each equal to gt_range + gt_overlap_count for that pair.  ``batch``: the reference scans
+    (CloudBatch); ``pose_ref`` float64 [n_ref, 4, 4] and ``radius`` (gt_scan_radius) on the device;
+    ``cur_ranges`` [n_cur, H, W] the frames' own images; ``pose_cur_inv`` float64 [n_cur, 4, 4] on the device.
+    ``counts`` may be a column slice of a wider int32 tensor (rows contiguous); ``n_pruned`` an int64 device
+    scalar that receives the number of pairs skipped by the range bound."""
+    n_ref, n_cur = batch.n, int(cur_ranges.shape[0])
+    if counts is None:
+      counts = torch.empty((n_cur, n_ref), dtype=torch.int32, device=self.device)
+    assert counts.dtype == torch.int32 and tuple(counts.shape) == (n_cur, n_ref) and counts.stride(1) == 1
+    ld = counts.stride(0) if n_cur > 1 else n_ref
+    offs = np.ascontiguousarray(batch.offsets_host, np.int64)
+    check(self._h, lib().ovn_gt_pairs_count(
+        self._h, _ptr(batch.points), offs.ctypes.data_as(C.c_void_p), n_ref, _ptr(pose_ref), _ptr(radius),
+        _ptr(cur_ranges), _ptr(pose_cur_inv), n_cur, float(max_range), int(tile_cur), int(tile_ref), _ptr(counts),
+        int(ld), _ptr(n_pruned), self._stream()), 'ovn_gt_pairs_count')
+    return counts
+
   def normals(self, rng, vertex):
     n = rng.shape[0]
     out = torch.empty((n, self.H, self.W, 3), dtype=torch.float32, device=self.device)
