@@ -75,8 +75,8 @@ int sanitize_indices(ovn_handle* h, const int32_t* d_in, int n, int64_t limit, i
 // The caller has queued everything on `s`; this copies the flag back, synchronises `s` and maps a
 // non-zero flag to a status (the flag is cleared so that the handle stays usable).
 int check_device_error(ovn_handle* h, cudaStream_t s) {
-  int* hp = reinterpret_cast<int*>(h->h_pinned);
-  if (!hp || !h->d_err) return OVN_OK;
+  if (!h->h_pinned || !h->d_err) return OVN_OK;
+  int32_t* hp = &h->stage()->err;
   OVN_CUDA(h, cudaMemcpyAsync(hp, h->d_err, sizeof(int), cudaMemcpyDeviceToHost, s));
   OVN_CUDA(h, cudaStreamSynchronize(s));
   const int e = *hp;
@@ -139,18 +139,32 @@ int ovn_feature_channels(const ovn_handle* h) { return h ? kFeatC : 0; }
     char _b[512];                                           \
     snprintf(_b, sizeof(_b), __VA_ARGS__);                  \
     g_create_error = _b;                                    \
-    if (h) ovn_destroy(h);                                  \
     return (code);                                          \
   } while (0)
 
+// consumes the error like OVN_CUDA, so that it is reported once
 #define CREATE_CUDA(call)                                                              \
   do {                                                                                 \
     cudaError_t _e = (call);                                                           \
-    if (_e != cudaSuccess) CREATE_FAIL(OVN_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(_e)); \
+    if (_e != cudaSuccess) {                                                           \
+      cudaGetLastError();                                                              \
+      CREATE_FAIL(OVN_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(_e));              \
+    }                                                                                  \
   } while (0)
 
+// a workspace allocation of ovn_create: its message is the one Buffer::ensure left in the handle
+#define CREATE_ALLOC(buf, bytes)                                                       \
+  do {                                                                                 \
+    if ((buf).ensure(h.get(), (bytes)) != OVN_OK) CREATE_FAIL(OVN_ERR_CUDA, "ovn_create: %s", h->last_error.c_str()); \
+  } while (0)
+
+ovn_handle::~ovn_handle() {
+  if (ev_bank) cudaEventDestroy(ev_bank);
+  if (own_stream) cudaStreamDestroy(own_stream);
+  for (auto& v : prof_ev) for (cudaEvent_t e : v) cudaEventDestroy(e);
+}
+
 int ovn_create(const ovn_config* cfg, ovn_handle** out) {
-  ovn_handle* h = nullptr;
   if (!cfg || !out) CREATE_FAIL(OVN_ERR_INVALID_ARG, "ovn_create: NULL argument");
   *out = nullptr;
   if (cfg->abi_version != OVN_ABI_VERSION)
@@ -167,7 +181,7 @@ int ovn_create(const ovn_config* cfg, ovn_handle** out) {
   if (prop.major != 9 || prop.minor != 0)
     CREATE_FAIL(OVN_ERR_NO_DEVICE, "ovn_create: device %d is sm_%d%d; this build targets sm_90a only", dev,
                 prop.major, prop.minor);
-  h = new ovn_handle();
+  std::unique_ptr<ovn_handle> h(new ovn_handle());
   h->cfg = *cfg;
   h->device = dev;
   h->sm_count = prop.multiProcessorCount;
@@ -225,54 +239,40 @@ int ovn_create(const ovn_config* cfg, ovn_handle** out) {
 
   // ---- workspaces
   const size_t HW = (size_t)c.proj_H * c.proj_W;
-  CREATE_CUDA(cudaMalloc(&h->d_keys, (size_t)c.max_batch_scans * HW * sizeof(unsigned long long)));
-  CREATE_CUDA(cudaMalloc(&h->d_input, (size_t)c.max_batch_scans * HW * h->C * sizeof(float)));
+  const size_t maxp = c.max_batch_pairs;
+  CREATE_ALLOC(h->d_keys, c.max_batch_scans * HW * sizeof(unsigned long long));
+  CREATE_ALLOC(h->d_input, c.max_batch_scans * HW * h->C * sizeof(float));
   size_t max_act = 1;
   for (int l = 0; l < h->n_leg; ++l) {
     size_t a = (size_t)h->leg[l].h_out * h->leg[l].w_out * h->leg[l].cout;
     if (a > max_act) max_act = a;
   }
-  h->cap_act = (int64_t)max_act * c.max_batch_scans;
-  CREATE_CUDA(cudaMalloc(&h->d_act[0], h->cap_act * sizeof(float)));
-  CREATE_CUDA(cudaMalloc(&h->d_act[1], h->cap_act * sizeof(float)));
-  CREATE_CUDA(cudaMalloc(&h->d_query_fv, (size_t)Wf * kFeatC * sizeof(float)));
-  CREATE_CUDA(cudaMalloc(&h->d_idx_tmp, (size_t)2 * c.max_batch_pairs * sizeof(int32_t)));
-  CREATE_CUDA(cudaMalloc(&h->d_idx_san, (size_t)3 * c.max_batch_pairs * sizeof(int32_t)));   // left, right, resident-row check
-  CREATE_CUDA(cudaMalloc(&h->d_err, sizeof(int)));
+  CREATE_ALLOC(h->d_act[0], max_act * c.max_batch_scans * sizeof(float));
+  CREATE_ALLOC(h->d_act[1], max_act * c.max_batch_scans * sizeof(float));
+  CREATE_ALLOC(h->d_query_fv, (size_t)Wf * kFeatC * sizeof(float));
+  CREATE_ALLOC(h->d_cand_idx, maxp * sizeof(int32_t));
+  CREATE_ALLOC(h->d_query_yaw, maxp * sizeof(int32_t));
+  CREATE_ALLOC(h->d_idx_san, 3 * maxp * sizeof(int32_t));   // left, right, resident-row check
+  CREATE_ALLOC(h->d_err, sizeof(int));
   CREATE_CUDA(cudaMemset(h->d_err, 0, sizeof(int)));
   CREATE_CUDA(cudaEventCreateWithFlags(&h->ev_bank, cudaEventDisableTiming));
-  // pinned staging of the host entry points: [err int, pad][offsets 2 x i64][3 training losses, pad][cand idx][overlap][yaw]
-  h->cap_pinned = 64 + (int64_t)c.max_batch_pairs * 12;
-  CREATE_CUDA(cudaHostAlloc(&h->h_pinned, (size_t)h->cap_pinned, cudaHostAllocDefault));
-  CREATE_CUDA(cudaMalloc(&h->d_logit, (size_t)c.max_batch_pairs * sizeof(float)));
-  if (h->net_ok) CREATE_CUDA(cudaMalloc(&h->d_G, (size_t)c.max_batch_pairs * Wf * Wf * sizeof(float)));
+  CREATE_ALLOC(h->h_pinned, sizeof(StageHeader) + maxp * 3 * sizeof(int32_t));
+  CREATE_ALLOC(h->d_query_overlap, maxp * sizeof(float));
   if (c.precision == OVN_PREC_FP32 && h->net_ok) {
-    CREATE_CUDA(cudaMalloc(&h->d_o1, (size_t)c.max_batch_pairs * h->o1_h * h->o1_w * 64 * sizeof(float)));
-    CREATE_CUDA(cudaMalloc(&h->d_o2, (size_t)c.max_batch_pairs * h->o2_h * h->o2_w * 128 * sizeof(float)));
+    CREATE_ALLOC(h->d_o1, maxp * h->o1_h * h->o1_w * 64 * sizeof(float));
+    CREATE_ALLOC(h->d_o2, maxp * h->o2_h * h->o2_w * 128 * sizeof(float));
+    CREATE_ALLOC(h->d_G, maxp * Wf * Wf * sizeof(float));
   } else if (c.precision != OVN_PREC_F16_TC && c.precision != OVN_PREC_FP32) {
     CREATE_FAIL(OVN_ERR_BAD_CONFIG, "ovn_create: unknown precision %d", c.precision);
   }
   CREATE_CUDA(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
-  *out = h;
+  *out = h.release();
   return OVN_OK;
 }
 
 int ovn_destroy(ovn_handle* h) {
   if (!h) return OVN_OK;
   DeviceGuard guard(h);
-  tc_free(h);
-  train_free(h);
-  for (auto& p : h->d_w) if (p) cudaFree(p);
-  for (auto& p : h->d_b) if (p) cudaFree(p);
-  for (auto& p : h->d_w16) if (p) cudaFree(p);
-  void* bufs[] = {h->d_keys, h->d_valid_words, h->d_word_prefix, h->d_scan_tmp, h->d_act[0], h->d_act[1],
-                  h->d_input, h->d_o1, h->d_o2, h->d_logit, h->d_G, h->d_idx_tmp, h->d_query_fv,
-                  h->d_stage_points, h->d_stage_offsets, h->d_idx_san, h->d_err, h->d_pair_keys, h->d_pair_prune};
-  for (void* b : bufs) if (b) cudaFree(b);
-  if (h->h_pinned) cudaFreeHost(h->h_pinned);
-  if (h->ev_bank) cudaEventDestroy(h->ev_bank);
-  if (h->own_stream) cudaStreamDestroy(h->own_stream);
-  for (auto& v : h->prof_ev) for (cudaEvent_t e : v) cudaEventDestroy(e);
   delete h;
   return OVN_OK;
 }
@@ -356,13 +356,8 @@ int ovn_set_weights(ovn_handle* h, const char* name, const float* k, const int64
 }
 
 static int upload(ovn_handle* h, int slot, const LayerWeights& w) {
-  if (h->d_w[slot]) { cudaFree(h->d_w[slot]); h->d_w[slot] = nullptr; }
-  if (h->d_b[slot]) { cudaFree(h->d_b[slot]); h->d_b[slot] = nullptr; }
-  OVN_CUDA(h, cudaMalloc(&h->d_w[slot], w.kernel.size() * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&h->d_b[slot], w.bias.size() * sizeof(float)));
-  OVN_CUDA(h, cudaMemcpy(h->d_w[slot], w.kernel.data(), w.kernel.size() * sizeof(float), cudaMemcpyHostToDevice));
-  OVN_CUDA(h, cudaMemcpy(h->d_b[slot], w.bias.data(), w.bias.size() * sizeof(float), cudaMemcpyHostToDevice));
-  return OVN_OK;
+  const int rc = upload_vec(h, h->d_w[slot], w.kernel);
+  return rc != OVN_OK ? rc : upload_vec(h, h->d_b[slot], w.bias);
 }
 
 int ovn_finalize_weights(ovn_handle* h) {
@@ -620,9 +615,9 @@ int ovn_heads_1vsN(ovn_handle* h, const float* d_bank, int64_t bank_size, const 
   const int maxp = h->cfg.max_batch_pairs;
   for (int p0 = 0; p0 < n_cand; p0 += maxp) {
     const int np = (n_cand - p0 < maxp) ? n_cand - p0 : maxp;
-    k_iota<<<(np + 255) / 256, 256, 0, s>>>(h->d_idx_tmp, np, p0);
+    k_iota<<<(np + 255) / 256, 256, 0, s>>>(h->d_cand_idx, np, p0);
     OVN_LAUNCH_CHECK(h);
-    int rc = heads_dispatch(h, d_bank, bank_size, d_query, h->d_idx_tmp, nullptr,
+    int rc = heads_dispatch(h, d_bank, bank_size, d_query, h->d_cand_idx, nullptr,
                             np, d_overlap + p0, d_yaw + p0,
                             d_corr ? d_corr + (size_t)p0 * h->cfg.leg_output_width : nullptr, s);
     if (rc != OVN_OK) return rc;
@@ -676,7 +671,7 @@ int ovn_head_gradients(ovn_handle* h, const float* d_bank, int64_t bank_size, co
   if (rc == OVN_OK)
     rc = head_gradients_fp32(h, d_bank, l, r, n_pairs, d_gt_overlap, d_gt_orientation, min_overlap_for_angle, s);
   if (rc != OVN_OK) return rc;
-  float* p_loss = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(h->h_pinned) + 48);
+  float* p_loss = h->stage()->loss;
   OVN_CUDA(h, cudaMemcpyAsync(p_loss, h->train->loss, 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
   rc = check_device_error(h, s);            // synchronises s; a bad index -> OVN_ERR_INVALID_ARG
   if (rc != OVN_OK) return rc;
@@ -773,17 +768,11 @@ int ovn_bank_release(ovn_handle* h, const float* d_bank) {
 }
 
 // ---- host-buffer entry points ---------------------------------------------------------------------
-static int ensure_stage(ovn_handle* h, int64_t n_points, int n_scans) {
-  if (n_points > h->cap_stage_points) {
-    if (h->d_stage_points) cudaFree(h->d_stage_points);
-    h->d_stage_points = nullptr;
-    const int64_t cap = n_points + n_points / 8 + 4096;
-    OVN_CUDA(h, cudaMalloc(&h->d_stage_points, cap * 4 * sizeof(float)));
-    h->cap_stage_points = cap;
-  }
-  if (!h->d_stage_offsets) OVN_CUDA(h, cudaMalloc(&h->d_stage_offsets, ((size_t)h->cfg.max_batch_scans + 1) * sizeof(int64_t)));
-  (void)n_scans;
-  return OVN_OK;
+static int ensure_stage(ovn_handle* h, int64_t n_points) {
+  const size_t point_bytes = 4 * sizeof(float);
+  const int rc = h->d_stage_points.ensure(h, n_points * point_bytes, (n_points + n_points / 8 + 4096) * point_bytes);
+  if (rc != OVN_OK) return rc;
+  return h->d_stage_offsets.ensure(h, ((size_t)h->cfg.max_batch_scans + 1) * sizeof(int64_t));
 }
 
 int ovn_encode_clouds_host(ovn_handle* h, const float* h_points, const int64_t* h_offsets, int32_t n_scans,
@@ -798,32 +787,29 @@ int ovn_encode_clouds_host(ovn_handle* h, const float* h_points, const int64_t* 
                 "use the device-pointer stages");
   cudaStream_t s = h->own_stream;
   const int Wf = h->cfg.leg_output_width;
-  float* d_fv = nullptr;
-  OVN_CUDA(h, cudaMalloc(&d_fv, (size_t)h->cfg.max_batch_scans * Wf * kFeatC * sizeof(float)));
-  int rc = OVN_OK;
-  for (int s0 = 0; s0 < n_scans && rc == OVN_OK; s0 += h->cfg.max_batch_scans) {
+  Buffer<float> d_fv;
+  int rc = d_fv.ensure(h, (size_t)h->cfg.max_batch_scans * Wf * kFeatC * sizeof(float));
+  if (rc != OVN_OK) return rc;
+  for (int s0 = 0; s0 < n_scans; s0 += h->cfg.max_batch_scans) {
     const int n = (n_scans - s0 < h->cfg.max_batch_scans) ? n_scans - s0 : h->cfg.max_batch_scans;
     const int64_t p0 = h_offsets[s0], p1 = h_offsets[s0 + n];
-    rc = ensure_stage(h, p1 - p0, n);
-    if (rc != OVN_OK) break;
+    rc = ensure_stage(h, p1 - p0);
+    if (rc != OVN_OK) return rc;
     std::vector<int64_t> rel(n + 1);
     for (int i = 0; i <= n; ++i) rel[i] = h_offsets[s0 + i] - p0;
-    cudaError_t e = cudaMemcpyAsync(h->d_stage_points, h_points + p0 * 4, (p1 - p0) * 4 * sizeof(float),
-                                    cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h->d_stage_offsets, rel.data(), (n + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);   // rel is a stack-lifetime buffer
-    if (e != cudaSuccess) { h->last_error = cudaGetErrorString(e); rc = OVN_ERR_CUDA; break; }
+    OVN_CUDA(h, cudaMemcpyAsync(h->d_stage_points, h_points + p0 * 4, (p1 - p0) * 4 * sizeof(float),
+                                cudaMemcpyHostToDevice, s));
+    OVN_CUDA(h, cudaMemcpyAsync(h->d_stage_offsets, rel.data(), (n + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    OVN_CUDA(h, cudaStreamSynchronize(s));   // rel is a stack-lifetime buffer
     rc = preprocess_batch(h, h->d_stage_points, h->d_stage_offsets, n, p1 - p0, nullptr, h->d_input, s);
     if (rc == OVN_OK) rc = ovn_leg_forward(h, h->d_input, n, d_fv, s);
-    if (rc == OVN_OK) {
-      e = cudaMemcpyAsync(h_fv + (size_t)s0 * Wf * kFeatC, d_fv, (size_t)n * Wf * kFeatC * sizeof(float),
-                          cudaMemcpyDeviceToHost, s);
-      if (e != cudaSuccess) { h->last_error = cudaGetErrorString(e); rc = OVN_ERR_CUDA; }
-      else rc = check_device_error(h, s);                 // synchronises s
-    }
+    if (rc != OVN_OK) return rc;
+    OVN_CUDA(h, cudaMemcpyAsync(h_fv + (size_t)s0 * Wf * kFeatC, d_fv, (size_t)n * Wf * kFeatC * sizeof(float),
+                                cudaMemcpyDeviceToHost, s));
+    rc = check_device_error(h, s);           // synchronises s
+    if (rc != OVN_OK) return rc;
   }
-  cudaFree(d_fv);
-  return rc;
+  return OVN_OK;
 }
 
 int ovn_query_cloud_vs_bank_host(ovn_handle* h, const float* h_points, int64_t n_points, const float* d_bank,
@@ -841,17 +827,14 @@ int ovn_query_cloud_vs_bank_host(ovn_handle* h, const float* h_points, int64_t n
   if (n_cand > h->cfg.max_batch_pairs)
     OVN_SET_ERR(h, OVN_ERR_CAPACITY, "n_cand=%d exceeds max_batch_pairs=%d", n_cand, h->cfg.max_batch_pairs);
   cudaStream_t s = h->own_stream;
-  int rc = ensure_stage(h, n_points, 1);
+  int rc = ensure_stage(h, n_points);
   if (rc != OVN_OK) return rc;
   const int Wf = h->cfg.leg_output_width;
-  const int maxp = h->cfg.max_batch_pairs;
-  // pinned staging: [0,64) error flag + the two offsets; then cand idx / overlap / yaw (4 B x max_batch_pairs each).
-  // Everything the device reads or writes asynchronously lives there, so the call has ONE host sync.
-  uint8_t* pin = reinterpret_cast<uint8_t*>(h->h_pinned);
-  int64_t* p_offs = reinterpret_cast<int64_t*>(pin + 16);
-  int32_t* p_idx = reinterpret_cast<int32_t*>(pin + 64);
-  float* p_ov = reinterpret_cast<float*>(pin + 64 + (size_t)maxp * 4);
-  int32_t* p_yaw = reinterpret_cast<int32_t*>(pin + 64 + (size_t)maxp * 8);
+  // Everything the device reads or writes asynchronously lives in the pinned staging, so the call has ONE host sync.
+  int64_t* p_offs = h->stage()->offsets;
+  int32_t* p_idx = h->stage_cand_idx();
+  float* p_ov = h->stage_overlap();
+  int32_t* p_yaw = h->stage_yaw();
   p_offs[0] = 0; p_offs[1] = n_points;
   // the bank's operand copies may have been prepared on another stream (ovn_bank_prepare records ev_bank)
   OVN_CUDA(h, cudaStreamWaitEvent(s, h->ev_bank, 0));
@@ -859,22 +842,22 @@ int ovn_query_cloud_vs_bank_host(ovn_handle* h, const float* h_points, int64_t n
   OVN_CUDA(h, cudaMemcpyAsync(h->d_stage_offsets, p_offs, 2 * sizeof(int64_t), cudaMemcpyHostToDevice, s));
   if (h_cand_idx && n_cand > 0) {
     memcpy(p_idx, h_cand_idx, (size_t)n_cand * sizeof(int32_t));
-    OVN_CUDA(h, cudaMemcpyAsync(h->d_idx_tmp, p_idx, (size_t)n_cand * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    OVN_CUDA(h, cudaMemcpyAsync(h->d_cand_idx, p_idx, (size_t)n_cand * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   }
   rc = preprocess_batch(h, h->d_stage_points, h->d_stage_offsets, 1, n_points, nullptr, h->d_input, s);
   if (rc != OVN_OK) return rc;
   rc = ovn_leg_forward(h, h->d_input, 1, h->d_query_fv, s);
   if (rc != OVN_OK) return rc;
   if (n_cand > 0) {
-    int32_t* d_yaw = h->d_idx_tmp + maxp;
     if (!h_cand_idx) {
-      k_iota<<<(n_cand + 255) / 256, 256, 0, s>>>(h->d_idx_tmp, n_cand, 0);
+      k_iota<<<(n_cand + 255) / 256, 256, 0, s>>>(h->d_cand_idx, n_cand, 0);
       OVN_LAUNCH_CHECK(h);
     }
-    rc = heads_dispatch(h, d_bank, bank_size, h->d_query_fv, h->d_idx_tmp, nullptr, n_cand, h->d_logit, d_yaw, nullptr, s);
+    rc = heads_dispatch(h, d_bank, bank_size, h->d_query_fv, h->d_cand_idx, nullptr, n_cand, h->d_query_overlap,
+                        h->d_query_yaw, nullptr, s);
     if (rc != OVN_OK) return rc;
-    OVN_CUDA(h, cudaMemcpyAsync(p_ov, h->d_logit, (size_t)n_cand * sizeof(float), cudaMemcpyDeviceToHost, s));
-    OVN_CUDA(h, cudaMemcpyAsync(p_yaw, d_yaw, (size_t)n_cand * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    OVN_CUDA(h, cudaMemcpyAsync(p_ov, h->d_query_overlap, (size_t)n_cand * sizeof(float), cudaMemcpyDeviceToHost, s));
+    OVN_CUDA(h, cudaMemcpyAsync(p_yaw, h->d_query_yaw, (size_t)n_cand * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   }
   if (h_query_fv)
     OVN_CUDA(h, cudaMemcpyAsync(h_query_fv, h->d_query_fv, (size_t)Wf * kFeatC * sizeof(float), cudaMemcpyDeviceToHost, s));

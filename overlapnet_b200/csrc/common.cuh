@@ -2,15 +2,69 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
+#include <stddef.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <memory>
 #include <string>
 #include <vector>
 #include <map>
 
 #include "../../include/ovn_b200.h"
 
+struct ovn_handle;
+
 namespace ovn {
+
+// The one owner of a cudaMalloc'ed block (cudaHostAlloc'ed when Pinned) of T; frees it on destruction.
+// Converts to T* so that kernels and runtime calls take it as a plain pointer.  ensure() is the only place
+// where the block and its capacity change; `buf = {}` hands the block to a temporary that frees it.
+template <class T, bool Pinned = false>
+class Buffer {
+ public:
+  Buffer() = default;
+  Buffer(Buffer&& o) noexcept { swap(o); }
+  Buffer& operator=(Buffer&& o) noexcept {
+    Buffer old(std::move(o));
+    swap(old);
+    return *this;
+  }
+  ~Buffer() {
+    if (!p_) return;
+    if (Pinned) cudaFreeHost(p_);
+    else cudaFree(p_);
+  }
+  operator T*() const { return p_; }
+  T* get() const { return p_; }
+  size_t bytes() const { return cap_; }
+  // At least `bytes` bytes; a grow frees the old block (cudaFree synchronises the device) and allocates
+  // max(bytes, reserve).  On failure the buffer is empty and the CUDA error is consumed, so the handle
+  // stays usable.
+  int ensure(ovn_handle* h, size_t bytes, size_t reserve = 0);
+
+ private:
+  void swap(Buffer& o) {
+    std::swap(p_, o.p_);
+    std::swap(cap_, o.cap_);
+  }
+  T* p_ = nullptr;
+  size_t cap_ = 0;
+};
+template <class T> using PinnedBuffer = Buffer<T, true>;
+
+// Head of ovn_handle::h_pinned, the pinned staging of the host entry points; the candidate indices, overlaps
+// and yaws of ovn_query_cloud_vs_bank_host follow it (ovn_handle::stage_*).
+struct StageHeader {
+  int32_t err;                   // ovn_handle::d_err, copied back by check_device_error
+  int32_t pad0[3];
+  int64_t offsets[2];            // point offsets of the one staged cloud
+  int64_t pad1[2];
+  float loss[3];                 // ovn_head_gradients: total, overlap, orientation
+  int32_t pad2;
+};
+static_assert(offsetof(StageHeader, offsets) == 16 && offsetof(StageHeader, loss) == 48 && sizeof(StageHeader) == 64,
+              "pinned staging layout");
+static_assert(sizeof(float) == sizeof(int32_t), "the three staging arrays are 4 B per pair");
 
 constexpr int kFeatC = 128;           // leg output channels (generateNet.py:214)
 constexpr int kMaxLegLayers = 12;
@@ -34,22 +88,23 @@ struct LayerWeights {
 
 namespace ovn {
 struct TcState;
+struct TcStateDelete { void operator()(TcState* t) const; };   // network_tc.cu: TcState is private to it
 
 // Training of the overlap head (fp32 handles; allocated when a handle first trains, sized by max_batch_pairs).
 // Gradients and Adagrad accumulators of c_conv1..3 / overlap_output: per layer [K + 1][N] floats at off[l]
 // (the kernel in Keras layout, then the bias).
 struct TrainState {
-  float* x4 = nullptr;          // [max_batch_pairs][dense_in] c_conv3 output, then dL/d(its pre-activation)
-  float* dx3 = nullptr;         // [max_batch_pairs][24][24][128] dL/dx3, then dL/d(pre-activation of c_conv2)
-  float* corr = nullptr;        // [max_batch_pairs][Wf] orientation logits
-  float* overlap = nullptr;     // [max_batch_pairs]
-  float* dz = nullptr;          // [max_batch_pairs] dL/d(Dense logit)
-  int32_t* yaw = nullptr;       // [max_batch_pairs]
-  float* w3t = nullptr;         // c_conv3 kernel with in / out swapped
-  float* part = nullptr;        // split-K partials of the weight gradients
-  float* grad = nullptr;        // [n_param]
-  float* accum = nullptr;       // [n_param] Adagrad accumulators
-  float* loss = nullptr;        // [3] total, overlap, orientation
+  Buffer<float> x4;             // [max_batch_pairs][dense_in] c_conv3 output, then dL/d(its pre-activation)
+  Buffer<float> dx3;            // [max_batch_pairs][24][24][128] dL/dx3, then dL/d(pre-activation of c_conv2)
+  Buffer<float> corr;           // [max_batch_pairs][Wf] orientation logits
+  Buffer<float> overlap;        // [max_batch_pairs]
+  Buffer<float> dz;             // [max_batch_pairs] dL/d(Dense logit)
+  Buffer<int32_t> yaw;          // [max_batch_pairs]
+  Buffer<float> w3t;            // c_conv3 kernel with in / out swapped
+  Buffer<float> part;           // split-K partials of the weight gradients
+  Buffer<float> grad;           // [n_param]
+  Buffer<float> accum;          // [n_param] Adagrad accumulators
+  Buffer<float> loss;           // [3] total, overlap, orientation
   int64_t off[4] = {};
   int64_t n_param = 0;
   bool grads_valid = false;     // the last ovn_head_gradients succeeded
@@ -78,44 +133,44 @@ struct ovn_handle {
   std::string net_error;
 
   // device weights, fp32 GEMM layout [K][N] (K = kh*kw*cin, Keras HWIO flattened is already that)
-  float* d_w[ovn::kMaxLegLayers + 4] = {};
-  float* d_b[ovn::kMaxLegLayers + 4] = {};
-  // fp16 packed weights for the tensor-core path (layout documented in network_tc.cu)
-  __half* d_w16[ovn::kMaxLegLayers + 4] = {};
+  ovn::Buffer<float> d_w[ovn::kMaxLegLayers + 4];
+  ovn::Buffer<float> d_b[ovn::kMaxLegLayers + 4];
 
-  // workspaces
-  unsigned long long* d_keys = nullptr;      // [max_batch_scans][H*W] atomic-min keys
-  unsigned long long* d_pair_keys = nullptr; // ovn_gt_pairs_count: [tile_cur][tile_ref][H*W] keys, allocated on first use
-  size_t cap_pair_keys = 0;
-  uint8_t* d_pair_prune = nullptr;           // ovn_gt_pairs_count: pruned-pair counter + [n_cur][n_ref] flags
-  size_t cap_pair_prune = 0;
-  uint32_t* d_valid_words = nullptr;         // validity bitmask, 1 bit per point
-  uint32_t* d_word_prefix = nullptr;         // exclusive prefix of popcounts
-  uint32_t* d_scan_tmp = nullptr;
-  int64_t cap_points = 0;
-  float* d_act[2] = {nullptr, nullptr};      // ping-pong activations for the leg
-  int64_t cap_act = 0;
-  float* d_input = nullptr;                  // [max_batch_scans][H][W][C]
-  float* d_o1 = nullptr;                     // [max_batch_pairs][360][24][64]
-  float* d_o2 = nullptr;                     // [max_batch_pairs][24][24][128]
-  float* d_logit = nullptr;                  // [max_batch_pairs]
-  float* d_G = nullptr;                      // [max_batch_pairs][360][360] (fp32 path corr)
-  int32_t* d_idx_tmp = nullptr;              // [max_batch_pairs] x2 scratch for 1vsN index lists
-  int32_t* d_idx_san = nullptr;              // [max_batch_pairs] x2 bounds-checked (clamped) copies of the caller's index lists
-  int* d_err = nullptr;                      // device error flag: pipeline barrier time-outs (1xx-8xx), bad indices (9xx)
+  // workspaces, allocated by ovn_create unless noted
+  ovn::Buffer<unsigned long long> d_keys;    // [max_batch_scans][H*W] atomic-min keys
+  ovn::Buffer<unsigned long long> d_pair_keys; // ovn_gt_pairs_count: [tile_cur][tile_ref][H*W] keys, grown on use
+  ovn::Buffer<uint8_t> d_pair_prune;         // ovn_gt_pairs_count: pruned-pair counter + [n_cur][n_ref] flags, grown on use
+  ovn::Buffer<uint32_t> d_valid_words;       // validity bitmask, 1 bit per point; these three grow with the points
+  ovn::Buffer<uint32_t> d_word_prefix;       //   of projections that return per-point indices
+  ovn::Buffer<uint32_t> d_scan_tmp;          //   (exclusive prefix of popcounts, block sums)
+  ovn::Buffer<float> d_act[2];               // ping-pong activations for the fp32 leg (f16_tc: layer 1 fallback)
+  ovn::Buffer<float> d_input;                // [max_batch_scans][H][W][C]
+  ovn::Buffer<float> d_o1;                   // fp32 only: [max_batch_pairs][360][24][64]
+  ovn::Buffer<float> d_o2;                   // fp32 only: [max_batch_pairs][24][24][128]
+  ovn::Buffer<float> d_G;                    // fp32 only: [max_batch_pairs][360][360] correlation Gram matrices
+  ovn::Buffer<int32_t> d_cand_idx;           // [max_batch_pairs] candidate indices of ovn_heads_1vsN / the host query
+  ovn::Buffer<int32_t> d_idx_san;            // [max_batch_pairs] x3 bounds-checked (clamped) copies of the caller's index lists
+  ovn::Buffer<int> d_err;                    // device error flag: pipeline barrier time-outs (1xx-8xx), bad indices (9xx)
   cudaEvent_t ev_bank = nullptr;             // recorded after ovn_bank_prepare: the host entry points (own stream) wait on it
-  float* d_query_fv = nullptr;               // [360][128]
-  float* d_stage_points = nullptr;           // host-entry staging of clouds
-  int64_t cap_stage_points = 0;
-  int64_t* d_stage_offsets = nullptr;
-  void* h_pinned = nullptr;                  // pinned staging for host entry points
-  int64_t cap_pinned = 0;
+  // ovn_query_cloud_vs_bank_host / ovn_encode_clouds_host
+  ovn::Buffer<float> d_query_fv;             // [360][128]
+  ovn::Buffer<float> d_query_overlap;        // [max_batch_pairs]
+  ovn::Buffer<int32_t> d_query_yaw;          // [max_batch_pairs]
+  ovn::Buffer<float> d_stage_points;         // staged clouds, grown on use
+  ovn::Buffer<int64_t> d_stage_offsets;      // [max_batch_scans + 1], allocated on first use
+  ovn::PinnedBuffer<uint8_t> h_pinned;       // StageHeader, then candidate indices / overlaps / yaws [max_batch_pairs]
   cudaStream_t own_stream = nullptr;
   // per-kernel profiling (ovn_profile_enable / ovn_profile_read)
   bool profiling = false;
   std::vector<cudaEvent_t> prof_ev[ovn::kProfKinds];   // start/stop pairs, in launch order
-  ovn::TcState* tc = nullptr;              // tensor-core path state (network_tc.cu)
-  ovn::TrainState* train = nullptr;        // overlap-head training state (network_fp32.cu), NULL until first used
+  std::unique_ptr<ovn::TcState, ovn::TcStateDelete> tc;   // tensor-core path state (network_tc.cu)
+  std::unique_ptr<ovn::TrainState> train;  // overlap-head training state (network_fp32.cu), NULL until first used
+
+  ~ovn_handle();                           // the streams and events; the buffers free themselves
+  ovn::StageHeader* stage() const { return reinterpret_cast<ovn::StageHeader*>(h_pinned.get()); }
+  int32_t* stage_cand_idx() const { return reinterpret_cast<int32_t*>(h_pinned + sizeof(ovn::StageHeader)); }
+  float* stage_overlap() const { return reinterpret_cast<float*>(stage_cand_idx() + cfg.max_batch_pairs); }
+  int32_t* stage_yaw() const { return reinterpret_cast<int32_t*>(stage_overlap() + cfg.max_batch_pairs); }
 };
 
 #define OVN_SET_ERR(h, code, ...)                                 \
@@ -126,10 +181,13 @@ struct ovn_handle {
     return (code);                                                \
   } while (0)
 
+// A failed runtime call is reported once: its error is consumed, so the next OVN_LAUNCH_CHECK does not blame
+// a kernel launch for it.
 #define OVN_CUDA(h, call)                                                                   \
   do {                                                                                      \
     cudaError_t _e = (call);                                                                \
     if (_e != cudaSuccess) {                                                                \
+      cudaGetLastError();                                                                   \
       OVN_SET_ERR(h, OVN_ERR_CUDA, "%s failed at %s:%d: %s", #call, __FILE__, __LINE__,     \
                   cudaGetErrorString(_e));                                                  \
     }                                                                                       \
@@ -146,6 +204,19 @@ struct ovn_handle {
   } while (0)
 
 namespace ovn {
+
+template <class T, bool Pinned>
+int Buffer<T, Pinned>::ensure(ovn_handle* h, size_t bytes, size_t reserve) {
+  if (bytes <= cap_) return OVN_OK;
+  *this = {};                           // free the old block first: the new one may need its memory
+  if (reserve < bytes) reserve = bytes;
+  void* p = nullptr;
+  if (Pinned) OVN_CUDA(h, cudaHostAlloc(&p, reserve, cudaHostAllocDefault));
+  else OVN_CUDA(h, cudaMalloc(&p, reserve));
+  p_ = static_cast<T*>(p);
+  cap_ = reserve;
+  return OVN_OK;
+}
 
 // Every ABI entry point runs on the device its handle was created on (ADVICE r1: Engine(device=1)
 // with another current device allocated on the wrong GPU).
@@ -169,6 +240,17 @@ inline void prof_mark(ovn_handle* h, int kind, cudaStream_t s) {
   if (cudaEventCreate(&e) != cudaSuccess) return;
   cudaEventRecord(e, s);
   h->prof_ev[kind].push_back(e);
+}
+
+// dst = a device copy of v, in a fresh block: freeing the old one synchronises the device, so no queued
+// kernel still reads it while it is overwritten
+template <class T>
+int upload_vec(ovn_handle* h, Buffer<T>& dst, const std::vector<T>& v) {
+  dst = {};
+  const int rc = dst.ensure(h, v.size() * sizeof(T));
+  if (rc != OVN_OK) return rc;
+  OVN_CUDA(h, cudaMemcpy(dst, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+  return OVN_OK;
 }
 
 // ---- stage entry points implemented in the .cu files (called from api.cu) -------------------
@@ -203,7 +285,6 @@ int heads_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query,
 
 // training of the overlap head (network_fp32.cu)
 int train_alloc(ovn_handle* h);
-void train_free(ovn_handle* h);
 int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left, const int32_t* right, int np,
                         const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
                         cudaStream_t s);
@@ -219,7 +300,6 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query,
 int tc_pack_weights(ovn_handle* h);
 int tc_bank_prepare(ovn_handle* h, const float* d_bank, int64_t capacity, int64_t first, int64_t count, cudaStream_t s);
 int tc_bank_release(ovn_handle* h, const float* d_bank);
-void tc_free(ovn_handle* h);
 int tc_set_center(ovn_handle* h, const float* h_mu);
 int tc_get_center(ovn_handle* h, float* h_mu, int32_t* is_set);
 int tc_calibrate(ovn_handle* h, const float* d_volume, cudaStream_t s);

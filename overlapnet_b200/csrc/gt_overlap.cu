@@ -299,21 +299,12 @@ int gt_pairs_count(ovn_handle* h, const float* d_points, const int64_t* h_offset
   if (n_cur == 0 || n_ref == 0) return OVN_OK;
   // workspaces, allocated by the first call that needs them
   const size_t key_bytes = (size_t)tc * tr * HW * sizeof(unsigned long long);
-  if (key_bytes > h->cap_pair_keys) {
-    if (h->d_pair_keys) cudaFree(h->d_pair_keys);
-    h->d_pair_keys = nullptr; h->cap_pair_keys = 0;
-    OVN_CUDA(h, cudaMalloc(&h->d_pair_keys, key_bytes));
-    h->cap_pair_keys = key_bytes;
-  }
-  const size_t prune_bytes = (size_t)n_cur * n_ref + sizeof(unsigned long long);
-  if (prune_bytes > h->cap_pair_prune) {
-    if (h->d_pair_prune) cudaFree(h->d_pair_prune);
-    h->d_pair_prune = nullptr; h->cap_pair_prune = 0;
-    OVN_CUDA(h, cudaMalloc(&h->d_pair_prune, prune_bytes));
-    h->cap_pair_prune = prune_bytes;
-  }
+  int rc = h->d_pair_keys.ensure(h, key_bytes);
+  if (rc != OVN_OK) return rc;
+  rc = h->d_pair_prune.ensure(h, (size_t)n_cur * n_ref + sizeof(unsigned long long));
+  if (rc != OVN_OK) return rc;
   // [8-byte pruned counter][n_cur][n_ref] flags
-  unsigned long long* cnt = reinterpret_cast<unsigned long long*>(h->d_pair_prune);
+  unsigned long long* cnt = reinterpret_cast<unsigned long long*>(h->d_pair_prune.get());
   uint8_t* prune = h->d_pair_prune + sizeof(unsigned long long);
   OVN_CUDA(h, cudaMemsetAsync(h->d_pair_keys, 0xFF, key_bytes, s));
   OVN_CUDA(h, cudaMemsetAsync(cnt, 0, sizeof(unsigned long long), s));

@@ -535,9 +535,11 @@ static void head_dims(const ovn_handle* h, int l, int* K, int* N) {
   else { *K = h->dense_in; *N = 1; }
 }
 
-static int train_alloc_buffers(ovn_handle* h, TrainState* t) {
+// h->train, complete or not at all
+int train_alloc(ovn_handle* h) {
   const int64_t maxp = h->cfg.max_batch_pairs, Wf = h->cfg.leg_output_width;
   const ConvSpec& L3 = h->head[2];
+  std::unique_ptr<TrainState> t(new TrainState());
   int64_t total = 0, max_part = 0;
   for (int l = 0; l < 4; ++l) {
     int K, N;
@@ -547,35 +549,21 @@ static int train_alloc_buffers(ovn_handle* h, TrainState* t) {
     if (l < 3 && (int64_t)(K + 1) * N > max_part) max_part = (int64_t)(K + 1) * N;
   }
   t->n_param = total;
-  OVN_CUDA(h, cudaMalloc(&t->x4, (size_t)maxp * h->dense_in * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->dx3, (size_t)maxp * L3.h_in * L3.w_in * L3.cin * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->corr, (size_t)maxp * Wf * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->overlap, (size_t)maxp * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->dz, (size_t)maxp * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->yaw, (size_t)maxp * sizeof(int32_t)));
-  OVN_CUDA(h, cudaMalloc(&t->w3t, (size_t)L3.kh * L3.kw * L3.cin * L3.cout * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->part, (size_t)kMaxSplit * max_part * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->grad, (size_t)total * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->accum, (size_t)total * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->loss, 4 * sizeof(float)));
+  int rc;
+  if ((rc = t->x4.ensure(h, (size_t)maxp * h->dense_in * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t->dx3.ensure(h, (size_t)maxp * L3.h_in * L3.w_in * L3.cin * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t->corr.ensure(h, (size_t)maxp * Wf * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t->overlap.ensure(h, (size_t)maxp * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t->dz.ensure(h, (size_t)maxp * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t->yaw.ensure(h, (size_t)maxp * sizeof(int32_t))) != OVN_OK) return rc;
+  if ((rc = t->w3t.ensure(h, (size_t)L3.kh * L3.kw * L3.cin * L3.cout * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t->part.ensure(h, (size_t)kMaxSplit * max_part * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t->grad.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t->accum.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t->loss.ensure(h, 4 * sizeof(float))) != OVN_OK) return rc;
   OVN_CUDA(h, cudaMemset(t->accum, 0, (size_t)total * sizeof(float)));
+  h->train = std::move(t);
   return OVN_OK;
-}
-
-int train_alloc(ovn_handle* h) {
-  h->train = new TrainState();
-  const int rc = train_alloc_buffers(h, h->train);
-  if (rc != OVN_OK) train_free(h);
-  return rc;
-}
-
-void train_free(ovn_handle* h) {
-  TrainState* t = h->train;
-  if (!t) return;
-  void* bufs[] = {t->x4, t->dx3, t->corr, t->overlap, t->dz, t->yaw, t->w3t, t->part, t->grad, t->accum, t->loss};
-  for (void* b : bufs) if (b) cudaFree(b);
-  delete t;
-  h->train = nullptr;
 }
 
 // [Kc + 1][N] weight + bias gradient = A^T dY summed over Kred rows, split over K in fixed slices

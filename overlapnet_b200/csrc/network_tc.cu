@@ -36,43 +36,45 @@ constexpr int PAIR_ROWS = NB * NB;      // 576 rows of c_conv2 output per pair
 constexpr int K4_PITCH = CF;            // fp16 row pitch of the L / R operand copies of k_delta_conv1_wgmma (k4_pos)
 
 struct TcState {
-  __half* w1p = nullptr;        // [60 steps][4][64][8]
-  __half* w2p = nullptr;        // [15 di][hi, lo][128 n][64 o] SWIZZLE_128B tiles (W2 = hi + lo in fp16)
-  __half* w3p = nullptr;        // [2 halves][36 slabs][4][128][8]
-  float* b2eff = nullptr;       // c_conv2 bias + the c_conv1 bias pushed through W2 (both layers are linear)
+  Buffer<__half> w1p;           // [60 steps][4][64][8]
+  Buffer<__half> w2p;           // [15 di][hi, lo][128 n][64 o] SWIZZLE_128B tiles (W2 = hi + lo in fp16)
+  Buffer<__half> w3p;           // [2 halves][36 slabs][4][128][8]
+  Buffer<float> b2eff;          // c_conv2 bias + the c_conv1 bias pushed through W2 (both layers are linear)
   // tensor-core leg (layers 2..): packed weights per layer, ping-pong activation planes
-  __half* wres[kMaxLegLayers] = {};      // [cout/64][kh*kw*3 slabs (tap, term)][C_in/8][64][8]; term 0, 1 = hi, 2 = lo
-  __half* actp[2] = {nullptr, nullptr};
-  float* leg_part = nullptr;    // K-slice sums of the single-scan leg: [n_split][rows][w_out][cout] fp32
-  __half* l16 = nullptr;        // [max_pairs][360][128]
-  __half* r16 = nullptr;        // [max_pairs][360][128] (pair mode) / [1][360][128] (query mode)
-  __half* o1 = nullptr;         // [rows_pad/128][15 di][128][64]: SWIZZLE_128B A tiles of c_conv2 (o1_chunk_offset)
-  __half* x3 = nullptr;         // [16 planes][rows_pad][8], row = pair*576 + jb*24 + ib
-  float* partial = nullptr;     // [rows_pad][2]
-  __half* lc = nullptr;         // correlation operands: [max_pairs][6 tiles][hi,lo][16][64][8]
-  __half* rc = nullptr;         // [max_pairs or 1][3 thirds][hi,lo][16][128][8]
-  float* corr_part = nullptr;   // [max_pairs][6 LEFT tiles][3 RIGHT thirds][360]
+  Buffer<__half> wres[kMaxLegLayers];    // [cout/64][kh*kw*3 slabs (tap, term)][C_in/8][64][8]; term 0, 1 = hi, 2 = lo
+  Buffer<__half> actp[2];
+  Buffer<float> leg_part;       // K-slice sums of the single-scan leg: [n_split][rows][w_out][cout] fp32
+  Buffer<__half> l16;           // [max_pairs][360][128]
+  Buffer<__half> r16;           // [max_pairs][360][128] (pair mode) / [1][360][128] (query mode)
+  Buffer<__half> o1;            // [rows_pad/128][15 di][128][64]: SWIZZLE_128B A tiles of c_conv2 (o1_chunk_offset)
+  Buffer<__half> x3;            // [16 planes][rows_pad][8], row = pair*576 + jb*24 + ib
+  Buffer<float> partial;        // [rows_pad][2]
+  Buffer<__half> lc;            // correlation operands: [max_pairs][6 tiles][hi,lo][16][64][8]
+  Buffer<__half> rc;            // [max_pairs or 1][3 thirds][hi,lo][16][128][8]
+  Buffer<float> corr_part;      // [max_pairs][6 LEFT tiles][3 RIGHT thirds][360]
   // resident bank (ovn_bank_prepare): operand copies of the LEFT volumes, indexed by bank row
   const float* pb_key = nullptr;
-  int64_t pb_cap = 0, pb_rows = 0;      // capacity / rows [0, pb_rows) prepared
-  __half* pb_l16 = nullptr;             // [cap][360][K4_PITCH]
-  __half* pb_lc = nullptr;              // [cap] x C6_VOL_L_BYTES
+  int64_t pb_rows = 0;                  // rows [0, pb_rows) prepared
+  Buffer<__half> pb_l16;                // [cap][360][K4_PITCH]
+  Buffer<__half> pb_lc;                 // [cap] x C6_VOL_L_BYTES
   // per-channel centre of the feature volumes: the delta head only sees |l - r|, which is invariant
   // to a common offset, so both operands are stored as fp16(x - mu[c]) -- smaller magnitudes, smaller
   // fp16 rounding error of the (coherently re-used) volumes.  mu is calibrated once (first bank rows /
   // first RIGHT volume seen) or set through ovn_set_feature_center; values are fp16-representable.
-  float* mu = nullptr;          // [128] device
+  Buffer<float> mu;             // [128] device
   bool mu_set = false;
   // The same trick one and two layers further on: c_conv2 and c_conv3 are linear in their inputs, so
   // o1 and x3 are stored as fp16(x - mean[channel]) and the mean's image under the layer is folded into
   // that layer's bias (b2eff / b3eff).  Calibrated on the first pairs the handle scores.
-  float* mu_o1 = nullptr;       // [64]
-  float* mu_x3 = nullptr;       // [128]
-  float* b2base = nullptr;      // c_conv2 bias + c_conv1 bias pushed through W2
-  float* b3eff = nullptr;       // c_conv3 bias + mu_x3 pushed through the fp16 W3
+  Buffer<float> mu_o1;          // [64]
+  Buffer<float> mu_x3;          // [128]
+  Buffer<float> b2base;         // c_conv2 bias + c_conv1 bias pushed through W2
+  Buffer<float> b3eff;          // c_conv3 bias + mu_x3 pushed through the fp16 W3
   bool act_set = false;
   int64_t rows_pad = 0;
 };
+
+void TcStateDelete::operator()(TcState* t) const { delete t; }
 
 // ------------------------------------------------------------------------------------------------
 // fp32 feature volumes -> fp16 rows gathered by index (the tensor-core operands)
@@ -1215,32 +1217,6 @@ static int tc_supported(const ovn_handle* h) {
   return h->net_ok && h->cfg.leg_output_width == WF && h->cfg.conv1size == S15;
 }
 
-void tc_free(ovn_handle* h) {
-  TcState* t = h->tc;
-  if (!t) return;
-  void* bufs[] = {t->w1p, t->w2p, t->w3p, t->b2eff,
-                  t->l16, t->r16, t->o1, t->x3, t->partial, t->mu, t->lc, t->rc, t->corr_part,
-                  t->mu_o1, t->mu_x3, t->b2base, t->b3eff};
-  for (void* b : bufs) if (b) cudaFree(b);
-  for (int l = 0; l < kMaxLegLayers; ++l) {
-    if (t->wres[l]) cudaFree(t->wres[l]);
-  }
-  if (t->pb_l16) cudaFree(t->pb_l16);
-  if (t->pb_lc) cudaFree(t->pb_lc);
-  if (t->actp[0]) cudaFree(t->actp[0]);
-  if (t->actp[1]) cudaFree(t->actp[1]);
-  if (t->leg_part) cudaFree(t->leg_part);
-  delete t;
-  h->tc = nullptr;
-}
-
-template <class T>
-static int upload_vec(ovn_handle* h, T** dst, const std::vector<T>& v) {
-  OVN_CUDA(h, cudaMalloc(dst, v.size() * sizeof(T)));
-  OVN_CUDA(h, cudaMemcpy(*dst, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-  return OVN_OK;
-}
-
 // K slices of a leg layer (2..) for n scans.  A single scan gives layers 3.. only 14-42 output tiles of 64 pixels
 // x 64 channels for 132 SMs, each a chain of up to 144 K iterations whose loads miss a cold L2; n <= 2 (the
 // threshold of k_leg_layer1_small) splits K into slices of >= 4 iterations, up to about 4 CTAs per SM.
@@ -1257,9 +1233,10 @@ static int leg_split(const ovn_handle* h, const ConvSpec& L, int n) {
 int tc_pack_weights(ovn_handle* h) {
   if (!tc_supported(h))
     OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "precision f16_tc supports leg_output_width=360, conv1size=15 only");
-  tc_free(h);
-  TcState* t = new TcState();
-  h->tc = t;
+  // h->tc, complete or not at all: a failed re-pack leaves no half-built state for the heads to read.  The old
+  // state is freed first, so that the new one can use its memory.
+  h->tc.reset();
+  std::unique_ptr<TcState, TcStateDelete> t(new TcState());
   const LayerWeights& w1 = h->host_w["c_conv1"];   // (1,15,128,64)
   const LayerWeights& w2 = h->host_w["c_conv2"];   // (15,1,64,128)
   const LayerWeights& w3 = h->host_w["c_conv3"];   // (3,3,128,256)
@@ -1315,16 +1292,16 @@ int tc_pack_weights(ovn_handle* h) {
     }
   }
   int rc;
-  if ((rc = upload_vec(h, &t->b2eff, b2e)) != OVN_OK) return rc;
-  if ((rc = upload_vec(h, &t->b2base, b2e)) != OVN_OK) return rc;
-  if ((rc = upload_vec(h, &t->b3eff, w3.bias)) != OVN_OK) return rc;
-  OVN_CUDA(h, cudaMalloc(&t->mu_o1, 64 * sizeof(float)));
+  if ((rc = upload_vec(h, t->b2eff, b2e)) != OVN_OK) return rc;
+  if ((rc = upload_vec(h, t->b2base, b2e)) != OVN_OK) return rc;
+  if ((rc = upload_vec(h, t->b3eff, w3.bias)) != OVN_OK) return rc;
+  if ((rc = t->mu_o1.ensure(h, 64 * sizeof(float))) != OVN_OK) return rc;
   OVN_CUDA(h, cudaMemset(t->mu_o1, 0, 64 * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->mu_x3, 128 * sizeof(float)));
+  if ((rc = t->mu_x3.ensure(h, 128 * sizeof(float))) != OVN_OK) return rc;
   OVN_CUDA(h, cudaMemset(t->mu_x3, 0, 128 * sizeof(float)));
-  if ((rc = upload_vec(h, &t->w1p, p1)) != OVN_OK) return rc;
-  if ((rc = upload_vec(h, &t->w2p, p2)) != OVN_OK) return rc;
-  if ((rc = upload_vec(h, &t->w3p, p3)) != OVN_OK) return rc;
+  if ((rc = upload_vec(h, t->w1p, p1)) != OVN_OK) return rc;
+  if ((rc = upload_vec(h, t->w2p, p2)) != OVN_OK) return rc;
+  if ((rc = upload_vec(h, t->w3p, p3)) != OVN_OK) return rc;
   // ---- leg layers 2.. : weights as (tap, term) slabs.  Three-term split product
   // x*w ~= xh*wh + xl*wh + xh*wl  (x = xh + xl, w = wh + wl in fp16): slab = (dh, dw, term)
   size_t max_planes_bytes = 0;
@@ -1357,7 +1334,7 @@ int tc_pack_weights(ovn_handle* h) {
                     br[((((size_t)z * nsl + sl) * c8in + c8) * 64 + n) * 8 + k] = (term == 2) ? wl : wh;
                   }
             }
-      if ((rc2 = upload_vec(h, &t->wres[l], br)) != OVN_OK) return rc2;
+      if ((rc2 = upload_vec(h, t->wres[l], br)) != OVN_OK) return rc2;
     }
   }
   size_t part_bytes = 0;
@@ -1368,35 +1345,36 @@ int tc_pack_weights(ovn_handle* h) {
       const size_t b = sp > 1 ? (size_t)sp * n * L.h_out * L.w_out * L.cout * sizeof(float) : 0;
       if (b > part_bytes) part_bytes = b;
     }
-  if (part_bytes) OVN_CUDA(h, cudaMalloc(&t->leg_part, part_bytes));
+  if ((rc = t->leg_part.ensure(h, part_bytes)) != OVN_OK) return rc;
   for (int b = 0; b < 2; ++b) {
     const size_t bytes = max_planes_bytes * h->cfg.max_batch_scans + 32768;   // + tile overrun slack
-    OVN_CUDA(h, cudaMalloc(&t->actp[b], bytes));
+    if ((rc = t->actp[b].ensure(h, bytes)) != OVN_OK) return rc;
     OVN_CUDA(h, cudaMemset(t->actp[b], 0, bytes));
   }
   const int64_t maxp = h->cfg.max_batch_pairs;
   // + slack for the last 256-row tile of c_conv2 / c_conv3 (255 rows) and c_conv3's window (50 rows); whole tiles
   t->rows_pad = ((maxp * PAIR_ROWS + 1024 + 255) / 256) * 256;
-  OVN_CUDA(h, cudaMalloc(&t->l16, (size_t)maxp * WF * K4_PITCH * sizeof(__half)));
-  OVN_CUDA(h, cudaMalloc(&t->r16, (size_t)maxp * WF * K4_PITCH * sizeof(__half)));
+  if ((rc = t->l16.ensure(h, (size_t)maxp * WF * K4_PITCH * sizeof(__half))) != OVN_OK) return rc;
+  if ((rc = t->r16.ensure(h, (size_t)maxp * WF * K4_PITCH * sizeof(__half))) != OVN_OK) return rc;
   OVN_CUDA(h, cudaMemset(t->l16, 0, (size_t)maxp * WF * K4_PITCH * sizeof(__half)));
   OVN_CUDA(h, cudaMemset(t->r16, 0, (size_t)maxp * WF * K4_PITCH * sizeof(__half)));
-  OVN_CUDA(h, cudaMalloc(&t->o1, (size_t)120 * t->rows_pad * 8 * sizeof(__half)));
-  OVN_CUDA(h, cudaMalloc(&t->x3, (size_t)16 * t->rows_pad * 8 * sizeof(__half)));
-  OVN_CUDA(h, cudaMalloc(&t->partial, (size_t)t->rows_pad * 2 * sizeof(float)));
-  OVN_CUDA(h, cudaMalloc(&t->lc, (size_t)maxp * C6_VOL_L_BYTES));
-  OVN_CUDA(h, cudaMalloc(&t->rc, (size_t)maxp * C6_VOL_R_BYTES));
-  OVN_CUDA(h, cudaMalloc(&t->corr_part, (size_t)maxp * C6_PARTS * WF * sizeof(float)));
+  if ((rc = t->o1.ensure(h, (size_t)120 * t->rows_pad * 8 * sizeof(__half))) != OVN_OK) return rc;
+  if ((rc = t->x3.ensure(h, (size_t)16 * t->rows_pad * 8 * sizeof(__half))) != OVN_OK) return rc;
+  if ((rc = t->partial.ensure(h, (size_t)t->rows_pad * 2 * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t->lc.ensure(h, (size_t)maxp * C6_VOL_L_BYTES)) != OVN_OK) return rc;
+  if ((rc = t->rc.ensure(h, (size_t)maxp * C6_VOL_R_BYTES)) != OVN_OK) return rc;
+  if ((rc = t->corr_part.ensure(h, (size_t)maxp * C6_PARTS * WF * sizeof(float))) != OVN_OK) return rc;
   OVN_CUDA(h, cudaFuncSetAttribute(k_delta_conv1_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K4Smem)));
   OVN_CUDA(h, cudaFuncSetAttribute(k_conv2_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM));
   OVN_CUDA(h, cudaFuncSetAttribute(k_conv3_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(C3Smem)));
   OVN_CUDA(h, cudaFuncSetAttribute(k_corr_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(C6Smem)));
-  OVN_CUDA(h, cudaMalloc(&t->mu, CF * sizeof(float)));
+  if ((rc = t->mu.ensure(h, CF * sizeof(float))) != OVN_OK) return rc;
   OVN_CUDA(h, cudaMemset(t->mu, 0, CF * sizeof(float)));
   OVN_CUDA(h, cudaMemset(t->o1, 0, (size_t)120 * t->rows_pad * 8 * sizeof(__half)));
   OVN_CUDA(h, cudaMemset(t->x3, 0, (size_t)16 * t->rows_pad * 8 * sizeof(__half)));
   OVN_CUDA(h, cudaFuncSetAttribute(k_leg_layer1_small<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   OVN_CUDA(h, cudaFuncSetAttribute(k_leg_layer1_small<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  h->tc = std::move(t);
   return OVN_OK;
 }
 
@@ -1426,7 +1404,7 @@ k_nhwc_to_planes(const float* __restrict__ x, int64_t total_chunks, int H, int W
 int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cudaStream_t s) {
   // layer 1 (C_in = 4..25, stride (2,2), N = 16: K = 16 per MMA would be mostly padding) runs on the
   // direct SIMT kernels and writes hi/lo fp16 C8-interleaved planes; layers 2.. run on k_leg_mma.
-  TcState* t = h->tc;
+  TcState* t = h->tc.get();
   if (!t) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "tensor-core weights not packed");
   prof_mark(h, PROF_LEG, s);
   {
@@ -1493,27 +1471,28 @@ int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cuda
 static int calibrate_all(ovn_handle* h, const float* d_vols, const int32_t* d_idx, bool keep_mu, cudaStream_t s);
 
 int tc_bank_release(ovn_handle* h, const float* d_bank) {
-  TcState* t = h->tc;
+  TcState* t = h->tc.get();
   if (!t || (d_bank && t->pb_key != d_bank)) return OVN_OK;
   OVN_CUDA(h, cudaDeviceSynchronize());
-  if (t->pb_l16) cudaFree(t->pb_l16);
-  if (t->pb_lc) cudaFree(t->pb_lc);
-  t->pb_l16 = t->pb_lc = nullptr;
+  t->pb_l16 = {};
+  t->pb_lc = {};
   t->pb_key = nullptr;
-  t->pb_cap = t->pb_rows = 0;
+  t->pb_rows = 0;
   return OVN_OK;
 }
 
 int tc_bank_prepare(ovn_handle* h, const float* d_bank, int64_t capacity, int64_t first, int64_t count, cudaStream_t s) {
-  TcState* t = h->tc;
+  TcState* t = h->tc.get();
   if (!t) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "tensor-core weights not packed");
-  if (t->pb_key != d_bank || capacity > t->pb_cap) {
-    if (t->pb_key != nullptr || t->pb_l16) { int rc = tc_bank_release(h, nullptr); if (rc != OVN_OK) return rc; }
-    OVN_CUDA(h, cudaMalloc(&t->pb_l16, (size_t)capacity * WF * K4_PITCH * sizeof(__half)));
-    OVN_CUDA(h, cudaMalloc(&t->pb_lc, (size_t)capacity * C6_VOL_L_BYTES));
-    OVN_CUDA(h, cudaMemsetAsync(t->pb_l16, 0, (size_t)capacity * WF * K4_PITCH * sizeof(__half), s));
+  const size_t l16_bytes = (size_t)capacity * WF * K4_PITCH * sizeof(__half);
+  if (t->pb_key != d_bank || l16_bytes > t->pb_l16.bytes()) {      // a new bank, allocated to its capacity
+    int rc = OVN_OK;
+    if (t->pb_key != nullptr || t->pb_l16) rc = tc_bank_release(h, nullptr);
+    if (rc == OVN_OK) rc = t->pb_l16.ensure(h, l16_bytes);
+    if (rc == OVN_OK) rc = t->pb_lc.ensure(h, (size_t)capacity * C6_VOL_L_BYTES);
+    if (rc != OVN_OK) return rc;
+    OVN_CUDA(h, cudaMemsetAsync(t->pb_l16, 0, l16_bytes, s));
     t->pb_key = d_bank;
-    t->pb_cap = capacity;
     t->pb_rows = 0;
     if (first != 0) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_bank_prepare: a new bank must be prepared from row 0");
   }
@@ -1543,7 +1522,7 @@ int tc_bank_prepare(ovn_handle* h, const float* d_bank, int64_t capacity, int64_
 // -> mean of x3 -> fold into b3eff.  All on the stream, fixed summation orders: two handles calibrated on
 // the same volume (e.g. every rank of a sharded bank) give bit-identical results.
 static int calibrate_all(ovn_handle* h, const float* d_vols, const int32_t* d_idx, bool keep_mu, cudaStream_t s) {
-  TcState* t = h->tc;
+  TcState* t = h->tc.get();
   const int base = kMaxLegLayers;
   const int64_t per = (int64_t)WF * CF / 4;
   if (!keep_mu) {
@@ -1580,7 +1559,7 @@ static int calibrate_all(ovn_handle* h, const float* d_vols, const int32_t* d_id
 }
 
 int tc_calibrate(ovn_handle* h, const float* d_volume, cudaStream_t s) {
-  TcState* t = h->tc;
+  TcState* t = h->tc.get();
   if (!t) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "tensor-core weights not packed");
   if (t->pb_key != nullptr)
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_calibrate: release the resident bank first (its operand copies were built "
@@ -1589,7 +1568,7 @@ int tc_calibrate(ovn_handle* h, const float* d_volume, cudaStream_t s) {
 }
 
 int tc_set_center(ovn_handle* h, const float* h_mu) {
-  TcState* t = h->tc;
+  TcState* t = h->tc.get();
   if (!t) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "tensor-core weights not packed");
   if (t->pb_key != nullptr)
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_set_feature_center: release the resident bank first (its operand copies "
@@ -1611,7 +1590,7 @@ int tc_set_center(ovn_handle* h, const float* h_mu) {
 }
 
 int tc_get_center(ovn_handle* h, float* h_mu, int32_t* is_set) {
-  TcState* t = h->tc;
+  TcState* t = h->tc.get();
   if (!t) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "tensor-core weights not packed");
   OVN_CUDA(h, cudaDeviceSynchronize());
   OVN_CUDA(h, cudaMemcpy(h_mu, t->mu, CF * sizeof(float), cudaMemcpyDeviceToHost));
@@ -1622,7 +1601,7 @@ int tc_get_center(ovn_handle* h, float* h_mu, int32_t* is_set) {
 int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* d_left,
                      const int32_t* d_right, int n, float* d_overlap, int32_t* d_yaw, float* d_corr,
                      cudaStream_t s) {
-  TcState* t = h->tc;
+  TcState* t = h->tc.get();
   if (!t) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "tensor-core weights not packed");
   const int maxp = h->cfg.max_batch_pairs;
   const int base = kMaxLegLayers;

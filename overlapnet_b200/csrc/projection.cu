@@ -432,19 +432,16 @@ k_pack_input(const float* __restrict__ depth, const float* __restrict__ normal,
 // ------------------------------------------------------------------------------------------
 // host-side drivers
 // ------------------------------------------------------------------------------------------
+// rank workspaces for n_total points; a grow leaves room for 1/8 more points + 1024.  What must fit is counted
+// in bitmask words, on purpose: the kernels use ceil(n_total / 32) words and one block sum per 1024 words, so a
+// count up to 31 points past the last grow's headroom still fits and does not reallocate.
 static int ensure_point_capacity(ovn_handle* h, int64_t n_total) {
-  if (n_total <= h->cap_points) return OVN_OK;
-  if (h->d_valid_words) cudaFree(h->d_valid_words);
-  if (h->d_word_prefix) cudaFree(h->d_word_prefix);
-  if (h->d_scan_tmp) cudaFree(h->d_scan_tmp);
-  h->d_valid_words = h->d_word_prefix = h->d_scan_tmp = nullptr;
   const int64_t cap = n_total + n_total / 8 + 1024;
-  const int64_t words = cap / 32 + 2;
-  OVN_CUDA(h, cudaMalloc(&h->d_valid_words, words * sizeof(uint32_t)));
-  OVN_CUDA(h, cudaMalloc(&h->d_word_prefix, words * sizeof(uint32_t)));
-  OVN_CUDA(h, cudaMalloc(&h->d_scan_tmp, (words / 1024 + 2) * sizeof(uint32_t)));
-  h->cap_points = cap;
-  return OVN_OK;
+  const size_t need = n_total / 32 + 2, words = cap / 32 + 2;       // bitmask words
+  int rc;
+  if ((rc = h->d_valid_words.ensure(h, need * sizeof(uint32_t), words * sizeof(uint32_t))) != OVN_OK) return rc;
+  if ((rc = h->d_word_prefix.ensure(h, need * sizeof(uint32_t), words * sizeof(uint32_t))) != OVN_OK) return rc;
+  return h->d_scan_tmp.ensure(h, (need / 1024 + 2) * sizeof(uint32_t), (words / 1024 + 2) * sizeof(uint32_t));
 }
 
 static int run_projection(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans,
@@ -467,7 +464,7 @@ static int run_projection(ovn_handle* h, const float* d_points, const int64_t* d
     prof_mark(h, PROF_SCATTER, s);
     k_project_scatter<<<(unsigned)blocks, 256, 0, s>>>(reinterpret_cast<const float4*>(d_points), d_offsets,
                                                        n_scans, n_total, P, h->d_keys,
-                                                       need_rank ? h->d_valid_words : nullptr);
+                                                       need_rank ? h->d_valid_words.get() : nullptr);
     prof_mark(h, PROF_SCATTER, s);
     OVN_LAUNCH_CHECK(h);
     if (need_rank) {

@@ -73,3 +73,20 @@ def test_product_never_imports_oracle():
       if f.endswith(('.py', '.cu', '.cuh', '.h')):
         txt = open(os.path.join(dp, f)).read()
         assert 'import oracle' not in txt and 'from oracle' not in txt, os.path.join(dp, f)
+
+
+def test_only_buffer_allocates_and_frees():
+  """Every device and pinned block is owned by ovn::Buffer (common.cuh): its class body and Buffer::ensure are
+  the only code that allocates or frees one."""
+  csrc = os.path.join(ROOT, 'overlapnet_b200', 'csrc')
+  alloc = re.compile(r'\bcuda(Malloc\w*|Free\w*|HostAlloc)\s*\(')
+  owner = re.compile(r'^class Buffer \{$.*?^\};$|^int Buffer<T, Pinned>::ensure\(.*?^\}$', re.S | re.M)
+  seen_owner = 0
+  for f in sorted(os.listdir(csrc)):
+    src = open(os.path.join(csrc, f)).read()
+    if f == 'common.cuh':
+      seen_owner = len(owner.findall(src))
+      src = owner.sub('', src)
+    code = re.sub(r'//.*', '', src)
+    assert not alloc.search(code), (f, alloc.findall(code))
+  assert seen_owner == 2

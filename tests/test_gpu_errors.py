@@ -106,6 +106,34 @@ def test_pipeline_failure_is_reported(bank_np):
   eng.close()
 
 
+def test_failed_workspace_allocation_leaves_handle_usable():
+  """A projection whose rank workspace is larger than the device is refused by cudaMalloc before any kernel
+  runs.  The handle reports OVN_ERR_CUDA once, then projects like a fresh handle: the workspace, which held
+  this cloud's capacity before the failed grow, was left empty rather than with that stale capacity, and the
+  next call does not report the old error again."""
+  from overlapnet_b200._cabi import lib
+  from overlapnet_b200.engine import _ptr
+  eng = Engine(model=MODEL, precision='f16_tc', max_batch_scans=1, max_batch_pairs=8)
+  batch = eng.upload_clouds([synth.kitti_like_cloud(0, n_points=30000)])
+  eng.project(batch)                                        # the rank workspace now has room for this cloud
+  eng.check()
+  idx = torch.empty((1, eng.H, eng.W), dtype=torch.int32, device=eng.device)
+  n_huge = 16 * torch.cuda.mem_get_info(eng.device)[1]     # validity bitmask: 4 B per 32 points, > 2x the device
+  st = lib().ovn_project_batch(eng._h, _ptr(batch.points), _ptr(batch.offsets), 1, n_huge, -1.0, None, None, None,
+                               _ptr(idx), eng._stream())
+  assert lib().ovn_status_string(st) == b'OVN_ERR_CUDA'
+  assert b'cudaMalloc' in lib().ovn_last_error(eng._h)
+  out = eng.project(batch)
+  eng.check()
+  fresh = Engine(model=MODEL, precision='f16_tc', max_batch_scans=1, max_batch_pairs=8)
+  ref = fresh.project(batch)
+  fresh.check()
+  for k in ('range', 'vertex', 'intensity', 'idx'):
+    assert torch.equal(out[k].view(torch.int32), ref[k].view(torch.int32)), k
+  eng.close()
+  fresh.close()
+
+
 def test_engine_on_non_current_device():
   """ADVICE r1: a handle is bound to its device; calls work whatever the caller's current device is."""
   if torch.cuda.device_count() < 2:
