@@ -58,7 +58,7 @@ static __global__ void k_peer_wait(const int32_t* __restrict__ flags, int n, int
     int v;
     asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(flags + i) : "memory");
     if (v >= value) break;
-    if (clock64() - t0 > (1ll << 32)) { atomicCAS(err, 0, 950); break; }     // ~2 s: a peer died
+    if (clock64() - t0 > (1ll << 32)) { atomicCAS(err, 0, kErrPeerWait); break; }     // ~2 s: a peer died
     __nanosleep(32);
   }
 }
@@ -82,11 +82,26 @@ int check_device_error(ovn_handle* h, cudaStream_t s) {
   const int e = *hp;
   if (e == 0) return OVN_OK;
   OVN_CUDA(h, cudaMemsetAsync(h->d_err, 0, sizeof(int), s));
-  if (e == kErrBadIndex) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "a pair / candidate index is outside [0, bank_size)");
-  if (e == kErrRowNotPrepared)
-    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "resident bank: an indexed row was never passed to ovn_bank_prepare");
-  if (e == 950) OVN_SET_ERR(h, OVN_ERR_CUDA, "ovn_peer_wait timed out: a peer rank never signalled");
-  OVN_SET_ERR(h, OVN_ERR_CUDA, "tensor-core pipeline failed (code %d: barrier time-out or injected fault); outputs of the call are poisoned (NaN / INT32_MIN)", e);
+  const char* ring = nullptr;          // a ring wait timed out: producer codes are 1xx, consumer codes 2xx / 4xx
+  switch (e) {
+    case kErrBadIndex: OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "a pair / candidate index is outside [0, bank_size)");
+    case kErrRowNotPrepared:
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "resident bank: an indexed row was never passed to ovn_bank_prepare");
+    case kErrPeerWait: OVN_SET_ERR(h, OVN_ERR_CUDA, "ovn_peer_wait timed out: a peer rank never signalled");
+    case kErrInjectedFault: OVN_SET_ERR(h, OVN_ERR_CUDA, "tensor-core pipeline failed: k_conv2_wgmma: fault injected by "
+                                        "OVN_DEBUG_FAULT (code %d); outputs of the call are poisoned (NaN / INT32_MIN)", e);
+    case kErrDeltaLeftProducer: case kErrDeltaLeftConsumer: ring = "k_delta_conv1_wgmma: LEFT volume ring"; break;
+    case kErrDeltaRightProducer: case kErrDeltaRightConsumer: ring = "k_delta_conv1_wgmma: RIGHT window ring"; break;
+    case kErrDeltaW1Producer: case kErrDeltaW1Consumer: ring = "k_delta_conv1_wgmma: W1 ring"; break;
+    case kErrConv2Producer: case kErrConv2Consumer: ring = "k_conv2_wgmma: o1 + W2 ring"; break;
+    case kErrConv3X3Producer: case kErrConv3X3Consumer: ring = "k_conv3_wgmma: x3 ring"; break;
+    case kErrConv3W3Producer: case kErrConv3W3Consumer: ring = "k_conv3_wgmma: W3 ring"; break;
+    case kErrCorrRightProducer: case kErrCorrRightConsumer: ring = "k_corr_wgmma: RIGHT third ring"; break;
+    case kErrCorrLeftProducer: case kErrCorrLeftConsumer: ring = "k_corr_wgmma: LEFT tile ring"; break;
+  }
+  if (!ring) OVN_SET_ERR(h, OVN_ERR_CUDA, "unknown device error code %d", e);
+  OVN_SET_ERR(h, OVN_ERR_CUDA, "tensor-core pipeline failed: %s, %s wait timed out (code %d); outputs of the call are "
+              "poisoned (NaN / INT32_MIN)", ring, e < 200 ? "producer" : "consumer", e);
 }
 
 }  // namespace ovn
@@ -242,13 +257,6 @@ int ovn_create(const ovn_config* cfg, ovn_handle** out) {
   const size_t maxp = c.max_batch_pairs;
   CREATE_ALLOC(h->d_keys, c.max_batch_scans * HW * sizeof(unsigned long long));
   CREATE_ALLOC(h->d_input, c.max_batch_scans * HW * h->C * sizeof(float));
-  size_t max_act = 1;
-  for (int l = 0; l < h->n_leg; ++l) {
-    size_t a = (size_t)h->leg[l].h_out * h->leg[l].w_out * h->leg[l].cout;
-    if (a > max_act) max_act = a;
-  }
-  CREATE_ALLOC(h->d_act[0], max_act * c.max_batch_scans * sizeof(float));
-  CREATE_ALLOC(h->d_act[1], max_act * c.max_batch_scans * sizeof(float));
   CREATE_ALLOC(h->d_query_fv, (size_t)Wf * kFeatC * sizeof(float));
   CREATE_ALLOC(h->d_cand_idx, maxp * sizeof(int32_t));
   CREATE_ALLOC(h->d_query_yaw, maxp * sizeof(int32_t));
@@ -259,6 +267,13 @@ int ovn_create(const ovn_config* cfg, ovn_handle** out) {
   CREATE_ALLOC(h->h_pinned, sizeof(StageHeader) + maxp * 3 * sizeof(int32_t));
   CREATE_ALLOC(h->d_query_overlap, maxp * sizeof(float));
   if (c.precision == OVN_PREC_FP32 && h->net_ok) {
+    size_t max_act = 0;
+    for (int l = 0; l < h->n_leg; ++l) {
+      const size_t a = (size_t)h->leg[l].h_out * h->leg[l].w_out * h->leg[l].cout;
+      if (a > max_act) max_act = a;
+    }
+    CREATE_ALLOC(h->d_act[0], max_act * c.max_batch_scans * sizeof(float));
+    CREATE_ALLOC(h->d_act[1], max_act * c.max_batch_scans * sizeof(float));
     CREATE_ALLOC(h->d_o1, maxp * h->o1_h * h->o1_w * 64 * sizeof(float));
     CREATE_ALLOC(h->d_o2, maxp * h->o2_h * h->o2_w * 128 * sizeof(float));
     CREATE_ALLOC(h->d_G, maxp * Wf * Wf * sizeof(float));

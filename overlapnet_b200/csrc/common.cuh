@@ -143,14 +143,14 @@ struct ovn_handle {
   ovn::Buffer<uint32_t> d_valid_words;       // validity bitmask, 1 bit per point; these three grow with the points
   ovn::Buffer<uint32_t> d_word_prefix;       //   of projections that return per-point indices
   ovn::Buffer<uint32_t> d_scan_tmp;          //   (exclusive prefix of popcounts, block sums)
-  ovn::Buffer<float> d_act[2];               // ping-pong activations for the fp32 leg (f16_tc: layer 1 fallback)
+  ovn::Buffer<float> d_act[2];               // fp32 only: ping-pong activations of the leg
   ovn::Buffer<float> d_input;                // [max_batch_scans][H][W][C]
   ovn::Buffer<float> d_o1;                   // fp32 only: [max_batch_pairs][360][24][64]
   ovn::Buffer<float> d_o2;                   // fp32 only: [max_batch_pairs][24][24][128]
   ovn::Buffer<float> d_G;                    // fp32 only: [max_batch_pairs][360][360] correlation Gram matrices
   ovn::Buffer<int32_t> d_cand_idx;           // [max_batch_pairs] candidate indices of ovn_heads_1vsN / the host query
   ovn::Buffer<int32_t> d_idx_san;            // [max_batch_pairs] x3 bounds-checked (clamped) copies of the caller's index lists
-  ovn::Buffer<int> d_err;                    // device error flag: pipeline barrier time-outs (1xx-8xx), bad indices (9xx)
+  ovn::Buffer<int> d_err;                    // device error flag: 0 or an ovn::DeviceError
   cudaEvent_t ev_bank = nullptr;             // recorded after ovn_bank_prepare: the host entry points (own stream) wait on it
   // ovn_query_cloud_vs_bank_host / ovn_encode_clouds_host
   ovn::Buffer<float> d_query_fv;             // [360][128]
@@ -229,9 +229,23 @@ struct DeviceGuard {
   ~DeviceGuard() { if (switched) cudaSetDevice(prev); }
 };
 
-// error codes written to ovn_handle::d_err by kernels
-constexpr int kErrBadIndex = 900;        // a pair / candidate index outside [0, bank_size)
-constexpr int kErrRowNotPrepared = 901;  // resident bank: the row was never passed to ovn_bank_prepare
+// Every value a kernel writes to ovn_handle::d_err (0: no error); check_device_error maps each to a status and
+// a message.  The numbers appear in messages, so they do not change.
+enum DeviceError : int {
+  // a bounded wait on an mbarrier ring timed out: 1xx in the producer, 2xx / 4xx in a consumer
+  kErrDeltaLeftProducer = 101, kErrDeltaLeftConsumer = 402,      // k_delta_conv1_wgmma: LEFT volume
+  kErrDeltaRightProducer = 103, kErrDeltaRightConsumer = 404,    //   RIGHT window
+  kErrDeltaW1Producer = 102, kErrDeltaW1Consumer = 202,          //   W1 groups
+  kErrConv2Producer = 111, kErrConv2Consumer = 211,              // k_conv2_wgmma: o1 + W2 stages
+  kErrConv3X3Producer = 121, kErrConv3X3Consumer = 221,          // k_conv3_wgmma: x3 rows
+  kErrConv3W3Producer = 122, kErrConv3W3Consumer = 222,          //   W3 slabs
+  kErrCorrRightProducer = 131, kErrCorrRightConsumer = 231,      // k_corr_wgmma: RIGHT third
+  kErrCorrLeftProducer = 132, kErrCorrLeftConsumer = 232,        //   LEFT tiles
+  kErrInjectedFault = 501,        // k_conv2_wgmma under OVN_DEBUG_FAULT (the error-path test hook)
+  kErrBadIndex = 900,             // a pair / candidate index outside [0, bank_size)
+  kErrRowNotPrepared = 901,       // resident bank: the row was never passed to ovn_bank_prepare
+  kErrPeerWait = 950,             // ovn_peer_wait: a peer rank never signalled
+};
 
 // RAII-free profiling helpers: record an event on `s` before / after a launch when enabled
 inline void prof_mark(ovn_handle* h, int kind, cudaStream_t s) {
@@ -278,7 +292,7 @@ int pack_input(ovn_handle* h, const float* d_depth, const float* d_normal, const
                const float* d_intensity, int n_scans, float* d_input, cudaStream_t s);
 
 int leg_forward_fp32(ovn_handle* h, const float* d_input, int n, float* d_fv, cudaStream_t s);
-int leg_layer_fp32(ovn_handle* h, int l, const float* x, float* y, int n, cudaStream_t s);
+// the heads_forward_* score n <= max_batch_pairs pairs (heads_dispatch cuts larger calls into such chunks)
 int heads_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query,
                        const int32_t* d_left, const int32_t* d_right, int n, float* d_overlap,
                        int32_t* d_yaw, float* d_corr, cudaStream_t s);

@@ -1,6 +1,6 @@
 // hopper.cuh -- hand-written PTX wrappers for the Hopper (sm_90a) building blocks used by network_tc.cu:
-// wgmma (warpgroup MMA; B from shared memory, A from registers or shared memory), mbarrier, cp.async.bulk
-// (TMA engine, 1-D).
+// wgmma (warpgroup MMA; B from shared memory, A from registers or shared memory), mbarrier and the pipeline
+// ring built on it, cp.async.bulk (TMA engine, 1-D).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -35,6 +35,53 @@ __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, long l
     if (clock64() - t0 > max_cycles) return false;
   return true;
 }
+constexpr long long kMbarWaitCycles = 1ll << 28;
+
+// A ring of D pipeline stages, each guarded by a full / empty mbarrier pair.  The producer fills the stages in
+// order; fill i uses stage i % D in phase (i / D) & 1.  The fill counters belong to the kernels, which pass the
+// fill index.  full[s] completes on the producer's arrive plus the bytes of its bulk copies; empty[s] completes
+// when every consumer arrival has released the stage.
+template <int D>
+struct MbarRing {
+  uint64_t full[D], empty[D];
+  __device__ __forceinline__ void init(uint32_t consumer_arrivals) {
+    for (int s = 0; s < D; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], consumer_arrivals); }
+  }
+  static __device__ __forceinline__ uint32_t slot(uint32_t i) { return i % D; }
+  static __device__ __forceinline__ uint32_t parity(uint32_t i) { return (i / D) & 1; }
+  // producer: wait (bounded) until fill i's stage is free, then expect `bytes` on it.  False on time-out.
+  __device__ __forceinline__ bool acquire(uint32_t i, uint32_t bytes) {
+    if (!mbar_wait(&empty[slot(i)], parity(i) ^ 1, kMbarWaitCycles)) return false;
+    mbar_arrive_expect_tx(&full[slot(i)], bytes);
+    return true;
+  }
+  // producer, without waiting: false if fill i's stage is not free yet
+  __device__ __forceinline__ bool try_acquire(uint32_t i, uint32_t bytes) {
+    if (!mbar_try_wait(&empty[slot(i)], parity(i) ^ 1)) return false;
+    mbar_arrive_expect_tx(&full[slot(i)], bytes);
+    return true;
+  }
+  // the barrier the bulk copies of fill i complete on
+  __device__ __forceinline__ uint64_t* bar(uint32_t i) { return &full[slot(i)]; }
+  // consumer: wait (bounded) until fill i has landed.  False on time-out.
+  __device__ __forceinline__ bool wait(uint32_t i) { return mbar_wait(&full[slot(i)], parity(i), kMbarWaitCycles); }
+  // consumer: this warp is done with fill i's stage (one arrival per warp)
+  __device__ __forceinline__ void release(uint32_t i) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[slot(i)]);
+  }
+};
+
+// The bounded waits of a kernel with an `int* err` flag and a `done:` label before its end; `ok` is a ring's
+// acquire or wait, `code` an ovn::DeviceError.
+// A producer, or a consumer with no wgmma groups in flight: on time-out raise `code` and leave the kernel.
+#define PIPE_WAIT(ok, code) \
+  if (!(ok)) { atomicExch(err, (code)); goto done; }
+// A consumer with wgmma groups in flight: leaving the loop there would make the compiler wait for them on a
+// divergent path, which serialises every wgmma of the kernel.  A time-out raises `code` and sets the local
+// `failed`; later waits are skipped, and the consumer leaves (`if (failed) goto done`) once its groups retire.
+#define INFLIGHT_WAIT(ok, code) \
+  if (!failed && !(ok)) { atomicExch(err, (code)); failed = true; }
 
 // barrier `id` (1..15) among the `count` threads (a multiple of 32) that reach it, e.g. one warpgroup
 __device__ __forceinline__ void named_bar_sync(int id, int count) {

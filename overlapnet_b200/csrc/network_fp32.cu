@@ -320,13 +320,6 @@ k_corr_readout(const float* __restrict__ G, int Wf, float* __restrict__ corr_out
 }
 
 // ---- drivers ----------------------------------------------------------------------------------
-int leg_layer_fp32(ovn_handle* h, int l, const float* x, float* y, int n, cudaStream_t s) {
-  const ConvSpec& L = h->leg[l];
-  ConvOperand a{x, L.h_in, L.w_in, L.cin, L.kw, L.sh, L.sw, L.h_out, L.w_out};
-  BOperand b{h->d_w[l], nullptr, nullptr, 0, 0};
-  return launch_gemm(h, a, b, h->d_b[l], y, n * L.h_out * L.w_out, L.cout, L.kh * L.kw * L.cin, 1, L.relu, s);
-}
-
 int leg_forward_fp32(ovn_handle* h, const float* d_input, int n, float* d_fv, cudaStream_t s) {
   const float* x = d_input;
   prof_mark(h, PROF_LEG, s);
@@ -399,20 +392,10 @@ static int overlap_head_fp32(ovn_handle* h, const float* d_bank, const float* d_
 int heads_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* d_left,
                        const int32_t* d_right, int n, float* d_overlap, int32_t* d_yaw, float* d_corr,
                        cudaStream_t s) {
-  const int Wf = h->cfg.leg_output_width;
-  const int maxp = h->cfg.max_batch_pairs;
-  for (int p0 = 0; p0 < n; p0 += maxp) {
-    const int np = (n - p0 < maxp) ? n - p0 : maxp;
-    const int32_t* left = d_left + p0;
-    const int32_t* right = d_right ? d_right + p0 : nullptr;
-    // the o3 buffer is d_o1 (o1 is dead after c_conv2)
-    int rc = overlap_head_fp32(h, d_bank, d_query, left, right, np, h->d_o1, d_overlap + p0, s);
-    if (rc != OVN_OK) return rc;
-    rc = corr_forward_fp32(h, d_bank, d_query, left, right, np, d_yaw + p0,
-                           d_corr ? d_corr + (int64_t)p0 * Wf : nullptr, s);
-    if (rc != OVN_OK) return rc;
-  }
-  return OVN_OK;
+  // the o3 buffer is d_o1 (o1 is dead after c_conv2)
+  int rc = overlap_head_fp32(h, d_bank, d_query, d_left, d_right, n, h->d_o1, d_overlap, s);
+  if (rc != OVN_OK) return rc;
+  return corr_forward_fp32(h, d_bank, d_query, d_left, d_right, n, d_yaw, d_corr, s);
 }
 
 // ---- training of the overlap head with a frozen leg -------------------------------------------

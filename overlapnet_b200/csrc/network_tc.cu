@@ -251,23 +251,23 @@ constexpr int K4_RING = 4;
 constexpr int K4_BSLICE = 4096;                        // bytes of W1 per slice: [4 k8][64 o][8]
 constexpr uint32_t K4_VOL_BYTES = WF * K4_PITCH * 2;
 constexpr uint32_t K4_RWIN_BYTES = S15 * K4_PITCH * 2;
-constexpr long long kWaitCycles = 1ll << 28;
 
 struct K4Smem {
   __half L[WF * K4_PITCH];
   __half Rw[2][S15 * K4_PITCH];
   __half B[K4_RING][K4_GROUP * K4_BSLICE / 2];
-  uint64_t full[K4_RING], empty[K4_RING], l_full, l_empty, rw_full[2], rw_empty[2];
+  MbarRing<K4_RING> w1;
+  MbarRing<1> left;
+  MbarRing<2> right;
 };
 static_assert(sizeof(K4Smem) <= 232448, "k_delta_conv1_wgmma shared memory");
 static_assert(offsetof(K4Smem, B) % 16 == 0 && offsetof(K4Smem, Rw) % 16 == 0, "bulk-copy alignment");
 
-// bounded wait of a pipeline stage: on time-out raise `code` and leave the kernel (label `done`)
-#define PIPE_WAIT(bar, parity, code)                       \
-  if (!mbar_wait((bar), (parity), kWaitCycles)) {          \
-    atomicExch(err, (code));                               \
-    goto done;                                             \
-  }
+// [begin, end) of the contiguous share of n work items that part `part` of `parts` takes (a persistent CTA)
+struct Share { int64_t begin, end; };
+__device__ __forceinline__ Share work_share(int64_t n, uint32_t part, uint32_t parts) {
+  return {n * part / parts, n * (part + 1) / parts};
+}
 
 __global__ void __launch_bounds__(K4_THREADS, 1)
 k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ l_idx, const __half* __restrict__ R16,
@@ -276,13 +276,12 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
   extern __shared__ __align__(128) uint8_t smem_raw[];
   K4Smem& S = *reinterpret_cast<K4Smem*>(smem_raw);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int64_t n_units = (int64_t)n_pairs * NB;
-  const int u_begin = (int)(n_units * blockIdx.x / gridDim.x), u_end = (int)(n_units * (blockIdx.x + 1) / gridDim.x);
-  constexpr uint32_t kConsumerWarps = K4_WG * 4;
+  const Share share = work_share((int64_t)n_pairs * NB, blockIdx.x, gridDim.x);
+  const int u_begin = (int)share.begin, u_end = (int)share.end;
   if (tid == 0) {
-    for (int s = 0; s < K4_RING; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], kConsumerWarps); }
-    mbar_init(&S.l_full, 1); mbar_init(&S.l_empty, kConsumerWarps);
-    for (int b = 0; b < 2; ++b) { mbar_init(&S.rw_full[b], 1); mbar_init(&S.rw_empty[b], kConsumerWarps); }
+    S.w1.init(K4_WG * 4);
+    S.left.init(K4_WG * 4);
+    S.right.init(K4_WG * 4);
     mbar_fence_init();
   }
   __syncthreads();
@@ -294,21 +293,16 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
       for (int u = u_begin; u < u_end; ++u, ++ui) {
         const int p = u / NB, jb = u - p * NB;
         if (u == u_begin || jb == 0) {
-          PIPE_WAIT(&S.l_empty, (pi & 1) ^ 1, 101);
-          mbar_arrive_expect_tx(&S.l_full, K4_VOL_BYTES);
-          bulk_g2s(S.L, L16 + (size_t)(l_idx ? l_idx[p] : p) * WF * K4_PITCH, K4_VOL_BYTES, &S.l_full);
+          PIPE_WAIT(S.left.acquire(pi, K4_VOL_BYTES), kErrDeltaLeftProducer);
+          bulk_g2s(S.L, L16 + (size_t)(l_idx ? l_idx[p] : p) * WF * K4_PITCH, K4_VOL_BYTES, S.left.bar(pi));
           ++pi;
         }
-        const uint32_t b = ui & 1;
-        PIPE_WAIT(&S.rw_empty[b], ((ui >> 1) & 1) ^ 1, 103);
-        mbar_arrive_expect_tx(&S.rw_full[b], K4_RWIN_BYTES);
-        bulk_g2s(S.Rw[b], R16 + (r_per_pair ? (size_t)p * WF * K4_PITCH : 0) + (size_t)jb * S15 * K4_PITCH, K4_RWIN_BYTES,
-                 &S.rw_full[b]);
+        PIPE_WAIT(S.right.acquire(ui, K4_RWIN_BYTES), kErrDeltaRightProducer);
+        bulk_g2s(S.Rw[S.right.slot(ui)], R16 + (r_per_pair ? (size_t)p * WF * K4_PITCH : 0) + (size_t)jb * S15 * K4_PITCH,
+                 K4_RWIN_BYTES, S.right.bar(ui));
         for (int grp = 0; grp < K4_NGROUPS; ++grp, ++gi) {
-          const uint32_t s = gi % K4_RING, ph = (gi / K4_RING) & 1;
-          PIPE_WAIT(&S.empty[s], ph ^ 1, 102);
-          mbar_arrive_expect_tx(&S.full[s], K4_GROUP * K4_BSLICE);
-          bulk_g2s(S.B[s], W1p + (size_t)grp * K4_GROUP * (K4_BSLICE / 2), K4_GROUP * K4_BSLICE, &S.full[s]);
+          PIPE_WAIT(S.w1.acquire(gi, K4_GROUP * K4_BSLICE), kErrDeltaW1Producer);
+          bulk_g2s(S.B[S.w1.slot(gi)], W1p + (size_t)grp * K4_GROUP * (K4_BSLICE / 2), K4_GROUP * K4_BSLICE, S.w1.bar(gi));
         }
       }
     }
@@ -326,9 +320,9 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
     uint32_t pi = 0, gi = 0, ui = 0;
     for (int u = u_begin; u < u_end; ++u, ++ui) {
       const int p = u / NB, jb = u - p * NB;
-      if (u == u_begin || jb == 0) { PIPE_WAIT(&S.l_full, pi & 1, 402); ++pi; }
-      const uint32_t wb = ui & 1;
-      PIPE_WAIT(&S.rw_full[wb], (ui >> 1) & 1, 404);
+      if (u == u_begin || jb == 0) { PIPE_WAIT(S.left.wait(pi), kErrDeltaLeftConsumer); ++pi; }
+      const uint32_t wb = S.right.slot(ui);
+      PIPE_WAIT(S.right.wait(ui), kErrDeltaRightConsumer);
       float acc[2][32];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {             // read per unit rather than held in 16 registers across the loop
@@ -354,7 +348,7 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
               Lr[tt][h][0] = v.x; Lr[tt][h][1] = v.y; Lr[tt][h][2] = v.z; Lr[tt][h][3] = v.w;
             }
         }
-        const uint32_t s = gi % K4_RING;
+        const uint32_t s = S.w1.slot(gi);
         // slice sl of the stage, K16 step kk: W1 chunks k8 = 2 kk, 2 kk + 1 (LBO = 1024 B between them, SBO = 128 B
         // per 8 outputs) at sl * 4096 + kk * 2048 bytes, i.e. (sl * 4096 + kk * 2048) >> 4 in the descriptor
         const uint64_t bdesc = desc_kmajor(b_base + s * (K4_GROUP * K4_BSLICE), 1024, 128, kNoSwizzle);
@@ -363,7 +357,7 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
         const __half* rw = S.Rw[wb] + dj0 * K4_PITCH + 8 * t;
         const __half* rp[2] = {rw + ((cc ^ par) << 5), rw + ((cc ^ par ^ 1) << 5)};
         uint4 rv = *reinterpret_cast<const uint4*>(rp[0]);
-        PIPE_WAIT(&S.full[s], (gi / K4_RING) & 1, 202);
+        PIPE_WAIT(S.w1.wait(gi), kErrDeltaW1Consumer);
 #pragma unroll
         for (int sl = 0; sl < K4_GROUP; ++sl) {
           uint32_t A[2][2][4];                // [tile][kk]
@@ -391,14 +385,10 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
           if (sl + 1 < K4_GROUP) rv = *reinterpret_cast<const uint4*>(rp[(sl + 1) & 1] + (sl + 1) * K4_PITCH);
           wgmma_wait<0>();
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&S.empty[s]);
+        S.w1.release(gi);
       }
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&S.rw_empty[wb]);
-        if (jb == NB - 1 || u == u_end - 1) mbar_arrive(&S.l_empty);
-      }
+      S.right.release(ui);
+      if (jb == NB - 1 || u == u_end - 1) S.left.release(pi - 1);
       const int64_t mrow = (int64_t)p * PAIR_ROWS + jb * NB;
 #pragma unroll
       for (int tt = 0; tt < 2; ++tt)
@@ -417,15 +407,6 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
 done:
   return;
 }
-
-// Wait of a consumer with wgmma groups in flight: leaving the loop there would make the compiler wait for them
-// on a divergent path, which serialises every wgmma of the kernel.  A time-out raises `code`, later waits are
-// skipped, and the consumer leaves (`if (failed) goto done`) once its groups are retired.
-#define INFLIGHT_WAIT(bar, parity, code)                                      \
-  if (!failed && !mbar_wait((bar), (parity), kWaitCycles)) {                  \
-    atomicExch(err, (code));                                                  \
-    failed = true;                                                            \
-  }
 
 // ------------------------------------------------------------------------------------------------
 // k_conv2_wgmma -- c_conv2 (15x1 stride 15, 64 -> 128, ReLU) as a GEMM [M x 960] x [960 x 128], W2 applied as
@@ -450,7 +431,7 @@ constexpr int C2_RING = 3;
 struct C2Smem {
   __half A[C2_RING][TC_WG][C2_TILE / 2];               // o1 of one di: rows [r0, r0 + 128), [r0 + 128, r0 + 256)
   __half B[C2_RING][2][C2_TILE / 2];                   // W2 of that di: hi, lo
-  uint64_t full[C2_RING], empty[C2_RING];
+  MbarRing<C2_RING> ring;
 };
 constexpr size_t C2_SMEM = sizeof(C2Smem) + 1024;      // + the round-up of the base to a 1024-byte swizzle atom
 static_assert(C2_SMEM <= 232448, "k_conv2_wgmma shared memory");
@@ -461,17 +442,15 @@ k_conv2_wgmma(const __half* __restrict__ o1, const __half* __restrict__ W2s, con
               const float* __restrict__ mu_x3, __half* __restrict__ x3, int64_t out_pitch, int64_t M, int fault,
               int* __restrict__ err) {
   if (fault) {
-    if (threadIdx.x == 0 && blockIdx.x == 0) atomicExch(err, 501);
+    if (threadIdx.x == 0 && blockIdx.x == 0) atomicExch(err, kErrInjectedFault);
     return;
   }
   extern __shared__ __align__(128) uint8_t smem_raw[];
   C2Smem& S = *reinterpret_cast<C2Smem*>(smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023));
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int64_t n_tiles = (M + TC_ROWS - 1) / TC_ROWS;
-  const int64_t t_begin = n_tiles * blockIdx.x / gridDim.x, t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
-  constexpr uint32_t kConsumerWarps = TC_WG * 4;
+  const Share tiles = work_share((M + TC_ROWS - 1) / TC_ROWS, blockIdx.x, gridDim.x);
   if (tid == 0) {
-    for (int s = 0; s < C2_RING; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], kConsumerWarps); }
+    S.ring.init(TC_WG * 4);
     mbar_fence_init();
   }
   __syncthreads();
@@ -480,14 +459,13 @@ k_conv2_wgmma(const __half* __restrict__ o1, const __half* __restrict__ W2s, con
     // ===================== producer ==========================================================
     if (lane == 0) {
       uint32_t gi = 0;
-      for (int64_t tile = t_begin; tile < t_end; ++tile)
+      for (int64_t tile = tiles.begin; tile < tiles.end; ++tile)
         for (int di = 0; di < S15; ++di, ++gi) {
-          const uint32_t s = gi % C2_RING;
-          PIPE_WAIT(&S.empty[s], ((gi / C2_RING) & 1) ^ 1, 111);
-          mbar_arrive_expect_tx(&S.full[s], 4 * C2_TILE);
+          const uint32_t s = S.ring.slot(gi);
+          PIPE_WAIT(S.ring.acquire(gi, 4 * C2_TILE), kErrConv2Producer);
           for (int h = 0; h < TC_WG; ++h)      // o1 tile (m / 128, di) of the rows m = 256 tile + 128 h + [0, 128)
-            bulk_g2s(S.A[s][h], o1 + ((size_t)(tile * TC_WG + h) * S15 + di) * (C2_TILE / 2), C2_TILE, &S.full[s]);
-          bulk_g2s(S.B[s], W2s + (size_t)di * C2_TILE, 2 * C2_TILE, &S.full[s]);
+            bulk_g2s(S.A[s][h], o1 + ((size_t)(tile * TC_WG + h) * S15 + di) * (C2_TILE / 2), C2_TILE, S.ring.bar(gi));
+          bulk_g2s(S.B[s], W2s + (size_t)di * C2_TILE, 2 * C2_TILE, S.ring.bar(gi));
         }
     }
   } else {
@@ -495,7 +473,7 @@ k_conv2_wgmma(const __half* __restrict__ o1, const __half* __restrict__ W2s, con
     const int wg = warp >> 2, wi = warp & 3, g = lane >> 2, t = lane & 3;
     uint32_t gi = 0;
     bool failed = false;
-    for (int64_t tile = t_begin; tile < t_end; ++tile) {
+    for (int64_t tile = tiles.begin; tile < tiles.end; ++tile) {
       float acc[2][64];                       // [m64 sub-tile][D fragment]
 #pragma unroll
       for (int sub = 0; sub < 2; ++sub)
@@ -503,8 +481,8 @@ k_conv2_wgmma(const __half* __restrict__ o1, const __half* __restrict__ W2s, con
         for (int e = 0; e < 64; ++e) acc[sub][e] = 0.f;
 #pragma unroll 1
       for (int di = 0; di < S15; ++di, ++gi) {
-        const uint32_t s = gi % C2_RING;
-        INFLIGHT_WAIT(&S.full[s], (gi / C2_RING) & 1, 211);
+        const uint32_t s = S.ring.slot(gi);
+        INFLIGHT_WAIT(S.ring.wait(gi), kErrConv2Consumer);
         const uint32_t a_base = smem_u32(S.A[s][wg]), b_base = smem_u32(S.B[s][0]);
         wgmma_fence();
 #pragma unroll
@@ -518,15 +496,11 @@ k_conv2_wgmma(const __half* __restrict__ o1, const __half* __restrict__ W2s, con
           }
         wgmma_commit();
         wgmma_wait<1>();                      // the previous di's group is done: its stage can be refilled
-        if (di > 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&S.empty[(gi - 1) % C2_RING]);
-        }
+        if (di > 0) S.ring.release(gi - 1);
       }
       wgmma_wait<0>();
       if (failed) goto done;
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&S.empty[(gi - 1) % C2_RING]);
+      S.ring.release(gi - 1);
       // b2eff, ReLU, minus the x3 centre, fp16 into the C8-interleaved planes (rows past M are not stored)
 #pragma unroll
       for (int sub = 0; sub < 2; ++sub)
@@ -572,7 +546,8 @@ constexpr int C3_RING = 4;
 struct C3Smem {
   __half A[2][16 * C3_PLANE / 2];                      // [buffer][plane c / 8][row][8]
   __half B[C3_RING][C3_GROUP * C3_SLAB / 2];
-  uint64_t full[C3_RING], empty[C3_RING], a_full[2], a_empty[2];
+  MbarRing<C3_RING> w3;
+  MbarRing<2> x3;
 };
 static_assert(sizeof(C3Smem) <= 232448, "k_conv3_wgmma shared memory");
 static_assert(offsetof(C3Smem, B) % 16 == 0 && C3_PLANE % 16 == 0, "bulk-copy alignment");
@@ -583,12 +558,10 @@ k_conv3_wgmma(const __half* __restrict__ X3, int64_t a_pitch, const __half* __re
   extern __shared__ __align__(128) uint8_t smem_raw[];
   C3Smem& S = *reinterpret_cast<C3Smem*>(smem_raw);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int64_t n_tiles = 2 * ((M + TC_ROWS - 1) / TC_ROWS);     // tile = 2 * row block + nh
-  const int64_t t_begin = n_tiles * blockIdx.x / gridDim.x, t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
-  constexpr uint32_t kConsumerWarps = TC_WG * 4;
+  const Share tiles = work_share(2 * ((M + TC_ROWS - 1) / TC_ROWS), blockIdx.x, gridDim.x);   // 2 * row block + nh
   if (tid == 0) {
-    for (int s = 0; s < C3_RING; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], kConsumerWarps); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&S.a_full[b], 1); mbar_init(&S.a_empty[b], kConsumerWarps); }
+    S.w3.init(TC_WG * 4);
+    S.x3.init(TC_WG * 4);
     mbar_fence_init();
   }
   __syncthreads();
@@ -596,30 +569,27 @@ k_conv3_wgmma(const __half* __restrict__ X3, int64_t a_pitch, const __half* __re
   if (warp == TC_WG * 4) {
     // ===================== producer ==========================================================
     if (lane == 0) {
-      const uint32_t nt = (uint32_t)(t_end - t_begin);
+      const uint32_t nt = (uint32_t)(tiles.end - tiles.begin);
       uint32_t ai = 0, gi = 0;                // tiles whose x3 rows were issued, W3 stages issued
       for (uint32_t ti = 0; ti < nt; ++ti) {
-        const int nh = (int)((t_begin + ti) & 1);
+        const int nh = (int)((tiles.begin + ti) & 1);
         for (int st = 0; st < C3_NSTAGES; ++st, ++gi) {
           // x3 rows of this tile (must go now) and of the next one (as soon as its buffer is free, i.e. once
           // the tile before this one is done), so that they load while this tile computes
           while (ai < nt && ai <= ti + 1) {
-            const uint32_t b = ai & 1, par = ((ai >> 1) & 1) ^ 1;
             if (ai > ti) {
-              if (!mbar_try_wait(&S.a_empty[b], par)) break;
+              if (!S.x3.try_acquire(ai, 16 * C3_PLANE)) break;
             } else {
-              PIPE_WAIT(&S.a_empty[b], par, 121);
+              PIPE_WAIT(S.x3.acquire(ai, 16 * C3_PLANE), kErrConv3X3Producer);
             }
-            const int64_t r0 = ((t_begin + ai) >> 1) * TC_ROWS;
-            mbar_arrive_expect_tx(&S.a_full[b], 16 * C3_PLANE);
+            const int64_t r0 = ((tiles.begin + ai) >> 1) * TC_ROWS;
             for (int pl = 0; pl < 16; ++pl)
-              bulk_g2s(S.A[b] + pl * (C3_PLANE / 2), X3 + ((size_t)pl * a_pitch + r0) * 8, C3_PLANE, &S.a_full[b]);
+              bulk_g2s(S.A[S.x3.slot(ai)] + pl * (C3_PLANE / 2), X3 + ((size_t)pl * a_pitch + r0) * 8, C3_PLANE, S.x3.bar(ai));
             ++ai;
           }
-          const uint32_t s = gi % C3_RING;
-          PIPE_WAIT(&S.empty[s], ((gi / C3_RING) & 1) ^ 1, 122);
-          mbar_arrive_expect_tx(&S.full[s], C3_GROUP * C3_SLAB);
-          bulk_g2s(S.B[s], W3p + ((size_t)nh * 36 + st * C3_GROUP) * (C3_SLAB / 2), C3_GROUP * C3_SLAB, &S.full[s]);
+          PIPE_WAIT(S.w3.acquire(gi, C3_GROUP * C3_SLAB), kErrConv3W3Producer);
+          bulk_g2s(S.B[S.w3.slot(gi)], W3p + ((size_t)nh * 36 + st * C3_GROUP) * (C3_SLAB / 2), C3_GROUP * C3_SLAB,
+                   S.w3.bar(gi));
         }
       }
     }
@@ -629,12 +599,12 @@ k_conv3_wgmma(const __half* __restrict__ X3, int64_t a_pitch, const __half* __re
     const uint32_t b_base = smem_u32(S.B[0]);
     uint32_t gi = 0;
     bool failed = false;
-    for (int64_t tile = t_begin; tile < t_end; ++tile) {
-      const uint32_t ti = (uint32_t)(tile - t_begin), ab = ti & 1;
+    for (int64_t tile = tiles.begin; tile < tiles.end; ++tile) {
+      const uint32_t ti = (uint32_t)(tile - tiles.begin);
       const int nh = (int)(tile & 1);
       const int64_t r0 = (tile >> 1) * TC_ROWS;
-      PIPE_WAIT(&S.a_full[ab], (ti >> 1) & 1, 221);
-      const uint32_t a_rows = smem_u32(S.A[ab]) + wg * 128 * 16;
+      PIPE_WAIT(S.x3.wait(ti), kErrConv3X3Consumer);
+      const uint32_t a_rows = smem_u32(S.A[S.x3.slot(ti)]) + wg * 128 * 16;
       float acc[2][64];                       // [m64 sub-tile][D fragment]
 #pragma unroll
       for (int sub = 0; sub < 2; ++sub)
@@ -642,8 +612,8 @@ k_conv3_wgmma(const __half* __restrict__ X3, int64_t a_pitch, const __half* __re
         for (int e = 0; e < 64; ++e) acc[sub][e] = 0.f;
 #pragma unroll 1
       for (int st = 0; st < C3_NSTAGES; ++st, ++gi) {
-        const uint32_t s = gi % C3_RING;
-        INFLIGHT_WAIT(&S.full[s], (gi / C3_RING) & 1, 222);
+        const uint32_t s = S.w3.slot(gi);
+        INFLIGHT_WAIT(S.w3.wait(gi), kErrConv3W3Consumer);
         wgmma_fence();
 #pragma unroll
         for (int sl = 0; sl < C3_GROUP; ++sl) {
@@ -662,18 +632,12 @@ k_conv3_wgmma(const __half* __restrict__ X3, int64_t a_pitch, const __half* __re
         }
         wgmma_commit();
         wgmma_wait<1>();                      // the previous stage's group is done: its slot can be refilled
-        if (st > 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&S.empty[(gi - 1) % C3_RING]);
-        }
+        if (st > 0) S.w3.release(gi - 1);
       }
       wgmma_wait<0>();
       if (failed) goto done;
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&S.empty[(gi - 1) % C3_RING]);
-        mbar_arrive(&S.a_empty[ab]);
-      }
+      S.w3.release(gi - 1);
+      S.x3.release(ti);
 #pragma unroll
       for (int sub = 0; sub < 2; ++sub)
 #pragma unroll
@@ -727,7 +691,8 @@ struct C6Smem {
   __half R[C6_R_BYTES / 2];
   __half L[C6_RING][C6_L_BYTES / 2];
   float G[C6_WG][C6_LROWS * C6_GPITCH];
-  uint64_t full[C6_RING], empty[C6_RING], r_full, r_empty;
+  MbarRing<C6_RING> left;
+  MbarRing<1> right;
 };
 static_assert(sizeof(C6Smem) <= 232448, "k_corr_wgmma shared memory");
 static_assert(offsetof(C6Smem, L) % 16 == 0, "bulk-copy alignment");
@@ -738,12 +703,12 @@ k_corr_wgmma(const __half* __restrict__ Lc, const int32_t* __restrict__ l_idx, c
   extern __shared__ __align__(128) uint8_t smem_raw[];
   C6Smem& S = *reinterpret_cast<C6Smem*>(smem_raw);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int q = blockIdx.x % C6_RT, c = blockIdx.x / C6_RT, nc = gridDim.x / C6_RT;
-  const int64_t n_units = (int64_t)n_pairs * C6_LT;
-  const int u_begin = (int)(n_units * c / nc), u_end = (int)(n_units * (c + 1) / nc);
+  const int q = blockIdx.x % C6_RT;
+  const Share share = work_share((int64_t)n_pairs * C6_LT, blockIdx.x / C6_RT, gridDim.x / C6_RT);
+  const int u_begin = (int)share.begin, u_end = (int)share.end;
   if (tid == 0) {
-    for (int s = 0; s < C6_RING; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], 4); }  // one warpgroup per unit
-    mbar_init(&S.r_full, 1); mbar_init(&S.r_empty, C6_WG * 4);
+    S.left.init(4);                           // one warpgroup per unit
+    S.right.init(C6_WG * 4);
     mbar_fence_init();
   }
   __syncthreads();
@@ -751,21 +716,19 @@ k_corr_wgmma(const __half* __restrict__ Lc, const int32_t* __restrict__ l_idx, c
   if (warp == C6_WG * 4) {
     // ===================== producer ==========================================================
     if (lane == 0) {
-      uint32_t ri = 0;
+      uint32_t ri = 0, ui = 0;
       int key = -1;                           // pair whose RIGHT third is loaded (0 in query mode)
-      for (int u = u_begin, ui = 0; u < u_end; ++u, ++ui) {
+      for (int u = u_begin; u < u_end; ++u, ++ui) {
         const int p = u / C6_LT, a = u - p * C6_LT;
         if ((r_per_pair ? p : 0) != key) {
           key = r_per_pair ? p : 0;
-          PIPE_WAIT(&S.r_empty, (ri & 1) ^ 1, 131);
-          mbar_arrive_expect_tx(&S.r_full, C6_R_BYTES);
-          bulk_g2s(S.R, Rc + ((size_t)key * C6_RT + q) * (C6_R_BYTES / 2), C6_R_BYTES, &S.r_full);
+          PIPE_WAIT(S.right.acquire(ri, C6_R_BYTES), kErrCorrRightProducer);
+          bulk_g2s(S.R, Rc + ((size_t)key * C6_RT + q) * (C6_R_BYTES / 2), C6_R_BYTES, S.right.bar(ri));
           ++ri;
         }
-        const uint32_t s = ui % C6_RING;
-        PIPE_WAIT(&S.empty[s], ((ui / C6_RING) & 1) ^ 1, 132);
-        mbar_arrive_expect_tx(&S.full[s], C6_L_BYTES);
-        bulk_g2s(S.L[s], Lc + ((size_t)(l_idx ? l_idx[p] : p) * C6_LT + a) * (C6_L_BYTES / 2), C6_L_BYTES, &S.full[s]);
+        PIPE_WAIT(S.left.acquire(ui, C6_L_BYTES), kErrCorrLeftProducer);
+        bulk_g2s(S.L[S.left.slot(ui)], Lc + ((size_t)(l_idx ? l_idx[p] : p) * C6_LT + a) * (C6_L_BYTES / 2), C6_L_BYTES,
+                 S.left.bar(ui));
       }
     }
   } else {
@@ -775,20 +738,20 @@ k_corr_wgmma(const __half* __restrict__ Lc, const int32_t* __restrict__ l_idx, c
     const int wg = warp >> 2, wi = warp & 3, g = lane >> 2, t = lane & 3, tw = tid & 127;
     float* Gw = S.G[wg];
     const uint32_t r_base = smem_u32(S.R);
-    uint32_t ri = 0;
+    uint32_t ri = 0, ui = 0;
     int key = -1;
     bool failed = false;
-    for (int u = u_begin, ui = 0; u < u_end; ++u, ++ui) {
+    for (int u = u_begin; u < u_end; ++u, ++ui) {
       const int p = u / C6_LT, a = u - p * C6_LT;
       if ((r_per_pair ? p : 0) != key) {      // both warpgroups follow every change of the RIGHT third
-        if (key >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&S.r_empty); }
+        if (key >= 0) S.right.release(ri - 1);
         key = r_per_pair ? p : 0;
-        INFLIGHT_WAIT(&S.r_full, ri & 1, 231);
+        INFLIGHT_WAIT(S.right.wait(ri), kErrCorrRightConsumer);
         ++ri;
       }
-      if ((ui & 1) != wg) continue;
-      const uint32_t s = ui % C6_RING;
-      INFLIGHT_WAIT(&S.full[s], (ui / C6_RING) & 1, 232);
+      if ((int)(ui & 1) != wg) continue;
+      const uint32_t s = S.left.slot(ui);
+      INFLIGHT_WAIT(S.left.wait(ui), kErrCorrLeftConsumer);
       const uint32_t l_base = smem_u32(S.L[s]);
       float acc[64];
 #pragma unroll
@@ -807,9 +770,8 @@ k_corr_wgmma(const __half* __restrict__ Lc, const int32_t* __restrict__ l_idx, c
       }
       wgmma_commit();
       wgmma_wait<0>();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&S.empty[s]);
-      named_bar_sync(1 + wg, 128);            // this warpgroup's previous diagonal sums have read Gw
+      S.left.release(ui);
+      named_bar_sync(1 + wg, 128);           // this warpgroup's previous diagonal sums have read Gw
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         float* r0 = Gw + (wi * 16 + g) * C6_GPITCH + j * 8 + 2 * t;
@@ -1061,6 +1023,9 @@ k_dense_finalize(const float* __restrict__ partial, const float* __restrict__ bd
   if (threadIdx.x == 0) overlap[p] = (*err != 0) ? __int_as_float(0x7fc00000) : 1.0f / (1.0f + expf(-(red[0] + bd[0])));
 }
 
+constexpr size_t L1_DIRECT_SMEM = 48 * 1024;           // k_leg_layer1_direct: one kernel row of the weights
+constexpr size_t L1_SMALL_SMEM = 200 * 1024;           // k_leg_layer1_small: all of them
+
 // Leg layer 1 (5x15 stride (2,2), C_in = 4..25 -> 16, ReLU) straight from the fp32 NHWC input
 // image to the hi/lo fp16 planes layer 2 reads.  K = kh*kw*C_in is only 300 for the geometric cues
 // and N = 16: as a 64x64-tiled SIMT GEMM this took 61 us of a 245 us single-scan leg.  One thread
@@ -1233,6 +1198,10 @@ static int leg_split(const ovn_handle* h, const ConvSpec& L, int n) {
 int tc_pack_weights(ovn_handle* h) {
   if (!tc_supported(h))
     OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "precision f16_tc supports leg_output_width=360, conv1size=15 only");
+  const ConvSpec& L1 = h->leg[0];              // leg_forward_tc runs layer 1 on k_leg_layer1_small or _direct only
+  const size_t l1_row_bytes = (size_t)L1.kw * L1.cin * L1.cout * sizeof(float);
+  if (L1.cout != 16 || l1_row_bytes > L1_DIRECT_SMEM || l1_row_bytes * L1.kh > L1_SMALL_SMEM)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "tensor-core leg: layer %s does not fit k_leg_layer1_direct / _small", L1.name);
   // h->tc, complete or not at all: a failed re-pack leaves no half-built state for the heads to read.  The old
   // state is freed first, so that the new one can use its memory.
   h->tc.reset();
@@ -1372,33 +1341,10 @@ int tc_pack_weights(ovn_handle* h) {
   OVN_CUDA(h, cudaMemset(t->mu, 0, CF * sizeof(float)));
   OVN_CUDA(h, cudaMemset(t->o1, 0, (size_t)120 * t->rows_pad * 8 * sizeof(__half)));
   OVN_CUDA(h, cudaMemset(t->x3, 0, (size_t)16 * t->rows_pad * 8 * sizeof(__half)));
-  OVN_CUDA(h, cudaFuncSetAttribute(k_leg_layer1_small<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  OVN_CUDA(h, cudaFuncSetAttribute(k_leg_layer1_small<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  OVN_CUDA(h, cudaFuncSetAttribute(k_leg_layer1_small<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L1_SMALL_SMEM));
+  OVN_CUDA(h, cudaFuncSetAttribute(k_leg_layer1_small<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L1_SMALL_SMEM));
   h->tc = std::move(t);
   return OVN_OK;
-}
-
-// fp32 NHWC [n][H][W][C] -> hi/lo fp16 C8-interleaved planes [n][H][hi,lo][C/8][W][8]
-__global__ void __launch_bounds__(256)
-k_nhwc_to_planes(const float* __restrict__ x, int64_t total_chunks, int H, int W, int C8, __half* __restrict__ out) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;      // (img, h, c8, w)
-  if (i >= total_chunks) return;
-  const int w = (int)(i % W);
-  int64_t r = i / W;
-  const int c8 = (int)(r % C8); r /= C8;                                   // r = img*H + h
-  const float* src = x + (r * W + w) * (int64_t)(C8 * 8) + c8 * 8;
-  const float4 a = __ldg(reinterpret_cast<const float4*>(src));
-  const float4 b = __ldg(reinterpret_cast<const float4*>(src + 4));
-  const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-  __half hi[8], lo[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    hi[e] = __float2half_rn(v[e]);
-    lo[e] = __float2half_rn(v[e] - __half2float(hi[e]));
-  }
-  const int64_t plane_hi = r * (2 * C8) + c8;
-  *reinterpret_cast<uint4*>(out + ((size_t)plane_hi * W + w) * 8) = *reinterpret_cast<const uint4*>(hi);
-  *reinterpret_cast<uint4*>(out + ((size_t)(plane_hi + C8) * W + w) * 8) = *reinterpret_cast<const uint4*>(lo);
 }
 
 int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cudaStream_t s) {
@@ -1408,19 +1354,18 @@ int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cuda
   if (!t) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "tensor-core weights not packed");
   prof_mark(h, PROF_LEG, s);
   {
-    const ConvSpec& L = h->leg[0];
-    const int64_t chunks = (int64_t)n * L.h_out * (L.cout / 8) * L.w_out;
+    const ConvSpec& L = h->leg[0];                 // tc_pack_weights checked that both kernels take its shape
     const size_t w_bytes = (size_t)L.kw * L.cin * L.cout * sizeof(float);        // one kernel row of taps
     const size_t w_all = w_bytes * L.kh;
-    if (n <= 2 && w_all <= 200 * 1024 && L.cout % 8 == 0) {
-      const unsigned grid = (unsigned)((chunks + 255) / 256);
+    if (n <= 2) {
+      const unsigned grid = (unsigned)(((int64_t)n * L.h_out * (L.cout / 8) * L.w_out + 255) / 256);
       if (L.cin == 4)
         k_leg_layer1_small<true><<<grid, 256, w_all, s>>>(d_input, h->d_w[0], h->d_b[0], n, L.h_in, L.w_in, L.cin, L.kh, L.kw,
                                                          L.sh, L.sw, L.h_out, L.w_out, L.cout, L.relu, t->actp[0]);
       else
         k_leg_layer1_small<false><<<grid, 256, w_all, s>>>(d_input, h->d_w[0], h->d_b[0], n, L.h_in, L.w_in, L.cin, L.kh, L.kw,
                                                           L.sh, L.sw, L.h_out, L.w_out, L.cout, L.relu, t->actp[0]);
-    } else if (w_bytes <= 48 * 1024 && L.cout == 16) {
+    } else {
       const int64_t work = (int64_t)n * L.h_out * ((L.w_out + 1) / 2);          // one thread per pixel pair
       const unsigned grid = (unsigned)((work + 511) / 512);
       if (L.cin == 4)
@@ -1429,11 +1374,6 @@ int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cuda
       else
         k_leg_layer1_direct<false><<<grid, 512, w_bytes, s>>>(d_input, h->d_w[0], h->d_b[0], n, L.h_in, L.w_in, L.cin, L.kh, L.kw,
                                                              L.sh, L.sw, L.h_out, L.w_out, L.relu, t->actp[0]);
-    } else {
-      int rc = leg_layer_fp32(h, 0, d_input, h->d_act[0], n, s);
-      if (rc != OVN_OK) return rc;
-      k_nhwc_to_planes<<<(unsigned)((chunks + 255) / 256), 256, 0, s>>>(h->d_act[0], chunks, L.h_out, L.w_out,
-                                                                       L.cout / 8, t->actp[0]);
     }
     OVN_LAUNCH_CHECK(h);
   }
@@ -1610,82 +1550,63 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
     int rc = d_query ? calibrate_all(h, d_query, nullptr, t->mu_set, s) : calibrate_all(h, d_bank, d_right, t->mu_set, s);
     if (rc != OVN_OK) return rc;
   }
-  if (d_query) {
-    k_gather_rows_f16<<<(unsigned)((per + 255) / 256), 256, 0, s>>>(d_query, nullptr, 1, t->mu, 0, t->r16);
+  // resident bank: the LEFT operand copies already exist, the kernels index them through `lidx`
+  // (indices arrive bounds-checked against bank_size; rows past the prepared range raise kErrRowNotPrepared)
+  const bool resident = (t->pb_key == d_bank) && t->pb_rows > 0;
+  const __half* l16 = resident ? t->pb_l16 : t->l16;
+  const __half* lc = resident ? t->pb_lc : t->lc;
+  int32_t* lidx = nullptr;
+  if (resident) {
+    lidx = h->d_idx_san + 2 * (size_t)maxp;
+    int rc = sanitize_indices(h, d_left, n, t->pb_rows, kErrRowNotPrepared, lidx, s);
+    if (rc != OVN_OK) return rc;
+  } else {
+    k_gather_rows_f16<<<(unsigned)((n * per + 255) / 256), 256, 0, s>>>(d_bank, d_left, n, t->mu, 0, t->l16);
     OVN_LAUNCH_CHECK(h);
   }
+  if (d_query) k_gather_rows_f16<<<(unsigned)((per + 255) / 256), 256, 0, s>>>(d_query, nullptr, 1, t->mu, 0, t->r16);
+  else k_gather_rows_f16<<<(unsigned)((n * per + 255) / 256), 256, 0, s>>>(d_bank, d_right, n, t->mu, 0, t->r16);
+  OVN_LAUNCH_CHECK(h);
+  const int64_t M = (int64_t)n * PAIR_ROWS;
+  const int64_t tiles = (M + TC_ROWS - 1) / TC_ROWS;                 // 256-row tiles of c_conv2 / c_conv3
+  const int grid2 = tiles < h->sm_count ? (int)tiles : h->sm_count;
+  const int grid3 = 2 * tiles < h->sm_count ? (int)(2 * tiles) : h->sm_count;
+  prof_mark(h, PROF_DELTA, s);
+  const int64_t units = (int64_t)n * NB;
+  const int grid4 = units < h->sm_count ? (int)units : h->sm_count;
+  k_delta_conv1_wgmma<<<grid4, K4_THREADS, sizeof(K4Smem), s>>>(l16, lidx, t->r16, d_query ? 0 : 1, t->w1p, t->mu_o1, t->o1,
+                                                               n, h->d_err);
+  prof_mark(h, PROF_DELTA, s);
+  OVN_LAUNCH_CHECK(h);
   const bool inject_fault = getenv("OVN_DEBUG_FAULT") != nullptr;            // error-path test hook
-  for (int p0 = 0; p0 < n; p0 += maxp) {
-    const int np = (n - p0 < maxp) ? n - p0 : maxp;
-    const int32_t* left = d_left + p0;
-    const int32_t* right = d_right ? d_right + p0 : nullptr;
-    // resident bank: the LEFT operand copies already exist, the kernels index them through `left`
-    // (indices arrive bounds-checked against bank_size; rows past the prepared range raise error 901)
-    const bool resident = (t->pb_key == d_bank) && t->pb_rows > 0;
-    const __half* l16 = resident ? t->pb_l16 : t->l16;
-    const __half* lc = resident ? t->pb_lc : t->lc;
-    const int32_t* lidx = resident ? left : nullptr;
-    if (resident) {
-      int rc = sanitize_indices(h, left, np, t->pb_rows, kErrRowNotPrepared, h->d_idx_san + 2 * (size_t)maxp, s);
-      if (rc != OVN_OK) return rc;
-      lidx = left = h->d_idx_san + 2 * (size_t)maxp;
-    } else {
-      k_gather_rows_f16<<<(unsigned)((np * per + 255) / 256), 256, 0, s>>>(d_bank, left, np, t->mu, 0, t->l16);
-      OVN_LAUNCH_CHECK(h);
-    }
-    if (!d_query) {
-      k_gather_rows_f16<<<(unsigned)((np * per + 255) / 256), 256, 0, s>>>(d_bank, right, np, t->mu, 0, t->r16);
-      OVN_LAUNCH_CHECK(h);
-    }
-    const int64_t M = (int64_t)np * PAIR_ROWS;
-    const int64_t tiles = (M + TC_ROWS - 1) / TC_ROWS;                 // 256-row tiles of c_conv2 / c_conv3
-    const int grid2 = tiles < h->sm_count ? (int)tiles : h->sm_count;
-    const int grid3 = 2 * tiles < h->sm_count ? (int)(2 * tiles) : h->sm_count;
-    prof_mark(h, PROF_DELTA, s);
-    const int64_t units = (int64_t)np * NB;
-    const int grid4 = units < h->sm_count ? (int)units : h->sm_count;
-    k_delta_conv1_wgmma<<<grid4, K4_THREADS, sizeof(K4Smem), s>>>(l16, lidx, t->r16, d_query ? 0 : 1, t->w1p, t->mu_o1, t->o1,
-                                                                 np, h->d_err);
-    prof_mark(h, PROF_DELTA, s);
+  prof_mark(h, PROF_CONV2, s);
+  k_conv2_wgmma<<<grid2, TC_THREADS, C2_SMEM, s>>>(t->o1, t->w2p, t->b2eff, t->mu_x3, t->x3, t->rows_pad, M,
+                                                   inject_fault ? 1 : 0, h->d_err);
+  prof_mark(h, PROF_CONV2, s);
+  OVN_LAUNCH_CHECK(h);
+  prof_mark(h, PROF_CONV3, s);
+  k_conv3_wgmma<<<grid3, TC_THREADS, sizeof(C3Smem), s>>>(t->x3, t->rows_pad, t->w3p, t->b3eff, M, h->d_w[base + 3],
+                                                          t->partial, h->d_err);
+  prof_mark(h, PROF_CONV3, s);
+  OVN_LAUNCH_CHECK(h);
+  k_dense_finalize<<<n, 256, 0, s>>>(t->partial, h->d_b[base + 3], PAIR_ROWS, d_overlap, h->d_err);
+  OVN_LAUNCH_CHECK(h);
+  // correlation head (tensor cores, hi/lo split operands)
+  const int64_t perL = 16 * C6_LT * C6_LROWS, perR = 16 * C6_RT * C6_RROWS;
+  if (!resident) {
+    k_pack_corr<C6_LROWS, C6_LT><<<(unsigned)((n * perL + 255) / 256), 256, 0, s>>>(d_bank, d_left, n, t->lc);
     OVN_LAUNCH_CHECK(h);
-    prof_mark(h, PROF_CONV2, s);
-    k_conv2_wgmma<<<grid2, TC_THREADS, C2_SMEM, s>>>(t->o1, t->w2p, t->b2eff, t->mu_x3, t->x3, t->rows_pad, M,
-                                                     inject_fault ? 1 : 0, h->d_err);
-    prof_mark(h, PROF_CONV2, s);
-    OVN_LAUNCH_CHECK(h);
-    prof_mark(h, PROF_CONV3, s);
-    k_conv3_wgmma<<<grid3, TC_THREADS, sizeof(C3Smem), s>>>(t->x3, t->rows_pad, t->w3p, t->b3eff, M, h->d_w[base + 3],
-                                                            t->partial, h->d_err);
-    prof_mark(h, PROF_CONV3, s);
-    OVN_LAUNCH_CHECK(h);
-    k_dense_finalize<<<np, 256, 0, s>>>(t->partial, h->d_b[base + 3], PAIR_ROWS, d_overlap + p0, h->d_err);
-    OVN_LAUNCH_CHECK(h);
-    // correlation head (tensor cores, hi/lo split operands)
-    {
-      const int64_t perL = 16 * C6_LT * C6_LROWS, perR = 16 * C6_RT * C6_RROWS;
-      if (!resident) {
-        k_pack_corr<C6_LROWS, C6_LT><<<(unsigned)((np * perL + 255) / 256), 256, 0, s>>>(d_bank, left, np, t->lc);
-        OVN_LAUNCH_CHECK(h);
-      }
-      if (d_query) {
-        if (p0 == 0) {
-          k_pack_corr<C6_RROWS, C6_RT><<<(unsigned)((perR + 255) / 256), 256, 0, s>>>(d_query, nullptr, 1, t->rc);
-          OVN_LAUNCH_CHECK(h);
-        }
-      } else {
-        k_pack_corr<C6_RROWS, C6_RT><<<(unsigned)((np * perR + 255) / 256), 256, 0, s>>>(d_bank, right, np, t->rc);
-        OVN_LAUNCH_CHECK(h);
-      }
-      prof_mark(h, PROF_CORR, s);
-      const int64_t units = (int64_t)np * C6_LT;
-      const int nc = units < h->sm_count / C6_RT ? (int)units : h->sm_count / C6_RT;
-      k_corr_wgmma<<<nc * C6_RT, C6_THREADS, sizeof(C6Smem), s>>>(lc, lidx, t->rc, d_query ? 0 : 1, np, t->corr_part, h->d_err);
-      prof_mark(h, PROF_CORR, s);
-      OVN_LAUNCH_CHECK(h);
-      k_corr_finalize<<<np, 384, 0, s>>>(t->corr_part, d_corr ? d_corr + (int64_t)p0 * WF : nullptr, d_yaw + p0, h->d_err);
-      OVN_LAUNCH_CHECK(h);
-    }
   }
+  if (d_query) k_pack_corr<C6_RROWS, C6_RT><<<(unsigned)((perR + 255) / 256), 256, 0, s>>>(d_query, nullptr, 1, t->rc);
+  else k_pack_corr<C6_RROWS, C6_RT><<<(unsigned)((n * perR + 255) / 256), 256, 0, s>>>(d_bank, d_right, n, t->rc);
+  OVN_LAUNCH_CHECK(h);
+  prof_mark(h, PROF_CORR, s);
+  const int nc = (int64_t)n * C6_LT < h->sm_count / C6_RT ? n * C6_LT : h->sm_count / C6_RT;
+  k_corr_wgmma<<<nc * C6_RT, C6_THREADS, sizeof(C6Smem), s>>>(lc, lidx, t->rc, d_query ? 0 : 1, n, t->corr_part, h->d_err);
+  prof_mark(h, PROF_CORR, s);
+  OVN_LAUNCH_CHECK(h);
+  k_corr_finalize<<<n, 384, 0, s>>>(t->corr_part, d_corr, d_yaw, h->d_err);
+  OVN_LAUNCH_CHECK(h);
   static const bool debug_sync = getenv("OVN_DEBUG_SYNC") != nullptr;
   if (debug_sync) return check_device_error(h, s);
   return OVN_OK;

@@ -85,8 +85,8 @@ def test_host_entry_point_reports_bad_candidates(bank_np):
 
 
 def test_pipeline_failure_is_reported(bank_np):
-  """OVN_DEBUG_FAULT makes k_conv2_mma skip its work and raise the pipeline-failure flag: the finalize
-  kernels poison the outputs and the next synchronising call returns OVN_ERR_CUDA."""
+  """OVN_DEBUG_FAULT makes k_conv2_wgmma skip its work and raise the pipeline-failure flag: the finalize
+  kernels poison the outputs and the next synchronising call returns OVN_ERR_CUDA, naming the fault."""
   eng = Engine(model=MODEL, precision='f16_tc', max_batch_scans=1, max_batch_pairs=8)
   eng.load_weights(N.glorot_weights(4, MODEL, seed=0))
   bank = torch.from_numpy(bank_np).to(eng.device)
@@ -95,7 +95,7 @@ def test_pipeline_failure_is_reported(bank_np):
   os.environ['OVN_DEBUG_FAULT'] = '1'
   try:
     ov, yaw, _ = eng.heads_1vsN(bank, bank[0], n_cand=6)
-    with pytest.raises(OvnError, match='OVN_ERR_CUDA.*pipeline failed'):
+    with pytest.raises(OvnError, match='OVN_ERR_CUDA.*pipeline failed: k_conv2_wgmma: fault injected.*code 501'):
       eng.check()
     assert torch.isnan(ov).all() and (yaw == -2 ** 31).all()
   finally:
