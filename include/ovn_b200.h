@@ -237,8 +237,24 @@ int ovn_head_gradients(ovn_handle* h, const float* d_bank, int64_t bank_size,
  * a += g^2; w -= lr g / (sqrt(a) + 1e-7), accumulators start at 0); refuses (INVALID_ARG) when there are
  * none.  ovn_finalize_weights resets the accumulators. */
 int ovn_head_adagrad_step(ovn_handle* h, float learning_rate, void* stream);
+/* ---- training of the whole network (legsType 360OutputkLegs, generateNet.py:119-219) ----------
+ * fp32 handles only (OVN_ERR_BAD_CONFIG otherwise); n_pairs <= max_batch_pairs and n_pairs <= 485 at
+ * leg_output_width 360 (the launch grid of the heads' c_conv1), else OVN_ERR_CAPACITY.
+ * Forward of leg + both heads for LEFT = images[left], RIGHT = images[right] (d_images: [n_images][H][W][C]),
+ * the losses of training.py, and the backward of the whole network: the correlation head's loss now reaches
+ * the leg.  Synchronous: h_loss[3].  d_fv_grad (may be NULL) receives dL/d(LEFT volume), dL/d(RIGHT volume)
+ * as [2][n_pairs][Wf][128], before s_conv10's ReLU mask.  An index outside the image bank returns
+ * OVN_ERR_INVALID_ARG and leaves no usable gradients.  The buffers are allocated on the first call. */
+int ovn_net_gradients(ovn_handle* h, const float* d_images, int64_t n_images,
+                      const int32_t* d_left_idx, const int32_t* d_right_idx, int32_t n_pairs,
+                      const float* d_gt_overlap, const int32_t* d_gt_orientation,
+                      float min_overlap_for_angle, float* h_loss, float* d_fv_grad, void* stream);
+/* Adagrad over every leg and head layer from the last ovn_net_gradients; INVALID_ARG otherwise (also after an
+ * ovn_head_gradients call).  The head layers share their accumulators with ovn_head_adagrad_step. */
+int ovn_net_adagrad_step(ovn_handle* h, float learning_rate, void* stream);
 /* Current weights / last gradients of a layer, Keras layout, host buffers (same shapes as ovn_set_weights).
- * Both synchronise the device.  ovn_get_gradients applies to the head layers only. */
+ * Both synchronise the device.  ovn_get_gradients returns the head layers after ovn_head_gradients and every
+ * layer after ovn_net_gradients. */
 int ovn_get_weights(ovn_handle* h, const char* layer_name, float* h_kernel, float* h_bias);
 int ovn_get_gradients(ovn_handle* h, const char* layer_name, float* h_kernel, float* h_bias);
 

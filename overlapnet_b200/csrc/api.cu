@@ -400,7 +400,10 @@ int ovn_finalize_weights(ovn_handle* h) {
   }
   if (h->train) {                        // new weights: Adagrad starts over, old gradients are stale
     OVN_CUDA(h, cudaMemset(h->train->accum, 0, (size_t)h->train->n_param * sizeof(float)));
+    if (h->train->leg_accum)
+      OVN_CUDA(h, cudaMemset(h->train->leg_accum, 0, (size_t)h->train->n_leg_param * sizeof(float)));
     h->train->grads_valid = false;
+    h->train->net_grads_valid = false;
   }
   h->weights_ready = true;
   return OVN_OK;
@@ -443,11 +446,13 @@ int ovn_get_gradients(ovn_handle* h, const char* name, float* h_kernel, float* h
   int64_t nk, nb;
   bool head;
   const int slot = layer_slot(h, name, &nk, &nb, &head);
-  if (slot < 0 || !head)
-    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_get_gradients: '%s' is not a layer of the overlap head", name);
+  if (slot < 0) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_get_gradients: '%s' is not a layer of the network", name);
+  if (!head && (!h->train || !h->train->net_grads_valid))
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_get_gradients: no valid gradients of leg layer '%s' (call "
+                "ovn_net_gradients first)", name);
   if (!h->train || !h->train->grads_valid)
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_get_gradients: no valid gradients (call ovn_head_gradients first)");
-  const float* g = h->train->grad + h->train->off[slot - kMaxLegLayers];
+  const float* g = head ? h->train->grad + h->train->off[slot - kMaxLegLayers] : h->train->leg_grad + h->train->leg_off[slot];
   OVN_CUDA(h, cudaDeviceSynchronize());
   OVN_CUDA(h, cudaMemcpy(h_kernel, g, nk * sizeof(float), cudaMemcpyDeviceToHost));
   OVN_CUDA(h, cudaMemcpy(h_bias, g + nk, nb * sizeof(float), cudaMemcpyDeviceToHost));
@@ -678,6 +683,7 @@ int ovn_head_gradients(ovn_handle* h, const float* d_bank, int64_t bank_size, co
     if (rc != OVN_OK) return rc;
   }
   h->train->grads_valid = false;
+  h->train->net_grads_valid = false;
   cudaStream_t s = (cudaStream_t)stream;
   int32_t* l = h->d_idx_san;
   int32_t* r = h->d_idx_san + maxp;
@@ -703,6 +709,61 @@ int ovn_head_adagrad_step(ovn_handle* h, float learning_rate, void* stream) {
   if (!h->train || !h->train->grads_valid)
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_head_adagrad_step: no valid gradients (call ovn_head_gradients first)");
   return head_adagrad_fp32(h, learning_rate, (cudaStream_t)stream);
+}
+
+// ---- training of the whole network (360OutputkLegs) -----------------------------------------------
+int ovn_net_gradients(ovn_handle* h, const float* d_images, int64_t n_images, const int32_t* d_left_idx,
+                      const int32_t* d_right_idx, int32_t n_pairs, const float* d_gt_overlap,
+                      const int32_t* d_gt_orientation, float min_overlap_for_angle, float* h_loss, float* d_fv_grad,
+                      void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_net_gradients: %s", h->net_error.c_str());
+  if (h->cfg.precision != OVN_PREC_FP32)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_net_gradients: training needs a precision fp32 handle");
+  if (!h->weights_ready) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "ovn_net_gradients: weights not finalised");
+  REQUIRE(h, n_pairs > 0 && n_images > 0, "n_pairs and n_images must be positive");
+  REQUIRE(h, d_images && d_left_idx && d_right_idx && d_gt_overlap && d_gt_orientation && h_loss, "NULL pointer");
+  const int maxp = h->cfg.max_batch_pairs;
+  if (n_pairs > maxp)
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "ovn_net_gradients: n_pairs=%d exceeds max_batch_pairs=%d", n_pairs, maxp);
+  if (n_pairs > net_max_pairs(h))
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "ovn_net_gradients: n_pairs=%d exceeds the %d pairs one call can launch", n_pairs,
+                net_max_pairs(h));
+  if (!h->train) {
+    int rc = train_alloc(h);
+    if (rc != OVN_OK) return rc;
+  }
+  h->train->grads_valid = false;
+  h->train->net_grads_valid = false;
+  cudaStream_t s = (cudaStream_t)stream;
+  int32_t* l = h->d_idx_san;
+  int32_t* r = h->d_idx_san + maxp;
+  int rc = sanitize_indices(h, d_left_idx, n_pairs, n_images, kErrBadIndex, l, s);
+  if (rc == OVN_OK) rc = sanitize_indices(h, d_right_idx, n_pairs, n_images, kErrBadIndex, r, s);
+  if (rc == OVN_OK)
+    rc = net_gradients_fp32(h, d_images, l, r, n_pairs, d_gt_overlap, d_gt_orientation, min_overlap_for_angle,
+                            d_fv_grad, s);
+  if (rc != OVN_OK) return rc;
+  float* p_loss = h->stage()->loss;
+  OVN_CUDA(h, cudaMemcpyAsync(p_loss, h->train->loss, 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  rc = check_device_error(h, s);            // synchronises s; a bad index -> OVN_ERR_INVALID_ARG
+  if (rc != OVN_OK) return rc;
+  memcpy(h_loss, p_loss, 3 * sizeof(float));
+  h->train->grads_valid = true;
+  h->train->net_grads_valid = true;
+  return OVN_OK;
+}
+
+int ovn_net_adagrad_step(ovn_handle* h, float learning_rate, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  if (h->cfg.precision != OVN_PREC_FP32)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_net_adagrad_step: training needs a precision fp32 handle");
+  if (!h->train || !h->train->net_grads_valid)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_net_adagrad_step: no valid whole-network gradients (call "
+                "ovn_net_gradients first)");
+  return net_adagrad_fp32(h, learning_rate, (cudaStream_t)stream);
 }
 
 int ovn_bank_prepare(ovn_handle* h, const float* d_bank, int64_t bank_capacity, int64_t first, int64_t count,

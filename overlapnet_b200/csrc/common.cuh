@@ -107,7 +107,21 @@ struct TrainState {
   Buffer<float> loss;           // [3] total, overlap, orientation
   int64_t off[4] = {};
   int64_t n_param = 0;
-  bool grads_valid = false;     // the last ovn_head_gradients succeeded
+  bool grads_valid = false;     // the last ovn_head_gradients / ovn_net_gradients succeeded
+  // Whole-network training (ovn_net_gradients): allocated on its first call, the per-batch buffers grown to
+  // the batch.  The 2n images of an n-pair batch are LEFT 0..n-1, then RIGHT 0..n-1.
+  Buffer<float> images;         // [2n][H][W][C] the gathered input images
+  Buffer<float> acts;           // every leg layer's output for those images, layer after layer
+  Buffer<float> dact[2];        // ping-pong gradients of the leg activations (dact[0] first holds dL/d(volumes))
+  Buffer<float> dfv_part;       // k_delta_dgrad partials: LEFT [n][nb][Wf][128], then RIGHT [n][row tiles][Wf][128]
+  Buffer<float> dcorr;          // [n][Wf] dL/d(correlation logits)
+  Buffer<int32_t> pair_rows;    // [2n] 0..2n-1: LEFT / RIGHT rows of the batch's volumes
+  Buffer<float> wt;             // a leg kernel with in / out swapped
+  Buffer<float> leg_grad;       // [n_leg_param] per leg layer [K + 1][N] at leg_off[l], like grad
+  Buffer<float> leg_accum;      // [n_leg_param] Adagrad accumulators
+  int64_t leg_off[kMaxLegLayers] = {};
+  int64_t n_leg_param = 0;
+  bool net_grads_valid = false; // the last ovn_net_gradients succeeded (leg_grad and grad are of one batch)
 };
 }  // namespace ovn
 
@@ -303,6 +317,12 @@ int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left,
                         const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
                         cudaStream_t s);
 int head_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s);
+// training of the whole network (network_fp32.cu): left / right index the image bank and are bounds-checked
+int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left, const int32_t* right, int np,
+                       const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
+                       float* d_fv_grad, cudaStream_t s);
+int net_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s);
+int net_max_pairs(const ovn_handle* h);   // largest n_pairs of one ovn_net_gradients call (launch grid limits)
 
 int corr_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* left,
                       const int32_t* right, int np, int32_t* d_yaw, float* d_corr, cudaStream_t s);

@@ -170,6 +170,34 @@ struct ConvDgradOperand {
   }
 };
 
+// Input gradient of a strided valid conv:  A[m, k] = dY[img, (h - dh) / sh, (w - dw) / sw, n] where both
+// divisions are exact and land inside dY, else 0.  m = (img, h, w), k = (dh, dw, n), B as in ConvDgradOperand.
+// An input row that no output reads (row H - 1 of an even-height input under a stride-2, 3-row kernel) gets 0.
+struct ConvDgradStridedOperand {
+  const float* dY;
+  int Ho, Wo, Cout, kw, H, W, sh, sw;
+  __device__ __forceinline__ int64_t row_base(int m, int) const { return (int64_t)(m / (H * W)) * Ho * Wo * Cout; }
+  __device__ __forceinline__ int64_t row_base2(int m, int) const {
+    const int t = m / W;
+    return ((int64_t)(t % H) << 16) | (m % W);
+  }
+  __device__ __forceinline__ int col_off(int k) const { return k % Cout; }
+  __device__ __forceinline__ int col_off2(int k) const {
+    const int rowlen = kw * Cout;
+    const int dh = k / rowlen;
+    return (dh << 16) | ((k - dh * rowlen) / Cout);
+  }
+  __device__ __forceinline__ float load(int64_t rb, int n, int64_t hw, int tap) const {
+    int y = (int)(hw >> 16) - (tap >> 16);
+    int x = (int)(hw & 0xffff) - (tap & 0xffff);
+    if (y < 0 || x < 0 || y % sh || x % sw) return 0.f;
+    y /= sh;
+    x /= sw;
+    if (y >= Ho || x >= Wo) return 0.f;
+    return __ldg(dY + rb + ((int64_t)y * Wo + x) * Cout + n);
+  }
+};
+
 struct BOperand {
   const float* B;             // weights [K][N] (b_nk = 0) or per-batch [N][K] (b_nk = 1)
   const float* query;         // b_nk: RIGHT volume = query for every z when non-null
@@ -640,6 +668,363 @@ int head_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s) {
     k_adagrad<<<blocks_for(nk), 256, 0, s>>>(h->d_w[kMaxLegLayers + l], g, a, nk, lr);
     OVN_LAUNCH_CHECK(h);
     k_adagrad<<<blocks_for(N), 256, 0, s>>>(h->d_b[kMaxLegLayers + l], g + nk, a + nk, N, lr);
+    OVN_LAUNCH_CHECK(h);
+  }
+  return OVN_OK;
+}
+
+// ---- training of the whole network (360OutputkLegs) -------------------------------------------
+// The leg is trained too: the gradient of both heads flows back into the two feature volumes (through |l - r|
+// and the correlation head) and from there through the leg's convolutions.  Same rules as the head: fp32,
+// fixed-order reductions, no floating-point atomics.
+
+constexpr int kDgT = 64;         // k_delta_dgrad tile: 64 rows i x 64 channels c, K = the 64 c_conv1 outputs
+constexpr int kCorrRows = 8;     // k_corr_backward: output rows per CTA
+
+// out[v] = images[left[v]] for v < np, images[right[v - np]] for v >= np  (indices already bounds-checked)
+__global__ void k_gather_images(const float* __restrict__ images, const int32_t* __restrict__ left,
+                                const int32_t* __restrict__ right, int np, int64_t img, float* __restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 2 * np * img) return;
+  const int v = (int)(i / img);
+  const int src = v < np ? left[v] : right[v - np];
+  out[i] = __ldg(images + (int64_t)src * img + (i - (int64_t)v * img));
+}
+
+__global__ void k_pair_rows(int32_t* __restrict__ rows, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) rows[i] = i;
+}
+
+// dL/d(correlation logit) of the orientation loss of k_train_loss (loss weight 1):
+//   dcorr[p, k] = ((1 - t) - (1 + (Wf - 1) t) sigmoid(-corr)) / (np Wf),  t = [k == gt_or_p and gt_ov_p > min_ov]
+__global__ void k_corr_dlogit(const float* __restrict__ corr, const float* __restrict__ gt_ov,
+                              const int32_t* __restrict__ gt_or, int np, int Wf, float min_ov, float* __restrict__ dcorr) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= np * Wf) return;
+  const int p = e / Wf, k = e - p * Wf;
+  const float t = (k == gt_or[p] && gt_ov[p] > min_ov) ? 1.f : 0.f;
+  const float sg = 1.f / (1.f + expf(corr[e]));
+  dcorr[e] = ((1.f - t) - (1.f + ((float)Wf - 1.f) * t) * sg) / ((float)np * (float)Wf);
+}
+
+// Backward of corr[p, k] = sum_{j,c} L[(k + j + Wf/2) mod Wf, c] R[j, c]  (RangePadding2D.py:31-38 +
+// NormalizedCorrelation2D.py:96-109), a circulant times a volume:
+//   side 0: dL[p, i, :] = sum_j dcorr[p, (i - j - Wf/2) mod Wf] R[j, :]  -> dfv[p]
+//   side 1: dR[p, j, :] = sum_i dcorr[p, (i - j - Wf/2) mod Wf] L[i, :]  -> dfv[np + p]
+// CTA = (kCorrRows output rows, pair, side), one thread per channel; the sum runs over q in order.
+__global__ void __launch_bounds__(kFeatC)
+k_corr_backward(const float* __restrict__ dcorr, const float* __restrict__ fv, const int32_t* __restrict__ left,
+                const int32_t* __restrict__ right, int np, int Wf, float* __restrict__ dfv) {
+  extern __shared__ float s_d[];
+  const int r0 = blockIdx.x * kCorrRows, p = blockIdx.y, side = blockIdx.z, c = threadIdx.x;
+  for (int k = c; k < Wf; k += kFeatC) s_d[k] = dcorr[(int64_t)p * Wf + k];
+  __syncthreads();
+  const float* X = fv + (int64_t)(side ? left[p] : right[p]) * Wf * kFeatC;
+  const int half = Wf / 2;
+  // index of dcorr for output row r0 + rr and input row q: side 0 (r0 + rr - q - half), side 1 (q - r0 - rr - half)
+  int base = side ? (-r0 - half) % Wf : (r0 - half) % Wf;
+  if (base < 0) base += Wf;
+  float acc[kCorrRows] = {};
+  for (int q = 0; q < Wf; ++q) {
+    const float x = __ldg(X + (int64_t)q * kFeatC + c);
+#pragma unroll
+    for (int rr = 0; rr < kCorrRows; ++rr) {
+      int idx = side ? base - rr : base + rr;   // wraps once when Wf >= kCorrRows, more often below that
+      while (idx < 0) idx += Wf;
+      while (idx >= Wf) idx -= Wf;
+      acc[rr] = fmaf(s_d[idx], x, acc[rr]);
+    }
+    base = side ? (base + 1 == Wf ? 0 : base + 1) : (base == 0 ? Wf - 1 : base - 1);
+  }
+#pragma unroll
+  for (int rr = 0; rr < kCorrRows; ++rr)
+    if (r0 + rr < Wf) dfv[(((int64_t)side * np + p) * Wf + r0 + rr) * kFeatC + c] = acc[rr];
+}
+
+// Backward of c_conv1 on |l - r| (generateNet.py:45-59,96-100) without the 66 MB delta tensor.  With
+// do1[p, i, jb, o] = dL/d(c_conv1 output) (h->d_o1, stored [p][ho][jb][dh][o], i = s ho + dh), j = s jb + dj:
+//   G[i, dj, c] = sum_o do1[p, i, jb, o] W1[dj, c, o],   sg = sign(L[i, c] - R[j, c])  (sign(0) = 0, TF's abs)
+//   dL[p, i, c] = sum_{jb, dj} sg G,   dR[p, j, c] = -sum_i sg G
+// CTA = (64 channels, 64 rows i, jb + nb p): the do1 tile stays in shared memory while the CTA loops over the
+// s taps dj; each tap is a 64 x 64 x 64 product in registers whose epilogue applies the signs.  Fixed-order
+// partials, reduced by k_delta_dgrad_reduce:  part_l[p][jb][i][c] (this CTA's sum over dj) and
+// part_r[p][row tile][j][c] (this CTA's sum over its 64 rows, in order).
+__global__ void __launch_bounds__(256)
+k_delta_dgrad(const float* __restrict__ do1, const float* __restrict__ w1, const float* __restrict__ fv,
+              const int32_t* __restrict__ left, const int32_t* __restrict__ right, int Wf, int s, int nb, int nho,
+              float* __restrict__ part_l, float* __restrict__ part_r) {
+  __shared__ __align__(16) float As[kDgT][kDgT + 4];     // [o][i]
+  __shared__ __align__(16) float Bs[kDgT][kDgT + 4];     // [o][c]
+  __shared__ float red[16][kDgT];
+  const int tid = threadIdx.x, ty = tid / 16, tx = tid % 16;
+  const int c0 = blockIdx.x * kDgT, itile = blockIdx.y, i0 = itile * kDgT;
+  const int jb = blockIdx.z % nb, p = blockIdx.z / nb;
+  const int nit = gridDim.y;
+  // The tiles are stored transposed: a thread reads 4 consecutive o of one row and consecutive threads take
+  // consecutive rows, so the shared-memory stores of a warp hit 32 different banks.
+  for (int f = tid; f < kDgT * kDgT / 4; f += 256) {
+    const int r = f % kDgT, o = (f / kDgT) * 4, i = i0 + r;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (i < Wf) {
+      const int ho = i / s, dh = i - ho * s;
+      v = __ldg(reinterpret_cast<const float4*>(do1 + ((((int64_t)p * nho + ho) * nb + jb) * s + dh) * kDgT + o));
+    }
+    As[o][r] = v.x; As[o + 1][r] = v.y; As[o + 2][r] = v.z; As[o + 3][r] = v.w;
+  }
+  const float* L = fv + (int64_t)left[p] * Wf * kFeatC;
+  const float* R = fv + (int64_t)right[p] * Wf * kFeatC;
+  float lv[4][4], accl[4][4];
+#pragma unroll
+  for (int ii = 0; ii < 4; ++ii) {
+    const int i = i0 + ty * 4 + ii;
+    const float4 v = i < Wf ? __ldg(reinterpret_cast<const float4*>(L + (int64_t)i * kFeatC + c0 + tx * 4))
+                            : make_float4(0.f, 0.f, 0.f, 0.f);
+    lv[ii][0] = v.x; lv[ii][1] = v.y; lv[ii][2] = v.z; lv[ii][3] = v.w;
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) accl[ii][jj] = 0.f;
+  }
+  for (int dj = 0; dj < s; ++dj) {
+    for (int f = tid; f < kDgT * kDgT / 4; f += 256) {
+      const int c = f % kDgT, o = (f / kDgT) * 4;
+      const float4 v = __ldg(reinterpret_cast<const float4*>(w1 + ((int64_t)dj * kFeatC + c0 + c) * kDgT + o));
+      Bs[o][c] = v.x; Bs[o + 1][c] = v.y; Bs[o + 2][c] = v.z; Bs[o + 3][c] = v.w;
+    }
+    __syncthreads();
+    float acc[4][4] = {};
+#pragma unroll 8
+    for (int o = 0; o < kDgT; ++o) {
+      const float4 a = *reinterpret_cast<const float4*>(&As[o][ty * 4]);
+      const float4 b = *reinterpret_cast<const float4*>(&Bs[o][tx * 4]);
+      const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+      for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) acc[ii][jj] = fmaf(av[ii], bv[jj], acc[ii][jj]);
+    }
+    const int j = s * jb + dj;
+    const float4 r4 = __ldg(reinterpret_cast<const float4*>(R + (int64_t)j * kFeatC + c0 + tx * 4));
+    const float rv[4] = {r4.x, r4.y, r4.z, r4.w};
+    float col[4] = {};
+#pragma unroll
+    for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const float d = lv[ii][jj] - rv[jj];
+        const float v = d > 0.f ? acc[ii][jj] : (d < 0.f ? -acc[ii][jj] : 0.f);
+        accl[ii][jj] += v;
+        col[jj] += v;
+      }
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) red[ty][tx * 4 + jj] = col[jj];
+    __syncthreads();
+    if (tid < kDgT) {
+      float v = 0.f;
+#pragma unroll
+      for (int y = 0; y < 16; ++y) v += red[y][tid];
+      part_r[(((int64_t)p * nit + itile) * Wf + j) * kFeatC + c0 + tid] = -v;
+    }
+  }
+#pragma unroll
+  for (int ii = 0; ii < 4; ++ii) {
+    const int i = i0 + ty * 4 + ii;
+    if (i < Wf)
+      *reinterpret_cast<float4*>(part_l + (((int64_t)p * nb + jb) * Wf + i) * kFeatC + c0 + tx * 4) =
+          make_float4(accl[ii][0], accl[ii][1], accl[ii][2], accl[ii][3]);
+  }
+}
+
+// dfv[v] += the partials of volume v in order: LEFT p (v = p) sums nb partials, RIGHT p (v = np + p) nit
+__global__ void k_delta_dgrad_reduce(const float* __restrict__ part_l, const float* __restrict__ part_r, int np, int nb,
+                                     int nit, int64_t vol, float* __restrict__ dfv) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 2 * np * vol) return;
+  const int v = (int)(i / vol);
+  const int64_t e = i - (int64_t)v * vol;
+  const float* src = v < np ? part_l + (int64_t)v * nb * vol + e : part_r + (int64_t)(v - np) * nit * vol + e;
+  const int n = v < np ? nb : nit;
+  float acc = dfv[i];
+  for (int z = 0; z < n; ++z) acc += src[(int64_t)z * vol];
+  dfv[i] = acc;
+}
+
+constexpr int64_t kMaxGridY = 65535;   // k_simt_gemm puts row tiles on grid.y, k_delta_dgrad pairs x jb on grid.z
+
+// Images per k_simt_gemm launch of the leg, whose rows are `rows` per image: the row tiles must fit grid.y.
+// Every output element is computed the same way in any launch, so splitting changes no result.
+static int images_per_launch(int64_t rows) {
+  const int64_t n = kMaxGridY * BM / rows;
+  return n < 1 ? 1 : (int)(n > INT32_MAX ? INT32_MAX : n);
+}
+
+// The largest batch ovn_net_gradients can launch: the heads put np * 360 * 24 rows of c_conv1 on one grid
+// (485 pairs at Wf = 360), k_delta_dgrad puts np * 24 CTAs on grid.z.  The leg launches split over images.
+int net_max_pairs(const ovn_handle* h) {
+  const int64_t by_rows = kMaxGridY * BM / ((int64_t)h->o1_h * h->o1_w);
+  const int64_t by_z = kMaxGridY / h->o1_w;
+  return (int)(by_rows < by_z ? by_rows : by_z);
+}
+
+// [K][N] size of leg layer l's kernel
+static int64_t leg_kernel_size(const ConvSpec& L) { return (int64_t)L.kh * L.kw * L.cin * L.cout; }
+
+// The whole-network buffers of an np-pair batch; the leg gradients and accumulators on first use
+static int net_alloc(ovn_handle* h, int np) {
+  TrainState& t = *h->train;
+  const int64_t n2 = 2 * (int64_t)np, Wf = h->cfg.leg_output_width, vol = Wf * kFeatC;
+  const int64_t img = (int64_t)h->cfg.proj_H * h->cfg.proj_W * h->C;
+  const int nb = h->o1_w, nit = (int)((Wf + kDgT - 1) / kDgT);
+  int64_t acts = 0, max_act = vol, max_w = 0, max_part = 0;
+  for (int l = 0; l < h->n_leg; ++l) {
+    const ConvSpec& L = h->leg[l];
+    const int64_t a = (int64_t)L.h_out * L.w_out * L.cout;
+    acts += a;
+    if (a > max_act) max_act = a;
+    if (l > 0 && (int64_t)L.h_in * L.w_in * L.cin > max_act) max_act = (int64_t)L.h_in * L.w_in * L.cin;
+    if (leg_kernel_size(L) > max_w) max_w = leg_kernel_size(L);
+    const int64_t g = ((int64_t)L.kh * L.kw * L.cin + 1) * L.cout;
+    if (g > max_part) max_part = g;
+  }
+  int rc;
+  if ((rc = t.images.ensure(h, (size_t)(n2 * img) * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t.acts.ensure(h, (size_t)(n2 * acts) * sizeof(float))) != OVN_OK) return rc;
+  for (int k = 0; k < 2; ++k)
+    if ((rc = t.dact[k].ensure(h, (size_t)(n2 * max_act) * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t.dfv_part.ensure(h, (size_t)(np * (int64_t)(nb + nit) * vol) * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t.dcorr.ensure(h, (size_t)(np * Wf) * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t.pair_rows.ensure(h, (size_t)n2 * sizeof(int32_t))) != OVN_OK) return rc;
+  if ((rc = t.wt.ensure(h, (size_t)max_w * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t.part.ensure(h, (size_t)kMaxSplit * max_part * sizeof(float))) != OVN_OK) return rc;
+  if (!t.leg_grad) {
+    int64_t total = 0;
+    for (int l = 0; l < h->n_leg; ++l) {
+      t.leg_off[l] = total;
+      total += leg_kernel_size(h->leg[l]) + h->leg[l].cout;
+    }
+    if ((rc = t.leg_accum.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
+    OVN_CUDA(h, cudaMemset(t.leg_accum, 0, (size_t)total * sizeof(float)));
+    if ((rc = t.leg_grad.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
+    t.n_leg_param = total;
+  }
+  return OVN_OK;
+}
+
+// Forward of the leg on the 2 np gathered images (the launches of leg_forward_fp32, every output kept), both
+// heads, the losses, and the backward of the whole network.  Head gradients land in train->grad, leg gradients
+// in train->leg_grad, the losses in train->loss; d_fv_grad (may be null) receives dL/d(volumes) before
+// s_conv10's ReLU mask, [2][np][Wf][128].
+int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left, const int32_t* right, int np,
+                       const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
+                       float* d_fv_grad, cudaStream_t s) {
+  int rc = net_alloc(h, np);
+  if (rc != OVN_OK) return rc;
+  TrainState& t = *h->train;
+  const int Wf = h->cfg.leg_output_width, n2 = 2 * np, sz = h->cfg.conv1size;
+  const int64_t img = (int64_t)h->cfg.proj_H * h->cfg.proj_W * h->C, vol = (int64_t)Wf * kFeatC;
+  const int nb = h->o1_w, nit = (Wf + kDgT - 1) / kDgT;
+  k_gather_images<<<blocks_for(n2 * img), 256, 0, s>>>(d_images, left, right, np, img, t.images);
+  OVN_LAUNCH_CHECK(h);
+  // leg forward
+  float* act[kMaxLegLayers];
+  {
+    float* y = t.acts;
+    const float* x = t.images;
+    prof_mark(h, PROF_LEG, s);
+    for (int l = 0; l < h->n_leg; ++l) {
+      const ConvSpec& L = h->leg[l];
+      act[l] = y;
+      BOperand b{h->d_w[l], nullptr, nullptr, 0, 0};
+      const int per = images_per_launch((int64_t)L.h_out * L.w_out);
+      for (int i0 = 0; i0 < n2; i0 += per) {
+        const int ni = n2 - i0 < per ? n2 - i0 : per;
+        ConvOperand a{x + (int64_t)i0 * L.h_in * L.w_in * L.cin, L.h_in, L.w_in, L.cin, L.kw, L.sh, L.sw, L.h_out,
+                      L.w_out};
+        rc = launch_gemm(h, a, b, h->d_b[l], y + (int64_t)i0 * L.h_out * L.w_out * L.cout, ni * L.h_out * L.w_out,
+                         L.cout, L.kh * L.kw * L.cin, 1, L.relu, s);
+        if (rc != OVN_OK) return rc;
+      }
+      x = y;
+      y += (int64_t)n2 * L.h_out * L.w_out * L.cout;
+    }
+    prof_mark(h, PROF_LEG, s);
+  }
+  const float* fv = act[h->n_leg - 1];
+  k_pair_rows<<<blocks_for(n2), 256, 0, s>>>(t.pair_rows, n2);
+  OVN_LAUNCH_CHECK(h);
+  const int32_t* lrow = t.pair_rows;
+  const int32_t* rrow = t.pair_rows + np;
+  // both heads forward, losses, overlap-head backward: do1 = dL/d(c_conv1 output) is left in h->d_o1
+  rc = head_gradients_fp32(h, fv, lrow, rrow, np, d_gt_overlap, d_gt_orientation, min_overlap, s);
+  if (rc != OVN_OK) return rc;
+  // dL/d(volumes) = correlation-head part + |l - r| part
+  float* dfv = t.dact[0];
+  k_corr_dlogit<<<blocks_for((int64_t)np * Wf), 256, 0, s>>>(t.corr, d_gt_overlap, d_gt_orientation, np, Wf,
+                                                              min_overlap, t.dcorr);
+  OVN_LAUNCH_CHECK(h);
+  k_corr_backward<<<dim3((Wf + kCorrRows - 1) / kCorrRows, np, 2), kFeatC, Wf * sizeof(float), s>>>(
+      t.dcorr, fv, lrow, rrow, np, Wf, dfv);
+  OVN_LAUNCH_CHECK(h);
+  float* part_l = t.dfv_part;
+  float* part_r = part_l + (int64_t)np * nb * vol;
+  k_delta_dgrad<<<dim3(kFeatC / kDgT, nit, nb * np), 256, 0, s>>>(h->d_o1, h->d_w[kMaxLegLayers], fv, lrow, rrow, Wf,
+                                                                   sz, nb, h->head[1].h_out, part_l, part_r);
+  OVN_LAUNCH_CHECK(h);
+  k_delta_dgrad_reduce<<<blocks_for(n2 * vol), 256, 0, s>>>(part_l, part_r, np, nb, nit, vol, dfv);
+  OVN_LAUNCH_CHECK(h);
+  if (d_fv_grad) OVN_CUDA(h, cudaMemcpyAsync(d_fv_grad, dfv, (size_t)(n2 * vol) * sizeof(float),
+                                             cudaMemcpyDeviceToDevice, s));
+  // leg backward: dy = dL/d(pre-activation of layer l), then its weight + bias gradient and its input gradient
+  float* dy = dfv;
+  float* dx = t.dact[1];
+  k_relu_grad<<<blocks_for(n2 * vol), 256, 0, s>>>(dy, fv, n2 * vol);
+  OVN_LAUNCH_CHECK(h);
+  for (int l = h->n_leg - 1; l >= 0; --l) {
+    const ConvSpec& L = h->leg[l];
+    const float* X = l ? act[l - 1] : t.images;
+    const int Kc = L.kh * L.kw * L.cin;
+    ConvWgradOperand a{X, L.h_in, L.w_in, L.cin, L.kw, L.sh, L.sw, L.h_out, L.w_out, Kc};
+    rc = wgrad_gemm(h, a, dy, Kc, L.cout, n2 * L.h_out * L.w_out, t.leg_grad + t.leg_off[l], s);
+    if (rc != OVN_OK) return rc;
+    if (l == 0) break;
+    k_swap_io<<<blocks_for(leg_kernel_size(L)), 256, 0, s>>>(h->d_w[l], t.wt, L.kh * L.kw, L.cin, L.cout);
+    OVN_LAUNCH_CHECK(h);
+    BOperand b{t.wt, nullptr, nullptr, 0, 0};
+    const int64_t rows_in = (int64_t)L.h_in * L.w_in, K = L.kh * L.kw * L.cout;
+    const int per = images_per_launch(rows_in);
+    for (int i0 = 0; i0 < n2 && rc == OVN_OK; i0 += per) {
+      const int ni = n2 - i0 < per ? n2 - i0 : per;
+      const float* dyi = dy + (int64_t)i0 * L.h_out * L.w_out * L.cout;
+      float* dxi = dx + (int64_t)i0 * rows_in * L.cin;
+      if (L.sh == 1 && L.sw == 1) {
+        ConvDgradOperand d{dyi, L.h_out, L.w_out, L.cout, L.kw, L.h_in, L.w_in};
+        rc = launch_gemm(h, d, b, nullptr, dxi, (int)(ni * rows_in), L.cin, (int)K, 1, 0, s);
+      } else {
+        ConvDgradStridedOperand d{dyi, L.h_out, L.w_out, L.cout, L.kw, L.h_in, L.w_in, L.sh, L.sw};
+        rc = launch_gemm(h, d, b, nullptr, dxi, (int)(ni * rows_in), L.cin, (int)K, 1, 0, s);
+      }
+    }
+    if (rc != OVN_OK) return rc;
+    const int64_t nx = n2 * rows_in * L.cin;
+    k_relu_grad<<<blocks_for(nx), 256, 0, s>>>(dx, X, nx);
+    OVN_LAUNCH_CHECK(h);
+    float* tmp = dy;
+    dy = dx;
+    dx = tmp;
+  }
+  return OVN_OK;
+}
+
+int net_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s) {
+  int rc = head_adagrad_fp32(h, lr, s);
+  if (rc != OVN_OK) return rc;
+  TrainState& t = *h->train;
+  for (int l = 0; l < h->n_leg; ++l) {
+    const int64_t nk = leg_kernel_size(h->leg[l]), N = h->leg[l].cout;
+    float* g = t.leg_grad + t.leg_off[l];
+    float* a = t.leg_accum + t.leg_off[l];
+    k_adagrad<<<blocks_for(nk), 256, 0, s>>>(h->d_w[l], g, a, nk, lr);
+    OVN_LAUNCH_CHECK(h);
+    k_adagrad<<<blocks_for(N), 256, 0, s>>>(h->d_b[l], g + nk, a + nk, N, lr);
     OVN_LAUNCH_CHECK(h);
   }
   return OVN_OK;

@@ -17,6 +17,13 @@ FEAT_C = 128
 HEAD_LAYERS = ('c_conv1', 'c_conv2', 'c_conv3', 'overlap_output')
 
 
+def leg_layers(model=None):
+  """Names of the leg layers (generateNet.py:161-217) of a ``model:`` section, input to output: s_conv3a
+  only with ``additional_unsymmetric_layer3a``."""
+  use3a = bool(dict(model or {}).get('additional_unsymmetric_layer3a', False))
+  return tuple(name for name, *_, opt in _weights.LEG_TABLE if use3a or not opt)
+
+
 def _ptr(t):
   return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
@@ -357,6 +364,44 @@ class Engine:
     """ovn_head_adagrad_step: Adagrad update of the head weights from the last gradients."""
     check(self._h, lib().ovn_head_adagrad_step(self._h, float(lr), self._stream()), 'ovn_head_adagrad_step')
 
+  # ---- training of the whole network (fp32 handles) -------------------------------------------------
+  def net_gradients(self, images, left_idx, right_idx, gt_overlap, gt_orientation, min_overlap_for_angle=0.7,
+                    fv_grad=False):
+    """ovn_net_gradients: forward of leg + both heads for LEFT = images[left_idx], RIGHT = images[right_idx]
+    (``images`` [n, H, W, C] float32 cuda), the losses of training.py and the backward of every layer.
+    Synchronous; returns the losses (total, overlap, orientation), plus dL/d(volumes) [2, n, Wf, 128] before
+    s_conv10's ReLU mask when ``fv_grad``.  The batch gradients stay in the handle."""
+    n = left_idx.numel()
+    dev = self.device
+    x = images.contiguous()
+    li = left_idx.to(device=dev, dtype=torch.int32).contiguous()
+    ri = right_idx.to(device=dev, dtype=torch.int32).contiguous()
+    gov = torch.as_tensor(gt_overlap).to(device=dev, dtype=torch.float32).contiguous()
+    gor = torch.as_tensor(gt_orientation).to(device=dev, dtype=torch.int32).contiguous()
+    assert ri.numel() == n and gov.numel() == n and gor.numel() == n
+    assert tuple(x.shape[1:]) == (self.H, self.W, self.C) and x.dtype == torch.float32
+    dfv = torch.empty((2, n, self.Wf, FEAT_C), dtype=torch.float32, device=dev) if fv_grad else None
+    loss = np.zeros(3, np.float32)
+    check(self._h, lib().ovn_net_gradients(self._h, _ptr(x), int(x.shape[0]), _ptr(li), _ptr(ri), n, _ptr(gov),
+                                          _ptr(gor), float(min_overlap_for_angle), loss.ctypes.data_as(C.c_void_p),
+                                          _ptr(dfv), self._stream()), 'ovn_net_gradients')
+    loss = tuple(float(v) for v in loss)
+    return (loss, dfv) if fv_grad else loss
+
+  def net_adagrad_step(self, lr):
+    """ovn_net_adagrad_step: Adagrad update of every leg and head layer from the last net_gradients."""
+    check(self._h, lib().ovn_net_adagrad_step(self._h, float(lr), self._stream()), 'ovn_net_adagrad_step')
+
+  @property
+  def leg_layers(self):
+    """Names of the leg layers of this handle's config, input to output."""
+    return leg_layers(self.model)
+
+  @property
+  def layers(self):
+    """Every layer of this handle's config: the leg layers, then HEAD_LAYERS."""
+    return self.leg_layers + HEAD_LAYERS
+
   def _layer_shapes(self):
     return _weights.layer_shapes(self.C, self.model, self.H, self.W)
 
@@ -378,7 +423,8 @@ class Engine:
     return self._read_layers(lib().ovn_get_weights, names, 'ovn_get_weights')
 
   def get_gradients(self, names=HEAD_LAYERS):
-    """Gradients of the last head_gradients call {layer name: (kernel, bias)}, head layers only."""
+    """Gradients of the last head_gradients call {layer name: (kernel, bias)} (head layers), or of the last
+    net_gradients call (any layer, e.g. ``names=eng.layers``)."""
     return self._read_layers(lib().ovn_get_gradients, names, 'ovn_get_gradients')
 
   # ---- host-buffer entry points (synchronous) ------------------------------------------------

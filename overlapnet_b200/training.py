@@ -9,8 +9,11 @@ computed and logged as part of the total loss like training.py does.
 
   python -m overlapnet_b200.training config.yml
 
-Not supported (an Exception says so): a trainable leg (legsType 360OutputkLegs), ``rotate_training_data``
-(it would re-encode the rolled RIGHT image for every pair of every epoch) and TensorBoard output.
+The same command trains the whole network when the config's legsType is 360OutputkLegs: ``main`` hands such
+a config to ``overlapnet_b200.training_leg``, which runs this loop with the leg's backward added.
+
+Not supported (an Exception says so): ``rotate_training_data`` (it would re-encode the rolled RIGHT image for
+every pair of every epoch) and TensorBoard output.
 """
 import logging
 import os
@@ -40,10 +43,15 @@ def check_config(config):
   model = config['model']
   legs = model.get('legsType')
   if legs == '360OutputkLegs':
-    raise Exception('legsType 360OutputkLegs trains the leg, which needs the backward of the leg '
-                    'convolutions and of |l - r|; only 360OutputkLegsFixed (frozen leg) is supported')
+    raise Exception('legsType 360OutputkLegs trains the leg: that is overlapnet_b200.training_leg (python -m '
+                    'overlapnet_b200.training dispatches it); this flow trains 360OutputkLegsFixed (frozen leg)')
   if legs != '360OutputkLegsFixed':
     raise Exception('legsType %r is not supported for training; use 360OutputkLegsFixed' % (legs,))
+  check_unsupported_options(config)
+
+
+def check_unsupported_options(config):
+  """Options neither training flow implements."""
   if config.get('rotate_training_data', 0) != 0:
     raise Exception('rotate_training_data != 0 is not supported: with a frozen leg it would re-encode the '
                     'rolled RIGHT image of every pair in every epoch')
@@ -94,11 +102,36 @@ def save_weights(path, weights):
     _weights.save_npz(f, weights)
 
 
+class FrozenLeg:
+  """The training step of 360OutputkLegsFixed: every distinct scan is encoded once by the frozen leg into a
+  feature bank on the GPU; a step trains the overlap head on it."""
+
+  def __init__(self, infer, keys):
+    logger.info('Encoding %d scans with the frozen leg ...', len(keys))
+    self.eng = infer._engine
+    self.bank, self.rows = _encode_bank(infer, keys)
+
+  def step(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, lr):
+    loss = self.eng.head_gradients(self.bank, left, right, gt_overlap, gt_orientation, min_overlap_for_angle)
+    self.eng.adagrad_step(lr)
+    return loss
+
+  def evaluate(self, left, right):
+    """(overlap, yaw) device tensors of the validation pairs with the current weights."""
+    ov, yaw, _ = self.eng.heads(self.bank, left, right)
+    return ov, yaw
+
+
 def train(config, device=None):
   """Run the training of training.py for a loaded YAML dict.  Returns a dict with the per-epoch
   losses, the batch losses, the validation statistics and the weight file name."""
-  from .infer import Infer
   check_config(config)
+  return run(config, device, FrozenLeg)
+
+
+def run(config, device, flow):
+  """The loop of training.py with ``flow`` (FrozenLeg or training_leg.WholeNetwork) making the steps."""
+  from .infer import Infer
   model = config['model']
   root = config.get('data_root_folder', '')
   imgpath = config.get('imgpath', root)
@@ -110,13 +143,13 @@ def train(config, device=None):
   if logger.level == logging.NOTSET or logger.level > logging.INFO:
     logger.setLevel(logging.INFO)
   try:
-    return _train(config, model, imgpath, out_dir, device, Infer)
+    return _train(config, model, imgpath, out_dir, device, Infer, flow)
   finally:
     logger.removeHandler(handler)
     handler.close()
 
 
-def _train(config, model, imgpath, out_dir, device, Infer):
+def _train(config, model, imgpath, out_dir, device, Infer, flow):
   weights_filename = os.path.join(out_dir, model['modelType'] + '_' + config['testname'] + '.weight')
   initial_lr = float(config['learning_rate'])
   lr_alpha = float(config.get('lr_alpha', 0.99))
@@ -151,8 +184,8 @@ def _train(config, model, imgpath, out_dir, device, Infer):
     logger.info('Load old weights from %s', cfg['pretrained_weightsfilename'])
 
   keys = set(zip(t_d1, t_f1)) | set(zip(t_d2, t_f2)) | set(zip(v_d1, v_f1)) | set(zip(v_d2, v_f2))
-  logger.info('Encoding %d scans with the frozen leg ...', len(keys))
-  bank, rows = _encode_bank(infer, keys)
+  steps = flow(infer, keys)
+  rows = steps.rows
   dev = eng.device
   t_left = torch.tensor([rows[k] for k in zip(t_d1, t_f1)], dtype=torch.int32, device=dev)
   t_right = torch.tensor([rows[k] for k in zip(t_d2, t_f2)], dtype=torch.int32, device=dev)
@@ -173,9 +206,7 @@ def _train(config, model, imgpath, out_dir, device, Infer):
     losses, sizes = [], []
     for b in np.random.permutation(n_batches):                     # Keras reshuffles a Sequence's batches
       s0, s1 = b * batch_size, min(n, (b + 1) * batch_size)
-      loss = eng.head_gradients(bank, t_left[s0:s1], t_right[s0:s1], t_ov_d[s0:s1], t_or_d[s0:s1],
-                                min_overlap_for_angle)
-      eng.adagrad_step(lr)
+      loss = steps.step(t_left[s0:s1], t_right[s0:s1], t_ov_d[s0:s1], t_or_d[s0:s1], min_overlap_for_angle, lr)
       losses.append(loss)
       sizes.append(s1 - s0)
       logger.info('  epoch %d batch %d: loss %.6f (overlap %.6f, orientation %.6f)', epoch + 1, len(losses),
@@ -188,7 +219,7 @@ def _train(config, model, imgpath, out_dir, device, Infer):
     save_weights(weights_filename, eng.get_weights())
 
     logger.info('  Evaluation on test data ...')                                       # training.py:352-415
-    ov, yaw, _ = eng.heads(bank, v_left, v_right)
+    ov, yaw = steps.evaluate(v_left, v_right)
     eng.check()
     overlap = ov.cpu().numpy().astype(np.float64)
     argmax = width // 2 - yaw.cpu().numpy().astype(np.int64)
@@ -212,7 +243,12 @@ def main(argv=None):
   logging.basicConfig(format='%(message)s', level=logging.INFO)
   configfilename = argv[0] if argv else 'network.yml'                                  # training.py:102-104
   logger.info('Using configuration file %s.', configfilename)
-  train(load_config(configfilename))
+  config = load_config(configfilename)
+  if config['model'].get('legsType') == '360OutputkLegs':      # the reference's default (network.yml:70)
+    from . import training_leg
+    training_leg.train(config)
+  else:
+    train(config)
 
 
 if __name__ == '__main__':
