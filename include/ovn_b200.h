@@ -186,7 +186,8 @@ int ovn_leg_forward(ovn_handle* h, const float* d_input, int32_t n_scans, float*
 /* ---- stage 3: heads (generateNet.py:15-116, 327-354; readout infer.py:157-158) ------------- */
 /* Pair p uses LEFT = d_bank[left_idx[p]], RIGHT = d_bank[right_idx[p]]
  * (ImagePairOverlapSequenceFeatureVolume.py:44-45).  Outputs: d_overlap [n] f32,
- * d_yaw [n] i32 = 180 - argmax(corr) (first maximum), d_corr [n][360] f32 or NULL. */
+ * d_yaw [n] i32 = 180 - argmax(corr) (first maximum; 180 at every leg_output_width, as infer.py:158),
+ * d_corr [n][leg_output_width] f32 or NULL. */
 int ovn_heads_forward(ovn_handle* h, const float* d_bank, int64_t bank_size,
                       const int32_t* d_left_idx, const int32_t* d_right_idx, int32_t n_pairs,
                       float* d_overlap, int32_t* d_yaw, float* d_corr, void* stream);

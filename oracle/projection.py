@@ -56,11 +56,8 @@ def point_depth(points):
   return _norm3_rows(np.ascontiguousarray(points[:, :3], dtype=F32))
 
 
-def projection_bins(points, fov_up=3.0, fov_down=-25.0, proj_H=64, proj_W=900, max_range=50):
-  """Per-point (valid mask, depth, proj_y, proj_x) following utils.py:69-104.
-
-  ``valid`` is the filter of utils.py:76-77; bins are int32 and only meaningful where valid.
-  """
+def projection_prefloor(points, fov_up=3.0, fov_down=-25.0, proj_H=64, proj_W=900):
+  """Per-point (depth, proj_y, proj_x) following utils.py:69-95: the float32 values the reference floors."""
   points = np.asarray(points)
   if points.dtype != F32:
     raise TypeError('oracle.projection handles the float32 path only (gen_*_data.py read .bin as float32)')
@@ -69,8 +66,6 @@ def projection_bins(points, fov_up=3.0, fov_down=-25.0, proj_H=64, proj_W=900, m
   fov = abs(fov_down_r) + abs(fov_up_r)
 
   depth = point_depth(points)                # utils.py:75
-  with np.errstate(invalid='ignore'):
-    valid = (depth > 0) & (depth < F32(max_range))          # utils.py:76-77 (weak scalar -> float32)
   x, y, z = points[:, 0], points[:, 1], points[:, 2]
 
   with np.errstate(all='ignore'):
@@ -84,7 +79,18 @@ def projection_bins(points, fov_up=3.0, fov_down=-25.0, proj_H=64, proj_W=900, m
     proj_y = F32(1.0) - (pitch + F32(abs(fov_down_r))) / F32(fov)
     proj_x = proj_x * F32(proj_W)
     proj_y = proj_y * F32(proj_H)
+  return depth, proj_y, proj_x
 
+
+def projection_bins(points, fov_up=3.0, fov_down=-25.0, proj_H=64, proj_W=900, max_range=50):
+  """Per-point (valid mask, depth, proj_y, proj_x) following utils.py:69-104.
+
+  ``valid`` is the filter of utils.py:76-77; bins are int32 and only meaningful where valid.
+  """
+  depth, proj_y, proj_x = projection_prefloor(points, fov_up, fov_down, proj_H, proj_W)
+  with np.errstate(invalid='ignore'):
+    valid = (depth > 0) & (depth < F32(max_range))          # utils.py:76-77 (weak scalar -> float32)
+  with np.errstate(all='ignore'):
     # utils.py:98-104
     proj_x = np.maximum(F32(0), np.minimum(F32(proj_W - 1), np.floor(proj_x)))
     proj_y = np.maximum(F32(0), np.minimum(F32(proj_H - 1), np.floor(proj_y)))
@@ -162,13 +168,13 @@ def gen_normal_map(current_range, current_vertex, proj_H=64, proj_W=900):
   return out
 
 
-def gen_semantic_image(points, probs, proj_H=64, proj_W=900):
+def gen_semantic_image(points, probs, proj_H=64, proj_W=900, fov_up=3.0, fov_down=-25.0):
   """Oracle of the per-scan body of ``gen_semantic_data`` (gen_semantic_data.py:36-46).
 
   Reproduces the reference's quirk: ``proj_idx`` indexes the filtered cloud but is used to index
   the unfiltered ``probs``.
   """
-  _, _, _, proj_idx = range_projection(points, proj_H=proj_H, proj_W=proj_W, max_range=np.inf)
+  _, _, _, proj_idx = range_projection(points, fov_up, fov_down, proj_H=proj_H, proj_W=proj_W, max_range=np.inf)
   proj_prob = np.full((proj_H, proj_W, probs.shape[1]), -1, dtype=F32)
   proj_prob[proj_idx >= 0] = probs[proj_idx[proj_idx >= 0]]
   return proj_prob

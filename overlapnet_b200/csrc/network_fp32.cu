@@ -320,7 +320,8 @@ k_dense_sigmoid(const float* __restrict__ o3, const float* __restrict__ wd, cons
 
 // ---- circular diagonal sums of the Gram matrix + argmax readout -------------------------------
 //   corr[k] = sum_j G[(k + j + W/2) mod W, j]      (RangePadding2D.py:34 + NormalizedCorrelation2D.py:96-109)
-//   yaw     = W/2 - argmax_k corr[k], first maximum (infer.py:158)
+//   yaw     = 180 - argmax_k corr[k], first maximum, at every Wf (infer.py:158, :198, :233 subtract from the
+//             literal 180, not from Wf / 2)
 __global__ void __launch_bounds__(384)
 k_corr_readout(const float* __restrict__ G, int Wf, float* __restrict__ corr_out, int32_t* __restrict__ yaw) {
   extern __shared__ float s_corr[];
@@ -343,7 +344,7 @@ k_corr_readout(const float* __restrict__ G, int Wf, float* __restrict__ corr_out
     float bv = s_corr[0];
     for (int k = 1; k < Wf; ++k)
       if (s_corr[k] > bv) { bv = s_corr[k]; best = k; }
-    yaw[p] = Wf / 2 - best;
+    yaw[p] = 180 - best;
   }
 }
 

@@ -940,7 +940,7 @@ k_corr_finalize(const float* __restrict__ part, float* __restrict__ corr_out, in
     for (int k = 1; k < WF; ++k)
       if (s_corr[k] > bv) { bv = s_corr[k]; best = k; }
     // a raised error flag (pipeline failure, bad index) poisons the result: garbage never looks valid
-    yaw[p] = (*err != 0) ? INT32_MIN : WF / 2 - best;
+    yaw[p] = (*err != 0) ? INT32_MIN : 180 - best;   // infer.py:158, as k_corr_readout
   }
 }
 

@@ -18,10 +18,9 @@
 //                image with coalesced stores; normals are computed in the reference's rounding
 //                order (float32 products, double accumulate, one rounding -- NumPy's sdot).
 //   Bit-exact bins: atan2/asin are defined as the correctly rounded float32 values (oracle
-//                docstring).  The fast path evaluates atan2f/asinf (<= 2 ulp), brackets the result
-//                by +-6e-7 relative and runs the reference's float32 bin pipeline on both ends;
-//                the pipeline is monotone, so equal bins prove the bin.  Only when the bracket
-//                straddles a bin edge (~4e-4 of the points) is the float64 function evaluated.
+//                docstring).  The fast path estimates the pre-floor bin from atan2f/asinf and keeps
+//                its floor when it is further from a bin edge than a margin derived from H, W and the
+//                fov (make_params); otherwise the float64 function is evaluated (see K1).
 #include "common.cuh"
 
 namespace ovn {
@@ -35,7 +34,33 @@ struct ProjParams {
   float max_range;
   float kx, cx;          // fast estimate of the pre-floor x bin: yaw * W / (2 pi) + W / 2
   float ky, cy;          // ... and of the y bin: -pitch * H / fov + (1 - |fov_down| / fov) * H
+  float mx, my;          // the estimate decides a bin when it lies further than this from a bin edge
 };
+
+// float32 ulp in the binade of a > 0
+static double ulp32(double a) {
+  int e;
+  frexp(a, &e);
+  return ldexp(1.0, e - 24);
+}
+
+// Worst-case distance, in bins, between the fast estimate t and the exact pre-floor value P(fl32(angle))
+// (DESIGN.md section 4).  Three sources: atan2f / asinf against the correctly rounded angle (3 / 2 ulp in the
+// CUDA Programming Guide's table, + 1/2 ulp for the rounding of the exact angle), the roundings of the
+// reference's float32 pipeline (pi32 and fov32 included), and the estimate's own (kx / ky / cy and the fma).
+// x: |yaw| <= pi.  y: the estimate only decides points inside the fov, so |pitch| <= max(|fov_up|, |fov_down|).
+static double bound_x(int W) {
+  const double pi = 3.14159265358979323846, e24 = ldexp(1.0, -24);
+  const double kx = W / (2.0 * pi);
+  return kx * 3.5 * ulp32(pi) + 0.5 * W * 3.5 * e24 + ulp32(W);
+}
+static double bound_y(int H, double fu, double fd) {
+  const double e24 = ldexp(1.0, -24);
+  const double fov = fabs(fd) + fabs(fu), ky = H / fov;
+  const double pmax = fmax(fabs(fu), fabs(fd)) * (1.0 + 1e-6);
+  return ky * (2.5 * ulp32(pmax) + pmax * e24 + 0.5 * ulp32(fabs(fd)) + 0.5 * ulp32(pmax + fabs(fd))) +
+         H * 4.0 * e24 + ulp32(H);
+}
 
 static ProjParams make_params(const ovn_handle* h, float max_range) {
   ProjParams p;
@@ -55,6 +80,10 @@ static ProjParams make_params(const ovn_handle* h, float max_range) {
   p.cx = (float)(p.W / 2.0);
   p.ky = (float)(-(double)p.H / fov);
   p.cy = (float)((1.0 - fabs(fd) / fov) * p.H);
+  // twice the worst case, and never below the margins of the 64 x 900, 28-degree default (1e-3 / 1e-4, where
+  // the bounds are 2.8e-4 / 4.2e-5): the default geometry keeps its fast-path decisions
+  p.mx = (float)fmax(1e-3, 2.0 * bound_x(p.W));
+  p.my = (float)fmax(1e-4, 2.0 * bound_y(p.H, fu, fd));
   return p;
 }
 
@@ -120,11 +149,12 @@ k_project_scatter(const float4* __restrict__ pts, const int64_t* __restrict__ of
     if (valid) {
       // Bins: the exact answer is floor(P(fl32(angle))) with P the reference's float32 pipeline (bin_x /
       // bin_y, monotone) and fl32 the correctly rounded float32 angle.  Fast path: ONE fused estimate
-      // t = angle * scale + offset of the pre-floor value; all error sources together (atan2f / asinf <= 2
-      // ulp, the pipeline's four roundings, the estimate's own rounding) stay below 3.3e-4 bins for x
-      // and 3e-5 bins for y, so whenever t is further than 1e-3 (1e-4) from an integer -- and inside the
-      // image -- floor(t) IS the reference's bin.  Otherwise (0.2 % of the points) the float64 function is
-      // rounded once and pushed through the exact pipeline.  The first version ran the exact pipeline on
+      // t = angle * scale + offset of the pre-floor value; all error sources together (atan2f <= 3 ulp,
+      // asinf <= 2 ulp, the pipeline's roundings, the estimate's own) stay below bound_x / bound_y bins
+      // (2.8e-4 / 4.2e-5 at 64 x 900 and the default fov), so whenever t is further than P.mx (P.my, at
+      // least twice the bound) from an integer -- and inside the image -- floor(t) IS the reference's bin.
+      // Otherwise (0.2 % of the points at 64 x 900) the float64 function is rounded once and pushed through
+      // the exact pipeline.  The first version ran the exact pipeline on
       // both ends of an error bracket for every point: 4 correctly rounded divisions, 295 instructions per
       // point, issue-bound.
       // ---- yaw bin (utils.py:86,90,94,98-100)
@@ -134,7 +164,7 @@ k_project_scatter(const float4* __restrict__ pts, const int64_t* __restrict__ of
         const float t = fmaf(yaw_f, P.kx, P.cx);
         const float fl = floorf(t);
         const float fr = t - fl;
-        if (fr > 1e-3f && fr < 1.0f - 1e-3f && t > 1e-3f && t < P.W32 - 1e-3f) {
+        if (fr > P.mx && fr < 1.0f - P.mx && t > P.mx && t < P.W32 - P.mx) {
           bx = (int)fl;
         } else {
           const float yaw_cr = __double2float_rn(-atan2((double)p.y, (double)p.x));
@@ -149,7 +179,7 @@ k_project_scatter(const float4* __restrict__ pts, const int64_t* __restrict__ of
         const float t = fmaf(pit_f, P.ky, P.cy);
         const float fl = floorf(t);
         const float fr = t - fl;
-        if (fr > 1e-4f && fr < 1.0f - 1e-4f && t > 1e-4f && t < P.H32 - 1e-4f) {
+        if (fr > P.my && fr < 1.0f - P.my && t > P.my && t < P.H32 - P.my) {
           by = (int)fl;
         } else {
           const float pit_cr = __double2float_rn(asin((double)q));

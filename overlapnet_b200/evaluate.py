@@ -80,6 +80,12 @@ def error_statistics(model_overlap, model_argmax, gt_overlap, gt_orientation, ne
   return stats
 
 
+def yaw_to_argmax(yaw):
+  """The correlation head's argmax from the yaw ``Infer`` returns: yaw = 180 - argmax at every
+  leg_output_width (infer.py:158, :198, :233), so argmax = 180 - yaw, in [0, leg_output_width)."""
+  return 180 - np.asarray(yaw, dtype=np.int64)
+
+
 def evaluate_pairs(infer, imgf1, imgf2, gt_overlap, gt_orientation, out_dir=None):
   """Encode each distinct scan once, run the heads on every pair with LEFT = imgf1, RIGHT = imgf2
   (ImagePairOverlapSequenceFeatureVolume.py:44-45), and evaluate.  Returns (overlapmatrix (n,4)
@@ -91,7 +97,7 @@ def evaluate_pairs(infer, imgf1, imgf2, gt_overlap, gt_orientation, out_dir=None
   logger.info('Compute head for all %d test pairs ...', idx.shape[0])
   overlap, yaw = infer._run_heads(idx)
   overlap = np.squeeze(overlap, axis=1)
-  argmax = infer.network_output_size // 2 - yaw            # yaw = 180 - argmax (infer.py:158)
+  argmax = yaw_to_argmax(yaw)
   stats = error_statistics(overlap, argmax, gt_overlap, gt_orientation, infer.network_output_size)
   m = np.zeros((len(imgf1), 4))
   m[:, 0] = np.array(imgf1).astype(float)

@@ -222,7 +222,7 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow):
     ov, yaw = steps.evaluate(v_left, v_right)
     eng.check()
     overlap = ov.cpu().numpy().astype(np.float64)
-    argmax = width // 2 - yaw.cpu().numpy().astype(np.int64)
+    argmax = 180 - yaw.cpu().numpy().astype(np.int64)             # yaw = 180 - argmax (infer.py:158)
     diffs = np.abs(overlap - v_ov)
     stats = {'mean': float(np.mean(diffs)), 'max': float(np.max(diffs)),
              'rms': float(np.sqrt(np.mean(diffs * diffs))), 'learning_rate': float(lr),
