@@ -253,6 +253,20 @@ int ovn_net_gradients(ovn_handle* h, const float* d_images, int64_t n_images,
 /* Adagrad over every leg and head layer from the last ovn_net_gradients; INVALID_ARG otherwise (also after an
  * ovn_head_gradients call).  The head layers share their accumulators with ovn_head_adagrad_step. */
 int ovn_net_adagrad_step(ovn_handle* h, float learning_rate, void* stream);
+/* ---- yaw augmentation of training images (DESIGN.md section 7) ------------------------------------
+ * The reference's rotate_training_data rolls the RIGHT image by randint(0, width) columns but leaves its yaw
+ * label where it was, and rolls the normal channels without rotating the vectors
+ * (ImagePairOverlapOrientationSequence.py:76-80, 114-121, 209-212).  This is the geometric version: rolling a
+ * range image by s columns is the image of the cloud rotated about z by theta = -2 pi s / W (utils.py:86-90),
+ * so the normals are rotated by theta too and the caller moves the label by -s Wf / W bins.
+ * d_out[i][y][x][c] = d_images[d_rows[i]][y][(x - d_shift[i]) mod W][c] for i < n; the normal channels get
+ * (nx, ny) -> (cos nx - sin ny, sin nx + cos ny) with d_rot[i] = (cos theta, sin theta), rounded like NumPy's
+ * float32 (no FMA); a normal pixel equal to the fill (-1, -1, -1) and every other channel are copied.
+ * d_shift NULL = every shift 0, d_rot NULL = normals not rotated.  A row outside [0, n_images) is clamped and
+ * reported as OVN_ERR_INVALID_ARG by the next ovn_check.  Both precisions. */
+int ovn_gather_images(ovn_handle* h, const float* d_images, int64_t n_images, const int32_t* d_rows,
+                      const int32_t* d_shift, const float* d_rot /* [n][2] */, int32_t n,
+                      float* d_out /* [n][H][W][C] */, void* stream);
 /* Current weights / last gradients of a layer, Keras layout, host buffers (same shapes as ovn_set_weights).
  * Both synchronise the device.  ovn_get_gradients returns the head layers after ovn_head_gradients and every
  * layer after ovn_net_gradients. */

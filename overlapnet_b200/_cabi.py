@@ -22,7 +22,7 @@ SYMBOLS = [
     'ovn_query_cloud_vs_bank_host', 'ovn_check', 'ovn_set_feature_center', 'ovn_get_feature_center',
     'ovn_heads_rows_vs_bank', 'ovn_calibrate', 'ovn_peer_signal', 'ovn_peer_wait',
     'ovn_head_gradients', 'ovn_head_adagrad_step', 'ovn_get_weights', 'ovn_get_gradients',
-    'ovn_net_gradients', 'ovn_net_adagrad_step',
+    'ovn_net_gradients', 'ovn_net_adagrad_step', 'ovn_gather_images',
 ]
 
 
@@ -101,6 +101,7 @@ def lib():
   L.ovn_head_adagrad_step.argtypes = [vp, f32, vp]
   L.ovn_net_gradients.argtypes = [vp, vp, i64, vp, vp, i32, vp, vp, f32, vp, vp, vp]
   L.ovn_net_adagrad_step.argtypes = [vp, f32, vp]
+  L.ovn_gather_images.argtypes = [vp, vp, i64, vp, vp, vp, i32, vp, vp]
   L.ovn_get_weights.argtypes = [vp, C.c_char_p, vp, vp]
   L.ovn_get_gradients.argtypes = [vp, C.c_char_p, vp, vp]
   L.ovn_encode_clouds_host.argtypes = [vp, vp, vp, i32, vp]

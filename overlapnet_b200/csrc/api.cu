@@ -766,6 +766,15 @@ int ovn_net_adagrad_step(ovn_handle* h, float learning_rate, void* stream) {
   return net_adagrad_fp32(h, learning_rate, (cudaStream_t)stream);
 }
 
+int ovn_gather_images(ovn_handle* h, const float* d_images, int64_t n_images, const int32_t* d_rows,
+                      const int32_t* d_shift, const float* d_rot, int32_t n, float* d_out, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, n > 0 && n_images > 0, "n and n_images must be positive");
+  REQUIRE(h, d_images && d_rows && d_out, "NULL pointer");
+  return gather_images(h, d_images, n_images, d_rows, d_shift, d_rot, n, d_out, (cudaStream_t)stream);
+}
+
 int ovn_bank_prepare(ovn_handle* h, const float* d_bank, int64_t bank_capacity, int64_t first, int64_t count,
                      void* stream) {
   if (!h) return OVN_ERR_INVALID_ARG;

@@ -323,6 +323,9 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
                        float* d_fv_grad, cudaStream_t s);
 int net_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s);
 int net_max_pairs(const ovn_handle* h);   // largest n_pairs of one ovn_net_gradients call (launch grid limits)
+// yaw augmentation of training images (projection.cu): rows are bounds-checked on the device (kErrBadIndex)
+int gather_images(ovn_handle* h, const float* d_images, int64_t n_images, const int32_t* d_rows,
+                  const int32_t* d_shift, const float* d_rot, int n, float* d_out, cudaStream_t s);
 
 int corr_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* left,
                       const int32_t* right, int np, int32_t* d_yaw, float* d_corr, cudaStream_t s);

@@ -459,6 +459,43 @@ k_pack_input(const float* __restrict__ depth, const float* __restrict__ normal,
   if (intensity) o[c++] = intensity[i];
 }
 
+// out[i][y][x][c] = images[rows[i]][y][(x - shift[i]) mod W][c]: image i of the cloud rotated about z by
+// theta = -2 pi shift / W (utils.py:86-90).  The normal channels [c_normal, c_normal + 3) of that image get
+// (nx, ny) -> (cos nx - sin ny, sin nx + cos ny) in NumPy's float32 order (no FMA contraction); the
+// gen_normal_map fill (-1, -1, -1) and every other channel are copied.  One thread per output float.
+__global__ void __launch_bounds__(256)
+k_gather_images(const float* __restrict__ images, int64_t n_images, const int32_t* __restrict__ rows,
+                const int32_t* __restrict__ shift, const float* __restrict__ rot, size_t total, int H, int W, int C,
+                int c_normal, float* __restrict__ out, int* __restrict__ err) {
+  const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= total) return;
+  const int c = (int)(e % C);
+  const size_t pix = e / C;
+  const int x = (int)(pix % W);
+  const size_t iy = pix / W;
+  const int y = (int)(iy % H);
+  const int i = (int)(iy / H);
+  int64_t r = rows[i];
+  if (r < 0 || r >= n_images) {
+    if (e == (size_t)i * H * W * C) atomicCAS(err, 0, kErrBadIndex);    // one thread per image raises the flag
+    r = r < 0 ? 0 : n_images - 1;
+  }
+  int s = shift ? shift[i] % W : 0;
+  if (s < 0) s += W;
+  const int xs = x >= s ? x - s : x - s + W;
+  const float* src = images + (((size_t)r * H + y) * W + xs) * C;
+  float v = src[c];
+  if (rot && c_normal >= 0 && c >= c_normal && c < c_normal + 2) {
+    const float nx = src[c_normal], ny = src[c_normal + 1], nz = src[c_normal + 2];
+    if (!(nx == -1.f && ny == -1.f && nz == -1.f)) {
+      const float cs = rot[2 * i], sn = rot[2 * i + 1];
+      v = c == c_normal ? __fsub_rn(__fmul_rn(cs, nx), __fmul_rn(sn, ny))
+                        : __fadd_rn(__fmul_rn(sn, nx), __fmul_rn(cs, ny));
+    }
+  }
+  out[e] = v;
+}
+
 // ------------------------------------------------------------------------------------------
 // host-side drivers
 // ------------------------------------------------------------------------------------------
@@ -574,6 +611,17 @@ int pack_input(ovn_handle* h, const float* d_depth, const float* d_normal, const
   const size_t n_pix = (size_t)n_scans * h->cfg.proj_H * h->cfg.proj_W;
   k_pack_input<<<(unsigned)((n_pix + 255) / 256), 256, 0, s>>>(d_depth, d_normal, d_prob, d_intensity, n_pix,
                                                               h->C, h->cfg.n_prob_channels, d_input);
+  OVN_LAUNCH_CHECK(h);
+  return OVN_OK;
+}
+
+int gather_images(ovn_handle* h, const float* d_images, int64_t n_images, const int32_t* d_rows,
+                  const int32_t* d_shift, const float* d_rot, int n, float* d_out, cudaStream_t s) {
+  const size_t total = (size_t)n * h->cfg.proj_H * h->cfg.proj_W * h->C;
+  const int c_normal = h->cfg.use_normals ? (h->cfg.use_depth ? 1 : 0) : -1;
+  k_gather_images<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(d_images, n_images, d_rows, d_shift, d_rot, total,
+                                                                  h->cfg.proj_H, h->cfg.proj_W, h->C, c_normal, d_out,
+                                                                  h->d_err);
   OVN_LAUNCH_CHECK(h);
   return OVN_OK;
 }

@@ -278,12 +278,35 @@ class Engine:
                                        _ptr(out), self._stream()), 'ovn_pack_input')
     return out
 
+  def gather_images(self, images, rows, shifts=None, rot=None, out=None):
+    """ovn_gather_images: out[i] = images[rows[i]] rolled by shifts[i] columns with its normals rotated by
+    rot[i] = (cos theta, sin theta) (overlapnet_b200.augment).  ``images`` [n_images, H, W, C] float32 cuda;
+    ``shifts`` int32 [n] / ``rot`` float32 [n, 2] or None (no roll / no rotation); ``out`` [n, H, W, C] or None.
+    A row outside the bank raises OVN_ERR_INVALID_ARG at the next check()."""
+    dev = self.device
+    x = images.contiguous()
+    assert tuple(x.shape[1:]) == (self.H, self.W, self.C) and x.dtype == torch.float32
+    ri = torch.as_tensor(rows).to(device=dev, dtype=torch.int32).contiguous()
+    n = ri.numel()
+    sh = None if shifts is None else torch.as_tensor(shifts).to(device=dev, dtype=torch.int32).contiguous()
+    ro = None if rot is None else torch.as_tensor(rot).to(device=dev, dtype=torch.float32).contiguous()
+    assert (sh is None or sh.numel() == n) and (ro is None or tuple(ro.shape) == (n, 2))
+    if out is None:
+      out = torch.empty((n, self.H, self.W, self.C), dtype=torch.float32, device=dev)
+    assert tuple(out.shape) == (n, self.H, self.W, self.C) and out.dtype == torch.float32 and out.is_contiguous()
+    check(self._h, lib().ovn_gather_images(self._h, _ptr(x), int(x.shape[0]), _ptr(ri), _ptr(sh), _ptr(ro), n,
+                                          _ptr(out), self._stream()), 'ovn_gather_images')
+    return out
+
   # ---- network -------------------------------------------------------------------------------
-  def leg(self, x_nhwc):
-    """[n, H, W, C] float32 cuda -> feature volumes [n, 360, 128] float32 cuda."""
+  def leg(self, x_nhwc, out=None):
+    """[n, H, W, C] float32 cuda -> feature volumes [n, 360, 128] float32 cuda (written into ``out``, a contiguous
+    tensor of that shape, when given)."""
     x = x_nhwc.contiguous()
     n = x.shape[0]
-    out = torch.empty((n, self.Wf, FEAT_C), dtype=torch.float32, device=self.device)
+    if out is None:
+      out = torch.empty((n, self.Wf, FEAT_C), dtype=torch.float32, device=self.device)
+    assert tuple(out.shape) == (n, self.Wf, FEAT_C) and out.dtype == torch.float32 and out.is_contiguous()
     check(self._h, lib().ovn_leg_forward(self._h, _ptr(x), n, _ptr(out), self._stream()), 'ovn_leg_forward')
     return out
 

@@ -14,6 +14,11 @@ a config to ``overlapnet_b200.training_leg``, which runs this loop with the leg'
 
 Not supported (an Exception says so): ``rotate_training_data`` (it would re-encode the rolled RIGHT image for
 every pair of every epoch) and TensorBoard output.
+
+``yaw_augmentation: True`` (both legsTypes, default False) is the geometric version of that rotation
+(overlapnet_b200.augment): every epoch each training pair's RIGHT scan is rotated about z by a random multiple of
+the column pitch, its normals with it, and its orientation label moved to match.  Here the frozen leg encodes
+each step's rotated RIGHT images.  Validation is never augmented.
 """
 import logging
 import os
@@ -22,6 +27,7 @@ import sys
 import numpy as np
 import torch
 
+from . import augment
 from . import evaluate
 from . import weights as _weights
 from .config import load_config
@@ -48,6 +54,19 @@ def check_config(config):
   if legs != '360OutputkLegsFixed':
     raise Exception('legsType %r is not supported for training; use 360OutputkLegsFixed' % (legs,))
   check_unsupported_options(config)
+  check_yaw_augmentation(config)
+
+
+def check_yaw_augmentation(config):
+  """``yaw_augmentation: True`` needs a rotation that moves the label by whole bins: some multiple of the column
+  pitch below W (overlapnet_b200.augment)."""
+  if not config.get('yaw_augmentation', False):
+    return
+  model = config['model']
+  W, Wf = int(model['inputShape'][1]), int(model.get('leg_output_width', 360))
+  if augment.column_pitch(W, Wf) == W:
+    raise Exception('yaw_augmentation: no rotation of a W = %d image moves the Wf = %d orientation label by whole '
+                    'bins (gcd(W, Wf) = 1)' % (W, Wf))
 
 
 def check_unsupported_options(config):
@@ -106,12 +125,28 @@ class FrozenLeg:
   """The training step of 360OutputkLegsFixed: every distinct scan is encoded once by the frozen leg into a
   feature bank on the GPU; a step trains the overlap head on it."""
 
-  def __init__(self, infer, keys):
+  def __init__(self, infer, keys, rotate_keys=None):
     logger.info('Encoding %d scans with the frozen leg ...', len(keys))
     self.eng = infer._engine
     self.bank, self.rows = _encode_bank(infer, keys)
+    if rotate_keys:
+      # Yaw augmentation: the images of the scans a step may rotate, and max_batch_scans scratch rows after the
+      # bank that receive a step's rotated RIGHT volumes.
+      from .training_leg import load_image_bank
+      self.images, self.image_rows = load_image_bank(infer, rotate_keys)
+      n, B = len(self.rows), self.eng.max_batch_scans
+      self.bank = torch.cat([self.bank, self.bank.new_empty((B,) + tuple(self.bank.shape[1:]))])
+      self.scratch = torch.arange(n, n + B, dtype=torch.int32, device=self.eng.device)
 
-  def step(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, lr):
+  def step(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, lr, rotate=None):
+    """``rotate`` = (image rows, column shifts, (cos, sin)) of the batch's RIGHT scans, or None: the rotated
+    images are encoded by the frozen leg into the scratch rows, which then stand in for ``right``."""
+    if rotate is not None:
+      rows, shifts, rot = rotate
+      n, n0 = rows.numel(), len(self.rows)
+      x = self.eng.gather_images(self.images, rows, shifts, rot)
+      self.eng.leg(x, out=self.bank[n0:n0 + n])
+      right = self.scratch[:n]
     loss = self.eng.head_gradients(self.bank, left, right, gt_overlap, gt_orientation, min_overlap_for_angle)
     self.eng.adagrad_step(lr)
     return loss
@@ -158,6 +193,7 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow):
   no_epochs = int(config['no_epochs'])
   no_test_pairs = int(config['no_test_pairs'])
   min_overlap_for_angle = float(config.get('min_overlap_for_angle', 0.7))
+  yaw_augmentation = bool(config.get('yaw_augmentation', False))
 
   train_files, val_files = npz_files(config)
   logger.info('load training data ...')
@@ -184,7 +220,7 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow):
     logger.info('Load old weights from %s', cfg['pretrained_weightsfilename'])
 
   keys = set(zip(t_d1, t_f1)) | set(zip(t_d2, t_f2)) | set(zip(v_d1, v_f1)) | set(zip(v_d2, v_f2))
-  steps = flow(infer, keys)
+  steps = flow(infer, keys, set(zip(t_d2, t_f2))) if yaw_augmentation else flow(infer, keys)
   rows = steps.rows
   dev = eng.device
   t_left = torch.tensor([rows[k] for k in zip(t_d1, t_f1)], dtype=torch.int32, device=dev)
@@ -199,14 +235,30 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow):
   logger.info('  batch size is           : %d', batch_size)
   logger.info('  number of training pairs: %d', n)
   logger.info('  number of test pairs    : %d', n_val)
-  logger.info('  NO rotation of training data')
+  if yaw_augmentation:
+    W = eng.W
+    pitch = augment.column_pitch(W, width)
+    t_right_img = torch.tensor([steps.image_rows[k] for k in zip(t_d2, t_f2)], dtype=torch.int32, device=dev)
+    logger.info('  rotation of training data: RIGHT images by a random multiple of %d columns (%d bins), labels '
+                'moved', pitch, pitch * width // W)
+  else:
+    logger.info('  NO rotation of training data')
   history = {'epoch_loss': [], 'batch_losses': [], 'validation': [], 'weights_filename': weights_filename}
   for epoch in range(no_epochs):
     lr = learning_rate(epoch, initial_lr, lr_alpha)
     losses, sizes = [], []
+    t_or_epoch, rotate = t_or_d, None
+    if yaw_augmentation:                                           # one rotation per training pair and epoch
+      shifts = augment.sample_shifts(n, W, width)
+      shifts_d = torch.from_numpy(shifts).to(dev)
+      rot_d = torch.from_numpy(augment.rotation(shifts, W)).to(dev)
+      t_or_epoch = augment.move_labels(t_or_d, shifts_d, W, width)
     for b in np.random.permutation(n_batches):                     # Keras reshuffles a Sequence's batches
       s0, s1 = b * batch_size, min(n, (b + 1) * batch_size)
-      loss = steps.step(t_left[s0:s1], t_right[s0:s1], t_ov_d[s0:s1], t_or_d[s0:s1], min_overlap_for_angle, lr)
+      if yaw_augmentation:
+        rotate = (t_right_img[s0:s1], shifts_d[s0:s1], rot_d[s0:s1])
+      loss = steps.step(t_left[s0:s1], t_right[s0:s1], t_ov_d[s0:s1], t_or_epoch[s0:s1], min_overlap_for_angle, lr,
+                        rotate)
       losses.append(loss)
       sizes.append(s1 - s0)
       logger.info('  epoch %d batch %d: loss %.6f (overlap %.6f, orientation %.6f)', epoch + 1, len(losses),

@@ -12,6 +12,7 @@ weight file are those of ``overlapnet_b200.training``.
 
 Not supported (an Exception says so): ``rotate_training_data`` -- the reference rolls the RIGHT image without
 moving its yaw label (ImagePairOverlapOrientationSequence.py:112,209-212) -- and TensorBoard output.
+``yaw_augmentation: True`` is the geometric version (overlapnet_b200.training, overlapnet_b200.augment).
 """
 import torch
 
@@ -28,6 +29,7 @@ def check_config(config):
   if legs != '360OutputkLegs':
     raise Exception('legsType %r is not supported for training; use 360OutputkLegs' % (legs,))
   training.check_unsupported_options(config)
+  training.check_yaw_augmentation(config)
 
 
 def load_image_bank(infer, keys, chunk=256):
@@ -52,14 +54,27 @@ def load_image_bank(infer, keys, chunk=256):
 class WholeNetwork:
   """The training step of 360OutputkLegs on an image bank."""
 
-  def __init__(self, infer, keys):
+  def __init__(self, infer, keys, rotate_keys=None):
     self.eng = infer._engine
     self.images, self.rows = load_image_bank(infer, keys)
+    self.image_rows = self.rows
     logger.info('Loaded %d scans into the image bank (%.1f MB on the GPU)', len(self.rows),
                 self.images.numel() * 4 / 1e6)
 
-  def step(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, lr):
-    loss = self.eng.net_gradients(self.images, left, right, gt_overlap, gt_orientation, min_overlap_for_angle)
+  def step(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, lr, rotate=None):
+    """``rotate`` = (image rows, column shifts, (cos, sin)) of the batch's RIGHT scans, or None: the step then
+    trains on a 2n-image batch of the LEFT images and the rotated RIGHT images."""
+    images = self.images
+    if rotate is not None:
+      rows, shifts, rot = rotate
+      n = left.numel()
+      images = self.images.new_empty((2 * n,) + tuple(self.images.shape[1:]))
+      # LEFT is copied without a rotation: even a rotation by (1, 0) could flip the sign of a zero normal component
+      self.eng.gather_images(self.images, left, out=images[:n])
+      self.eng.gather_images(self.images, rows, shifts, rot, out=images[n:])
+      pairs = torch.arange(2 * n, dtype=torch.int32, device=self.eng.device)
+      left, right = pairs[:n], pairs[n:]
+    loss = self.eng.net_gradients(images, left, right, gt_overlap, gt_orientation, min_overlap_for_angle)
     self.eng.net_adagrad_step(lr)
     return loss
 
