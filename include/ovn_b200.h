@@ -253,6 +253,28 @@ int ovn_net_gradients(ovn_handle* h, const float* d_images, int64_t n_images,
 /* Adagrad over every leg and head layer from the last ovn_net_gradients; INVALID_ARG otherwise (also after an
  * ovn_head_gradients call).  The head layers share their accumulators with ovn_head_adagrad_step. */
 int ovn_net_adagrad_step(ovn_handle* h, float learning_rate, void* stream);
+/* ---- data-parallel training (overlapnet_b200/training.py, DESIGN.md section 6) --------------------------
+ * Each rank computes the gradients of its share of a batch with ovn_head_gradients / ovn_net_gradients, copies
+ * them into one flat float32 vector, the ranks exchange those vectors, and every rank applies the same
+ * weighted sum to its weights.  The flat layout: c_conv1..3 and overlap_output, then (whole_network != 0) every
+ * leg layer input to output; each layer [K + 1][N], its kernel in Keras layout, then its bias.
+ *   ovn_train_gradient_size: *n = the number of floats of that vector (665 025 for the heads at the default
+ *                    geometry; 1 769 137 for the whole network at C = 4 with s_conv3a).
+ *   ovn_copy_gradients: d_out[n] = the gradients of the last valid ovn_head_gradients / ovn_net_gradients call,
+ *                    asynchronous on `stream`.  fp32 handles (OVN_ERR_BAD_CONFIG otherwise); OVN_ERR_INVALID_ARG
+ *                    when there are none, or when whole_network asks for leg layers after ovn_head_gradients.
+ *   ovn_adagrad_step_sum: per element, in part order, g = w0 p0 + w1 p1 + ... (d_parts [n_parts][n], h_weights
+ *                    [n_parts] on the host; each product and sum rounded to float32, no FMA contraction; parts
+ *                    with weight 0 are skipped), then the update of ovn_head_adagrad_step (whole_network = 0) or
+ *                    ovn_net_adagrad_step with g, rounded as those calls round it: a = fma(g, g, a);
+ *                    w -= (lr g) / (sqrt(a) + 1e-7).  One part of weight 1 reproduces those calls bit for bit.
+ *                    It does not need the handle's own gradients; fp32 handles and finalised weights only.
+ *                    n_parts < 1 or a NULL pointer: OVN_ERR_INVALID_ARG; n_parts > 64: OVN_ERR_CAPACITY.  One
+ *                    launch. */
+int ovn_train_gradient_size(ovn_handle* h, int32_t whole_network, int64_t* n);
+int ovn_copy_gradients(ovn_handle* h, int32_t whole_network, float* d_out, void* stream);
+int ovn_adagrad_step_sum(ovn_handle* h, int32_t whole_network, const float* d_parts, int32_t n_parts,
+                         const float* h_weights, float learning_rate, void* stream);
 /* ---- yaw augmentation of training images (DESIGN.md section 7) ------------------------------------
  * The reference's rotate_training_data rolls the RIGHT image by randint(0, width) columns but leaves its yaw
  * label where it was, and rolls the normal channels without rotating the vectors

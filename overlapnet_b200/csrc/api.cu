@@ -766,6 +766,53 @@ int ovn_net_adagrad_step(ovn_handle* h, float learning_rate, void* stream) {
   return net_adagrad_fp32(h, learning_rate, (cudaStream_t)stream);
 }
 
+// ---- data-parallel training ---------------------------------------------------------------------------------
+int ovn_train_gradient_size(ovn_handle* h, int32_t whole_network, int64_t* n) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  REQUIRE(h, n, "NULL pointer");
+  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_train_gradient_size: %s", h->net_error.c_str());
+  *n = train_gradient_size(h, whole_network != 0);
+  return OVN_OK;
+}
+
+int ovn_copy_gradients(ovn_handle* h, int32_t whole_network, float* d_out, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  if (h->cfg.precision != OVN_PREC_FP32)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_copy_gradients: training needs a precision fp32 handle");
+  REQUIRE(h, d_out, "NULL pointer");
+  if (!h->train || !h->train->grads_valid)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_copy_gradients: no valid gradients (call ovn_head_gradients or "
+                "ovn_net_gradients first)");
+  if (whole_network && !h->train->net_grads_valid)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_copy_gradients: no valid whole-network gradients (call "
+                "ovn_net_gradients first)");
+  return copy_gradients_fp32(h, whole_network != 0, d_out, (cudaStream_t)stream);
+}
+
+int ovn_adagrad_step_sum(ovn_handle* h, int32_t whole_network, const float* d_parts, int32_t n_parts,
+                         const float* h_weights, float learning_rate, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_adagrad_step_sum: %s", h->net_error.c_str());
+  if (h->cfg.precision != OVN_PREC_FP32)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_adagrad_step_sum: training needs a precision fp32 handle");
+  if (!h->weights_ready) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "ovn_adagrad_step_sum: weights not finalised");
+  REQUIRE(h, n_parts >= 1, "n_parts must be at least 1");
+  if (n_parts > kMaxSumParts)
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "ovn_adagrad_step_sum: n_parts=%d exceeds %d", n_parts, kMaxSumParts);
+  REQUIRE(h, d_parts && h_weights, "NULL pointer");
+  if (!h->train) {
+    int rc = train_alloc(h);
+    if (rc != OVN_OK) return rc;
+  }
+  if (whole_network) {
+    int rc = leg_train_alloc(h);
+    if (rc != OVN_OK) return rc;
+  }
+  return adagrad_sum_fp32(h, whole_network != 0, d_parts, n_parts, h_weights, learning_rate, (cudaStream_t)stream);
+}
+
 int ovn_gather_images(ovn_handle* h, const float* d_images, int64_t n_images, const int32_t* d_rows,
                       const int32_t* d_shift, const float* d_rot, int32_t n, float* d_out, void* stream) {
   if (!h) return OVN_ERR_INVALID_ARG;

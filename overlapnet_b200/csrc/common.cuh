@@ -323,6 +323,14 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
                        float* d_fv_grad, cudaStream_t s);
 int net_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s);
 int net_max_pairs(const ovn_handle* h);   // largest n_pairs of one ovn_net_gradients call (launch grid limits)
+// data-parallel training (network_fp32.cu): the flat gradient vector is the heads' [n_param] and then, with
+// whole_network, the leg's [n_leg_param]
+constexpr int kMaxSumParts = 64;
+int64_t train_gradient_size(const ovn_handle* h, bool whole_network);
+int leg_train_alloc(ovn_handle* h);        // train->leg_grad / leg_accum / leg_off, once
+int copy_gradients_fp32(ovn_handle* h, bool whole_network, float* d_out, cudaStream_t s);
+int adagrad_sum_fp32(ovn_handle* h, bool whole_network, const float* d_parts, int n_parts, const float* h_weights,
+                     float lr, cudaStream_t s);
 // yaw augmentation of training images (projection.cu): rows are bounds-checked on the device (kErrBadIndex)
 int gather_images(ovn_handle* h, const float* d_images, int64_t n_images, const int32_t* d_rows,
                   const int32_t* d_shift, const float* d_rot, int n, float* d_out, cudaStream_t s);

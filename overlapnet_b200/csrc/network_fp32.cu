@@ -896,17 +896,24 @@ static int net_alloc(ovn_handle* h, int np) {
   if ((rc = t.pair_rows.ensure(h, (size_t)n2 * sizeof(int32_t))) != OVN_OK) return rc;
   if ((rc = t.wt.ensure(h, (size_t)max_w * sizeof(float))) != OVN_OK) return rc;
   if ((rc = t.part.ensure(h, (size_t)kMaxSplit * max_part * sizeof(float))) != OVN_OK) return rc;
-  if (!t.leg_grad) {
-    int64_t total = 0;
-    for (int l = 0; l < h->n_leg; ++l) {
-      t.leg_off[l] = total;
-      total += leg_kernel_size(h->leg[l]) + h->leg[l].cout;
-    }
-    if ((rc = t.leg_accum.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
-    OVN_CUDA(h, cudaMemset(t.leg_accum, 0, (size_t)total * sizeof(float)));
-    if ((rc = t.leg_grad.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
-    t.n_leg_param = total;
+  return leg_train_alloc(h);
+}
+
+// The leg gradients and accumulators, on first use (ovn_net_gradients, or ovn_adagrad_step_sum on a rank
+// that has not computed a gradient yet)
+int leg_train_alloc(ovn_handle* h) {
+  TrainState& t = *h->train;
+  if (t.leg_grad) return OVN_OK;
+  int64_t total = 0;
+  for (int l = 0; l < h->n_leg; ++l) {
+    t.leg_off[l] = total;
+    total += leg_kernel_size(h->leg[l]) + h->leg[l].cout;
   }
+  int rc;
+  if ((rc = t.leg_accum.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
+  OVN_CUDA(h, cudaMemset(t.leg_accum, 0, (size_t)total * sizeof(float)));
+  if ((rc = t.leg_grad.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
+  t.n_leg_param = total;
   return OVN_OK;
 }
 
@@ -1028,6 +1035,102 @@ int net_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s) {
     k_adagrad<<<blocks_for(N), 256, 0, s>>>(h->d_b[l], g + nk, a + nk, N, lr);
     OVN_LAUNCH_CHECK(h);
   }
+  return OVN_OK;
+}
+
+// ---- data-parallel training -------------------------------------------------------------------------
+// The flat gradient vector is train->grad (the heads) followed by train->leg_grad (the leg): each is already
+// [K + 1][N] per layer, so a copy is one or two memcpys, and the accumulators have the same layout.
+
+int64_t train_gradient_size(const ovn_handle* h, bool whole_network) {
+  int64_t n = 0;
+  for (int l = 0; l < 4; ++l) {
+    int K, N;
+    head_dims(h, l, &K, &N);
+    n += (int64_t)(K + 1) * N;
+  }
+  if (whole_network)
+    for (int l = 0; l < h->n_leg; ++l) n += leg_kernel_size(h->leg[l]) + h->leg[l].cout;
+  return n;
+}
+
+int copy_gradients_fp32(ovn_handle* h, bool whole_network, float* d_out, cudaStream_t s) {
+  const TrainState& t = *h->train;
+  OVN_CUDA(h, cudaMemcpyAsync(d_out, t.grad, (size_t)t.n_param * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  if (whole_network)
+    OVN_CUDA(h, cudaMemcpyAsync(d_out + t.n_param, t.leg_grad, (size_t)t.n_leg_param * sizeof(float),
+                                cudaMemcpyDeviceToDevice, s));
+  return OVN_OK;
+}
+
+// One weight tensor's run of the flat vector: elements [start, next segment's start) update w[i - start] and
+// a[i - start]
+struct SumSegment {
+  int64_t start;
+  float* w;
+  float* a;
+};
+constexpr int kMaxSumSegments = 2 * (kMaxLegLayers + 4);
+struct SumArgs {
+  SumSegment seg[kMaxSumSegments];   // in flat order
+  int64_t n;                         // floats per part
+  int n_seg;
+  int n_parts;                       // the parts with a nonzero weight, in part order
+  int part[kMaxSumParts];
+  float weight[kMaxSumParts];
+};
+
+// g = w0 p0 + w1 p1 + ... in part order, every product and sum rounded on its own, then k_adagrad's update as
+// it compiles (its a + g * g contracts to one FFMA; sqrt and the division are IEEE): one part of weight 1 gives
+// k_adagrad's result bit for bit.  The table is read through the constant bank (__grid_constant__), so the
+// segment search does not copy it to local memory.
+__global__ void k_adagrad_sum(const float* __restrict__ parts, const __grid_constant__ SumArgs p, float lr) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= p.n) return;
+  float g = 0.f;
+  for (int k = 0; k < p.n_parts; ++k) {
+    const float v = __fmul_rn(p.weight[k], parts[(int64_t)p.part[k] * p.n + i]);
+    g = k ? __fadd_rn(g, v) : v;
+  }
+  int s = 0;
+  while (s + 1 < p.n_seg && i >= p.seg[s + 1].start) ++s;
+  const int64_t j = i - p.seg[s].start;
+  float* w = p.seg[s].w;
+  float* a = p.seg[s].a;
+  const float ai = __fmaf_rn(g, g, a[j]);
+  a[j] = ai;
+  w[j] = __fsub_rn(w[j], __fdiv_rn(__fmul_rn(lr, g), __fadd_rn(__fsqrt_rn(ai), 1e-7f)));
+}
+
+int adagrad_sum_fp32(ovn_handle* h, bool whole_network, const float* d_parts, int n_parts, const float* h_weights,
+                     float lr, cudaStream_t s) {
+  TrainState& t = *h->train;
+  SumArgs p = {};
+  int k = 0;
+  for (int l = 0; l < 4; ++l) {
+    int K, N;
+    head_dims(h, l, &K, &N);
+    const int64_t o = t.off[l], nk = (int64_t)K * N;
+    p.seg[k++] = {o, h->d_w[kMaxLegLayers + l], t.accum + o};
+    p.seg[k++] = {o + nk, h->d_b[kMaxLegLayers + l], t.accum + o + nk};
+  }
+  p.n = t.n_param;
+  if (whole_network) {
+    for (int l = 0; l < h->n_leg; ++l) {
+      const int64_t o = t.leg_off[l], nk = leg_kernel_size(h->leg[l]);
+      p.seg[k++] = {p.n + o, h->d_w[l], t.leg_accum + o};
+      p.seg[k++] = {p.n + o + nk, h->d_b[l], t.leg_accum + o + nk};
+    }
+    p.n += t.n_leg_param;
+  }
+  p.n_seg = k;
+  for (int r = 0; r < n_parts; ++r) {
+    if (h_weights[r] == 0.f) continue;
+    p.part[p.n_parts] = r;
+    p.weight[p.n_parts++] = h_weights[r];
+  }
+  k_adagrad_sum<<<blocks_for(p.n), 256, 0, s>>>(d_parts, p, lr);
+  OVN_LAUNCH_CHECK(h);
   return OVN_OK;
 }
 

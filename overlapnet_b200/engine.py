@@ -415,6 +415,38 @@ class Engine:
     """ovn_net_adagrad_step: Adagrad update of every leg and head layer from the last net_gradients."""
     check(self._h, lib().ovn_net_adagrad_step(self._h, float(lr), self._stream()), 'ovn_net_adagrad_step')
 
+  # ---- data-parallel training (fp32 handles) -------------------------------------------------------
+  def gradient_size(self, whole_network=False):
+    """ovn_train_gradient_size: floats of the flat gradient vector (the head layers, then the leg layers with
+    ``whole_network``)."""
+    n = C.c_int64(0)
+    check(self._h, lib().ovn_train_gradient_size(self._h, int(bool(whole_network)), C.byref(n)),
+          'ovn_train_gradient_size')
+    return int(n.value)
+
+  def copy_gradients(self, whole_network=False, out=None):
+    """ovn_copy_gradients: the last batch's gradients as one flat float32 cuda tensor [gradient_size]
+    (written into ``out`` when given)."""
+    n = self.gradient_size(whole_network)
+    if out is None:
+      out = torch.empty((n,), dtype=torch.float32, device=self.device)
+    assert out.numel() == n and out.dtype == torch.float32 and out.is_contiguous() and out.device == self.device
+    check(self._h, lib().ovn_copy_gradients(self._h, int(bool(whole_network)), _ptr(out), self._stream()),
+          'ovn_copy_gradients')
+    return out
+
+  def adagrad_step_sum(self, parts, weights, lr, whole_network=False):
+    """ovn_adagrad_step_sum: one Adagrad step with g = sum_k weights[k] parts[k] (in order, float32, weight-0
+    parts skipped).  ``parts`` [n_parts, gradient_size] float32 cuda, ``weights`` n_parts floats."""
+    n = self.gradient_size(whole_network)
+    p = parts.reshape(-1, n)
+    assert p.dtype == torch.float32 and p.is_contiguous() and p.device == self.device
+    w = np.ascontiguousarray(weights, np.float32).reshape(-1)
+    assert w.size == p.shape[0]
+    check(self._h, lib().ovn_adagrad_step_sum(self._h, int(bool(whole_network)), _ptr(p), int(p.shape[0]),
+                                             w.ctypes.data_as(C.c_void_p), float(lr), self._stream()),
+          'ovn_adagrad_step_sum')
+
   @property
   def leg_layers(self):
     """Names of the leg layers of this handle's config, input to output."""

@@ -19,6 +19,13 @@ every pair of every epoch) and TensorBoard output.
 (overlapnet_b200.augment): every epoch each training pair's RIGHT scan is rotated about z by a random multiple of
 the column pitch, its normals with it, and its orientation label moved to match.  Here the frozen leg encodes
 each step's rotated RIGHT images.  Validation is never augmented.
+
+Both flows train data-parallel over the GPUs of a node (overlapnet_b200.data_parallel, DESIGN.md section 6):
+
+  python -m torch.distributed.run --nproc_per_node G -m overlapnet_b200.training config.yml
+
+``batch_size`` stays the global batch; each rank trains on a contiguous share of every batch, and the ranks'
+gradients are all-gathered and summed in rank order on the device, so every rank keeps the same weights.
 """
 import logging
 import os
@@ -28,6 +35,7 @@ import numpy as np
 import torch
 
 from . import augment
+from . import data_parallel
 from . import evaluate
 from . import weights as _weights
 from .config import load_config
@@ -138,18 +146,24 @@ class FrozenLeg:
       self.bank = torch.cat([self.bank, self.bank.new_empty((B,) + tuple(self.bank.shape[1:]))])
       self.scratch = torch.arange(n, n + B, dtype=torch.int32, device=self.eng.device)
 
+  whole_network = False          # the layers the gradients cover (Engine.copy_gradients, adagrad_step_sum)
+
   def step(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, lr, rotate=None):
     """``rotate`` = (image rows, column shifts, (cos, sin)) of the batch's RIGHT scans, or None: the rotated
     images are encoded by the frozen leg into the scratch rows, which then stand in for ``right``."""
+    loss = self.gradients(left, right, gt_overlap, gt_orientation, min_overlap_for_angle, rotate)
+    self.eng.adagrad_step(lr)
+    return loss
+
+  def gradients(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, rotate=None):
+    """``step`` without its update: the losses; the gradients stay in the handle (the data-parallel step)."""
     if rotate is not None:
       rows, shifts, rot = rotate
       n, n0 = rows.numel(), len(self.rows)
       x = self.eng.gather_images(self.images, rows, shifts, rot)
       self.eng.leg(x, out=self.bank[n0:n0 + n])
       right = self.scratch[:n]
-    loss = self.eng.head_gradients(self.bank, left, right, gt_overlap, gt_orientation, min_overlap_for_angle)
-    self.eng.adagrad_step(lr)
-    return loss
+    return self.eng.head_gradients(self.bank, left, right, gt_overlap, gt_orientation, min_overlap_for_angle)
 
   def evaluate(self, left, right):
     """(overlap, yaw) device tensors of the validation pairs with the current weights."""
@@ -165,26 +179,35 @@ def train(config, device=None):
 
 
 def run(config, device, flow):
-  """The loop of training.py with ``flow`` (FrozenLeg or training_leg.WholeNetwork) making the steps."""
+  """The loop of training.py with ``flow`` (FrozenLeg or training_leg.WholeNetwork) making the steps.  Trains
+  data-parallel over the ranks of the default process group when one with more than one rank is initialised
+  (overlapnet_b200.data_parallel); only rank 0 then writes the log and the weight file."""
   from .infer import Infer
+  dp = data_parallel.default_group()
   model = config['model']
   root = config.get('data_root_folder', '')
   imgpath = config.get('imgpath', root)
   out_dir = os.path.join(config['experiments_path'], config['testname'])
-  os.makedirs(out_dir, exist_ok=True)
-  handler = logging.FileHandler(os.path.join(out_dir, 'training.log'), mode='w')      # training.py:204-208
-  handler.setFormatter(logging.Formatter(fmt='%(asctime)s %(message)s', datefmt='%H:%M:%S'))
-  logger.addHandler(handler)
+  handler = None
+  if dp is None or dp.rank == 0:
+    os.makedirs(out_dir, exist_ok=True)
+    handler = logging.FileHandler(os.path.join(out_dir, 'training.log'), mode='w')    # training.py:204-208
+    handler.setFormatter(logging.Formatter(fmt='%(asctime)s %(message)s', datefmt='%H:%M:%S'))
+    logger.addHandler(handler)
   if logger.level == logging.NOTSET or logger.level > logging.INFO:
     logger.setLevel(logging.INFO)
   try:
-    return _train(config, model, imgpath, out_dir, device, Infer, flow)
+    return _train(config, model, imgpath, out_dir, device, Infer, flow, dp=dp)
   finally:
-    logger.removeHandler(handler)
-    handler.close()
+    if handler is not None:
+      logger.removeHandler(handler)
+      handler.close()
 
 
-def _train(config, model, imgpath, out_dir, device, Infer, flow):
+def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
+  """The loop; ``dp`` (a data_parallel.DataParallel) makes it data-parallel: the config's batch_size is the
+  global batch, rank 0 makes every random draw a one-process run makes and hands the results to the other
+  ranks, and each step is data_parallel's gradient sum."""
   weights_filename = os.path.join(out_dir, model['modelType'] + '_' + config['testname'] + '.weight')
   initial_lr = float(config['learning_rate'])
   lr_alpha = float(config.get('lr_alpha', 0.99))
@@ -197,7 +220,11 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow):
 
   train_files, val_files = npz_files(config)
   logger.info('load training data ...')
-  t_f1, t_f2, t_d1, t_d2, t_ov, t_or = evaluate.load_overlap_npz(train_files)
+  if dp is None:
+    t_f1, t_f2, t_d1, t_d2, t_ov, t_or = evaluate.load_overlap_npz(train_files)
+  else:                                                            # rank 0's shuffle
+    t_f1, t_f2, t_d1, t_d2, t_ov, t_or = dp.broadcast(evaluate.load_overlap_npz(train_files) if dp.rank == 0
+                                                      else None)
   n = min(len(t_ov), batch_size * no_batches_in_epoch)                                # training.py:275-286
   t_f1, t_f2, t_d1, t_d2, t_ov, t_or = t_f1[:n], t_f2[:n], t_d1[:n], t_d2[:n], t_ov[:n], t_or[:n]
   logger.info('load validation data ...')
@@ -218,6 +245,10 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow):
   width = infer.network_output_size
   if len(cfg['pretrained_weightsfilename']) > 0:
     logger.info('Load old weights from %s', cfg['pretrained_weightsfilename'])
+  if dp is not None:               # one start for every rank (glorot_init draws from its own generator)
+    start = dp.broadcast(eng.get_weights() if dp.rank == 0 else None)
+    if dp.rank != 0:
+      eng.load_weights(start)
 
   keys = set(zip(t_d1, t_f1)) | set(zip(t_d2, t_f2)) | set(zip(v_d1, v_f1)) | set(zip(v_d2, v_f2))
   steps = flow(infer, keys, set(zip(t_d2, t_f2))) if yaw_augmentation else flow(infer, keys)
@@ -243,22 +274,39 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow):
                 'moved', pitch, pitch * width // W)
   else:
     logger.info('  NO rotation of training data')
+  if dp is not None:
+    whole = steps.whole_network
+    grad = torch.zeros((eng.gradient_size(whole),), dtype=torch.float32, device=dev)
+    parts = torch.empty((dp.world, grad.numel()), dtype=torch.float32, device=dev)
+    logger.info('  data-parallel over %d ranks: each step all-gathers %d gradients per rank', dp.world,
+                grad.numel())
   history = {'epoch_loss': [], 'batch_losses': [], 'validation': [], 'weights_filename': weights_filename}
   for epoch in range(no_epochs):
     lr = learning_rate(epoch, initial_lr, lr_alpha)
     losses, sizes = [], []
     t_or_epoch, rotate = t_or_d, None
-    if yaw_augmentation:                                           # one rotation per training pair and epoch
-      shifts = augment.sample_shifts(n, W, width)
+    shifts = perm = None
+    if dp is None or dp.rank == 0:
+      if yaw_augmentation:                                         # one rotation per training pair and epoch
+        shifts = augment.sample_shifts(n, W, width)
+      perm = np.random.permutation(n_batches)                      # Keras reshuffles a Sequence's batches
+    if dp is not None:
+      shifts, perm = dp.broadcast((shifts, perm))
+    if yaw_augmentation:
       shifts_d = torch.from_numpy(shifts).to(dev)
       rot_d = torch.from_numpy(augment.rotation(shifts, W)).to(dev)
       t_or_epoch = augment.move_labels(t_or_d, shifts_d, W, width)
-    for b in np.random.permutation(n_batches):                     # Keras reshuffles a Sequence's batches
+    for b in perm:
       s0, s1 = b * batch_size, min(n, (b + 1) * batch_size)
-      if yaw_augmentation:
-        rotate = (t_right_img[s0:s1], shifts_d[s0:s1], rot_d[s0:s1])
-      loss = steps.step(t_left[s0:s1], t_right[s0:s1], t_ov_d[s0:s1], t_or_epoch[s0:s1], min_overlap_for_angle, lr,
-                        rotate)
+      if dp is not None:
+        loss = _data_parallel_step(dp, steps, eng, grad, parts, s0, s1, t_left, t_right, t_ov_d, t_or_epoch,
+                                   min_overlap_for_angle, lr,
+                                   (t_right_img, shifts_d, rot_d) if yaw_augmentation else None)
+      else:
+        if yaw_augmentation:
+          rotate = (t_right_img[s0:s1], shifts_d[s0:s1], rot_d[s0:s1])
+        loss = steps.step(t_left[s0:s1], t_right[s0:s1], t_ov_d[s0:s1], t_or_epoch[s0:s1], min_overlap_for_angle,
+                          lr, rotate)
       losses.append(loss)
       sizes.append(s1 - s0)
       logger.info('  epoch %d batch %d: loss %.6f (overlap %.6f, orientation %.6f)', epoch + 1, len(losses),
@@ -268,13 +316,24 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow):
     history['batch_losses'].append([l[0] for l in losses])
 
     logger.info('                  saving model weights ...')                          # training.py:346-349
-    save_weights(weights_filename, eng.get_weights())
+    if dp is None or dp.rank == 0:
+      save_weights(weights_filename, eng.get_weights())
 
     logger.info('  Evaluation on test data ...')                                       # training.py:352-415
-    ov, yaw = steps.evaluate(v_left, v_right)
-    eng.check()
-    overlap = ov.cpu().numpy().astype(np.float64)
-    argmax = 180 - yaw.cpu().numpy().astype(np.int64)             # yaw = 180 - argmax (infer.py:158)
+    if dp is None:
+      ov, yaw = steps.evaluate(v_left, v_right)
+      eng.check()
+      overlap = ov.cpu().numpy().astype(np.float64)
+      argmax = 180 - yaw.cpu().numpy().astype(np.int64)           # yaw = 180 - argmax (infer.py:158)
+    else:                                                          # a share per rank, gathered in rank order
+      bounds, _ = data_parallel.shares(n_val, dp.world)
+      lo, hi = bounds[dp.rank]
+      ov, yaw = steps.evaluate(v_left[lo:hi], v_right[lo:hi])
+      eng.check()
+      mine = np.stack([ov.cpu().numpy().astype(np.float64), yaw.cpu().numpy().astype(np.float64)], axis=1)
+      both = dp.gather_rows(mine, [b - a for a, b in bounds])
+      overlap = both[:, 0]
+      argmax = 180 - both[:, 1].astype(np.int64)
     diffs = np.abs(overlap - v_ov)
     stats = {'mean': float(np.mean(diffs)), 'max': float(np.max(diffs)),
              'rms': float(np.sqrt(np.mean(diffs * diffs))), 'learning_rate': float(lr),
@@ -290,7 +349,29 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow):
   return history
 
 
+def _data_parallel_step(dp, steps, eng, grad, parts, s0, s1, t_left, t_right, t_ov, t_or, min_overlap_for_angle,
+                        lr, rotate):
+  """One step of the global batch [s0, s1): this rank's share's gradients, all-gathered, and the same weighted
+  Adagrad step on every rank.  ``rotate`` = (RIGHT image rows, shifts, rotations) of every training pair, or
+  None.  Returns the batch loss sum_r w_r loss_r (float64, rank order)."""
+  bounds, weights = data_parallel.shares(s1 - s0, dp.world)
+  a, b = s0 + bounds[dp.rank][0], s0 + bounds[dp.rank][1]
+  loss = (0.0, 0.0, 0.0)
+  if b > a:
+    share_rotate = None if rotate is None else tuple(t[a:b] for t in rotate)
+    loss = steps.gradients(t_left[a:b], t_right[a:b], t_ov[a:b], t_or[a:b], min_overlap_for_angle, share_rotate)
+    eng.copy_gradients(steps.whole_network, out=grad)
+  else:                                                            # weight 0: skipped by the sum
+    grad.zero_()
+  dp.gather_flat(grad, parts)
+  eng.adagrad_step_sum(parts, weights, lr, steps.whole_network)
+  all_losses = dp.gather_rows(np.asarray([loss], np.float64), [1] * dp.world)
+  return tuple(float(sum(w * l[k] for w, l in zip(weights, all_losses))) for k in range(3))
+
+
 def main(argv=None):
+  """``python -m overlapnet_b200.training config.yml``; under ``torch.distributed.run`` with WORLD_SIZE > 1
+  every rank joins the NCCL group and trains on GPU LOCAL_RANK, data-parallel."""
   argv = sys.argv[1:] if argv is None else argv
   logging.basicConfig(format='%(message)s', level=logging.INFO)
   configfilename = argv[0] if argv else 'network.yml'                                  # training.py:102-104
@@ -298,9 +379,20 @@ def main(argv=None):
   config = load_config(configfilename)
   if config['model'].get('legsType') == '360OutputkLegs':      # the reference's default (network.yml:70)
     from . import training_leg
-    training_leg.train(config)
+    train_fn = training_leg.train
   else:
-    train(config)
+    train_fn = train
+  if int(os.environ.get('WORLD_SIZE', '1')) <= 1:
+    train_fn(config)
+    return
+  import torch.distributed as dist
+  device = int(os.environ.get('LOCAL_RANK', '0'))
+  torch.cuda.set_device(device)
+  dist.init_process_group('nccl')
+  try:
+    train_fn(config, device)
+  finally:
+    dist.destroy_process_group()
 
 
 if __name__ == '__main__':

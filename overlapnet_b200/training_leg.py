@@ -61,9 +61,17 @@ class WholeNetwork:
     logger.info('Loaded %d scans into the image bank (%.1f MB on the GPU)', len(self.rows),
                 self.images.numel() * 4 / 1e6)
 
+  whole_network = True           # the layers the gradients cover (Engine.copy_gradients, adagrad_step_sum)
+
   def step(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, lr, rotate=None):
     """``rotate`` = (image rows, column shifts, (cos, sin)) of the batch's RIGHT scans, or None: the step then
     trains on a 2n-image batch of the LEFT images and the rotated RIGHT images."""
+    loss = self.gradients(left, right, gt_overlap, gt_orientation, min_overlap_for_angle, rotate)
+    self.eng.net_adagrad_step(lr)
+    return loss
+
+  def gradients(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, rotate=None):
+    """``step`` without its update: the losses; the gradients stay in the handle (the data-parallel step)."""
     images = self.images
     if rotate is not None:
       rows, shifts, rot = rotate
@@ -74,9 +82,7 @@ class WholeNetwork:
       self.eng.gather_images(self.images, rows, shifts, rot, out=images[n:])
       pairs = torch.arange(2 * n, dtype=torch.int32, device=self.eng.device)
       left, right = pairs[:n], pairs[n:]
-    loss = self.eng.net_gradients(images, left, right, gt_overlap, gt_orientation, min_overlap_for_angle)
-    self.eng.net_adagrad_step(lr)
-    return loss
+    return self.eng.net_gradients(images, left, right, gt_overlap, gt_orientation, min_overlap_for_angle)
 
   def evaluate(self, left, right):
     """(overlap, yaw) device tensors of the validation pairs: the scans re-encoded by the current leg."""
