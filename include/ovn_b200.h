@@ -250,9 +250,30 @@ int ovn_net_gradients(ovn_handle* h, const float* d_images, int64_t n_images,
                       const int32_t* d_left_idx, const int32_t* d_right_idx, int32_t n_pairs,
                       const float* d_gt_overlap, const int32_t* d_gt_orientation,
                       float min_overlap_for_angle, float* h_loss, float* d_fv_grad, void* stream);
+/* The feature volumes of the last valid ovn_net_gradients batch, as its leg forward computed them (at the handle's
+ * training precision): d_out [2][n_pairs][Wf][128], LEFT then RIGHT, asynchronous on `stream`.  fp32 handles
+ * (OVN_ERR_BAD_CONFIG otherwise); OVN_ERR_INVALID_ARG when there is no such batch. */
+int ovn_copy_net_volumes(ovn_handle* h, float* d_out, void* stream);
 /* Adagrad over every leg and head layer from the last ovn_net_gradients; INVALID_ARG otherwise (also after an
  * ovn_head_gradients call).  The head layers share their accumulators with ovn_head_adagrad_step. */
 int ovn_net_adagrad_step(ovn_handle* h, float learning_rate, void* stream);
+/* ---- training precision -------------------------------------------------------------------------------
+ * The arithmetic of every GEMM-shaped product inside ovn_head_gradients and ovn_net_gradients, forward and
+ * backward, and of the |l - r| backward of ovn_net_gradients.  OVN_TRAIN_FP32 (the default): fp32 SIMT FMAs.
+ * OVN_TRAIN_TF32X3: tensor cores (mma.sync TF32).  Each operand x is split into x_hi = tf32(x) and
+ * x_lo = tf32(x - x_hi), both rounded to nearest with ties away from zero; a product is
+ * a_lo b_hi + a_hi b_lo + a_hi b_hi, accumulated in fp32; a_lo b_lo (at most 2^-22 |a b|) is dropped.  The
+ * gradients stay fp32-grade (DESIGN.md section 2 gives the measured deviations) and two identical calls still
+ * give bit-identical results.  Only those two gradient calls are affected: the correlation backward, the losses,
+ * the Dense and ReLU backward, the split-K sums and every Adagrad step stay fp32, and so does every other entry
+ * point (ovn_leg_forward, ovn_heads_forward, ...).  ovn_copy_gradients and ovn_adagrad_step_sum work on whatever
+ * gradients the last gradient call left.  Allowed between any two calls.  OVN_ERR_BAD_CONFIG on a handle whose
+ * precision is not OVN_PREC_FP32; OVN_ERR_INVALID_ARG for a value not in ovn_train_precision. */
+typedef enum ovn_train_precision {
+  OVN_TRAIN_FP32 = 0,
+  OVN_TRAIN_TF32X3 = 1
+} ovn_train_precision;
+int ovn_set_train_precision(ovn_handle* h, int32_t train_precision);
 /* ---- data-parallel training (overlapnet_b200/training.py, DESIGN.md section 6) --------------------------
  * Each rank computes the gradients of its share of a batch with ovn_head_gradients / ovn_net_gradients, copies
  * them into one flat float32 vector, the ranks exchange those vectors, and every rank applies the same

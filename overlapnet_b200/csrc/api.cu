@@ -663,12 +663,33 @@ int ovn_heads_rows_vs_bank(ovn_handle* h, const float* d_bank, int64_t bank_size
   return OVN_OK;
 }
 
+// ---- training precision ---------------------------------------------------------------------------
+int ovn_set_train_precision(ovn_handle* h, int32_t train_precision) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  if (h->cfg.precision != OVN_PREC_FP32)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_set_train_precision: training needs a precision fp32 handle");
+  if (train_precision != OVN_TRAIN_FP32 && train_precision != OVN_TRAIN_TF32X3)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_set_train_precision: unknown training precision %d (0: fp32, 1: tf32x3)",
+                train_precision);
+  h->train_precision = train_precision;
+  return OVN_OK;
+}
+
+// The two gradient calls run their products at the handle's training precision; every other entry point, and
+// every return path of these two, leaves h->train_tc false.
+struct TrainPrecisionScope {
+  ovn_handle* h;
+  explicit TrainPrecisionScope(ovn_handle* hh) : h(hh) { h->train_tc = h->train_precision == OVN_TRAIN_TF32X3; }
+  ~TrainPrecisionScope() { h->train_tc = false; }
+};
+
 // ---- training of the overlap head (frozen leg) ----------------------------------------------------
 int ovn_head_gradients(ovn_handle* h, const float* d_bank, int64_t bank_size, const int32_t* d_left_idx,
                        const int32_t* d_right_idx, int32_t n_pairs, const float* d_gt_overlap,
                        const int32_t* d_gt_orientation, float min_overlap_for_angle, float* h_loss, void* stream) {
   if (!h) return OVN_ERR_INVALID_ARG;
   DeviceGuard guard(h);
+  TrainPrecisionScope precision(h);
   if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_head_gradients: %s", h->net_error.c_str());
   if (h->cfg.precision != OVN_PREC_FP32)
     OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_head_gradients: training needs a precision fp32 handle");
@@ -718,6 +739,7 @@ int ovn_net_gradients(ovn_handle* h, const float* d_images, int64_t n_images, co
                       void* stream) {
   if (!h) return OVN_ERR_INVALID_ARG;
   DeviceGuard guard(h);
+  TrainPrecisionScope precision(h);
   if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_net_gradients: %s", h->net_error.c_str());
   if (h->cfg.precision != OVN_PREC_FP32)
     OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_net_gradients: training needs a precision fp32 handle");
@@ -788,6 +810,18 @@ int ovn_copy_gradients(ovn_handle* h, int32_t whole_network, float* d_out, void*
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_copy_gradients: no valid whole-network gradients (call "
                 "ovn_net_gradients first)");
   return copy_gradients_fp32(h, whole_network != 0, d_out, (cudaStream_t)stream);
+}
+
+int ovn_copy_net_volumes(ovn_handle* h, float* d_out, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  if (h->cfg.precision != OVN_PREC_FP32)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_copy_net_volumes: training needs a precision fp32 handle");
+  REQUIRE(h, d_out, "NULL pointer");
+  if (!h->train || !h->train->net_grads_valid)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_copy_net_volumes: no valid whole-network batch (call ovn_net_gradients "
+                "first)");
+  return copy_net_volumes_fp32(h, d_out, (cudaStream_t)stream);
 }
 
 int ovn_adagrad_step_sum(ovn_handle* h, int32_t whole_network, const float* d_parts, int32_t n_parts,

@@ -122,6 +122,8 @@ struct TrainState {
   int64_t leg_off[kMaxLegLayers] = {};
   int64_t n_leg_param = 0;
   bool net_grads_valid = false; // the last ovn_net_gradients succeeded (leg_grad and grad are of one batch)
+  int64_t net_fv_off = 0;       // the last ovn_net_gradients batch: its volumes [2 net_np][Wf][128] at acts + net_fv_off
+  int net_np = 0;
 };
 }  // namespace ovn
 
@@ -179,6 +181,10 @@ struct ovn_handle {
   std::vector<cudaEvent_t> prof_ev[ovn::kProfKinds];   // start/stop pairs, in launch order
   std::unique_ptr<ovn::TcState, ovn::TcStateDelete> tc;   // tensor-core path state (network_tc.cu)
   std::unique_ptr<ovn::TrainState> train;  // overlap-head training state (network_fp32.cu), NULL until first used
+  int32_t train_precision = OVN_TRAIN_FP32;  // ovn_set_train_precision
+  bool train_tc = false;                   // inside ovn_head_gradients / ovn_net_gradients at OVN_TRAIN_TF32X3:
+                                           // launch_gemm and the |l - r| backward take their 3xTF32 kernels
+  bool dgrad_tc_smem = false;              // k_delta_dgrad_tc's dynamic shared-memory limit is raised on this device
 
   ~ovn_handle();                           // the streams and events; the buffers free themselves
   ovn::StageHeader* stage() const { return reinterpret_cast<ovn::StageHeader*>(h_pinned.get()); }
@@ -329,6 +335,7 @@ constexpr int kMaxSumParts = 64;
 int64_t train_gradient_size(const ovn_handle* h, bool whole_network);
 int leg_train_alloc(ovn_handle* h);        // train->leg_grad / leg_accum / leg_off, once
 int copy_gradients_fp32(ovn_handle* h, bool whole_network, float* d_out, cudaStream_t s);
+int copy_net_volumes_fp32(ovn_handle* h, float* d_out, cudaStream_t s);
 int adagrad_sum_fp32(ovn_handle* h, bool whole_network, const float* d_parts, int n_parts, const float* h_weights,
                      float lr, cudaStream_t s);
 // yaw augmentation of training images (projection.cu): rows are bounds-checked on the device (kErrBadIndex)

@@ -288,11 +288,180 @@ k_simt_gemm(AOp a, BOperand bop, const float* __restrict__ bias, float* __restri
   }
 }
 
+// ---- 3xTF32 tensor-core bodies of the training products (ovn_set_train_precision) -------------------------
+// x = hi + lo with hi = tf32_rna(x) and lo = tf32_rna(x - hi) (x - hi is exact in fp32), so |x - hi - lo| <=
+// 2^-22 |x|.  A product a b is lo_a hi_b + hi_a lo_b + hi_a hi_b, three mma.sync m16n8k8 into fp32 accumulators
+// in that order (the small terms first); lo_a lo_b <= 2^-22 |a b| is dropped.
+// The tensor core truncates (rounds toward zero) when it adds to its accumulator, so a chain of MMAs into one
+// accumulator drifts toward zero by up to an ulp per MMA: 3 K / 8 of them, 4e-5 of the overlap loss at K = 1920
+// on an H100.  So the six MMAs of a K16 tile start from zero and the tile's partial is added to the running sum
+// with a rounded FADD (add_tile): the truncation error then stays a few ulp of the sum of |terms| at any K.
+// Fragment ownership (PTX ISA, "Matrix fragments for mma.m16n8k8", .tf32): g = lane / 4, t = lane % 4;
+//   A (16 x 8, row): a0 = (g, t), a1 = (g + 8, t), a2 = (g, t + 4), a3 = (g + 8, t + 4)
+//   B (8 x 8, col):  b0 = (k = t, n = g), b1 = (k = t + 4, n = g)
+//   C (16 x 8):      c0 = (g, 2t), c1 = (g, 2t + 1), c2 = (g + 8, 2t), c3 = (g + 8, 2t + 1)
+// The shared tiles are k-major [k][kTcPitch] hi and lo planes.  A fragment load reads word t * kTcPitch + g
+// (+ a constant) in each lane; kTcPitch = 8 (mod 32) puts the 32 lanes on 32 different banks.
+constexpr int kTcPitch = BM + 8;
+
+__device__ __forceinline__ uint32_t tf32_rna(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return r & 0xffffe000u;                 // the low 13 bits are not part of the tf32 value
+}
+
+__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
+  hi = __uint_as_float(tf32_rna(x));
+  lo = __uint_as_float(tf32_rna(__fsub_rn(x, hi)));
+}
+
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+
+// One K8 step of a warp's 32 x 16 tile at rows wm, columns wn: acc[mi][ni] (rows wm + 16 mi, columns wn + 8 ni)
+// += A[rows][k, k + 8) B[k, k + 8)[columns] in 3xTF32.  A: ah / al [k][m], B: bh / bl [k][n].
+__device__ __forceinline__ void warp_mma_3xtf32(float (&acc)[2][2][4], const float (*ah)[kTcPitch],
+                                                const float (*al)[kTcPitch], const float (*bh)[kTcPitch],
+                                                const float (*bl)[kTcPitch], int k, int wm, int wn, int g, int t) {
+  uint32_t a_hi[2][4], a_lo[2][4], b_hi[2][2], b_lo[2][2];
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi) {
+    const int r = wm + mi * 16 + g;
+    a_hi[mi][0] = __float_as_uint(ah[k + t][r]);
+    a_hi[mi][1] = __float_as_uint(ah[k + t][r + 8]);
+    a_hi[mi][2] = __float_as_uint(ah[k + t + 4][r]);
+    a_hi[mi][3] = __float_as_uint(ah[k + t + 4][r + 8]);
+    a_lo[mi][0] = __float_as_uint(al[k + t][r]);
+    a_lo[mi][1] = __float_as_uint(al[k + t][r + 8]);
+    a_lo[mi][2] = __float_as_uint(al[k + t + 4][r]);
+    a_lo[mi][3] = __float_as_uint(al[k + t + 4][r + 8]);
+  }
+#pragma unroll
+  for (int ni = 0; ni < 2; ++ni) {
+    const int c = wn + ni * 8 + g;
+    b_hi[ni][0] = __float_as_uint(bh[k + t][c]);
+    b_hi[ni][1] = __float_as_uint(bh[k + t + 4][c]);
+    b_lo[ni][0] = __float_as_uint(bl[k + t][c]);
+    b_lo[ni][1] = __float_as_uint(bl[k + t + 4][c]);
+  }
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 2; ++ni) {
+      mma_tf32(acc[mi][ni], a_lo[mi], b_hi[ni]);
+      mma_tf32(acc[mi][ni], a_hi[mi], b_lo[ni]);
+      mma_tf32(acc[mi][ni], a_hi[mi], b_hi[ni]);
+    }
+}
+
+// The 3xTF32 product of a K16 tile (two K8 steps from zero), added to acc with round-to-nearest
+__device__ __forceinline__ void add_tile(float (&acc)[2][2][4], const float (*ah)[kTcPitch],
+                                         const float (*al)[kTcPitch], const float (*bh)[kTcPitch],
+                                         const float (*bl)[kTcPitch], int k, int wm, int wn, int g, int t) {
+  float part[2][2][4] = {};
+  warp_mma_3xtf32(part, ah, al, bh, bl, k, wm, wn, g, t);
+  warp_mma_3xtf32(part, ah, al, bh, bl, k + 8, wm, wn, g, t);
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) acc[mi][ni][r] = __fadd_rn(acc[mi][ni][r], part[mi][ni][r]);
+}
+
+// k_simt_gemm's product on tensor cores: the same arguments, grid, 64 x 64 x 16 block tile, operand staging
+// (bounds rules and zero fill) and epilogue.  Eight warps in 2 (M) x 4 (N), each a 32 x 16 tile of 2 x 2 MMA
+// tiles.  A thread stages its elements of the next K16 tile in registers while the warps multiply the current
+// one.
+template <class AOp>
+__global__ void __launch_bounds__(256)
+k_tc_gemm(AOp a, BOperand bop, const float* __restrict__ bias, float* __restrict__ C, int M, int N, int K,
+          int relu, int kchunk) {
+  __shared__ float Ah[BK][kTcPitch], Al[BK][kTcPitch];
+  __shared__ float Bh[BK][kTcPitch], Bl[BK][kTcPitch];
+  __shared__ int64_t s_rb[BM];
+  __shared__ int64_t s_rb2[BM];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int g = lane >> 2, t = lane & 3;
+  const int wm = (warp >> 2) * 32, wn = (warp & 3) * 16;
+  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN, z = blockIdx.z;
+  const int zb = kchunk ? 0 : z;
+  const int kbeg = kchunk ? z * kchunk : 0;
+  const int kend = kchunk ? min(K, kbeg + kchunk) : K;
+  if (tid < BM) {
+    const int m = m0 + tid;
+    s_rb[tid] = m < M ? a.row_base(m, zb) : -1;
+    s_rb2[tid] = m < M ? a.row_base2(m, zb) : 0;
+  }
+  const float* Bz = bop.B;
+  if (bop.b_nk) Bz = bop.query ? bop.query : bop.B + (int64_t)bop.right[zb] * bop.vol_stride;
+  __syncthreads();
+  float va[4], vb[4];
+  // element e = tid + 256 i of the A tile is (kk = e % BK, mm = e / BK); of the B tile (kk = e / BN, nn = e % BN)
+  // for b_nk = 0, (kk = e % BK, nn = e / BK) for b_nk = 1: k_simt_gemm's assignment
+  auto load = [&](int k0) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int e = tid + i * 256;
+      const int kk = e % BK, mm = e / BK;
+      const int k = k0 + kk;
+      va[i] = 0.f;
+      if (k < kend && s_rb[mm] >= 0) va[i] = a.load(s_rb[mm], a.col_off(k), s_rb2[mm], a.col_off2(k));
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int e = tid + i * 256;
+      vb[i] = 0.f;
+      if (!bop.b_nk) {
+        const int nn = e % BN, kk = e / BN;
+        if (k0 + kk < kend && n0 + nn < N) vb[i] = __ldg(Bz + (int64_t)(k0 + kk) * N + n0 + nn);
+      } else {
+        const int kk = e % BK, nn = e / BK;
+        if (k0 + kk < kend && n0 + nn < N) vb[i] = __ldg(Bz + (int64_t)(n0 + nn) * K + k0 + kk);
+      }
+    }
+  };
+  float acc[2][2][4] = {};
+  if (kbeg < kend) load(kbeg);
+  for (int k0 = kbeg; k0 < kend; k0 += BK) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int e = tid + i * 256;
+      split_tf32(va[i], Ah[e % BK][e / BK], Al[e % BK][e / BK]);
+      if (!bop.b_nk) split_tf32(vb[i], Bh[e / BN][e % BN], Bl[e / BN][e % BN]);
+      else split_tf32(vb[i], Bh[e % BK][e / BK], Bl[e % BK][e / BK]);
+    }
+    __syncthreads();
+    if (k0 + BK < kend) load(k0 + BK);
+    add_tile(acc, Ah, Al, Bh, Bl, 0, wm, wn, g, t);
+    __syncthreads();
+  }
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int m = m0 + wm + mi * 16 + g + (r >> 1) * 8;
+        const int n = n0 + wn + ni * 8 + 2 * t + (r & 1);
+        if (m >= M || n >= N) continue;
+        float v = acc[mi][ni][r] + (bias ? __ldg(bias + n) : 0.f);
+        if (relu) v = fmaxf(v, 0.f);
+        C[((int64_t)z * M + m) * N + n] = v;
+      }
+}
+
+// The training entry points set h->train_tc for their duration when the handle's training precision is
+// OVN_TRAIN_TF32X3 (TrainPrecisionScope in api.cu); every other caller gets k_simt_gemm.
 template <class AOp>
 static int launch_gemm(ovn_handle* h, const AOp& a, const BOperand& b, const float* bias, float* C, int M,
                        int N, int K, int batch, int relu, cudaStream_t s, int kchunk = 0) {
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM, batch);
-  k_simt_gemm<AOp><<<grid, 256, 0, s>>>(a, b, bias, C, M, N, K, relu, kchunk);
+  if (h->train_tc) k_tc_gemm<AOp><<<grid, 256, 0, s>>>(a, b, bias, C, M, N, K, relu, kchunk);
+  else k_simt_gemm<AOp><<<grid, 256, 0, s>>>(a, b, bias, C, M, N, K, relu, kchunk);
   OVN_LAUNCH_CHECK(h);
   return OVN_OK;
 }
@@ -835,6 +1004,119 @@ k_delta_dgrad(const float* __restrict__ do1, const float* __restrict__ w1, const
   }
 }
 
+// k_delta_dgrad with its per-tap G = do1 W1^T on 3xTF32 mma.sync: the same grid, CTA tile, partial layout and
+// sign rule.  The do1 tile is split into hi / lo planes once, each tap's W1 tile when it is staged.  Eight warps
+// in 2 (rows i) x 4 (channels c), each a 32 x 16 tile; the signs are applied to the accumulator fragments.  A
+// tap's column sums for part_r add a thread's four rows, then the eight lanes of a column (butterfly over lane
+// bits 2..4), then the two row warps, always in that order.
+constexpr int kDgTcSmem = (4 * kDgT * kTcPitch + 2 * kDgT) * (int)sizeof(float);
+
+__global__ void __launch_bounds__(256)
+k_delta_dgrad_tc(const float* __restrict__ do1, const float* __restrict__ w1, const float* __restrict__ fv,
+                 const int32_t* __restrict__ left, const int32_t* __restrict__ right, int Wf, int s, int nb, int nho,
+                 float* __restrict__ part_l, float* __restrict__ part_r) {
+  extern __shared__ __align__(16) float smem[];
+  float (*Ah)[kTcPitch] = reinterpret_cast<float (*)[kTcPitch]>(smem);     // [o][i]
+  float (*Al)[kTcPitch] = Ah + kDgT;
+  float (*Bh)[kTcPitch] = Al + kDgT;                                      // [o][c]
+  float (*Bl)[kTcPitch] = Bh + kDgT;
+  float (*red)[kDgT] = reinterpret_cast<float (*)[kDgT]>(Bl + kDgT);    // [row warp][c]
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int g = lane >> 2, t = lane & 3;
+  const int wm = (warp >> 2) * 32, wn = (warp & 3) * 16;
+  const int c0 = blockIdx.x * kDgT, itile = blockIdx.y, i0 = itile * kDgT;
+  const int jb = blockIdx.z % nb, p = blockIdx.z / nb;
+  const int nit = gridDim.y;
+  for (int f = tid; f < kDgT * kDgT / 4; f += 256) {
+    const int r = f % kDgT, o = (f / kDgT) * 4, i = i0 + r;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (i < Wf) {
+      const int ho = i / s, dh = i - ho * s;
+      v = __ldg(reinterpret_cast<const float4*>(do1 + ((((int64_t)p * nho + ho) * nb + jb) * s + dh) * kDgT + o));
+    }
+    split_tf32(v.x, Ah[o][r], Al[o][r]);
+    split_tf32(v.y, Ah[o + 1][r], Al[o + 1][r]);
+    split_tf32(v.z, Ah[o + 2][r], Al[o + 2][r]);
+    split_tf32(v.w, Ah[o + 3][r], Al[o + 3][r]);
+  }
+  const float* L = fv + (int64_t)left[p] * Wf * kFeatC;
+  const float* R = fv + (int64_t)right[p] * Wf * kFeatC;
+  // fragment element (mi, ni, r): row i0 + wm + 16 mi + g + 8 (r / 2), channel c0 + wn + 8 ni + 2 t + r % 2
+  float lv[2][2][4], accl[2][2][4];
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int h8 = 0; h8 < 2; ++h8) {
+      const int i = i0 + wm + mi * 16 + g + h8 * 8;
+#pragma unroll
+      for (int ni = 0; ni < 2; ++ni) {
+        const float2 v = i < Wf ? __ldg(reinterpret_cast<const float2*>(L + (int64_t)i * kFeatC + c0 + wn + ni * 8 + 2 * t))
+                                : make_float2(0.f, 0.f);
+        lv[mi][ni][2 * h8] = v.x;
+        lv[mi][ni][2 * h8 + 1] = v.y;
+        accl[mi][ni][2 * h8] = 0.f;
+        accl[mi][ni][2 * h8 + 1] = 0.f;
+      }
+    }
+  for (int dj = 0; dj < s; ++dj) {
+    for (int f = tid; f < kDgT * kDgT / 4; f += 256) {
+      const int c = f % kDgT, o = (f / kDgT) * 4;
+      const float4 v = __ldg(reinterpret_cast<const float4*>(w1 + ((int64_t)dj * kFeatC + c0 + c) * kDgT + o));
+      split_tf32(v.x, Bh[o][c], Bl[o][c]);
+      split_tf32(v.y, Bh[o + 1][c], Bl[o + 1][c]);
+      split_tf32(v.z, Bh[o + 2][c], Bl[o + 2][c]);
+      split_tf32(v.w, Bh[o + 3][c], Bl[o + 3][c]);
+    }
+    __syncthreads();
+    float acc[2][2][4] = {};
+#pragma unroll
+    for (int k = 0; k < kDgT; k += 16) add_tile(acc, Ah, Al, Bh, Bl, k, wm, wn, g, t);
+    const int j = s * jb + dj;
+    float rv[2][2], col[2][2] = {};
+#pragma unroll
+    for (int ni = 0; ni < 2; ++ni) {
+      const float2 v = __ldg(reinterpret_cast<const float2*>(R + (int64_t)j * kFeatC + c0 + wn + ni * 8 + 2 * t));
+      rv[ni][0] = v.x;
+      rv[ni][1] = v.y;
+    }
+#pragma unroll
+    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+      for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const float d = lv[mi][ni][r] - rv[ni][r & 1];
+          const float a = acc[mi][ni][r];
+          const float v = d > 0.f ? a : (d < 0.f ? -a : 0.f);
+          accl[mi][ni][r] += v;
+          col[ni][r & 1] += v;
+        }
+#pragma unroll
+    for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+      for (int b = 0; b < 2; ++b) {
+        float v = col[ni][b];
+        v += __shfl_xor_sync(0xffffffffu, v, 4);
+        v += __shfl_xor_sync(0xffffffffu, v, 8);
+        v += __shfl_xor_sync(0xffffffffu, v, 16);
+        if (g == 0) red[wm / 32][wn + ni * 8 + 2 * t + b] = v;
+      }
+    __syncthreads();
+    if (tid < kDgT) part_r[(((int64_t)p * nit + itile) * Wf + j) * kFeatC + c0 + tid] = -(red[0][tid] + red[1][tid]);
+  }
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int h8 = 0; h8 < 2; ++h8) {
+      const int i = i0 + wm + mi * 16 + g + h8 * 8;
+      if (i >= Wf) continue;
+#pragma unroll
+      for (int ni = 0; ni < 2; ++ni)
+        *reinterpret_cast<float2*>(part_l + (((int64_t)p * nb + jb) * Wf + i) * kFeatC + c0 + wn + ni * 8 + 2 * t) =
+            make_float2(accl[mi][ni][2 * h8], accl[mi][ni][2 * h8 + 1]);
+    }
+}
+
 // dfv[v] += the partials of volume v in order: LEFT p (v = p) sums nb partials, RIGHT p (v = np + p) nit
 __global__ void k_delta_dgrad_reduce(const float* __restrict__ part_l, const float* __restrict__ part_r, int np, int nb,
                                      int nit, int64_t vol, float* __restrict__ dfv) {
@@ -957,6 +1239,8 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
     prof_mark(h, PROF_LEG, s);
   }
   const float* fv = act[h->n_leg - 1];
+  t.net_fv_off = fv - t.acts.get();
+  t.net_np = np;
   k_pair_rows<<<blocks_for(n2), 256, 0, s>>>(t.pair_rows, n2);
   OVN_LAUNCH_CHECK(h);
   const int32_t* lrow = t.pair_rows;
@@ -974,8 +1258,18 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
   OVN_LAUNCH_CHECK(h);
   float* part_l = t.dfv_part;
   float* part_r = part_l + (int64_t)np * nb * vol;
-  k_delta_dgrad<<<dim3(kFeatC / kDgT, nit, nb * np), 256, 0, s>>>(h->d_o1, h->d_w[kMaxLegLayers], fv, lrow, rrow, Wf,
-                                                                   sz, nb, h->head[1].h_out, part_l, part_r);
+  const dim3 dg_grid(kFeatC / kDgT, nit, nb * np);
+  if (h->train_tc) {
+    if (!h->dgrad_tc_smem) {
+      OVN_CUDA(h, cudaFuncSetAttribute(k_delta_dgrad_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, kDgTcSmem));
+      h->dgrad_tc_smem = true;
+    }
+    k_delta_dgrad_tc<<<dg_grid, 256, kDgTcSmem, s>>>(h->d_o1, h->d_w[kMaxLegLayers], fv, lrow, rrow, Wf, sz, nb,
+                                                     h->head[1].h_out, part_l, part_r);
+  } else {
+    k_delta_dgrad<<<dg_grid, 256, 0, s>>>(h->d_o1, h->d_w[kMaxLegLayers], fv, lrow, rrow, Wf, sz, nb,
+                                          h->head[1].h_out, part_l, part_r);
+  }
   OVN_LAUNCH_CHECK(h);
   k_delta_dgrad_reduce<<<blocks_for(n2 * vol), 256, 0, s>>>(part_l, part_r, np, nb, nit, vol, dfv);
   OVN_LAUNCH_CHECK(h);
@@ -1060,6 +1354,15 @@ int copy_gradients_fp32(ovn_handle* h, bool whole_network, float* d_out, cudaStr
   if (whole_network)
     OVN_CUDA(h, cudaMemcpyAsync(d_out + t.n_param, t.leg_grad, (size_t)t.n_leg_param * sizeof(float),
                                 cudaMemcpyDeviceToDevice, s));
+  return OVN_OK;
+}
+
+// The volumes of the last ovn_net_gradients batch, [2][np][Wf][128] (LEFT, then RIGHT): the leg's output as that
+// call computed it, at its training precision (the backward reads every activation, and none is overwritten)
+int copy_net_volumes_fp32(ovn_handle* h, float* d_out, cudaStream_t s) {
+  const TrainState& t = *h->train;
+  const size_t n = (size_t)2 * t.net_np * h->cfg.leg_output_width * kFeatC;
+  OVN_CUDA(h, cudaMemcpyAsync(d_out, t.acts + t.net_fv_off, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return OVN_OK;
 }
 

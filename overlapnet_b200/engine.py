@@ -70,6 +70,7 @@ class Engine:
     self.cfg = cfg
     self.model = model
     self.precision = precision
+    self.train_precision = 'fp32'
     self.H, self.W = proj_H, proj_W
     self._h = C.c_void_p(0)
     with torch.cuda.device(self.device):
@@ -409,11 +410,28 @@ class Engine:
                                           _ptr(gor), float(min_overlap_for_angle), loss.ctypes.data_as(C.c_void_p),
                                           _ptr(dfv), self._stream()), 'ovn_net_gradients')
     loss = tuple(float(v) for v in loss)
+    self._net_pairs = n
     return (loss, dfv) if fv_grad else loss
+
+  def net_volumes(self):
+    """ovn_copy_net_volumes: the feature volumes [2, n, Wf, 128] (LEFT, RIGHT) of the last net_gradients batch, as
+    its leg forward computed them at the training precision."""
+    out = torch.empty((2, getattr(self, '_net_pairs', 0), self.Wf, FEAT_C), dtype=torch.float32, device=self.device)
+    check(self._h, lib().ovn_copy_net_volumes(self._h, _ptr(out), self._stream()), 'ovn_copy_net_volumes')
+    return out
 
   def net_adagrad_step(self, lr):
     """ovn_net_adagrad_step: Adagrad update of every leg and head layer from the last net_gradients."""
     check(self._h, lib().ovn_net_adagrad_step(self._h, float(lr), self._stream()), 'ovn_net_adagrad_step')
+
+  def set_train_precision(self, precision):
+    """ovn_set_train_precision: 'fp32' (the default) or 'tf32x3', the arithmetic of head_gradients and
+    net_gradients (3xTF32 tensor-core products with fp32 accumulation).  Every other call stays fp32."""
+    if precision not in _cabi.TRAIN_PRECISIONS:
+      raise ValueError('training precision %r: use one of %s' % (precision, ', '.join(_cabi.TRAIN_PRECISIONS)))
+    check(self._h, lib().ovn_set_train_precision(self._h, _cabi.TRAIN_PRECISIONS[precision]),
+          'ovn_set_train_precision')
+    self.train_precision = precision
 
   # ---- data-parallel training (fp32 handles) -------------------------------------------------------
   def gradient_size(self, whole_network=False):

@@ -20,6 +20,9 @@ every pair of every epoch) and TensorBoard output.
 the column pitch, its normals with it, and its orientation label moved to match.  Here the frozen leg encodes
 each step's rotated RIGHT images.  Validation is never augmented.
 
+``training_precision: tf32x3`` (both legsTypes, default fp32) runs every product of the gradient steps on tensor
+cores in 3xTF32 with fp32 accumulation (Engine.set_train_precision); validation stays fp32.
+
 Both flows train data-parallel over the GPUs of a node (overlapnet_b200.data_parallel, DESIGN.md section 6):
 
   python -m torch.distributed.run --nproc_per_node G -m overlapnet_b200.training config.yml
@@ -63,6 +66,18 @@ def check_config(config):
     raise Exception('legsType %r is not supported for training; use 360OutputkLegsFixed' % (legs,))
   check_unsupported_options(config)
   check_yaw_augmentation(config)
+  check_training_precision(config)
+
+
+TRAINING_PRECISIONS = ('fp32', 'tf32x3')
+
+
+def check_training_precision(config):
+  """``training_precision`` (both legsTypes, default fp32) is the arithmetic of the gradient steps:
+  ``tf32x3`` runs their products on tensor cores in 3xTF32 (Engine.set_train_precision)."""
+  p = config.get('training_precision', 'fp32')
+  if p not in TRAINING_PRECISIONS:
+    raise Exception('training_precision %r is not supported; use one of %s' % (p, ', '.join(TRAINING_PRECISIONS)))
 
 
 def check_yaw_augmentation(config):
@@ -243,6 +258,9 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
   infer = Infer(cfg, precision='fp32', device=device, max_batch_pairs=batch_size)
   eng = infer._engine
   width = infer.network_output_size
+  if 'training_precision' in config:        # every rank, so that data-parallel ranks compute alike
+    eng.set_train_precision(config['training_precision'])
+    logger.info('Training precision: %s', config['training_precision'])
   if len(cfg['pretrained_weightsfilename']) > 0:
     logger.info('Load old weights from %s', cfg['pretrained_weightsfilename'])
   if dp is not None:               # one start for every rank (glorot_init draws from its own generator)

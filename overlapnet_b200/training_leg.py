@@ -30,6 +30,7 @@ def check_config(config):
     raise Exception('legsType %r is not supported for training; use 360OutputkLegs' % (legs,))
   training.check_unsupported_options(config)
   training.check_yaw_augmentation(config)
+  training.check_training_precision(config)
 
 
 def load_image_bank(infer, keys, chunk=256):

@@ -6,7 +6,10 @@ The card name and power limit are read in the same run, because they are part of
 --yaw-augmentation times the step of ``yaw_augmentation: True`` (overlapnet_b200.training.FrozenLeg): the 16
 RIGHT images are gathered from a synthetic image bank, rolled and rotated (ovn_gather_images), encoded by the
 frozen fp32 leg into scratch rows after the volume bank, and the heads train on those rows.  The TFLOP/s figure
-counts the heads only."""
+counts the heads only.
+
+--training-precision tf32x3 times the 3xTF32 tensor-core step (Engine.set_train_precision); tflops_issued counts
+its three MMAs per product."""
 import json
 import os
 import subprocess
@@ -34,10 +37,11 @@ def card():
     return '%s (power limit unknown: %s)' % (torch.cuda.get_device_name(), e)
 
 
-def main():
-  yaw_aug = '--yaw-augmentation' in sys.argv[1:]
+def run(yaw_aug=False, precision='fp32'):
+  """The timing of one configuration, as the dict main prints."""
   eng = Engine(model=MODEL, precision='fp32', max_batch_scans=16, max_batch_pairs=PAIRS)
   eng.load_weights(W.glorot_init(4, MODEL, seed=0))
+  eng.set_train_precision(precision)
   g = torch.Generator(device='cuda').manual_seed(0)
   bank = torch.rand((BANK + (PAIRS if yaw_aug else 0), 360, 128), device='cuda', generator=g)
   if yaw_aug:
@@ -66,11 +70,20 @@ def main():
     if i >= WARMUP:
       ms.append(e0.elapsed_time(e1))
   med = float(np.median(ms))
-  res = {'card': card(), 'yaw_augmentation': yaw_aug, 'pairs_per_step': PAIRS, 'steps': STEPS, 'ms_per_step_median': round(med, 3),
+  eng.close()
+  res = {'card': card(), 'training_precision': precision, 'yaw_augmentation': yaw_aug, 'pairs_per_step': PAIRS, 'steps': STEPS, 'ms_per_step_median': round(med, 3),
          'ms_per_step_min': round(float(np.min(ms)), 3), 'ms_per_step_max': round(float(np.max(ms)), 3),
          'pairs_per_s': round(PAIRS / med * 1e3, 1),
          'tflops': round(PAIRS * GFLOP_PER_PAIR / med, 3)}
-  print(json.dumps(res))
+  if precision == 'tf32x3':             # three MMAs per product
+    res['tflops_issued'] = round(3 * res['tflops'], 3)
+  return res
+
+
+def main():
+  argv = sys.argv[1:]
+  precision = argv[argv.index('--training-precision') + 1] if '--training-precision' in argv else 'fp32'
+  print(json.dumps(run('--yaw-augmentation' in argv, precision)))
 
 
 if __name__ == '__main__':

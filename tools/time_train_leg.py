@@ -5,7 +5,10 @@ The card name and power limit are read in the same run, because they are part of
 
 --yaw-augmentation times the step of ``yaw_augmentation: True`` (overlapnet_b200.training_leg.WholeNetwork): the
 16 LEFT images and the 16 rolled and rotated RIGHT images are gathered into a 32-image batch (ovn_gather_images)
-that ovn_net_gradients then trains on."""
+that ovn_net_gradients then trains on.
+
+--training-precision tf32x3 times the 3xTF32 tensor-core step (Engine.set_train_precision); tflops_issued counts
+its three MMAs per product."""
 import json
 import os
 import sys
@@ -24,10 +27,11 @@ GFLOP_PER_PAIR = 17.9
 PAIRS, BANK, WARMUP, STEPS = 16, 64, 3, 20
 
 
-def main():
-  yaw_aug = '--yaw-augmentation' in sys.argv[1:]
+def run(yaw_aug=False, precision='fp32'):
+  """The timing of one configuration, as the dict main prints."""
   eng = Engine(model=MODEL, precision='fp32', max_batch_scans=16, max_batch_pairs=PAIRS)
   eng.load_weights(W.glorot_init(4, MODEL, seed=0))
+  eng.set_train_precision(precision)
   images = torch.from_numpy(synth.range_like_images(0, BANK, 4)).cuda()
   rng = np.random.default_rng(0)
   batches = []
@@ -56,11 +60,20 @@ def main():
     if i >= WARMUP:
       ms.append(e0.elapsed_time(e1))
   med = float(np.median(ms))
-  res = {'card': card(), 'yaw_augmentation': yaw_aug, 'pairs_per_step': PAIRS, 'steps': STEPS, 'ms_per_step_median': round(med, 3),
+  eng.close()
+  res = {'card': card(), 'training_precision': precision, 'yaw_augmentation': yaw_aug, 'pairs_per_step': PAIRS, 'steps': STEPS, 'ms_per_step_median': round(med, 3),
          'ms_per_step_min': round(float(np.min(ms)), 3), 'ms_per_step_max': round(float(np.max(ms)), 3),
          'pairs_per_s': round(PAIRS / med * 1e3, 1),
          'tflops': round(PAIRS * GFLOP_PER_PAIR / med, 3)}
-  print(json.dumps(res))
+  if precision == 'tf32x3':             # three MMAs per product
+    res['tflops_issued'] = round(3 * res['tflops'], 3)
+  return res
+
+
+def main():
+  argv = sys.argv[1:]
+  precision = argv[argv.index('--training-precision') + 1] if '--training-precision' in argv else 'fp32'
+  print(json.dumps(run('--yaw-augmentation' in argv, precision)))
 
 
 if __name__ == '__main__':
