@@ -220,7 +220,8 @@ int ovn_bank_release(ovn_handle* h, const float* d_bank);
  * generateNet.py:222-324) ------------------------------------------------------------------------
  * c_conv1..3 and overlap_output are trained, the leg is never touched.  fp32 arithmetic; every reduction
  * runs in a fixed order, so identical calls give bit-identical weights.  The gradient, Adagrad-accumulator
- * and activation buffers are allocated when a handle first trains (sized by max_batch_pairs).
+ * and activation buffers are allocated when a handle first trains (sized by max_batch_pairs); the gradients and
+ * accumulators then cover every layer, leg included.
  * Losses (training.py:71-92,255-257): L = 5 L_ov + L_or,
  *   L_ov = mean_p sigmoid((|overlap_p - gt_overlap_p| + 0.25) * 24 - 12),
  *   L_or = mean_p mean_k weighted_cross_entropy_with_logits(t_pk, corr_pk, pos_weight = 360),
@@ -236,7 +237,7 @@ int ovn_head_gradients(ovn_handle* h, const float* d_bank, int64_t bank_size,
                        float min_overlap_for_angle, float* h_loss, void* stream);
 /* Adagrad update of c_conv1..3 / overlap_output from the last valid gradients (Keras 2.1.5:
  * a += g^2; w -= lr g / (sqrt(a) + 1e-7), accumulators start at 0); refuses (INVALID_ARG) when there are
- * none.  ovn_finalize_weights resets the accumulators. */
+ * none.  ovn_finalize_weights resets the accumulators.  One launch. */
 int ovn_head_adagrad_step(ovn_handle* h, float learning_rate, void* stream);
 /* ---- training of the whole network (legsType 360OutputkLegs, generateNet.py:119-219) ----------
  * fp32 handles only (OVN_ERR_BAD_CONFIG otherwise); n_pairs <= max_batch_pairs and n_pairs <= 485 at
@@ -245,7 +246,7 @@ int ovn_head_adagrad_step(ovn_handle* h, float learning_rate, void* stream);
  * the losses of training.py, and the backward of the whole network: the correlation head's loss now reaches
  * the leg.  Synchronous: h_loss[3].  d_fv_grad (may be NULL) receives dL/d(LEFT volume), dL/d(RIGHT volume)
  * as [2][n_pairs][Wf][128], before s_conv10's ReLU mask.  An index outside the image bank returns
- * OVN_ERR_INVALID_ARG and leaves no usable gradients.  The buffers are allocated on the first call. */
+ * OVN_ERR_INVALID_ARG and leaves no usable gradients.  The per-batch buffers are allocated on the first call. */
 int ovn_net_gradients(ovn_handle* h, const float* d_images, int64_t n_images,
                       const int32_t* d_left_idx, const int32_t* d_right_idx, int32_t n_pairs,
                       const float* d_gt_overlap, const int32_t* d_gt_orientation,
@@ -255,7 +256,7 @@ int ovn_net_gradients(ovn_handle* h, const float* d_images, int64_t n_images,
  * (OVN_ERR_BAD_CONFIG otherwise); OVN_ERR_INVALID_ARG when there is no such batch. */
 int ovn_copy_net_volumes(ovn_handle* h, float* d_out, void* stream);
 /* Adagrad over every leg and head layer from the last ovn_net_gradients; INVALID_ARG otherwise (also after an
- * ovn_head_gradients call).  The head layers share their accumulators with ovn_head_adagrad_step. */
+ * ovn_head_gradients call).  The head layers share their accumulators with ovn_head_adagrad_step.  One launch. */
 int ovn_net_adagrad_step(ovn_handle* h, float learning_rate, void* stream);
 /* ---- training precision -------------------------------------------------------------------------------
  * The arithmetic of every GEMM-shaped product inside ovn_head_gradients and ovn_net_gradients, forward and

@@ -20,6 +20,17 @@ static void set_spec(ConvSpec& L, const char* name, int kh, int kw, int sh, int 
   L.w_out = (w_in - kw) / sw + 1;
 }
 
+// kernel and bias sizes of the layer in weight slot `slot`
+static void slot_sizes(const ovn_handle* h, int slot, int64_t* n_kernel, int64_t* n_bias) {
+  if (slot == kMaxLegLayers + 3) {   // overlap_output
+    *n_kernel = h->dense_in; *n_bias = 1;
+    return;
+  }
+  const ConvSpec& L = slot < kMaxLegLayers ? h->leg[slot] : h->head[slot - kMaxLegLayers];
+  *n_kernel = (int64_t)L.kh * L.kw * L.cin * L.cout;
+  *n_bias = L.cout;
+}
+
 static __global__ void k_iota(int32_t* p, int n, int start) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = start + i;
@@ -250,6 +261,15 @@ int ovn_create(const ovn_config* cfg, ovn_handle** out) {
     h->o2_h = h->head[1].h_out; h->o2_w = h->head[1].w_out;
     h->o3_h = h->head[2].h_out; h->o3_w = h->head[2].w_out;
     h->dense_in = h->o3_h * h->o3_w * h->head[2].cout;
+    ParamLayout& P = h->params;
+    for (int i = 0; i < 4 + h->n_leg; ++i) {
+      const int slot = flat_slot(i);
+      int64_t nb;
+      P.off[slot] = P.n_total;
+      slot_sizes(h.get(), slot, &P.n_kernel[slot], &nb);
+      P.n_total += P.n_kernel[slot] + nb;
+      if (i == 3) P.n_head = P.n_total;
+    }
   }
 
   // ---- workspaces
@@ -399,11 +419,8 @@ int ovn_finalize_weights(ovn_handle* h) {
     if (rc != OVN_OK) return rc;
   }
   if (h->train) {                        // new weights: Adagrad starts over, old gradients are stale
-    OVN_CUDA(h, cudaMemset(h->train->accum, 0, (size_t)h->train->n_param * sizeof(float)));
-    if (h->train->leg_accum)
-      OVN_CUDA(h, cudaMemset(h->train->leg_accum, 0, (size_t)h->train->n_leg_param * sizeof(float)));
-    h->train->grads_valid = false;
-    h->train->net_grads_valid = false;
+    OVN_CUDA(h, cudaMemset(h->train->accum, 0, (size_t)h->params.n_total * sizeof(float)));
+    h->train->grads = kNoGrads;
   }
   h->weights_ready = true;
   return OVN_OK;
@@ -411,15 +428,9 @@ int ovn_finalize_weights(ovn_handle* h) {
 
 // kernel / bias sizes and weight slot of a layer; dense = overlap_output
 static int layer_slot(const ovn_handle* h, const char* name, int64_t* n_kernel, int64_t* n_bias, bool* head) {
-  if (strcmp(name, "overlap_output") == 0) {
-    *n_kernel = h->dense_in; *n_bias = 1; *head = true;
-    return kMaxLegLayers + 3;
-  }
-  int slot = -1;
-  const ConvSpec* L = find_layer(h, name, &slot);
-  if (!L) return -1;
-  *n_kernel = (int64_t)L->kh * L->kw * L->cin * L->cout;
-  *n_bias = L->cout;
+  int slot = kMaxLegLayers + 3;
+  if (strcmp(name, "overlap_output") != 0 && !find_layer(h, name, &slot)) return -1;
+  slot_sizes(h, slot, n_kernel, n_bias);
   *head = slot >= kMaxLegLayers;
   return slot;
 }
@@ -447,12 +458,12 @@ int ovn_get_gradients(ovn_handle* h, const char* name, float* h_kernel, float* h
   bool head;
   const int slot = layer_slot(h, name, &nk, &nb, &head);
   if (slot < 0) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_get_gradients: '%s' is not a layer of the network", name);
-  if (!head && (!h->train || !h->train->net_grads_valid))
+  if (!head && (!h->train || h->train->grads < kNetGrads))
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_get_gradients: no valid gradients of leg layer '%s' (call "
                 "ovn_net_gradients first)", name);
-  if (!h->train || !h->train->grads_valid)
+  if (!h->train || h->train->grads < kHeadGrads)
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_get_gradients: no valid gradients (call ovn_head_gradients first)");
-  const float* g = head ? h->train->grad + h->train->off[slot - kMaxLegLayers] : h->train->leg_grad + h->train->leg_off[slot];
+  const float* g = h->train->grad + h->params.off[slot];
   OVN_CUDA(h, cudaDeviceSynchronize());
   OVN_CUDA(h, cudaMemcpy(h_kernel, g, nk * sizeof(float), cudaMemcpyDeviceToHost));
   OVN_CUDA(h, cudaMemcpy(h_bias, g + nk, nb * sizeof(float), cudaMemcpyDeviceToHost));
@@ -683,56 +694,66 @@ struct TrainPrecisionScope {
   ~TrainPrecisionScope() { h->train_tc = false; }
 };
 
-// ---- training of the overlap head (frozen leg) ----------------------------------------------------
-int ovn_head_gradients(ovn_handle* h, const float* d_bank, int64_t bank_size, const int32_t* d_left_idx,
-                       const int32_t* d_right_idx, int32_t n_pairs, const float* d_gt_overlap,
-                       const int32_t* d_gt_orientation, float min_overlap_for_angle, float* h_loss, void* stream) {
-  if (!h) return OVN_ERR_INVALID_ARG;
-  DeviceGuard guard(h);
-  TrainPrecisionScope precision(h);
-  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_head_gradients: %s", h->net_error.c_str());
+// ---- training: the overlap head with a frozen leg, or the whole network (360OutputkLegs) ---------------------
+// What ovn_head_gradients (rows: the feature-volume bank) and ovn_net_gradients (rows: the image set) share: the
+// checks, the training state, both index lists bounds-checked against the n_rows rows, and after the flow's own
+// work (`run`) the losses and the device error flag.
+}  // extern "C"
+template <class Run>
+static int gradients_call(ovn_handle* h, bool whole_network, const float* d_rows, int64_t n_rows,
+                          const int32_t* d_left_idx, const int32_t* d_right_idx, int32_t n_pairs,
+                          const float* d_gt_overlap, const int32_t* d_gt_orientation, float* h_loss, cudaStream_t s,
+                          Run run) {
+  const char* fn = whole_network ? "ovn_net_gradients" : "ovn_head_gradients";
+  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "%s: %s", fn, h->net_error.c_str());
   if (h->cfg.precision != OVN_PREC_FP32)
-    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_head_gradients: training needs a precision fp32 handle");
-  if (!h->weights_ready) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "ovn_head_gradients: weights not finalised");
-  REQUIRE(h, n_pairs > 0 && bank_size > 0, "n_pairs and bank_size must be positive");
-  REQUIRE(h, d_bank && d_left_idx && d_right_idx && d_gt_overlap && d_gt_orientation && h_loss, "NULL pointer");
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "%s: training needs a precision fp32 handle", fn);
+  if (!h->weights_ready) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "%s: weights not finalised", fn);
+  if (n_pairs <= 0 || n_rows <= 0)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: n_pairs and %s must be positive", fn,
+                whole_network ? "n_images" : "bank_size");
+  if (!(d_rows && d_left_idx && d_right_idx && d_gt_overlap && d_gt_orientation && h_loss))
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: NULL pointer", fn);
   const int maxp = h->cfg.max_batch_pairs;
-  if (n_pairs > maxp)
-    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "ovn_head_gradients: n_pairs=%d exceeds max_batch_pairs=%d", n_pairs, maxp);
+  if (n_pairs > maxp) OVN_SET_ERR(h, OVN_ERR_CAPACITY, "%s: n_pairs=%d exceeds max_batch_pairs=%d", fn, n_pairs, maxp);
+  if (whole_network && n_pairs > net_max_pairs(h))
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "%s: n_pairs=%d exceeds the %d pairs one call can launch", fn, n_pairs,
+                net_max_pairs(h));
   if (!h->train) {
     int rc = train_alloc(h);
     if (rc != OVN_OK) return rc;
   }
-  h->train->grads_valid = false;
-  h->train->net_grads_valid = false;
-  cudaStream_t s = (cudaStream_t)stream;
+  h->train->grads = kNoGrads;
   int32_t* l = h->d_idx_san;
   int32_t* r = h->d_idx_san + maxp;
-  int rc = sanitize_indices(h, d_left_idx, n_pairs, bank_size, kErrBadIndex, l, s);
-  if (rc == OVN_OK) rc = sanitize_indices(h, d_right_idx, n_pairs, bank_size, kErrBadIndex, r, s);
-  if (rc == OVN_OK)
-    rc = head_gradients_fp32(h, d_bank, l, r, n_pairs, d_gt_overlap, d_gt_orientation, min_overlap_for_angle, s);
+  int rc = sanitize_indices(h, d_left_idx, n_pairs, n_rows, kErrBadIndex, l, s);
+  if (rc == OVN_OK) rc = sanitize_indices(h, d_right_idx, n_pairs, n_rows, kErrBadIndex, r, s);
+  if (rc == OVN_OK) rc = run(l, r);
   if (rc != OVN_OK) return rc;
   float* p_loss = h->stage()->loss;
   OVN_CUDA(h, cudaMemcpyAsync(p_loss, h->train->loss, 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
   rc = check_device_error(h, s);            // synchronises s; a bad index -> OVN_ERR_INVALID_ARG
   if (rc != OVN_OK) return rc;
   memcpy(h_loss, p_loss, 3 * sizeof(float));
-  h->train->grads_valid = true;
+  h->train->grads = whole_network ? kNetGrads : kHeadGrads;
   return OVN_OK;
 }
+extern "C" {
 
-int ovn_head_adagrad_step(ovn_handle* h, float learning_rate, void* stream) {
+int ovn_head_gradients(ovn_handle* h, const float* d_bank, int64_t bank_size, const int32_t* d_left_idx,
+                       const int32_t* d_right_idx, int32_t n_pairs, const float* d_gt_overlap,
+                       const int32_t* d_gt_orientation, float min_overlap_for_angle, float* h_loss, void* stream) {
   if (!h) return OVN_ERR_INVALID_ARG;
   DeviceGuard guard(h);
-  if (h->cfg.precision != OVN_PREC_FP32)
-    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_head_adagrad_step: training needs a precision fp32 handle");
-  if (!h->train || !h->train->grads_valid)
-    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_head_adagrad_step: no valid gradients (call ovn_head_gradients first)");
-  return head_adagrad_fp32(h, learning_rate, (cudaStream_t)stream);
+  TrainPrecisionScope precision(h);
+  cudaStream_t s = (cudaStream_t)stream;
+  return gradients_call(h, false, d_bank, bank_size, d_left_idx, d_right_idx, n_pairs, d_gt_overlap,
+                        d_gt_orientation, h_loss, s, [&](const int32_t* l, const int32_t* r) {
+                          return head_gradients_fp32(h, d_bank, l, r, n_pairs, d_gt_overlap, d_gt_orientation,
+                                                     min_overlap_for_angle, s);
+                        });
 }
 
-// ---- training of the whole network (360OutputkLegs) -----------------------------------------------
 int ovn_net_gradients(ovn_handle* h, const float* d_images, int64_t n_images, const int32_t* d_left_idx,
                       const int32_t* d_right_idx, int32_t n_pairs, const float* d_gt_overlap,
                       const int32_t* d_gt_orientation, float min_overlap_for_angle, float* h_loss, float* d_fv_grad,
@@ -740,52 +761,34 @@ int ovn_net_gradients(ovn_handle* h, const float* d_images, int64_t n_images, co
   if (!h) return OVN_ERR_INVALID_ARG;
   DeviceGuard guard(h);
   TrainPrecisionScope precision(h);
-  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_net_gradients: %s", h->net_error.c_str());
-  if (h->cfg.precision != OVN_PREC_FP32)
-    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_net_gradients: training needs a precision fp32 handle");
-  if (!h->weights_ready) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "ovn_net_gradients: weights not finalised");
-  REQUIRE(h, n_pairs > 0 && n_images > 0, "n_pairs and n_images must be positive");
-  REQUIRE(h, d_images && d_left_idx && d_right_idx && d_gt_overlap && d_gt_orientation && h_loss, "NULL pointer");
-  const int maxp = h->cfg.max_batch_pairs;
-  if (n_pairs > maxp)
-    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "ovn_net_gradients: n_pairs=%d exceeds max_batch_pairs=%d", n_pairs, maxp);
-  if (n_pairs > net_max_pairs(h))
-    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "ovn_net_gradients: n_pairs=%d exceeds the %d pairs one call can launch", n_pairs,
-                net_max_pairs(h));
-  if (!h->train) {
-    int rc = train_alloc(h);
-    if (rc != OVN_OK) return rc;
-  }
-  h->train->grads_valid = false;
-  h->train->net_grads_valid = false;
   cudaStream_t s = (cudaStream_t)stream;
-  int32_t* l = h->d_idx_san;
-  int32_t* r = h->d_idx_san + maxp;
-  int rc = sanitize_indices(h, d_left_idx, n_pairs, n_images, kErrBadIndex, l, s);
-  if (rc == OVN_OK) rc = sanitize_indices(h, d_right_idx, n_pairs, n_images, kErrBadIndex, r, s);
-  if (rc == OVN_OK)
-    rc = net_gradients_fp32(h, d_images, l, r, n_pairs, d_gt_overlap, d_gt_orientation, min_overlap_for_angle,
-                            d_fv_grad, s);
-  if (rc != OVN_OK) return rc;
-  float* p_loss = h->stage()->loss;
-  OVN_CUDA(h, cudaMemcpyAsync(p_loss, h->train->loss, 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
-  rc = check_device_error(h, s);            // synchronises s; a bad index -> OVN_ERR_INVALID_ARG
-  if (rc != OVN_OK) return rc;
-  memcpy(h_loss, p_loss, 3 * sizeof(float));
-  h->train->grads_valid = true;
-  h->train->net_grads_valid = true;
-  return OVN_OK;
+  return gradients_call(h, true, d_images, n_images, d_left_idx, d_right_idx, n_pairs, d_gt_overlap,
+                        d_gt_orientation, h_loss, s, [&](const int32_t* l, const int32_t* r) {
+                          return net_gradients_fp32(h, d_images, l, r, n_pairs, d_gt_overlap, d_gt_orientation,
+                                                    min_overlap_for_angle, d_fv_grad, s);
+                        });
+}
+
+// ovn_head_adagrad_step / ovn_net_adagrad_step: the handle's own gradients as one part of weight 1
+static int adagrad_step(ovn_handle* h, bool whole_network, float learning_rate, void* stream) {
+  const char* fn = whole_network ? "ovn_net_adagrad_step" : "ovn_head_adagrad_step";
+  DeviceGuard guard(h);
+  if (h->cfg.precision != OVN_PREC_FP32)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "%s: training needs a precision fp32 handle", fn);
+  if (!h->train || h->train->grads < (whole_network ? kNetGrads : kHeadGrads))
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: %s", fn,
+                whole_network ? "no valid whole-network gradients (call ovn_net_gradients first)"
+                              : "no valid gradients (call ovn_head_gradients first)");
+  const float one = 1.f;
+  return adagrad_sum_fp32(h, whole_network, h->train->grad, 1, &one, learning_rate, (cudaStream_t)stream);
+}
+
+int ovn_head_adagrad_step(ovn_handle* h, float learning_rate, void* stream) {
+  return h ? adagrad_step(h, false, learning_rate, stream) : OVN_ERR_INVALID_ARG;
 }
 
 int ovn_net_adagrad_step(ovn_handle* h, float learning_rate, void* stream) {
-  if (!h) return OVN_ERR_INVALID_ARG;
-  DeviceGuard guard(h);
-  if (h->cfg.precision != OVN_PREC_FP32)
-    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_net_adagrad_step: training needs a precision fp32 handle");
-  if (!h->train || !h->train->net_grads_valid)
-    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_net_adagrad_step: no valid whole-network gradients (call "
-                "ovn_net_gradients first)");
-  return net_adagrad_fp32(h, learning_rate, (cudaStream_t)stream);
+  return h ? adagrad_step(h, true, learning_rate, stream) : OVN_ERR_INVALID_ARG;
 }
 
 // ---- data-parallel training ---------------------------------------------------------------------------------
@@ -793,7 +796,7 @@ int ovn_train_gradient_size(ovn_handle* h, int32_t whole_network, int64_t* n) {
   if (!h) return OVN_ERR_INVALID_ARG;
   REQUIRE(h, n, "NULL pointer");
   if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_train_gradient_size: %s", h->net_error.c_str());
-  *n = train_gradient_size(h, whole_network != 0);
+  *n = whole_network ? h->params.n_total : h->params.n_head;
   return OVN_OK;
 }
 
@@ -803,13 +806,16 @@ int ovn_copy_gradients(ovn_handle* h, int32_t whole_network, float* d_out, void*
   if (h->cfg.precision != OVN_PREC_FP32)
     OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_copy_gradients: training needs a precision fp32 handle");
   REQUIRE(h, d_out, "NULL pointer");
-  if (!h->train || !h->train->grads_valid)
+  if (!h->train || h->train->grads < kHeadGrads)
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_copy_gradients: no valid gradients (call ovn_head_gradients or "
                 "ovn_net_gradients first)");
-  if (whole_network && !h->train->net_grads_valid)
+  if (whole_network && h->train->grads < kNetGrads)
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_copy_gradients: no valid whole-network gradients (call "
                 "ovn_net_gradients first)");
-  return copy_gradients_fp32(h, whole_network != 0, d_out, (cudaStream_t)stream);
+  const int64_t n = whole_network ? h->params.n_total : h->params.n_head;
+  OVN_CUDA(h, cudaMemcpyAsync(d_out, h->train->grad, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice,
+                              (cudaStream_t)stream));
+  return OVN_OK;
 }
 
 int ovn_copy_net_volumes(ovn_handle* h, float* d_out, void* stream) {
@@ -818,7 +824,7 @@ int ovn_copy_net_volumes(ovn_handle* h, float* d_out, void* stream) {
   if (h->cfg.precision != OVN_PREC_FP32)
     OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_copy_net_volumes: training needs a precision fp32 handle");
   REQUIRE(h, d_out, "NULL pointer");
-  if (!h->train || !h->train->net_grads_valid)
+  if (!h->train || h->train->grads < kNetGrads)
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_copy_net_volumes: no valid whole-network batch (call ovn_net_gradients "
                 "first)");
   return copy_net_volumes_fp32(h, d_out, (cudaStream_t)stream);
@@ -838,10 +844,6 @@ int ovn_adagrad_step_sum(ovn_handle* h, int32_t whole_network, const float* d_pa
   REQUIRE(h, d_parts && h_weights, "NULL pointer");
   if (!h->train) {
     int rc = train_alloc(h);
-    if (rc != OVN_OK) return rc;
-  }
-  if (whole_network) {
-    int rc = leg_train_alloc(h);
     if (rc != OVN_OK) return rc;
   }
   return adagrad_sum_fp32(h, whole_network != 0, d_parts, n_parts, h_weights, learning_rate, (cudaStream_t)stream);

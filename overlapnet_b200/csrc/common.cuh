@@ -90,9 +90,23 @@ namespace ovn {
 struct TcState;
 struct TcStateDelete { void operator()(TcState* t) const; };   // network_tc.cu: TcState is private to it
 
-// Training of the overlap head (fp32 handles; allocated when a handle first trains, sized by max_batch_pairs).
-// Gradients and Adagrad accumulators of c_conv1..3 / overlap_output: per layer [K + 1][N] floats at off[l]
-// (the kernel in Keras layout, then the bias).
+// The flat parameter vector of training (ovn_copy_gradients' layout): c_conv1..3, overlap_output, then the leg
+// layers from input to output, each [K + 1][N] floats (the kernel [K][N] in Keras layout, then the bias [N]).
+// Set by ovn_create from the layer shapes.
+struct ParamLayout {
+  int64_t off[kMaxLegLayers + 4] = {};        // by weight slot (the index of d_w / d_b): the layer's kernel
+  int64_t n_kernel[kMaxLegLayers + 4] = {};   // K N: the layer's bias starts at off + n_kernel
+  int64_t n_head = 0;                         // the heads' prefix
+  int64_t n_total = 0;                        // the whole network
+};
+// weight slot of the i-th layer of the flat vector
+inline int flat_slot(int i) { return i < 4 ? kMaxLegLayers + i : i - 4; }
+
+// Which layers the last valid gradients (TrainState::grad) cover
+enum GradCover { kNoGrads = 0, kHeadGrads, kNetGrads };
+
+// Training (fp32 handles; allocated when a handle first trains, sized by max_batch_pairs).  The gradients and
+// Adagrad accumulators are whole ParamLayout vectors: a head-only call leaves the leg's part of grad unused.
 struct TrainState {
   Buffer<float> x4;             // [max_batch_pairs][dense_in] c_conv3 output, then dL/d(its pre-activation)
   Buffer<float> dx3;            // [max_batch_pairs][24][24][128] dL/dx3, then dL/d(pre-activation of c_conv2)
@@ -102,14 +116,12 @@ struct TrainState {
   Buffer<int32_t> yaw;          // [max_batch_pairs]
   Buffer<float> w3t;            // c_conv3 kernel with in / out swapped
   Buffer<float> part;           // split-K partials of the weight gradients
-  Buffer<float> grad;           // [n_param]
-  Buffer<float> accum;          // [n_param] Adagrad accumulators
+  Buffer<float> grad;           // [ParamLayout::n_total]
+  Buffer<float> accum;          // [ParamLayout::n_total] Adagrad accumulators
   Buffer<float> loss;           // [3] total, overlap, orientation
-  int64_t off[4] = {};
-  int64_t n_param = 0;
-  bool grads_valid = false;     // the last ovn_head_gradients / ovn_net_gradients succeeded
-  // Whole-network training (ovn_net_gradients): allocated on its first call, the per-batch buffers grown to
-  // the batch.  The 2n images of an n-pair batch are LEFT 0..n-1, then RIGHT 0..n-1.
+  GradCover grads = kNoGrads;   // set by the last successful ovn_head_gradients / ovn_net_gradients
+  // Whole-network training (ovn_net_gradients): allocated on its first call, grown to the batch.  The 2n images
+  // of an n-pair batch are LEFT 0..n-1, then RIGHT 0..n-1.
   Buffer<float> images;         // [2n][H][W][C] the gathered input images
   Buffer<float> acts;           // every leg layer's output for those images, layer after layer
   Buffer<float> dact[2];        // ping-pong gradients of the leg activations (dact[0] first holds dL/d(volumes))
@@ -117,11 +129,6 @@ struct TrainState {
   Buffer<float> dcorr;          // [n][Wf] dL/d(correlation logits)
   Buffer<int32_t> pair_rows;    // [2n] 0..2n-1: LEFT / RIGHT rows of the batch's volumes
   Buffer<float> wt;             // a leg kernel with in / out swapped
-  Buffer<float> leg_grad;       // [n_leg_param] per leg layer [K + 1][N] at leg_off[l], like grad
-  Buffer<float> leg_accum;      // [n_leg_param] Adagrad accumulators
-  int64_t leg_off[kMaxLegLayers] = {};
-  int64_t n_leg_param = 0;
-  bool net_grads_valid = false; // the last ovn_net_gradients succeeded (leg_grad and grad are of one batch)
   int64_t net_fv_off = 0;       // the last ovn_net_gradients batch: its volumes [2 net_np][Wf][128] at acts + net_fv_off
   int net_np = 0;
 };
@@ -142,6 +149,7 @@ struct ovn_handle {
   int o2_h = 0, o2_w = 0;               // c_conv2 output (24, 24)
   int o3_h = 0, o3_w = 0;               // c_conv3 output (22, 22)
   int dense_in = 0;
+  ovn::ParamLayout params;              // the flat gradient / accumulator layout of training
 
   std::map<std::string, ovn::LayerWeights> host_w;
   bool weights_ready = false;
@@ -322,20 +330,15 @@ int train_alloc(ovn_handle* h);
 int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left, const int32_t* right, int np,
                         const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
                         cudaStream_t s);
-int head_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s);
 // training of the whole network (network_fp32.cu): left / right index the image bank and are bounds-checked
 int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left, const int32_t* right, int np,
                        const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
                        float* d_fv_grad, cudaStream_t s);
-int net_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s);
 int net_max_pairs(const ovn_handle* h);   // largest n_pairs of one ovn_net_gradients call (launch grid limits)
-// data-parallel training (network_fp32.cu): the flat gradient vector is the heads' [n_param] and then, with
-// whole_network, the leg's [n_leg_param]
-constexpr int kMaxSumParts = 64;
-int64_t train_gradient_size(const ovn_handle* h, bool whole_network);
-int leg_train_alloc(ovn_handle* h);        // train->leg_grad / leg_accum / leg_off, once
-int copy_gradients_fp32(ovn_handle* h, bool whole_network, float* d_out, cudaStream_t s);
 int copy_net_volumes_fp32(ovn_handle* h, float* d_out, cudaStream_t s);
+// The Adagrad step of the heads' (or with whole_network every layer's) prefix of the flat vector, from the
+// weighted sum of d_parts [n_parts][that length]: one launch
+constexpr int kMaxSumParts = 64;
 int adagrad_sum_fp32(ovn_handle* h, bool whole_network, const float* d_parts, int n_parts, const float* h_weights,
                      float lr, cudaStream_t s);
 // yaw augmentation of training images (projection.cu): rows are bounds-checked on the device (kErrBadIndex)

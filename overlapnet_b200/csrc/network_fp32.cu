@@ -206,6 +206,80 @@ struct BOperand {
   int b_nk;
 };
 
+// ---- the staging k_simt_gemm and k_tc_gemm share ----
+// A CTA of either kernel: the 64 x 64 output tile at (m0, n0) of batch / split index z, its K slice [kbeg, kend)
+// and its B operand Bz.  gemm_tile also writes the row bases of the tile's BM rows to s_rb / s_rb2 (-1: past M);
+// the caller synchronises before gemm_fetch reads them.
+struct GemmTile {
+  int m0, n0, z, kbeg, kend;
+  const float* Bz;
+};
+
+template <class AOp>
+__device__ __forceinline__ GemmTile gemm_tile(const AOp& a, const BOperand& bop, int M, int K, int kchunk,
+                                              int64_t* s_rb, int64_t* s_rb2) {
+  GemmTile t;
+  t.m0 = blockIdx.y * BM;
+  t.n0 = blockIdx.x * BN;
+  t.z = blockIdx.z;
+  const int zb = kchunk ? 0 : t.z;
+  t.kbeg = kchunk ? t.z * kchunk : 0;
+  t.kend = kchunk ? min(K, t.kbeg + kchunk) : K;
+  if (threadIdx.x < BM) {
+    const int m = t.m0 + threadIdx.x;
+    s_rb[threadIdx.x] = m < M ? a.row_base(m, zb) : -1;
+    s_rb2[threadIdx.x] = m < M ? a.row_base2(m, zb) : 0;
+  }
+  t.Bz = bop.B;
+  if (bop.b_nk) t.Bz = bop.query ? bop.query : bop.B + (int64_t)bop.right[zb] * bop.vol_stride;
+  return t;
+}
+
+// The place (kk, mm) in the A tile of element e = tid + 256 i of a K16 tile: consecutive threads take consecutive
+// k, contiguous in memory.  Its place (kk, nn) in the B tile: for b_nk = 0 consecutive threads take consecutive n.
+__device__ __forceinline__ int2 a_place(int e) { return make_int2(e % BK, e / BK); }
+__device__ __forceinline__ int2 b_place(int b_nk, int e) {
+  return b_nk ? make_int2(e % BK, e / BK) : make_int2(e / BN, e % BN);
+}
+
+// A thread's four A and four B elements of the K16 tile at k0, zero outside [k0, kend), past M and past N:
+// put_a(kk, mm, v) and put_b(kk, nn, v) take them at their places.
+template <class AOp, class PutA, class PutB>
+__device__ __forceinline__ void gemm_fetch(const AOp& a, const BOperand& bop, const GemmTile& t, int k0, int N, int K,
+                                           const int64_t* s_rb, const int64_t* s_rb2, PutA put_a, PutB put_b) {
+  const int tid = threadIdx.x;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int2 q = a_place(tid + i * 256);
+    const int k = k0 + q.x, mm = q.y;
+    float v = 0.f;
+    if (k < t.kend && s_rb[mm] >= 0) v = a.load(s_rb[mm], a.col_off(k), s_rb2[mm], a.col_off2(k));
+    put_a(i, q.x, mm, v);
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float v = 0.f;
+    if (!bop.b_nk) {
+      const int2 q = b_place(0, tid + i * 256);
+      if (k0 + q.x < t.kend && t.n0 + q.y < N) v = __ldg(t.Bz + (int64_t)(k0 + q.x) * N + t.n0 + q.y);
+      put_b(i, q.x, q.y, v);
+    } else {
+      const int2 q = b_place(1, tid + i * 256);
+      if (k0 + q.x < t.kend && t.n0 + q.y < N) v = __ldg(t.Bz + (int64_t)(t.n0 + q.y) * K + k0 + q.x);
+      put_b(i, q.x, q.y, v);
+    }
+  }
+}
+
+// The epilogue of output element (m, n) of the tile: C[z][m][n] = act(acc + bias[n]) inside M x N
+__device__ __forceinline__ void gemm_store(const GemmTile& t, float acc, int m, int n, const float* bias, int relu,
+                                           float* C, int M, int N) {
+  if (m >= M || n >= N) return;
+  float v = acc + (bias ? __ldg(bias + n) : 0.f);
+  if (relu) v = fmaxf(v, 0.f);
+  C[((int64_t)t.z * M + m) * N + n] = v;
+}
+
 // C[m, n] = act(sum_k A[m,k] * B[k,n] + bias[n]);  C row-major [z][M][N].
 // kchunk == 0: z = blockIdx.z is the batch index of the operands.  kchunk > 0 (split-K): every z works on
 // the same product and sums only k in [z*kchunk, (z+1)*kchunk); C[z] is that slice's partial, which
@@ -219,45 +293,13 @@ k_simt_gemm(AOp a, BOperand bop, const float* __restrict__ bias, float* __restri
   __shared__ int64_t s_rb[BM];
   __shared__ int64_t s_rb2[BM];
   const int tid = threadIdx.x;
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN, z = blockIdx.z;
-  const int zb = kchunk ? 0 : z;
-  const int kbeg = kchunk ? z * kchunk : 0;
-  const int kend = kchunk ? min(K, kbeg + kchunk) : K;
-  if (tid < BM) {
-    const int m = m0 + tid;
-    s_rb[tid] = m < M ? a.row_base(m, zb) : -1;
-    s_rb2[tid] = m < M ? a.row_base2(m, zb) : 0;
-  }
-  const float* Bz = bop.B;
-  if (bop.b_nk) Bz = bop.query ? bop.query : bop.B + (int64_t)bop.right[zb] * bop.vol_stride;
+  const GemmTile t = gemm_tile(a, bop, M, K, kchunk, s_rb, s_rb2);
   __syncthreads();
   const int ty = tid / 16, tx = tid % 16;
   float acc[4][4] = {};
-  for (int k0 = kbeg; k0 < kend; k0 += BK) {
-    // A tile: 64 x 16 elements, consecutive threads -> consecutive k (contiguous in memory)
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int e = tid + i * 256;
-      const int kk = e % BK, mm = e / BK;
-      const int k = k0 + kk;
-      float v = 0.f;
-      if (k < kend && s_rb[mm] >= 0) v = a.load(s_rb[mm], a.col_off(k), s_rb2[mm], a.col_off2(k));
-      As[kk][mm] = v;
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int e = tid + i * 256;
-      float v = 0.f;
-      if (!bop.b_nk) {
-        const int nn = e % BN, kk = e / BN;
-        if (k0 + kk < kend && n0 + nn < N) v = __ldg(Bz + (int64_t)(k0 + kk) * N + n0 + nn);
-        Bs[kk][nn] = v;
-      } else {
-        const int kk = e % BK, nn = e / BK;
-        if (k0 + kk < kend && n0 + nn < N) v = __ldg(Bz + (int64_t)(n0 + nn) * K + k0 + kk);
-        Bs[kk][nn] = v;
-      }
-    }
+  for (int k0 = t.kbeg; k0 < t.kend; k0 += BK) {
+    gemm_fetch(a, bop, t, k0, N, K, s_rb, s_rb2, [&](int, int kk, int mm, float v) { As[kk][mm] = v; },
+               [&](int, int kk, int nn, float v) { Bs[kk][nn] = v; });
     __syncthreads();
 #pragma unroll
     for (int kk = 0; kk < BK; ++kk) {
@@ -274,18 +316,9 @@ k_simt_gemm(AOp a, BOperand bop, const float* __restrict__ bias, float* __restri
     __syncthreads();
   }
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int m = m0 + ty * 4 + i;
-    if (m >= M) continue;
+  for (int i = 0; i < 4; ++i)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int n = n0 + tx * 4 + j;
-      if (n >= N) continue;
-      float v = acc[i][j] + (bias ? __ldg(bias + n) : 0.f);
-      if (relu) v = fmaxf(v, 0.f);
-      C[((int64_t)z * M + m) * N + n] = v;
-    }
-  }
+    for (int j = 0; j < 4; ++j) gemm_store(t, acc[i][j], t.m0 + ty * 4 + i, t.n0 + tx * 4 + j, bias, relu, C, M, N);
 }
 
 // ---- 3xTF32 tensor-core bodies of the training products (ovn_set_train_precision) -------------------------
@@ -372,10 +405,9 @@ __device__ __forceinline__ void add_tile(float (&acc)[2][2][4], const float (*ah
       for (int r = 0; r < 4; ++r) acc[mi][ni][r] = __fadd_rn(acc[mi][ni][r], part[mi][ni][r]);
 }
 
-// k_simt_gemm's product on tensor cores: the same arguments, grid, 64 x 64 x 16 block tile, operand staging
-// (bounds rules and zero fill) and epilogue.  Eight warps in 2 (M) x 4 (N), each a 32 x 16 tile of 2 x 2 MMA
-// tiles.  A thread stages its elements of the next K16 tile in registers while the warps multiply the current
-// one.
+// k_simt_gemm's product on tensor cores, with its arguments, grid, 64 x 64 x 16 block tile and staging
+// (gemm_tile, gemm_fetch, gemm_store).  Eight warps in 2 (M) x 4 (N), each a 32 x 16 tile of 2 x 2 MMA tiles.
+// A thread stages its elements of the next K16 tile in registers while the warps multiply the current one.
 template <class AOp>
 __global__ void __launch_bounds__(256)
 k_tc_gemm(AOp a, BOperand bop, const float* __restrict__ bias, float* __restrict__ C, int M, int N, int K,
@@ -387,55 +419,25 @@ k_tc_gemm(AOp a, BOperand bop, const float* __restrict__ bias, float* __restrict
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t = lane & 3;
   const int wm = (warp >> 2) * 32, wn = (warp & 3) * 16;
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN, z = blockIdx.z;
-  const int zb = kchunk ? 0 : z;
-  const int kbeg = kchunk ? z * kchunk : 0;
-  const int kend = kchunk ? min(K, kbeg + kchunk) : K;
-  if (tid < BM) {
-    const int m = m0 + tid;
-    s_rb[tid] = m < M ? a.row_base(m, zb) : -1;
-    s_rb2[tid] = m < M ? a.row_base2(m, zb) : 0;
-  }
-  const float* Bz = bop.B;
-  if (bop.b_nk) Bz = bop.query ? bop.query : bop.B + (int64_t)bop.right[zb] * bop.vol_stride;
+  const GemmTile tile = gemm_tile(a, bop, M, K, kchunk, s_rb, s_rb2);
   __syncthreads();
+  // the next K16 tile waits in registers
   float va[4], vb[4];
-  // element e = tid + 256 i of the A tile is (kk = e % BK, mm = e / BK); of the B tile (kk = e / BN, nn = e % BN)
-  // for b_nk = 0, (kk = e % BK, nn = e / BK) for b_nk = 1: k_simt_gemm's assignment
   auto load = [&](int k0) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int e = tid + i * 256;
-      const int kk = e % BK, mm = e / BK;
-      const int k = k0 + kk;
-      va[i] = 0.f;
-      if (k < kend && s_rb[mm] >= 0) va[i] = a.load(s_rb[mm], a.col_off(k), s_rb2[mm], a.col_off2(k));
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int e = tid + i * 256;
-      vb[i] = 0.f;
-      if (!bop.b_nk) {
-        const int nn = e % BN, kk = e / BN;
-        if (k0 + kk < kend && n0 + nn < N) vb[i] = __ldg(Bz + (int64_t)(k0 + kk) * N + n0 + nn);
-      } else {
-        const int kk = e % BK, nn = e / BK;
-        if (k0 + kk < kend && n0 + nn < N) vb[i] = __ldg(Bz + (int64_t)(n0 + nn) * K + k0 + kk);
-      }
-    }
+    gemm_fetch(a, bop, tile, k0, N, K, s_rb, s_rb2, [&](int i, int, int, float v) { va[i] = v; },
+               [&](int i, int, int, float v) { vb[i] = v; });
   };
   float acc[2][2][4] = {};
-  if (kbeg < kend) load(kbeg);
-  for (int k0 = kbeg; k0 < kend; k0 += BK) {
+  if (tile.kbeg < tile.kend) load(tile.kbeg);
+  for (int k0 = tile.kbeg; k0 < tile.kend; k0 += BK) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const int e = tid + i * 256;
-      split_tf32(va[i], Ah[e % BK][e / BK], Al[e % BK][e / BK]);
-      if (!bop.b_nk) split_tf32(vb[i], Bh[e / BN][e % BN], Bl[e / BN][e % BN]);
-      else split_tf32(vb[i], Bh[e % BK][e / BK], Bl[e % BK][e / BK]);
+      const int2 qa = a_place(tid + i * 256), qb = b_place(bop.b_nk, tid + i * 256);
+      split_tf32(va[i], Ah[qa.x][qa.y], Al[qa.x][qa.y]);
+      split_tf32(vb[i], Bh[qb.x][qb.y], Bl[qb.x][qb.y]);
     }
     __syncthreads();
-    if (k0 + BK < kend) load(k0 + BK);
+    if (k0 + BK < tile.kend) load(k0 + BK);
     add_tile(acc, Ah, Al, Bh, Bl, 0, wm, wn, g, t);
     __syncthreads();
   }
@@ -444,14 +446,9 @@ k_tc_gemm(AOp a, BOperand bop, const float* __restrict__ bias, float* __restrict
 #pragma unroll
     for (int ni = 0; ni < 2; ++ni)
 #pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        const int m = m0 + wm + mi * 16 + g + (r >> 1) * 8;
-        const int n = n0 + wn + ni * 8 + 2 * t + (r & 1);
-        if (m >= M || n >= N) continue;
-        float v = acc[mi][ni][r] + (bias ? __ldg(bias + n) : 0.f);
-        if (relu) v = fmaxf(v, 0.f);
-        C[((int64_t)z * M + m) * N + n] = v;
-      }
+      for (int r = 0; r < 4; ++r)
+        gemm_store(tile, acc[mi][ni][r], tile.m0 + wm + mi * 16 + g + (r >> 1) * 8,
+                   tile.n0 + wn + ni * 8 + 2 * t + (r & 1), bias, relu, C, M, N);
 }
 
 // The training entry points set h->train_tc for their duration when the handle's training precision is
@@ -696,17 +693,6 @@ __global__ void k_splitk_reduce(const float* __restrict__ part, int nsplit, int6
   out[i] = v;
 }
 
-// Adagrad as Keras 2.1.5 does it: a += g^2;  w -= lr * g / (sqrt(a) + 1e-7)
-__global__ void k_adagrad(float* __restrict__ w, const float* __restrict__ g, float* __restrict__ a, int64_t n,
-                          float lr) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float gi = g[i];
-  const float ai = a[i] + gi * gi;
-  a[i] = ai;
-  w[i] -= lr * gi / (sqrtf(ai) + 1e-7f);
-}
-
 static unsigned blocks_for(int64_t n) { return (unsigned)((n + 255) / 256); }
 
 // rows K and columns N of the gradient of head layer l (c_conv1..3, overlap_output); the gradient
@@ -720,16 +706,14 @@ static void head_dims(const ovn_handle* h, int l, int* K, int* N) {
 int train_alloc(ovn_handle* h) {
   const int64_t maxp = h->cfg.max_batch_pairs, Wf = h->cfg.leg_output_width;
   const ConvSpec& L3 = h->head[2];
+  const int64_t total = h->params.n_total;
   std::unique_ptr<TrainState> t(new TrainState());
-  int64_t total = 0, max_part = 0;
-  for (int l = 0; l < 4; ++l) {
+  int64_t max_part = 0;
+  for (int l = 0; l < 3; ++l) {
     int K, N;
     head_dims(h, l, &K, &N);
-    t->off[l] = total;
-    total += (int64_t)(K + 1) * N;
-    if (l < 3 && (int64_t)(K + 1) * N > max_part) max_part = (int64_t)(K + 1) * N;
+    if ((int64_t)(K + 1) * N > max_part) max_part = (int64_t)(K + 1) * N;
   }
-  t->n_param = total;
   int rc;
   if ((rc = t->x4.ensure(h, (size_t)maxp * h->dense_in * sizeof(float))) != OVN_OK) return rc;
   if ((rc = t->dx3.ensure(h, (size_t)maxp * L3.h_in * L3.w_in * L3.cin * sizeof(float))) != OVN_OK) return rc;
@@ -776,6 +760,7 @@ int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left,
   TrainState& t = *h->train;
   const int Wf = h->cfg.leg_output_width, Cf = kFeatC, sz = h->cfg.conv1size;
   const int base = kMaxLegLayers;
+  const int64_t* off = h->params.off + base;   // gradients of c_conv1..3, overlap_output
   const ConvSpec& L1 = h->head[0];
   const ConvSpec& L2 = h->head[1];
   const ConvSpec& L3 = h->head[2];
@@ -785,16 +770,16 @@ int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left,
   if (rc == OVN_OK) rc = corr_forward_fp32(h, d_bank, nullptr, left, right, np, t.yaw, t.corr, s);
   if (rc != OVN_OK) return rc;
   k_train_loss<<<1, 256, 0, s>>>(t.overlap, t.corr, d_gt_overlap, d_gt_orientation, np, Wf, min_overlap, t.dz,
-                                 t.grad + t.off[3] + K[3], t.loss);
+                                 t.grad + off[3] + K[3], t.loss);
   OVN_LAUNCH_CHECK(h);
   // overlap_output (Dense): dWd, and x4 becomes dL/d(pre-activation of c_conv3)
   k_dense_backward<<<blocks_for(h->dense_in), 256, 0, s>>>(t.x4, h->d_w[base + 3], t.dz, np, h->dense_in,
-                                                           t.grad + t.off[3]);
+                                                           t.grad + off[3]);
   OVN_LAUNCH_CHECK(h);
   // c_conv3: dW3 = patches(x3)^T dpre3 (+ db3), then dx3 = transposed 3x3 conv of dpre3, masked by x3 > 0
   {
     ConvWgradOperand a{h->d_o2, L3.h_in, L3.w_in, L3.cin, L3.kw, L3.sh, L3.sw, L3.h_out, L3.w_out, K[2]};
-    rc = wgrad_gemm(h, a, t.x4, K[2], N[2], np * L3.h_out * L3.w_out, t.grad + t.off[2], s);
+    rc = wgrad_gemm(h, a, t.x4, K[2], N[2], np * L3.h_out * L3.w_out, t.grad + off[2], s);
     if (rc != OVN_OK) return rc;
     k_swap_io<<<blocks_for((int64_t)K[2] * N[2]), 256, 0, s>>>(h->d_w[base + 2], t.w3t, L3.kh * L3.kw, L3.cin,
                                                                L3.cout);
@@ -811,7 +796,7 @@ int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left,
   // exactly one output pixel: do1 is stored per output pixel, [p][ho][wo][dh][c], over the dead o1
   {
     ConvWgradOperand a{h->d_o1, L2.h_in, L2.w_in, L2.cin, L2.kw, L2.sh, L2.sw, L2.h_out, L2.w_out, K[1]};
-    rc = wgrad_gemm(h, a, t.dx3, K[1], N[1], np * L2.h_out * L2.w_out, t.grad + t.off[1], s);
+    rc = wgrad_gemm(h, a, t.dx3, K[1], N[1], np * L2.h_out * L2.w_out, t.grad + off[1], s);
     if (rc != OVN_OK) return rc;
     ConvOperand g{t.dx3, L2.h_out, L2.w_out, L2.cout, 1, 1, 1, L2.h_out, L2.w_out};
     BOperand w2t{h->d_w[base + 1], h->d_w[base + 1], nullptr, 0, 1};     // W2 read as [(dh, c)][n]
@@ -821,24 +806,8 @@ int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left,
   // c_conv1 (linear): dW1[dj, c, o] = sum |L[i, c] - R[15 jb + dj, c]| do1[i, jb, o], db1 = sum do1
   {
     DeltaWgradOperand a{d_bank, left, right, Wf, Cf, sz, h->o1_w, L2.h_out, K[0]};
-    rc = wgrad_gemm(h, a, h->d_o1, K[0], N[0], np * L1.h_out * L1.w_out, t.grad + t.off[0], s);
+    rc = wgrad_gemm(h, a, h->d_o1, K[0], N[0], np * L1.h_out * L1.w_out, t.grad + off[0], s);
     if (rc != OVN_OK) return rc;
-  }
-  return OVN_OK;
-}
-
-int head_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s) {
-  TrainState& t = *h->train;
-  for (int l = 0; l < 4; ++l) {
-    int K, N;
-    head_dims(h, l, &K, &N);
-    const int64_t nk = (int64_t)K * N;
-    float* g = t.grad + t.off[l];
-    float* a = t.accum + t.off[l];
-    k_adagrad<<<blocks_for(nk), 256, 0, s>>>(h->d_w[kMaxLegLayers + l], g, a, nk, lr);
-    OVN_LAUNCH_CHECK(h);
-    k_adagrad<<<blocks_for(N), 256, 0, s>>>(h->d_b[kMaxLegLayers + l], g + nk, a + nk, N, lr);
-    OVN_LAUNCH_CHECK(h);
   }
   return OVN_OK;
 }
@@ -920,6 +889,53 @@ k_corr_backward(const float* __restrict__ dcorr, const float* __restrict__ fv, c
 // s taps dj; each tap is a 64 x 64 x 64 product in registers whose epilogue applies the signs.  Fixed-order
 // partials, reduced by k_delta_dgrad_reduce:  part_l[p][jb][i][c] (this CTA's sum over dj) and
 // part_r[p][row tile][j][c] (this CTA's sum over its 64 rows, in order).
+//
+// k_delta_dgrad and k_delta_dgrad_tc share the CTA's addresses (DeltaDgradCta) and the staging of its do1 and W1
+// tiles.  The tiles are stored transposed: a thread reads 4 consecutive o of one row and consecutive threads take
+// consecutive rows, so the shared-memory stores of a warp hit 32 different banks.
+struct DeltaDgradCta {
+  int c0, itile, i0, jb, p, nit;
+  __device__ __forceinline__ explicit DeltaDgradCta(int nb)
+      : c0(blockIdx.x * kDgT), itile(blockIdx.y), i0(blockIdx.y * kDgT), jb(blockIdx.z % nb), p(blockIdx.z / nb),
+        nit(gridDim.y) {}
+  // the pair's LEFT (rows = left) or RIGHT (rows = right) volume
+  __device__ __forceinline__ const float* volume(const float* fv, const int32_t* rows, int Wf) const {
+    return fv + (int64_t)rows[p] * Wf * kFeatC;
+  }
+  // channel c0 of row i of this CTA's part_l, and of column j of its part_r
+  __device__ __forceinline__ float* part_l_at(float* part_l, int nb, int Wf, int i) const {
+    return part_l + (((int64_t)p * nb + jb) * Wf + i) * kFeatC + c0;
+  }
+  __device__ __forceinline__ float* part_r_at(float* part_r, int Wf, int j) const {
+    return part_r + (((int64_t)p * nit + itile) * Wf + j) * kFeatC + c0;
+  }
+};
+
+// put(o, r, v) for the do1 tile's 64 rows i0 + r (zero past Wf) and 64 outputs o
+template <class Put>
+__device__ __forceinline__ void stage_do1(const DeltaDgradCta& cta, const float* do1, int Wf, int s, int nb, int nho,
+                                          Put put) {
+  for (int f = threadIdx.x; f < kDgT * kDgT / 4; f += 256) {
+    const int r = f % kDgT, o = (f / kDgT) * 4, i = cta.i0 + r;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (i < Wf) {
+      const int ho = i / s, dh = i - ho * s;
+      v = __ldg(reinterpret_cast<const float4*>(do1 + ((((int64_t)cta.p * nho + ho) * nb + cta.jb) * s + dh) * kDgT + o));
+    }
+    put(o, r, v.x); put(o + 1, r, v.y); put(o + 2, r, v.z); put(o + 3, r, v.w);
+  }
+}
+
+// put(o, c, v) for tap dj's W1 tile: 64 channels c0 + c, 64 outputs o
+template <class Put>
+__device__ __forceinline__ void stage_w1(const DeltaDgradCta& cta, const float* w1, int dj, Put put) {
+  for (int f = threadIdx.x; f < kDgT * kDgT / 4; f += 256) {
+    const int c = f % kDgT, o = (f / kDgT) * 4;
+    const float4 v = __ldg(reinterpret_cast<const float4*>(w1 + ((int64_t)dj * kFeatC + cta.c0 + c) * kDgT + o));
+    put(o, c, v.x); put(o + 1, c, v.y); put(o + 2, c, v.z); put(o + 3, c, v.w);
+  }
+}
+
 __global__ void __launch_bounds__(256)
 k_delta_dgrad(const float* __restrict__ do1, const float* __restrict__ w1, const float* __restrict__ fv,
               const int32_t* __restrict__ left, const int32_t* __restrict__ right, int Wf, int s, int nb, int nho,
@@ -928,38 +944,22 @@ k_delta_dgrad(const float* __restrict__ do1, const float* __restrict__ w1, const
   __shared__ __align__(16) float Bs[kDgT][kDgT + 4];     // [o][c]
   __shared__ float red[16][kDgT];
   const int tid = threadIdx.x, ty = tid / 16, tx = tid % 16;
-  const int c0 = blockIdx.x * kDgT, itile = blockIdx.y, i0 = itile * kDgT;
-  const int jb = blockIdx.z % nb, p = blockIdx.z / nb;
-  const int nit = gridDim.y;
-  // The tiles are stored transposed: a thread reads 4 consecutive o of one row and consecutive threads take
-  // consecutive rows, so the shared-memory stores of a warp hit 32 different banks.
-  for (int f = tid; f < kDgT * kDgT / 4; f += 256) {
-    const int r = f % kDgT, o = (f / kDgT) * 4, i = i0 + r;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (i < Wf) {
-      const int ho = i / s, dh = i - ho * s;
-      v = __ldg(reinterpret_cast<const float4*>(do1 + ((((int64_t)p * nho + ho) * nb + jb) * s + dh) * kDgT + o));
-    }
-    As[o][r] = v.x; As[o + 1][r] = v.y; As[o + 2][r] = v.z; As[o + 3][r] = v.w;
-  }
-  const float* L = fv + (int64_t)left[p] * Wf * kFeatC;
-  const float* R = fv + (int64_t)right[p] * Wf * kFeatC;
+  const DeltaDgradCta cta(nb);
+  stage_do1(cta, do1, Wf, s, nb, nho, [&](int o, int r, float v) { As[o][r] = v; });
+  const float* L = cta.volume(fv, left, Wf);
+  const float* R = cta.volume(fv, right, Wf);
   float lv[4][4], accl[4][4];
 #pragma unroll
   for (int ii = 0; ii < 4; ++ii) {
-    const int i = i0 + ty * 4 + ii;
-    const float4 v = i < Wf ? __ldg(reinterpret_cast<const float4*>(L + (int64_t)i * kFeatC + c0 + tx * 4))
+    const int i = cta.i0 + ty * 4 + ii;
+    const float4 v = i < Wf ? __ldg(reinterpret_cast<const float4*>(L + (int64_t)i * kFeatC + cta.c0 + tx * 4))
                             : make_float4(0.f, 0.f, 0.f, 0.f);
     lv[ii][0] = v.x; lv[ii][1] = v.y; lv[ii][2] = v.z; lv[ii][3] = v.w;
 #pragma unroll
     for (int jj = 0; jj < 4; ++jj) accl[ii][jj] = 0.f;
   }
   for (int dj = 0; dj < s; ++dj) {
-    for (int f = tid; f < kDgT * kDgT / 4; f += 256) {
-      const int c = f % kDgT, o = (f / kDgT) * 4;
-      const float4 v = __ldg(reinterpret_cast<const float4*>(w1 + ((int64_t)dj * kFeatC + c0 + c) * kDgT + o));
-      Bs[o][c] = v.x; Bs[o + 1][c] = v.y; Bs[o + 2][c] = v.z; Bs[o + 3][c] = v.w;
-    }
+    stage_w1(cta, w1, dj, [&](int o, int c, float v) { Bs[o][c] = v; });
     __syncthreads();
     float acc[4][4] = {};
 #pragma unroll 8
@@ -972,8 +972,8 @@ k_delta_dgrad(const float* __restrict__ do1, const float* __restrict__ w1, const
 #pragma unroll
         for (int jj = 0; jj < 4; ++jj) acc[ii][jj] = fmaf(av[ii], bv[jj], acc[ii][jj]);
     }
-    const int j = s * jb + dj;
-    const float4 r4 = __ldg(reinterpret_cast<const float4*>(R + (int64_t)j * kFeatC + c0 + tx * 4));
+    const int j = s * cta.jb + dj;
+    const float4 r4 = __ldg(reinterpret_cast<const float4*>(R + (int64_t)j * kFeatC + cta.c0 + tx * 4));
     const float rv[4] = {r4.x, r4.y, r4.z, r4.w};
     float col[4] = {};
 #pragma unroll
@@ -992,14 +992,14 @@ k_delta_dgrad(const float* __restrict__ do1, const float* __restrict__ w1, const
       float v = 0.f;
 #pragma unroll
       for (int y = 0; y < 16; ++y) v += red[y][tid];
-      part_r[(((int64_t)p * nit + itile) * Wf + j) * kFeatC + c0 + tid] = -v;
+      cta.part_r_at(part_r, Wf, j)[tid] = -v;
     }
   }
 #pragma unroll
   for (int ii = 0; ii < 4; ++ii) {
-    const int i = i0 + ty * 4 + ii;
+    const int i = cta.i0 + ty * 4 + ii;
     if (i < Wf)
-      *reinterpret_cast<float4*>(part_l + (((int64_t)p * nb + jb) * Wf + i) * kFeatC + c0 + tx * 4) =
+      *reinterpret_cast<float4*>(cta.part_l_at(part_l, nb, Wf, i) + tx * 4) =
           make_float4(accl[ii][0], accl[ii][1], accl[ii][2], accl[ii][3]);
   }
 }
@@ -1024,33 +1024,20 @@ k_delta_dgrad_tc(const float* __restrict__ do1, const float* __restrict__ w1, co
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t = lane & 3;
   const int wm = (warp >> 2) * 32, wn = (warp & 3) * 16;
-  const int c0 = blockIdx.x * kDgT, itile = blockIdx.y, i0 = itile * kDgT;
-  const int jb = blockIdx.z % nb, p = blockIdx.z / nb;
-  const int nit = gridDim.y;
-  for (int f = tid; f < kDgT * kDgT / 4; f += 256) {
-    const int r = f % kDgT, o = (f / kDgT) * 4, i = i0 + r;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (i < Wf) {
-      const int ho = i / s, dh = i - ho * s;
-      v = __ldg(reinterpret_cast<const float4*>(do1 + ((((int64_t)p * nho + ho) * nb + jb) * s + dh) * kDgT + o));
-    }
-    split_tf32(v.x, Ah[o][r], Al[o][r]);
-    split_tf32(v.y, Ah[o + 1][r], Al[o + 1][r]);
-    split_tf32(v.z, Ah[o + 2][r], Al[o + 2][r]);
-    split_tf32(v.w, Ah[o + 3][r], Al[o + 3][r]);
-  }
-  const float* L = fv + (int64_t)left[p] * Wf * kFeatC;
-  const float* R = fv + (int64_t)right[p] * Wf * kFeatC;
+  const DeltaDgradCta cta(nb);
+  stage_do1(cta, do1, Wf, s, nb, nho, [&](int o, int r, float v) { split_tf32(v, Ah[o][r], Al[o][r]); });
+  const float* L = cta.volume(fv, left, Wf);
+  const float* R = cta.volume(fv, right, Wf);
   // fragment element (mi, ni, r): row i0 + wm + 16 mi + g + 8 (r / 2), channel c0 + wn + 8 ni + 2 t + r % 2
   float lv[2][2][4], accl[2][2][4];
 #pragma unroll
   for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
     for (int h8 = 0; h8 < 2; ++h8) {
-      const int i = i0 + wm + mi * 16 + g + h8 * 8;
+      const int i = cta.i0 + wm + mi * 16 + g + h8 * 8;
 #pragma unroll
       for (int ni = 0; ni < 2; ++ni) {
-        const float2 v = i < Wf ? __ldg(reinterpret_cast<const float2*>(L + (int64_t)i * kFeatC + c0 + wn + ni * 8 + 2 * t))
+        const float2 v = i < Wf ? __ldg(reinterpret_cast<const float2*>(L + (int64_t)i * kFeatC + cta.c0 + wn + ni * 8 + 2 * t))
                                 : make_float2(0.f, 0.f);
         lv[mi][ni][2 * h8] = v.x;
         lv[mi][ni][2 * h8 + 1] = v.y;
@@ -1059,23 +1046,16 @@ k_delta_dgrad_tc(const float* __restrict__ do1, const float* __restrict__ w1, co
       }
     }
   for (int dj = 0; dj < s; ++dj) {
-    for (int f = tid; f < kDgT * kDgT / 4; f += 256) {
-      const int c = f % kDgT, o = (f / kDgT) * 4;
-      const float4 v = __ldg(reinterpret_cast<const float4*>(w1 + ((int64_t)dj * kFeatC + c0 + c) * kDgT + o));
-      split_tf32(v.x, Bh[o][c], Bl[o][c]);
-      split_tf32(v.y, Bh[o + 1][c], Bl[o + 1][c]);
-      split_tf32(v.z, Bh[o + 2][c], Bl[o + 2][c]);
-      split_tf32(v.w, Bh[o + 3][c], Bl[o + 3][c]);
-    }
+    stage_w1(cta, w1, dj, [&](int o, int c, float v) { split_tf32(v, Bh[o][c], Bl[o][c]); });
     __syncthreads();
     float acc[2][2][4] = {};
 #pragma unroll
     for (int k = 0; k < kDgT; k += 16) add_tile(acc, Ah, Al, Bh, Bl, k, wm, wn, g, t);
-    const int j = s * jb + dj;
+    const int j = s * cta.jb + dj;
     float rv[2][2], col[2][2] = {};
 #pragma unroll
     for (int ni = 0; ni < 2; ++ni) {
-      const float2 v = __ldg(reinterpret_cast<const float2*>(R + (int64_t)j * kFeatC + c0 + wn + ni * 8 + 2 * t));
+      const float2 v = __ldg(reinterpret_cast<const float2*>(R + (int64_t)j * kFeatC + cta.c0 + wn + ni * 8 + 2 * t));
       rv[ni][0] = v.x;
       rv[ni][1] = v.y;
     }
@@ -1102,17 +1082,17 @@ k_delta_dgrad_tc(const float* __restrict__ do1, const float* __restrict__ w1, co
         if (g == 0) red[wm / 32][wn + ni * 8 + 2 * t + b] = v;
       }
     __syncthreads();
-    if (tid < kDgT) part_r[(((int64_t)p * nit + itile) * Wf + j) * kFeatC + c0 + tid] = -(red[0][tid] + red[1][tid]);
+    if (tid < kDgT) cta.part_r_at(part_r, Wf, j)[tid] = -(red[0][tid] + red[1][tid]);
   }
 #pragma unroll
   for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
     for (int h8 = 0; h8 < 2; ++h8) {
-      const int i = i0 + wm + mi * 16 + g + h8 * 8;
+      const int i = cta.i0 + wm + mi * 16 + g + h8 * 8;
       if (i >= Wf) continue;
 #pragma unroll
       for (int ni = 0; ni < 2; ++ni)
-        *reinterpret_cast<float2*>(part_l + (((int64_t)p * nb + jb) * Wf + i) * kFeatC + c0 + wn + ni * 8 + 2 * t) =
+        *reinterpret_cast<float2*>(cta.part_l_at(part_l, nb, Wf, i) + wn + ni * 8 + 2 * t) =
             make_float2(accl[mi][ni][2 * h8], accl[mi][ni][2 * h8 + 1]);
     }
 }
@@ -1148,10 +1128,7 @@ int net_max_pairs(const ovn_handle* h) {
   return (int)(by_rows < by_z ? by_rows : by_z);
 }
 
-// [K][N] size of leg layer l's kernel
-static int64_t leg_kernel_size(const ConvSpec& L) { return (int64_t)L.kh * L.kw * L.cin * L.cout; }
-
-// The whole-network buffers of an np-pair batch; the leg gradients and accumulators on first use
+// The whole-network buffers of an np-pair batch
 static int net_alloc(ovn_handle* h, int np) {
   TrainState& t = *h->train;
   const int64_t n2 = 2 * (int64_t)np, Wf = h->cfg.leg_output_width, vol = Wf * kFeatC;
@@ -1164,8 +1141,8 @@ static int net_alloc(ovn_handle* h, int np) {
     acts += a;
     if (a > max_act) max_act = a;
     if (l > 0 && (int64_t)L.h_in * L.w_in * L.cin > max_act) max_act = (int64_t)L.h_in * L.w_in * L.cin;
-    if (leg_kernel_size(L) > max_w) max_w = leg_kernel_size(L);
-    const int64_t g = ((int64_t)L.kh * L.kw * L.cin + 1) * L.cout;
+    const int64_t w = h->params.n_kernel[l], g = w + L.cout;
+    if (w > max_w) max_w = w;
     if (g > max_part) max_part = g;
   }
   int rc;
@@ -1177,32 +1154,13 @@ static int net_alloc(ovn_handle* h, int np) {
   if ((rc = t.dcorr.ensure(h, (size_t)(np * Wf) * sizeof(float))) != OVN_OK) return rc;
   if ((rc = t.pair_rows.ensure(h, (size_t)n2 * sizeof(int32_t))) != OVN_OK) return rc;
   if ((rc = t.wt.ensure(h, (size_t)max_w * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t.part.ensure(h, (size_t)kMaxSplit * max_part * sizeof(float))) != OVN_OK) return rc;
-  return leg_train_alloc(h);
-}
-
-// The leg gradients and accumulators, on first use (ovn_net_gradients, or ovn_adagrad_step_sum on a rank
-// that has not computed a gradient yet)
-int leg_train_alloc(ovn_handle* h) {
-  TrainState& t = *h->train;
-  if (t.leg_grad) return OVN_OK;
-  int64_t total = 0;
-  for (int l = 0; l < h->n_leg; ++l) {
-    t.leg_off[l] = total;
-    total += leg_kernel_size(h->leg[l]) + h->leg[l].cout;
-  }
-  int rc;
-  if ((rc = t.leg_accum.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
-  OVN_CUDA(h, cudaMemset(t.leg_accum, 0, (size_t)total * sizeof(float)));
-  if ((rc = t.leg_grad.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
-  t.n_leg_param = total;
-  return OVN_OK;
+  return t.part.ensure(h, (size_t)kMaxSplit * max_part * sizeof(float));
 }
 
 // Forward of the leg on the 2 np gathered images (the launches of leg_forward_fp32, every output kept), both
-// heads, the losses, and the backward of the whole network.  Head gradients land in train->grad, leg gradients
-// in train->leg_grad, the losses in train->loss; d_fv_grad (may be null) receives dL/d(volumes) before
-// s_conv10's ReLU mask, [2][np][Wf][128].
+// heads, the losses, and the backward of the whole network.  The gradients of every layer land in train->grad,
+// the losses in train->loss; d_fv_grad (may be null) receives dL/d(volumes) before s_conv10's ReLU mask,
+// [2][np][Wf][128].
 int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left, const int32_t* right, int np,
                        const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
                        float* d_fv_grad, cudaStream_t s) {
@@ -1285,10 +1243,10 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
     const float* X = l ? act[l - 1] : t.images;
     const int Kc = L.kh * L.kw * L.cin;
     ConvWgradOperand a{X, L.h_in, L.w_in, L.cin, L.kw, L.sh, L.sw, L.h_out, L.w_out, Kc};
-    rc = wgrad_gemm(h, a, dy, Kc, L.cout, n2 * L.h_out * L.w_out, t.leg_grad + t.leg_off[l], s);
+    rc = wgrad_gemm(h, a, dy, Kc, L.cout, n2 * L.h_out * L.w_out, t.grad + h->params.off[l], s);
     if (rc != OVN_OK) return rc;
     if (l == 0) break;
-    k_swap_io<<<blocks_for(leg_kernel_size(L)), 256, 0, s>>>(h->d_w[l], t.wt, L.kh * L.kw, L.cin, L.cout);
+    k_swap_io<<<blocks_for(h->params.n_kernel[l]), 256, 0, s>>>(h->d_w[l], t.wt, L.kh * L.kw, L.cin, L.cout);
     OVN_LAUNCH_CHECK(h);
     BOperand b{t.wt, nullptr, nullptr, 0, 0};
     const int64_t rows_in = (int64_t)L.h_in * L.w_in, K = L.kh * L.kw * L.cout;
@@ -1316,46 +1274,7 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
   return OVN_OK;
 }
 
-int net_adagrad_fp32(ovn_handle* h, float lr, cudaStream_t s) {
-  int rc = head_adagrad_fp32(h, lr, s);
-  if (rc != OVN_OK) return rc;
-  TrainState& t = *h->train;
-  for (int l = 0; l < h->n_leg; ++l) {
-    const int64_t nk = leg_kernel_size(h->leg[l]), N = h->leg[l].cout;
-    float* g = t.leg_grad + t.leg_off[l];
-    float* a = t.leg_accum + t.leg_off[l];
-    k_adagrad<<<blocks_for(nk), 256, 0, s>>>(h->d_w[l], g, a, nk, lr);
-    OVN_LAUNCH_CHECK(h);
-    k_adagrad<<<blocks_for(N), 256, 0, s>>>(h->d_b[l], g + nk, a + nk, N, lr);
-    OVN_LAUNCH_CHECK(h);
-  }
-  return OVN_OK;
-}
-
 // ---- data-parallel training -------------------------------------------------------------------------
-// The flat gradient vector is train->grad (the heads) followed by train->leg_grad (the leg): each is already
-// [K + 1][N] per layer, so a copy is one or two memcpys, and the accumulators have the same layout.
-
-int64_t train_gradient_size(const ovn_handle* h, bool whole_network) {
-  int64_t n = 0;
-  for (int l = 0; l < 4; ++l) {
-    int K, N;
-    head_dims(h, l, &K, &N);
-    n += (int64_t)(K + 1) * N;
-  }
-  if (whole_network)
-    for (int l = 0; l < h->n_leg; ++l) n += leg_kernel_size(h->leg[l]) + h->leg[l].cout;
-  return n;
-}
-
-int copy_gradients_fp32(ovn_handle* h, bool whole_network, float* d_out, cudaStream_t s) {
-  const TrainState& t = *h->train;
-  OVN_CUDA(h, cudaMemcpyAsync(d_out, t.grad, (size_t)t.n_param * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  if (whole_network)
-    OVN_CUDA(h, cudaMemcpyAsync(d_out + t.n_param, t.leg_grad, (size_t)t.n_leg_param * sizeof(float),
-                                cudaMemcpyDeviceToDevice, s));
-  return OVN_OK;
-}
 
 // The volumes of the last ovn_net_gradients batch, [2][np][Wf][128] (LEFT, then RIGHT): the leg's output as that
 // call computed it, at its training precision (the backward reads every activation, and none is overwritten)
@@ -1383,10 +1302,9 @@ struct SumArgs {
   float weight[kMaxSumParts];
 };
 
-// g = w0 p0 + w1 p1 + ... in part order, every product and sum rounded on its own, then k_adagrad's update as
-// it compiles (its a + g * g contracts to one FFMA; sqrt and the division are IEEE): one part of weight 1 gives
-// k_adagrad's result bit for bit.  The table is read through the constant bank (__grid_constant__), so the
-// segment search does not copy it to local memory.
+// g = w0 p0 + w1 p1 + ... in part order, every product and sum rounded on its own, then Adagrad as Keras 2.1.5
+// does it: a += g^2 as one FMA;  w -= lr * g / (sqrt(a) + 1e-7) with IEEE sqrt and division.  The table is read
+// through the constant bank (__grid_constant__), so the segment search does not copy it to local memory.
 __global__ void k_adagrad_sum(const float* __restrict__ parts, const __grid_constant__ SumArgs p, float lr) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= p.n) return;
@@ -1407,26 +1325,18 @@ __global__ void k_adagrad_sum(const float* __restrict__ parts, const __grid_cons
 
 int adagrad_sum_fp32(ovn_handle* h, bool whole_network, const float* d_parts, int n_parts, const float* h_weights,
                      float lr, cudaStream_t s) {
-  TrainState& t = *h->train;
+  const ParamLayout& L = h->params;
+  float* accum = h->train->accum;
   SumArgs p = {};
-  int k = 0;
-  for (int l = 0; l < 4; ++l) {
-    int K, N;
-    head_dims(h, l, &K, &N);
-    const int64_t o = t.off[l], nk = (int64_t)K * N;
-    p.seg[k++] = {o, h->d_w[kMaxLegLayers + l], t.accum + o};
-    p.seg[k++] = {o + nk, h->d_b[kMaxLegLayers + l], t.accum + o + nk};
+  const int n_layers = whole_network ? 4 + h->n_leg : 4;
+  for (int i = 0; i < n_layers; ++i) {
+    const int slot = flat_slot(i);
+    const int64_t o = L.off[slot], ob = o + L.n_kernel[slot];
+    p.seg[2 * i] = {o, h->d_w[slot], accum + o};
+    p.seg[2 * i + 1] = {ob, h->d_b[slot], accum + ob};
   }
-  p.n = t.n_param;
-  if (whole_network) {
-    for (int l = 0; l < h->n_leg; ++l) {
-      const int64_t o = t.leg_off[l], nk = leg_kernel_size(h->leg[l]);
-      p.seg[k++] = {p.n + o, h->d_w[l], t.leg_accum + o};
-      p.seg[k++] = {p.n + o + nk, h->d_b[l], t.leg_accum + o + nk};
-    }
-    p.n += t.n_leg_param;
-  }
-  p.n_seg = k;
+  p.n_seg = 2 * n_layers;
+  p.n = whole_network ? L.n_total : L.n_head;
   for (int r = 0; r < n_parts; ++r) {
     if (h_weights[r] == 0.f) continue;
     p.part[p.n_parts] = r;

@@ -74,23 +74,31 @@ def test_gradient_size():
 def test_one_part_of_weight_one_is_todays_step(kind):
   """Three steps: copy_gradients + adagrad_step_sum([g], [1]) against ovn_head_adagrad_step /
   ovn_net_adagrad_step, bit for bit after every step (each step's update divides by sqrt of the accumulator, so
-  equal weights after three different gradients need equal accumulators)."""
+  equal weights after three different gradients need equal accumulators).  The one-process step is one launch, and
+  matches the NumPy float32 oracle on the gradients copy_gradients returns."""
   w, x, _, _, _ = _setup(True)
   whole = kind == 'whole'
   engs = [_engine(w), _engine(w)]
   xs = torch.from_numpy(x).to(engs[0].device)
+  ref_w = _flatten(engs[0], engs[0].get_weights(), whole)
+  ref_a = np.zeros(ref_w.size, np.float32)
   for step in range(3):
     lr = 1e-3 * (step + 1)
     for k, eng in enumerate(engs):
       _gradients(eng, kind, xs, step, step + 4)
-      if k == 0 and whole:
-        eng.net_adagrad_step(lr)
-      elif k == 0:
-        eng.adagrad_step(lr)
+      g = eng.copy_gradients(whole)
+      if k == 0:
+        ref_w, ref_a = adagrad_sum_oracle(ref_w, ref_a, g.cpu().numpy()[None], [1.0], lr)
+        n0 = eng.launch_count()
+        if whole:
+          eng.net_adagrad_step(lr)
+        else:
+          eng.adagrad_step(lr)
+        assert eng.launch_count() == n0 + 1
       else:
-        g = eng.copy_gradients(whole)
         eng.adagrad_step_sum(g[None], [1.0], lr, whole)
     a, b = engs[0].get_weights(), engs[1].get_weights()
+    assert np.array_equal(bits(_flatten(engs[0], a, whole)), bits(ref_w)), step
     for name in a:
       for i in range(2):
         assert np.array_equal(bits(a[name][i]), bits(b[name][i])), (step, name, i)
@@ -131,7 +139,7 @@ def adagrad_sum_oracle(w, a, parts, weights, lr):
 
 @pytest.mark.parametrize('kind', KINDS)
 def test_weighted_sum_of_three_parts_matches_numpy_oracle(kind):
-  """On a handle that never computed a gradient (the leg state is allocated by the call): two steps with three
+  """On a handle that never computed a gradient (the training state is allocated by the call): two steps with three
   random parts, the middle one of weight 0, bit for bit against the oracle; the frozen leg is untouched."""
   w, _, _, _, _ = _setup(True)
   whole = kind == 'whole'
