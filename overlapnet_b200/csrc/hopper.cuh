@@ -88,6 +88,13 @@ __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" :: "r"(id), "r"(count) : "memory");
 }
 
+// ---- per-warpgroup register budget: every warp of a warpgroup executes the same call.  A producer warpgroup
+// gives registers back (dec) so that the consumer warpgroups can take them (inc blocks until they are free).
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(N)); }
+
 // ---- bulk async copy global -> shared, completes on an mbarrier (bytes and addresses multiples of 16)
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"

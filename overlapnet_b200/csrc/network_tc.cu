@@ -230,10 +230,11 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 // k_delta_conv1_wgmma -- DeltaLayer + c_conv1 without the delta tensor (83 % of the FLOPs of a pair).
 //   GEMM per work unit (pair, jb):  o1[i, o] = sum_{dj < 15, c < 128} |L[i, c] - R[15 jb + dj, c]| W1[dj, c, o] - mu_o1[o]
 //   M = 360 LEFT rows (6 row tiles of 64, rows past 360 masked), N = 64, K = 1920 (60 W1 slices of 32 channels).
-// Warp specialisation: warp 12 is the producer (one lane issues bulk copies): the LEFT volume of the current
-// pair (90 KB, once per pair), the 15 RIGHT rows of a unit (double-buffered) and W1 in groups of 5 slices
-// (20 KB) through a 4-deep ring, each buffer guarded by a full / empty mbarrier pair.  Warpgroups 0-2 are
-// the consumers: warpgroup w owns row tiles w and w + 3 (2 x 32 fp32 accumulators per thread).  The A
+// Warp specialisation: warpgroup 3 is the producer (one lane issues bulk copies; the warpgroup hands its registers
+// to the consumers with setmaxnreg): the LEFT volume of the current pair (90 KB, once per pair), the 15 RIGHT rows
+// of a unit (double-buffered) and W1 in groups of 5 slices (20 KB) through a 4-deep ring, each buffer guarded by a
+// full / empty mbarrier pair.  Warpgroups 0-2 are the consumers (160 registers): warpgroup w owns row tiles w and
+// w + 3 (2 x 32 fp32 accumulators per thread) and commits one group of 2 wgmma per K16 step.  The A
 // operand |l - r| is synthesised in registers from the LEFT rows (kept in registers for a 32-channel chunk)
 // and the broadcast RIGHT row, and multiplied by wgmma in register-A mode against the W1 slice in shared
 // memory: the 66 MB delta tensor of a pair is never written.  A group of 5 slices never straddles a 32-channel
@@ -243,7 +244,8 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 // Persistent: each CTA takes a contiguous range of the n_pairs * 24 units.
 // ------------------------------------------------------------------------------------------------
 constexpr int K4_WG = 3;                               // consumer warpgroups
-constexpr int K4_THREADS = K4_WG * 128 + 32;           // + the producer warp
+constexpr int K4_THREADS = (K4_WG + 1) * 128;          // + the producer warpgroup
+constexpr uint32_t K4_REG_PRODUCER = 32, K4_REG_CONSUMER = 160;   // per thread: 3 x 160 + 32 = 512 per SM quarter
 constexpr int K4_GROUP = 5;                            // W1 slices per bulk copy (divides the 15 dj of a chunk)
 constexpr int K4_NGROUPS = K4_STEPS / K4_GROUP;        // 12 per unit
 static_assert(S15 % K4_GROUP == 0, "a W1 group within one 32-channel chunk");
@@ -286,9 +288,10 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
   }
   __syncthreads();
 
-  if (warp == K4_WG * 4) {
+  if (warp >= K4_WG * 4) {
     // ===================== producer ==========================================================
-    if (lane == 0) {
+    setmaxnreg_dec<K4_REG_PRODUCER>();
+    if (warp == K4_WG * 4 && lane == 0) {
       uint32_t pi = 0, gi = 0, ui = 0;
       for (int u = u_begin; u < u_end; ++u, ++ui) {
         const int p = u / NB, jb = u - p * NB;
@@ -308,6 +311,7 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
     }
   } else {
     // ===================== consumers ==========================================================
+    setmaxnreg_inc<K4_REG_CONSUMER>();
     const int wg = warp >> 2, wi = warp & 3, g = lane >> 2, t = lane & 3;
     int rows[2][2];                         // [tile][a / b]: this thread's fragment rows
 #pragma unroll
@@ -358,33 +362,33 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
         const __half* rp[2] = {rw + ((cc ^ par) << 5), rw + ((cc ^ par ^ 1) << 5)};
         uint4 rv = *reinterpret_cast<const uint4*>(rp[0]);
         PIPE_WAIT(S.w1.wait(gi), kErrDeltaW1Consumer);
+        // One commit group per K16 step, waited for with wait_group 1: a warpgroup forms step kk's A while its
+        // previous step's MMAs run.  A[.][kk] is rewritten only after the group that last read it (two groups back)
+        // has retired.  Every group is drained at the end of the W1 group: ptxas keeps register-A wgmmas pipelined
+        // only when no group is in flight across the loop's back edge or a barrier wait.
+        uint32_t A[2][2][4];                  // [tile][kk]
 #pragma unroll
-        for (int sl = 0; sl < K4_GROUP; ++sl) {
-          uint32_t A[2][2][4];                // [tile][kk]
+        for (int sl = 0; sl < K4_GROUP; ++sl)
 #pragma unroll
-          for (int tt = 0; tt < 2; ++tt) {
-            A[tt][0][0] = absdiff_h2(Lr[tt][0][0], rv.x);
-            A[tt][0][1] = absdiff_h2(Lr[tt][1][0], rv.x);
-            A[tt][0][2] = absdiff_h2(Lr[tt][0][1], rv.y);
-            A[tt][0][3] = absdiff_h2(Lr[tt][1][1], rv.y);
-            A[tt][1][0] = absdiff_h2(Lr[tt][0][2], rv.z);
-            A[tt][1][1] = absdiff_h2(Lr[tt][1][2], rv.z);
-            A[tt][1][2] = absdiff_h2(Lr[tt][0][3], rv.w);
-            A[tt][1][3] = absdiff_h2(Lr[tt][1][3], rv.w);
-          }
-          wgmma_fence();
+          for (int kk = 0; kk < 2; ++kk) {
+            const uint32_t r0 = kk ? rv.z : rv.x, r1 = kk ? rv.w : rv.y;
 #pragma unroll
-          for (int kk = 0; kk < 2; ++kk)
+            for (int tt = 0; tt < 2; ++tt) {
+              A[tt][kk][0] = absdiff_h2(Lr[tt][0][2 * kk], r0);
+              A[tt][kk][1] = absdiff_h2(Lr[tt][1][2 * kk], r0);
+              A[tt][kk][2] = absdiff_h2(Lr[tt][0][2 * kk + 1], r1);
+              A[tt][kk][3] = absdiff_h2(Lr[tt][1][2 * kk + 1], r1);
+            }
+            wgmma_fence();
 #pragma unroll
             for (int tt = 0; tt < 2; ++tt)
               wgmma_m64n64k16_rs(acc[tt], A[tt][kk], bdesc + ((sl * K4_BSLICE + kk * 2048) >> 4));
-          wgmma_commit();
-          // the next RIGHT row loads while the MMAs run.  They are waited for at once and the three warpgroups supply
-          // the overlap: a second A register set for wait_group 1 spills at the 128-register cap of 13 warps, and
-          // the spill-light per-K16 form of it was slower (DESIGN §4)
-          if (sl + 1 < K4_GROUP) rv = *reinterpret_cast<const uint4*>(rp[(sl + 1) & 1] + (sl + 1) * K4_PITCH);
-          wgmma_wait<0>();
-        }
+            wgmma_commit();
+            // the next RIGHT row loads while the MMAs run
+            if (kk == 1 && sl + 1 < K4_GROUP) rv = *reinterpret_cast<const uint4*>(rp[(sl + 1) & 1] + (sl + 1) * K4_PITCH);
+            wgmma_wait<1>();
+          }
+        wgmma_wait<0>();
         S.w1.release(gi);
       }
       S.right.release(ui);
