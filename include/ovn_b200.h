@@ -297,6 +297,20 @@ int ovn_train_gradient_size(ovn_handle* h, int32_t whole_network, int64_t* n);
 int ovn_copy_gradients(ovn_handle* h, int32_t whole_network, float* d_out, void* stream);
 int ovn_adagrad_step_sum(ovn_handle* h, int32_t whole_network, const float* d_parts, int32_t n_parts,
                          const float* h_weights, float learning_rate, void* stream);
+/* ---- the training state, for checkpoints that resume a run (overlapnet_b200/training.py, DESIGN.md section 6) --
+ * The Adagrad accumulators as one flat float32 vector in the layout of ovn_copy_gradients:
+ * ovn_train_gradient_size(h, whole_network) floats, the heads' prefix (whole_network = 0) or every layer.
+ *   ovn_copy_train_state: d_out[n] = the accumulators, asynchronous on `stream`.  A handle that never trained
+ *                    returns zeros (what its first Adagrad step starts from).
+ *   ovn_set_train_state: the accumulators = d_in[n], asynchronous on `stream`; allocates the training state when
+ *                    the handle has none.  whole_network = 0 writes the heads' prefix only and leaves the leg's
+ *                    accumulators as they are.  The values are not checked: a negative or non-finite one makes the
+ *                    next Adagrad steps non-finite.
+ * ovn_finalize_weights resets the accumulators to zero, so a resumed run sets its weights first (ovn_set_weights,
+ * ovn_finalize_weights), then its state.  fp32 handles (OVN_ERR_BAD_CONFIG otherwise); OVN_ERR_INVALID_ARG for a
+ * NULL pointer or when the weights are not finalised. */
+int ovn_copy_train_state(ovn_handle* h, int32_t whole_network, float* d_out, void* stream);
+int ovn_set_train_state(ovn_handle* h, int32_t whole_network, const float* d_in, void* stream);
 /* ---- yaw augmentation of training images (DESIGN.md section 7) ------------------------------------
  * The reference's rotate_training_data rolls the RIGHT image by randint(0, width) columns but leaves its yaw
  * label where it was, and rolls the normal channels without rotating the vectors

@@ -24,7 +24,7 @@ SYMBOLS = [
     'ovn_head_gradients', 'ovn_head_adagrad_step', 'ovn_get_weights', 'ovn_get_gradients',
     'ovn_net_gradients', 'ovn_net_adagrad_step', 'ovn_gather_images',
     'ovn_train_gradient_size', 'ovn_copy_gradients', 'ovn_adagrad_step_sum', 'ovn_set_train_precision',
-    'ovn_copy_net_volumes',
+    'ovn_copy_net_volumes', 'ovn_copy_train_state', 'ovn_set_train_state',
 ]
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
 
@@ -110,6 +110,8 @@ def lib():
   L.ovn_adagrad_step_sum.argtypes = [vp, i32, vp, i32, vp, f32, vp]
   L.ovn_set_train_precision.argtypes = [vp, i32]
   L.ovn_copy_net_volumes.argtypes = [vp, vp, vp]
+  L.ovn_copy_train_state.argtypes = [vp, i32, vp, vp]
+  L.ovn_set_train_state.argtypes = [vp, i32, vp, vp]
   L.ovn_get_weights.argtypes = [vp, C.c_char_p, vp, vp]
   L.ovn_get_gradients.argtypes = [vp, C.c_char_p, vp, vp]
   L.ovn_encode_clouds_host.argtypes = [vp, vp, vp, i32, vp]

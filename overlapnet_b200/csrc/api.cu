@@ -830,6 +830,41 @@ int ovn_copy_net_volumes(ovn_handle* h, float* d_out, void* stream) {
   return copy_net_volumes_fp32(h, d_out, (cudaStream_t)stream);
 }
 
+// ovn_copy_train_state / ovn_set_train_state: the Adagrad accumulators, in the layout of ovn_copy_gradients
+static int train_state_call(ovn_handle* h, const char* fn, const void* ptr) {
+  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "%s: %s", fn, h->net_error.c_str());
+  if (h->cfg.precision != OVN_PREC_FP32)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "%s: training needs a precision fp32 handle", fn);
+  if (!ptr) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: NULL pointer", fn);
+  if (!h->weights_ready) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: weights not finalised", fn);
+  return OVN_OK;
+}
+
+int ovn_copy_train_state(ovn_handle* h, int32_t whole_network, float* d_out, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  int rc = train_state_call(h, "ovn_copy_train_state", d_out);
+  if (rc != OVN_OK) return rc;
+  const size_t bytes = (size_t)(whole_network ? h->params.n_total : h->params.n_head) * sizeof(float);
+  if (!h->train) {                         // never trained: the accumulators Adagrad would start from
+    OVN_CUDA(h, cudaMemsetAsync(d_out, 0, bytes, (cudaStream_t)stream));
+    return OVN_OK;
+  }
+  OVN_CUDA(h, cudaMemcpyAsync(d_out, h->train->accum, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return OVN_OK;
+}
+
+int ovn_set_train_state(ovn_handle* h, int32_t whole_network, const float* d_in, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  int rc = train_state_call(h, "ovn_set_train_state", d_in);
+  if (rc != OVN_OK) return rc;
+  if (!h->train && (rc = train_alloc(h)) != OVN_OK) return rc;
+  const size_t bytes = (size_t)(whole_network ? h->params.n_total : h->params.n_head) * sizeof(float);
+  OVN_CUDA(h, cudaMemcpyAsync(h->train->accum, d_in, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return OVN_OK;
+}
+
 int ovn_adagrad_step_sum(ovn_handle* h, int32_t whole_network, const float* d_parts, int32_t n_parts,
                          const float* h_weights, float learning_rate, void* stream) {
   if (!h) return OVN_ERR_INVALID_ARG;

@@ -465,6 +465,26 @@ class Engine:
                                              w.ctypes.data_as(C.c_void_p), float(lr), self._stream()),
           'ovn_adagrad_step_sum')
 
+  def train_state(self, whole_network=False, out=None):
+    """ovn_copy_train_state: the Adagrad accumulators as one flat float32 cuda tensor [gradient_size] in the
+    layout of copy_gradients (written into ``out`` when given); zeros on a handle that never trained."""
+    n = self.gradient_size(whole_network)
+    if out is None:
+      out = torch.empty((n,), dtype=torch.float32, device=self.device)
+    assert out.numel() == n and out.dtype == torch.float32 and out.is_contiguous() and out.device == self.device
+    check(self._h, lib().ovn_copy_train_state(self._h, int(bool(whole_network)), _ptr(out), self._stream()),
+          'ovn_copy_train_state')
+    return out
+
+  def set_train_state(self, vec, whole_network=False):
+    """ovn_set_train_state: the Adagrad accumulators from ``vec`` [gradient_size] (float32, a NumPy array or a
+    tensor); without ``whole_network`` only the head layers' part.  load_weights resets them, so call it after."""
+    n = self.gradient_size(whole_network)
+    v = torch.as_tensor(vec).to(device=self.device, dtype=torch.float32).contiguous().reshape(-1)
+    assert v.numel() == n
+    check(self._h, lib().ovn_set_train_state(self._h, int(bool(whole_network)), _ptr(v), self._stream()),
+          'ovn_set_train_state')
+
   @property
   def leg_layers(self):
     """Names of the leg layers of this handle's config, input to output."""

@@ -29,10 +29,21 @@ Both flows train data-parallel over the GPUs of a node (overlapnet_b200.data_par
 
 ``batch_size`` stays the global batch; each rank trains on a contiguous share of every batch, and the ranks'
 gradients are all-gathered and summed in rank order on the device, so every rank keeps the same weights.
+
+``checkpoint: True`` (both legsTypes, default False) writes ``<experiments_path>/<testname>/checkpoint.npz`` after
+every epoch, atomically: the weights, the Adagrad accumulators (Engine.train_state), NumPy's random state, the
+training pairs in the run's order, the history so far and a fingerprint of the config keys that fix the
+trajectory.  ``resume: True`` (implies ``checkpoint``) continues such a run from its last completed epoch up to
+``no_epochs``, with the same learning-rate schedule, batch orders and yaw shifts, so that its weights and history
+are those of the uninterrupted run bit for bit (DESIGN.md section 6).  It refuses a checkpoint whose fingerprint,
+layers or state do not fit the config; ``no_epochs``, ``no_test_pairs``, the validation files,
+``training_precision`` and the world size may change, and ``pretrained_weightsfilename`` is ignored.
 """
+import json
 import logging
 import os
 import sys
+import time
 
 import numpy as np
 import torch
@@ -46,6 +57,10 @@ from .config import load_config
 logger = logging.getLogger('overlapnet_b200.training')
 
 OVERLAP_THRESHOLDS = (0.3, 0.4, 0.5, 0.6, 0.7, 0.8, 0.9)          # training.py:398
+CUE_DEFAULTS = (('use_depth', True), ('use_normals', True), ('use_class_probabilities', False),
+                ('use_class_probabilities_pca', False), ('use_intensity', False))              # training.py:137-160
+CHECKPOINT = 'checkpoint.npz'
+CHECKPOINT_VERSION = 1
 
 
 def learning_rate(epoch, initial_lr=1e-3, alpha=0.99):
@@ -144,6 +159,133 @@ def save_weights(path, weights):
     _weights.save_npz(f, weights)
 
 
+def _plain(value):
+  """``value`` as JSON reads it back (tuples become lists), so that a config and a stored fingerprint compare."""
+  return json.loads(json.dumps(value, sort_keys=True))
+
+
+def trajectory_fingerprint(config):
+  """The config values that fix a run's trajectory -- its draws, batches, steps and learning rates -- as the loop
+  reads them.  A checkpoint is resumed only under the same values."""
+  fp = {'model': config['model']}
+  fp.update((key, config.get(key, default)) for key, default in CUE_DEFAULTS)
+  fp.update(batch_size=int(config['batch_size']), no_batches_in_epoch=int(config['no_batches_in_epoch']),
+            learning_rate=float(config['learning_rate']), lr_alpha=float(config.get('lr_alpha', 0.99)),
+            min_overlap_for_angle=float(config.get('min_overlap_for_angle', 0.7)),
+            yaw_augmentation=bool(config.get('yaw_augmentation', False)),
+            data_root_folder=config.get('data_root_folder', ''))
+  if 'training_seqs' in config:                                    # npz_files: the training files
+    fp.update(training_seqs=str(config['training_seqs']), traindata_npzfile=None)
+  else:
+    fp.update(training_seqs=None, traindata_npzfile=config['traindata_npzfile'])
+  return _plain(fp)
+
+
+def write_checkpoint(path, epochs, weights, accum, pairs, history, fingerprint):
+  """The state after ``epochs`` completed epochs, in an .npz that loads without pickle: a temp file in the same
+  directory, flushed to disk, then renamed over ``path``, so that ``path`` is always a whole checkpoint."""
+  _, keys, pos, has_gauss, cached_gaussian = np.random.get_state()
+  arrays = {'format_version': np.int64(CHECKPOINT_VERSION), 'epochs': np.int64(epochs),
+            'accum': np.asarray(accum, np.float32),
+            'rng_keys': np.asarray(keys, np.uint32), 'rng_pos': np.int64(pos), 'rng_has_gauss': np.int64(has_gauss),
+            'rng_cached_gaussian': np.float64(cached_gaussian),
+            'history': np.str_(json.dumps({k: history[k] for k in ('epoch_loss', 'batch_losses', 'validation')})),
+            'fingerprint': np.str_(json.dumps(fingerprint, sort_keys=True))}
+  for key, values in zip(('f1', 'f2', 'd1', 'd2'), pairs[:4]):
+    arrays[key] = np.asarray(values, np.str_)
+  arrays['overlap'], arrays['orientation'] = np.asarray(pairs[4]), np.asarray(pairs[5])
+  for name, (k, b) in weights.items():                             # the keys of weights.save_npz
+    arrays[name + '/kernel'] = np.asarray(k, np.float32)
+    arrays[name + '/bias'] = np.asarray(b, np.float32)
+  tmp = path + '.tmp'
+  with open(tmp, 'wb') as f:
+    np.savez(f, **arrays)
+    f.flush()
+    os.fsync(f.fileno())
+  os.replace(tmp, path)
+
+
+def read_checkpoint(path, fingerprint, no_epochs):
+  """The state write_checkpoint stored at ``path``, checked against this run: its format version, the
+  ``fingerprint`` of this config, its epoch count below ``no_epochs`` and its accumulators (finite, >= 0).  Returns
+  a dict (epochs, weights, accum, rng, pairs, history); raises an Exception that names the problem."""
+  try:
+    with np.load(path, allow_pickle=False) as z:
+      ck = {k: z[k] for k in z.files}
+  except Exception as e:
+    raise Exception('resume: cannot read the checkpoint %s: %s' % (path, e)) from e
+  if 'format_version' not in ck or int(ck['format_version']) != CHECKPOINT_VERSION:
+    raise Exception('resume: the checkpoint %s has format version %s; this code reads version %d'
+                    % (path, ck['format_version'] if 'format_version' in ck else 'none', CHECKPOINT_VERSION))
+  required = ('epochs', 'accum', 'rng_keys', 'rng_pos', 'rng_has_gauss', 'rng_cached_gaussian', 'history',
+              'fingerprint', 'f1', 'f2', 'd1', 'd2', 'overlap', 'orientation')
+  missing = [k for k in required if k not in ck]
+  if missing:
+    raise Exception('resume: the checkpoint %s lacks %s' % (path, ', '.join(missing)))
+  saved = json.loads(str(ck['fingerprint']))
+  for key in sorted(set(saved) | set(fingerprint)):
+    a, b = saved.get(key), fingerprint.get(key)
+    if a != b:
+      if key == 'model' and isinstance(a, dict) and isinstance(b, dict):
+        key = 'model.' + next(k for k in sorted(set(a) | set(b)) if a.get(k) != b.get(k))
+      raise Exception('resume: config key %s differs from the run that wrote %s; a resumed run must keep the '
+                      'keys that fix its trajectory' % (key, path))
+  epochs = int(ck['epochs'])
+  if epochs >= no_epochs:
+    raise Exception('resume: the checkpoint %s holds %d completed epochs, no_epochs is %d: nothing to train'
+                    % (path, epochs, no_epochs))
+  accum = ck['accum']
+  if accum.dtype != np.float32 or accum.ndim != 1:
+    raise Exception('resume: the accumulators in %s are %s %s, not a float32 vector' % (path, accum.dtype,
+                                                                                       accum.shape))
+  bad = ~np.isfinite(accum) | (accum < 0)
+  if bad.any():
+    raise Exception('resume: %d Adagrad accumulators in %s are negative or not finite (first at %d)'
+                    % (int(bad.sum()), path, int(np.argmax(bad))))
+  history = json.loads(str(ck['history']))
+  for stats in history['validation']:                              # JSON object keys are strings
+    stats['orientation_rms'] = {float(k): v for k, v in stats['orientation_rms'].items()}
+  names = sorted({k.split('/')[0] for k in ck if '/' in k})
+  return {'epochs': epochs, 'accum': accum, 'history': history,
+          'weights': {n: (ck[n + '/kernel'], ck[n + '/bias']) for n in names},
+          'rng': ('MT19937', ck['rng_keys'], int(ck['rng_pos']), int(ck['rng_has_gauss']),
+                  float(ck['rng_cached_gaussian'])),
+          'pairs': tuple(ck[k].tolist() for k in ('f1', 'f2', 'd1', 'd2')) + (ck['overlap'], ck['orientation'])}
+
+
+def _read_checkpoint_on_rank0(path, fingerprint, no_epochs, dp):
+  """read_checkpoint on rank 0; every rank gets its contents, or raises its refusal."""
+  if dp is None:
+    return read_checkpoint(path, fingerprint, no_epochs)
+  got = None
+  if dp.rank == 0:
+    try:
+      got = read_checkpoint(path, fingerprint, no_epochs)
+    except Exception as e:
+      got = str(e)
+  got = dp.broadcast(got)
+  if isinstance(got, str):
+    raise Exception(got)
+  return got
+
+
+def check_checkpoint_fits(ck, eng, whole_network, path):
+  """Refuse a checkpoint whose layers, shapes or accumulator length differ from the handle's."""
+  have = {n: (np.shape(k), np.shape(b)) for n, (k, b) in eng.get_weights().items()}
+  saved = {n: (np.shape(k), np.shape(b)) for n, (k, b) in ck['weights'].items()}
+  if sorted(have) != sorted(saved):
+    raise Exception('resume: the checkpoint %s has the layers %s; the model has %s' % (path, sorted(saved),
+                                                                                     sorted(have)))
+  for name in sorted(have):
+    if have[name] != saved[name]:
+      raise Exception('resume: layer %s of the checkpoint %s has kernel / bias shapes %s; the model has %s'
+                      % (name, path, saved[name], have[name]))
+  n = eng.gradient_size(whole_network)
+  if ck['accum'].size != n:
+    raise Exception('resume: the checkpoint %s holds %d Adagrad accumulators; this flow trains %d'
+                    % (path, ck['accum'].size, n))
+
+
 class FrozenLeg:
   """The training step of 360OutputkLegsFixed: every distinct scan is encoded once by the frozen leg into a
   feature bank on the GPU; a step trains the overlap head on it."""
@@ -206,7 +348,8 @@ def run(config, device, flow):
   handler = None
   if dp is None or dp.rank == 0:
     os.makedirs(out_dir, exist_ok=True)
-    handler = logging.FileHandler(os.path.join(out_dir, 'training.log'), mode='w')    # training.py:204-208
+    handler = logging.FileHandler(os.path.join(out_dir, 'training.log'),             # training.py:204-208
+                                  mode='a' if config.get('resume', False) else 'w')
     handler.setFormatter(logging.Formatter(fmt='%(asctime)s %(message)s', datefmt='%H:%M:%S'))
     logger.addHandler(handler)
   if logger.level == logging.NOTSET or logger.level > logging.INFO:
@@ -232,10 +375,17 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
   no_test_pairs = int(config['no_test_pairs'])
   min_overlap_for_angle = float(config.get('min_overlap_for_angle', 0.7))
   yaw_augmentation = bool(config.get('yaw_augmentation', False))
+  resume = bool(config.get('resume', False))
+  checkpoint = resume or bool(config.get('checkpoint', False))
+  checkpoint_path = os.path.join(out_dir, CHECKPOINT)
+  fingerprint = trajectory_fingerprint(config) if checkpoint else None
+  resumed = _read_checkpoint_on_rank0(checkpoint_path, fingerprint, no_epochs, dp) if resume else None
 
   train_files, val_files = npz_files(config)
   logger.info('load training data ...')
-  if dp is None:
+  if resumed is not None:                                          # the saved run's pairs, in its order
+    t_f1, t_f2, t_d1, t_d2, t_ov, t_or = resumed['pairs']
+  elif dp is None:
     t_f1, t_f2, t_d1, t_d2, t_ov, t_or = evaluate.load_overlap_npz(train_files)
   else:                                                            # rank 0's shuffle
     t_f1, t_f2, t_d1, t_d2, t_ov, t_or = dp.broadcast(evaluate.load_overlap_npz(train_files) if dp.rank == 0
@@ -248,13 +398,14 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
   v_f1, v_f2, v_d1, v_d2, v_ov, v_or = v_f1[:n_val], v_f2[:n_val], v_d1[:n_val], v_d2[:n_val], v_ov[:n_val], v_or[:n_val]
 
   cfg = dict(config)
-  for key, default in (('use_depth', True), ('use_normals', True), ('use_class_probabilities', False),
-                       ('use_class_probabilities_pca', False), ('use_intensity', False)):
-    cfg.setdefault(key, default)                                                        # training.py:137-160
+  for key, default in CUE_DEFAULTS:
+    cfg.setdefault(key, default)
   cfg['data_root_folder'] = imgpath
   cfg['infer_seqs'] = ''
   cfg['model'] = dict(model)
   cfg['model']['inputShape'] = list(model['inputShape'])
+  if resumed is not None:                                          # the checkpoint's weights replace them
+    cfg['pretrained_weightsfilename'] = ''
   infer = Infer(cfg, precision='fp32', device=device, max_batch_pairs=batch_size)
   eng = infer._engine
   width = infer.network_output_size
@@ -263,7 +414,11 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
     logger.info('Training precision: %s', config['training_precision'])
   if len(cfg['pretrained_weightsfilename']) > 0:
     logger.info('Load old weights from %s', cfg['pretrained_weightsfilename'])
-  if dp is not None:               # one start for every rank (glorot_init draws from its own generator)
+  if resumed is not None:          # every rank; the weights first: ovn_finalize_weights resets the accumulators
+    check_checkpoint_fits(resumed, eng, flow.whole_network, checkpoint_path)
+    eng.load_weights(resumed['weights'])
+    eng.set_train_state(resumed['accum'], flow.whole_network)
+  elif dp is not None:             # one start for every rank (glorot_init draws from its own generator)
     start = dp.broadcast(eng.get_weights() if dp.rank == 0 else None)
     if dp.rank != 0:
       eng.load_weights(start)
@@ -299,7 +454,14 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
     logger.info('  data-parallel over %d ranks: each step all-gathers %d gradients per rank', dp.world,
                 grad.numel())
   history = {'epoch_loss': [], 'batch_losses': [], 'validation': [], 'weights_filename': weights_filename}
-  for epoch in range(no_epochs):
+  first_epoch = 0
+  if resumed is not None:
+    history.update(resumed['history'])
+    first_epoch = resumed['epochs']
+    if dp is None or dp.rank == 0:                                 # the draws continue where the saved run stopped
+      np.random.set_state(resumed['rng'])
+    logger.info('Resuming from %s after epoch %d of %d', checkpoint_path, first_epoch, no_epochs)
+  for epoch in range(first_epoch, no_epochs):
     lr = learning_rate(epoch, initial_lr, lr_alpha)
     losses, sizes = [], []
     t_or_epoch, rotate = t_or_d, None
@@ -364,6 +526,13 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
     for thr, rms in stats['orientation_rms'].items():
       logger.info('           Evaluation: orientation RMS (overlap > %.1f): %f', thr, rms)
     logger.info('iteration %d, batch/epoch loss: %.9f  /  %.9f', epoch + 1, losses[-1][0], epoch_loss)
+    if checkpoint and (dp is None or dp.rank == 0):
+      t0 = time.perf_counter()
+      accum = eng.train_state(steps.whole_network).cpu().numpy()
+      write_checkpoint(checkpoint_path, epoch + 1, eng.get_weights(), accum, (t_f1, t_f2, t_d1, t_d2, t_ov, t_or),
+                       history, fingerprint)
+      logger.info('  checkpoint after epoch %d written to %s in %.3f s', epoch + 1, checkpoint_path,
+                  time.perf_counter() - t0)
   return history
 
 
