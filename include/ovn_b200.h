@@ -325,6 +325,23 @@ int ovn_set_train_state(ovn_handle* h, int32_t whole_network, const float* d_in,
 int ovn_gather_images(ovn_handle* h, const float* d_images, int64_t n_images, const int32_t* d_rows,
                       const int32_t* d_shift, const float* d_rot /* [n][2] */, int32_t n,
                       float* d_out /* [n][H][W][C] */, void* stream);
+/* ---- a training image bank in host memory (overlapnet_b200/image_bank.py, DESIGN.md section 6) ---------------
+ *   ovn_train_workspace_bytes: *bytes = the device memory the training buffers of this handle take once it has
+ *                    trained n_pairs-pair batches: the heads' buffers, gradients and accumulators, and with
+ *                    whole_network the leg activations of 2 n_pairs images and their backward buffers; the split-K
+ *                    partials counted once.  Allocates nothing.
+ *   ovn_host_register / ovn_host_unregister: page-lock (cudaHostRegister, portable) / release `bytes` of host
+ *                    memory the caller owns, so that copies from it are asynchronous.  OVN_ERR_CUDA with the
+ *                    runtime's message when the pin fails.
+ *   ovn_stage_rows:  for i < n, one cudaMemcpyAsync on `stream` of row h_rows[i] (row_bytes bytes) of the host
+ *                    block h_src [n_src_rows][row_bytes] to d_dst + i row_bytes.  h_rows is read on the host before
+ *                    any copy is issued; a row outside [0, n_src_rows) is OVN_ERR_INVALID_ARG and nothing is
+ *                    copied.  h_src must be page-locked for the copies to be asynchronous.  Both precisions. */
+int ovn_train_workspace_bytes(ovn_handle* h, int32_t whole_network, int32_t n_pairs, int64_t* bytes);
+int ovn_host_register(ovn_handle* h, void* h_ptr, int64_t bytes);
+int ovn_host_unregister(ovn_handle* h, void* h_ptr);
+int ovn_stage_rows(ovn_handle* h, const void* h_src, int64_t n_src_rows, int64_t row_bytes, const int64_t* h_rows,
+                   int32_t n, void* d_dst, void* stream);
 /* Current weights / last gradients of a layer, Keras layout, host buffers (same shapes as ovn_set_weights).
  * Both synchronise the device.  ovn_get_gradients returns the head layers after ovn_head_gradients and every
  * layer after ovn_net_gradients. */

@@ -893,6 +893,50 @@ int ovn_gather_images(ovn_handle* h, const float* d_images, int64_t n_images, co
   return gather_images(h, d_images, n_images, d_rows, d_shift, d_rot, n, d_out, (cudaStream_t)stream);
 }
 
+// ---- a training image bank in host memory -------------------------------------------------------------------
+int ovn_train_workspace_bytes(ovn_handle* h, int32_t whole_network, int32_t n_pairs, int64_t* bytes) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  REQUIRE(h, bytes, "NULL pointer");
+  REQUIRE(h, n_pairs > 0, "n_pairs must be positive");
+  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_train_workspace_bytes: %s", h->net_error.c_str());
+  *bytes = train_workspace_bytes(h, whole_network != 0, n_pairs);
+  return OVN_OK;
+}
+
+int ovn_host_register(ovn_handle* h, void* h_ptr, int64_t bytes) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, h_ptr && bytes > 0, "NULL pointer or no bytes");
+  OVN_CUDA(h, cudaHostRegister(h_ptr, (size_t)bytes, cudaHostRegisterPortable));
+  return OVN_OK;
+}
+
+int ovn_host_unregister(ovn_handle* h, void* h_ptr) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, h_ptr, "NULL pointer");
+  OVN_CUDA(h, cudaHostUnregister(h_ptr));
+  return OVN_OK;
+}
+
+int ovn_stage_rows(ovn_handle* h, const void* h_src, int64_t n_src_rows, int64_t row_bytes, const int64_t* h_rows,
+                   int32_t n, void* d_dst, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, n >= 0 && n_src_rows >= 0 && row_bytes > 0, "negative size");
+  REQUIRE(h, n == 0 || (h_src && h_rows && d_dst), "NULL pointer");
+  for (int32_t i = 0; i < n; ++i)          // all rows first: a refused call copies nothing
+    if (h_rows[i] < 0 || h_rows[i] >= n_src_rows)
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_stage_rows: row %lld of entry %d is outside [0, %lld)",
+                  (long long)h_rows[i], i, (long long)n_src_rows);
+  const char* src = (const char*)h_src;
+  char* dst = (char*)d_dst;
+  for (int32_t i = 0; i < n; ++i)
+    OVN_CUDA(h, cudaMemcpyAsync(dst + (size_t)i * row_bytes, src + (size_t)h_rows[i] * row_bytes, (size_t)row_bytes,
+                                cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  return OVN_OK;
+}
+
 int ovn_bank_prepare(ovn_handle* h, const float* d_bank, int64_t bank_capacity, int64_t first, int64_t count,
                      void* stream) {
   if (!h) return OVN_ERR_INVALID_ARG;

@@ -335,6 +335,7 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
                        const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
                        float* d_fv_grad, cudaStream_t s);
 int net_max_pairs(const ovn_handle* h);   // largest n_pairs of one ovn_net_gradients call (launch grid limits)
+int64_t train_workspace_bytes(const ovn_handle* h, bool whole_network, int np);   // ovn_train_workspace_bytes
 int copy_net_volumes_fp32(ovn_handle* h, float* d_out, cudaStream_t s);
 // The Adagrad step of the heads' (or with whole_network every layer's) prefix of the flat vector, from the
 // weighted sum of d_parts [n_parts][that length]: one launch

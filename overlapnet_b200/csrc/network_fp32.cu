@@ -702,30 +702,46 @@ static void head_dims(const ovn_handle* h, int l, int* K, int* N) {
   else { *K = h->dense_in; *N = 1; }
 }
 
-// h->train, complete or not at all
-int train_alloc(ovn_handle* h) {
+// The bytes of the buffers train_alloc makes, in its order: x4, dx3, corr, overlap, dz, yaw, w3t, grad, accum,
+// loss, then the split-K partials (part, which net_alloc may grow)
+constexpr int kTrainBufs = 11;
+static void train_sizes(const ovn_handle* h, size_t b[kTrainBufs]) {
   const int64_t maxp = h->cfg.max_batch_pairs, Wf = h->cfg.leg_output_width;
   const ConvSpec& L3 = h->head[2];
   const int64_t total = h->params.n_total;
-  std::unique_ptr<TrainState> t(new TrainState());
   int64_t max_part = 0;
   for (int l = 0; l < 3; ++l) {
     int K, N;
     head_dims(h, l, &K, &N);
     if ((int64_t)(K + 1) * N > max_part) max_part = (int64_t)(K + 1) * N;
   }
+  const size_t sizes[kTrainBufs] = {
+      (size_t)maxp * h->dense_in * sizeof(float), (size_t)maxp * L3.h_in * L3.w_in * L3.cin * sizeof(float),
+      (size_t)maxp * Wf * sizeof(float), (size_t)maxp * sizeof(float), (size_t)maxp * sizeof(float),
+      (size_t)maxp * sizeof(int32_t), (size_t)L3.kh * L3.kw * L3.cin * L3.cout * sizeof(float),
+      (size_t)total * sizeof(float), (size_t)total * sizeof(float), 4 * sizeof(float),
+      (size_t)kMaxSplit * max_part * sizeof(float)};
+  for (int i = 0; i < kTrainBufs; ++i) b[i] = sizes[i];
+}
+
+// h->train, complete or not at all
+int train_alloc(ovn_handle* h) {
+  const int64_t total = h->params.n_total;
+  std::unique_ptr<TrainState> t(new TrainState());
+  size_t b[kTrainBufs];
+  train_sizes(h, b);
   int rc;
-  if ((rc = t->x4.ensure(h, (size_t)maxp * h->dense_in * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t->dx3.ensure(h, (size_t)maxp * L3.h_in * L3.w_in * L3.cin * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t->corr.ensure(h, (size_t)maxp * Wf * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t->overlap.ensure(h, (size_t)maxp * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t->dz.ensure(h, (size_t)maxp * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t->yaw.ensure(h, (size_t)maxp * sizeof(int32_t))) != OVN_OK) return rc;
-  if ((rc = t->w3t.ensure(h, (size_t)L3.kh * L3.kw * L3.cin * L3.cout * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t->part.ensure(h, (size_t)kMaxSplit * max_part * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t->grad.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t->accum.ensure(h, (size_t)total * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t->loss.ensure(h, 4 * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t->x4.ensure(h, b[0])) != OVN_OK) return rc;
+  if ((rc = t->dx3.ensure(h, b[1])) != OVN_OK) return rc;
+  if ((rc = t->corr.ensure(h, b[2])) != OVN_OK) return rc;
+  if ((rc = t->overlap.ensure(h, b[3])) != OVN_OK) return rc;
+  if ((rc = t->dz.ensure(h, b[4])) != OVN_OK) return rc;
+  if ((rc = t->yaw.ensure(h, b[5])) != OVN_OK) return rc;
+  if ((rc = t->w3t.ensure(h, b[6])) != OVN_OK) return rc;
+  if ((rc = t->part.ensure(h, b[10])) != OVN_OK) return rc;
+  if ((rc = t->grad.ensure(h, b[7])) != OVN_OK) return rc;
+  if ((rc = t->accum.ensure(h, b[8])) != OVN_OK) return rc;
+  if ((rc = t->loss.ensure(h, b[9])) != OVN_OK) return rc;
   OVN_CUDA(h, cudaMemset(t->accum, 0, (size_t)total * sizeof(float)));
   h->train = std::move(t);
   return OVN_OK;
@@ -1128,9 +1144,10 @@ int net_max_pairs(const ovn_handle* h) {
   return (int)(by_rows < by_z ? by_rows : by_z);
 }
 
-// The whole-network buffers of an np-pair batch
-static int net_alloc(ovn_handle* h, int np) {
-  TrainState& t = *h->train;
+// The bytes of the whole-network buffers of an np-pair batch, in net_alloc's order: images, acts, dact[0],
+// dact[1], dfv_part, dcorr, pair_rows, wt, then the split-K partials (part, shared with train_alloc)
+constexpr int kNetBufs = 9;
+static void net_sizes(const ovn_handle* h, int np, size_t b[kNetBufs]) {
   const int64_t n2 = 2 * (int64_t)np, Wf = h->cfg.leg_output_width, vol = Wf * kFeatC;
   const int64_t img = (int64_t)h->cfg.proj_H * h->cfg.proj_W * h->C;
   const int nb = h->o1_w, nit = (int)((Wf + kDgT - 1) / kDgT);
@@ -1145,16 +1162,44 @@ static int net_alloc(ovn_handle* h, int np) {
     if (w > max_w) max_w = w;
     if (g > max_part) max_part = g;
   }
+  const size_t sizes[kNetBufs] = {
+      (size_t)(n2 * img) * sizeof(float), (size_t)(n2 * acts) * sizeof(float),
+      (size_t)(n2 * max_act) * sizeof(float), (size_t)(n2 * max_act) * sizeof(float),
+      (size_t)(np * (int64_t)(nb + nit) * vol) * sizeof(float), (size_t)(np * Wf) * sizeof(float),
+      (size_t)n2 * sizeof(int32_t), (size_t)max_w * sizeof(float), (size_t)kMaxSplit * max_part * sizeof(float)};
+  for (int i = 0; i < kNetBufs; ++i) b[i] = sizes[i];
+}
+
+static int net_alloc(ovn_handle* h, int np) {
+  TrainState& t = *h->train;
+  size_t b[kNetBufs];
+  net_sizes(h, np, b);
   int rc;
-  if ((rc = t.images.ensure(h, (size_t)(n2 * img) * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t.acts.ensure(h, (size_t)(n2 * acts) * sizeof(float))) != OVN_OK) return rc;
+  if ((rc = t.images.ensure(h, b[0])) != OVN_OK) return rc;
+  if ((rc = t.acts.ensure(h, b[1])) != OVN_OK) return rc;
   for (int k = 0; k < 2; ++k)
-    if ((rc = t.dact[k].ensure(h, (size_t)(n2 * max_act) * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t.dfv_part.ensure(h, (size_t)(np * (int64_t)(nb + nit) * vol) * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t.dcorr.ensure(h, (size_t)(np * Wf) * sizeof(float))) != OVN_OK) return rc;
-  if ((rc = t.pair_rows.ensure(h, (size_t)n2 * sizeof(int32_t))) != OVN_OK) return rc;
-  if ((rc = t.wt.ensure(h, (size_t)max_w * sizeof(float))) != OVN_OK) return rc;
-  return t.part.ensure(h, (size_t)kMaxSplit * max_part * sizeof(float));
+    if ((rc = t.dact[k].ensure(h, b[2 + k])) != OVN_OK) return rc;
+  if ((rc = t.dfv_part.ensure(h, b[4])) != OVN_OK) return rc;
+  if ((rc = t.dcorr.ensure(h, b[5])) != OVN_OK) return rc;
+  if ((rc = t.pair_rows.ensure(h, b[6])) != OVN_OK) return rc;
+  if ((rc = t.wt.ensure(h, b[7])) != OVN_OK) return rc;
+  return t.part.ensure(h, b[8]);
+}
+
+// The device bytes the training buffers of a handle take once it has trained n_pairs-pair batches: train_alloc's,
+// and with whole_network net_alloc's; the split-K partials are one buffer, the larger of the two
+int64_t train_workspace_bytes(const ovn_handle* h, bool whole_network, int np) {
+  size_t t[kTrainBufs], n[kNetBufs];
+  train_sizes(h, t);
+  int64_t bytes = 0;
+  for (int i = 0; i < kTrainBufs - 1; ++i) bytes += (int64_t)t[i];
+  size_t part = t[kTrainBufs - 1];
+  if (whole_network) {
+    net_sizes(h, np, n);
+    for (int i = 0; i < kNetBufs - 1; ++i) bytes += (int64_t)n[i];
+    if (n[kNetBufs - 1] > part) part = n[kNetBufs - 1];
+  }
+  return bytes + (int64_t)part;
 }
 
 // Forward of the leg on the 2 np gathered images (the launches of leg_forward_fp32, every output kept), both

@@ -85,6 +85,9 @@ class Engine:
 
   def close(self):
     if getattr(self, '_h', None) is not None and self._h.value:
+      for a in getattr(self, '_pinned', ()):                      # host_register'ed blocks still pinned
+        lib().ovn_host_unregister(self._h, a.ctypes.data_as(C.c_void_p))
+      self._pinned = []
       lib().ovn_destroy(self._h)
       self._h = C.c_void_p(0)
 
@@ -484,6 +487,41 @@ class Engine:
     assert v.numel() == n
     check(self._h, lib().ovn_set_train_state(self._h, int(bool(whole_network)), _ptr(v), self._stream()),
           'ovn_set_train_state')
+
+  # ---- a training image bank in host memory (overlapnet_b200.image_bank) ------------------------------------
+  def train_workspace_bytes(self, n_pairs, whole_network=False):
+    """ovn_train_workspace_bytes: device bytes of this handle's training buffers for n_pairs-pair batches."""
+    n = C.c_int64(0)
+    check(self._h, lib().ovn_train_workspace_bytes(self._h, int(bool(whole_network)), int(n_pairs), C.byref(n)),
+          'ovn_train_workspace_bytes')
+    return int(n.value)
+
+  def host_register(self, array):
+    """ovn_host_register: page-lock the memory of a C-contiguous NumPy array.  The handle keeps the array until
+    host_unregister or close releases it, so that its memory is never freed while pinned."""
+    assert array.flags['C_CONTIGUOUS']
+    check(self._h, lib().ovn_host_register(self._h, array.ctypes.data_as(C.c_void_p), int(array.nbytes)),
+          'ovn_host_register')
+    self._pinned = getattr(self, '_pinned', []) + [array]
+
+  def host_unregister(self, array):
+    """ovn_host_unregister of an array host_register pinned."""
+    kept = [a for a in getattr(self, '_pinned', []) if a is not array]
+    assert len(kept) < len(getattr(self, '_pinned', [])), 'the array is not pinned by this handle'
+    check(self._h, lib().ovn_host_unregister(self._h, array.ctypes.data_as(C.c_void_p)), 'ovn_host_unregister')
+    self._pinned = kept
+
+  def stage_rows(self, host, rows, out):
+    """ovn_stage_rows: out[i] = host[rows[i]], one asynchronous copy per row on the current stream.  ``host`` a
+    C-contiguous page-locked NumPy array, ``rows`` host integers, ``out`` a contiguous cuda tensor of at least
+    len(rows) rows of host's row size."""
+    r = np.ascontiguousarray(rows, np.int64).reshape(-1)
+    row_bytes = host[0].nbytes if host.shape[0] else 0
+    assert host.flags['C_CONTIGUOUS'] and out.is_contiguous() and out.device == self.device
+    assert out.shape[0] >= r.size and out[0].numel() * out.element_size() == row_bytes
+    check(self._h, lib().ovn_stage_rows(self._h, host.ctypes.data_as(C.c_void_p), int(host.shape[0]), row_bytes,
+                                        r.ctypes.data_as(C.c_void_p), int(r.size), _ptr(out), self._stream()),
+          'ovn_stage_rows')
 
   @property
   def leg_layers(self):

@@ -1,0 +1,213 @@
+"""Where a training flow keeps its image bank -- the packed input [n, H, W, C] float32 of every distinct scan it
+trains on -- and how a step's images reach the device when that bank lives in host memory (DESIGN.md sections 1
+and 6).
+
+The flow compares the bank's bytes with the device's free memory minus the working set of its largest step
+(``working_set_bytes``).  A bank that fits goes on the device, as it always did.  One that does not goes into one
+page-locked host block (``HostBank``), and every step copies only its own distinct rows into one of two device
+slots (``StagingRing``) on a copy stream, one copy per row, while the previous step computes.  The kernels a step
+runs are those of the device bank, on the same image values, so both placements train bit-identical weights.
+"""
+import collections
+import logging
+
+import numpy as np
+import torch
+
+from . import data_parallel
+from .engine import FEAT_C
+
+logger = logging.getLogger('overlapnet_b200.training')
+
+PLACEMENTS = ('device', 'host')
+MARGIN_BYTES = 1 << 30   # the CUDA context's own growth, allocator rounding and the small per-step tensors
+
+
+def image_bytes(eng):
+  return eng.H * eng.W * eng.C * 4
+
+
+def share_pairs(n_pairs, world):
+  """The largest share of an n_pairs batch that one of ``world`` data-parallel ranks trains."""
+  bounds, _ = data_parallel.shares(n_pairs, world)
+  return max(hi - lo for lo, hi in bounds)
+
+
+def working_set_bytes(eng, b_share, whole_network, gathered, features):
+  """Device bytes a training run needs besides its image bank, from the shapes of its largest step of
+  ``b_share`` pairs: the handle's training buffers (Engine.train_workspace_bytes: for the whole network the leg
+  activations of 2 b_share images, the split-K partials, the head buffers), the staging ring (two slots of
+  2 b_share images), ``gathered`` images of a step's gathered batch (yaw augmentation), ``features`` feature volumes
+  (the validation feature bank, the frozen leg's bank) and MARGIN_BYTES."""
+  return (eng.train_workspace_bytes(b_share, whole_network) + 2 * 2 * b_share * image_bytes(eng)
+          + gathered * image_bytes(eng) + features * eng.Wf * FEAT_C * 4 + MARGIN_BYTES)
+
+
+def choose_placement(bank_bytes, free_bytes, working_set):
+  """'device' when the bank fits into the free device memory left after the working set, else 'host'; and that
+  budget (free_bytes - working_set)."""
+  budget = int(free_bytes) - int(working_set)
+  return ('device' if int(bank_bytes) <= budget else 'host'), budget
+
+
+def free_device_bytes(eng):
+  return int(torch.cuda.mem_get_info(eng.device)[0])
+
+
+def plan_rows(*row_lists):
+  """The distinct rows of a step's row lists, in order of first appearance (the lists in the order given), and the
+  local index of every entry of every list among them: rows[local[k][i]] == row_lists[k][i].  Returns (rows int64,
+  [local int32 per list])."""
+  parts = [np.asarray(r, np.int64).reshape(-1) for r in row_lists]
+  cat = np.concatenate(parts) if parts else np.zeros(0, np.int64)
+  uniq, first, inverse = np.unique(cat, return_index=True, return_inverse=True)
+  order = np.argsort(first, kind='stable')
+  rank = np.empty(order.size, np.int64)
+  rank[order] = np.arange(order.size)
+  local = rank[inverse.reshape(-1)].astype(np.int32)
+  out, o = [], 0
+  for p in parts:
+    out.append(local[o:o + p.size])
+    o += p.size
+  return uniq[order], out
+
+
+class HostBank:
+  """The images [n, H, W, C] float32 in one page-locked host block, pinned through the handle
+  (Engine.host_register), which releases it on close() or when the handle closes."""
+
+  def __init__(self, eng, n):
+    self.eng = eng
+    shape = (int(n), eng.H, eng.W, eng.C)
+    nbytes = int(np.prod(shape)) * 4
+    try:
+      self.images = np.empty(shape, np.float32)
+      eng.host_register(self.images)
+    except Exception as e:
+      raise Exception('image bank in host memory: could not pin %d bytes (%.2f GB) for %d images of %d x %d x %d '
+                      'float32: %s' % (nbytes, nbytes / 1e9, shape[0], shape[1], shape[2], shape[3], e)) from e
+
+  @property
+  def nbytes(self):
+    return self.images.nbytes
+
+  def close(self):
+    if self.images is not None:
+      self.eng.host_unregister(self.images)
+      self.images = None
+
+
+class StagingRing:
+  """Two device slots of ``slot_rows`` images, filled from a HostBank on a copy stream of their own.
+
+  ``plan`` takes the row lists of the steps to come, in the order they will run; each step's distinct rows
+  (plan_rows) are copied into the next slot, one asynchronous copy per row.  ``take`` hands the compute stream the
+  oldest filled slot after making it wait for that slot's copy-done event, with the step's local indices;
+  ``release`` records the compute-done event of the step that read the slot, and issues the next planned copy into
+  it, which waits for that event.  So step k + 1's copies run while step k computes, and a slot is never written
+  while a step still reads it."""
+
+  def __init__(self, eng, host, slot_rows, timing=False):
+    self.eng, self.host, self.slot_rows = eng, host, int(slot_rows)
+    dev = eng.device
+    self.slots = [torch.empty((self.slot_rows, eng.H, eng.W, eng.C), dtype=torch.float32, device=dev)
+                  for _ in range(2)]
+    self.copy_stream = torch.cuda.Stream(device=dev)
+    self._copied = [torch.cuda.Event(), torch.cuda.Event()]
+    self._computed = [None, None]
+    self._queue = collections.deque()                 # planned, not yet issued: (rows, locals)
+    self._ready = collections.deque()                 # issued, not yet taken: (slot, locals)
+    self._next = 0                                    # the slot the next issue fills
+    self._taken = None
+    self.step_rows = 0                                # the distinct rows staged for the step taken last
+    self.timing = timing
+    self.waits = []                                   # with timing: (before, after) events around each wait
+
+  def plan(self, steps):
+    """``steps``: for each step to come, a tuple of row lists (plan_rows)."""
+    assert not self._queue and not self._ready and self._taken is None, 'the previous plan is not consumed'
+    for lists in steps:
+      rows, local = plan_rows(*lists)
+      assert rows.size <= self.slot_rows, (rows.size, self.slot_rows)
+      self._queue.append((rows, local))
+    while self._queue and len(self._ready) < 2:
+      self._issue()
+
+  def _issue(self):
+    rows, local = self._queue.popleft()
+    s = self._next
+    self._next ^= 1
+    with torch.cuda.stream(self.copy_stream):
+      if self._computed[s] is not None:
+        self.copy_stream.wait_event(self._computed[s])
+      self.eng.stage_rows(self.host.images, rows, self.slots[s])
+      self._copied[s].record(self.copy_stream)
+    self._ready.append((s, local, int(rows.size)))
+
+  def take(self):
+    """The next step's slot (a device tensor [slot_rows, H, W, C]) and its local indices (int32 device tensors,
+    one per row list), ordered after its copies on the current stream."""
+    assert self._taken is None and self._ready, 'take without a planned step'
+    s, local, self.step_rows = self._ready.popleft()
+    idx = [torch.from_numpy(l).to(self.eng.device) for l in local]
+    cur = torch.cuda.current_stream(self.eng.device)
+    if self.timing:
+      before, after = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+      before.record(cur)
+    cur.wait_event(self._copied[s])
+    if self.timing:
+      after.record(cur)
+      self.waits.append((before, after))
+    self._taken = s
+    return self.slots[s], idx
+
+  def release(self):
+    """The step that took the slot has queued its last read of it."""
+    s, self._taken = self._taken, None
+    if self._computed[s] is None:
+      self._computed[s] = torch.cuda.Event()
+    self._computed[s].record(torch.cuda.current_stream(self.eng.device))
+    if self._queue:
+      self._issue()
+
+  def wait_ms(self):
+    """With timing: for each take since the last call, the milliseconds the compute stream waited on the slot's
+    copy-done event.  Waits for those events only, not for the device, so copies still in flight on the copy
+    stream keep running."""
+    out = []
+    for before, after in self.waits:
+      after.synchronize()
+      out.append(before.elapsed_time(after))
+    self.waits = []
+    return out
+
+
+def open_bank(infer, keys, image_bank, b_share, whole_network, gathered, features, what):
+  """The image bank of the distinct (dir, scan) ``keys``: ``image_bank`` None chooses its placement from the free
+  device memory and the working set (working_set_bytes), 'device' or 'host' forces it.  Returns (placement, the
+  device tensor or HostBank, {key: row}).  ``what`` names the bank in the log."""
+  from .training_leg import bank_rows, fill_image_bank, load_image_bank
+  eng = infer._engine
+  if image_bank not in (None,) + PLACEMENTS:
+    raise ValueError('image_bank %r: use None, %s' % (image_bank, ' or '.join(repr(p) for p in PLACEMENTS)))
+  n = len(set(keys))
+  bank_bytes = n * image_bytes(eng)
+  placement = image_bank
+  if placement is None:
+    ws = working_set_bytes(eng, b_share, whole_network, gathered, features)
+    placement, budget = choose_placement(bank_bytes, free_device_bytes(eng), ws)
+    logger.info('%s: %d scans, %.1f MB; device budget %.1f MB (free memory minus a working set of %.1f MB): '
+                'on the %s', what, n, bank_bytes / 1e6, budget / 1e6, ws / 1e6,
+                'GPU' if placement == 'device' else 'host, pinned')
+  if placement == 'device':
+    images, rows = load_image_bank(infer, keys)
+    return placement, images, rows
+  rows = bank_rows(keys)
+  host = HostBank(eng, len(rows))
+  fill_image_bank(infer, rows, host.images)
+  dp = data_parallel.default_group()
+  world = 1 if dp is None else dp.world
+  logger.info('%s: %d scans in pinned host memory, %.1f MB per rank, %.1f MB on the node over %d ranks; each step '
+              'copies its rows into a ring of 2 x %d images on the GPU', what, len(rows), host.nbytes / 1e6,
+              world * host.nbytes / 1e6, world, 2 * b_share)
+  return placement, host, rows

@@ -20,6 +20,10 @@ every pair of every epoch) and TensorBoard output.
 the column pitch, its normals with it, and its orientation label moved to match.  Here the frozen leg encodes
 each step's rotated RIGHT images.  Validation is never augmented.
 
+An image bank (the whole network's; the frozen leg's RIGHT scans under yaw augmentation) that does not fit on the
+GPU beside the largest step's working set is kept in pinned host memory, and each step's images are staged to the
+GPU while the previous step computes (overlapnet_b200.image_bank, DESIGN.md section 6); the weights are the same.
+
 ``training_precision: tf32x3`` (both legsTypes, default fp32) runs every product of the gradient steps on tensor
 cores in 3xTF32 with fp32 accumulation (Engine.set_train_precision); validation stays fp32.
 
@@ -290,20 +294,35 @@ class FrozenLeg:
   """The training step of 360OutputkLegsFixed: every distinct scan is encoded once by the frozen leg into a
   feature bank on the GPU; a step trains the overlap head on it."""
 
-  def __init__(self, infer, keys, rotate_keys=None):
+  def __init__(self, infer, keys, rotate_keys=None, image_bank=None):
+    """``image_bank`` (yaw augmentation only: without it there is no image bank) None places the RIGHT scans'
+    images on the GPU when they fit beside the largest step's working set and in pinned host memory otherwise
+    (overlapnet_b200.image_bank); 'device' or 'host' forces a placement.  Both train the same bits."""
     logger.info('Encoding %d scans with the frozen leg ...', len(keys))
     self.eng = infer._engine
     self.bank, self.rows = _encode_bank(infer, keys)
+    self.image_bank = None
     if rotate_keys:
       # Yaw augmentation: the images of the scans a step may rotate, and max_batch_scans scratch rows after the
       # bank that receive a step's rotated RIGHT volumes.
-      from .training_leg import load_image_bank
-      self.images, self.image_rows = load_image_bank(infer, rotate_keys)
+      from . import image_bank as _image_bank
+      dp = data_parallel.default_group()
+      b_share = _image_bank.share_pairs(self.eng.max_batch_pairs, 1 if dp is None else dp.world)
       n, B = len(self.rows), self.eng.max_batch_scans
+      self.image_bank, self.images, self.image_rows = _image_bank.open_bank(
+          infer, rotate_keys, image_bank, b_share, False, b_share, n + B, 'Image bank of the rotated RIGHT scans')
+      if self.image_bank == 'host':
+        self.ring = _image_bank.StagingRing(self.eng, self.images, 2 * b_share)
       self.bank = torch.cat([self.bank, self.bank.new_empty((B,) + tuple(self.bank.shape[1:]))])
       self.scratch = torch.arange(n, n + B, dtype=torch.int32, device=self.eng.device)
 
   whole_network = False          # the layers the gradients cover (Engine.copy_gradients, adagrad_step_sum)
+  ring = None                    # the image_bank.StagingRing of a host image bank
+
+  def begin_epoch(self, spans, left, right, rotate_rows=None):
+    """With a host bank: the steps this rank runs in the coming epoch, in order -- pairs [a, b) of the training
+    pairs' RIGHT image rows ``rotate_rows`` (host array) -- whose images the ring then stages ahead of each step."""
+    self.ring.plan([(rotate_rows[a:b],) for a, b in spans])
 
   def step(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, lr, rotate=None):
     """``rotate`` = (image rows, column shifts, (cos, sin)) of the batch's RIGHT scans, or None: the rotated
@@ -316,8 +335,13 @@ class FrozenLeg:
     """``step`` without its update: the losses; the gradients stay in the handle (the data-parallel step)."""
     if rotate is not None:
       rows, shifts, rot = rotate
+      images = self.images
+      if self.ring is not None:                  # the next span begin_epoch planned, staged in the ring's slot
+        images, (rows,) = self.ring.take()
       n, n0 = rows.numel(), len(self.rows)
-      x = self.eng.gather_images(self.images, rows, shifts, rot)
+      x = self.eng.gather_images(images, rows, shifts, rot)
+      if self.ring is not None:
+        self.ring.release()
       self.eng.leg(x, out=self.bank[n0:n0 + n])
       right = self.scratch[:n]
     return self.eng.head_gradients(self.bank, left, right, gt_overlap, gt_orientation, min_overlap_for_angle)
@@ -447,6 +471,11 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
                 'moved', pitch, pitch * width // W)
   else:
     logger.info('  NO rotation of training data')
+  staged = getattr(steps, 'image_bank', None) == 'host'
+  if staged:                      # the image rows of the pairs (LEFT, RIGHT, rotated RIGHT) for begin_epoch's plans
+    right_h = np.asarray([steps.image_rows[k] for k in zip(t_d2, t_f2)], np.int64)
+    left_h = np.asarray([steps.image_rows[k] for k in zip(t_d1, t_f1)], np.int64) if steps.whole_network else None
+    t_rows_h = (left_h, right_h, right_h if yaw_augmentation else None)
   if dp is not None:
     whole = steps.whole_network
     grad = torch.zeros((eng.gradient_size(whole),), dtype=torch.float32, device=dev)
@@ -476,6 +505,14 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
       shifts_d = torch.from_numpy(shifts).to(dev)
       rot_d = torch.from_numpy(augment.rotation(shifts, W)).to(dev)
       t_or_epoch = augment.move_labels(t_or_d, shifts_d, W, width)
+    if staged:                                                     # this rank's pairs of each step, in order
+      spans = []
+      for b in perm:
+        s0, s1 = b * batch_size, min(n, (b + 1) * batch_size)
+        lo, hi = (0, s1 - s0) if dp is None else data_parallel.shares(s1 - s0, dp.world)[0][dp.rank]
+        if hi > lo:
+          spans.append((s0 + lo, s0 + hi))
+      steps.begin_epoch(spans, *t_rows_h)
     for b in perm:
       s0, s1 = b * batch_size, min(n, (b + 1) * batch_size)
       if dp is not None:
