@@ -297,6 +297,30 @@ int ovn_train_gradient_size(ovn_handle* h, int32_t whole_network, int64_t* n);
 int ovn_copy_gradients(ovn_handle* h, int32_t whole_network, float* d_out, void* stream);
 int ovn_adagrad_step_sum(ovn_handle* h, int32_t whole_network, const float* d_parts, int32_t n_parts,
                          const float* h_weights, float learning_rate, void* stream);
+/* ---- gradients per chunk of a batch (gradient_chunks in overlapnet_b200/training.py, DESIGN.md section 6) -------
+ * One call over the pairs [0, n_pairs) of a range, cut into n_chunks contiguous chunks: chunk c is the pairs
+ * [h_chunk_offsets[c], h_chunk_offsets[c + 1]) (host array of n_chunks + 1).  d_parts [n_chunks][n] (n =
+ * ovn_train_gradient_size(h, 0) for the heads call, (h, 1) for the whole-network call) and h_loss [n_chunks][3]:
+ * part c and h_loss[c] are bit for bit what ovn_head_gradients / ovn_net_gradients on the pairs of chunk c alone
+ * leave in h_loss and, through ovn_copy_gradients, in d_out -- at either training precision.  An empty chunk gives a
+ * zero part and zero losses.  The stages that compute each pair on its own (the leg and heads forward, every input
+ * gradient, the ReLU masks) run once over the range; the losses and every weight gradient run per chunk.
+ * Synchronous, like the one-chunk calls.  The call leaves no gradients and no batch in the handle:
+ * ovn_copy_gradients, ovn_copy_net_volumes, ovn_get_gradients, ovn_head_adagrad_step and ovn_net_adagrad_step
+ * return OVN_ERR_INVALID_ARG until the next ovn_head_gradients / ovn_net_gradients; ovn_adagrad_step_sum takes
+ * the parts.  Errors: those of the one-chunk calls for the whole range (n_pairs <= 485 at leg_output_width 360 for
+ * the whole network), plus n_chunks < 1, a NULL h_chunk_offsets or d_parts, or offsets that do not run
+ * non-decreasing from 0 to n_pairs (OVN_ERR_INVALID_ARG), and n_chunks > 64 (OVN_ERR_CAPACITY). */
+int ovn_head_gradients_chunks(ovn_handle* h, const float* d_bank, int64_t bank_size,
+                              const int32_t* d_left_idx, const int32_t* d_right_idx, int32_t n_pairs,
+                              const int32_t* h_chunk_offsets, int32_t n_chunks,
+                              const float* d_gt_overlap, const int32_t* d_gt_orientation,
+                              float min_overlap_for_angle, float* d_parts, float* h_loss, void* stream);
+int ovn_net_gradients_chunks(ovn_handle* h, const float* d_images, int64_t n_images,
+                             const int32_t* d_left_idx, const int32_t* d_right_idx, int32_t n_pairs,
+                             const int32_t* h_chunk_offsets, int32_t n_chunks,
+                             const float* d_gt_overlap, const int32_t* d_gt_orientation,
+                             float min_overlap_for_angle, float* d_parts, float* h_loss, void* stream);
 /* ---- the training state, for checkpoints that resume a run (overlapnet_b200/training.py, DESIGN.md section 6) --
  * The Adagrad accumulators as one flat float32 vector in the layout of ovn_copy_gradients:
  * ovn_train_gradient_size(h, whole_network) floats, the heads' prefix (whole_network = 0) or every layer.

@@ -26,6 +26,7 @@ SYMBOLS = [
     'ovn_train_gradient_size', 'ovn_copy_gradients', 'ovn_adagrad_step_sum', 'ovn_set_train_precision',
     'ovn_copy_net_volumes', 'ovn_copy_train_state', 'ovn_set_train_state',
     'ovn_train_workspace_bytes', 'ovn_host_register', 'ovn_host_unregister', 'ovn_stage_rows',
+    'ovn_head_gradients_chunks', 'ovn_net_gradients_chunks',
 ]
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
 
@@ -117,6 +118,8 @@ def lib():
   L.ovn_host_register.argtypes = [vp, vp, i64]
   L.ovn_host_unregister.argtypes = [vp, vp]
   L.ovn_stage_rows.argtypes = [vp, vp, i64, i64, vp, i32, vp, vp]
+  L.ovn_head_gradients_chunks.argtypes = [vp, vp, i64, vp, vp, i32, vp, i32, vp, vp, f32, vp, vp, vp]
+  L.ovn_net_gradients_chunks.argtypes = [vp, vp, i64, vp, vp, i32, vp, i32, vp, vp, f32, vp, vp, vp]
   L.ovn_get_weights.argtypes = [vp, C.c_char_p, vp, vp]
   L.ovn_get_gradients.argtypes = [vp, C.c_char_p, vp, vp]
   L.ovn_encode_clouds_host.argtypes = [vp, vp, vp, i32, vp]

@@ -695,16 +695,17 @@ struct TrainPrecisionScope {
 };
 
 // ---- training: the overlap head with a frozen leg, or the whole network (360OutputkLegs) ---------------------
-// What ovn_head_gradients (rows: the feature-volume bank) and ovn_net_gradients (rows: the image set) share: the
-// checks, the training state, both index lists bounds-checked against the n_rows rows, and after the flow's own
-// work (`run`) the losses and the device error flag.
+// What ovn_head_gradients (rows: the feature-volume bank) and ovn_net_gradients (rows: the image set), and their
+// _chunks forms, share: the checks, the training state, both index lists bounds-checked against the n_rows rows,
+// and after the flow's own work (`run`) the losses and the device error flag.  `ch` with grad NULL is a one-chunk
+// call into the handle's gradients; else the chunks of a _chunks call, whose parts and losses go to the caller.
 }  // extern "C"
 template <class Run>
-static int gradients_call(ovn_handle* h, bool whole_network, const float* d_rows, int64_t n_rows,
+static int gradients_call(ovn_handle* h, bool whole_network, const char* fn, const float* d_rows, int64_t n_rows,
                           const int32_t* d_left_idx, const int32_t* d_right_idx, int32_t n_pairs,
-                          const float* d_gt_overlap, const int32_t* d_gt_orientation, float* h_loss, cudaStream_t s,
-                          Run run) {
-  const char* fn = whole_network ? "ovn_net_gradients" : "ovn_head_gradients";
+                          const float* d_gt_overlap, const int32_t* d_gt_orientation, GradChunks& ch, float* h_loss,
+                          cudaStream_t s, Run run) {
+  const bool chunked = ch.grad != nullptr;
   if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "%s: %s", fn, h->net_error.c_str());
   if (h->cfg.precision != OVN_PREC_FP32)
     OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "%s: training needs a precision fp32 handle", fn);
@@ -723,19 +724,61 @@ static int gradients_call(ovn_handle* h, bool whole_network, const float* d_rows
     int rc = train_alloc(h);
     if (rc != OVN_OK) return rc;
   }
-  h->train->grads = kNoGrads;
+  TrainState& t = *h->train;
+  t.grads = kNoGrads;
+  float* p_loss = h->stage()->loss;
+  if (chunked) {
+    const size_t bytes = (size_t)kMaxSumParts * 3 * sizeof(float);
+    int rc = t.chunk_loss.ensure(h, bytes);
+    if (rc == OVN_OK) rc = t.chunk_loss_host.ensure(h, bytes);
+    if (rc != OVN_OK) return rc;
+    ch.loss = t.chunk_loss;
+    p_loss = t.chunk_loss_host;
+    for (int c = 0; c < ch.n; ++c) {         // an empty chunk: a zero part and zero losses
+      if (ch.size(c) > 0) continue;
+      OVN_CUDA(h, cudaMemsetAsync(ch.grad + c * ch.stride, 0, (size_t)ch.stride * sizeof(float), s));
+      OVN_CUDA(h, cudaMemsetAsync(ch.loss + 3 * c, 0, 3 * sizeof(float), s));
+    }
+  } else {
+    ch.n = 1;
+    ch.off[0] = 0;
+    ch.off[1] = n_pairs;
+    ch.grad = t.grad;
+    ch.loss = t.loss;
+  }
   int32_t* l = h->d_idx_san;
   int32_t* r = h->d_idx_san + maxp;
   int rc = sanitize_indices(h, d_left_idx, n_pairs, n_rows, kErrBadIndex, l, s);
   if (rc == OVN_OK) rc = sanitize_indices(h, d_right_idx, n_pairs, n_rows, kErrBadIndex, r, s);
   if (rc == OVN_OK) rc = run(l, r);
   if (rc != OVN_OK) return rc;
-  float* p_loss = h->stage()->loss;
-  OVN_CUDA(h, cudaMemcpyAsync(p_loss, h->train->loss, 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  OVN_CUDA(h, cudaMemcpyAsync(p_loss, ch.loss, (size_t)ch.n * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
   rc = check_device_error(h, s);            // synchronises s; a bad index -> OVN_ERR_INVALID_ARG
   if (rc != OVN_OK) return rc;
-  memcpy(h_loss, p_loss, 3 * sizeof(float));
-  h->train->grads = whole_network ? kNetGrads : kHeadGrads;
+  memcpy(h_loss, p_loss, (size_t)ch.n * 3 * sizeof(float));
+  if (!chunked) t.grads = whole_network ? kNetGrads : kHeadGrads;
+  return OVN_OK;
+}
+
+// The chunk table of a _chunks call: 1 <= n_chunks <= 64, offsets non-decreasing from 0 to n_pairs, parts of
+// ovn_train_gradient_size floats each
+static int chunk_table(ovn_handle* h, const char* fn, bool whole_network, int32_t n_pairs,
+                       const int32_t* h_chunk_offsets, int32_t n_chunks, float* d_parts, GradChunks* ch) {
+  if (n_chunks < 1) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: n_chunks must be at least 1", fn);
+  if (n_chunks > kMaxSumParts)
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "%s: n_chunks=%d exceeds %d", fn, n_chunks, kMaxSumParts);
+  if (!h_chunk_offsets || !d_parts) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: NULL pointer", fn);
+  if (h_chunk_offsets[0] != 0 || h_chunk_offsets[n_chunks] != n_pairs)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: the chunk offsets must run from 0 to n_pairs=%d (got %d .. %d)", fn,
+                n_pairs, h_chunk_offsets[0], h_chunk_offsets[n_chunks]);
+  for (int c = 0; c < n_chunks; ++c)
+    if (h_chunk_offsets[c + 1] < h_chunk_offsets[c])
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: chunk offset %d (%d) is below offset %d (%d)", fn, c + 1,
+                  h_chunk_offsets[c + 1], c, h_chunk_offsets[c]);
+  ch->n = n_chunks;
+  for (int c = 0; c <= n_chunks; ++c) ch->off[c] = h_chunk_offsets[c];
+  ch->grad = d_parts;
+  ch->stride = whole_network ? h->params.n_total : h->params.n_head;
   return OVN_OK;
 }
 extern "C" {
@@ -747,10 +790,11 @@ int ovn_head_gradients(ovn_handle* h, const float* d_bank, int64_t bank_size, co
   DeviceGuard guard(h);
   TrainPrecisionScope precision(h);
   cudaStream_t s = (cudaStream_t)stream;
-  return gradients_call(h, false, d_bank, bank_size, d_left_idx, d_right_idx, n_pairs, d_gt_overlap,
-                        d_gt_orientation, h_loss, s, [&](const int32_t* l, const int32_t* r) {
+  GradChunks ch;
+  return gradients_call(h, false, "ovn_head_gradients", d_bank, bank_size, d_left_idx, d_right_idx, n_pairs,
+                        d_gt_overlap, d_gt_orientation, ch, h_loss, s, [&](const int32_t* l, const int32_t* r) {
                           return head_gradients_fp32(h, d_bank, l, r, n_pairs, d_gt_overlap, d_gt_orientation,
-                                                     min_overlap_for_angle, s);
+                                                     min_overlap_for_angle, ch, s);
                         });
 }
 
@@ -762,10 +806,49 @@ int ovn_net_gradients(ovn_handle* h, const float* d_images, int64_t n_images, co
   DeviceGuard guard(h);
   TrainPrecisionScope precision(h);
   cudaStream_t s = (cudaStream_t)stream;
-  return gradients_call(h, true, d_images, n_images, d_left_idx, d_right_idx, n_pairs, d_gt_overlap,
-                        d_gt_orientation, h_loss, s, [&](const int32_t* l, const int32_t* r) {
+  GradChunks ch;
+  return gradients_call(h, true, "ovn_net_gradients", d_images, n_images, d_left_idx, d_right_idx, n_pairs,
+                        d_gt_overlap, d_gt_orientation, ch, h_loss, s, [&](const int32_t* l, const int32_t* r) {
                           return net_gradients_fp32(h, d_images, l, r, n_pairs, d_gt_overlap, d_gt_orientation,
-                                                    min_overlap_for_angle, d_fv_grad, s);
+                                                    min_overlap_for_angle, d_fv_grad, ch, s);
+                        });
+}
+
+int ovn_head_gradients_chunks(ovn_handle* h, const float* d_bank, int64_t bank_size, const int32_t* d_left_idx,
+                              const int32_t* d_right_idx, int32_t n_pairs, const int32_t* h_chunk_offsets,
+                              int32_t n_chunks, const float* d_gt_overlap, const int32_t* d_gt_orientation,
+                              float min_overlap_for_angle, float* d_parts, float* h_loss, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  TrainPrecisionScope precision(h);
+  cudaStream_t s = (cudaStream_t)stream;
+  const char* fn = "ovn_head_gradients_chunks";
+  GradChunks ch;
+  int rc = chunk_table(h, fn, false, n_pairs, h_chunk_offsets, n_chunks, d_parts, &ch);
+  if (rc != OVN_OK) return rc;
+  return gradients_call(h, false, fn, d_bank, bank_size, d_left_idx, d_right_idx, n_pairs, d_gt_overlap,
+                        d_gt_orientation, ch, h_loss, s, [&](const int32_t* l, const int32_t* r) {
+                          return head_gradients_fp32(h, d_bank, l, r, n_pairs, d_gt_overlap, d_gt_orientation,
+                                                     min_overlap_for_angle, ch, s);
+                        });
+}
+
+int ovn_net_gradients_chunks(ovn_handle* h, const float* d_images, int64_t n_images, const int32_t* d_left_idx,
+                             const int32_t* d_right_idx, int32_t n_pairs, const int32_t* h_chunk_offsets,
+                             int32_t n_chunks, const float* d_gt_overlap, const int32_t* d_gt_orientation,
+                             float min_overlap_for_angle, float* d_parts, float* h_loss, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  TrainPrecisionScope precision(h);
+  cudaStream_t s = (cudaStream_t)stream;
+  const char* fn = "ovn_net_gradients_chunks";
+  GradChunks ch;
+  int rc = chunk_table(h, fn, true, n_pairs, h_chunk_offsets, n_chunks, d_parts, &ch);
+  if (rc != OVN_OK) return rc;
+  return gradients_call(h, true, fn, d_images, n_images, d_left_idx, d_right_idx, n_pairs, d_gt_overlap,
+                        d_gt_orientation, ch, h_loss, s, [&](const int32_t* l, const int32_t* r) {
+                          return net_gradients_fp32(h, d_images, l, r, n_pairs, d_gt_overlap, d_gt_orientation,
+                                                    min_overlap_for_angle, nullptr, ch, s);
                         });
 }
 

@@ -119,6 +119,8 @@ struct TrainState {
   Buffer<float> grad;           // [ParamLayout::n_total]
   Buffer<float> accum;          // [ParamLayout::n_total] Adagrad accumulators
   Buffer<float> loss;           // [3] total, overlap, orientation
+  Buffer<float> chunk_loss;     // [64][3] the losses of each chunk of a *_gradients_chunks call
+  PinnedBuffer<float> chunk_loss_host;
   GradCover grads = kNoGrads;   // set by the last successful ovn_head_gradients / ovn_net_gradients
   // Whole-network training (ovn_net_gradients): allocated on its first call, grown to the batch.  The 2n images
   // of an n-pair batch are LEFT 0..n-1, then RIGHT 0..n-1.
@@ -325,21 +327,36 @@ int heads_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query,
                        const int32_t* d_left, const int32_t* d_right, int n, float* d_overlap,
                        int32_t* d_yaw, float* d_corr, cudaStream_t s);
 
+// The most parts of one ovn_adagrad_step_sum, and the most chunks of one *_gradients_chunks call
+constexpr int kMaxSumParts = 64;
+
+// Where a gradient call leaves its results.  Chunk c is the pairs [off[c], off[c + 1]) of the call: its flat
+// gradients go to grad + c * stride and its losses to loss[3 c .. 3 c + 2] (device), exactly as a call on those
+// pairs alone would compute them.  ovn_head_gradients / ovn_net_gradients are one chunk: off = {0, np},
+// grad = TrainState::grad, loss = TrainState::loss.  An empty chunk is skipped (the caller zeroes its results).
+struct GradChunks {
+  int n = 1;
+  int off[kMaxSumParts + 1] = {};
+  float* grad = nullptr;
+  int64_t stride = 0;
+  float* loss = nullptr;
+  __host__ __device__ int size(int c) const { return off[c + 1] - off[c]; }
+};
+
 // training of the overlap head (network_fp32.cu)
 int train_alloc(ovn_handle* h);
 int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left, const int32_t* right, int np,
                         const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
-                        cudaStream_t s);
+                        const GradChunks& ch, cudaStream_t s);
 // training of the whole network (network_fp32.cu): left / right index the image bank and are bounds-checked
 int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left, const int32_t* right, int np,
                        const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
-                       float* d_fv_grad, cudaStream_t s);
+                       float* d_fv_grad, const GradChunks& ch, cudaStream_t s);
 int net_max_pairs(const ovn_handle* h);   // largest n_pairs of one ovn_net_gradients call (launch grid limits)
 int64_t train_workspace_bytes(const ovn_handle* h, bool whole_network, int np);   // ovn_train_workspace_bytes
 int copy_net_volumes_fp32(ovn_handle* h, float* d_out, cudaStream_t s);
 // The Adagrad step of the heads' (or with whole_network every layer's) prefix of the flat vector, from the
 // weighted sum of d_parts [n_parts][that length]: one launch
-constexpr int kMaxSumParts = 64;
 int adagrad_sum_fp32(ovn_handle* h, bool whole_network, const float* d_parts, int n_parts, const float* h_weights,
                      float lr, cudaStream_t s);
 // yaw augmentation of training images (projection.cu): rows are bounds-checked on the device (kErrBadIndex)

@@ -769,10 +769,14 @@ static int wgrad_gemm(ovn_handle* h, const AOp& a, const float* dY, int Kc, int 
 // Forward of both heads, the losses and the backward of the overlap head for np <= max_batch_pairs pairs
 // (indices already bounds-checked).  Activations kept for the backward: o1 (h->d_o1), x3 = c_conv2 output
 // (h->d_o2), x4 = c_conv3 output (train->x4).  Each buffer is reused for a gradient once it is dead:
-// x4 -> dL/d(pre-act c_conv3), o1 -> dL/do1.  The losses are left in train->loss.
+// x4 -> dL/d(pre-act c_conv3), o1 -> dL/do1.  The losses are left in ch.loss.
+// The forward, every input gradient and every ReLU mask compute each pair on its own, so they run once over all np
+// pairs.  Where the batch enters a sum or a scale -- the losses and dz's 1 / n, the Dense sums over pairs and every
+// split-K weight gradient, whose slices follow its own reduction length -- each chunk runs on its own pairs, one
+// chunk after the other, into its own gradients.  One chunk is the launch sequence of a plain call.
 int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left, const int32_t* right, int np,
                         const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
-                        cudaStream_t s) {
+                        const GradChunks& ch, cudaStream_t s) {
   TrainState& t = *h->train;
   const int Wf = h->cfg.leg_output_width, Cf = kFeatC, sz = h->cfg.conv1size;
   const int base = kMaxLegLayers;
@@ -780,23 +784,35 @@ int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left,
   const ConvSpec& L1 = h->head[0];
   const ConvSpec& L2 = h->head[1];
   const ConvSpec& L3 = h->head[2];
+  const int64_t o1_pair = (int64_t)L2.h_in * L2.w_in * L2.cin, x3_pair = (int64_t)L3.h_in * L3.w_in * L3.cin;
   int K[4], N[4];
   for (int l = 0; l < 4; ++l) head_dims(h, l, &K[l], &N[l]);
   int rc = overlap_head_fp32(h, d_bank, nullptr, left, right, np, t.x4, t.overlap, s);
   if (rc == OVN_OK) rc = corr_forward_fp32(h, d_bank, nullptr, left, right, np, t.yaw, t.corr, s);
   if (rc != OVN_OK) return rc;
-  k_train_loss<<<1, 256, 0, s>>>(t.overlap, t.corr, d_gt_overlap, d_gt_orientation, np, Wf, min_overlap, t.dz,
-                                 t.grad + off[3] + K[3], t.loss);
-  OVN_LAUNCH_CHECK(h);
-  // overlap_output (Dense): dWd, and x4 becomes dL/d(pre-activation of c_conv3)
-  k_dense_backward<<<blocks_for(h->dense_in), 256, 0, s>>>(t.x4, h->d_w[base + 3], t.dz, np, h->dense_in,
-                                                           t.grad + off[3]);
-  OVN_LAUNCH_CHECK(h);
+  for (int c = 0; c < ch.n; ++c) {
+    const int a = ch.off[c], n = ch.size(c);
+    if (n == 0) continue;
+    float* g = ch.grad + c * ch.stride;
+    k_train_loss<<<1, 256, 0, s>>>(t.overlap + a, t.corr + (int64_t)a * Wf, d_gt_overlap + a, d_gt_orientation + a,
+                                   n, Wf, min_overlap, t.dz + a, g + off[3] + K[3], ch.loss + 3 * c);
+    OVN_LAUNCH_CHECK(h);
+    // overlap_output (Dense): dWd, and x4 becomes dL/d(pre-activation of c_conv3)
+    k_dense_backward<<<blocks_for(h->dense_in), 256, 0, s>>>(t.x4 + (int64_t)a * h->dense_in, h->d_w[base + 3],
+                                                             t.dz + a, n, h->dense_in, g + off[3]);
+    OVN_LAUNCH_CHECK(h);
+  }
   // c_conv3: dW3 = patches(x3)^T dpre3 (+ db3), then dx3 = transposed 3x3 conv of dpre3, masked by x3 > 0
   {
-    ConvWgradOperand a{h->d_o2, L3.h_in, L3.w_in, L3.cin, L3.kw, L3.sh, L3.sw, L3.h_out, L3.w_out, K[2]};
-    rc = wgrad_gemm(h, a, t.x4, K[2], N[2], np * L3.h_out * L3.w_out, t.grad + off[2], s);
-    if (rc != OVN_OK) return rc;
+    for (int c = 0; c < ch.n; ++c) {
+      const int a = ch.off[c], n = ch.size(c);
+      if (n == 0) continue;
+      ConvWgradOperand op{h->d_o2 + a * x3_pair, L3.h_in, L3.w_in, L3.cin, L3.kw, L3.sh, L3.sw, L3.h_out, L3.w_out,
+                          K[2]};
+      rc = wgrad_gemm(h, op, t.x4 + (int64_t)a * h->dense_in, K[2], N[2], n * L3.h_out * L3.w_out,
+                      ch.grad + c * ch.stride + off[2], s);
+      if (rc != OVN_OK) return rc;
+    }
     k_swap_io<<<blocks_for((int64_t)K[2] * N[2]), 256, 0, s>>>(h->d_w[base + 2], t.w3t, L3.kh * L3.kw, L3.cin,
                                                                L3.cout);
     OVN_LAUNCH_CHECK(h);
@@ -811,18 +827,27 @@ int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left,
   // c_conv2: dW2 = patches(o1)^T dpre2 (+ db2); do1 = dpre2 W2^T.  Stride = kernel, so every o1 row belongs to
   // exactly one output pixel: do1 is stored per output pixel, [p][ho][wo][dh][c], over the dead o1
   {
-    ConvWgradOperand a{h->d_o1, L2.h_in, L2.w_in, L2.cin, L2.kw, L2.sh, L2.sw, L2.h_out, L2.w_out, K[1]};
-    rc = wgrad_gemm(h, a, t.dx3, K[1], N[1], np * L2.h_out * L2.w_out, t.grad + off[1], s);
-    if (rc != OVN_OK) return rc;
+    for (int c = 0; c < ch.n; ++c) {
+      const int a = ch.off[c], n = ch.size(c);
+      if (n == 0) continue;
+      ConvWgradOperand op{h->d_o1 + a * o1_pair, L2.h_in, L2.w_in, L2.cin, L2.kw, L2.sh, L2.sw, L2.h_out, L2.w_out,
+                          K[1]};
+      rc = wgrad_gemm(h, op, t.dx3 + a * x3_pair, K[1], N[1], n * L2.h_out * L2.w_out,
+                      ch.grad + c * ch.stride + off[1], s);
+      if (rc != OVN_OK) return rc;
+    }
     ConvOperand g{t.dx3, L2.h_out, L2.w_out, L2.cout, 1, 1, 1, L2.h_out, L2.w_out};
     BOperand w2t{h->d_w[base + 1], h->d_w[base + 1], nullptr, 0, 1};     // W2 read as [(dh, c)][n]
     rc = launch_gemm(h, g, w2t, nullptr, h->d_o1, np * L2.h_out * L2.w_out, K[1], L2.cout, 1, 0, s);
     if (rc != OVN_OK) return rc;
   }
   // c_conv1 (linear): dW1[dj, c, o] = sum |L[i, c] - R[15 jb + dj, c]| do1[i, jb, o], db1 = sum do1
-  {
-    DeltaWgradOperand a{d_bank, left, right, Wf, Cf, sz, h->o1_w, L2.h_out, K[0]};
-    rc = wgrad_gemm(h, a, h->d_o1, K[0], N[0], np * L1.h_out * L1.w_out, t.grad + off[0], s);
+  for (int c = 0; c < ch.n; ++c) {
+    const int a = ch.off[c], n = ch.size(c);
+    if (n == 0) continue;
+    DeltaWgradOperand op{d_bank, left + a, right + a, Wf, Cf, sz, h->o1_w, L2.h_out, K[0]};
+    rc = wgrad_gemm(h, op, h->d_o1 + a * o1_pair, K[0], N[0], n * L1.h_out * L1.w_out,
+                    ch.grad + c * ch.stride + off[0], s);
     if (rc != OVN_OK) return rc;
   }
   return OVN_OK;
@@ -849,6 +874,17 @@ __global__ void k_gather_images(const float* __restrict__ images, const int32_t*
 __global__ void k_pair_rows(int32_t* __restrict__ rows, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) rows[i] = i;
+}
+
+// The volume rows of a chunked batch, whose images are chunk after chunk, each [LEFT of its pairs, RIGHT of its
+// pairs] from 2 off[c]: rows[p] = p + off[c] (LEFT of pair p of chunk c), rows[np + p] = p + off[c + 1] (RIGHT)
+__global__ void k_chunk_pair_rows(int32_t* __restrict__ rows, int np, const __grid_constant__ GradChunks ch) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= np) return;
+  int c = 0;
+  while (p >= ch.off[c + 1]) ++c;
+  rows[p] = p + ch.off[c];
+  rows[np + p] = p + ch.off[c + 1];
 }
 
 // dL/d(correlation logit) of the orientation loss of k_train_loss (loss weight 1):
@@ -1206,17 +1242,26 @@ int64_t train_workspace_bytes(const ovn_handle* h, bool whole_network, int np) {
 // heads, the losses, and the backward of the whole network.  The gradients of every layer land in train->grad,
 // the losses in train->loss; d_fv_grad (may be null) receives dL/d(volumes) before s_conv10's ReLU mask,
 // [2][np][Wf][128].
+// With chunks (head_gradients_fp32), the images of chunk c are gathered as a call on its pairs alone gathers them,
+// [LEFT, RIGHT] from image 2 off[c], so that a leg layer's weight gradient of chunk c reduces over the same rows in
+// the same order.  dL/d(volumes), which the head backward leaves as [LEFT][RIGHT] over all pairs, is copied into
+// that order before the leg backward.
 int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left, const int32_t* right, int np,
                        const float* d_gt_overlap, const int32_t* d_gt_orientation, float min_overlap,
-                       float* d_fv_grad, cudaStream_t s) {
+                       float* d_fv_grad, const GradChunks& ch, cudaStream_t s) {
   int rc = net_alloc(h, np);
   if (rc != OVN_OK) return rc;
   TrainState& t = *h->train;
   const int Wf = h->cfg.leg_output_width, n2 = 2 * np, sz = h->cfg.conv1size;
   const int64_t img = (int64_t)h->cfg.proj_H * h->cfg.proj_W * h->C, vol = (int64_t)Wf * kFeatC;
   const int nb = h->o1_w, nit = (Wf + kDgT - 1) / kDgT;
-  k_gather_images<<<blocks_for(n2 * img), 256, 0, s>>>(d_images, left, right, np, img, t.images);
-  OVN_LAUNCH_CHECK(h);
+  for (int c = 0; c < ch.n; ++c) {
+    const int a = ch.off[c], n = ch.size(c);
+    if (n == 0) continue;
+    k_gather_images<<<blocks_for(2 * n * img), 256, 0, s>>>(d_images, left + a, right + a, n, img,
+                                                            t.images + 2 * a * img);
+    OVN_LAUNCH_CHECK(h);
+  }
   // leg forward
   float* act[kMaxLegLayers];
   {
@@ -1244,18 +1289,24 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
   const float* fv = act[h->n_leg - 1];
   t.net_fv_off = fv - t.acts.get();
   t.net_np = np;
-  k_pair_rows<<<blocks_for(n2), 256, 0, s>>>(t.pair_rows, n2);
+  if (ch.n == 1) k_pair_rows<<<blocks_for(n2), 256, 0, s>>>(t.pair_rows, n2);
+  else k_chunk_pair_rows<<<blocks_for(np), 256, 0, s>>>(t.pair_rows, np, ch);
   OVN_LAUNCH_CHECK(h);
   const int32_t* lrow = t.pair_rows;
   const int32_t* rrow = t.pair_rows + np;
   // both heads forward, losses, overlap-head backward: do1 = dL/d(c_conv1 output) is left in h->d_o1
-  rc = head_gradients_fp32(h, fv, lrow, rrow, np, d_gt_overlap, d_gt_orientation, min_overlap, s);
+  rc = head_gradients_fp32(h, fv, lrow, rrow, np, d_gt_overlap, d_gt_orientation, min_overlap, ch, s);
   if (rc != OVN_OK) return rc;
   // dL/d(volumes) = correlation-head part + |l - r| part
   float* dfv = t.dact[0];
-  k_corr_dlogit<<<blocks_for((int64_t)np * Wf), 256, 0, s>>>(t.corr, d_gt_overlap, d_gt_orientation, np, Wf,
-                                                              min_overlap, t.dcorr);
-  OVN_LAUNCH_CHECK(h);
+  for (int c = 0; c < ch.n; ++c) {            // the orientation loss's 1 / (n Wf) is the chunk's
+    const int a = ch.off[c], n = ch.size(c);
+    if (n == 0) continue;
+    k_corr_dlogit<<<blocks_for((int64_t)n * Wf), 256, 0, s>>>(t.corr + (int64_t)a * Wf, d_gt_overlap + a,
+                                                               d_gt_orientation + a, n, Wf, min_overlap,
+                                                               t.dcorr + (int64_t)a * Wf);
+    OVN_LAUNCH_CHECK(h);
+  }
   k_corr_backward<<<dim3((Wf + kCorrRows - 1) / kCorrRows, np, 2), kFeatC, Wf * sizeof(float), s>>>(
       t.dcorr, fv, lrow, rrow, np, Wf, dfv);
   OVN_LAUNCH_CHECK(h);
@@ -1281,15 +1332,34 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
   // leg backward: dy = dL/d(pre-activation of layer l), then its weight + bias gradient and its input gradient
   float* dy = dfv;
   float* dx = t.dact[1];
+  if (ch.n > 1) {                             // into the images' order: chunk after chunk, LEFT then RIGHT
+    for (int c = 0; c < ch.n; ++c) {
+      const int64_t a = ch.off[c], n = ch.size(c);
+      if (n == 0) continue;
+      OVN_CUDA(h, cudaMemcpyAsync(dx + 2 * a * vol, dfv + a * vol, (size_t)(n * vol) * sizeof(float),
+                                  cudaMemcpyDeviceToDevice, s));
+      OVN_CUDA(h, cudaMemcpyAsync(dx + (2 * a + n) * vol, dfv + (np + a) * vol, (size_t)(n * vol) * sizeof(float),
+                                  cudaMemcpyDeviceToDevice, s));
+    }
+    dy = dx;
+    dx = dfv;
+  }
   k_relu_grad<<<blocks_for(n2 * vol), 256, 0, s>>>(dy, fv, n2 * vol);
   OVN_LAUNCH_CHECK(h);
   for (int l = h->n_leg - 1; l >= 0; --l) {
     const ConvSpec& L = h->leg[l];
     const float* X = l ? act[l - 1] : t.images;
     const int Kc = L.kh * L.kw * L.cin;
-    ConvWgradOperand a{X, L.h_in, L.w_in, L.cin, L.kw, L.sh, L.sw, L.h_out, L.w_out, Kc};
-    rc = wgrad_gemm(h, a, dy, Kc, L.cout, n2 * L.h_out * L.w_out, t.grad + h->params.off[l], s);
-    if (rc != OVN_OK) return rc;
+    const int64_t in_img = (int64_t)L.h_in * L.w_in * L.cin, out_img = (int64_t)L.h_out * L.w_out * L.cout;
+    for (int c = 0; c < ch.n; ++c) {
+      const int64_t a = ch.off[c];
+      const int n = ch.size(c);
+      if (n == 0) continue;
+      ConvWgradOperand op{X + 2 * a * in_img, L.h_in, L.w_in, L.cin, L.kw, L.sh, L.sw, L.h_out, L.w_out, Kc};
+      rc = wgrad_gemm(h, op, dy + 2 * a * out_img, Kc, L.cout, 2 * n * L.h_out * L.w_out,
+                      ch.grad + c * ch.stride + h->params.off[l], s);
+      if (rc != OVN_OK) return rc;
+    }
     if (l == 0) break;
     k_swap_io<<<blocks_for(h->params.n_kernel[l]), 256, 0, s>>>(h->d_w[l], t.wt, L.kh * L.kw, L.cin, L.cout);
     OVN_LAUNCH_CHECK(h);

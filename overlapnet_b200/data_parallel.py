@@ -28,6 +28,20 @@ def shares(n, world):
   return bounds, [(hi - lo) / float(n) for lo, hi in bounds]
 
 
+def chunk_plan(n, n_chunks, world, rank):
+  """A batch of n pairs cut into n_chunks contiguous chunks (``shares(n, n_chunks)``), of which each rank trains a
+  contiguous range of chunks (``shares(n_chunks, world)``; n_chunks >= world).  Returns the chunk bounds, the chunk
+  weights n_k / n, ``rank``'s chunk range (c0, c1) and the pairs [a, b) of the batch it covers."""
+  bounds, weights = shares(n, n_chunks)
+  c0, c1 = shard_range(n_chunks, rank, world)
+  return bounds, weights, (c0, c1), (bounds[c0][0], bounds[c1 - 1][1])
+
+
+def chunk_rows(n_chunks, world):
+  """The most chunks one rank trains, ceil(n_chunks / world): the rows each rank adds to the all-gathered parts."""
+  return -(-n_chunks // world)
+
+
 class DataParallel:
   """Rank, world size and the collectives of the training loop.  NCCL moves device tensors; on gloo they are
   staged through host memory."""

@@ -456,6 +456,45 @@ class Engine:
           'ovn_copy_gradients')
     return out
 
+  def _gradients_chunks(self, fn, rows, left_idx, right_idx, offsets, gt_overlap, gt_orientation,
+                        min_overlap_for_angle, whole_network, out):
+    n = left_idx.numel()
+    dev = self.device
+    li = left_idx.to(device=dev, dtype=torch.int32).contiguous()
+    ri = right_idx.to(device=dev, dtype=torch.int32).contiguous()
+    gov = torch.as_tensor(gt_overlap).to(device=dev, dtype=torch.float32).contiguous()
+    gor = torch.as_tensor(gt_orientation).to(device=dev, dtype=torch.int32).contiguous()
+    assert ri.numel() == n and gov.numel() == n and gor.numel() == n
+    off = np.ascontiguousarray(offsets, np.int32).reshape(-1)
+    k = max(off.size - 1, 0)
+    size = self.gradient_size(whole_network)
+    if out is None:
+      out = torch.empty((max(k, 1), size), dtype=torch.float32, device=dev)
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.device == dev and out.numel() >= k * size
+    loss = np.zeros((max(k, 1), 3), np.float32)
+    check(self._h, getattr(lib(), fn)(self._h, _ptr(rows), int(rows.shape[0]), _ptr(li), _ptr(ri), n,
+                                      off.ctypes.data_as(C.c_void_p), k, _ptr(gov), _ptr(gor),
+                                      float(min_overlap_for_angle), _ptr(out), loss.ctypes.data_as(C.c_void_p),
+                                      self._stream()), fn)
+    return [tuple(float(v) for v in row) for row in loss[:k]], out
+
+  def head_gradients_chunks(self, bank, left_idx, right_idx, offsets, gt_overlap, gt_orientation,
+                            min_overlap_for_angle=0.7, out=None):
+    """ovn_head_gradients_chunks: head_gradients + copy_gradients of each chunk [offsets[c], offsets[c + 1]) of the
+    pairs, in one call.  Returns the losses of each chunk and the parts [n_chunks, gradient_size(False)] (written
+    into ``out`` when given).  Leaves no gradients in the handle."""
+    return self._gradients_chunks('ovn_head_gradients_chunks', bank, left_idx, right_idx, offsets, gt_overlap,
+                                  gt_orientation, min_overlap_for_angle, False, out)
+
+  def net_gradients_chunks(self, images, left_idx, right_idx, offsets, gt_overlap, gt_orientation,
+                           min_overlap_for_angle=0.7, out=None):
+    """ovn_net_gradients_chunks: net_gradients + copy_gradients of each chunk of the pairs, in one call.  Returns
+    the losses of each chunk and the parts [n_chunks, gradient_size(True)]."""
+    x = images.contiguous()
+    assert tuple(x.shape[1:]) == (self.H, self.W, self.C) and x.dtype == torch.float32
+    return self._gradients_chunks('ovn_net_gradients_chunks', x, left_idx, right_idx, offsets, gt_overlap,
+                                  gt_orientation, min_overlap_for_angle, True, out)
+
   def adagrad_step_sum(self, parts, weights, lr, whole_network=False):
     """ovn_adagrad_step_sum: one Adagrad step with g = sum_k weights[k] parts[k] (in order, float32, weight-0
     parts skipped).  ``parts`` [n_parts, gradient_size] float32 cuda, ``weights`` n_parts floats."""

@@ -27,20 +27,34 @@ def image_bytes(eng):
   return eng.H * eng.W * eng.C * 4
 
 
-def share_pairs(n_pairs, world):
-  """The largest share of an n_pairs batch that one of ``world`` data-parallel ranks trains."""
-  bounds, _ = data_parallel.shares(n_pairs, world)
-  return max(hi - lo for lo, hi in bounds)
+def share_pairs(n_pairs, world, gradient_chunks=None):
+  """The largest share of an n_pairs batch that one of ``world`` data-parallel ranks trains; with gradient_chunks K
+  the largest sum of the chunks of one rank's chunk range (data_parallel.chunk_plan).  A full batch has the
+  largest chunks: a shorter one only makes some of them smaller."""
+  if gradient_chunks is None:
+    bounds, _ = data_parallel.shares(n_pairs, world)
+    return max(hi - lo for lo, hi in bounds)
+  return max(b - a for a, b in (data_parallel.chunk_plan(n_pairs, gradient_chunks, world, r)[3] for r in range(world)))
 
 
-def working_set_bytes(eng, b_share, whole_network, gathered, features):
+def parts_bytes(eng, whole_network, world, gradient_chunks=None):
+  """Device bytes of the per-chunk gradients of a step with gradient_chunks K: world ceil(K / world) all-gathered
+  parts, and with more than one rank ceil(K / world) local ones; 0 without chunks."""
+  if gradient_chunks is None:
+    return 0
+  m = data_parallel.chunk_rows(gradient_chunks, world)
+  return (world * m + (m if world > 1 else 0)) * eng.gradient_size(whole_network) * 4
+
+
+def working_set_bytes(eng, b_share, whole_network, gathered, features, parts=0):
   """Device bytes a training run needs besides its image bank, from the shapes of its largest step of
   ``b_share`` pairs: the handle's training buffers (Engine.train_workspace_bytes: for the whole network the leg
   activations of 2 b_share images, the split-K partials, the head buffers), the staging ring (two slots of
   2 b_share images), ``gathered`` images of a step's gathered batch (yaw augmentation), ``features`` feature volumes
-  (the validation feature bank, the frozen leg's bank) and MARGIN_BYTES."""
+  (the validation feature bank, the frozen leg's bank), ``parts`` bytes of per-chunk gradients (parts_bytes) and
+  MARGIN_BYTES."""
   return (eng.train_workspace_bytes(b_share, whole_network) + 2 * 2 * b_share * image_bytes(eng)
-          + gathered * image_bytes(eng) + features * eng.Wf * FEAT_C * 4 + MARGIN_BYTES)
+          + gathered * image_bytes(eng) + features * eng.Wf * FEAT_C * 4 + int(parts) + MARGIN_BYTES)
 
 
 def choose_placement(bank_bytes, free_bytes, working_set):
@@ -182,7 +196,7 @@ class StagingRing:
     return out
 
 
-def open_bank(infer, keys, image_bank, b_share, whole_network, gathered, features, what):
+def open_bank(infer, keys, image_bank, b_share, whole_network, gathered, features, what, parts=0):
   """The image bank of the distinct (dir, scan) ``keys``: ``image_bank`` None chooses its placement from the free
   device memory and the working set (working_set_bytes), 'device' or 'host' forces it.  Returns (placement, the
   device tensor or HostBank, {key: row}).  ``what`` names the bank in the log."""
@@ -194,7 +208,7 @@ def open_bank(infer, keys, image_bank, b_share, whole_network, gathered, feature
   bank_bytes = n * image_bytes(eng)
   placement = image_bank
   if placement is None:
-    ws = working_set_bytes(eng, b_share, whole_network, gathered, features)
+    ws = working_set_bytes(eng, b_share, whole_network, gathered, features, parts)
     placement, budget = choose_placement(bank_bytes, free_device_bytes(eng), ws)
     logger.info('%s: %d scans, %.1f MB; device budget %.1f MB (free memory minus a working set of %.1f MB): '
                 'on the %s', what, n, bank_bytes / 1e6, budget / 1e6, ws / 1e6,

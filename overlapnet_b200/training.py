@@ -34,6 +34,13 @@ Both flows train data-parallel over the GPUs of a node (overlapnet_b200.data_par
 ``batch_size`` stays the global batch; each rank trains on a contiguous share of every batch, and the ranks'
 gradients are all-gathered and summed in rank order on the device, so every rank keeps the same weights.
 
+``gradient_chunks: K`` (both legsTypes, 1 <= K <= min(64, batch_size), K >= the world size; default off) makes the
+bits independent of the world size: every batch of n pairs is cut into K contiguous chunks, each rank computes the
+gradients of its contiguous range of chunks in one call (Engine.head_gradients_chunks / net_gradients_chunks), and
+g = sum_k (n_k / n) g_k is summed in chunk order.  A run with the key gives the same weights, accumulators, history
+and checkpoints on any number of GPUs up to K, and may be resumed on another; K = 1 on one GPU is the run without
+the key.
+
 ``checkpoint: True`` (both legsTypes, default False) writes ``<experiments_path>/<testname>/checkpoint.npz`` after
 every epoch, atomically: the weights, the Adagrad accumulators (Engine.train_state), NumPy's random state, the
 training pairs in the run's order, the history so far and a fingerprint of the config keys that fix the
@@ -89,6 +96,27 @@ def check_config(config):
 
 
 TRAINING_PRECISIONS = ('fp32', 'tf32x3')
+MAX_GRADIENT_CHUNKS = 64             # the most parts of one ovn_adagrad_step_sum
+
+
+def check_gradient_chunks(config, world=1):
+  """``gradient_chunks: K`` (both legsTypes, default off): each batch's gradient is the weighted sum of the
+  gradients of K fixed chunks, so that the run's bits do not depend on the world size.  Returns K, or None without
+  the key; raises an Exception that names the problem for a K the loop cannot train on ``world`` ranks."""
+  if 'gradient_chunks' not in config:
+    return None
+  k = config['gradient_chunks']
+  if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or k < 1:
+    raise Exception('gradient_chunks %r is not an integer >= 1' % (k,))
+  k = int(k)
+  if k > MAX_GRADIENT_CHUNKS:
+    raise Exception('gradient_chunks %d exceeds %d, the most parts one Adagrad step sums' % (k, MAX_GRADIENT_CHUNKS))
+  batch_size = int(config['batch_size'])
+  if k > batch_size:
+    raise Exception('gradient_chunks %d exceeds batch_size %d: a full batch would have empty chunks' % (k, batch_size))
+  if k < world:
+    raise Exception('gradient_chunks %d is below the world size %d: every rank trains at least one chunk' % (k, world))
+  return k
 
 
 def check_training_precision(config):
@@ -182,6 +210,8 @@ def trajectory_fingerprint(config):
     fp.update(training_seqs=str(config['training_seqs']), traindata_npzfile=None)
   else:
     fp.update(training_seqs=None, traindata_npzfile=config['traindata_npzfile'])
+  if 'gradient_chunks' in config:          # only with the key, so that the fingerprints of other runs stay
+    fp.update(gradient_chunks=config['gradient_chunks'])
   return _plain(fp)
 
 
@@ -294,10 +324,11 @@ class FrozenLeg:
   """The training step of 360OutputkLegsFixed: every distinct scan is encoded once by the frozen leg into a
   feature bank on the GPU; a step trains the overlap head on it."""
 
-  def __init__(self, infer, keys, rotate_keys=None, image_bank=None):
+  def __init__(self, infer, keys, rotate_keys=None, image_bank=None, gradient_chunks=None):
     """``image_bank`` (yaw augmentation only: without it there is no image bank) None places the RIGHT scans'
     images on the GPU when they fit beside the largest step's working set and in pinned host memory otherwise
-    (overlapnet_b200.image_bank); 'device' or 'host' forces a placement.  Both train the same bits."""
+    (overlapnet_b200.image_bank); 'device' or 'host' forces a placement.  Both train the same bits.
+    ``gradient_chunks`` (the config key) sizes that working set for a rank's largest chunk range."""
     logger.info('Encoding %d scans with the frozen leg ...', len(keys))
     self.eng = infer._engine
     self.bank, self.rows = _encode_bank(infer, keys)
@@ -307,10 +338,12 @@ class FrozenLeg:
       # bank that receive a step's rotated RIGHT volumes.
       from . import image_bank as _image_bank
       dp = data_parallel.default_group()
-      b_share = _image_bank.share_pairs(self.eng.max_batch_pairs, 1 if dp is None else dp.world)
+      world = 1 if dp is None else dp.world
+      b_share = _image_bank.share_pairs(self.eng.max_batch_pairs, world, gradient_chunks)
       n, B = len(self.rows), self.eng.max_batch_scans
       self.image_bank, self.images, self.image_rows = _image_bank.open_bank(
-          infer, rotate_keys, image_bank, b_share, False, b_share, n + B, 'Image bank of the rotated RIGHT scans')
+          infer, rotate_keys, image_bank, b_share, False, b_share, n + B, 'Image bank of the rotated RIGHT scans',
+          _image_bank.parts_bytes(self.eng, False, world, gradient_chunks))
       if self.image_bank == 'host':
         self.ring = _image_bank.StagingRing(self.eng, self.images, 2 * b_share)
       self.bank = torch.cat([self.bank, self.bank.new_empty((B,) + tuple(self.bank.shape[1:]))])
@@ -331,8 +364,10 @@ class FrozenLeg:
     self.eng.adagrad_step(lr)
     return loss
 
-  def gradients(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, rotate=None):
-    """``step`` without its update: the losses; the gradients stay in the handle (the data-parallel step)."""
+  def gradients(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, rotate=None, chunks=None):
+    """``step`` without its update: the losses; the gradients stay in the handle (the data-parallel step).
+    ``chunks`` = (offsets, parts): the gradients of each chunk [offsets[c], offsets[c + 1]) of the pairs go to
+    parts[c] in one call (Engine.head_gradients_chunks), and the losses of each chunk are returned."""
     if rotate is not None:
       rows, shifts, rot = rotate
       images = self.images
@@ -344,6 +379,9 @@ class FrozenLeg:
         self.ring.release()
       self.eng.leg(x, out=self.bank[n0:n0 + n])
       right = self.scratch[:n]
+    if chunks is not None:
+      return self.eng.head_gradients_chunks(self.bank, left, right, chunks[0], gt_overlap, gt_orientation,
+                                            min_overlap_for_angle, out=chunks[1])[0]
     return self.eng.head_gradients(self.bank, left, right, gt_overlap, gt_orientation, min_overlap_for_angle)
 
   def evaluate(self, left, right):
@@ -399,6 +437,8 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
   no_test_pairs = int(config['no_test_pairs'])
   min_overlap_for_angle = float(config.get('min_overlap_for_angle', 0.7))
   yaw_augmentation = bool(config.get('yaw_augmentation', False))
+  world, rank = (1, 0) if dp is None else (dp.world, dp.rank)
+  gradient_chunks = check_gradient_chunks(config, world)
   resume = bool(config.get('resume', False))
   checkpoint = resume or bool(config.get('checkpoint', False))
   checkpoint_path = os.path.join(out_dir, CHECKPOINT)
@@ -448,7 +488,8 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
       eng.load_weights(start)
 
   keys = set(zip(t_d1, t_f1)) | set(zip(t_d2, t_f2)) | set(zip(v_d1, v_f1)) | set(zip(v_d2, v_f2))
-  steps = flow(infer, keys, set(zip(t_d2, t_f2))) if yaw_augmentation else flow(infer, keys)
+  chunk_kw = {} if gradient_chunks is None else {'gradient_chunks': gradient_chunks}
+  steps = flow(infer, keys, set(zip(t_d2, t_f2)), **chunk_kw) if yaw_augmentation else flow(infer, keys, **chunk_kw)
   rows = steps.rows
   dev = eng.device
   t_left = torch.tensor([rows[k] for k in zip(t_d1, t_f1)], dtype=torch.int32, device=dev)
@@ -476,7 +517,17 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
     right_h = np.asarray([steps.image_rows[k] for k in zip(t_d2, t_f2)], np.int64)
     left_h = np.asarray([steps.image_rows[k] for k in zip(t_d1, t_f1)], np.int64) if steps.whole_network else None
     t_rows_h = (left_h, right_h, right_h if yaw_augmentation else None)
-  if dp is not None:
+  if gradient_chunks is not None:
+    m = data_parallel.chunk_rows(gradient_chunks, world)
+    size = eng.gradient_size(steps.whole_network)
+    parts = torch.empty((world * m, size), dtype=torch.float32, device=dev)
+    local = parts if dp is None else torch.empty((m, size), dtype=torch.float32, device=dev)
+    ranges = data_parallel.shares(gradient_chunks, world)[0]
+    logger.info('  gradient chunks: %d per batch, summed in chunk order; chunk ranges by rank: %s', gradient_chunks,
+                ', '.join('%d: [%d, %d)' % (r, c0, c1) for r, (c0, c1) in enumerate(ranges)))
+    if dp is not None:
+      logger.info('  data-parallel over %d ranks: each step all-gathers %d x %d gradients per rank', world, m, size)
+  elif dp is not None:
     whole = steps.whole_network
     grad = torch.zeros((eng.gradient_size(whole),), dtype=torch.float32, device=dev)
     parts = torch.empty((dp.world, grad.numel()), dtype=torch.float32, device=dev)
@@ -509,13 +560,20 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
       spans = []
       for b in perm:
         s0, s1 = b * batch_size, min(n, (b + 1) * batch_size)
-        lo, hi = (0, s1 - s0) if dp is None else data_parallel.shares(s1 - s0, dp.world)[0][dp.rank]
+        if gradient_chunks is not None:
+          lo, hi = data_parallel.chunk_plan(s1 - s0, gradient_chunks, world, rank)[3]
+        else:
+          lo, hi = (0, s1 - s0) if dp is None else data_parallel.shares(s1 - s0, dp.world)[0][dp.rank]
         if hi > lo:
           spans.append((s0 + lo, s0 + hi))
       steps.begin_epoch(spans, *t_rows_h)
     for b in perm:
       s0, s1 = b * batch_size, min(n, (b + 1) * batch_size)
-      if dp is not None:
+      if gradient_chunks is not None:
+        loss = _chunked_step(dp, steps, eng, gradient_chunks, parts, local, s0, s1, t_left, t_right, t_ov_d,
+                             t_or_epoch, min_overlap_for_angle, lr,
+                             (t_right_img, shifts_d, rot_d) if yaw_augmentation else None)
+      elif dp is not None:
         loss = _data_parallel_step(dp, steps, eng, grad, parts, s0, s1, t_left, t_right, t_ov_d, t_or_epoch,
                                    min_overlap_for_angle, lr,
                                    (t_right_img, shifts_d, rot_d) if yaw_augmentation else None)
@@ -591,6 +649,40 @@ def _data_parallel_step(dp, steps, eng, grad, parts, s0, s1, t_left, t_right, t_
   eng.adagrad_step_sum(parts, weights, lr, steps.whole_network)
   all_losses = dp.gather_rows(np.asarray([loss], np.float64), [1] * dp.world)
   return tuple(float(sum(w * l[k] for w, l in zip(weights, all_losses))) for k in range(3))
+
+
+def _chunked_step(dp, steps, eng, n_chunks, parts, local, s0, s1, t_left, t_right, t_ov, t_or, min_overlap_for_angle,
+                  lr, rotate):
+  """One step of the global batch [s0, s1) cut into n_chunks chunks (``gradient_chunks``), on one process or on
+  every rank of ``dp``: this rank's chunk range in one gradient call into ``local`` [ceil(K / world), n]; with
+  several ranks the parts all-gathered into ``parts`` [world ceil(K / world), n] and moved into chunk order; then
+  the Adagrad step of g = sum_k (n_k / n) g_k over parts[:K].  Each g_k is what a call on chunk k alone computes, so
+  the step does not depend on how the chunks are spread over ranks.  Returns the batch loss sum_k (n_k / n) loss_k
+  (float64, chunk order)."""
+  world, rank = (1, 0) if dp is None else (dp.world, dp.rank)
+  bounds, weights, (c0, c1), (a, b) = data_parallel.chunk_plan(s1 - s0, n_chunks, world, rank)
+  a, b = s0 + a, s0 + b
+  mine = local[:c1 - c0]
+  losses = [(0.0, 0.0, 0.0)] * (c1 - c0)
+  if b > a:
+    offsets = [bounds[c][0] - bounds[c0][0] for c in range(c0, c1)] + [b - a]
+    chunk_rotate = None if rotate is None else tuple(t[a:b] for t in rotate)
+    losses = steps.gradients(t_left[a:b], t_right[a:b], t_ov[a:b], t_or[a:b], min_overlap_for_angle, chunk_rotate,
+                             chunks=(offsets, mine))
+  else:                                                            # every chunk empty: weight 0, skipped by the sum
+    mine.zero_()
+  losses = np.asarray(losses, np.float64).reshape(c1 - c0, 3)
+  if dp is not None:
+    m = local.shape[0]
+    dp.gather_flat(local.reshape(-1), parts.view(world, -1))
+    ranges = data_parallel.shares(n_chunks, world)[0]
+    for r, (d0, d1) in enumerate(ranges):          # rank r's rows [r m, r m + d1 - d0) to chunks [d0, d1)
+      for j in range(d1 - d0):                     # d0 <= r m: a row never lands on one still to be read
+        if d0 + j != r * m + j:
+          parts[d0 + j].copy_(parts[r * m + j])
+    losses = dp.gather_rows(losses, [d1 - d0 for d0, d1 in ranges])
+  eng.adagrad_step_sum(parts[:n_chunks], weights, lr, steps.whole_network)
+  return tuple(float(sum(w * l[k] for w, l in zip(weights, losses))) for k in range(3))
 
 
 def main(argv=None):

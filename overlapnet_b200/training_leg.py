@@ -79,12 +79,14 @@ class WholeNetwork:
   fits beside the largest step's working set and in pinned host memory otherwise (overlapnet_b200.image_bank);
   'device' or 'host' forces a placement.  Both train the same bits."""
 
-  def __init__(self, infer, keys, rotate_keys=None, image_bank=None):
+  def __init__(self, infer, keys, rotate_keys=None, image_bank=None, gradient_chunks=None):
     self.eng = infer._engine
     dp = data_parallel.default_group()
-    b_share = _image_bank.share_pairs(self.eng.max_batch_pairs, 1 if dp is None else dp.world)
+    world = 1 if dp is None else dp.world
+    b_share = _image_bank.share_pairs(self.eng.max_batch_pairs, world, gradient_chunks)
     self.image_bank, self.images, self.rows = _image_bank.open_bank(
-        infer, keys, image_bank, b_share, True, 2 * b_share if rotate_keys else 0, len(set(keys)), 'Image bank')
+        infer, keys, image_bank, b_share, True, 2 * b_share if rotate_keys else 0, len(set(keys)), 'Image bank',
+        _image_bank.parts_bytes(self.eng, True, world, gradient_chunks))
     self.image_rows = self.rows
     if self.image_bank == 'device':
       logger.info('Loaded %d scans into the image bank (%.1f MB on the GPU)', len(self.rows),
@@ -109,10 +111,12 @@ class WholeNetwork:
     self.eng.net_adagrad_step(lr)
     return loss
 
-  def gradients(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, rotate=None):
+  def gradients(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, rotate=None, chunks=None):
     """``step`` without its update: the losses; the gradients stay in the handle (the data-parallel step).  With
     a host bank, ``left``, ``right`` and the rows of ``rotate`` are the next span begin_epoch planned: the step
-    reads their images from the ring's slot, at the local indices of that plan."""
+    reads their images from the ring's slot, at the local indices of that plan.  ``chunks`` = (offsets, parts):
+    the gradients of each chunk [offsets[c], offsets[c + 1]) of the pairs go to parts[c] in one call
+    (Engine.net_gradients_chunks), and the losses of each chunk are returned."""
     images = self.images
     if self.ring is not None:
       images, (left, second) = self.ring.take()
@@ -132,6 +136,9 @@ class WholeNetwork:
         self.eng.gather_images(src, rows, shifts, rot, out=images[n:])
         pairs = torch.arange(2 * n, dtype=torch.int32, device=self.eng.device)
         left, right = pairs[:n], pairs[n:]
+      if chunks is not None:
+        return self.eng.net_gradients_chunks(images, left, right, chunks[0], gt_overlap, gt_orientation,
+                                             min_overlap_for_angle, out=chunks[1])[0]
       return self.eng.net_gradients(images, left, right, gt_overlap, gt_orientation, min_overlap_for_angle)
     finally:
       if self.ring is not None:
