@@ -20,6 +20,8 @@
  *     feature bank, SURVEY 8b "Threading").
  *   - Feature volumes cross the ABI as float32 [n][W_out=360][128] (what
  *     Infer.create_feature_volumes returns, infer.py:240-265, with the singleton H axis dropped).
+ *   - ovn_copy_heads_stage reads back the intermediate stages of the tensor-core heads (tests and
+ *     diagnostics only; the heads calls do no extra work for it).
  */
 #ifndef OVN_B200_H_
 #define OVN_B200_H_
@@ -373,14 +375,17 @@ int ovn_get_weights(ovn_handle* h, const char* layer_name, float* h_kernel, floa
 int ovn_get_gradients(ovn_handle* h, const char* layer_name, float* h_kernel, float* h_bias);
 
 /* ---- deferred device errors ------------------------------------------------------------------
- * The device-pointer entry points never synchronise, so two classes of error can only be detected on
+ * The device-pointer entry points never synchronise, so three classes of error can only be detected on
  * the device: an index outside [0, bank_size) (or, for a resident bank, a row that was never
- * prepared), and a bounded pipeline-barrier wait of a tensor-core kernel that timed out (GPU
- * time-slicing, debuggers).  Both raise a flag on the device; the kernels that write overlap / yaw
+ * prepared), a volume value the fp16 operands of the tensor-core heads cannot hold (NaN, inf, or more
+ * than 65504 away from the feature centre; raised by every heads call that reads such a volume -- a
+ * resident bank row keeps its mark from ovn_bank_prepare until it is prepared again), and a bounded
+ * pipeline-barrier wait of a tensor-core kernel that timed out (GPU time-slicing, debuggers).  Each raises
+ * a flag on the device; the kernels that write overlap / yaw
  * then POISON their outputs (overlap = NaN, yaw = INT32_MIN) so garbage never looks valid, indices are
  * clamped so no out-of-bounds read happens, and the flag is turned into a status by the next entry point
  * that synchronises anyway: ovn_check (synchronises `stream`), the *_host entry points and
- * ovn_profile_read.  OVN_ERR_INVALID_ARG for index errors, OVN_ERR_CUDA for time-outs; the flag is
+ * ovn_profile_read.  OVN_ERR_INVALID_ARG for index and value errors, OVN_ERR_CUDA for time-outs; the flag is
  * cleared when it is reported. */
 int ovn_check(ovn_handle* h, void* stream);
 
@@ -411,6 +416,32 @@ int ovn_get_feature_center(ovn_handle* h, float* h_mu /* [128] */, int32_t* is_s
  * the handle sees, or the one given here: ovn_calibrate(h, d_volume [360][128]) makes the calibration
  * explicit, so that handles on different GPUs (a sharded bank) produce bit-identical results. */
 int ovn_calibrate(ovn_handle* h, const float* d_volume, void* stream);
+
+/* ---- intermediate stages of the tensor-core heads (tests and diagnostics) -------------------------
+ * The stages are what the last chunk of the last heads call (ovn_heads_forward, ovn_heads_1vsN,
+ * ovn_heads_rows_vs_bank, ovn_query_cloud_vs_bank_host; a chunk is at most max_batch_pairs pairs) left in
+ * the handle.  ovn_heads_stage_pairs: *n_pairs = the pairs of that chunk, 0 when there are none (before the
+ * first heads call, after a calibration -- ovn_calibrate or the one a first ovn_bank_prepare runs -- which
+ * overwrites o1 and x3, and after a heads call that returned an error).  ovn_copy_heads_stage: d_out (float32,
+ * device) = pairs [first, first + count) of one stage, exactly count x the per-pair size below (CENTRES:
+ * first and count are ignored); pairs outside [0, n_pairs) are OVN_ERR_INVALID_ARG.  A plain copy and
+ * conversion of the stored values, asynchronous on `stream`:
+ *   OVN_STAGE_O1      [count][Wf=360][24][64] (i, jb, o): the fp16 c_conv1 output k_delta_conv1_wgmma stored,
+ *                     without the c_conv1 bias and minus the o1 centre
+ *   OVN_STAGE_X3      [count][24][24][128] (ib, jb, c): the fp16 ReLU(c_conv2) minus the x3 centre
+ *   OVN_STAGE_DENSE   [count][24][24][2] (ib, jb, half): the Dense(1) partial sum of each c_conv3 output pixel
+ *                     over output channels [128 half, 128 half + 128); exactly 0 where ib or jb >= 22
+ *   OVN_STAGE_CENTRES [64 + 128 + 128 + 256]: o1 centre, x3 centre, c_conv2 bias with both centres folded in
+ *                     (b2eff), c_conv3 bias with the x3 centre folded in (b3eff)
+ * Both return OVN_ERR_BAD_CONFIG on a precision fp32 handle.  The heads calls do no extra work for this. */
+typedef enum ovn_heads_stage {
+  OVN_STAGE_O1 = 0,
+  OVN_STAGE_X3 = 1,
+  OVN_STAGE_DENSE = 2,
+  OVN_STAGE_CENTRES = 3
+} ovn_heads_stage;
+int ovn_heads_stage_pairs(ovn_handle* h, int64_t* n_pairs);
+int ovn_copy_heads_stage(ovn_handle* h, int32_t stage, int64_t first, int64_t count, float* d_out, void* stream);
 
 /* ---- host-buffer convenience entry points (what a non-CUDA caller binds; bench.py e2e) ------ */
 /* Raw clouds on the host -> feature volumes on the host. */

@@ -26,4 +26,7 @@ gt.py          NumPy restatement of the ground-truth generator ``src/utils/com_o
                (tools/make_golden_gt.py -> tests/golden/gt_overlap_yaw.npz).
 infer_ref.py   restatement of the ``Infer`` class call semantics (``infer.py:22-265``) on top of
                projection.py + network.py.
+tc_heads.py    float64 model of the tensor-core heads (precision f16_tc) stage by stage, with the
+               kernels' fp16 roundings and a per-element bound for each stage; with the roundings
+               switched off its stages chain to network.py exactly (tests/test_oracle_tc_heads.py).
 """

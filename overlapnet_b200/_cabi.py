@@ -26,8 +26,10 @@ SYMBOLS = [
     'ovn_train_gradient_size', 'ovn_copy_gradients', 'ovn_adagrad_step_sum', 'ovn_set_train_precision',
     'ovn_copy_net_volumes', 'ovn_copy_train_state', 'ovn_set_train_state',
     'ovn_train_workspace_bytes', 'ovn_host_register', 'ovn_host_unregister', 'ovn_stage_rows',
-    'ovn_head_gradients_chunks', 'ovn_net_gradients_chunks',
+    'ovn_head_gradients_chunks', 'ovn_net_gradients_chunks', 'ovn_copy_heads_stage',
+    'ovn_heads_stage_pairs',
 ]
+HEADS_STAGES = {'o1': 0, 'x3': 1, 'dense': 2, 'centres': 3}     # ovn_heads_stage
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
 
 
@@ -100,6 +102,8 @@ def lib():
   L.ovn_set_feature_center.argtypes = [vp, vp]
   L.ovn_get_feature_center.argtypes = [vp, vp, C.POINTER(i32)]
   L.ovn_calibrate.argtypes = [vp, vp, vp]
+  L.ovn_copy_heads_stage.argtypes = [vp, i32, i64, i64, vp, vp]
+  L.ovn_heads_stage_pairs.argtypes = [vp, C.POINTER(i64)]
   L.ovn_peer_signal.argtypes = [vp, vp, i32, i32, vp]
   L.ovn_peer_wait.argtypes = [vp, vp, i32, i32, i32, vp]
   L.ovn_head_gradients.argtypes = [vp, vp, i64, vp, vp, i32, vp, vp, f32, vp, vp]

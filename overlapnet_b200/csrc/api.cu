@@ -37,7 +37,7 @@ static __global__ void k_iota(int32_t* p, int n, int start) {
 }
 
 static __global__ void k_sanitize_idx(const int32_t* __restrict__ in, int32_t* __restrict__ out, int n, int64_t limit,
-                                      int code, int* __restrict__ err) {
+                                      int code, const int32_t* __restrict__ row_bad, int* __restrict__ err) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   int64_t v = in[i];
@@ -45,6 +45,7 @@ static __global__ void k_sanitize_idx(const int32_t* __restrict__ in, int32_t* _
     atomicCAS(err, 0, code);              // the first error wins; results of this call are poisoned by the finalize kernels
     v = v < 0 ? 0 : limit - 1;
   }
+  if (row_bad && row_bad[v]) atomicCAS(err, 0, kErrNonFiniteOperand);
   out[i] = (int32_t)v;
 }
 
@@ -76,9 +77,10 @@ static __global__ void k_peer_wait(const int32_t* __restrict__ flags, int n, int
 
 namespace ovn {
 
-int sanitize_indices(ovn_handle* h, const int32_t* d_in, int n, int64_t limit, int code, int32_t* d_out, cudaStream_t s) {
+int sanitize_indices(ovn_handle* h, const int32_t* d_in, int n, int64_t limit, int code, int32_t* d_out, cudaStream_t s,
+                     const int32_t* row_bad) {
   if (n <= 0) return OVN_OK;
-  k_sanitize_idx<<<(n + 255) / 256, 256, 0, s>>>(d_in, d_out, n, limit < 1 ? 1 : limit, code, h->d_err);
+  k_sanitize_idx<<<(n + 255) / 256, 256, 0, s>>>(d_in, d_out, n, limit < 1 ? 1 : limit, code, row_bad, h->d_err);
   OVN_LAUNCH_CHECK(h);
   return OVN_OK;
 }
@@ -98,6 +100,9 @@ int check_device_error(ovn_handle* h, cudaStream_t s) {
     case kErrBadIndex: OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "a pair / candidate index is outside [0, bank_size)");
     case kErrRowNotPrepared:
       OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "resident bank: an indexed row was never passed to ovn_bank_prepare");
+    case kErrNonFiniteOperand:
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "a feature volume value is not finite in the fp16 operands of the tensor-core "
+                  "heads (NaN, inf, or |x - centre| > 65504); outputs of the call are poisoned (NaN / INT32_MIN)");
     case kErrPeerWait: OVN_SET_ERR(h, OVN_ERR_CUDA, "ovn_peer_wait timed out: a peer rank never signalled");
     case kErrInjectedFault: OVN_SET_ERR(h, OVN_ERR_CUDA, "tensor-core pipeline failed: k_conv2_wgmma: fault injected by "
                                         "OVN_DEBUG_FAULT (code %d); outputs of the call are poisoned (NaN / INT32_MIN)", e);
@@ -1076,6 +1081,24 @@ int ovn_calibrate(ovn_handle* h, const float* d_volume, void* stream) {
   if (h->cfg.precision != OVN_PREC_F16_TC) return OVN_OK;
   if (!h->weights_ready) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "ovn_calibrate: weights not finalised");
   return tc_calibrate(h, d_volume, (cudaStream_t)stream);
+}
+
+int ovn_heads_stage_pairs(ovn_handle* h, int64_t* n_pairs) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  REQUIRE(h, n_pairs != nullptr, "NULL pointer");
+  if (h->cfg.precision != OVN_PREC_F16_TC)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_heads_stage_pairs: the stages exist on precision f16_tc handles only");
+  *n_pairs = tc_heads_stage_pairs(h);
+  return OVN_OK;
+}
+
+int ovn_copy_heads_stage(ovn_handle* h, int32_t stage, int64_t first, int64_t count, float* d_out, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  if (h->cfg.precision != OVN_PREC_F16_TC)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_copy_heads_stage: the stages exist on precision f16_tc handles only");
+  REQUIRE(h, stage >= OVN_STAGE_O1 && stage <= OVN_STAGE_CENTRES, "unknown ovn_heads_stage");
+  return tc_copy_heads_stage(h, stage, first, count, d_out, (cudaStream_t)stream);
 }
 
 int ovn_get_feature_center(ovn_handle* h, float* h_mu, int32_t* is_set) {

@@ -274,6 +274,7 @@ enum DeviceError : int {
   kErrInjectedFault = 501,        // k_conv2_wgmma under OVN_DEBUG_FAULT (the error-path test hook)
   kErrBadIndex = 900,             // a pair / candidate index outside [0, bank_size)
   kErrRowNotPrepared = 901,       // resident bank: the row was never passed to ovn_bank_prepare
+  kErrNonFiniteOperand = 910,     // a tensor-core operand copy is not finite in fp16 (NaN, inf, |x - mu| > 65504)
   kErrPeerWait = 950,             // ovn_peer_wait: a peer rank never signalled
 };
 
@@ -376,8 +377,12 @@ int tc_bank_release(ovn_handle* h, const float* d_bank);
 int tc_set_center(ovn_handle* h, const float* h_mu);
 int tc_get_center(ovn_handle* h, float* h_mu, int32_t* is_set);
 int tc_calibrate(ovn_handle* h, const float* d_volume, cudaStream_t s);
-// bounds-checked copies of index lists (d_idx_san): out-of-range entries are clamped and flagged in d_err
-int sanitize_indices(ovn_handle* h, const int32_t* d_in, int n, int64_t limit, int code, int32_t* d_out, cudaStream_t s);
+int tc_copy_heads_stage(ovn_handle* h, int stage, int64_t first, int64_t count, float* d_out, cudaStream_t s);
+int64_t tc_heads_stage_pairs(const ovn_handle* h);   // pairs whose stages ovn_copy_heads_stage can copy
+// bounds-checked copies of index lists (d_idx_san): out-of-range entries are clamped and flagged in d_err; with
+// row_bad (a resident bank's marks), an index whose row is marked raises kErrNonFiniteOperand
+int sanitize_indices(ovn_handle* h, const int32_t* d_in, int n, int64_t limit, int code, int32_t* d_out, cudaStream_t s,
+                     const int32_t* row_bad = nullptr);
 // read (and clear) the device error flag after the caller has synchronised `s`; maps it to a status
 int check_device_error(ovn_handle* h, cudaStream_t s);
 

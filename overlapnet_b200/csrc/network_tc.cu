@@ -57,6 +57,7 @@ struct TcState {
   int64_t pb_rows = 0;                  // rows [0, pb_rows) prepared
   Buffer<__half> pb_l16;                // [cap][360][K4_PITCH]
   Buffer<__half> pb_lc;                 // [cap] x C6_VOL_L_BYTES
+  Buffer<int32_t> pb_bad;               // [cap] 1: the row holds a value its fp16 copies cannot (kErrNonFiniteOperand)
   // per-channel centre of the feature volumes: the delta head only sees |l - r|, which is invariant
   // to a common offset, so both operands are stored as fp16(x - mu[c]) -- smaller magnitudes, smaller
   // fp16 rounding error of the (coherently re-used) volumes.  mu is calibrated once (first bank rows /
@@ -72,6 +73,7 @@ struct TcState {
   Buffer<float> b3eff;          // c_conv3 bias + mu_x3 pushed through the fp16 W3
   bool act_set = false;
   int64_t rows_pad = 0;
+  int64_t last_n = 0;           // pairs of the last heads chunk whose o1 / x3 / partial are stored (0: none or unknown)
 };
 
 void TcStateDelete::operator()(TcState* t) const { delete t; }
@@ -88,9 +90,17 @@ __host__ __device__ __forceinline__ int k4_pos(int r, int c) {
   return (((c >> 5) ^ (r & 1)) << 5) + ((k & 7) >> 1) * 8 + (k >> 3) * 2 + (k & 1);
 }
 
+// An fp16 value that is not finite (exponent field all ones): its source was NaN, inf or beyond fp16's range.  The
+// heads' ReLUs (fmaxf) turn NaN into 0 and the argmax skips it, so such an operand would give plausible outputs:
+// the operand kernels raise kErrNonFiniteOperand instead, which poisons the outputs of the call.
+__device__ __forceinline__ bool h2_nonfinite(__half2 v) {
+  const uint32_t b = *reinterpret_cast<const uint32_t*>(&v);
+  return (b & 0x7c00u) == 0x7c00u || (b & 0x7c000000u) == 0x7c000000u;
+}
+
 __global__ void __launch_bounds__(256)
 k_gather_rows_f16(const float* __restrict__ bank, const int32_t* __restrict__ idx, int n, const float* __restrict__ mu,
-                  int row_shift, __half* __restrict__ out) {
+                  int row_shift, __half* __restrict__ out, int* __restrict__ err, int32_t* __restrict__ row_bad) {
   const int64_t per = (int64_t)WF * CF / 4;            // float4 per volume
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)n * per) return;
@@ -103,6 +113,10 @@ k_gather_rows_f16(const float* __restrict__ bank, const int32_t* __restrict__ id
   const float4 v = __ldg(reinterpret_cast<const float4*>(bank + (row * WF + rs) * CF) + c4);
   const float4 m = __ldg(reinterpret_cast<const float4*>(mu) + c4);
   __half2 a = __floats2half2_rn(v.x - m.x, v.y - m.y), b = __floats2half2_rn(v.z - m.z, v.w - m.w);
+  if (h2_nonfinite(a) || h2_nonfinite(b)) {
+    if (row_bad) row_bad[p] = 1;          // a resident bank row: the heads calls that read it raise the flag
+    else atomicCAS(err, 0, kErrNonFiniteOperand);
+  }
   __half* o = out + ((int64_t)p * WF + r) * K4_PITCH;
   *reinterpret_cast<uint32_t*>(o + k4_pos(r, 4 * c4)) = *reinterpret_cast<uint32_t*>(&a);
   *reinterpret_cast<uint32_t*>(o + k4_pos(r, 4 * c4 + 2)) = *reinterpret_cast<uint32_t*>(&b);
@@ -164,7 +178,8 @@ constexpr int C6_VOL_R_BYTES = C6_RT * C6_R_BYTES;
 // fp32 volumes -> hi/lo fp16 split in the tiled operand layout above; one thread per (volume, plane, row)
 template <int TR, int NT>
 __global__ void __launch_bounds__(256)
-k_pack_corr(const float* __restrict__ bank, const int32_t* __restrict__ idx, int n, __half* __restrict__ out) {
+k_pack_corr(const float* __restrict__ bank, const int32_t* __restrict__ idx, int n, __half* __restrict__ out,
+            int* __restrict__ err, int32_t* __restrict__ row_bad) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t per = 16 * NT * TR;
   if (i >= (int64_t)n * per) return;
@@ -188,6 +203,13 @@ k_pack_corr(const float* __restrict__ bank, const int32_t* __restrict__ idx, int
   for (int e = 0; e < 8; ++e) {
     hi[e] = __float2half_rn(v[e]);
     lo[e] = __float2half_rn(v[e] - __half2float(hi[e]));
+  }
+  bool bad = false;                       // lo is finite whenever hi is
+#pragma unroll
+  for (int e = 0; e < 8; e += 2) bad |= h2_nonfinite(__halves2half2(hi[e], hi[e + 1]));
+  if (bad) {
+    if (row_bad) row_bad[p] = 1;
+    else atomicCAS(err, 0, kErrNonFiniteOperand);
   }
   __half* base = out + ((size_t)p * NT + tile) * (2 * 16 * TR * 8);
   *reinterpret_cast<uint4*>(base + ((size_t)pl * TR + row) * 8) = *reinterpret_cast<const uint4*>(hi);
@@ -1420,6 +1442,7 @@ int tc_bank_release(ovn_handle* h, const float* d_bank) {
   OVN_CUDA(h, cudaDeviceSynchronize());
   t->pb_l16 = {};
   t->pb_lc = {};
+  t->pb_bad = {};
   t->pb_key = nullptr;
   t->pb_rows = 0;
   return OVN_OK;
@@ -1434,6 +1457,7 @@ int tc_bank_prepare(ovn_handle* h, const float* d_bank, int64_t capacity, int64_
     if (t->pb_key != nullptr || t->pb_l16) rc = tc_bank_release(h, nullptr);
     if (rc == OVN_OK) rc = t->pb_l16.ensure(h, l16_bytes);
     if (rc == OVN_OK) rc = t->pb_lc.ensure(h, (size_t)capacity * C6_VOL_L_BYTES);
+    if (rc == OVN_OK) rc = t->pb_bad.ensure(h, (size_t)capacity * sizeof(int32_t));
     if (rc != OVN_OK) return rc;
     OVN_CUDA(h, cudaMemsetAsync(t->pb_l16, 0, l16_bytes, s));
     t->pb_key = d_bank;
@@ -1448,11 +1472,15 @@ int tc_bank_prepare(ovn_handle* h, const float* d_bank, int64_t capacity, int64_
     int rc = calibrate_all(h, src, nullptr, false, s);
     if (rc != OVN_OK) return rc;
   }
+  // the rows' non-finite marks start clear and are set by the two conversions; heads calls check them through lidx
+  OVN_CUDA(h, cudaMemsetAsync(t->pb_bad + first, 0, (size_t)count * sizeof(int32_t), s));
   k_gather_rows_f16<<<(unsigned)((count * per + 255) / 256), 256, 0, s>>>(src, nullptr, (int)count, t->mu, 0,
-                                                                         t->pb_l16 + (size_t)first * WF * K4_PITCH);
+                                                                         t->pb_l16 + (size_t)first * WF * K4_PITCH, h->d_err,
+                                                                         t->pb_bad + first);
   OVN_LAUNCH_CHECK(h);
   k_pack_corr<C6_LROWS, C6_LT><<<(unsigned)((count * perL + 255) / 256), 256, 0, s>>>(src, nullptr, (int)count,
-                                                                      t->pb_lc + (size_t)first * (C6_VOL_L_BYTES / 2));
+                                                                      t->pb_lc + (size_t)first * (C6_VOL_L_BYTES / 2), h->d_err,
+                                                                      t->pb_bad + first);
   OVN_LAUNCH_CHECK(h);
   if (first + count > t->pb_rows) t->pb_rows = first + count;
   return OVN_OK;
@@ -1475,10 +1503,11 @@ static int calibrate_all(ovn_handle* h, const float* d_vols, const int32_t* d_id
   }
   OVN_CUDA(h, cudaMemsetAsync(t->mu_o1, 0, 64 * sizeof(float), s));
   OVN_CUDA(h, cudaMemsetAsync(t->mu_x3, 0, 128 * sizeof(float), s));
-  k_gather_rows_f16<<<(unsigned)((per + 255) / 256), 256, 0, s>>>(d_vols, d_idx, 1, t->mu, 0, t->l16);
+  k_gather_rows_f16<<<(unsigned)((per + 255) / 256), 256, 0, s>>>(d_vols, d_idx, 1, t->mu, 0, t->l16, h->d_err, nullptr);
   OVN_LAUNCH_CHECK(h);
-  k_gather_rows_f16<<<(unsigned)((per + 255) / 256), 256, 0, s>>>(d_vols, d_idx, 1, t->mu, WF / 2, t->r16);
+  k_gather_rows_f16<<<(unsigned)((per + 255) / 256), 256, 0, s>>>(d_vols, d_idx, 1, t->mu, WF / 2, t->r16, h->d_err, nullptr);
   OVN_LAUNCH_CHECK(h);
+  t->last_n = 0;                        // o1 and x3 now hold the calibration pair
   const int64_t Mc = PAIR_ROWS;
   const int g4c = NB < h->sm_count ? NB : h->sm_count;
   const int64_t tiles_c = (Mc + TC_ROWS - 1) / TC_ROWS;
@@ -1550,6 +1579,7 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
   const int maxp = h->cfg.max_batch_pairs;
   const int base = kMaxLegLayers;
   const int64_t per = (int64_t)WF * CF / 4;
+  t->last_n = 0;                                  // o1 / x3 / partial are overwritten from here on
   if ((!t->mu_set || !t->act_set) && n > 0) {     // first pairs seen by this handle: calibrate on the first RIGHT volume
     int rc = d_query ? calibrate_all(h, d_query, nullptr, t->mu_set, s) : calibrate_all(h, d_bank, d_right, t->mu_set, s);
     if (rc != OVN_OK) return rc;
@@ -1562,14 +1592,16 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
   int32_t* lidx = nullptr;
   if (resident) {
     lidx = h->d_idx_san + 2 * (size_t)maxp;
-    int rc = sanitize_indices(h, d_left, n, t->pb_rows, kErrRowNotPrepared, lidx, s);
+    int rc = sanitize_indices(h, d_left, n, t->pb_rows, kErrRowNotPrepared, lidx, s, t->pb_bad);
     if (rc != OVN_OK) return rc;
   } else {
-    k_gather_rows_f16<<<(unsigned)((n * per + 255) / 256), 256, 0, s>>>(d_bank, d_left, n, t->mu, 0, t->l16);
+    k_gather_rows_f16<<<(unsigned)((n * per + 255) / 256), 256, 0, s>>>(d_bank, d_left, n, t->mu, 0, t->l16, h->d_err, nullptr);
     OVN_LAUNCH_CHECK(h);
   }
-  if (d_query) k_gather_rows_f16<<<(unsigned)((per + 255) / 256), 256, 0, s>>>(d_query, nullptr, 1, t->mu, 0, t->r16);
-  else k_gather_rows_f16<<<(unsigned)((n * per + 255) / 256), 256, 0, s>>>(d_bank, d_right, n, t->mu, 0, t->r16);
+  if (d_query)
+    k_gather_rows_f16<<<(unsigned)((per + 255) / 256), 256, 0, s>>>(d_query, nullptr, 1, t->mu, 0, t->r16, h->d_err, nullptr);
+  else
+    k_gather_rows_f16<<<(unsigned)((n * per + 255) / 256), 256, 0, s>>>(d_bank, d_right, n, t->mu, 0, t->r16, h->d_err, nullptr);
   OVN_LAUNCH_CHECK(h);
   const int64_t M = (int64_t)n * PAIR_ROWS;
   const int64_t tiles = (M + TC_ROWS - 1) / TC_ROWS;                 // 256-row tiles of c_conv2 / c_conv3
@@ -1598,11 +1630,13 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
   // correlation head (tensor cores, hi/lo split operands)
   const int64_t perL = 16 * C6_LT * C6_LROWS, perR = 16 * C6_RT * C6_RROWS;
   if (!resident) {
-    k_pack_corr<C6_LROWS, C6_LT><<<(unsigned)((n * perL + 255) / 256), 256, 0, s>>>(d_bank, d_left, n, t->lc);
+    k_pack_corr<C6_LROWS, C6_LT><<<(unsigned)((n * perL + 255) / 256), 256, 0, s>>>(d_bank, d_left, n, t->lc, h->d_err, nullptr);
     OVN_LAUNCH_CHECK(h);
   }
-  if (d_query) k_pack_corr<C6_RROWS, C6_RT><<<(unsigned)((perR + 255) / 256), 256, 0, s>>>(d_query, nullptr, 1, t->rc);
-  else k_pack_corr<C6_RROWS, C6_RT><<<(unsigned)((n * perR + 255) / 256), 256, 0, s>>>(d_bank, d_right, n, t->rc);
+  if (d_query)
+    k_pack_corr<C6_RROWS, C6_RT><<<(unsigned)((perR + 255) / 256), 256, 0, s>>>(d_query, nullptr, 1, t->rc, h->d_err, nullptr);
+  else
+    k_pack_corr<C6_RROWS, C6_RT><<<(unsigned)((n * perR + 255) / 256), 256, 0, s>>>(d_bank, d_right, n, t->rc, h->d_err, nullptr);
   OVN_LAUNCH_CHECK(h);
   prof_mark(h, PROF_CORR, s);
   const int nc = (int64_t)n * C6_LT < h->sm_count / C6_RT ? n * C6_LT : h->sm_count / C6_RT;
@@ -1611,8 +1645,66 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
   OVN_LAUNCH_CHECK(h);
   k_corr_finalize<<<n, 384, 0, s>>>(t->corr_part, d_corr, d_yaw, h->d_err);
   OVN_LAUNCH_CHECK(h);
+  t->last_n = n;
   static const bool debug_sync = getenv("OVN_DEBUG_SYNC") != nullptr;
   if (debug_sync) return check_device_error(h, s);
+  return OVN_OK;
+}
+
+// ovn_copy_heads_stage: the stored o1 / x3 / partial of pairs [first, first + n) as float32, in the reference's
+// orientation; a copy and a conversion only.  One thread per output element.
+//   O1 [n][360][24][64] (i, jb, o) from the o1 tiles, X3 [n][24][24][128] (ib, jb, c) from the C8 planes,
+//   DENSE [n][24][24][2] (ib, jb, half) from partial; row m = pair * 576 + jb * 24 + ib in all three.
+__global__ void __launch_bounds__(256)
+k_copy_heads_stage(int stage, const __half* __restrict__ o1, const __half* __restrict__ x3, int64_t x3_pitch,
+                   const float* __restrict__ partial, int64_t first, int64_t total, float* __restrict__ out) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= total) return;
+  out += e;
+  if (stage == OVN_STAGE_O1) {
+    const int o = (int)(e % 64), jb = (int)(e / 64 % NB), i = (int)(e / (64 * NB) % WF);
+    const int64_t p = first + e / (64 * NB * WF);
+    const int64_t m = p * PAIR_ROWS + jb * NB + i / S15;
+    *out = __half2float(o1[o1_chunk_offset(m, i % S15, o >> 3) + (o & 7)]);
+  } else if (stage == OVN_STAGE_X3) {
+    const int c = (int)(e % 128), jb = (int)(e / 128 % NB), ib = (int)(e / (128 * NB) % NB);
+    const int64_t m = (first + e / (128 * PAIR_ROWS)) * PAIR_ROWS + jb * NB + ib;
+    *out = __half2float(x3[((size_t)(c >> 3) * x3_pitch + m) * 8 + (c & 7)]);
+  } else {
+    const int half = (int)(e % 2), jb = (int)(e / 2 % NB), ib = (int)(e / (2 * NB) % NB);
+    const int64_t m = (first + e / (2 * PAIR_ROWS)) * PAIR_ROWS + jb * NB + ib;
+    *out = partial[m * 2 + half];
+  }
+}
+
+int64_t tc_heads_stage_pairs(const ovn_handle* h) {
+  const TcState* t = h->tc.get();
+  return t ? t->last_n : 0;
+}
+
+int tc_copy_heads_stage(ovn_handle* h, int stage, int64_t first, int64_t count, float* d_out, cudaStream_t s) {
+  TcState* t = h->tc.get();
+  if (!t || t->last_n == 0)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_copy_heads_stage: no stored stages (no complete heads call since the "
+                "weights were packed or the centres calibrated)");
+  if (!d_out) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_copy_heads_stage: NULL pointer");
+  if (stage != OVN_STAGE_CENTRES && (first < 0 || count < 1 || first + count > t->last_n))
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_copy_heads_stage: pairs [%lld, %lld) outside the %lld stored",
+                (long long)first, (long long)(first + count), (long long)t->last_n);
+  if (stage == OVN_STAGE_CENTRES) {
+    const Buffer<float>* parts[4] = {&t->mu_o1, &t->mu_x3, &t->b2eff, &t->b3eff};
+    const size_t len[4] = {64, 128, 128, 256};
+    for (int k = 0; k < 4; ++k) {
+      OVN_CUDA(h, cudaMemcpyAsync(d_out, *parts[k], len[k] * sizeof(float), cudaMemcpyDeviceToDevice, s));
+      d_out += len[k];
+    }
+    return OVN_OK;
+  }
+  const int64_t per = stage == OVN_STAGE_O1 ? (int64_t)WF * NB * 64 : stage == OVN_STAGE_X3 ? PAIR_ROWS * 128 : PAIR_ROWS * 2;
+  const int64_t total = count * per;
+  k_copy_heads_stage<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(stage, t->o1, t->x3, t->rows_pad, t->partial, first,
+                                                                       total, d_out);
+  OVN_LAUNCH_CHECK(h);
   return OVN_OK;
 }
 

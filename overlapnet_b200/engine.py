@@ -326,6 +326,31 @@ class Engine:
                                           _ptr(yaw), _ptr(corr), self._stream()), 'ovn_heads_forward')
     return ov, yaw, corr
 
+  def heads_stage_pairs(self):
+    """ovn_heads_stage_pairs (precision f16_tc): the pairs of the last chunk of the last heads call whose stages are
+    stored (0 when there are none)."""
+    n = C.c_int64(0)
+    check(self._h, lib().ovn_heads_stage_pairs(self._h, C.byref(n)), 'ovn_heads_stage_pairs')
+    return int(n.value)
+
+  def heads_stage(self, stage, first=0, count=None):
+    """ovn_copy_heads_stage (precision f16_tc): pairs [first, first + count) (default: all of them) of what the last
+    chunk of the last heads call stored, as a float32 cuda tensor.  ``stage``: 'o1' [count, 360, 24, 64] (i, jb, o:
+    c_conv1 output without its bias, minus the o1 centre), 'x3' [count, 24, 24, 128] (ib, jb, c: ReLU(c_conv2) minus
+    the x3 centre), 'dense' [count, 24, 24, 2] (the Dense partial sums of each c_conv3 pixel over output channels
+    [0, 128) and [128, 256); 0 where ib or jb >= 22), 'centres' [576] (o1 centre 64, x3 centre 128, b2eff 128, b3eff
+    256; first and count ignored)."""
+    if count is None:
+      count = self.heads_stage_pairs() - first
+    nb = self.Wf // 15
+    shape = {'o1': (count, self.Wf, nb, 64), 'x3': (count, nb, nb, 128), 'dense': (count, nb, nb, 2),
+             'centres': (576,)}[stage]
+    out = torch.empty(shape, dtype=torch.float32, device=self.device)
+    # the library writes exactly `count` pairs (576 floats for the centres) and refuses a range it does not hold
+    check(self._h, lib().ovn_copy_heads_stage(self._h, _cabi.HEADS_STAGES[stage], int(first), int(count), _ptr(out),
+                                             self._stream()), 'ovn_copy_heads_stage')
+    return out
+
   def heads_1vsN(self, bank, query, cand_idx=None, n_cand=None, want_corr=False, out=None):
     """RIGHT = query [360,128] for every pair, LEFT = bank[cand_idx] (None = first n_cand rows).
     ``out`` = (overlap f32 [n], yaw i32 [n]) tensors to write into -- they may live in another GPU's

@@ -6,6 +6,7 @@ import pytest
 import torch
 
 from oracle import network as N
+from oracle import tc_heads as T
 from overlapnet_b200 import synth
 from overlapnet_b200.engine import Engine
 
@@ -24,13 +25,16 @@ YAW_TIE_REL = 2e-4          # a yaw flip is accepted only if the oracle's two sc
 SPREAD_STD = {'fp32': 1.5, 'f16_tc': 1.5}
 
 
-def check_yaw(yaw_gpu, yaw_ref, corr_ref):
+def check_yaw(yaw_gpu, yaw_ref, corr_ref, bound=None):
+  """A yaw flip is accepted on a near-tie of the oracle's scores: within YAW_TIE_REL of the score range, or, given
+  the per-bin bound of the path (oracle/tc_heads.py), within the two bins' bounds."""
   bad = []
   for p in range(len(yaw_ref)):
     if int(yaw_gpu[p]) != int(yaw_ref[p]):
       kg, kr = 180 - int(yaw_gpu[p]), 180 - int(yaw_ref[p])
       gap = corr_ref[p, kr] - corr_ref[p, kg]
-      if gap > YAW_TIE_REL * np.abs(corr_ref[p]).max():
+      tie = YAW_TIE_REL * np.abs(corr_ref[p]).max() if bound is None else bound[p, kr] + bound[p, kg]
+      if gap > tie:
         bad.append((p, int(yaw_gpu[p]), int(yaw_ref[p]), float(gap)))
   assert not bad, bad
 
@@ -80,10 +84,18 @@ def test_heads_match_oracle(setup, prec):
         % (prec, SPREAD_STD[prec], np.abs(ov - ov_ref).max(), len(left), ov_ref.min(), ov_ref.max()))
   assert np.abs(ov - ov_ref).max() <= OVERLAP_TOL, (ov, ov_ref)
   assert ov_ref.max() - ov_ref.min() > 0.25                      # the test is not degenerate
-  check_yaw(yaw, yaw_ref, corr_ref)
+  # f16_tc: the per-bin gate of its hi/lo split correlation (oracle/tc_heads.py, 2.9e-6 of the bin's magnitude: the
+  # split's bound plus an empirical allowance for the fp32 accumulation); plain fp16 operands are 1e-5 off and fail it
+  bound = np.stack([T.corr_stage(bank_np[a], bank_np[b])[1] for a, b in zip(left, right)]) if prec == 'f16_tc' else None
+  check_yaw(yaw, yaw_ref, corr_ref, bound)
   assert yaw_ref[1] == -37 and yaw[1] == -37 and yaw[2] == 120 and yaw[5] == 0 and yaw[7] == 157
   rel = np.abs(corr - corr_ref).max() / np.abs(corr_ref).max()
-  assert rel <= (1e-5 if prec == 'fp32' else 2e-3), rel
+  if prec == 'fp32':
+    assert rel <= 1e-5, rel
+  else:
+    r = (np.abs(corr - corr_ref) / bound).max()
+    print('[parity] heads f16_tc: corr max rel err %.3e, %.3f of the per-bin bound' % (rel, r))
+    assert r <= 1.0, (rel, r)
   # 1-vs-N entry point == pair list with RIGHT fixed
   ov1, yaw1, _ = eng.heads_1vsN(bank, bank[5], cand_idx=torch.tensor([0, 1, 2, 3, 4, 5], dtype=torch.int32))
   assert np.array_equal(ov1.cpu().numpy(), ov[:6]) and np.array_equal(yaw1.cpu().numpy(), yaw[:6])
