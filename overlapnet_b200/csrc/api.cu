@@ -109,6 +109,7 @@ int check_device_error(ovn_handle* h, cudaStream_t s) {
     case kErrDeltaLeftProducer: case kErrDeltaLeftConsumer: ring = "k_delta_conv1_wgmma: LEFT volume ring"; break;
     case kErrDeltaRightProducer: case kErrDeltaRightConsumer: ring = "k_delta_conv1_wgmma: RIGHT window ring"; break;
     case kErrDeltaW1Producer: case kErrDeltaW1Consumer: ring = "k_delta_conv1_wgmma: W1 ring"; break;
+    case kErrDeltaO1Producer: case kErrDeltaO1Consumer: ring = "k_delta_conv1_wgmma: o1 staging"; break;
     case kErrConv2Producer: case kErrConv2Consumer: ring = "k_conv2_wgmma: o1 + W2 ring"; break;
     case kErrConv3X3Producer: case kErrConv3X3Consumer: ring = "k_conv3_wgmma: x3 ring"; break;
     case kErrConv3W3Producer: case kErrConv3W3Consumer: ring = "k_conv3_wgmma: W3 ring"; break;

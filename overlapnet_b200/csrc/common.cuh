@@ -266,6 +266,7 @@ enum DeviceError : int {
   kErrDeltaLeftProducer = 101, kErrDeltaLeftConsumer = 402,      // k_delta_conv1_wgmma: LEFT volume
   kErrDeltaRightProducer = 103, kErrDeltaRightConsumer = 404,    //   RIGHT window
   kErrDeltaW1Producer = 102, kErrDeltaW1Consumer = 202,          //   W1 groups
+  kErrDeltaO1Producer = 104, kErrDeltaO1Consumer = 405,          //   o1 staging (the store lane / the writers)
   kErrConv2Producer = 111, kErrConv2Consumer = 211,              // k_conv2_wgmma: o1 + W2 stages
   kErrConv3X3Producer = 121, kErrConv3X3Consumer = 221,          // k_conv3_wgmma: x3 rows
   kErrConv3W3Producer = 122, kErrConv3W3Consumer = 222,          //   W3 slabs

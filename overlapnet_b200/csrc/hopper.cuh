@@ -1,6 +1,6 @@
 // hopper.cuh -- hand-written PTX wrappers for the Hopper (sm_90a) building blocks used by network_tc.cu:
 // wgmma (warpgroup MMA; B from shared memory, A from registers or shared memory), mbarrier and the pipeline
-// ring built on it, cp.async.bulk (TMA engine, 1-D).
+// ring built on it, cp.async.bulk (TMA engine, 1-D, both directions).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -41,11 +41,14 @@ constexpr long long kMbarWaitCycles = 1ll << 28;
 // order; fill i uses stage i % D in phase (i / D) & 1.  The fill counters belong to the kernels, which pass the
 // fill index.  full[s] completes on the producer's arrive plus the bytes of its bulk copies; empty[s] completes
 // when every consumer arrival has released the stage.
+//
+// A ring can also be filled by threads rather than by bulk copies: init with one producer arrival per writing
+// warp; each writing warp waits with wait_free, writes, and signals the fill with publish.
 template <int D>
 struct MbarRing {
   uint64_t full[D], empty[D];
-  __device__ __forceinline__ void init(uint32_t consumer_arrivals) {
-    for (int s = 0; s < D; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], consumer_arrivals); }
+  __device__ __forceinline__ void init(uint32_t consumer_arrivals, uint32_t producer_arrivals = 1) {
+    for (int s = 0; s < D; ++s) { mbar_init(&full[s], producer_arrivals); mbar_init(&empty[s], consumer_arrivals); }
   }
   static __device__ __forceinline__ uint32_t slot(uint32_t i) { return i % D; }
   static __device__ __forceinline__ uint32_t parity(uint32_t i) { return (i / D) & 1; }
@@ -69,6 +72,18 @@ struct MbarRing {
   __device__ __forceinline__ void release(uint32_t i) {
     __syncwarp();
     if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[slot(i)]);
+  }
+  // consumer that is a single thread: it is done with fill i's stage
+  __device__ __forceinline__ void release_thread(uint32_t i) { mbar_arrive(&empty[slot(i)]); }
+  // writing warp: wait (bounded) until fill i's stage is free.  False on time-out.
+  __device__ __forceinline__ bool wait_free(uint32_t i) {
+    return mbar_wait(&empty[slot(i)], parity(i) ^ 1, kMbarWaitCycles);
+  }
+  // writing warp: this warp has written its part of fill i (one arrival per warp).  Writes that a bulk copy will
+  // read must be followed by fence_proxy_async_smem() in each writing thread first.
+  __device__ __forceinline__ void publish(uint32_t i) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&full[slot(i)]);
   }
 };
 
@@ -100,6 +115,21 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                :: "r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
+
+// ---- bulk async copy shared -> global, tracked by bulk async-groups (bytes and addresses multiples of 16)
+__device__ __forceinline__ void bulk_s2g(void* gmem_dst, const void* smem_src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+               :: "l"(gmem_dst), "r"(smem_u32(smem_src)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's committed groups still read their shared-memory sources (which may then be rewritten)
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" :: "n"(N) : "memory"); }
+// at most N of this thread's committed groups are still incomplete (their global writes not yet performed)
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" :: "n"(N) : "memory"); }
+// orders this thread's earlier shared-memory writes before later bulk copies (async proxy) that read them
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- wgmma ------------------------------------------------------------------------------------------
 // Shared-memory matrix descriptor of a K-major operand (16-bit types):

@@ -148,9 +148,11 @@ constexpr int K4_STEPS = 60;            // W1 slices: 4 channel chunks x 15 dj
 // chunks are XOR-swizzled by the row):
 //   row m = pair*576 + jb*24 + ib (i = ib*15 + di), K = di*64 + o
 //   o1[(m / 128) * 15 + di][m % 128][chunk (o/8) ^ (m & 7)][o % 8]
+__host__ __device__ __forceinline__ size_t o1_row_offset(int64_t m, int di) {
+  return ((size_t)((m >> 7) * S15 + di) * 128 + (size_t)(m & 127)) * 64;
+}
 __host__ __device__ __forceinline__ size_t o1_chunk_offset(int64_t m, int di, int c8) {
-  const int r = (int)(m & 127);
-  return ((size_t)((m >> 7) * S15 + di) * 128 + r) * 64 + (size_t)((c8 ^ (r & 7)) * 8);
+  return o1_row_offset(m, di) + (size_t)((c8 ^ (int)(m & 7)) * 8);
 }
 
 struct LegArgs {
@@ -262,7 +264,9 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 // memory: the 66 MB delta tensor of a pair is never written.  A group of 5 slices never straddles a 32-channel
 // chunk (15 dj each), so the slice loop is unrolled straight-line code whose W1 descriptors and RIGHT rows are
 // fixed offsets from bases computed once per group; a RIGHT row is one 128-bit load (k4_pos).  The accumulators
-// start at the fp16-rounded -mu_o1 (the centre that k_fold_bias2 pushes through c_conv2).  Output: fp16 o1 tiles.
+// start at the fp16-rounded -mu_o1 (the centre that k_fold_bias2 pushes through c_conv2).  Output: fp16 o1 tiles,
+// written by the consumers into a staging buffer laid out as the tiles and stored with bulk copies by a second
+// producer lane, while the consumers go on with the next unit.
 // Persistent: each CTA takes a contiguous range of the n_pairs * 24 units.
 // ------------------------------------------------------------------------------------------------
 constexpr int K4_WG = 3;                               // consumer warpgroups
@@ -275,17 +279,24 @@ constexpr int K4_RING = 4;
 constexpr int K4_BSLICE = 4096;                        // bytes of W1 per slice: [4 k8][64 o][8]
 constexpr uint32_t K4_VOL_BYTES = WF * K4_PITCH * 2;
 constexpr uint32_t K4_RWIN_BYTES = S15 * K4_PITCH * 2;
+// o1 staging of a unit: per di, its 24 rows exactly as they land in the o1 tiles (128 B each, chunk-swizzled), then
+// 16 bytes of padding, so that the 8 rows of a fragment store (8 consecutive i, i.e. 8 different di) hit 8
+// different 16-byte bank groups
+constexpr int K4_O1S_PITCH = NB * 64 + 8;              // fp16 per di
 
 struct K4Smem {
   __half L[WF * K4_PITCH];
   __half Rw[2][S15 * K4_PITCH];
   __half B[K4_RING][K4_GROUP * K4_BSLICE / 2];
+  __half O1s[S15 * K4_O1S_PITCH];
   MbarRing<K4_RING> w1;
   MbarRing<1> left;
   MbarRing<2> right;
+  MbarRing<1> o1s;
 };
 static_assert(sizeof(K4Smem) <= 232448, "k_delta_conv1_wgmma shared memory");
-static_assert(offsetof(K4Smem, B) % 16 == 0 && offsetof(K4Smem, Rw) % 16 == 0, "bulk-copy alignment");
+static_assert(offsetof(K4Smem, B) % 16 == 0 && offsetof(K4Smem, Rw) % 16 == 0 && offsetof(K4Smem, O1s) % 16 == 0 &&
+              K4_O1S_PITCH * 2 % 16 == 0, "bulk-copy alignment");
 
 // [begin, end) of the contiguous share of n work items that part `part` of `parts` takes (a persistent CTA)
 struct Share { int64_t begin, end; };
@@ -306,6 +317,7 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
     S.w1.init(K4_WG * 4);
     S.left.init(K4_WG * 4);
     S.right.init(K4_WG * 4);
+    S.o1s.init(1, K4_WG * 4);
     mbar_fence_init();
   }
   __syncthreads();
@@ -330,6 +342,26 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
           bulk_g2s(S.B[S.w1.slot(gi)], W1p + (size_t)grp * K4_GROUP * (K4_BSLICE / 2), K4_GROUP * K4_BSLICE, S.w1.bar(gi));
         }
       }
+    } else if (warp == K4_WG * 4 + 1 && lane == 0) {
+      // o1 stores: per unit and di, one bulk copy of the staged rows, or two when the unit's 24 rows cross a
+      // 128-row o1 block (576 = 4.5 x 128)
+      uint32_t ui = 0;
+      for (int u = u_begin; u < u_end; ++u, ++ui) {
+        const int p = u / NB, jb = u - p * NB;
+        const int64_t m0 = (int64_t)p * PAIR_ROWS + jb * NB;
+        const int n0 = min(NB, 128 - (int)(m0 & 127));
+        if (!S.o1s.wait(ui)) { atomicExch(err, kErrDeltaO1Producer); break; }
+#pragma unroll 1
+        for (int di = 0; di < S15; ++di) {
+          const __half* src = S.O1s + di * K4_O1S_PITCH;
+          bulk_s2g(o1 + o1_row_offset(m0, di), src, n0 * 128);
+          if (n0 < NB) bulk_s2g(o1 + o1_row_offset(m0 + n0, di), src + n0 * 64, (NB - n0) * 128);
+        }
+        bulk_commit();
+        bulk_wait_read<0>();
+        S.o1s.release_thread(ui);
+      }
+      bulk_wait<0>();                         // the next kernel reads o1
     }
   } else {
     // ===================== consumers ==========================================================
@@ -415,7 +447,9 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
       }
       S.right.release(ui);
       if (jb == NB - 1 || u == u_end - 1) S.left.release(pi - 1);
-      const int64_t mrow = (int64_t)p * PAIR_ROWS + jb * NB;
+      // o1 into the staging buffer, once the store lane's copies of the previous unit have read it.  Row m of the
+      // unit is pair * 576 + jb * 24 + ib, so its chunk swizzle m & 7 is ib & 7.
+      if (!S.o1s.wait_free(ui)) { atomicExch(err, kErrDeltaO1Consumer); goto done; }
 #pragma unroll
       for (int tt = 0; tt < 2; ++tt)
 #pragma unroll
@@ -423,11 +457,14 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
           const int i = rows[tt][h];
           if (i >= WF) continue;
           const int ibk = i / S15, di = i - ibk * S15;
+          __half* st = S.O1s + di * K4_O1S_PITCH + ibk * 64 + 2 * t;
 #pragma unroll
           for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<uint32_t*>(o1 + o1_chunk_offset(mrow + ibk, di, j) + 2 * t) =
+            *reinterpret_cast<uint32_t*>(st + ((j ^ (ibk & 7)) << 3)) =
                 pack_h2(acc[tt][4 * j + 2 * h], acc[tt][4 * j + 2 * h + 1]);
         }
+      fence_proxy_async_smem();
+      S.o1s.publish(ui);
     }
   }
 done:
