@@ -20,8 +20,9 @@
  *     feature bank, SURVEY 8b "Threading").
  *   - Feature volumes cross the ABI as float32 [n][W_out=360][128] (what
  *     Infer.create_feature_volumes returns, infer.py:240-265, with the singleton H axis dropped).
- *   - ovn_copy_heads_stage reads back the intermediate stages of the tensor-core heads (tests and
- *     diagnostics only; the heads calls do no extra work for it).
+ *   - ovn_copy_heads_stage reads back the intermediate stages of the tensor-core heads and ovn_leg_stage
+ *     one layer of the tensor-core leg (tests and diagnostics only; the heads and leg calls do no extra
+ *     work for them).
  */
 #ifndef OVN_B200_H_
 #define OVN_B200_H_
@@ -379,7 +380,11 @@ int ovn_get_gradients(ovn_handle* h, const char* layer_name, float* h_kernel, fl
  * the device: an index outside [0, bank_size) (or, for a resident bank, a row that was never
  * prepared), a volume value the fp16 operands of the tensor-core heads cannot hold (NaN, inf, or more
  * than 65504 away from the feature centre; raised by every heads call that reads such a volume -- a
- * resident bank row keeps its mark from ovn_bank_prepare until it is prepared again), and a bounded
+ * resident bank row keeps its mark from ovn_bank_prepare until it is prepared again) or, in the
+ * tensor-core leg (ovn_leg_forward and the *_host entry points at precision f16_tc), an input pixel that
+ * is NaN or inf or an activation of any layer but the last above 65504, which the hi / lo fp16 planes
+ * between the layers cannot hold (the feature volumes of that call are not valid: without the flag the
+ * next layer's ReLU would turn the NaN into ordinary zeros), and a bounded
  * pipeline-barrier wait of a tensor-core kernel that timed out (GPU time-slicing, debuggers).  Each raises
  * a flag on the device; the kernels that write overlap / yaw
  * then POISON their outputs (overlap = NaN, yaw = INT32_MIN) so garbage never looks valid, indices are
@@ -442,6 +447,16 @@ typedef enum ovn_heads_stage {
 } ovn_heads_stage;
 int ovn_heads_stage_pairs(ovn_handle* h, int64_t* n_pairs);
 int ovn_copy_heads_stage(ovn_handle* h, int32_t stage, int64_t first, int64_t count, float* d_out, void* stream);
+
+/* ---- one layer of the tensor-core leg (tests and diagnostics) --------------------------------------
+ * Runs ovn_leg_forward's own launch sequence on n_scans <= max_batch_scans scans (the same kernels, grids and
+ * K slices as a leg call of that many scans) and stops after leg layer `layer` (0 = s_conv1 ... the last layer
+ * but one; the last layer's float32 volume is ovn_leg_forward).  d_hi, d_lo (float32, device)
+ * [n_scans][h_out][w_out][cout] of that layer = the fp16 halves of its activation as stored for the next layer,
+ * hi = fp16(v), lo = fp16(v - hi), converted exactly.  OVN_ERR_BAD_CONFIG on a precision fp32 handle,
+ * OVN_ERR_WEIGHTS before ovn_finalize_weights, OVN_ERR_INVALID_ARG for a layer or n_scans out of range. */
+int ovn_leg_stage(ovn_handle* h, const float* d_input, int32_t n_scans, int32_t layer, float* d_hi, float* d_lo,
+                  void* stream);
 
 /* ---- host-buffer convenience entry points (what a non-CUDA caller binds; bench.py e2e) ------ */
 /* Raw clouds on the host -> feature volumes on the host. */

@@ -27,7 +27,7 @@ SYMBOLS = [
     'ovn_copy_net_volumes', 'ovn_copy_train_state', 'ovn_set_train_state',
     'ovn_train_workspace_bytes', 'ovn_host_register', 'ovn_host_unregister', 'ovn_stage_rows',
     'ovn_head_gradients_chunks', 'ovn_net_gradients_chunks', 'ovn_copy_heads_stage',
-    'ovn_heads_stage_pairs',
+    'ovn_heads_stage_pairs', 'ovn_leg_stage',
 ]
 HEADS_STAGES = {'o1': 0, 'x3': 1, 'dense': 2, 'centres': 3}     # ovn_heads_stage
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
@@ -104,6 +104,7 @@ def lib():
   L.ovn_calibrate.argtypes = [vp, vp, vp]
   L.ovn_copy_heads_stage.argtypes = [vp, i32, i64, i64, vp, vp]
   L.ovn_heads_stage_pairs.argtypes = [vp, C.POINTER(i64)]
+  L.ovn_leg_stage.argtypes = [vp, vp, i32, i32, vp, vp, vp]
   L.ovn_peer_signal.argtypes = [vp, vp, i32, i32, vp]
   L.ovn_peer_wait.argtypes = [vp, vp, i32, i32, i32, vp]
   L.ovn_head_gradients.argtypes = [vp, vp, i64, vp, vp, i32, vp, vp, f32, vp, vp]

@@ -101,8 +101,10 @@ int check_device_error(ovn_handle* h, cudaStream_t s) {
     case kErrRowNotPrepared:
       OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "resident bank: an indexed row was never passed to ovn_bank_prepare");
     case kErrNonFiniteOperand:
-      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "a feature volume value is not finite in the fp16 operands of the tensor-core "
-                  "heads (NaN, inf, or |x - centre| > 65504); outputs of the call are poisoned (NaN / INT32_MIN)");
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "a value is not finite in the fp16 operands of the tensor-core path: a feature "
+                  "volume given to the heads (NaN, inf, or |x - centre| > 65504; outputs of the call are poisoned, NaN / "
+                  "INT32_MIN), or in the tensor-core leg an input pixel (NaN, inf) or an activation of s_conv1 .. the "
+                  "last layer but one (above 65504; the feature volumes of the call are not valid)");
     case kErrPeerWait: OVN_SET_ERR(h, OVN_ERR_CUDA, "ovn_peer_wait timed out: a peer rank never signalled");
     case kErrInjectedFault: OVN_SET_ERR(h, OVN_ERR_CUDA, "tensor-core pipeline failed: k_conv2_wgmma: fault injected by "
                                         "OVN_DEBUG_FAULT (code %d); outputs of the call are poisoned (NaN / INT32_MIN)", e);
@@ -1100,6 +1102,20 @@ int ovn_copy_heads_stage(ovn_handle* h, int32_t stage, int64_t first, int64_t co
     OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_copy_heads_stage: the stages exist on precision f16_tc handles only");
   REQUIRE(h, stage >= OVN_STAGE_O1 && stage <= OVN_STAGE_CENTRES, "unknown ovn_heads_stage");
   return tc_copy_heads_stage(h, stage, first, count, d_out, (cudaStream_t)stream);
+}
+
+int ovn_leg_stage(ovn_handle* h, const float* d_input, int32_t n_scans, int32_t layer, float* d_hi, float* d_lo,
+                  void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  if (h->cfg.precision != OVN_PREC_F16_TC)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_leg_stage: the hi / lo planes exist on precision f16_tc handles only");
+  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_leg_stage: %s", h->net_error.c_str());
+  if (!h->weights_ready) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "ovn_leg_stage: weights not finalised");
+  REQUIRE(h, d_input && d_hi && d_lo, "NULL pointer");
+  REQUIRE(h, n_scans >= 1 && n_scans <= h->cfg.max_batch_scans, "n_scans outside [1, max_batch_scans]");
+  REQUIRE(h, layer >= 0 && layer <= h->n_leg - 2, "layer outside [0, leg layers - 2]");
+  return tc_leg_stage(h, d_input, n_scans, layer, d_hi, d_lo, (cudaStream_t)stream);
 }
 
 int ovn_get_feature_center(ovn_handle* h, float* h_mu, int32_t* is_set) {

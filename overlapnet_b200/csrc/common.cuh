@@ -275,7 +275,7 @@ enum DeviceError : int {
   kErrInjectedFault = 501,        // k_conv2_wgmma under OVN_DEBUG_FAULT (the error-path test hook)
   kErrBadIndex = 900,             // a pair / candidate index outside [0, bank_size)
   kErrRowNotPrepared = 901,       // resident bank: the row was never passed to ovn_bank_prepare
-  kErrNonFiniteOperand = 910,     // a tensor-core operand copy is not finite in fp16 (NaN, inf, |x - mu| > 65504)
+  kErrNonFiniteOperand = 910,     // an fp16 operand of the tensor-core heads or leg is not finite (NaN, inf, > 65504)
   kErrPeerWait = 950,             // ovn_peer_wait: a peer rank never signalled
 };
 
@@ -368,7 +368,9 @@ int gather_images(ovn_handle* h, const float* d_images, int64_t n_images, const 
 int corr_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* left,
                       const int32_t* right, int np, int32_t* d_yaw, float* d_corr, cudaStream_t s);
 
-int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cudaStream_t s);
+// leg layers 0 .. stop_layer of n <= max_batch_scans scans; the last layer writes d_fv, the others hi / lo planes
+int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cudaStream_t s, int stop_layer = kMaxLegLayers);
+int tc_leg_stage(ovn_handle* h, const float* d_input, int n, int layer, float* d_hi, float* d_lo, cudaStream_t s);
 int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query,
                      const int32_t* d_left, const int32_t* d_right, int n, float* d_overlap,
                      int32_t* d_yaw, float* d_corr, cudaStream_t s);

@@ -165,7 +165,13 @@ struct LegArgs {
   __half* out_planes; int64_t out_pitch; int out_run_planes;   // EPI 4
   float* out_f32;                                               // EPI 3
   int n_split; float* part;                                     // K slices; EPI 5: [n_split][rows][M][n_valid] fp32
+  int* err;                                                     // ovn_handle::d_err (EPI 4: kErrNonFiniteOperand)
 };
+
+// A leg pre-activation v whose ReLU the hi / lo planes cannot hold: NaN, +-inf, or a value that rounds to an infinite
+// fp16 (hi = inf, lo = -inf: the next layer's MMAs make NaN of them).  fmaxf returns 0 for NaN, so without this test
+// such a layer hands on ordinary-looking zeros; the kernels that write planes raise kErrNonFiniteOperand instead.
+__device__ __forceinline__ bool leg_act_unstorable(float v) { return !(v < 65520.f) || v == -INFINITY; }
 
 // Correlation operands (k_corr_wgmma): a volume is cut into row tiles of TR rows (64 for LEFT, 128 for RIGHT),
 // each tile one contiguous [hi, lo][16 planes = c / 8][TR rows][8] block of fp16, zero rows past 360: the
@@ -931,9 +937,10 @@ k_leg_mma(LegArgs g) {
             make_float2(acc[j][2 * h], acc[j][2 * h + 1]);
         continue;
       }
-      const float a = fmaxf(acc[j][2 * h] + __ldg(g.bias + n), 0.f);
-      const float b = fmaxf(acc[j][2 * h + 1] + __ldg(g.bias + n + 1), 0.f);
+      const float pre_a = acc[j][2 * h] + __ldg(g.bias + n), pre_b = acc[j][2 * h + 1] + __ldg(g.bias + n + 1);
+      const float a = fmaxf(pre_a, 0.f), b = fmaxf(pre_b, 0.f);
       if (EPI == 4) {
+        if (leg_act_unstorable(pre_a) || leg_act_unstorable(pre_b)) atomicCAS(g.err, 0, kErrNonFiniteOperand);
         const __half2 hi = __floats2half2_rn(a, b);
         const float2 hf = __half22float2(hi);
         const int64_t pl = (int64_t)y * g.out_run_planes + (n >> 3);
@@ -965,9 +972,15 @@ k_leg_splitk_reduce(LegArgs g, int rows) {
     const float4 b = __ldg(reinterpret_cast<const float4*>(src + sl * slice_stride + 4));
     v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w; v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
   }
+  bool bad = false;
 #pragma unroll
-  for (int e = 0; e < 8; ++e) v[e] = fmaxf(v[e] + __ldg(g.bias + c8 * 8 + e), 0.f);
+  for (int e = 0; e < 8; ++e) {
+    v[e] += __ldg(g.bias + c8 * 8 + e);
+    bad |= leg_act_unstorable(v[e]);
+    v[e] = fmaxf(v[e], 0.f);
+  }
   if (EPI == 4) {
+    if (bad) atomicCAS(g.err, 0, kErrNonFiniteOperand);
     __half hi[8], lo[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
@@ -1096,10 +1109,10 @@ constexpr size_t L1_SMALL_SMEM = 200 * 1024;           // k_leg_layer1_small: al
 // once from shared memory (4 broadcast LDS.128) and feed 32 FFMAs -- the first version (one pixel x 8
 // channels per thread: 8 LDS per 32 FFMA) was bound by the load/store unit.
 template <bool CIN4>
-__global__ void __launch_bounds__(512)
+__global__ void __launch_bounds__(512, CIN4 ? 0 : 2)      // generic C_in: two blocks per SM (64 registers); C_in = 4: no minimum
 k_leg_layer1_direct(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
                     int n, int H_in, int W_in, int cin, int kh, int kw, int sh, int sw, int H_out, int W_out,
-                    int relu, __half* __restrict__ out) {
+                    int relu, __half* __restrict__ out, int* __restrict__ err) {
   constexpr int CO = 16;                                     // generateNet.py:161-164
   extern __shared__ __align__(16) float w_s[];              // [kw*cin][16]: the taps of ONE kernel row at a time
   const int pairs = (W_out + 1) / 2;                        //   (C_in = 25: 24 KB instead of 120 KB -> 4x the occupancy)
@@ -1162,12 +1175,15 @@ k_leg_layer1_direct(const float* __restrict__ x, const float* __restrict__ w, co
 #pragma unroll
     for (int g = 0; g < 2; ++g) {
       __half hi[8], lo[8];
+      bool bad = false;
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
         const float v = relu ? fmaxf(acc[g * 8 + e], 0.f) : acc[g * 8 + e];
+        bad |= leg_act_unstorable(relu ? acc[g * 8 + e] : fabsf(acc[g * 8 + e]));
         hi[e] = __float2half_rn(v);
         lo[e] = __float2half_rn(v - __half2float(hi[e]));
       }
+      if (bad) atomicCAS(err, 0, kErrNonFiniteOperand);
       const int64_t plane_hi = r * 4 + g;
       *reinterpret_cast<uint4*>(out + ((size_t)plane_hi * W_out + xo + p) * 8) = *reinterpret_cast<const uint4*>(hi);
       *reinterpret_cast<uint4*>(out + ((size_t)(plane_hi + 2) * W_out + xo + p) * 8) = *reinterpret_cast<const uint4*>(lo);
@@ -1179,7 +1195,7 @@ template <bool CIN4>
 __global__ void __launch_bounds__(256)
 k_leg_layer1_small(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
                     int n, int H_in, int W_in, int cin, int kh, int kw, int sh, int sw, int H_out, int W_out, int cout,
-                    int relu, __half* __restrict__ out) {
+                    int relu, __half* __restrict__ out, int* __restrict__ err) {
   // latency-mode variant (1-2 scans): one thread per (pixel, 8 output channels) -- four times the threads of
   // k_leg_layer1_direct, which matters when a single scan has to fill every SM
   extern __shared__ __align__(16) float w_s[];              // [kh*kw*cin][cout]
@@ -1227,12 +1243,15 @@ k_leg_layer1_small(const float* __restrict__ x, const float* __restrict__ w, con
     }
   }
   __half hi[8], lo[8];
+  bool bad = false;
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
     const float v = relu ? fmaxf(acc[e], 0.f) : acc[e];
+    bad |= leg_act_unstorable(relu ? acc[e] : fabsf(acc[e]));
     hi[e] = __float2half_rn(v);
     lo[e] = __float2half_rn(v - __half2float(hi[e]));
   }
+  if (bad) atomicCAS(err, 0, kErrNonFiniteOperand);
   const int64_t plane_hi = r * (2 * C8) + g;                               // [img][y][hi,lo][c8][x][8]
   *reinterpret_cast<uint4*>(out + ((size_t)plane_hi * W_out + xo) * 8) = *reinterpret_cast<const uint4*>(hi);
   *reinterpret_cast<uint4*>(out + ((size_t)(plane_hi + C8) * W_out + xo) * 8) = *reinterpret_cast<const uint4*>(lo);
@@ -1410,7 +1429,8 @@ int tc_pack_weights(ovn_handle* h) {
   return OVN_OK;
 }
 
-int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cudaStream_t s) {
+int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cudaStream_t s, int stop_layer) {
+  // Leg layers 0 .. stop_layer (the whole leg by default); layer l leaves its planes in actp[l & 1].
   // layer 1 (C_in = 4..25, stride (2,2), N = 16: K = 16 per MMA would be mostly padding) runs on the
   // direct SIMT kernels and writes hi/lo fp16 C8-interleaved planes; layers 2.. run on k_leg_mma.
   TcState* t = h->tc.get();
@@ -1424,24 +1444,24 @@ int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cuda
       const unsigned grid = (unsigned)(((int64_t)n * L.h_out * (L.cout / 8) * L.w_out + 255) / 256);
       if (L.cin == 4)
         k_leg_layer1_small<true><<<grid, 256, w_all, s>>>(d_input, h->d_w[0], h->d_b[0], n, L.h_in, L.w_in, L.cin, L.kh, L.kw,
-                                                         L.sh, L.sw, L.h_out, L.w_out, L.cout, L.relu, t->actp[0]);
+                                                         L.sh, L.sw, L.h_out, L.w_out, L.cout, L.relu, t->actp[0], h->d_err);
       else
         k_leg_layer1_small<false><<<grid, 256, w_all, s>>>(d_input, h->d_w[0], h->d_b[0], n, L.h_in, L.w_in, L.cin, L.kh, L.kw,
-                                                          L.sh, L.sw, L.h_out, L.w_out, L.cout, L.relu, t->actp[0]);
+                                                          L.sh, L.sw, L.h_out, L.w_out, L.cout, L.relu, t->actp[0], h->d_err);
     } else {
       const int64_t work = (int64_t)n * L.h_out * ((L.w_out + 1) / 2);          // one thread per pixel pair
       const unsigned grid = (unsigned)((work + 511) / 512);
       if (L.cin == 4)
         k_leg_layer1_direct<true><<<grid, 512, w_bytes, s>>>(d_input, h->d_w[0], h->d_b[0], n, L.h_in, L.w_in, L.cin, L.kh, L.kw,
-                                                            L.sh, L.sw, L.h_out, L.w_out, L.relu, t->actp[0]);
+                                                            L.sh, L.sw, L.h_out, L.w_out, L.relu, t->actp[0], h->d_err);
       else
         k_leg_layer1_direct<false><<<grid, 512, w_bytes, s>>>(d_input, h->d_w[0], h->d_b[0], n, L.h_in, L.w_in, L.cin, L.kh, L.kw,
-                                                             L.sh, L.sw, L.h_out, L.w_out, L.relu, t->actp[0]);
+                                                             L.sh, L.sw, L.h_out, L.w_out, L.relu, t->actp[0], h->d_err);
     }
     OVN_LAUNCH_CHECK(h);
   }
   int cur = 0;
-  for (int l = 1; l < h->n_leg; ++l) {
+  for (int l = 1; l < h->n_leg && l <= stop_layer; ++l) {
     const ConvSpec& L = h->leg[l];
     const bool last = (l == h->n_leg - 1);
     const int nz = (L.cout + 63) / 64;
@@ -1451,7 +1471,7 @@ int leg_forward_tc(ovn_handle* h, const float* d_input, int n, float* d_fv, cuda
     la.in_run_planes = L.sh * 2 * (L.cin / 8); la.kh = L.kh; la.kw = L.kw; la.c8in = L.cin / 8; la.Bp = t->wres[l];
     la.bias = h->d_b[l]; la.n_valid = L.cout; la.M = L.w_out; la.out_planes = t->actp[cur ^ 1]; la.out_pitch = L.w_out;
     la.out_run_planes = 2 * (L.cout / 8); la.out_f32 = d_fv;
-    la.n_split = leg_split(h, L, n); la.part = t->leg_part;
+    la.n_split = leg_split(h, L, n); la.part = t->leg_part; la.err = h->d_err;
     const dim3 grid((unsigned)(n * L.h_out), (unsigned)((L.w_out + MMA_ROWS - 1) / MMA_ROWS), (unsigned)(nz * la.n_split));
     if (la.n_split > 1) {
       k_leg_mma<5><<<grid, MMA_THREADS, 0, s>>>(la);
@@ -1741,6 +1761,31 @@ int tc_copy_heads_stage(ovn_handle* h, int stage, int64_t first, int64_t count, 
   const int64_t total = count * per;
   k_copy_heads_stage<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(stage, t->o1, t->x3, t->rows_pad, t->partial, first,
                                                                        total, d_out);
+  OVN_LAUNCH_CHECK(h);
+  return OVN_OK;
+}
+
+// ovn_leg_stage: the hi / lo planes of one leg layer ([img][y][hi, lo][c8][x][8] fp16, leg_forward_tc) as two NHWC
+// float32 arrays [n][h_out][w_out][cout]; a copy and a conversion only.  One thread per output element.
+__global__ void __launch_bounds__(256)
+k_copy_leg_stage(const __half* __restrict__ planes, int w_out, int cout, int64_t total, float* __restrict__ hi,
+                 float* __restrict__ lo) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= total) return;
+  const int c = (int)(e % cout), x = (int)(e / cout % w_out);
+  const int64_t row = e / cout / w_out;                                  // img * h_out + y
+  const int c8n = cout / 8;
+  const __half* p = planes + ((size_t)(row * 2 * c8n + (c >> 3)) * w_out + x) * 8 + (c & 7);
+  hi[e] = __half2float(p[0]);
+  lo[e] = __half2float(p[(size_t)c8n * w_out * 8]);
+}
+
+int tc_leg_stage(ovn_handle* h, const float* d_input, int n, int layer, float* d_hi, float* d_lo, cudaStream_t s) {
+  const int rc = leg_forward_tc(h, d_input, n, nullptr, s, layer);
+  if (rc != OVN_OK) return rc;
+  const ConvSpec& L = h->leg[layer];
+  const int64_t total = (int64_t)n * L.h_out * L.w_out * L.cout;
+  k_copy_leg_stage<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->tc->actp[layer & 1], L.w_out, L.cout, total, d_hi, d_lo);
   OVN_LAUNCH_CHECK(h);
   return OVN_OK;
 }

@@ -314,6 +314,23 @@ class Engine:
     check(self._h, lib().ovn_leg_forward(self._h, _ptr(x), n, _ptr(out), self._stream()), 'ovn_leg_forward')
     return out
 
+  def leg_stage(self, x_nhwc, layer):
+    """ovn_leg_stage (precision f16_tc): the leg's own launches on [n <= max_batch_scans, H, W, C] scans up to leg
+    layer ``layer`` (0 = s_conv1 ... the last but one) -> (hi, lo), float32 cuda [n, h_out, w_out, cout]: the fp16
+    halves of that layer's activations as the next layer reads them."""
+    x = x_nhwc.contiguous()
+    h, w, cout = self.H, self.W, self.C
+    s1 = tuple(self.model.get('strides_layer1', (2, 2)))
+    table = [r for r in _weights.LEG_TABLE if r[0] in self.leg_layers]
+    for name, kh, kw, sh, sw, cout, _ in table[:int(layer) + 1]:
+      sh, sw = s1 if sh is None else (sh, sw)
+      h, w = (h - kh) // sh + 1, (w - kw) // sw + 1
+    hi, lo = (torch.empty((x.shape[0], h, w, cout), dtype=torch.float32, device=self.device) for _ in range(2))
+    # the library refuses a layer outside [0, leg layers - 2] and more than max_batch_scans scans before it writes
+    check(self._h, lib().ovn_leg_stage(self._h, _ptr(x), int(x.shape[0]), int(layer), _ptr(hi), _ptr(lo), self._stream()),
+          'ovn_leg_stage')
+    return hi, lo
+
   def heads(self, bank, left_idx, right_idx, want_corr=False):
     """LEFT = bank[left_idx], RIGHT = bank[right_idx] -> (overlap [n] f32, yaw [n] i32, corr|None)."""
     n = left_idx.numel()

@@ -106,6 +106,36 @@ def test_pipeline_failure_is_reported(bank_np):
   eng.close()
 
 
+@pytest.mark.parametrize('n', [1, 3])
+@pytest.mark.parametrize('what', ['nan pixel', 'inf pixel', '-inf pixel', 'activation above 65504'])
+def test_tensor_core_leg_reports_what_its_fp16_planes_cannot_hold(what, n):
+  """The tensor-core leg hands each layer's activations to the next as hi / lo fp16 planes.  A NaN or infinite
+  input pixel, or an activation above 65504 (hi = inf, lo = -inf, NaN in the next layer's MMAs, which its ReLU
+  turns into 0), used to come back as an ordinary finite volume with OVN_OK.  The kernel that writes the planes
+  now raises the deferred error: one scan (k_leg_layer1_small, k_leg_splitk_reduce) and a batch of 3
+  (k_leg_layer1_direct, k_leg_mma's own epilogue).  The fp32 leg has no fp16 planes and propagates the value."""
+  w = N.glorot_weights(4, MODEL, seed=0)
+  x = synth.range_like_images(1234, n, 4)
+  eng = Engine(model=MODEL, precision='f16_tc', max_batch_scans=n, max_batch_pairs=1)
+  eng.load_weights(w)
+  good = eng.leg(torch.from_numpy(x).to(eng.device)).clone()
+  eng.check()
+  if what == 'activation above 65504':               # s_conv5's activations reach 2.9 with these weights: x 2^15
+    f = np.float32(2.0 ** 15)
+    eng.load_weights(dict(w, s_conv5=(w['s_conv5'][0] * f, w['s_conv5'][1] * f)))
+    bad = x
+  else:
+    bad = x.copy()
+    bad[n - 1, 40, 451, 0] = {'nan pixel': np.nan, 'inf pixel': np.inf, '-inf pixel': -np.inf}[what]
+  fv = eng.leg(torch.from_numpy(bad).to(eng.device))
+  with pytest.raises(OvnError, match='OVN_ERR_INVALID_ARG.*tensor-core leg'):
+    eng.check()
+  eng.load_weights(w)                                  # the flag is cleared when reported: the handle keeps working
+  assert torch.equal(eng.leg(torch.from_numpy(x).to(eng.device)), good)
+  eng.check()
+  eng.close()
+
+
 def test_failed_workspace_allocation_leaves_handle_usable():
   """A projection whose rank workspace is larger than the device is refused by cudaMalloc before any kernel
   runs.  The handle reports OVN_ERR_CUDA once, then projects like a fresh handle: the workspace, which held

@@ -412,7 +412,8 @@ def test_legs_match_oracle_at_layer1_strides(strides):
   errs = {k: float(np.abs(v.cpu().numpy() - ref).max() / scale) for k, v in fv.items()}
   between = (fv['tc5'] - fv['tc1']).abs().max().item() / scale
   print('\n[geometry] strides %s (%d x %d): leg rel err %s, 1 vs 5 scans %.2e' % (strides, H, W, errs, between))
-  assert errs['tc1'] <= 4e-3 and errs['tc5'] <= 1e-4 and errs['fp32'] <= 2e-5, errs
+  # one scan per call is K-sliced, five are one accumulation chain per layer (tests/test_gpu_network.py, LEG_TC_TOL_*)
+  assert errs['tc1'] <= 2e-5 and errs['tc5'] <= 1e-4 and errs['fp32'] <= 2e-5, errs
   assert between <= 1e-4
   # the tensor-core heads once on these volumes
   tc = engs['tc5']

@@ -85,7 +85,7 @@ def test_infer_api_matches_reference_semantics(dataset, prec):
   fv = inf.create_feature_volumes(['000000', '000003'])
   fv_r = ref.create_feature_volumes(['000000', '000003'])
   assert fv.shape == (2, 1, 360, 128) and fv.dtype == np.float32
-  assert np.abs(fv - fv_r).max() / np.abs(fv_r).max() <= (2e-5 if prec == 'fp32' else 4e-3)
+  assert np.abs(fv - fv_r).max() / np.abs(fv_r).max() <= (2e-5 if prec == 'fp32' else 1e-4)
 
   # ---- infer_multiple: stateful bank, ids must come 0,1,2,...
   assert inf.infer_multiple(0, []) is None and ref.infer_multiple(0, []) is None

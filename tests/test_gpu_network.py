@@ -47,7 +47,17 @@ def setup():
   return w, x, fv_ref
 
 
-@pytest.mark.parametrize('prec,leg_tol', [('fp32', 2e-5), ('f16_tc', 4e-3)])
+# End-to-end gates of the tensor-core leg, as max |error| / max |volume| against the float64 oracle.  The hi / lo split
+# alone costs 1.6e-6 (tests/test_oracle_tc_leg.py); the rest is the tensor cores' truncating fp32 accumulation, which
+# errs in one direction and so grows with the length of an accumulation chain: a call of 1-2 scans cuts every layer's
+# K walk into 6-36 slices that are added with round-to-nearest (3.2e-6 .. 4.0e-6 measured on an H100 at 700 W), a
+# batch walks it in one chain (3.4e-5 .. 3.6e-5 measured; every layer sits at half its per-element bound in
+# tests/test_gpu_leg_stages.py, against 0.2-0.4 for the sliced layers).
+LEG_TC_TOL_SLICED = 2e-5
+LEG_TC_TOL_BATCH = 1e-4
+
+
+@pytest.mark.parametrize('prec,leg_tol', [('fp32', 2e-5), ('f16_tc', LEG_TC_TOL_BATCH)])
 def test_leg_matches_oracle(setup, prec, leg_tol):
   w, x, fv_ref = setup
   eng = Engine(model=MODEL, precision=prec, max_batch_scans=4, max_batch_pairs=16)
@@ -55,6 +65,7 @@ def test_leg_matches_oracle(setup, prec, leg_tol):
   fv = eng.leg(torch.from_numpy(x).to(eng.device)).cpu().numpy()      # 6 scans > max_batch_scans=4
   ref = fv_ref[:, 0]
   err = np.abs(fv - ref).max() / np.abs(ref).max()
+  print('\n[parity] leg %s, chunks of 4 and 2 scans: max rel err vs float64 oracle = %.3e' % (prec, err))
   assert err <= leg_tol, err
   assert (fv >= 0).all()
   eng.close()
@@ -137,12 +148,14 @@ def test_leg_other_channel_counts(channels, use):
   w = N.glorot_weights(channels, MODEL, seed=2)
   x = synth.range_like_images(7, 2, channels)
   ref = N.leg_forward(x, w, MODEL)[:, 0]
-  for prec, tol in (('fp32', 2e-5), ('f16_tc', 4e-3)):
+  for prec, tol in (('fp32', 2e-5), ('f16_tc', LEG_TC_TOL_SLICED)):
     eng = Engine(use=use, model=MODEL, precision=prec, max_batch_scans=2, max_batch_pairs=1)
     assert eng.C == channels
     eng.load_weights(w)
     fv = eng.leg(torch.from_numpy(x).to(eng.device)).cpu().numpy()
-    assert np.abs(fv - ref).max() / np.abs(ref).max() <= tol
+    err = np.abs(fv - ref).max() / np.abs(ref).max()
+    print('\n[parity] leg %s C=%d, 2 scans: max rel err vs float64 oracle = %.3e' % (prec, channels, err))
+    assert err <= tol, err
     eng.close()
 
 
@@ -264,8 +277,9 @@ def test_single_scan_leg_is_bit_reproducible_and_matches_batched():
   b = eng6.leg(xt)
   ref = N.leg_forward(x, w, MODEL)[:, 0]
   scale = np.abs(ref).max()
-  assert np.abs(a.cpu().numpy() - ref).max() / scale <= 4e-3
-  assert np.abs(b.cpu().numpy() - ref).max() / scale <= 4e-3
+  err1, err6 = (np.abs(t.cpu().numpy() - ref).max() / scale for t in (a, b))
+  print('\n[parity] leg f16_tc: max rel err vs float64 oracle, one scan per call %.3e, six %.3e' % (err1, err6))
+  assert err1 <= LEG_TC_TOL_SLICED and err6 <= LEG_TC_TOL_BATCH, (err1, err6)
   assert (a - b).abs().max().item() / scale <= 1e-4
   eng1.close(); eng6.close()
 
