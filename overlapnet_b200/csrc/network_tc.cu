@@ -258,11 +258,15 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 
 // ------------------------------------------------------------------------------------------------
 // k_delta_conv1_wgmma -- DeltaLayer + c_conv1 without the delta tensor (83 % of the FLOPs of a pair).
-//   GEMM per work unit (pair, jb):  o1[i, o] = sum_{dj < 15, c < 128} |L[i, c] - R[15 jb + dj, c]| W1[dj, c, o] - mu_o1[o]
-//   M = 360 LEFT rows (6 row tiles of 64, rows past 360 masked), N = 64, K = 1920 (60 W1 slices of 32 channels).
+//   GEMM per work unit (block, jb):  o1[g, o] = sum_{dj < 15, c < 128} |L[g, c] - R[15 jb + dj, c]| W1[dj, c, o] - mu_o1[o]
+//   M = the LEFT rows g of a block (6 row tiles of 64, rows past the block masked), N = 64, K = 1920 (60 W1 slices
+//   of 32 channels).  A block is a range of the flat LEFT rows g = pair * 360 + i (k4_block): in pair mode one pair's
+//   360 rows; in query mode, where every pair meets the same RIGHT volume, 384 consecutive rows that may straddle
+//   two pairs, so that no row tile multiplies padding except in the last block.
 // Warp specialisation: warpgroup 3 is the producer (one lane issues bulk copies; the warpgroup hands its registers
-// to the consumers with setmaxnreg): the LEFT volume of the current pair (90 KB, once per pair), the 15 RIGHT rows
-// of a unit (double-buffered) and W1 in groups of 5 slices (20 KB) through a 4-deep ring, each buffer guarded by a
+// to the consumers with setmaxnreg): the LEFT rows of the current block (96 KB at most, once per block, one bulk
+// copy per pair it touches), the 15 RIGHT rows of a unit (double-buffered) and W1 in groups of 5 slices (20 KB)
+// through a 3-deep ring, each buffer guarded by a
 // full / empty mbarrier pair.  Warpgroups 0-2 are the consumers (160 registers): warpgroup w owns row tiles w and
 // w + 3 (2 x 32 fp32 accumulators per thread) and commits one group of 2 wgmma per K16 step.  The A
 // operand |l - r| is synthesised in registers from the LEFT rows (kept in registers for a 32-channel chunk)
@@ -271,27 +275,44 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 // chunk (15 dj each), so the slice loop is unrolled straight-line code whose W1 descriptors and RIGHT rows are
 // fixed offsets from bases computed once per group; a RIGHT row is one 128-bit load (k4_pos).  The accumulators
 // start at the fp16-rounded -mu_o1 (the centre that k_fold_bias2 pushes through c_conv2).  Output: fp16 o1 tiles,
-// written by the consumers into a staging buffer laid out as the tiles and stored with bulk copies by a second
-// producer lane, while the consumers go on with the next unit.
-// Persistent: each CTA takes a contiguous range of the n_pairs * 24 units.
+// written by the consumers into a staging buffer laid out as the tiles and stored with bulk copies by 15 lanes of a
+// second producer warp, while the consumers go on with the next unit.
+// Persistent: each CTA takes a contiguous range of the blocks * 24 units, ordered (block, jb).
 // ------------------------------------------------------------------------------------------------
 constexpr int K4_WG = 3;                               // consumer warpgroups
 constexpr int K4_THREADS = (K4_WG + 1) * 128;          // + the producer warpgroup
 constexpr uint32_t K4_REG_PRODUCER = 32, K4_REG_CONSUMER = 160;   // per thread: 3 x 160 + 32 = 512 per SM quarter
 constexpr int K4_GROUP = 5;                            // W1 slices per bulk copy (divides the 15 dj of a chunk)
+constexpr int K4_CHUNK_GROUPS = S15 / K4_GROUP;        // W1 groups per 32-channel chunk
 constexpr int K4_NGROUPS = K4_STEPS / K4_GROUP;        // 12 per unit
 static_assert(S15 % K4_GROUP == 0, "a W1 group within one 32-channel chunk");
-constexpr int K4_RING = 4;
+constexpr int K4_RING = 3;
 constexpr int K4_BSLICE = 4096;                        // bytes of W1 per slice: [4 k8][64 o][8]
-constexpr uint32_t K4_VOL_BYTES = WF * K4_PITCH * 2;
+constexpr int K4_BLOCK_ROWS = 2 * K4_WG * 64;          // LEFT rows of a query-mode block: the 6 row tiles
 constexpr uint32_t K4_RWIN_BYTES = S15 * K4_PITCH * 2;
-// o1 staging of a unit: per di, its 24 rows exactly as they land in the o1 tiles (128 B each, chunk-swizzled), then
-// 16 bytes of padding, so that the 8 rows of a fragment store (8 consecutive i, i.e. 8 different di) hit 8
-// different 16-byte bank groups
-constexpr int K4_O1S_PITCH = NB * 64 + 8;              // fp16 per di
+// Blocks start on a multiple of 24 rows (360 and 384 are), so a block row has the parity of its volume row (the
+// k4_pos chunk order carries over), a block spans at most two pairs and at most 27 values of q = g / 15.
+static_assert(WF % NB == 0 && K4_BLOCK_ROWS % NB == 0, "blocks start on a multiple of 24 rows");
+constexpr int K4_O1S_Q = (K4_BLOCK_ROWS + S15 - 2) / S15 + 1;     // 27
+// o1 staging of a unit: per di, the rows g = 15 q + di of the block at slot q - g0 / 15, exactly as they land in the
+// o1 tiles (128 B each, chunk-swizzled), then 16 bytes of padding, so that the 8 rows of a fragment store (8
+// consecutive g, i.e. 8 different di) hit 8 different 16-byte bank groups
+constexpr int K4_O1S_PITCH = K4_O1S_Q * 64 + 8;        // fp16 per di
+
+// Block b of the n_pairs x 360 flat LEFT rows g = pair * 360 + i: rows [g0, g0 + rows).  Pair mode (a RIGHT volume
+// per pair) keeps one pair per block; query mode packs 384 rows per block, the last one partial.
+struct K4Block { int g0, rows; };
+__host__ __device__ __forceinline__ int k4_blocks(int n_pairs, int r_per_pair) {
+  return r_per_pair ? n_pairs : (n_pairs * WF + K4_BLOCK_ROWS - 1) / K4_BLOCK_ROWS;
+}
+__device__ __forceinline__ K4Block k4_block(int b, int r_per_pair, int n_pairs) {
+  if (r_per_pair) return {b * WF, WF};
+  const int g0 = b * K4_BLOCK_ROWS;
+  return {g0, min(K4_BLOCK_ROWS, n_pairs * WF - g0)};
+}
 
 struct K4Smem {
-  __half L[WF * K4_PITCH];
+  __half L[K4_BLOCK_ROWS * K4_PITCH];
   __half Rw[2][S15 * K4_PITCH];
   __half B[K4_RING][K4_GROUP * K4_BSLICE / 2];
   __half O1s[S15 * K4_O1S_PITCH];
@@ -317,7 +338,7 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
   extern __shared__ __align__(128) uint8_t smem_raw[];
   K4Smem& S = *reinterpret_cast<K4Smem*>(smem_raw);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const Share share = work_share((int64_t)n_pairs * NB, blockIdx.x, gridDim.x);
+  const Share share = work_share((int64_t)k4_blocks(n_pairs, r_per_pair) * NB, blockIdx.x, gridDim.x);
   const int u_begin = (int)share.begin, u_end = (int)share.end;
   if (tid == 0) {
     S.w1.init(K4_WG * 4);
@@ -334,40 +355,60 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
     if (warp == K4_WG * 4 && lane == 0) {
       uint32_t pi = 0, gi = 0, ui = 0;
       for (int u = u_begin; u < u_end; ++u, ++ui) {
-        const int p = u / NB, jb = u - p * NB;
+        const int b = u / NB, jb = u - b * NB;
         if (u == u_begin || jb == 0) {
-          PIPE_WAIT(S.left.acquire(pi, K4_VOL_BYTES), kErrDeltaLeftProducer);
-          bulk_g2s(S.L, L16 + (size_t)(l_idx ? l_idx[p] : p) * WF * K4_PITCH, K4_VOL_BYTES, S.left.bar(pi));
+          // rows [i0, i0 + n1) of pair p, then the block's rest from the start of pair p + 1
+          const K4Block blk = k4_block(b, r_per_pair, n_pairs);
+          const int p = blk.g0 / WF, i0 = blk.g0 - p * WF, n1 = min(blk.rows, WF - i0);
+          PIPE_WAIT(S.left.acquire(pi, blk.rows * K4_PITCH * 2), kErrDeltaLeftProducer);
+          bulk_g2s(S.L, L16 + ((size_t)(l_idx ? l_idx[p] : p) * WF + i0) * K4_PITCH, n1 * K4_PITCH * 2, S.left.bar(pi));
+          if (n1 < blk.rows)
+            bulk_g2s(S.L + n1 * K4_PITCH, L16 + (size_t)(l_idx ? l_idx[p + 1] : p + 1) * WF * K4_PITCH,
+                     (blk.rows - n1) * K4_PITCH * 2, S.left.bar(pi));
           ++pi;
         }
         PIPE_WAIT(S.right.acquire(ui, K4_RWIN_BYTES), kErrDeltaRightProducer);
-        bulk_g2s(S.Rw[S.right.slot(ui)], R16 + (r_per_pair ? (size_t)p * WF * K4_PITCH : 0) + (size_t)jb * S15 * K4_PITCH,
+        bulk_g2s(S.Rw[S.right.slot(ui)], R16 + (r_per_pair ? (size_t)b * WF * K4_PITCH : 0) + (size_t)jb * S15 * K4_PITCH,
                  K4_RWIN_BYTES, S.right.bar(ui));
         for (int grp = 0; grp < K4_NGROUPS; ++grp, ++gi) {
           PIPE_WAIT(S.w1.acquire(gi, K4_GROUP * K4_BSLICE), kErrDeltaW1Producer);
           bulk_g2s(S.B[S.w1.slot(gi)], W1p + (size_t)grp * K4_GROUP * (K4_BSLICE / 2), K4_GROUP * K4_BSLICE, S.w1.bar(gi));
         }
       }
-    } else if (warp == K4_WG * 4 + 1 && lane == 0) {
-      // o1 stores: per unit and di, one bulk copy of the staged rows, or two when the unit's 24 rows cross a
-      // 128-row o1 block (576 = 4.5 x 128)
+    } else if (warp == K4_WG * 4 + 1) {
+      // o1 stores, lane di of producer warp 1 for di < 15 (the warp shares its SM sub-partition's issue slots with
+      // consumer warps, so the 15 store loops run side by side): per unit, the block's rows g = 15 q + di,
+      // q in [qa, qb], land at o1 rows m = (q / 24) * 576 + jb * 24 + q % 24, one contiguous run per pair, each
+      // split in two where it crosses a 128-row o1 block (576 = 4.5 x 128), so up to 4 bulk copies per lane.  Each
+      // lane waits for its own copies to have read the staging buffer; lane 0 then frees it.
+      const int di = lane;
       uint32_t ui = 0;
       for (int u = u_begin; u < u_end; ++u, ++ui) {
-        const int p = u / NB, jb = u - p * NB;
-        const int64_t m0 = (int64_t)p * PAIR_ROWS + jb * NB;
-        const int n0 = min(NB, 128 - (int)(m0 & 127));
-        if (!S.o1s.wait(ui)) { atomicExch(err, kErrDeltaO1Producer); break; }
-#pragma unroll 1
-        for (int di = 0; di < S15; ++di) {
-          const __half* src = S.O1s + di * K4_O1S_PITCH;
-          bulk_s2g(o1 + o1_row_offset(m0, di), src, n0 * 128);
-          if (n0 < NB) bulk_s2g(o1 + o1_row_offset(m0 + n0, di), src + n0 * 64, (NB - n0) * 128);
+        const int b = u / NB, jb = u - b * NB;
+        const K4Block blk = k4_block(b, r_per_pair, n_pairs);
+        if (!__all_sync(0xffffffffu, S.o1s.wait(ui))) {
+          if (lane == 0) atomicExch(err, kErrDeltaO1Producer);
+          break;
         }
-        bulk_commit();
-        bulk_wait_read<0>();
-        S.o1s.release_thread(ui);
+        if (di < S15) {
+          const int q0 = blk.g0 / S15, qb = (blk.g0 + blk.rows - 1 - di) / S15;
+#pragma unroll 1
+          for (int q = (blk.g0 + S15 - 1 - di) / S15; q <= qb;) {
+            const int p = q / NB, ib = q - p * NB, len = min(qb - q + 1, NB - ib);
+            const int64_t m = (int64_t)p * PAIR_ROWS + jb * NB + ib;
+            const int n0 = min(len, 128 - (int)(m & 127));
+            const __half* src = S.O1s + di * K4_O1S_PITCH + (q - q0) * 64;
+            bulk_s2g(o1 + o1_row_offset(m, di), src, n0 * 128);
+            if (n0 < len) bulk_s2g(o1 + o1_row_offset(m + n0, di), src + n0 * 64, (len - n0) * 128);
+            q += len;
+          }
+          bulk_commit();
+          bulk_wait_read<0>();
+        }
+        __syncwarp();
+        if (lane == 0) S.o1s.release_thread(ui);
       }
-      bulk_wait<0>();                         // the next kernel reads o1
+      if (di < S15) bulk_wait<0>();           // the next kernel reads o1
     }
   } else {
     // ===================== consumers ==========================================================
@@ -382,9 +423,25 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
     }
     const uint32_t b_base = smem_u32(S.B[0]);
     uint32_t pi = 0, gi = 0, ui = 0;
+    uint32_t sto[2][2][8];                  // byte offsets of this thread's 32 o1 staging stores, set once per block
     for (int u = u_begin; u < u_end; ++u, ++ui) {
-      const int p = u / NB, jb = u - p * NB;
-      if (u == u_begin || jb == 0) { PIPE_WAIT(S.left.wait(pi), kErrDeltaLeftConsumer); ++pi; }
+      const int b = u / NB, jb = u - b * NB;
+      const K4Block blk = k4_block(b, r_per_pair, n_pairs);
+      if (u == u_begin || jb == 0) {
+        PIPE_WAIT(S.left.wait(pi), kErrDeltaLeftConsumer);
+        ++pi;
+        // Row g = 15 q + di of the block is staged at slot q - g0 / 15 of di and lands at o1 row
+        // m = (q / 24) * 576 + jb * 24 + ib with ib = q % 24, so its chunk swizzle m & 7 is ib & 7 for every jb.
+#pragma unroll
+        for (int tt = 0; tt < 2; ++tt)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int g = blk.g0 + rows[tt][h], q = g / S15, di = g - q * S15, ib = q % NB;
+            const uint32_t st = (uint32_t)offsetof(K4Smem, O1s) + 2 * (di * K4_O1S_PITCH + (q - blk.g0 / S15) * 64 + 2 * t);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) sto[tt][h][j] = st + ((j ^ (ib & 7)) << 4);
+          }
+      }
       const uint32_t wb = S.right.slot(ui);
       PIPE_WAIT(S.right.wait(ui), kErrDeltaRightConsumer);
       float acc[2][32];
@@ -401,13 +458,13 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
       uint32_t Lr[2][2][4];                   // LEFT values of the chunk: [tile][row a / b][kk0 lo, hi, kk1 lo, hi]
 #pragma unroll 1
       for (int grp = 0; grp < K4_NGROUPS; ++grp, ++gi) {
-        const int cc = grp / 3, dj0 = (grp - 3 * cc) * K4_GROUP;
+        const int cc = grp / K4_CHUNK_GROUPS, dj0 = (grp - K4_CHUNK_GROUPS * cc) * K4_GROUP;
         if (dj0 == 0) {
 #pragma unroll
           for (int tt = 0; tt < 2; ++tt)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-              const int r = rows[tt][h] < WF ? rows[tt][h] : WF - 1;
+              const int r = rows[tt][h] < blk.rows ? rows[tt][h] : blk.rows - 1;
               const uint4 v = *reinterpret_cast<const uint4*>(S.L + r * K4_PITCH + ((cc ^ (r & 1)) << 5) + 8 * t);
               Lr[tt][h][0] = v.x; Lr[tt][h][1] = v.y; Lr[tt][h][2] = v.z; Lr[tt][h][3] = v.w;
             }
@@ -453,21 +510,16 @@ k_delta_conv1_wgmma(const __half* __restrict__ L16, const int32_t* __restrict__ 
       }
       S.right.release(ui);
       if (jb == NB - 1 || u == u_end - 1) S.left.release(pi - 1);
-      // o1 into the staging buffer, once the store lane's copies of the previous unit have read it.  Row m of the
-      // unit is pair * 576 + jb * 24 + ib, so its chunk swizzle m & 7 is ib & 7.
+      // o1 into the staging buffer, once the store warp's copies of the previous unit have read it
       if (!S.o1s.wait_free(ui)) { atomicExch(err, kErrDeltaO1Consumer); goto done; }
 #pragma unroll
       for (int tt = 0; tt < 2; ++tt)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int i = rows[tt][h];
-          if (i >= WF) continue;
-          const int ibk = i / S15, di = i - ibk * S15;
-          __half* st = S.O1s + di * K4_O1S_PITCH + ibk * 64 + 2 * t;
+          if (rows[tt][h] >= blk.rows) continue;
 #pragma unroll
           for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<uint32_t*>(st + ((j ^ (ibk & 7)) << 3)) =
-                pack_h2(acc[tt][4 * j + 2 * h], acc[tt][4 * j + 2 * h + 1]);
+            *reinterpret_cast<uint32_t*>(smem_raw + sto[tt][h][j]) = pack_h2(acc[tt][4 * j + 2 * h], acc[tt][4 * j + 2 * h + 1]);
         }
       fence_proxy_async_smem();
       S.o1s.publish(ui);
@@ -1665,7 +1717,7 @@ int heads_forward_tc(ovn_handle* h, const float* d_bank, const float* d_query, c
   const int grid2 = tiles < h->sm_count ? (int)tiles : h->sm_count;
   const int grid3 = 2 * tiles < h->sm_count ? (int)(2 * tiles) : h->sm_count;
   prof_mark(h, PROF_DELTA, s);
-  const int64_t units = (int64_t)n * NB;
+  const int64_t units = (int64_t)k4_blocks(n, d_query ? 0 : 1) * NB;
   const int grid4 = units < h->sm_count ? (int)units : h->sm_count;
   k_delta_conv1_wgmma<<<grid4, K4_THREADS, sizeof(K4Smem), s>>>(l16, lidx, t->r16, d_query ? 0 : 1, t->w1p, t->mu_o1, t->o1,
                                                                n, h->d_err);
