@@ -178,6 +178,18 @@ int ovn_preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* d_
                          int32_t n_scans, int64_t n_points_total, const float* d_probs,
                          float* d_input, void* stream);
 
+/* The fused path with every cue as the reference's cue files give it.  Depth, normals and intensity are
+ * gen_depth/normal/intensity_data.py's (the configured max_range); the class probabilities are
+ * gen_semantic_data.py:33-46's: projected with max_range = inf (:39), and the probabilities of each pixel's
+ * nearest point are read from the scan's RAW probability array at that point's index among the points with
+ * 0 < depth < inf (:41-46, the reference's filtered-index quirk).  So d_input equals ovn_pack_input of those
+ * four cues bit for bit, from one scatter (two key images per scan) and one gather.  d_probs:
+ * [n_points_total][n_prob_channels] float32 (device), required iff n_prob_channels > 0, NULL otherwise
+ * (OVN_ERR_INVALID_ARG); on a handle without probability channels this is ovn_preprocess_batch. */
+int ovn_preprocess_cues_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets,
+                              int32_t n_scans, int64_t n_points_total, const float* d_probs,
+                              float* d_input, void* stream);
+
 /* Pack separately computed cue images into the NHWC network input (same channel order). */
 int ovn_pack_input(ovn_handle* h, const float* d_depth, const float* d_normal, const float* d_prob,
                    const float* d_intensity, int32_t n_scans, float* d_input, void* stream);
@@ -459,15 +471,29 @@ int ovn_leg_stage(ovn_handle* h, const float* d_input, int32_t n_scans, int32_t 
                   void* stream);
 
 /* ---- host-buffer convenience entry points (what a non-CUDA caller binds; bench.py e2e) ------ */
-/* Raw clouds on the host -> feature volumes on the host. */
+/* Raw clouds on the host -> feature volumes on the host.  OVN_ERR_BAD_CONFIG on a handle with
+ * probability channels. */
 int ovn_encode_clouds_host(ovn_handle* h, const float* h_points, const int64_t* h_offsets,
                            int32_t n_scans, float* h_fv);
 /* One raw query cloud on the host vs a device-resident bank: preprocess + leg + heads.
- * h_overlap [n_cand], h_yaw [n_cand]; h_query_fv [360][128] may be NULL. */
+ * h_overlap [n_cand], h_yaw [n_cand]; h_query_fv [360][128] may be NULL.  OVN_ERR_BAD_CONFIG on a
+ * handle with probability channels. */
 int ovn_query_cloud_vs_bank_host(ovn_handle* h, const float* h_points, int64_t n_points,
                                  const float* d_bank, int64_t bank_size,
                                  const int32_t* h_cand_idx, int32_t n_cand,
                                  float* h_overlap, int32_t* h_yaw, float* h_query_fv);
+/* The same two with per-point class probabilities, through ovn_preprocess_cues_batch: the semantic
+ * cue as gen_semantic_data.py:33-46 makes it from the clouds and their .label files.  h_probs:
+ * [n_points][n_prob_channels] float32 host rows, one per point of h_points, in the same order;
+ * required iff the handle has probability channels (else NULL; OVN_ERR_INVALID_ARG).  The rows are
+ * staged next to the cloud (80 B per point at 20 classes); the query keeps its one host
+ * synchronisation. */
+int ovn_encode_clouds_probs_host(ovn_handle* h, const float* h_points, const int64_t* h_offsets,
+                                 int32_t n_scans, const float* h_probs, float* h_fv);
+int ovn_query_cloud_probs_vs_bank_host(ovn_handle* h, const float* h_points, int64_t n_points,
+                                       const float* h_probs, const float* d_bank, int64_t bank_size,
+                                       const int32_t* h_cand_idx, int32_t n_cand,
+                                       float* h_overlap, int32_t* h_yaw, float* h_query_fv);
 
 #ifdef __cplusplus
 }

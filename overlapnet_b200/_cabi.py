@@ -16,7 +16,7 @@ SYMBOLS = [
     'ovn_abi_version', 'ovn_input_channels', 'ovn_feature_width', 'ovn_feature_channels',
     'ovn_launch_count', 'ovn_profile_enable', 'ovn_profile_read', 'ovn_set_weights', 'ovn_finalize_weights', 'ovn_project_batch',
     'ovn_normals_batch', 'ovn_semantic_batch', 'ovn_gt_range_batch', 'ovn_gt_overlap_count', 'ovn_gt_scan_radius',
-    'ovn_gt_pairs_count', 'ovn_preprocess_batch',
+    'ovn_gt_pairs_count', 'ovn_preprocess_batch', 'ovn_preprocess_cues_batch',
     'ovn_pack_input',
     'ovn_leg_forward', 'ovn_heads_forward', 'ovn_heads_1vsN', 'ovn_bank_prepare', 'ovn_bank_release', 'ovn_encode_clouds_host',
     'ovn_query_cloud_vs_bank_host', 'ovn_check', 'ovn_set_feature_center', 'ovn_get_feature_center',
@@ -27,7 +27,7 @@ SYMBOLS = [
     'ovn_copy_net_volumes', 'ovn_copy_train_state', 'ovn_set_train_state',
     'ovn_train_workspace_bytes', 'ovn_host_register', 'ovn_host_unregister', 'ovn_stage_rows',
     'ovn_head_gradients_chunks', 'ovn_net_gradients_chunks', 'ovn_copy_heads_stage',
-    'ovn_heads_stage_pairs', 'ovn_leg_stage',
+    'ovn_heads_stage_pairs', 'ovn_leg_stage', 'ovn_encode_clouds_probs_host', 'ovn_query_cloud_probs_vs_bank_host',
 ]
 HEADS_STAGES = {'o1': 0, 'x3': 1, 'dense': 2, 'centres': 3}     # ovn_heads_stage
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
@@ -91,6 +91,7 @@ def lib():
   L.ovn_gt_pairs_count.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, i32, f32, i32, i32, vp, i64, vp, vp]
   L.ovn_semantic_batch.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp]
   L.ovn_preprocess_batch.argtypes = [vp, vp, vp, i32, i64, vp, vp, vp]
+  L.ovn_preprocess_cues_batch.argtypes = [vp, vp, vp, i32, i64, vp, vp, vp]
   L.ovn_pack_input.argtypes = [vp, vp, vp, vp, vp, i32, vp, vp]
   L.ovn_leg_forward.argtypes = [vp, vp, i32, vp, vp]
   L.ovn_heads_forward.argtypes = [vp, vp, i64, vp, vp, i32, vp, vp, vp, vp]
@@ -129,6 +130,8 @@ def lib():
   L.ovn_get_gradients.argtypes = [vp, C.c_char_p, vp, vp]
   L.ovn_encode_clouds_host.argtypes = [vp, vp, vp, i32, vp]
   L.ovn_query_cloud_vs_bank_host.argtypes = [vp, vp, i64, vp, i64, vp, i32, vp, vp, vp]
+  L.ovn_encode_clouds_probs_host.argtypes = [vp, vp, vp, i32, vp, vp]
+  L.ovn_query_cloud_probs_vs_bank_host.argtypes = [vp, vp, i64, vp, vp, i64, vp, i32, vp, vp, vp]
   _lib = L
   return L
 

@@ -283,7 +283,8 @@ int ovn_create(const ovn_config* cfg, ovn_handle** out) {
   // ---- workspaces
   const size_t HW = (size_t)c.proj_H * c.proj_W;
   const size_t maxp = c.max_batch_pairs;
-  CREATE_ALLOC(h->d_keys, c.max_batch_scans * HW * sizeof(unsigned long long));
+  // a handle with probability channels keeps a second key image per scan for ovn_preprocess_cues_batch
+  CREATE_ALLOC(h->d_keys, (c.n_prob_channels > 0 ? 2 : 1) * c.max_batch_scans * HW * sizeof(unsigned long long));
   CREATE_ALLOC(h->d_input, c.max_batch_scans * HW * h->C * sizeof(float));
   CREATE_ALLOC(h->d_query_fv, (size_t)Wf * kFeatC * sizeof(float));
   CREATE_ALLOC(h->d_cand_idx, maxp * sizeof(int32_t));
@@ -565,6 +566,15 @@ int ovn_preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* d_
   REQUIRE(h, n_scans >= 0 && n_total >= 0, "negative size");
   REQUIRE(h, n_scans == 0 || (d_offsets && d_input), "NULL pointer");
   return preprocess_batch(h, d_points, d_offsets, n_scans, n_total, d_probs, d_input, (cudaStream_t)stream);
+}
+
+int ovn_preprocess_cues_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int32_t n_scans,
+                              int64_t n_total, const float* d_probs, float* d_input, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, n_scans >= 0 && n_total >= 0, "negative size");
+  REQUIRE(h, n_scans == 0 || (d_offsets && d_input), "NULL pointer");
+  return preprocess_cues_batch(h, d_points, d_offsets, n_scans, n_total, d_probs, d_input, (cudaStream_t)stream);
 }
 
 int ovn_pack_input(ovn_handle* h, const float* d_depth, const float* d_normal, const float* d_prob,
@@ -1138,11 +1148,50 @@ int ovn_bank_release(ovn_handle* h, const float* d_bank) {
 }
 
 // ---- host-buffer entry points ---------------------------------------------------------------------
-static int ensure_stage(ovn_handle* h, int64_t n_points) {
-  const size_t point_bytes = 4 * sizeof(float);
+// d_stage_points holds the staged cloud, [n_points][4], then its probabilities, [n_points][n_prob]
+static int ensure_stage(ovn_handle* h, int64_t n_points, int n_prob = 0) {
+  const size_t point_bytes = (4 + n_prob) * sizeof(float);
   const int rc = h->d_stage_points.ensure(h, n_points * point_bytes, (n_points + n_points / 8 + 4096) * point_bytes);
   if (rc != OVN_OK) return rc;
   return h->d_stage_offsets.ensure(h, ((size_t)h->cfg.max_batch_scans + 1) * sizeof(int64_t));
+}
+
+// ovn_encode_clouds_host and ovn_encode_clouds_probs_host after their argument checks; h_probs is NULL or
+// [n_points][n_prob_channels]
+static int encode_clouds_host(ovn_handle* h, const float* h_points, const int64_t* h_offsets, int32_t n_scans,
+                              const float* h_probs, float* h_fv) {
+  cudaStream_t s = h->own_stream;
+  const int Wf = h->cfg.leg_output_width;
+  const int n_prob = h_probs ? h->cfg.n_prob_channels : 0;
+  Buffer<float> d_fv;
+  int rc = d_fv.ensure(h, (size_t)h->cfg.max_batch_scans * Wf * kFeatC * sizeof(float));
+  if (rc != OVN_OK) return rc;
+  for (int s0 = 0; s0 < n_scans; s0 += h->cfg.max_batch_scans) {
+    const int n = (n_scans - s0 < h->cfg.max_batch_scans) ? n_scans - s0 : h->cfg.max_batch_scans;
+    const int64_t p0 = h_offsets[s0], p1 = h_offsets[s0 + n];
+    rc = ensure_stage(h, p1 - p0, n_prob);
+    if (rc != OVN_OK) return rc;
+    std::vector<int64_t> rel(n + 1);
+    for (int i = 0; i <= n; ++i) rel[i] = h_offsets[s0 + i] - p0;
+    OVN_CUDA(h, cudaMemcpyAsync(h->d_stage_points, h_points + p0 * 4, (p1 - p0) * 4 * sizeof(float),
+                                cudaMemcpyHostToDevice, s));
+    float* d_probs = nullptr;
+    if (n_prob > 0) {
+      d_probs = h->d_stage_points + (p1 - p0) * 4;
+      OVN_CUDA(h, cudaMemcpyAsync(d_probs, h_probs + p0 * n_prob, (p1 - p0) * n_prob * sizeof(float),
+                                  cudaMemcpyHostToDevice, s));
+    }
+    OVN_CUDA(h, cudaMemcpyAsync(h->d_stage_offsets, rel.data(), (n + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    OVN_CUDA(h, cudaStreamSynchronize(s));   // rel is a stack-lifetime buffer
+    rc = preprocess_cues_batch(h, h->d_stage_points, h->d_stage_offsets, n, p1 - p0, d_probs, h->d_input, s);
+    if (rc == OVN_OK) rc = ovn_leg_forward(h, h->d_input, n, d_fv, s);
+    if (rc != OVN_OK) return rc;
+    OVN_CUDA(h, cudaMemcpyAsync(h_fv + (size_t)s0 * Wf * kFeatC, d_fv, (size_t)n * Wf * kFeatC * sizeof(float),
+                                cudaMemcpyDeviceToHost, s));
+    rc = check_device_error(h, s);           // synchronises s
+    if (rc != OVN_OK) return rc;
+  }
+  return OVN_OK;
 }
 
 int ovn_encode_clouds_host(ovn_handle* h, const float* h_points, const int64_t* h_offsets, int32_t n_scans,
@@ -1155,49 +1204,30 @@ int ovn_encode_clouds_host(ovn_handle* h, const float* h_points, const int64_t* 
   if (h->cfg.n_prob_channels != 0)
     OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_encode_clouds_host: semantic channels need per-point probabilities; "
                 "use the device-pointer stages");
-  cudaStream_t s = h->own_stream;
-  const int Wf = h->cfg.leg_output_width;
-  Buffer<float> d_fv;
-  int rc = d_fv.ensure(h, (size_t)h->cfg.max_batch_scans * Wf * kFeatC * sizeof(float));
-  if (rc != OVN_OK) return rc;
-  for (int s0 = 0; s0 < n_scans; s0 += h->cfg.max_batch_scans) {
-    const int n = (n_scans - s0 < h->cfg.max_batch_scans) ? n_scans - s0 : h->cfg.max_batch_scans;
-    const int64_t p0 = h_offsets[s0], p1 = h_offsets[s0 + n];
-    rc = ensure_stage(h, p1 - p0);
-    if (rc != OVN_OK) return rc;
-    std::vector<int64_t> rel(n + 1);
-    for (int i = 0; i <= n; ++i) rel[i] = h_offsets[s0 + i] - p0;
-    OVN_CUDA(h, cudaMemcpyAsync(h->d_stage_points, h_points + p0 * 4, (p1 - p0) * 4 * sizeof(float),
-                                cudaMemcpyHostToDevice, s));
-    OVN_CUDA(h, cudaMemcpyAsync(h->d_stage_offsets, rel.data(), (n + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
-    OVN_CUDA(h, cudaStreamSynchronize(s));   // rel is a stack-lifetime buffer
-    rc = preprocess_batch(h, h->d_stage_points, h->d_stage_offsets, n, p1 - p0, nullptr, h->d_input, s);
-    if (rc == OVN_OK) rc = ovn_leg_forward(h, h->d_input, n, d_fv, s);
-    if (rc != OVN_OK) return rc;
-    OVN_CUDA(h, cudaMemcpyAsync(h_fv + (size_t)s0 * Wf * kFeatC, d_fv, (size_t)n * Wf * kFeatC * sizeof(float),
-                                cudaMemcpyDeviceToHost, s));
-    rc = check_device_error(h, s);           // synchronises s
-    if (rc != OVN_OK) return rc;
-  }
-  return OVN_OK;
+  return encode_clouds_host(h, h_points, h_offsets, n_scans, nullptr, h_fv);
 }
 
-int ovn_query_cloud_vs_bank_host(ovn_handle* h, const float* h_points, int64_t n_points, const float* d_bank,
-                                 int64_t bank_size, const int32_t* h_cand_idx, int32_t n_cand, float* h_overlap,
-                                 int32_t* h_yaw, float* h_query_fv) {
+int ovn_encode_clouds_probs_host(ovn_handle* h, const float* h_points, const int64_t* h_offsets, int32_t n_scans,
+                                 const float* h_probs, float* h_fv) {
   if (!h) return OVN_ERR_INVALID_ARG;
   DeviceGuard guard(h);
-  REQUIRE(h, n_points >= 0 && n_cand >= 0, "negative size");
-  REQUIRE(h, h_points, "h_points is NULL");
-  REQUIRE(h, n_cand == 0 || (d_bank && h_overlap && h_yaw), "NULL pointer");
-  REQUIRE(h, n_cand == 0 || bank_size > 0, "bank_size must be positive");
-  REQUIRE(h, h_cand_idx != nullptr || n_cand <= bank_size, "n_cand exceeds bank_size");
-  if (h->cfg.n_prob_channels != 0)
-    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_query_cloud_vs_bank_host: semantic channels are not supported here");
+  REQUIRE(h, n_scans >= 0, "negative size");
+  if (n_scans == 0) return OVN_OK;
+  REQUIRE(h, h_points && h_offsets && h_fv, "NULL pointer");
+  REQUIRE(h, (h_probs != nullptr) == (h->cfg.n_prob_channels != 0),
+          "h_probs must be given exactly when the handle has probability channels");
+  return encode_clouds_host(h, h_points, h_offsets, n_scans, h_probs, h_fv);
+}
+
+// ovn_query_cloud_vs_bank_host and ovn_query_cloud_probs_vs_bank_host after their argument checks
+static int query_cloud_vs_bank_host(ovn_handle* h, const float* h_points, int64_t n_points, const float* h_probs,
+                                    const float* d_bank, int64_t bank_size, const int32_t* h_cand_idx,
+                                    int32_t n_cand, float* h_overlap, int32_t* h_yaw, float* h_query_fv) {
   if (n_cand > h->cfg.max_batch_pairs)
     OVN_SET_ERR(h, OVN_ERR_CAPACITY, "n_cand=%d exceeds max_batch_pairs=%d", n_cand, h->cfg.max_batch_pairs);
   cudaStream_t s = h->own_stream;
-  int rc = ensure_stage(h, n_points);
+  const int n_prob = h_probs ? h->cfg.n_prob_channels : 0;
+  int rc = ensure_stage(h, n_points, n_prob);
   if (rc != OVN_OK) return rc;
   const int Wf = h->cfg.leg_output_width;
   // Everything the device reads or writes asynchronously lives in the pinned staging, so the call has ONE host sync.
@@ -1209,12 +1239,17 @@ int ovn_query_cloud_vs_bank_host(ovn_handle* h, const float* h_points, int64_t n
   // the bank's operand copies may have been prepared on another stream (ovn_bank_prepare records ev_bank)
   OVN_CUDA(h, cudaStreamWaitEvent(s, h->ev_bank, 0));
   OVN_CUDA(h, cudaMemcpyAsync(h->d_stage_points, h_points, (size_t)n_points * 4 * sizeof(float), cudaMemcpyHostToDevice, s));
+  float* d_probs = nullptr;
+  if (n_prob > 0) {
+    d_probs = h->d_stage_points + (size_t)n_points * 4;
+    OVN_CUDA(h, cudaMemcpyAsync(d_probs, h_probs, (size_t)n_points * n_prob * sizeof(float), cudaMemcpyHostToDevice, s));
+  }
   OVN_CUDA(h, cudaMemcpyAsync(h->d_stage_offsets, p_offs, 2 * sizeof(int64_t), cudaMemcpyHostToDevice, s));
   if (h_cand_idx && n_cand > 0) {
     memcpy(p_idx, h_cand_idx, (size_t)n_cand * sizeof(int32_t));
     OVN_CUDA(h, cudaMemcpyAsync(h->d_cand_idx, p_idx, (size_t)n_cand * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   }
-  rc = preprocess_batch(h, h->d_stage_points, h->d_stage_offsets, 1, n_points, nullptr, h->d_input, s);
+  rc = preprocess_cues_batch(h, h->d_stage_points, h->d_stage_offsets, 1, n_points, d_probs, h->d_input, s);
   if (rc != OVN_OK) return rc;
   rc = ovn_leg_forward(h, h->d_input, 1, h->d_query_fv, s);
   if (rc != OVN_OK) return rc;
@@ -1237,6 +1272,38 @@ int ovn_query_cloud_vs_bank_host(ovn_handle* h, const float* h_points, int64_t n
     memcpy(h_yaw, p_yaw, (size_t)n_cand * sizeof(int32_t));
   }
   return rc;
+}
+
+int ovn_query_cloud_vs_bank_host(ovn_handle* h, const float* h_points, int64_t n_points, const float* d_bank,
+                                 int64_t bank_size, const int32_t* h_cand_idx, int32_t n_cand, float* h_overlap,
+                                 int32_t* h_yaw, float* h_query_fv) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, n_points >= 0 && n_cand >= 0, "negative size");
+  REQUIRE(h, h_points, "h_points is NULL");
+  REQUIRE(h, n_cand == 0 || (d_bank && h_overlap && h_yaw), "NULL pointer");
+  REQUIRE(h, n_cand == 0 || bank_size > 0, "bank_size must be positive");
+  REQUIRE(h, h_cand_idx != nullptr || n_cand <= bank_size, "n_cand exceeds bank_size");
+  if (h->cfg.n_prob_channels != 0)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_query_cloud_vs_bank_host: semantic channels are not supported here");
+  return query_cloud_vs_bank_host(h, h_points, n_points, nullptr, d_bank, bank_size, h_cand_idx, n_cand, h_overlap,
+                                  h_yaw, h_query_fv);
+}
+
+int ovn_query_cloud_probs_vs_bank_host(ovn_handle* h, const float* h_points, int64_t n_points, const float* h_probs,
+                                       const float* d_bank, int64_t bank_size, const int32_t* h_cand_idx,
+                                       int32_t n_cand, float* h_overlap, int32_t* h_yaw, float* h_query_fv) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, n_points >= 0 && n_cand >= 0, "negative size");
+  REQUIRE(h, h_points, "h_points is NULL");
+  REQUIRE(h, n_cand == 0 || (d_bank && h_overlap && h_yaw), "NULL pointer");
+  REQUIRE(h, n_cand == 0 || bank_size > 0, "bank_size must be positive");
+  REQUIRE(h, h_cand_idx != nullptr || n_cand <= bank_size, "n_cand exceeds bank_size");
+  REQUIRE(h, (h_probs != nullptr) == (h->cfg.n_prob_channels != 0),
+          "h_probs must be given exactly when the handle has probability channels");
+  return query_cloud_vs_bank_host(h, h_points, n_points, h_probs, d_bank, bank_size, h_cand_idx, n_cand, h_overlap,
+                                  h_yaw, h_query_fv);
 }
 
 }  // extern "C"

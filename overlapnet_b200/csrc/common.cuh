@@ -163,7 +163,8 @@ struct ovn_handle {
   ovn::Buffer<float> d_b[ovn::kMaxLegLayers + 4];
 
   // workspaces, allocated by ovn_create unless noted
-  ovn::Buffer<unsigned long long> d_keys;    // [max_batch_scans][H*W] atomic-min keys
+  ovn::Buffer<unsigned long long> d_keys;    // [max_batch_scans][H*W] atomic-min keys; twice that with probability
+                                             //   channels (the two key images of ovn_preprocess_cues_batch)
   ovn::Buffer<unsigned long long> d_pair_keys; // ovn_gt_pairs_count: [tile_cur][tile_ref][H*W] keys, grown on use
   ovn::Buffer<uint8_t> d_pair_prune;         // ovn_gt_pairs_count: pruned-pair counter + [n_cur][n_ref] flags, grown on use
   ovn::Buffer<uint32_t> d_valid_words;       // validity bitmask, 1 bit per point; these three grow with the points
@@ -310,6 +311,8 @@ int semantic_batch(ovn_handle* h, const int32_t* d_idx, const float* d_probs,
                    cudaStream_t s);
 int preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans,
                      int64_t n_total, const float* d_probs, float* d_input, cudaStream_t s);
+int preprocess_cues_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans,
+                          int64_t n_total, const float* d_probs, float* d_input, cudaStream_t s);
 int gt_range_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans, int64_t n_total,
                    const double* d_pose_ref, const double* d_pose_cur_inv, float max_range, float* d_range,
                    cudaStream_t s);

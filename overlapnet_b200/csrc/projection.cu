@@ -125,7 +125,12 @@ __device__ __forceinline__ int find_scan(const int64_t* __restrict__ offsets, in
 
 // ------------------------------------------------------------------------------------------
 // K1: scatter.  grid = ceil(n_total / 256), block = 256.
+// kCues (ovn_preprocess_cues_batch): two key images per call, keys = A [n_scans][H*W] then B [n_scans][H*W].  A takes
+// the points of the configured filter (0 < depth < max_range, utils.py:76-77), B those of the semantic cue's
+// (0 < depth < inf, gen_semantic_data.py:39; NaN fails both).  The bins are computed once per point, and the
+// validity bits (the ranks) follow B's filter: the probability gather indexes with B's filtered index.
 // ------------------------------------------------------------------------------------------
+template <bool kCues>
 __global__ void __launch_bounds__(256)
 k_project_scatter(const float4* __restrict__ pts, const int64_t* __restrict__ offsets, int n_scans,
                   int64_t n_total, ProjParams P, unsigned long long* __restrict__ keys,
@@ -145,7 +150,8 @@ k_project_scatter(const float4* __restrict__ pts, const int64_t* __restrict__ of
     // utils.py:75  np.linalg.norm(xyz, 2, axis=1): sqrt((x*x + y*y) + z*z), float32, no FMA
     const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(p.x, p.x), __fmul_rn(p.y, p.y)), __fmul_rn(p.z, p.z));
     const float depth = __fsqrt_rn(d2);
-    valid = (depth > 0.0f) && (depth < P.max_range);       // utils.py:76-77
+    const bool in_a = (depth > 0.0f) && (depth < P.max_range);   // utils.py:76-77
+    valid = kCues ? (depth > 0.0f) && (depth < __int_as_float(0x7f800000)) : in_a;
     if (valid) {
       // Bins: the exact answer is floor(P(fl32(angle))) with P the reference's float32 pipeline (bin_x /
       // bin_y, monotone) and fl32 the correctly rounded float32 angle.  Fast path: ONE fused estimate
@@ -188,7 +194,9 @@ k_project_scatter(const float4* __restrict__ pts, const int64_t* __restrict__ of
       }
       const uint32_t local = (uint32_t)(g - offsets[b]);
       const unsigned long long key = ((unsigned long long)__float_as_uint(depth) << 32) | local;
-      atomicMin(keys + (size_t)b * P.H * P.W + (size_t)by * P.W + bx, key);
+      const size_t pix = (size_t)b * P.H * P.W + (size_t)by * P.W + bx;
+      if (!kCues || in_a) atomicMin(keys + pix, key);
+      if (kCues) atomicMin(keys + (size_t)n_scans * P.H * P.W + pix, key);
     }
   }
   if (valid_words != nullptr) {
@@ -326,6 +334,9 @@ struct GatherOut {
 
 constexpr int TILE_R = 8, TILE_C = 32;
 
+// kCues: keys holds A then B (k_project_scatter<true>); depth, normals and intensity come from A's winners, the
+// probabilities from B's, indexed with B's rank (the validity bits are B's filter); out.idx is not written.
+template <bool kCues>
 __global__ void __launch_bounds__(256)
 k_project_gather(const float4* __restrict__ pts, const int64_t* __restrict__ offsets, ProjParams P,
                  const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ valid_words,
@@ -367,7 +378,7 @@ k_project_gather(const float4* __restrict__ pts, const int64_t* __restrict__ off
   const bool has = depth > 0.0f;   // valid points have depth > 0; empty pixels hold -1
 
   int32_t fidx = -1;
-  if (has && (out.idx != nullptr || out.n_prob > 0)) {
+  if (!kCues && has && (out.idx != nullptr || out.n_prob > 0)) {
     // index into the FILTERED cloud (utils.py:76,117-118)
     fidx = (int32_t)(valid_before(valid_words, word_prefix, off + s_local[ty][tx]) -
                      valid_before(valid_words, word_prefix, off));
@@ -397,8 +408,17 @@ k_project_gather(const float4* __restrict__ pts, const int64_t* __restrict__ off
       if (out.c_intensity >= 0) o[out.c_intensity] = has ? p.w : -1.0f;
       if (out.c_prob >= 0) {
         // gen_semantic_data.py:46 -- raw probs indexed with the filtered index (reference quirk)
-        const float* src = out.probs + (size_t)(off + (has ? fidx : 0)) * out.n_prob;
-        for (int c = 0; c < out.n_prob; ++c) o[out.c_prob + c] = has ? __ldg(src + c) : -1.0f;
+        bool has_p = has;
+        int32_t pidx = fidx;
+        if (kCues) {   // B's winner and its rank among the points of 0 < depth < inf (gen_semantic_data.py:39-46)
+          const unsigned long long k = keys[((size_t)gridDim.z + b) * P.H * P.W + (size_t)y * P.W + x];
+          has_p = k != kEmptyKey;
+          if (has_p)
+            pidx = (int32_t)(valid_before(valid_words, word_prefix, off + (uint32_t)(k & 0xFFFFFFFFull)) -
+                             valid_before(valid_words, word_prefix, off));
+        }
+        const float* src = out.probs + (size_t)(off + (has_p ? pidx : 0)) * out.n_prob;
+        for (int c = 0; c < out.n_prob; ++c) o[out.c_prob + c] = has_p ? __ldg(src + c) : -1.0f;
       }
     }
   }
@@ -511,16 +531,20 @@ static int ensure_point_capacity(ovn_handle* h, int64_t n_total) {
   return h->d_scan_tmp.ensure(h, (need / 1024 + 2) * sizeof(uint32_t), (words / 1024 + 2) * sizeof(uint32_t));
 }
 
+// cues: the two key images of ovn_preprocess_cues_batch (k_project_scatter<true>); the handle's d_keys holds them
+// only when it has probability channels (ovn_create)
 static int run_projection(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans,
-                          int64_t n_total, float max_range, const GatherOut& out_in, cudaStream_t s) {
+                          int64_t n_total, float max_range, const GatherOut& out_in, cudaStream_t s,
+                          bool cues = false) {
   if (n_scans <= 0) return OVN_OK;
   if (n_scans > h->cfg.max_batch_scans)
     OVN_SET_ERR(h, OVN_ERR_CAPACITY, "n_scans=%d exceeds max_batch_scans=%d", n_scans, h->cfg.max_batch_scans);
   GatherOut out = out_in;
   const ProjParams P = make_params(h, max_range);
-  const bool need_rank = out.idx != nullptr || out.n_prob > 0;
+  const bool need_rank = cues || out.idx != nullptr || out.n_prob > 0;
   const size_t HW = (size_t)P.H * P.W;
-  OVN_CUDA(h, cudaMemsetAsync(h->d_keys, 0xFF, (size_t)n_scans * HW * sizeof(unsigned long long), s));
+  const size_t n_images = cues ? 2 : 1;
+  OVN_CUDA(h, cudaMemsetAsync(h->d_keys, 0xFF, n_images * n_scans * HW * sizeof(unsigned long long), s));
   int64_t n_words = (n_total + 31) / 32;
   if (need_rank) {
     int rc = ensure_point_capacity(h, n_total);
@@ -529,9 +553,9 @@ static int run_projection(ovn_handle* h, const float* d_points, const int64_t* d
   if (n_total > 0) {
     const int64_t blocks = (n_total + 255) / 256;
     prof_mark(h, PROF_SCATTER, s);
-    k_project_scatter<<<(unsigned)blocks, 256, 0, s>>>(reinterpret_cast<const float4*>(d_points), d_offsets,
-                                                       n_scans, n_total, P, h->d_keys,
-                                                       need_rank ? h->d_valid_words.get() : nullptr);
+    auto scatter = cues ? k_project_scatter<true> : k_project_scatter<false>;
+    scatter<<<(unsigned)blocks, 256, 0, s>>>(reinterpret_cast<const float4*>(d_points), d_offsets, n_scans, n_total,
+                                             P, h->d_keys, need_rank ? h->d_valid_words.get() : nullptr);
     prof_mark(h, PROF_SCATTER, s);
     OVN_LAUNCH_CHECK(h);
     if (need_rank) {
@@ -546,8 +570,9 @@ static int run_projection(ovn_handle* h, const float* d_points, const int64_t* d
   }
   dim3 grid((P.W + TILE_C - 1) / TILE_C, (P.H + TILE_R - 1) / TILE_R, n_scans);
   prof_mark(h, PROF_GATHER, s);
-  k_project_gather<<<grid, 256, 0, s>>>(reinterpret_cast<const float4*>(d_points), d_offsets, P, h->d_keys,
-                                        h->d_valid_words, h->d_word_prefix, out);
+  auto gather = cues ? k_project_gather<true> : k_project_gather<false>;
+  gather<<<grid, 256, 0, s>>>(reinterpret_cast<const float4*>(d_points), d_offsets, P, h->d_keys, h->d_valid_words,
+                              h->d_word_prefix, out);
   prof_mark(h, PROF_GATHER, s);
   OVN_LAUNCH_CHECK(h);
   return OVN_OK;
@@ -563,8 +588,9 @@ int project_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets
                         max_range < 0 ? h->cfg.max_range : max_range, out, s);
 }
 
-int preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans,
-                     int64_t n_total, const float* d_probs, float* d_input, cudaStream_t s) {
+// the packed input's channels in prepareOneInput's order (Sequence.py:143-207): depth, normals, probabilities,
+// intensity
+static GatherOut packed_channels(const ovn_handle* h, const float* d_probs, float* d_input) {
   GatherOut out = {};
   out.packed = d_input;
   out.C = h->C;
@@ -573,15 +599,37 @@ int preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* d_offs
   if (h->cfg.use_depth) { out.c_depth = c; c += 1; }
   if (h->cfg.use_normals) { out.c_normal = c; c += 3; }
   if (h->cfg.n_prob_channels > 0) {
-    if (d_probs == nullptr) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "d_probs is NULL but n_prob_channels=%d", h->cfg.n_prob_channels);
     out.c_prob = c; out.n_prob = h->cfg.n_prob_channels; out.probs = d_probs; c += out.n_prob;
   }
   if (h->cfg.use_intensity) { out.c_intensity = c; c += 1; }
+  return out;
+}
+
+int preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans,
+                     int64_t n_total, const float* d_probs, float* d_input, cudaStream_t s) {
+  if (h->cfg.n_prob_channels > 0 && d_probs == nullptr)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "d_probs is NULL but n_prob_channels=%d", h->cfg.n_prob_channels);
   // semantic channels are generated with max_range=inf in the reference (gen_semantic_data.py:39)
-  // while depth/normal/intensity use max_range=50; the fused path uses the configured max_range
-  // for every cue, so it is bit-identical to the reference only for the geometric cues.  The
-  // Python wrapper routes the semantic cue through ovn_project_batch(inf)+ovn_semantic_batch.
-  return run_projection(h, d_points, d_offsets, n_scans, n_total, h->cfg.max_range, out, s);
+  // while depth/normal/intensity use max_range=50; this path uses the configured max_range
+  // for every cue, so it is bit-identical to the reference only for the geometric cues.
+  // preprocess_cues_batch gives every cue the reference's range.
+  return run_projection(h, d_points, d_offsets, n_scans, n_total, h->cfg.max_range,
+                        packed_channels(h, d_probs, d_input), s);
+}
+
+// Every channel as the reference's cue files give it (gen_depth/normal/intensity_data.py at max_range,
+// gen_semantic_data.py:33-46 at max_range = inf), in one scatter and one gather: see k_project_scatter<true>.
+int preprocess_cues_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans,
+                          int64_t n_total, const float* d_probs, float* d_input, cudaStream_t s) {
+  if (h->cfg.n_prob_channels == 0) {
+    if (d_probs != nullptr)
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "d_probs must be NULL: the handle has no probability channels");
+    return preprocess_batch(h, d_points, d_offsets, n_scans, n_total, nullptr, d_input, s);
+  }
+  if (d_probs == nullptr)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "d_probs is NULL but n_prob_channels=%d", h->cfg.n_prob_channels);
+  return run_projection(h, d_points, d_offsets, n_scans, n_total, h->cfg.max_range,
+                        packed_channels(h, d_probs, d_input), s, true);
 }
 
 int normals_batch(ovn_handle* h, const float* d_range, const float* d_vertex, int n_scans,

@@ -28,6 +28,22 @@ def _ptr(t):
   return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
+def check_probs(probs, n_points, n_prob, what):
+  """Refuse per-point class probabilities that do not fit a handle with ``n_prob`` probability channels before
+  anything reaches the device: any array on a handle without such channels, and any shape but
+  (n_points, n_prob), one row per point.  None is passed through (the library refuses it on a semantic
+  handle with OVN_ERR_INVALID_ARG)."""
+  if probs is None:
+    return None
+  if n_prob == 0:
+    raise ValueError('%s: class probabilities given, but the handle has no probability channels' % what)
+  shape = tuple(probs.shape)
+  if shape != (n_points, n_prob):
+    raise ValueError('%s: class probabilities of shape %s, expected (%d, %d): one row of %d per point'
+                     % (what, shape, n_points, n_prob, n_prob))
+  return probs
+
+
 class CloudBatch:
   """Clouds back to back on the device: points [sum N, 4] f32, offsets [n+1] i64 (+ a host copy)."""
 
@@ -79,6 +95,7 @@ class Engine:
       raise OvnError('ovn_create failed: %s (%s)' % (L.ovn_status_string(st).decode(),
                                                      L.ovn_last_error(None).decode()))
     self.C = L.ovn_input_channels(self._h)
+    self.n_prob = int(cfg.n_prob_channels)
     self.Wf = L.ovn_feature_width(self._h)
     self.max_batch_scans = int(max_batch_scans)
     self.max_batch_pairs = int(max_batch_pairs)
@@ -272,6 +289,24 @@ class Engine:
       pr = probs[p0:p1] if probs is not None else None
       check(self._h, L.ovn_preprocess_batch(self._h, _ptr(pts), _ptr(offs), s1 - s0, p1 - p0, _ptr(pr),
                                             _ptr(out[s0:s1]), self._stream()), 'ovn_preprocess_batch')
+    return out
+
+  def preprocess_cues(self, batch, probs=None):
+    """ovn_preprocess_cues_batch: raw clouds (CloudBatch) -> packed NHWC network input [n, H, W, C] with every
+    channel as the reference's cue files give it: the class probabilities projected at max_range = inf and
+    gathered like gen_semantic_data.py:36-46, the other cues at the configured max_range.  ``probs``: [sum N,
+    n_prob] float32 (a CUDA tensor or anything torch.as_tensor takes), the points' rows in batch order;
+    required iff the handle has probability channels."""
+    n_total = int(batch.offsets_host[-1])
+    probs = check_probs(probs, n_total, self.n_prob, 'preprocess_cues')
+    if probs is not None:
+      probs = torch.as_tensor(probs).to(device=self.device, dtype=torch.float32).contiguous()
+    out = torch.empty((batch.n, self.H, self.W, self.C), dtype=torch.float32, device=self.device)
+    L = lib()
+    for s0, s1, p0, p1, pts, offs in self._chunks(batch):
+      pr = probs[p0:p1] if probs is not None else None
+      check(self._h, L.ovn_preprocess_cues_batch(self._h, _ptr(pts), _ptr(offs), s1 - s0, p1 - p0, _ptr(pr),
+                                                 _ptr(out[s0:s1]), self._stream()), 'ovn_preprocess_cues_batch')
     return out
 
   def pack_input(self, depth=None, normal=None, prob=None, intensity=None):
@@ -640,26 +675,47 @@ class Engine:
     return self._read_layers(lib().ovn_get_gradients, names, 'ovn_get_gradients')
 
   # ---- host-buffer entry points (synchronous) ------------------------------------------------
-  def encode_clouds_host(self, clouds):
+  def encode_clouds_host(self, clouds, probs=None):
+    """list of (N_i, 4) float32 host clouds -> host feature volumes [n, Wf, 128].  ``probs``: a list of (N_i, n_prob)
+    per-point class probabilities, one per cloud; given, the call is ovn_encode_clouds_probs_host."""
+    if probs is not None:
+      if len(probs) != len(clouds):
+        raise ValueError('encode_clouds_host: %d probability arrays for %d clouds' % (len(probs), len(clouds)))
+      probs = [check_probs(p, c.shape[0], self.n_prob, 'encode_clouds_host') for c, p in zip(clouds, probs)]
     offs = np.zeros(len(clouds) + 1, np.int64)
     for i, c in enumerate(clouds):
       offs[i + 1] = offs[i] + c.shape[0]
     flat = np.ascontiguousarray(np.concatenate([np.asarray(c, np.float32).reshape(-1, 4) for c in clouds]))
     out = np.empty((len(clouds), self.Wf, FEAT_C), np.float32)
-    check(self._h, lib().ovn_encode_clouds_host(self._h, flat.ctypes.data_as(C.c_void_p),
-                                               offs.ctypes.data_as(C.c_void_p), len(clouds),
-                                               out.ctypes.data_as(C.c_void_p)), 'ovn_encode_clouds_host')
+    if probs is None:
+      check(self._h, lib().ovn_encode_clouds_host(self._h, flat.ctypes.data_as(C.c_void_p),
+                                                 offs.ctypes.data_as(C.c_void_p), len(clouds),
+                                                 out.ctypes.data_as(C.c_void_p)), 'ovn_encode_clouds_host')
+      return out
+    flat_probs = np.ascontiguousarray(np.concatenate([np.asarray(p, np.float32) for p in probs]))
+    check(self._h, lib().ovn_encode_clouds_probs_host(self._h, flat.ctypes.data_as(C.c_void_p),
+                                                     offs.ctypes.data_as(C.c_void_p), len(clouds),
+                                                     flat_probs.ctypes.data_as(C.c_void_p),
+                                                     out.ctypes.data_as(C.c_void_p)), 'ovn_encode_clouds_probs_host')
     return out
 
   def query_cloud_vs_bank_host(self, points_host, bank, cand_idx_host=None, n_cand=None, out_overlap=None,
-                               out_yaw=None, out_query_fv=None):
-    """points_host: (N,4) float32 numpy or pinned CPU tensor; bank: cuda [n,360,128].
+                               out_yaw=None, out_query_fv=None, probs=None):
+    """points_host: (N,4) float32 numpy or pinned CPU tensor; bank: cuda [n,360,128]; probs: the points' (N, n_prob)
+    class probabilities (float32 numpy or CPU tensor), given: the call is ovn_query_cloud_probs_vs_bank_host.
     Returns (overlap float32 [n_cand], yaw int32 [n_cand]) host arrays."""
     if isinstance(points_host, torch.Tensor):
       p_ptr, npts = C.c_void_p(points_host.data_ptr()), int(points_host.shape[0])
     else:
       points_host = np.ascontiguousarray(points_host, np.float32)
       p_ptr, npts = points_host.ctypes.data_as(C.c_void_p), int(points_host.shape[0])
+    probs = check_probs(probs, npts, self.n_prob, 'query_cloud_vs_bank_host')
+    if isinstance(probs, torch.Tensor):
+      assert probs.device.type == 'cpu' and probs.dtype == torch.float32 and probs.is_contiguous()
+      pr_ptr = C.c_void_p(probs.data_ptr())
+    elif probs is not None:
+      probs = np.ascontiguousarray(probs, np.float32)
+      pr_ptr = probs.ctypes.data_as(C.c_void_p)
     if cand_idx_host is not None:
       cand_idx_host = np.ascontiguousarray(cand_idx_host, np.int32)
       n = cand_idx_host.size
@@ -672,7 +728,13 @@ class Engine:
     def hp(a):
       if a is None: return C.c_void_p(0)
       return C.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else a.ctypes.data_as(C.c_void_p)
-    check(self._h, lib().ovn_query_cloud_vs_bank_host(self._h, p_ptr, npts, _ptr(bank), int(bank.shape[0]), c_ptr,
-                                                     n, hp(ov), hp(yw), hp(out_query_fv)),
-          'ovn_query_cloud_vs_bank_host')
+    if probs is None:
+      check(self._h, lib().ovn_query_cloud_vs_bank_host(self._h, p_ptr, npts, _ptr(bank), int(bank.shape[0]), c_ptr,
+                                                       n, hp(ov), hp(yw), hp(out_query_fv)),
+            'ovn_query_cloud_vs_bank_host')
+    else:
+      check(self._h, lib().ovn_query_cloud_probs_vs_bank_host(self._h, p_ptr, npts, pr_ptr, _ptr(bank),
+                                                             int(bank.shape[0]), c_ptr, n, hp(ov), hp(yw),
+                                                             hp(out_query_fv)),
+            'ovn_query_cloud_probs_vs_bank_host')
     return ov, yw

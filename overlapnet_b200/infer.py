@@ -17,7 +17,7 @@ import torch
 
 from . import weights as _weights
 from .config import check_model
-from .engine import Engine, FEAT_C
+from .engine import Engine, FEAT_C, check_probs
 
 
 class _ModelShim:
@@ -295,21 +295,37 @@ class Infer():
     return torch.cat(outs)
 
   # ---- extensions: raw clouds in, no .npy round trip -----------------------------------------
-  def encode_clouds(self, clouds):
+  def encode_clouds(self, clouds, probs=None):
     """list of (N,4) float32 raw clouds -> device feature volumes [n,360,128] through the fused
-    projection + normal + packing kernels (geometric cues and intensity only)."""
-    if self.use_class_probabilities:
-      raise Exception('encode_clouds: semantic probabilities need per-point class scores')
+    projection + normal + packing kernels, every cue as the reference's .npy files give it.  A config with class
+    probabilities needs ``probs``: one (N, 20) -- (N, 3) with use_class_probabilities_pca -- float32 array per
+    cloud, the per-point scores a .label file holds (gen_semantic_data.py:33); other configs refuse them."""
+    n_prob = self._engine.n_prob
+    if self.use_class_probabilities and probs is None:
+      raise Exception('encode_clouds: semantic probabilities need per-point class scores (probs)')
+    if probs is not None:
+      if not self.use_class_probabilities:
+        raise Exception('encode_clouds: class probabilities given, but the config does not use them')
+      if len(probs) != len(clouds):
+        raise Exception('encode_clouds: %d probability arrays for %d clouds' % (len(probs), len(clouds)))
+      probs = [check_probs(p, np.shape(c)[0], n_prob, 'encode_clouds') for c, p in zip(clouds, probs)]
+      probs = np.concatenate([np.asarray(p, np.float32) for p in probs]) if probs else np.zeros((0, n_prob), np.float32)
     batch = self._engine.upload_clouds(clouds)
-    return self._engine.leg(self._engine.preprocess(batch))
+    return self._engine.leg(self._engine.preprocess_cues(batch, probs))
 
-  def infer_one_raw(self, filepath1, filepath2):
-    """Like ``infer_one`` but reads the raw .bin scans (LEFT = file2, RIGHT = file1)."""
+  def infer_one_raw(self, filepath1, filepath2, labels1=None, labels2=None):
+    """Like ``infer_one`` but reads the raw .bin scans (LEFT = file2, RIGHT = file1).  A config with class
+    probabilities also reads each scan's .label file of per-point scores, as gen_semantic_data.py:33 does."""
     if not filepath1.endswith('.bin') or not filepath2.endswith('.bin'):
       raise Exception('Please check the LiDAR file format, '
                       'this implementation currently only works with .bin files.')
     clouds = [np.fromfile(p, dtype=np.float32).reshape((-1, 4)) for p in (filepath2, filepath1)]
-    fv = self.encode_clouds(clouds)
+    probs = None
+    if labels1 is not None or labels2 is not None:
+      if labels1 is None or labels2 is None:
+        raise Exception('infer_one_raw: give the .label files of both scans')
+      probs = [np.fromfile(p, dtype=np.float32).reshape((-1, self._engine.n_prob or 20)) for p in (labels2, labels1)]
+    fv = self.encode_clouds(clouds, probs)
     ov, yaw, _ = self._engine.heads(fv, torch.tensor([0], dtype=torch.int32), torch.tensor([1], dtype=torch.int32))
     self._engine.check()
     return ov.cpu().numpy(), yaw.cpu().numpy().astype(np.int64)
