@@ -96,7 +96,7 @@ int64_t     ovn_launch_count(const ovn_handle* h);
 /* ---- per-kernel device timing (bench.py roofline): CUDA events recorded around the named kernels
  * on the launching stream while enabled.  ovn_profile_read synchronises the device, returns the
  * accumulated milliseconds / launch count since the last read and resets them.  Names:
- * "delta_conv1", "conv2", "conv3", "corr", "project_scatter", "project_gather", "leg". */
+ * "delta_conv1", "conv2", "conv3", "corr", "project_scatter", "project_gather", "leg", "gather_rows". */
 int ovn_profile_enable(ovn_handle* h, int on);
 int ovn_profile_read(ovn_handle* h, const char* kernel, double* total_ms, int64_t* launches);
 
@@ -381,6 +381,33 @@ int ovn_host_register(ovn_handle* h, void* h_ptr, int64_t bytes);
 int ovn_host_unregister(ovn_handle* h, void* h_ptr);
 int ovn_stage_rows(ovn_handle* h, const void* h_src, int64_t n_src_rows, int64_t row_bytes, const int64_t* h_rows,
                    int32_t n, void* d_dst, void* stream);
+/* ---- a training image bank sharded over the GPUs of a node (overlapnet_b200/image_bank.py, DESIGN.md section 6) --
+ * Each rank holds a contiguous block of the bank's rows in a shard of its own device memory; a step's rows are
+ * gathered into a device slot straight from the owners' memory (over NVLink, or within one device).
+ *   ovn_shard_create: allocates a shard of `bytes` > 0 bytes, owned by the handle: one cudaMalloc of exactly that
+ *                    size, so that *d_ptr is the allocation's base.  Writes its CUDA IPC handle (cudaIpcGetMemHandle,
+ *                    64 bytes) to h_ipc.  OVN_ERR_CUDA with the runtime's message when either call fails.
+ *   ovn_shard_open:  maps another process's shard from its 64-byte IPC handle (cudaIpcOpenMemHandle, peer access
+ *                    enabled lazily); the mapping is owned by the handle.  A handle that cannot be opened (a device
+ *                    without peer access, a zeroed or stale handle, a shard of this same process) is OVN_ERR_CUDA
+ *                    with the runtime's message; nothing is mapped and the handle stays usable.
+ *   ovn_shard_close: synchronises the device, then unmaps a shard ovn_shard_open mapped or frees one
+ *                    ovn_shard_create allocated.  Any other pointer is OVN_ERR_INVALID_ARG.  The caller makes sure
+ *                    no other process still reads an own shard (a barrier after every rank closed its mappings).
+ *                    ovn_destroy closes the remaining mappings before it frees the remaining own shards.
+ *   ovn_gather_rows: for i < n, d_dst + i row_bytes = row h_rows[i] (row_bytes bytes) of the bank of which shard s
+ *                    (a device pointer: own or mapped) holds rows [h_first[s], h_first[s + 1]).  One launch of
+ *                    k_gather_rows on `stream` per 1024 rows, 16-byte loads and stores; the source of every row
+ *                    travels in the launch's parameters, so the host arrays may be reused once the call returns.
+ *                    Checked on the host before anything is issued: n < 0, n_shards < 1, h_first not starting at
+ *                    0 or decreasing, row_bytes not a positive multiple of 16, a NULL or not 16-byte aligned shard
+ *                    pointer or d_dst, a row outside [0, h_first[n_shards]) are OVN_ERR_INVALID_ARG and nothing is
+ *                    copied.  Both precisions; profiled as "gather_rows". */
+int ovn_shard_create(ovn_handle* h, int64_t bytes, void** d_ptr, void* h_ipc /* 64 bytes */);
+int ovn_shard_open(ovn_handle* h, const void* h_ipc /* 64 bytes */, void** d_ptr);
+int ovn_shard_close(ovn_handle* h, void* d_ptr);
+int ovn_gather_rows(ovn_handle* h, const void* const* h_shards, const int64_t* h_first /* [n_shards + 1] */,
+                    int32_t n_shards, int64_t row_bytes, const int64_t* h_rows, int32_t n, void* d_dst, void* stream);
 /* Current weights / last gradients of a layer, Keras layout, host buffers (same shapes as ovn_set_weights).
  * Both synchronise the device.  ovn_get_gradients returns the head layers after ovn_head_gradients and every
  * layer after ovn_net_gradients. */

@@ -28,7 +28,9 @@ SYMBOLS = [
     'ovn_train_workspace_bytes', 'ovn_host_register', 'ovn_host_unregister', 'ovn_stage_rows',
     'ovn_head_gradients_chunks', 'ovn_net_gradients_chunks', 'ovn_copy_heads_stage',
     'ovn_heads_stage_pairs', 'ovn_leg_stage', 'ovn_encode_clouds_probs_host', 'ovn_query_cloud_probs_vs_bank_host',
+    'ovn_shard_create', 'ovn_shard_open', 'ovn_shard_close', 'ovn_gather_rows',
 ]
+IPC_HANDLE_BYTES = 64     # ovn_shard_create / ovn_shard_open
 HEADS_STAGES = {'o1': 0, 'x3': 1, 'dense': 2, 'centres': 3}     # ovn_heads_stage
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
 
@@ -124,6 +126,10 @@ def lib():
   L.ovn_host_register.argtypes = [vp, vp, i64]
   L.ovn_host_unregister.argtypes = [vp, vp]
   L.ovn_stage_rows.argtypes = [vp, vp, i64, i64, vp, i32, vp, vp]
+  L.ovn_shard_create.argtypes = [vp, i64, C.POINTER(vp), vp]
+  L.ovn_shard_open.argtypes = [vp, vp, C.POINTER(vp)]
+  L.ovn_shard_close.argtypes = [vp, vp]
+  L.ovn_gather_rows.argtypes = [vp, vp, vp, i32, i64, vp, i32, vp, vp]
   L.ovn_head_gradients_chunks.argtypes = [vp, vp, i64, vp, vp, i32, vp, i32, vp, vp, f32, vp, vp, vp]
   L.ovn_net_gradients_chunks.argtypes = [vp, vp, i64, vp, vp, i32, vp, i32, vp, vp, f32, vp, vp, vp]
   L.ovn_get_weights.argtypes = [vp, C.c_char_p, vp, vp]

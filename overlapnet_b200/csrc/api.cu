@@ -4,6 +4,7 @@
 #include "common.cuh"
 #include <math.h>
 #include <string.h>
+#include <algorithm>
 
 using namespace ovn;
 
@@ -317,6 +318,11 @@ int ovn_create(const ovn_config* cfg, ovn_handle** out) {
 int ovn_destroy(ovn_handle* h) {
   if (!h) return OVN_OK;
   DeviceGuard guard(h);
+  if (!h->open_shards.empty() || !h->own_shards.empty()) {
+    cudaDeviceSynchronize();               // no queued gather still reads a shard; then the mappings, then the own shards
+    h->open_shards.clear();
+    h->own_shards.clear();
+  }
   delete h;
   return OVN_OK;
 }
@@ -333,7 +339,7 @@ int ovn_profile_read(ovn_handle* h, const char* kernel, double* total_ms, int64_
   DeviceGuard guard(h);
   if (!kernel || !total_ms || !launches) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_profile_read: NULL argument");
   static const char* names[kProfKinds] = {"delta_conv1", "conv2", "conv3", "corr", "project_scatter",
-                                          "project_gather", "leg"};
+                                          "project_gather", "leg", "gather_rows"};
   int kind = -1;
   for (int i = 0; i < kProfKinds; ++i) if (strcmp(kernel, names[i]) == 0) kind = i;
   if (kind < 0) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_profile_read: unknown kernel '%s'", kernel);
@@ -1036,6 +1042,92 @@ int ovn_stage_rows(ovn_handle* h, const void* h_src, int64_t n_src_rows, int64_t
     OVN_CUDA(h, cudaMemcpyAsync(dst + (size_t)i * row_bytes, src + (size_t)h_rows[i] * row_bytes, (size_t)row_bytes,
                                 cudaMemcpyHostToDevice, (cudaStream_t)stream));
   return OVN_OK;
+}
+
+// ---- a training image bank sharded over the GPUs of a node --------------------------------------------------
+static_assert(sizeof(cudaIpcMemHandle_t) == 64, "ovn_shard_create writes 64 bytes of IPC handle");
+
+int ovn_shard_create(ovn_handle* h, int64_t bytes, void** d_ptr, void* h_ipc) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, d_ptr && h_ipc, "NULL pointer");
+  REQUIRE(h, bytes > 0, "bytes must be positive");
+  *d_ptr = nullptr;
+  Buffer<uint8_t> shard;
+  int rc = shard.ensure(h, (size_t)bytes);          // exactly `bytes`: the IPC handle names the allocation's base
+  if (rc != OVN_OK) return rc;
+  cudaIpcMemHandle_t ipc;
+  OVN_CUDA(h, cudaIpcGetMemHandle(&ipc, shard.get()));
+  memcpy(h_ipc, &ipc, sizeof(ipc));
+  *d_ptr = shard.get();
+  h->own_shards.push_back(std::move(shard));
+  return OVN_OK;
+}
+
+int ovn_shard_open(ovn_handle* h, const void* h_ipc, void** d_ptr) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, d_ptr && h_ipc, "NULL pointer");
+  *d_ptr = nullptr;
+  cudaIpcMemHandle_t ipc;
+  memcpy(&ipc, h_ipc, sizeof(ipc));
+  void* p = nullptr;
+  OVN_CUDA(h, cudaIpcOpenMemHandle(&p, ipc, cudaIpcMemLazyEnablePeerAccess));
+  h->open_shards.emplace_back(p);
+  *d_ptr = p;
+  return OVN_OK;
+}
+
+int ovn_shard_close(ovn_handle* h, void* d_ptr) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, d_ptr, "NULL pointer");
+  for (size_t i = 0; i < h->open_shards.size(); ++i)
+    if (h->open_shards[i].get() == d_ptr) {
+      OVN_CUDA(h, cudaDeviceSynchronize());           // no queued gather still reads the mapping
+      h->open_shards.erase(h->open_shards.begin() + i);
+      return OVN_OK;
+    }
+  for (size_t i = 0; i < h->own_shards.size(); ++i)
+    if (h->own_shards[i].get() == d_ptr) {
+      OVN_CUDA(h, cudaDeviceSynchronize());
+      h->own_shards.erase(h->own_shards.begin() + i);
+      return OVN_OK;
+    }
+  OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_shard_close: %p is neither a shard of this handle nor one it opened", d_ptr);
+}
+
+int ovn_gather_rows(ovn_handle* h, const void* const* h_shards, const int64_t* h_first, int32_t n_shards,
+                    int64_t row_bytes, const int64_t* h_rows, int32_t n, void* d_dst, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, n >= 0, "n must not be negative");
+  REQUIRE(h, n_shards >= 1, "n_shards must be at least 1");
+  REQUIRE(h, h_shards && h_first, "NULL shard table");
+  REQUIRE(h, row_bytes > 0 && row_bytes % 16 == 0, "row_bytes must be a positive multiple of 16");
+  REQUIRE(h, h_first[0] == 0, "h_first[0] must be 0");
+  for (int32_t s = 0; s < n_shards; ++s) {
+    if (h_first[s + 1] < h_first[s])
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_gather_rows: h_first decreases at shard %d", s);
+    if (!h_shards[s] || (uintptr_t)h_shards[s] % 16 != 0)
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_gather_rows: shard %d pointer %p is NULL or not 16-byte aligned", s,
+                  h_shards[s]);
+  }
+  if (n == 0) return OVN_OK;
+  REQUIRE(h, h_rows && d_dst, "NULL pointer");
+  REQUIRE(h, (uintptr_t)d_dst % 16 == 0, "d_dst is not 16-byte aligned");
+  const int64_t n_rows = h_first[n_shards];
+  std::vector<const void*> src(n);
+  for (int32_t i = 0; i < n; ++i) {                    // all rows first: a refused call copies nothing
+    const int64_t r = h_rows[i];
+    if (r < 0 || r >= n_rows)
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_gather_rows: row %lld of entry %d is outside [0, %lld)", (long long)r, i,
+                  (long long)n_rows);
+    // the last shard whose first row is <= r: an empty shard before it has the same first row
+    const int32_t s = (int32_t)(std::upper_bound(h_first, h_first + n_shards + 1, r) - h_first) - 1;
+    src[i] = static_cast<const uint8_t*>(h_shards[s]) + (r - h_first[s]) * row_bytes;
+  }
+  return gather_rows(h, src.data(), n, row_bytes, d_dst, (cudaStream_t)stream);
 }
 
 int ovn_bank_prepare(ovn_handle* h, const float* d_bank, int64_t bank_capacity, int64_t first, int64_t count,

@@ -68,7 +68,29 @@ static_assert(sizeof(float) == sizeof(int32_t), "the three staging arrays are 4 
 
 constexpr int kFeatC = 128;           // leg output channels (generateNet.py:214)
 constexpr int kMaxLegLayers = 12;
-enum ProfKind { PROF_DELTA = 0, PROF_CONV2, PROF_CONV3, PROF_CORR, PROF_SCATTER, PROF_GATHER, PROF_LEG, kProfKinds };
+enum ProfKind { PROF_DELTA = 0, PROF_CONV2, PROF_CONV3, PROF_CORR, PROF_SCATTER, PROF_GATHER, PROF_LEG, PROF_GATHER_ROWS,
+                kProfKinds };
+
+// The one owner of another process's shard mapped by ovn_shard_open (cudaIpcOpenMemHandle); unmaps it on
+// destruction.  Move-only, like Buffer.
+class IpcMapping {
+ public:
+  IpcMapping() = default;
+  explicit IpcMapping(void* p) : p_(p) {}
+  IpcMapping(IpcMapping&& o) noexcept { std::swap(p_, o.p_); }
+  IpcMapping& operator=(IpcMapping&& o) noexcept {
+    IpcMapping old(std::move(o));
+    std::swap(p_, old.p_);
+    return *this;
+  }
+  ~IpcMapping() {
+    if (p_) cudaIpcCloseMemHandle(p_);
+  }
+  void* get() const { return p_; }
+
+ private:
+  void* p_ = nullptr;
+};
 
 struct ConvSpec {                      // one Conv2D layer (valid padding, bias)
   char name[24];
@@ -186,6 +208,10 @@ struct ovn_handle {
   ovn::Buffer<float> d_stage_points;         // staged clouds, grown on use
   ovn::Buffer<int64_t> d_stage_offsets;      // [max_batch_scans + 1], allocated on first use
   ovn::PinnedBuffer<uint8_t> h_pinned;       // StageHeader, then candidate indices / overlaps / yaws [max_batch_pairs]
+  // a sharded training image bank (ovn_shard_*): this process's shards, then the other processes' shards it
+  // mapped.  Declared in this order so that the mappings are closed before the own shards are freed.
+  std::vector<ovn::Buffer<uint8_t>> own_shards;
+  std::vector<ovn::IpcMapping> open_shards;
   cudaStream_t own_stream = nullptr;
   // per-kernel profiling (ovn_profile_enable / ovn_profile_read)
   bool profiling = false;
@@ -367,6 +393,10 @@ int adagrad_sum_fp32(ovn_handle* h, bool whole_network, const float* d_parts, in
 // yaw augmentation of training images (projection.cu): rows are bounds-checked on the device (kErrBadIndex)
 int gather_images(ovn_handle* h, const float* d_images, int64_t n_images, const int32_t* d_rows,
                   const int32_t* d_shift, const float* d_rot, int n, float* d_out, cudaStream_t s);
+// rows of a sharded image bank (bank_shard.cu): d_dst + i row_bytes = row_bytes bytes at h_src[i], one launch of
+// k_gather_rows per kGatherRowsCap rows; the caller has checked every pointer and row_bytes % 16 == 0
+constexpr int kGatherRowsCap = 1024;
+int gather_rows(ovn_handle* h, const void* const* h_src, int n, int64_t row_bytes, void* d_dst, cudaStream_t s);
 
 int corr_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* left,
                       const int32_t* right, int np, int32_t* d_yaw, float* d_corr, cudaStream_t s);

@@ -44,6 +44,14 @@ def check_probs(probs, n_points, n_prob, what):
   return probs
 
 
+class _DeviceBlock:
+  """A float32 block of device memory the handle owns, as torch.as_tensor takes it (__cuda_array_interface__)."""
+
+  def __init__(self, ptr, shape):
+    self.__cuda_array_interface__ = {'data': (int(ptr), False), 'shape': tuple(shape), 'typestr': '<f4',
+                                     'strides': None, 'version': 3}
+
+
 class CloudBatch:
   """Clouds back to back on the device: points [sum N, 4] f32, offsets [n+1] i64 (+ a host copy)."""
 
@@ -105,6 +113,7 @@ class Engine:
       for a in getattr(self, '_pinned', ()):                      # host_register'ed blocks still pinned
         lib().ovn_host_unregister(self._h, a.ctypes.data_as(C.c_void_p))
       self._pinned = []
+      self._shards = {}                                            # ovn_destroy closes and frees the shards
       lib().ovn_destroy(self._h)
       self._h = C.c_void_p(0)
 
@@ -638,6 +647,55 @@ class Engine:
     check(self._h, lib().ovn_stage_rows(self._h, host.ctypes.data_as(C.c_void_p), int(host.shape[0]), row_bytes,
                                         r.ctypes.data_as(C.c_void_p), int(r.size), _ptr(out), self._stream()),
           'ovn_stage_rows')
+
+  # ---- a training image bank sharded over the GPUs of a node (overlapnet_b200.image_bank) -------------------
+  def shard_create(self, n_rows):
+    """ovn_shard_create: a shard of ``n_rows`` images [n_rows, H, W, C] float32 in this handle's device memory (at
+    least one image's bytes, so that every shard has an address).  Returns (a torch view of it, zero-copy; its
+    device address; its 64-byte IPC handle as bytes).  The view is valid until shard_close or close."""
+    n_rows = int(n_rows)
+    row = self.H * self.W * self.C * 4
+    ptr, ipc = C.c_void_p(0), (C.c_uint8 * _cabi.IPC_HANDLE_BYTES)()
+    check(self._h, lib().ovn_shard_create(self._h, max(n_rows, 1) * row, C.byref(ptr), ipc), 'ovn_shard_create')
+    self._shards = getattr(self, '_shards', {})
+    self._shards[ptr.value] = 'own'
+    view = torch.as_tensor(_DeviceBlock(ptr.value, (max(n_rows, 1), self.H, self.W, self.C)), device=self.device)
+    return view[:n_rows], int(ptr.value), bytes(ipc)
+
+  def shard_open(self, ipc):
+    """ovn_shard_open: the device address of another process's shard, from its IPC handle (bytes)."""
+    ipc = bytes(ipc)
+    assert len(ipc) == _cabi.IPC_HANDLE_BYTES, len(ipc)
+    buf = (C.c_uint8 * _cabi.IPC_HANDLE_BYTES).from_buffer_copy(ipc)
+    ptr = C.c_void_p(0)
+    check(self._h, lib().ovn_shard_open(self._h, buf, C.byref(ptr)), 'ovn_shard_open')
+    self._shards = getattr(self, '_shards', {})
+    self._shards[ptr.value] = 'open'
+    return int(ptr.value)
+
+  def shard_close(self, ptr):
+    """ovn_shard_close: synchronises the device, then unmaps a shard shard_open mapped or frees one shard_create
+    made (its view must not be used afterwards)."""
+    check(self._h, lib().ovn_shard_close(self._h, C.c_void_p(int(ptr))), 'ovn_shard_close')
+    self._shards.pop(int(ptr), None)
+
+  def open_shard_count(self):
+    """The other processes' shards this handle has mapped and not closed."""
+    return sum(1 for kind in getattr(self, '_shards', {}).values() if kind == 'open')
+
+  def gather_rows(self, shards, first, rows, out):
+    """ovn_gather_rows: out[i] = row rows[i] of the bank of which shards[s] (device addresses) holds rows
+    [first[s], first[s + 1]), one launch on the current stream.  ``rows`` host integers, ``out`` a contiguous cuda
+    tensor of at least len(rows) images."""
+    r = np.ascontiguousarray(rows, np.int64).reshape(-1)
+    f = np.ascontiguousarray(first, np.int64).reshape(-1)
+    s = (C.c_void_p * max(len(shards), 1))(*[int(p) for p in shards])
+    assert f.size == len(shards) + 1 and out.is_contiguous() and out.device == self.device
+    assert out.shape[0] >= r.size and out.dtype == torch.float32
+    row_bytes = out[0].numel() * 4 if out.shape[0] else self.H * self.W * self.C * 4
+    check(self._h, lib().ovn_gather_rows(self._h, s, f.ctypes.data_as(C.c_void_p), len(shards), row_bytes,
+                                         r.ctypes.data_as(C.c_void_p), int(r.size), _ptr(out), self._stream()),
+          'ovn_gather_rows')
 
   @property
   def leg_layers(self):

@@ -23,6 +23,8 @@ each step's rotated RIGHT images.  Validation is never augmented.
 An image bank (the whole network's; the frozen leg's RIGHT scans under yaw augmentation) that does not fit on the
 GPU beside the largest step's working set is kept in pinned host memory, and each step's images are staged to the
 GPU while the previous step computes (overlapnet_b200.image_bank, DESIGN.md section 6); the weights are the same.
+Under data-parallel training on one node, a bank whose 1/world share fits every GPU is instead sharded over the
+ranks' GPUs, and each step gathers its images from the owners' memory.
 
 ``training_precision: tf32x3`` (both legsTypes, default fp32) runs every product of the gradient steps on tensor
 cores in 3xTF32 with fp32 accumulation (Engine.set_train_precision); validation stays fp32.
@@ -62,6 +64,7 @@ import torch
 from . import augment
 from . import data_parallel
 from . import evaluate
+from . import image_bank as _image_bank
 from . import weights as _weights
 from .config import load_config
 
@@ -326,8 +329,9 @@ class FrozenLeg:
 
   def __init__(self, infer, keys, rotate_keys=None, image_bank=None, gradient_chunks=None):
     """``image_bank`` (yaw augmentation only: without it there is no image bank) None places the RIGHT scans'
-    images on the GPU when they fit beside the largest step's working set and in pinned host memory otherwise
-    (overlapnet_b200.image_bank); 'device' or 'host' forces a placement.  Both train the same bits.
+    images on the GPU when they fit beside the largest step's working set, sharded over the GPUs of a node's
+    data-parallel ranks or in pinned host memory otherwise (overlapnet_b200.image_bank); 'device', 'host' or
+    'sharded' forces a placement.  All train the same bits.
     ``gradient_chunks`` (the config key) sizes that working set for a rank's largest chunk range."""
     logger.info('Encoding %d scans with the frozen leg ...', len(keys))
     self.eng = infer._engine
@@ -336,7 +340,6 @@ class FrozenLeg:
     if rotate_keys:
       # Yaw augmentation: the images of the scans a step may rotate, and max_batch_scans scratch rows after the
       # bank that receive a step's rotated RIGHT volumes.
-      from . import image_bank as _image_bank
       dp = data_parallel.default_group()
       world = 1 if dp is None else dp.world
       b_share = _image_bank.share_pairs(self.eng.max_batch_pairs, world, gradient_chunks)
@@ -344,17 +347,18 @@ class FrozenLeg:
       self.image_bank, self.images, self.image_rows = _image_bank.open_bank(
           infer, rotate_keys, image_bank, b_share, False, b_share, n + B, 'Image bank of the rotated RIGHT scans',
           _image_bank.parts_bytes(self.eng, False, world, gradient_chunks))
-      if self.image_bank == 'host':
+      if self.image_bank in _image_bank.STAGED:
         self.ring = _image_bank.StagingRing(self.eng, self.images, 2 * b_share)
       self.bank = torch.cat([self.bank, self.bank.new_empty((B,) + tuple(self.bank.shape[1:]))])
       self.scratch = torch.arange(n, n + B, dtype=torch.int32, device=self.eng.device)
 
   whole_network = False          # the layers the gradients cover (Engine.copy_gradients, adagrad_step_sum)
-  ring = None                    # the image_bank.StagingRing of a host image bank
+  ring = None                    # the image_bank.StagingRing of a host or sharded image bank
 
   def begin_epoch(self, spans, left, right, rotate_rows=None):
-    """With a host bank: the steps this rank runs in the coming epoch, in order -- pairs [a, b) of the training
-    pairs' RIGHT image rows ``rotate_rows`` (host array) -- whose images the ring then stages ahead of each step."""
+    """With a host or sharded bank: the steps this rank runs in the coming epoch, in order -- pairs [a, b) of the
+    training pairs' RIGHT image rows ``rotate_rows`` (host array) -- whose images the ring then stages ahead of each
+    step."""
     self.ring.plan([(rotate_rows[a:b],) for a, b in spans])
 
   def step(self, left, right, gt_overlap, gt_orientation, min_overlap_for_angle, lr, rotate=None):
@@ -390,6 +394,13 @@ class FrozenLeg:
     return ov, yaw
 
 
+def close_image_bank(flow):
+  """Release a flow's sharded image bank (ShardedImageBank.close, collective); a host bank is released with its
+  handle."""
+  if getattr(flow, 'image_bank', None) == 'sharded':
+    flow.images.close()
+
+
 def train(config, device=None):
   """Run the training of training.py for a loaded YAML dict.  Returns a dict with the per-epoch
   losses, the batch losses, the validation statistics and the weight file name."""
@@ -416,18 +427,21 @@ def run(config, device, flow):
     logger.addHandler(handler)
   if logger.level == logging.NOTSET or logger.level > logging.INFO:
     logger.setLevel(logging.INFO)
+  made = []                 # the flow _train builds: its sharded image bank is closed here, also after an exception
   try:
-    return _train(config, model, imgpath, out_dir, device, Infer, flow, dp=dp)
+    return _train(config, model, imgpath, out_dir, device, Infer, flow, dp=dp, made=made)
   finally:
+    for steps in made:
+      close_image_bank(steps)
     if handler is not None:
       logger.removeHandler(handler)
       handler.close()
 
 
-def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
+def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None, made=None):
   """The loop; ``dp`` (a data_parallel.DataParallel) makes it data-parallel: the config's batch_size is the
   global batch, rank 0 makes every random draw a one-process run makes and hands the results to the other
-  ranks, and each step is data_parallel's gradient sum."""
+  ranks, and each step is data_parallel's gradient sum.  The flow it builds is appended to ``made``."""
   weights_filename = os.path.join(out_dir, model['modelType'] + '_' + config['testname'] + '.weight')
   initial_lr = float(config['learning_rate'])
   lr_alpha = float(config.get('lr_alpha', 0.99))
@@ -490,6 +504,8 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
   keys = set(zip(t_d1, t_f1)) | set(zip(t_d2, t_f2)) | set(zip(v_d1, v_f1)) | set(zip(v_d2, v_f2))
   chunk_kw = {} if gradient_chunks is None else {'gradient_chunks': gradient_chunks}
   steps = flow(infer, keys, set(zip(t_d2, t_f2)), **chunk_kw) if yaw_augmentation else flow(infer, keys, **chunk_kw)
+  if made is not None:
+    made.append(steps)
   rows = steps.rows
   dev = eng.device
   t_left = torch.tensor([rows[k] for k in zip(t_d1, t_f1)], dtype=torch.int32, device=dev)
@@ -512,7 +528,7 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None):
                 'moved', pitch, pitch * width // W)
   else:
     logger.info('  NO rotation of training data')
-  staged = getattr(steps, 'image_bank', None) == 'host'
+  staged = getattr(steps, 'image_bank', None) in _image_bank.STAGED
   if staged:                      # the image rows of the pairs (LEFT, RIGHT, rotated RIGHT) for begin_epoch's plans
     right_h = np.asarray([steps.image_rows[k] for k in zip(t_d2, t_f2)], np.int64)
     left_h = np.asarray([steps.image_rows[k] for k in zip(t_d1, t_f1)], np.int64) if steps.whole_network else None

@@ -3,8 +3,9 @@
 included, so a model can be trained from scratch and the orientation loss reaches the weights through the leg.
 
 Every distinct scan's packed input is loaded once, through Infer's cue loader, into an image bank: on the GPU
-when it fits beside the largest step's working set, else in pinned host memory, from which each step's images are
-staged through a two-slot device ring while the previous step computes (overlapnet_b200.image_bank).
+when it fits beside the largest step's working set, else sharded over the GPUs of a node's data-parallel ranks or
+in pinned host memory, from which each step's images are staged through a two-slot device ring while the previous
+step computes (overlapnet_b200.image_bank).
 A training step gathers its 2B images from that bank, runs the leg and both heads forward and the whole
 network backward (``ovn_net_gradients``), then an Adagrad update of every layer (``ovn_net_adagrad_step``).
 Each epoch re-encodes the image bank with the current leg for the validation pairs.  The loop, the logging, the history and the
@@ -76,8 +77,9 @@ def load_image_bank(infer, keys, chunk=256):
 
 class WholeNetwork:
   """The training step of 360OutputkLegs on an image bank.  ``image_bank`` None places the bank on the GPU when it
-  fits beside the largest step's working set and in pinned host memory otherwise (overlapnet_b200.image_bank);
-  'device' or 'host' forces a placement.  Both train the same bits."""
+  fits beside the largest step's working set, sharded over the GPUs of a node's data-parallel ranks or in pinned host
+  memory otherwise (overlapnet_b200.image_bank); 'device', 'host' or 'sharded' forces a placement.  All train the
+  same bits."""
 
   def __init__(self, infer, keys, rotate_keys=None, image_bank=None, gradient_chunks=None):
     self.eng = infer._engine
@@ -95,7 +97,7 @@ class WholeNetwork:
       self.ring = _image_bank.StagingRing(self.eng, self.images, 2 * b_share)
 
   whole_network = True           # the layers the gradients cover (Engine.copy_gradients, adagrad_step_sum)
-  ring = None                    # the image_bank.StagingRing of a host image bank
+  ring = None                    # the image_bank.StagingRing of a host or sharded image bank
 
   def begin_epoch(self, spans, left, right, rotate_rows=None):
     """With a host bank: the steps this rank runs in the coming epoch, in order -- pairs [a, b) of the training
