@@ -22,7 +22,7 @@
  *     Infer.create_feature_volumes returns, infer.py:240-265, with the singleton H axis dropped).
  *   - ovn_copy_heads_stage reads back the intermediate stages of the tensor-core heads and ovn_leg_stage
  *     one layer of the tensor-core leg (tests and diagnostics only; the heads and leg calls do no extra
- *     work for them).
+ *     work for them).  ovn_set_train_stop / ovn_copy_train_stage do the same for the training step.
  */
 #ifndef OVN_B200_H_
 #define OVN_B200_H_
@@ -496,6 +496,63 @@ int ovn_copy_heads_stage(ovn_handle* h, int32_t stage, int64_t first, int64_t co
  * OVN_ERR_WEIGHTS before ovn_finalize_weights, OVN_ERR_INVALID_ARG for a layer or n_scans out of range. */
 int ovn_leg_stage(ovn_handle* h, const float* d_input, int32_t n_scans, int32_t layer, float* d_hi, float* d_lo,
                   void* stream);
+
+/* ---- stages of a training step (tests and diagnostics; oracle/train_stages.py, DESIGN.md section 4) ---------
+ * The buffers of the last ovn_head_gradients / ovn_net_gradients call (chunked forms included) of n_pairs pairs,
+ * read back as float32.  Wf = leg_output_width, s = conv1size, nb = Wf / s, nit = ceil(Wf / 64); "images order" is
+ * the order of the gathered images: chunk after chunk, the chunk's LEFT images then its RIGHT images (one chunk:
+ * LEFT 0..n-1, RIGHT 0..n-1).
+ * Stop stages: values the step overwrites later in place.  ovn_set_train_stop(h, stage, layer) makes the next
+ * gradient call stop right after that value is complete (stage = -1: no stop); the stop is consumed by that call
+ * whatever it returns, and a stop its flow never reaches (a whole-network stage in ovn_head_gradients) lets the
+ * call run to the end.  A call that stopped writes no losses and leaves no gradients and no batch:
+ * ovn_get_gradients, ovn_copy_gradients, ovn_copy_net_volumes, ovn_head_adagrad_step, ovn_net_adagrad_step and
+ * ovn_adagrad_step_sum return OVN_ERR_INVALID_ARG until a call runs to the end; the parts of a stopped _chunks call
+ * are incomplete.  The next whole call computes exactly what it computes on a fresh handle.
+ *   OVN_TRAIN_STAGE_O1        [n][Wf][nb][64] (i, jb, o) c_conv1 output with its bias
+ *   OVN_TRAIN_STAGE_X4        [n][o3_h][o3_w][256] ReLU(c_conv3), the Dense input
+ *   OVN_TRAIN_STAGE_DFV_CORR  [2][n][Wf][128] (LEFT, RIGHT) dL/d(volumes) of the correlation head (k_corr_backward)
+ *   OVN_TRAIN_STAGE_LEG_DY    layer l: [2n][h_out][w_out][cout] in images order, dL/d(pre-activation of leg layer l)
+ *                             (the top layer's is the |l - r| and correlation parts summed, masked by the volumes)
+ * Stages read after a call that ran to the end:
+ *   OVN_TRAIN_STAGE_X3        [n][o2_h][o2_w][128] ReLU(c_conv2)
+ *   OVN_TRAIN_STAGE_OVERLAP   [n] yhat;  OVN_TRAIN_STAGE_CORR [n][Wf] orientation logits
+ *   OVN_TRAIN_STAGE_DZ        [n] dL/d(Dense logit), each chunk's own 1 / n
+ *   OVN_TRAIN_STAGE_DPRE3     [n][o3_h][o3_w][256] dL/d(pre-activation of c_conv3)
+ *   OVN_TRAIN_STAGE_DX3       [n][o2_h][o2_w][128] dL/d(pre-activation of c_conv2)
+ *   OVN_TRAIN_STAGE_DO1       [n][o2_h][nb][s][64] (ho, jb, dh, o) dL/d(c_conv1 output) at row i = s ho + dh
+ *   OVN_TRAIN_STAGE_DCORR     [n][Wf] dL/d(orientation logits)                       (whole network only, so on)
+ *   OVN_TRAIN_STAGE_PART_L    [n][nb][Wf][128] k_delta_dgrad partials of dL/dLEFT, one per jb
+ *   OVN_TRAIN_STAGE_PART_R    [n][nit][Wf][128] partials of dL/dRIGHT, one per 64-row tile of i
+ *   OVN_TRAIN_STAGE_IMAGES    [2n][H][W][C] the gathered images, images order
+ *   OVN_TRAIN_STAGE_ACT       layer l: [2n][h_out][w_out][cout] leg layer l's output, images order
+ * ovn_train_stage_size: *n = the floats of the stage; ovn_copy_train_stage: d_out[*n] = the stage, asynchronous on
+ * `stream`.  Both OVN_ERR_INVALID_ARG for a stage the handle does not hold: no successful gradient call, a
+ * whole-network stage after ovn_head_gradients, a stop stage other than the one the call stopped at, or any other
+ * stage after a stopped call.  layer is the leg layer (0 = s_conv1) for LEG_DY and ACT, 0 for every other stage.
+ * fp32 handles (OVN_ERR_BAD_CONFIG otherwise).  The gradient calls issue the same launches with or without a
+ * readback; a stop only ends the call early. */
+typedef enum ovn_train_stage {
+  OVN_TRAIN_STAGE_O1 = 0,
+  OVN_TRAIN_STAGE_X4 = 1,
+  OVN_TRAIN_STAGE_DFV_CORR = 2,
+  OVN_TRAIN_STAGE_LEG_DY = 3,
+  OVN_TRAIN_STAGE_X3 = 4,
+  OVN_TRAIN_STAGE_OVERLAP = 5,
+  OVN_TRAIN_STAGE_CORR = 6,
+  OVN_TRAIN_STAGE_DZ = 7,
+  OVN_TRAIN_STAGE_DPRE3 = 8,
+  OVN_TRAIN_STAGE_DX3 = 9,
+  OVN_TRAIN_STAGE_DO1 = 10,
+  OVN_TRAIN_STAGE_DCORR = 11,
+  OVN_TRAIN_STAGE_PART_L = 12,
+  OVN_TRAIN_STAGE_PART_R = 13,
+  OVN_TRAIN_STAGE_IMAGES = 14,
+  OVN_TRAIN_STAGE_ACT = 15
+} ovn_train_stage;
+int ovn_set_train_stop(ovn_handle* h, int32_t stage, int32_t layer);
+int ovn_train_stage_size(ovn_handle* h, int32_t stage, int32_t layer, int64_t* n);
+int ovn_copy_train_stage(ovn_handle* h, int32_t stage, int32_t layer, float* d_out, void* stream);
 
 /* ---- host-buffer convenience entry points (what a non-CUDA caller binds; bench.py e2e) ------ */
 /* Raw clouds on the host -> feature volumes on the host.  OVN_ERR_BAD_CONFIG on a handle with

@@ -29,10 +29,15 @@ SYMBOLS = [
     'ovn_head_gradients_chunks', 'ovn_net_gradients_chunks', 'ovn_copy_heads_stage',
     'ovn_heads_stage_pairs', 'ovn_leg_stage', 'ovn_encode_clouds_probs_host', 'ovn_query_cloud_probs_vs_bank_host',
     'ovn_shard_create', 'ovn_shard_open', 'ovn_shard_close', 'ovn_gather_rows',
+    'ovn_set_train_stop', 'ovn_train_stage_size', 'ovn_copy_train_stage',
 ]
 IPC_HANDLE_BYTES = 64     # ovn_shard_create / ovn_shard_open
 HEADS_STAGES = {'o1': 0, 'x3': 1, 'dense': 2, 'centres': 3}     # ovn_heads_stage
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
+TRAIN_STAGES = {'o1': 0, 'x4': 1, 'dfv_corr': 2, 'leg_dy': 3, 'x3': 4, 'overlap': 5, 'corr': 6, 'dz': 7,
+                'dpre3': 8, 'dx3': 9, 'do1': 10, 'dcorr': 11, 'part_l': 12, 'part_r': 13, 'images': 14,
+                'act': 15}      # ovn_train_stage
+TRAIN_STOPS = ('o1', 'x4', 'dfv_corr', 'leg_dy')
 
 
 class OvnConfig(C.Structure):
@@ -108,6 +113,9 @@ def lib():
   L.ovn_copy_heads_stage.argtypes = [vp, i32, i64, i64, vp, vp]
   L.ovn_heads_stage_pairs.argtypes = [vp, C.POINTER(i64)]
   L.ovn_leg_stage.argtypes = [vp, vp, i32, i32, vp, vp, vp]
+  L.ovn_set_train_stop.argtypes = [vp, i32, i32]
+  L.ovn_train_stage_size.argtypes = [vp, i32, i32, C.POINTER(i64)]
+  L.ovn_copy_train_stage.argtypes = [vp, i32, i32, vp, vp]
   L.ovn_peer_signal.argtypes = [vp, vp, i32, i32, vp]
   L.ovn_peer_wait.argtypes = [vp, vp, i32, i32, i32, vp]
   L.ovn_head_gradients.argtypes = [vp, vp, i64, vp, vp, i32, vp, vp, f32, vp, vp]

@@ -750,6 +750,12 @@ static int gradients_call(ovn_handle* h, bool whole_network, const char* fn, con
   }
   TrainState& t = *h->train;
   t.grads = kNoGrads;
+  t.stage_np = 0;
+  t.stopped = false;
+  struct ConsumeStop {                       // the stop applies to this one call, whatever it returns
+    TrainState& t;
+    ~ConsumeStop() { t.stop_stage = t.stop_layer = -1; }
+  } consume{t};
   float* p_loss = h->stage()->loss;
   if (chunked) {
     const size_t bytes = (size_t)kMaxSumParts * 3 * sizeof(float);
@@ -776,9 +782,15 @@ static int gradients_call(ovn_handle* h, bool whole_network, const char* fn, con
   if (rc == OVN_OK) rc = sanitize_indices(h, d_right_idx, n_pairs, n_rows, kErrBadIndex, r, s);
   if (rc == OVN_OK) rc = run(l, r);
   if (rc != OVN_OK) return rc;
-  OVN_CUDA(h, cudaMemcpyAsync(p_loss, ch.loss, (size_t)ch.n * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (!t.stopped)
+    OVN_CUDA(h, cudaMemcpyAsync(p_loss, ch.loss, (size_t)ch.n * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
   rc = check_device_error(h, s);            // synchronises s; a bad index -> OVN_ERR_INVALID_ARG
   if (rc != OVN_OK) return rc;
+  t.stage_np = n_pairs;
+  t.stage_net = whole_network;
+  t.stage_stop = t.stopped ? t.stop_stage : -1;
+  t.stage_stop_layer = t.stopped ? t.stop_layer : -1;
+  if (t.stopped) return OVN_OK;             // no losses, no gradients, no batch
   memcpy(h_loss, p_loss, (size_t)ch.n * 3 * sizeof(float));
   if (!chunked) t.grads = whole_network ? kNetGrads : kHeadGrads;
   return OVN_OK;
@@ -937,6 +949,79 @@ int ovn_copy_net_volumes(ovn_handle* h, float* d_out, void* stream) {
   return copy_net_volumes_fp32(h, d_out, (cudaStream_t)stream);
 }
 
+// ---- stages of a gradient call (tests and diagnostics) ------------------------------------------------------
+static bool stop_stage(int32_t stage) { return stage >= OVN_TRAIN_STAGE_O1 && stage <= OVN_TRAIN_STAGE_LEG_DY; }
+static bool layer_stage(int32_t stage) { return stage == OVN_TRAIN_STAGE_LEG_DY || stage == OVN_TRAIN_STAGE_ACT; }
+static bool net_stage(int32_t stage) {
+  return stage == OVN_TRAIN_STAGE_DFV_CORR || stage == OVN_TRAIN_STAGE_LEG_DY || stage >= OVN_TRAIN_STAGE_DCORR;
+}
+
+// A stage and layer the handle's network has: OVN_ERR_INVALID_ARG otherwise
+static int check_train_stage(ovn_handle* h, const char* fn, int32_t stage, int32_t layer) {
+  if (h->cfg.precision != OVN_PREC_FP32)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "%s: training needs a precision fp32 handle", fn);
+  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "%s: %s", fn, h->net_error.c_str());
+  if (stage < OVN_TRAIN_STAGE_O1 || stage > OVN_TRAIN_STAGE_ACT)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: unknown ovn_train_stage %d", fn, stage);
+  if (layer_stage(stage) ? (layer < 0 || layer >= h->n_leg) : layer != 0)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: layer %d of stage %d (a leg layer 0..%d for LEG_DY and ACT, else 0)", fn,
+                layer, stage, h->n_leg - 1);
+  return OVN_OK;
+}
+
+int ovn_set_train_stop(ovn_handle* h, int32_t stage, int32_t layer) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  const char* fn = "ovn_set_train_stop";
+  if (stage != -1) {
+    int rc = check_train_stage(h, fn, stage, layer);
+    if (rc != OVN_OK) return rc;
+    if (!stop_stage(stage))
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: stage %d is read after a whole call, not a stop", fn, stage);
+  }
+  if (!h->train) {
+    int rc = train_alloc(h);
+    if (rc != OVN_OK) return rc;
+  }
+  h->train->stop_stage = stage;
+  h->train->stop_layer = stage == -1 ? -1 : layer;
+  return OVN_OK;
+}
+
+// The stage is held when the last gradient call succeeded, ran the flow the stage belongs to and stopped at it (a
+// stop stage) or ran to the end (any other stage)
+static int held_stage(ovn_handle* h, const char* fn, int32_t stage, int32_t layer) {
+  int rc = check_train_stage(h, fn, stage, layer);
+  if (rc != OVN_OK) return rc;
+  const TrainState* t = h->train.get();
+  if (!t || t->stage_np == 0)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: no stages (no successful gradient call since the handle trained last)",
+                fn);
+  if (net_stage(stage) && !t->stage_net)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: stage %d exists after a whole-network call only", fn, stage);
+  if (stop_stage(stage) ? (t->stage_stop != stage || t->stage_stop_layer != layer) : t->stage_stop != -1)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: stage %d layer %d is not held (the last call stopped at stage %d layer %d)",
+                fn, stage, layer, t->stage_stop, t->stage_stop_layer);
+  return OVN_OK;
+}
+
+int ovn_train_stage_size(ovn_handle* h, int32_t stage, int32_t layer, int64_t* n) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  REQUIRE(h, n, "NULL pointer");
+  int rc = held_stage(h, "ovn_train_stage_size", stage, layer);
+  if (rc != OVN_OK) return rc;
+  *n = train_stage_floats(h, stage, layer);
+  return OVN_OK;
+}
+
+int ovn_copy_train_stage(ovn_handle* h, int32_t stage, int32_t layer, float* d_out, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, d_out, "NULL pointer");
+  int rc = held_stage(h, "ovn_copy_train_stage", stage, layer);
+  if (rc != OVN_OK) return rc;
+  return copy_train_stage_fp32(h, stage, layer, d_out, (cudaStream_t)stream);
+}
+
 // ovn_copy_train_state / ovn_set_train_state: the Adagrad accumulators, in the layout of ovn_copy_gradients
 static int train_state_call(ovn_handle* h, const char* fn, const void* ptr) {
   if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "%s: %s", fn, h->net_error.c_str());
@@ -984,6 +1069,8 @@ int ovn_adagrad_step_sum(ovn_handle* h, int32_t whole_network, const float* d_pa
   if (n_parts > kMaxSumParts)
     OVN_SET_ERR(h, OVN_ERR_CAPACITY, "ovn_adagrad_step_sum: n_parts=%d exceeds %d", n_parts, kMaxSumParts);
   REQUIRE(h, d_parts && h_weights, "NULL pointer");
+  REQUIRE(h, !h->train || h->train->stage_np == 0 || h->train->stage_stop == -1,
+          "the last gradient call stopped at a stage (ovn_set_train_stop): its parts are not gradients");
   if (!h->train) {
     int rc = train_alloc(h);
     if (rc != OVN_OK) return rc;

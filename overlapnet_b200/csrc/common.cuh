@@ -155,7 +155,24 @@ struct TrainState {
   Buffer<float> wt;             // a leg kernel with in / out swapped
   int64_t net_fv_off = 0;       // the last ovn_net_gradients batch: its volumes [2 net_np][Wf][128] at acts + net_fv_off
   int net_np = 0;
+  // Stage readback (ovn_set_train_stop / ovn_copy_train_stage).  stop_*: the point where the next gradient call
+  // stops, -1 = none; consumed by that call.  stopped: the running call reached it.  The stages of the last
+  // gradient call: its pairs (0 = none), its flow and where it stopped (-1 = it ran to the end).
+  int stop_stage = -1, stop_layer = -1;
+  bool stopped = false;
+  const float* stop_buf = nullptr;   // the live buffer of the stage the call stopped at
+  int stage_np = 0;
+  bool stage_net = false;
+  int stage_stop = -1, stage_stop_layer = -1;
 };
+// true when the running gradient call stops at (stage, layer), whose value is in `live`, or has stopped before
+inline bool train_stop_here(TrainState& t, int stage, int layer, const float* live) {
+  if (!t.stopped && t.stop_stage == stage && t.stop_layer == layer) {
+    t.stopped = true;
+    t.stop_buf = live;
+  }
+  return t.stopped;
+}
 }  // namespace ovn
 
 struct ovn_handle {
@@ -386,6 +403,10 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
 int net_max_pairs(const ovn_handle* h);   // largest n_pairs of one ovn_net_gradients call (launch grid limits)
 int64_t train_workspace_bytes(const ovn_handle* h, bool whole_network, int np);   // ovn_train_workspace_bytes
 int copy_net_volumes_fp32(ovn_handle* h, float* d_out, cudaStream_t s);
+// ovn_train_stage_size / ovn_copy_train_stage: the floats of a stage of the last gradient call, and a copy of them
+// (the caller has checked that the stage is held)
+int64_t train_stage_floats(const ovn_handle* h, int stage, int layer);
+int copy_train_stage_fp32(ovn_handle* h, int stage, int layer, float* d_out, cudaStream_t s);
 // The Adagrad step of the heads' (or with whole_network every layer's) prefix of the flat vector, from the
 // weighted sum of d_parts [n_parts][that length]: one launch
 int adagrad_sum_fp32(ovn_handle* h, bool whole_network, const float* d_parts, int n_parts, const float* h_weights,

@@ -608,6 +608,9 @@ constexpr int kSplitBlocks = 528;      // target CTAs of a split-K launch (4 per
 //          tf.nn.weighted_cross_entropy_with_logits, the logits are raw correlation sums)
 //   L = 5 L_ov + L_or;  dL/dyhat_p = 5 sigmoid'(u_p) * 24 * sign(yhat_p - y_p) / B  (sign(0) = 0, TF's abs)
 //   dz_p = dL/dyhat_p * yhat_p (1 - yhat_p);  the Dense bias gradient = sum_p dz_p.
+// dz is evaluated in double from the float32 yhat and y and rounded once, with sigmoid'(u) = e / (1 + e)^2,
+// e = exp(-u): in float32, 1 - sigmoid(u) cancels as |yhat - y| grows (29 % off at 0.9, 0 at 0.95).  1 - yhat is
+// exact for yhat >= 1/2, so yhat (1 - yhat) adds no cancellation of its own to the stored yhat's.
 __global__ void __launch_bounds__(256)
 k_train_loss(const float* __restrict__ ov, const float* __restrict__ corr, const float* __restrict__ gt_ov,
              const int32_t* __restrict__ gt_or, int np, int Wf, float min_ov, float* __restrict__ dz,
@@ -620,8 +623,10 @@ k_train_loss(const float* __restrict__ ov, const float* __restrict__ corr, const
     const float u = (fabsf(d) + 0.25f) * 24.f - 12.f;
     const float sg = 1.f / (1.f + expf(-u));
     a += sg;
-    const float sgn = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);
-    dz[p] = 5.f * sg * (1.f - sg) * 24.f * sgn / (float)np * (y * (1.f - y));
+    const double dd = (double)y - (double)gt_ov[p];
+    const double e = exp(-((fabs(dd) + 0.25) * 24.0 - 12.0));
+    const double sgn = dd > 0.0 ? 1.0 : (dd < 0.0 ? -1.0 : 0.0);
+    dz[p] = (float)(5.0 * 24.0 * e / ((1.0 + e) * (1.0 + e)) * sgn / np * ((double)y * (1.0 - (double)y)));
   }
   const float q = (float)Wf;
   for (int e = t; e < np * Wf; e += 256) {
@@ -790,6 +795,8 @@ int head_gradients_fp32(ovn_handle* h, const float* d_bank, const int32_t* left,
   int rc = overlap_head_fp32(h, d_bank, nullptr, left, right, np, t.x4, t.overlap, s);
   if (rc == OVN_OK) rc = corr_forward_fp32(h, d_bank, nullptr, left, right, np, t.yaw, t.corr, s);
   if (rc != OVN_OK) return rc;
+  if (train_stop_here(t, OVN_TRAIN_STAGE_O1, 0, h->d_o1) || train_stop_here(t, OVN_TRAIN_STAGE_X4, 0, t.x4))
+    return OVN_OK;
   for (int c = 0; c < ch.n; ++c) {
     const int a = ch.off[c], n = ch.size(c);
     if (n == 0) continue;
@@ -1296,7 +1303,7 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
   const int32_t* rrow = t.pair_rows + np;
   // both heads forward, losses, overlap-head backward: do1 = dL/d(c_conv1 output) is left in h->d_o1
   rc = head_gradients_fp32(h, fv, lrow, rrow, np, d_gt_overlap, d_gt_orientation, min_overlap, ch, s);
-  if (rc != OVN_OK) return rc;
+  if (rc != OVN_OK || t.stopped) return rc;
   // dL/d(volumes) = correlation-head part + |l - r| part
   float* dfv = t.dact[0];
   for (int c = 0; c < ch.n; ++c) {            // the orientation loss's 1 / (n Wf) is the chunk's
@@ -1310,6 +1317,7 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
   k_corr_backward<<<dim3((Wf + kCorrRows - 1) / kCorrRows, np, 2), kFeatC, Wf * sizeof(float), s>>>(
       t.dcorr, fv, lrow, rrow, np, Wf, dfv);
   OVN_LAUNCH_CHECK(h);
+  if (train_stop_here(t, OVN_TRAIN_STAGE_DFV_CORR, 0, dfv)) return OVN_OK;
   float* part_l = t.dfv_part;
   float* part_r = part_l + (int64_t)np * nb * vol;
   const dim3 dg_grid(kFeatC / kDgT, nit, nb * np);
@@ -1347,6 +1355,7 @@ int net_gradients_fp32(ovn_handle* h, const float* d_images, const int32_t* left
   k_relu_grad<<<blocks_for(n2 * vol), 256, 0, s>>>(dy, fv, n2 * vol);
   OVN_LAUNCH_CHECK(h);
   for (int l = h->n_leg - 1; l >= 0; --l) {
+    if (train_stop_here(t, OVN_TRAIN_STAGE_LEG_DY, l, dy)) return OVN_OK;
     const ConvSpec& L = h->leg[l];
     const float* X = l ? act[l - 1] : t.images;
     const int Kc = L.kh * L.kw * L.cin;
@@ -1397,6 +1406,57 @@ int copy_net_volumes_fp32(ovn_handle* h, float* d_out, cudaStream_t s) {
   const TrainState& t = *h->train;
   const size_t n = (size_t)2 * t.net_np * h->cfg.leg_output_width * kFeatC;
   OVN_CUDA(h, cudaMemcpyAsync(d_out, t.acts + t.net_fv_off, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  return OVN_OK;
+}
+
+// ---- stages of the last gradient call (ovn_copy_train_stage) ----------------------------------------------
+// Where a stage lives and how many floats it has, for the np pairs of the last call: *src = null for a stop stage,
+// whose buffer the call recorded when it stopped
+static int64_t train_stage_at(const ovn_handle* h, int stage, int layer, const float** src) {
+  const TrainState& t = *h->train;
+  const int64_t np = t.stage_np, n2 = 2 * np, Wf = h->cfg.leg_output_width, vol = Wf * kFeatC;
+  const int64_t nb = h->o1_w, nit = (Wf + kDgT - 1) / kDgT;
+  const ConvSpec& L2 = h->head[1];
+  const ConvSpec& L3 = h->head[2];
+  const int64_t o1_pair = (int64_t)L2.h_in * L2.w_in * L2.cin, x3_pair = (int64_t)L3.h_in * L3.w_in * L3.cin;
+  auto leg_out = [&](int l) { const ConvSpec& L = h->leg[l]; return n2 * L.h_out * L.w_out * L.cout; };
+  *src = nullptr;
+  switch (stage) {
+    case OVN_TRAIN_STAGE_O1: return np * o1_pair;
+    case OVN_TRAIN_STAGE_X4: return np * h->dense_in;
+    case OVN_TRAIN_STAGE_DFV_CORR: return n2 * vol;
+    case OVN_TRAIN_STAGE_LEG_DY: return leg_out(layer);
+    case OVN_TRAIN_STAGE_X3: *src = h->d_o2; return np * x3_pair;
+    case OVN_TRAIN_STAGE_OVERLAP: *src = t.overlap; return np;
+    case OVN_TRAIN_STAGE_CORR: *src = t.corr; return np * Wf;
+    case OVN_TRAIN_STAGE_DZ: *src = t.dz; return np;
+    case OVN_TRAIN_STAGE_DPRE3: *src = t.x4; return np * h->dense_in;
+    case OVN_TRAIN_STAGE_DX3: *src = t.dx3; return np * x3_pair;
+    case OVN_TRAIN_STAGE_DO1: *src = h->d_o1; return np * o1_pair;
+    case OVN_TRAIN_STAGE_DCORR: *src = t.dcorr; return np * Wf;
+    case OVN_TRAIN_STAGE_PART_L: *src = t.dfv_part; return np * nb * vol;
+    case OVN_TRAIN_STAGE_PART_R: *src = t.dfv_part + np * nb * vol; return np * nit * vol;
+    case OVN_TRAIN_STAGE_IMAGES: *src = t.images; return n2 * h->cfg.proj_H * h->cfg.proj_W * h->C;
+    case OVN_TRAIN_STAGE_ACT: {
+      int64_t off = 0;
+      for (int l = 0; l < layer; ++l) off += leg_out(l);
+      *src = t.acts + off;
+      return leg_out(layer);
+    }
+  }
+  return 0;
+}
+
+int64_t train_stage_floats(const ovn_handle* h, int stage, int layer) {
+  const float* src;
+  return train_stage_at(h, stage, layer, &src);
+}
+
+int copy_train_stage_fp32(ovn_handle* h, int stage, int layer, float* d_out, cudaStream_t s) {
+  const float* src;
+  const int64_t n = train_stage_at(h, stage, layer, &src);
+  if (!src) src = h->train->stop_buf;
+  OVN_CUDA(h, cudaMemcpyAsync(d_out, src, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return OVN_OK;
 }
 

@@ -509,6 +509,24 @@ class Engine:
     check(self._h, lib().ovn_copy_net_volumes(self._h, _ptr(out), self._stream()), 'ovn_copy_net_volumes')
     return out
 
+  def set_train_stop(self, stage=None, layer=0):
+    """ovn_set_train_stop: the next gradient call stops once ``stage`` ('o1', 'x4', 'dfv_corr', or 'leg_dy' of leg
+    layer ``layer``) is complete, before the step overwrites it.  None: no stop."""
+    code = -1 if stage is None else _cabi.TRAIN_STAGES[stage]
+    check(self._h, lib().ovn_set_train_stop(self._h, code, int(layer) if stage is not None else -1),
+          'ovn_set_train_stop')
+
+  def train_stage(self, stage, layer=0):
+    """ovn_copy_train_stage: a stage of the last gradient call as a flat float32 cuda tensor (layouts in
+    include/ovn_b200.h, ovn_train_stage).  ``layer``: the leg layer of 'leg_dy' and 'act'."""
+    code = _cabi.TRAIN_STAGES[stage]
+    n = C.c_int64(0)
+    check(self._h, lib().ovn_train_stage_size(self._h, code, int(layer), C.byref(n)), 'ovn_train_stage_size')
+    out = torch.empty((int(n.value),), dtype=torch.float32, device=self.device)
+    check(self._h, lib().ovn_copy_train_stage(self._h, code, int(layer), _ptr(out), self._stream()),
+          'ovn_copy_train_stage')
+    return out
+
   def net_adagrad_step(self, lr):
     """ovn_net_adagrad_step: Adagrad update of every leg and head layer from the last net_gradients."""
     check(self._h, lib().ovn_net_adagrad_step(self._h, float(lr), self._stream()), 'ovn_net_adagrad_step')
