@@ -96,7 +96,8 @@ int64_t     ovn_launch_count(const ovn_handle* h);
 /* ---- per-kernel device timing (bench.py roofline): CUDA events recorded around the named kernels
  * on the launching stream while enabled.  ovn_profile_read synchronises the device, returns the
  * accumulated milliseconds / launch count since the last read and resets them.  Names:
- * "delta_conv1", "conv2", "conv3", "corr", "project_scatter", "project_gather", "leg", "gather_rows". */
+ * "delta_conv1", "conv2", "conv3", "corr", "project_scatter", "project_gather", "leg", "gather_rows",
+ * "rows_topk". */
 int ovn_profile_enable(ovn_handle* h, int on);
 int ovn_profile_read(ovn_handle* h, const char* kernel, double* total_ms, int64_t* launches);
 
@@ -220,6 +221,28 @@ int ovn_heads_1vsN(ovn_handle* h, const float* d_bank, int64_t bank_size, const 
  * The loop over rows runs inside the library (no per-row host round trip through the caller). */
 int ovn_heads_rows_vs_bank(ovn_handle* h, const float* d_bank, int64_t bank_size, int64_t row_lo, int64_t row_hi,
                            float* d_overlap, int32_t* d_yaw, void* stream);
+
+/* ---- best matches of each row, reduced on the device (loop-closure evaluation, DESIGN.md section 7) -------
+ * A row's records are ordered by overlap, descending, then by index, ascending; NaN ranks above every number
+ * and -0 equals +0.  Each record carries the overlap and yaw stored at its index.  Slots beyond min(k, the row's
+ * length) hold index = -1, overlap = -1, yaw = 0.  Outputs: d_top_overlap f32 / d_top_index i32 / d_top_yaw i32,
+ * each [rows][k].  k must be in [1, 32].  Every argument is checked before anything is launched
+ * (OVN_ERR_INVALID_ARG).  The kernel is profiled as "rows_topk".
+ *
+ * ovn_rows_topk: the best k records of each row of a caller's score matrix, e.g. ovn_heads_rows_vs_bank's output.
+ * Row r is d_overlap / d_yaw [r * stride, r * stride + h_n[r]); h_n: host, [rows], each in [0, stride]. */
+int ovn_rows_topk(ovn_handle* h, const float* d_overlap, const int32_t* d_yaw, int64_t rows, int64_t stride,
+                  const int32_t* h_n /* [rows], host */, int32_t k, float* d_top_overlap, int32_t* d_top_index,
+                  int32_t* d_top_yaw, void* stream);
+
+/* ovn_heads_prefix_topk: for each row i in [row_lo, row_hi), ovn_heads_1vsN with query d_bank[i] (RIGHT) against
+ * the candidates [0, h_n_cand[i - row_lo]) (LEFT), then the best k records of that row, index = candidate j.
+ * The rows' scores go to a handle-owned scratch of at most 2^21 pairs (16 MiB, allocated by the first call); one
+ * k_rows_topk launch reduces the rows the scratch holds whenever the next row does not fit, so only the [rows][k]
+ * records leave the call.  h_n_cand: host, [row_hi - row_lo], each in [0, bank_size]. */
+int ovn_heads_prefix_topk(ovn_handle* h, const float* d_bank, int64_t bank_size, int64_t row_lo, int64_t row_hi,
+                          const int32_t* h_n_cand /* [row_hi - row_lo], host */, int32_t k, float* d_top_overlap,
+                          int32_t* d_top_index, int32_t* d_top_yaw, void* stream);
 
 /* ---- resident bank (Infer keeps self.feature_volumes across calls, infer.py:113,184-193) ---------
  * The tensor-core heads consume fp16 / hi-lo split copies of the LEFT volumes.  Without this call

@@ -30,7 +30,9 @@ SYMBOLS = [
     'ovn_heads_stage_pairs', 'ovn_leg_stage', 'ovn_encode_clouds_probs_host', 'ovn_query_cloud_probs_vs_bank_host',
     'ovn_shard_create', 'ovn_shard_open', 'ovn_shard_close', 'ovn_gather_rows',
     'ovn_set_train_stop', 'ovn_train_stage_size', 'ovn_copy_train_stage',
+    'ovn_rows_topk', 'ovn_heads_prefix_topk',
 ]
+TOPK_MAX = 32     # ovn_rows_topk / ovn_heads_prefix_topk: k in [1, TOPK_MAX]
 IPC_HANDLE_BYTES = 64     # ovn_shard_create / ovn_shard_open
 HEADS_STAGES = {'o1': 0, 'x3': 1, 'dense': 2, 'centres': 3}     # ovn_heads_stage
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
@@ -105,6 +107,8 @@ def lib():
   L.ovn_heads_1vsN.argtypes = [vp, vp, i64, vp, vp, i32, vp, vp, vp, vp]
   L.ovn_bank_prepare.argtypes = [vp, vp, i64, i64, i64, vp]
   L.ovn_heads_rows_vs_bank.argtypes = [vp, vp, i64, i64, i64, vp, vp, vp]
+  L.ovn_rows_topk.argtypes = [vp, vp, vp, i64, i64, vp, i32, vp, vp, vp, vp]
+  L.ovn_heads_prefix_topk.argtypes = [vp, vp, i64, i64, i64, vp, i32, vp, vp, vp, vp]
   L.ovn_bank_release.argtypes = [vp, vp]
   L.ovn_check.argtypes = [vp, vp]
   L.ovn_set_feature_center.argtypes = [vp, vp]

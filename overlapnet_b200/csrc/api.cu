@@ -339,7 +339,7 @@ int ovn_profile_read(ovn_handle* h, const char* kernel, double* total_ms, int64_
   DeviceGuard guard(h);
   if (!kernel || !total_ms || !launches) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_profile_read: NULL argument");
   static const char* names[kProfKinds] = {"delta_conv1", "conv2", "conv3", "corr", "project_scatter",
-                                          "project_gather", "leg", "gather_rows"};
+                                          "project_gather", "leg", "gather_rows", "rows_topk"};
   int kind = -1;
   for (int i = 0; i < kProfKinds; ++i) if (strcmp(kernel, names[i]) == 0) kind = i;
   if (kind < 0) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_profile_read: unknown kernel '%s'", kernel);
@@ -696,6 +696,80 @@ int ovn_heads_rows_vs_bank(ovn_handle* h, const float* d_bank, int64_t bank_size
     if (rc != OVN_OK) return rc;
   }
   return OVN_OK;
+}
+
+int ovn_rows_topk(ovn_handle* h, const float* d_overlap, const int32_t* d_yaw, int64_t rows, int64_t stride,
+                  const int32_t* h_n, int32_t k, float* d_top_overlap, int32_t* d_top_index, int32_t* d_top_yaw,
+                  void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, k >= 1 && k <= kTopkMax, "k must be in [1, 32]");
+  REQUIRE(h, rows >= 0 && stride >= 0 && stride <= INT32_MAX, "rows and stride must be in [0, 2^31)");
+  if (rows == 0) return OVN_OK;
+  REQUIRE(h, d_overlap && d_yaw && h_n && d_top_overlap && d_top_index && d_top_yaw, "NULL pointer");
+  std::vector<int64_t> off((size_t)rows);
+  for (int64_t r = 0; r < rows; ++r) {
+    if (h_n[r] < 0 || h_n[r] > stride)
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_rows_topk: n[%lld] = %d is outside [0, stride = %lld]", (long long)r,
+                  h_n[r], (long long)stride);
+    off[(size_t)r] = r * stride;
+  }
+  return rows_topk(h, d_overlap, d_yaw, off.data(), h_n, rows, k, d_top_overlap, d_top_index, d_top_yaw,
+                   (cudaStream_t)stream);
+}
+
+int ovn_heads_prefix_topk(ovn_handle* h, const float* d_bank, int64_t bank_size, int64_t row_lo, int64_t row_hi,
+                          const int32_t* h_n_cand, int32_t k, float* d_top_overlap, int32_t* d_top_index,
+                          int32_t* d_top_yaw, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, k >= 1 && k <= kTopkMax, "k must be in [1, 32]");
+  REQUIRE(h, bank_size >= 0 && bank_size <= INT32_MAX && row_lo >= 0 && row_lo <= row_hi && row_hi <= bank_size,
+          "bad row range");
+  if (row_lo == row_hi) return OVN_OK;
+  REQUIRE(h, d_bank && h_n_cand && d_top_overlap && d_top_index && d_top_yaw, "NULL pointer");
+  const int64_t rows = row_hi - row_lo;
+  for (int64_t r = 0; r < rows; ++r)
+    if (h_n_cand[r] < 0 || h_n_cand[r] > bank_size || h_n_cand[r] > kTopkScratchPairs)
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_heads_prefix_topk: n_cand[%lld] = %d is outside [0, bank_size = %lld]",
+                  (long long)r, h_n_cand[r], (long long)bank_size);
+  if (!h->net_ok) OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "ovn_heads_prefix_topk: %s", h->net_error.c_str());
+  if (!h->weights_ready) OVN_SET_ERR(h, OVN_ERR_WEIGHTS, "ovn_heads_prefix_topk: weights not finalised");
+  int rc = h->d_topk_scratch.ensure(h, (size_t)kTopkScratchPairs * (sizeof(float) + sizeof(int32_t)));
+  if (rc != OVN_OK) return rc;
+  float* s_ov = reinterpret_cast<float*>(h->d_topk_scratch.get());
+  int32_t* s_yaw = reinterpret_cast<int32_t*>(s_ov + kTopkScratchPairs);
+  const size_t vol = (size_t)h->cfg.leg_output_width * kFeatC;
+  cudaStream_t s = (cudaStream_t)stream;
+  // Rows are scored into the scratch back to back.  When the next row does not fit, one k_rows_topk launch reduces
+  // the rows the scratch holds (a "fill"), and the next fill reuses it in stream order.
+  std::vector<int64_t> off;
+  std::vector<int32_t> len;
+  int64_t used = 0, first = 0;
+  auto reduce_fill = [&]() -> int {
+    const int rc2 = rows_topk(h, s_ov, s_yaw, off.data(), len.data(), (int64_t)off.size(), k,
+                              d_top_overlap + first * k, d_top_index + first * k, d_top_yaw + first * k, s);
+    first += (int64_t)off.size();
+    off.clear();
+    len.clear();
+    used = 0;
+    return rc2;
+  };
+  for (int64_t r = 0; r < rows; ++r) {
+    const int32_t n = h_n_cand[r];
+    if (used + n > kTopkScratchPairs || (int64_t)off.size() == kTopkRowsPerLaunch) {
+      if ((rc = reduce_fill()) != OVN_OK) return rc;
+    }
+    if (n > 0) {
+      rc = ovn_heads_1vsN(h, d_bank, bank_size, d_bank + (size_t)(row_lo + r) * vol, nullptr, n, s_ov + used,
+                          s_yaw + used, nullptr, stream);
+      if (rc != OVN_OK) return rc;
+    }
+    off.push_back(used);
+    len.push_back(n);
+    used += n;
+  }
+  return reduce_fill();
 }
 
 // ---- training precision ---------------------------------------------------------------------------

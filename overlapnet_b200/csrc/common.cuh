@@ -69,7 +69,7 @@ static_assert(sizeof(float) == sizeof(int32_t), "the three staging arrays are 4 
 constexpr int kFeatC = 128;           // leg output channels (generateNet.py:214)
 constexpr int kMaxLegLayers = 12;
 enum ProfKind { PROF_DELTA = 0, PROF_CONV2, PROF_CONV3, PROF_CORR, PROF_SCATTER, PROF_GATHER, PROF_LEG, PROF_GATHER_ROWS,
-                kProfKinds };
+                PROF_ROWS_TOPK, kProfKinds };
 
 // The one owner of another process's shard mapped by ovn_shard_open (cudaIpcOpenMemHandle); unmaps it on
 // destruction.  Move-only, like Buffer.
@@ -225,6 +225,9 @@ struct ovn_handle {
   ovn::Buffer<float> d_stage_points;         // staged clouds, grown on use
   ovn::Buffer<int64_t> d_stage_offsets;      // [max_batch_scans + 1], allocated on first use
   ovn::PinnedBuffer<uint8_t> h_pinned;       // StageHeader, then candidate indices / overlaps / yaws [max_batch_pairs]
+  // ovn_rows_topk / ovn_heads_prefix_topk, allocated on first use
+  ovn::Buffer<uint8_t> d_topk_rows;          // one k_rows_topk launch's row offsets (int64) then row lengths (int32)
+  ovn::Buffer<uint8_t> d_topk_scratch;       // ovn_heads_prefix_topk: kTopkScratchPairs overlaps (f32), then yaws (i32)
   // a sharded training image bank (ovn_shard_*): this process's shards, then the other processes' shards it
   // mapped.  Declared in this order so that the mappings are closed before the own shards are freed.
   std::vector<ovn::Buffer<uint8_t>> own_shards;
@@ -418,6 +421,15 @@ int gather_images(ovn_handle* h, const float* d_images, int64_t n_images, const 
 // k_gather_rows per kGatherRowsCap rows; the caller has checked every pointer and row_bytes % 16 == 0
 constexpr int kGatherRowsCap = 1024;
 int gather_rows(ovn_handle* h, const void* const* h_src, int n, int64_t row_bytes, void* d_dst, cudaStream_t s);
+
+// the best k <= kTopkMax records of each row (rows_topk.cu): row r is the h_len[r] overlaps / yaws at h_off[r]
+// (element offsets into d_ov / d_yaw, host arrays); one k_rows_topk launch per kTopkRowsPerLaunch rows.  The
+// caller has checked k and every length.
+constexpr int kTopkMax = 32;
+constexpr int64_t kTopkRowsPerLaunch = 65536;
+constexpr int64_t kTopkScratchPairs = int64_t(1) << 21;   // ovn_heads_prefix_topk's scratch: 16 MiB
+int rows_topk(ovn_handle* h, const float* d_ov, const int32_t* d_yaw, const int64_t* h_off, const int32_t* h_len,
+              int64_t rows, int k, float* d_top_ov, int32_t* d_top_idx, int32_t* d_top_yaw, cudaStream_t s);
 
 int corr_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* left,
                       const int32_t* right, int np, int32_t* d_yaw, float* d_corr, cudaStream_t s);

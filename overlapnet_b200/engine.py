@@ -445,6 +445,38 @@ class Engine:
                                                self._stream()), 'ovn_heads_rows_vs_bank')
     return ov, yaw
 
+  def _topk_out(self, rows, k):
+    dev = self.device
+    return (torch.empty((rows, k), dtype=torch.float32, device=dev), torch.empty((rows, k), dtype=torch.int32, device=dev),
+            torch.empty((rows, k), dtype=torch.int32, device=dev))
+
+  def rows_topk(self, overlap, yaw, n, k):
+    """ovn_rows_topk: the best k (1..32) records of each row of ``overlap`` f32 / ``yaw`` i32 [rows, stride] cuda
+    tensors, row r's first n[r] entries (``n``: host integers).  Returns (overlap f32, index i32, yaw i32), each
+    [rows, k] cuda; ordered by overlap descending, then index ascending; empty slots index -1, overlap -1, yaw 0."""
+    assert overlap.dtype == torch.float32 and yaw.dtype == torch.int32 and overlap.shape == yaw.shape
+    assert overlap.dim() == 2 and overlap.is_contiguous() and yaw.is_contiguous()
+    rows, stride = int(overlap.shape[0]), int(overlap.shape[1])
+    nn = np.ascontiguousarray(n, np.int32).reshape(-1)
+    assert nn.size == rows
+    out = self._topk_out(rows, int(k))
+    check(self._h, lib().ovn_rows_topk(self._h, _ptr(overlap), _ptr(yaw), rows, stride, nn.ctypes.data_as(C.c_void_p),
+                                       int(k), *[_ptr(t) for t in out], self._stream()), 'ovn_rows_topk')
+    return out
+
+  def heads_prefix_topk(self, bank, row_lo, row_hi, n_cand, k):
+    """ovn_heads_prefix_topk: for each row i in [row_lo, row_hi), query bank[i] (RIGHT) against the candidates
+    bank[0 : n_cand[i - row_lo]] (LEFT), reduced on the device to its best k (1..32) records.  ``n_cand``: host
+    integers.  Returns (overlap f32, index i32, yaw i32), each [row_hi - row_lo, k] cuda, ordered as rows_topk."""
+    rows = int(row_hi) - int(row_lo)
+    nn = np.ascontiguousarray(n_cand, np.int32).reshape(-1)
+    assert nn.size == max(rows, 0)
+    out = self._topk_out(max(rows, 0), int(k))
+    check(self._h, lib().ovn_heads_prefix_topk(self._h, _ptr(bank), int(bank.shape[0]), int(row_lo), int(row_hi),
+                                               nn.ctypes.data_as(C.c_void_p), int(k), *[_ptr(t) for t in out],
+                                               self._stream()), 'ovn_heads_prefix_topk')
+    return out
+
   def bank_prepare(self, bank, first=0, count=None):
     """Keep the tensor-core operand copies of bank rows [first, first+count) resident: later heads
     calls on this same tensor skip the per-call conversion (ovn_bank_prepare)."""

@@ -1,0 +1,371 @@
+"""Loop-closure evaluation of a trained model over a whole sequence, on the GPU: the experiment of the OverlapNet
+paper, with the candidate rules of the reference's demo 3 (demo/demo3_lcd.py).
+
+  python -m overlapnet_b200.lcd_eval [config/demo.yml] [--top-k K] [--exclude-frames 100] [--exclude-distance 50]
+                                     [--gt-overlap 0.3]
+  torchrun --nproc_per_node G -m overlapnet_b200.lcd_eval ...            (the rows split over G GPUs)
+
+The protocol (DESIGN.md section 7):
+  poses       demo 3's LiDAR-frame poses T_velo_cam . pose0^-1 . pose . T_cam_velo (gt_files.kitti_poses_in_lidar);
+              the travelled distance L_i accumulates the xy steps as lcd.LoopClosureDetector.step does.
+  candidates  of query i: the scans j < i - exclude_frames with L_i - L_j > exclude_distance (gate_candidates'
+              time and distance rules, without the covariance ellipse).  L is non-decreasing, so they are a
+              prefix [0, c_i) (``past_prefix``).
+  direction   LEFT = candidate j, RIGHT = query i, as demo 3 calls Infer.infer_multiple.
+  records     the best k of each row, by overlap descending then index ascending, with the heads' yaw
+              (Engine.heads_prefix_topk); empty slots are index -1, overlap -1, yaw 0.
+  truth       g[i, j] = the overlap of row j of com_overlap_yaw(frame_idx = i) (gt.overlap_yaw_all_pairs);
+              query i is positive when max_{j < c_i} g[i, j] > gt_overlap, and correct when g[i, j*_i] > gt_overlap
+              for its top record j*_i.  Queries are the rows with c_i > 0.
+  curve       for every distinct top score t, the queries with s_i >= t are declared (``metrics``).
+
+Scans are encoded from the raw ``.bin`` files (Infer.encode_clouds); configs with class probabilities are
+refused, since they would need a ``.label`` file per scan.  Results go to ``<experiments_path>/<testname>`` of
+the network config: ``lcd_results.npz`` and ``lcd_summary.json``."""
+import argparse
+import json
+import logging
+import os
+import sys
+
+import numpy as np
+import torch
+
+from ._cabi import TOPK_MAX
+
+logger = logging.getLogger('overlapnet_b200.lcd_eval')
+
+OPERATING_POINT = 0.3          # demo3_lcd.py:119 declares a loop when max overlap > 0.3 (strict)
+
+
+# ---- the candidate prefix ---------------------------------------------------------------------------------
+def travelled_distance(traj):
+  """L_i: the xy steps of ``traj`` (n, 2) accumulated one by one, as lcd.LoopClosureDetector.step does."""
+  traj = np.asarray(traj, dtype=float)
+  L = [0]
+  for i in range(1, len(traj)):
+    L.append(L[-1] + np.linalg.norm(traj[i] - traj[i - 1]))
+  return np.asarray(L, dtype=float)
+
+
+def past_prefix(traj, exclude_frames=100, exclude_distance=50):
+  """c (int64 [n]): query i's candidates are the scans [0, c_i), those with j < i - exclude_frames and
+  L_i - L_j > exclude_distance (lcd.gate_candidates' time and distance rules)."""
+  L = travelled_distance(traj)
+  n = L.size
+  c = np.zeros(n, np.int64)
+  for i in range(n):
+    m = max(i - int(exclude_frames), 0)
+    # L is non-decreasing, so L_i - L_j > d holds on a prefix of j: count it with the rule's own expression
+    c[i] = int(np.count_nonzero(L[i] - L[:m] > exclude_distance))
+  return c
+
+
+def split_rows(c, world):
+  """Contiguous row ranges [(lo, hi)] of equal sum of c, up to one row: rank r starts at the first row whose
+  preceding sum reaches r * sum(c) / world."""
+  c = np.asarray(c, np.int64)
+  before = np.concatenate([[0], np.cumsum(c)])[:-1]
+  total = int(c.sum())
+  cuts = [0] + [int(np.searchsorted(before * world, r * total, side='left')) for r in range(1, world)] + [c.size]
+  for r in range(1, world + 1):
+    cuts[r] = max(cuts[r], cuts[r - 1])
+  return [(cuts[r], cuts[r + 1]) for r in range(world)]
+
+
+# ---- search and ground truth --------------------------------------------------------------------------------
+def search(engine, bank, c, k, row_lo=0, row_hi=None):
+  """Rows [row_lo, row_hi) of the causal search: each scan's best k records among its candidates [0, c_i).
+  Returns host arrays (overlap f32, index i32, yaw i32), each [rows, k]."""
+  row_hi = int(bank.shape[0]) if row_hi is None else int(row_hi)
+  ov, idx, yaw = engine.heads_prefix_topk(bank, row_lo, row_hi, np.asarray(c)[row_lo:row_hi], k)
+  engine.check()
+  return ov.cpu().numpy(), idx.cpu().numpy(), yaw.cpu().numpy()
+
+
+def ground_truth(clouds, poses, rows, c, top_index, width=360, local=False):
+  """The ground truth of ``rows`` (one per query; ``c`` and ``top_index`` [rows, k] are theirs): a dict of
+  best (float64: max_{j < c_i} g[i, j], -1 when c_i = 0), top_overlap (float64 [rows, k]: g at each record, -1 in
+  an empty slot) and top_yaw_bin (int64 [rows, k]: the ground-truth yaw bin of each record, 0 in an empty slot).
+  Only rows with candidates are computed, with gt.overlap_yaw_all_pairs; ``width``: the yaw bins' resolution
+  (leg_output_width); ``local``: on this process only, even in a process group."""
+  from . import gt
+  rows = np.asarray(rows, np.int64)
+  c = np.asarray(c, np.int64)
+  k = top_index.shape[1]
+  best = np.full(rows.size, -1.0)
+  top_ov = np.full((rows.size, k), -1.0)
+  top_bin = np.zeros((rows.size, k), np.int64)
+  live = np.flatnonzero(c > 0)
+  if live.size:
+    if local:
+      # the ranks of a node may share a GPU: each takes half of the free memory over the world size for the clouds
+      budget = torch.cuda.mem_get_info()[0] // (2 * torch.distributed.get_world_size())
+      res = gt._all_pairs_local(clouds, np.asarray(poses, np.float64), rows[live], width, budget, 0, 0)
+    else:
+      res = gt.overlap_yaw_all_pairs(clouds, poses, frames=rows[live], leg_output_width=width)
+    if np.any(res.valid_num == 0):
+      raise ZeroDivisionError('a query scan has no valid pixel (valid_num = 0)')
+    g = res.counts.astype(np.int64) / res.valid_num.astype(np.int64)[:, None]    # as gt.all_pairs_rows divides
+    for q, r in enumerate(live):
+      best[r] = g[q, :c[r]].max()
+      ok = top_index[r] >= 0
+      top_ov[r, ok] = g[q, top_index[r, ok]]
+      top_bin[r, ok] = res.yaw_bin[q, top_index[r, ok]]
+  return {'best': best, 'top_overlap': top_ov, 'top_yaw_bin': top_bin}
+
+
+# ---- metrics ------------------------------------------------------------------------------------------------
+def metrics(top_overlap, top_index, gt_top_overlap, gt_best, gt_overlap=0.3, operating_point=OPERATING_POINT):
+  """Precision-recall of the detector from the records (``top_overlap`` / ``top_index`` [rows, k]) and their
+  ground truth (``gt_top_overlap`` [rows, k], ``gt_best`` [rows]).  Queries are the rows whose top record exists;
+  a NaN score raises.  Returns (summary dict, curve dict of arrays over the thresholds, descending)."""
+  top_overlap = np.asarray(top_overlap, np.float32)
+  top_index = np.asarray(top_index)
+  gt_top = np.asarray(gt_top_overlap, np.float64)
+  query = top_index[:, 0] >= 0
+  s = top_overlap[query, 0].astype(np.float64)
+  if np.isnan(s).any():
+    raise ValueError('a query has a NaN top overlap: the scores are poisoned')
+  correct_k = (top_index[query] >= 0) & (gt_top[query] > gt_overlap)
+  correct = correct_k[:, 0]
+  positive = np.asarray(gt_best, np.float64)[query] > gt_overlap
+  n_pos = int(positive.sum())
+  thr = np.unique(s)[::-1]
+  order = np.argsort(-s, kind='stable')
+  tp_cum = np.cumsum(correct[order])
+  # declared at threshold t: every query with s >= t, i.e. the first (number of scores >= t) of the descending order
+  n_decl = np.searchsorted(-s[order], -thr, side='right')
+  tp = tp_cum[n_decl - 1] if thr.size else np.zeros(0, np.int64)
+  fp = n_decl - tp
+  precision = np.where(n_decl > 0, tp / np.maximum(n_decl, 1), 1.0)
+  recall = tp / n_pos if n_pos else np.full(thr.size, np.nan)
+  if n_pos:
+    ap = float(np.sum(np.diff(np.concatenate([[0.0], recall])) * precision))
+    pr = precision + recall
+    f1 = np.where(pr > 0, 2 * precision * recall / np.where(pr > 0, pr, 1), 0.0)
+    b = int(np.argmax(f1)) if thr.size else -1
+  else:
+    ap, f1, b = float('nan'), np.full(thr.size, np.nan), -1
+  op = s > operating_point
+  op_tp = int((op & correct).sum())
+  op_n = int(op.sum())
+  summary = {
+      'queries': int(query.sum()), 'positives': n_pos, 'average_precision': ap,
+      'f1_max': float(f1[b]) if b >= 0 else float('nan'),
+      'f1_max_threshold': float(thr[b]) if b >= 0 else float('nan'),
+      'precision_at_f1_max': float(precision[b]) if b >= 0 else float('nan'),
+      'recall_at_f1_max': float(recall[b]) if b >= 0 else float('nan'),
+      'operating_point': operating_point,
+      'precision_at_operating_point': op_tp / op_n if op_n else 1.0,
+      'recall_at_operating_point': op_tp / n_pos if n_pos else float('nan'),
+      'recall_at_1': float((positive & correct).sum()) / n_pos if n_pos else float('nan'),
+      'recall_at_k': float((positive & correct_k.any(1)).sum()) / n_pos if n_pos else float('nan'),
+      'k': int(top_index.shape[1]),
+  }
+  curve = {'threshold': thr, 'tp': tp.astype(np.int64), 'fp': fp.astype(np.int64), 'precision': precision,
+           'recall': recall, 'f1': f1}
+  return summary, curve
+
+
+def true_positives_at(top_overlap, top_index, gt_top_overlap, threshold, gt_overlap=0.3):
+  """The rows whose top record is declared at ``threshold`` (s_i >= t) and correct."""
+  s = np.asarray(top_overlap)[:, 0]
+  return np.flatnonzero((np.asarray(top_index)[:, 0] >= 0) & (s >= threshold) &
+                        (np.asarray(gt_top_overlap)[:, 0] > gt_overlap))
+
+
+def yaw_errors(engine, bank, rows, cand, gt_bin, width=360):
+  """Circular yaw-bin errors of the pairs LEFT = bank[rows], RIGHT = bank[cand] (the direction of testing.py and
+  the training labels), scored by one heads call, against the ground-truth bins ``gt_bin``."""
+  from .evaluate import yaw_to_argmax
+  if len(rows) == 0:
+    return np.zeros(0, np.float64)
+  _, yaw, _ = engine.heads(bank, torch.as_tensor(np.asarray(rows, np.int32)), torch.as_tensor(np.asarray(cand, np.int32)))
+  engine.check()
+  a = np.abs(yaw_to_argmax(yaw.cpu().numpy()).astype(float) - np.asarray(gt_bin, float))
+  return np.minimum(a, width - a)                                  # evaluate.error_statistics' circular rule
+
+
+# ---- the driver ---------------------------------------------------------------------------------------------
+def _dist():
+  dist = torch.distributed
+  if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+    return dist, dist.get_rank(), dist.get_world_size()
+  return None, 0, 1
+
+
+def encode_share(infer, clouds, rank=0, world=1):
+  """This rank's share of the scans' volumes on the device, and every rank's share [(lo, hi)].  The scans are
+  encoded in batches of the Infer's batch_size at fixed positions of the sequence, and each rank takes a
+  contiguous run of whole batches: every volume comes out of the same batch, so the same bits, at any world size."""
+  from .search import shard_range
+  n = len(clouds)
+  bs = max(1, int(infer.batch_size))
+  n_batches = (n + bs - 1) // bs
+  shares = [tuple(min(n, bs * b) for b in shard_range(n_batches, r, world)) for r in range(world)]
+  lo, hi = shares[rank]
+  eng = infer._engine
+  out = torch.empty((hi - lo, eng.Wf, 128), dtype=torch.float32, device=eng.device)
+  for s0 in range(lo, hi, bs):
+    s1 = min(hi, s0 + bs)
+    batch = [np.ascontiguousarray(clouds[i]() if callable(clouds[i]) else clouds[i], np.float32) for i in range(s0, s1)]
+    out[s0 - lo:s1 - lo] = infer.encode_clouds(batch)
+  return out, shares
+
+
+def gather_bank(local, shares):
+  """The whole bank on every rank: one all_gather of the padded shares (as ShardedSearch.gather_bank), on the
+  device with NCCL and through host memory with other backends."""
+  dist = torch.distributed
+  on_device = dist.get_backend() == 'nccl'
+  pad = torch.zeros((max(hi - lo for lo, hi in shares),) + tuple(local.shape[1:]), dtype=local.dtype,
+                    device=local.device if on_device else 'cpu')
+  pad[:local.shape[0]] = local
+  parts = [torch.empty_like(pad) for _ in shares]
+  dist.all_gather(parts, pad)
+  return torch.cat([parts[r][:hi - lo] for r, (lo, hi) in enumerate(shares)]).to(local.device)
+
+
+def save_npz(path, arrays):
+  """np.savez with a fixed time stamp on every member: the same arrays give the same bytes."""
+  import zipfile
+  with zipfile.ZipFile(path, 'w', zipfile.ZIP_STORED, allowZip64=True) as z:
+    for key in sorted(arrays):
+      info = zipfile.ZipInfo(key + '.npy', date_time=(1980, 1, 1, 0, 0, 0))
+      with z.open(info, 'w', force_zip64=True) as f:
+        np.lib.format.write_array(f, np.asanyarray(arrays[key]), allow_pickle=False)
+
+
+def evaluate_clouds(infer, clouds, poses, top_k=5, exclude_frames=100, exclude_distance=50, gt_overlap=0.3,
+                    out_dir=None):
+  """Evaluate loop closure over a sequence: ``clouds`` (N, 4) float32 arrays or zero-argument callables returning
+  one, ``poses`` (n, 4, 4) LiDAR-frame poses, ``infer`` an overlapnet_b200.Infer.  In a process group every rank
+  encodes a contiguous share of the scans, the bank is all-gathered, every rank scores and labels the rows of an
+  equal share of the pairs, and rank 0 gathers them; the results do not depend on the world size.  Returns on
+  rank 0 (summary dict, results dict of arrays), None elsewhere; rank 0 writes lcd_results.npz and
+  lcd_summary.json to ``out_dir`` when given."""
+  if not 1 <= int(top_k) <= TOPK_MAX:
+    raise ValueError('top_k must be in [1, %d], got %r' % (TOPK_MAX, top_k))
+  top_k = int(top_k)
+  poses = np.asarray(poses, np.float64)
+  n = len(clouds)
+  if poses.shape != (n, 4, 4):
+    raise ValueError('poses has shape %s, expected (%d, 4, 4)' % (poses.shape, n))
+  dist, rank, world = _dist()
+  eng = infer._engine
+  c = past_prefix(poses[:, :2, 3], exclude_frames, exclude_distance)
+  local, shares = encode_share(infer, clouds, rank, world)
+  full = gather_bank(local, shares) if world > 1 else local
+  del local
+  # the tensor-core heads' numeric centres from volume 0 on every handle, before the operand copies are built
+  eng.calibrate(full[0])
+  infer._set_bank(full)
+  bank = infer._bank
+  r_lo, r_hi = split_rows(c, world)[rank]
+  top_ov, top_idx, top_yaw = search(eng, bank, c, top_k, r_lo, r_hi)
+  truth = ground_truth(clouds, poses, np.arange(r_lo, r_hi), c[r_lo:r_hi], top_idx, eng.Wf, local=world > 1)
+  part = (top_ov, top_idx, top_yaw, truth['best'], truth['top_overlap'], truth['top_yaw_bin'])
+  if world > 1:
+    parts = [None] * world if rank == 0 else None
+    dist.gather_object(part, parts, dst=0)
+    if rank != 0:
+      return None
+    part = tuple(np.concatenate([p[f] for p in parts]) for f in range(len(part)))
+  top_ov, top_idx, top_yaw, gt_best, gt_top, gt_bin = part
+  summary, curve = metrics(top_ov, top_idx, gt_top, gt_best, gt_overlap)
+  t = summary['f1_max_threshold']
+  tp_rows = true_positives_at(top_ov, top_idx, gt_top, t, gt_overlap) if np.isfinite(t) else np.zeros(0, np.int64)
+  d_yaw = yaw_errors(eng, bank, tp_rows, top_idx[tp_rows, 0], gt_bin[tp_rows, 0], eng.Wf)
+  summary.update(
+      scans=n, pairs=int(c.sum()), exclude_frames=exclude_frames, exclude_distance=exclude_distance,
+      gt_overlap=gt_overlap, world_size=world, true_positives_at_f1_max=int(tp_rows.size),
+      yaw_error_mean=float(d_yaw.mean()) if d_yaw.size else float('nan'),
+      yaw_error_max=float(d_yaw.max()) if d_yaw.size else float('nan'),
+      yaw_error_rms=float(np.sqrt(np.mean(d_yaw * d_yaw))) if d_yaw.size else float('nan'))
+  results = {'c': c, 'top_overlap': top_ov, 'top_index': top_idx, 'top_yaw': top_yaw, 'gt_top_overlap': gt_top,
+             'gt_top_yaw_bin': gt_bin, 'gt_best': gt_best, 'positive': gt_best > gt_overlap,
+             'true_positive_rows': tp_rows, 'yaw_error': d_yaw}
+  results.update({'curve_' + key: v for key, v in curve.items()})
+  if out_dir is not None:
+    os.makedirs(out_dir, exist_ok=True)
+    save_npz(os.path.join(out_dir, 'lcd_results.npz'), results)
+    with open(os.path.join(out_dir, 'lcd_summary.json'), 'w') as f:
+      json.dump(summary, f, indent=1, sort_keys=True)
+  return summary, results
+
+
+# ---- the command line ---------------------------------------------------------------------------------------
+def parse_args(argv):
+  p = argparse.ArgumentParser(prog='python -m overlapnet_b200.lcd_eval',
+                              description='Loop-closure precision-recall of a model over a whole sequence.')
+  p.add_argument('config', nargs='?', default='config/demo.yml', help='YAML file with a Demo3 section')
+  p.add_argument('--top-k', type=int, default=5, help='records kept per query, 1..%d (default 5)' % TOPK_MAX)
+  p.add_argument('--exclude-frames', type=int, default=100, help='the most recent frames skipped (default 100)')
+  p.add_argument('--exclude-distance', type=float, default=50.0, help='metres of travel skipped (default 50)')
+  p.add_argument('--gt-overlap', type=float, default=0.3, help='ground-truth overlap of a true loop (default 0.3)')
+  p.add_argument('--precision', default='f16_tc', choices=('f16_tc', 'fp32'))
+  args = p.parse_args(argv)
+  if not 1 <= args.top_k <= TOPK_MAX:
+    p.error('--top-k must be in [1, %d], got %d' % (TOPK_MAX, args.top_k))
+  return args
+
+
+def network_config(config):
+  """The network config of a demo.yml dict's Demo3 section, refused when it uses class probabilities."""
+  from .config import load_config
+  net = load_config(config['Demo3']['network_config'])
+  if net.get('use_class_probabilities', False):
+    raise Exception('lcd_eval: the network config uses class probabilities, which would need a .label file per '
+                    'scan; only geometric configs are evaluated from raw scans')
+  return net
+
+
+def main(argv=None):
+  from . import gt
+  from .config import load_config
+  from .gt_files import kitti_poses_in_lidar
+  from .infer import Infer
+  from .preprocess import _read_scan, load_files
+  logging.basicConfig(level=logging.INFO, format='%(message)s')
+  args = parse_args(sys.argv[1:] if argv is None else argv)
+  config = load_config(args.config)
+  net = network_config(config)
+  d = config['Demo3']
+  world = int(os.environ.get('WORLD_SIZE', '1'))
+  if world > 1:
+    local_rank = int(os.environ.get('LOCAL_RANK', '0'))
+    torch.cuda.set_device(local_rank)
+    torch.distributed.init_process_group('nccl', device_id=torch.device('cuda', local_rank))
+  scan_paths = load_files(d['scan_folder'])
+  poses = kitti_poses_in_lidar(gt.load_poses(d['poses_file']), gt.load_calib(d['calib_file']))
+  clouds = [(lambda p=p: _read_scan(p)) for p in scan_paths]
+  for key, default in (('use_depth', True), ('use_normals', True), ('use_class_probabilities', False),
+                       ('use_class_probabilities_pca', False), ('use_intensity', False)):
+    net.setdefault(key, default)
+  net.setdefault('infer_seqs', d.get('infer_seqs', ''))
+  net.setdefault('data_root_folder', '')
+  infer = Infer(net, precision=args.precision)
+  out_dir = os.path.join(net.get('experiments_path', '/tmp'), net.get('testname', 'experiment_test'))
+  res = evaluate_clouds(infer, clouds, poses, args.top_k, args.exclude_frames, args.exclude_distance,
+                        args.gt_overlap, out_dir)
+  if res is not None:
+    s = res[0]
+    logger.info('Loop closure over %d scans, %d queries, %d positive (ground-truth overlap > %g), %d pairs scored',
+                s['scans'], s['queries'], s['positives'], s['gt_overlap'], s['pairs'])
+    logger.info('  average precision:              %f', s['average_precision'])
+    logger.info('  F1max:                          %f at overlap >= %f', s['f1_max'], s['f1_max_threshold'])
+    logger.info('  precision / recall at > %g:    %f / %f', s['operating_point'], s['precision_at_operating_point'],
+                s['recall_at_operating_point'])
+    logger.info('  recall@1 / recall@%d:            %f / %f', s['k'], s['recall_at_1'], s['recall_at_k'])
+    logger.info('  yaw error of the %d true positives at F1max: mean %f, max %f, RMS %f bins',
+                s['true_positives_at_f1_max'], s['yaw_error_mean'], s['yaw_error_max'], s['yaw_error_rms'])
+    logger.info('  written to %s', out_dir)
+  if world > 1:
+    torch.distributed.barrier()
+    torch.distributed.destroy_process_group()
+  return res
+
+
+if __name__ == '__main__':
+  main()
