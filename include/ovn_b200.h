@@ -244,6 +244,63 @@ int ovn_heads_prefix_topk(ovn_handle* h, const float* d_bank, int64_t bank_size,
                           const int32_t* h_n_cand /* [row_hi - row_lo], host */, int32_t k, float* d_top_overlap,
                           int32_t* d_top_index, int32_t* d_top_yaw, void* stream);
 
+/* ---- overlap-based Monte Carlo localization (overlapnet_b200/mcl.py, DESIGN.md sections 4 and 7) ---------------
+ * A particle filter over planar poses (x, y, theta), float64, with float64 log-weights, on the device.  The map is K
+ * keyframes and a raster [rows][cols] whose cell (r, c) covers x0 + c cell <= x < x0 + (c + 1) cell, likewise y from
+ * y0, and holds the index of the keyframe nearest to its centre, or -1.  Random numbers: Philox4x32-10 keyed by the
+ * seed, counter (particle, step, stream, block); stream 0 motion, 1 initialisation, 2 resampling.  Every reduction
+ * runs in an order fixed by N: the same seed, map, observations and N give bit-identical particles and estimates.
+ *   ovn_mcl_set_map: h_keyframes [K][3] (x, y, theta), h_raster [rows][cols] with entries in [-1, K); cell > 0 and
+ *                    finite.  Synchronous; drops the particle set.
+ *   ovn_mcl_init:    n particles, 1 <= n <= 2^24.  OVN_MCL_INIT_GLOBAL: keyframe floor(u K), uniform in the disk of
+ *                    init_radius around it, theta uniform; h_pose / h_sigma ignored.  OVN_MCL_INIT_POSE: Gaussian
+ *                    around h_pose [3] with standard deviations h_sigma [3] (each >= 0).  Log-weights -log n.
+ *   ovn_mcl_predict: moves every particle by the odometry h_odom [3] (dx, dy, dtheta in the previous query frame) with
+ *                    noise h_sigma [3] (>= 0), looks up its keyframe and writes the touched keyframes, ascending, to
+ *                    d_touched [K]; *h_n_touched = their number.  Synchronous.
+ *   ovn_mcl_update:  the heads' overlap d_overlap [n] and yaw d_yaw [n] (180 - argmax) of LEFT = keyframe d_touched[j],
+ *                    RIGHT = the query; n must be the last predict's count (the pointers may be NULL when it is 0).
+ *                    Adds each particle's log-likelihood, normalises, and resamples systematically when the ESS falls
+ *                    below rho N.  sigma_overlap, sigma_yaw > 0 (radians), rho in [0, 1].  Synchronous: *h_est.
+ *   ovn_mcl_copy_particles: d_out [4][N] float64 x, y, theta, log-weight of the current set, asynchronous.
+ *   ovn_mcl_copy_stage: d_out = a stage of the last step, asynchronous: MOTION [3][N] f64 (x, y, theta after the last
+ *                    predict), LOOKUP [N] i32 (the keyframe of each particle after it, -1 outside), LOGLIK [N] f64,
+ *                    WEIGHTS [N] f64 (the normalised weights), PREFIX [N] f64 (their inclusive prefix sum) and
+ *                    ANCESTORS [N] i32 of the last update; the last two only when it resampled.
+ *   ovn_mcl_philox:  d_out [n][4] = the Philox4x32-10 words of the counters d_ctr [n][4] under the seed (tests).
+ * Invalid arguments, a call before ovn_mcl_set_map / ovn_mcl_init, an update without a predict and a stage the handle
+ * does not hold are OVN_ERR_INVALID_ARG with nothing launched; the handle stays usable. */
+typedef enum ovn_mcl_init_mode {
+  OVN_MCL_INIT_GLOBAL = 0,
+  OVN_MCL_INIT_POSE = 1
+} ovn_mcl_init_mode;
+typedef enum ovn_mcl_stage {
+  OVN_MCL_STAGE_MOTION = 0,
+  OVN_MCL_STAGE_LOOKUP = 1,
+  OVN_MCL_STAGE_LOGLIK = 2,
+  OVN_MCL_STAGE_WEIGHTS = 3,
+  OVN_MCL_STAGE_PREFIX = 4,
+  OVN_MCL_STAGE_ANCESTORS = 5
+} ovn_mcl_stage;
+typedef struct ovn_mcl_estimate {
+  double x, y, theta;             /* weighted means; theta = atan2(sum w sin, sum w cos) */
+  double ess;                     /* 1 / sum w^2 before resampling */
+  int32_t n_touched;              /* keyframes the heads scored */
+  int32_t resampled;              /* 1 when the update resampled */
+  int64_t step;                   /* predicts since ovn_mcl_init */
+} ovn_mcl_estimate;
+int ovn_mcl_set_map(ovn_handle* h, const double* h_keyframes, int32_t n_keyframes, const int32_t* h_raster,
+                    int32_t rows, int32_t cols, double x0, double y0, double cell);
+int ovn_mcl_init(ovn_handle* h, int32_t mode, int32_t n, uint64_t seed, const double* h_pose, const double* h_sigma,
+                 double init_radius, void* stream);
+int ovn_mcl_predict(ovn_handle* h, const double* h_odom, const double* h_sigma, int32_t* d_touched,
+                    int32_t* h_n_touched, void* stream);
+int ovn_mcl_update(ovn_handle* h, const float* d_overlap, const int32_t* d_yaw, int32_t n, double sigma_overlap,
+                   double sigma_yaw, double rho, ovn_mcl_estimate* h_est, void* stream);
+int ovn_mcl_copy_particles(ovn_handle* h, double* d_out, void* stream);
+int ovn_mcl_copy_stage(ovn_handle* h, int32_t stage, void* d_out, void* stream);
+int ovn_mcl_philox(ovn_handle* h, uint64_t seed, const uint32_t* d_ctr, int32_t n, uint32_t* d_out, void* stream);
+
 /* ---- resident bank (Infer keeps self.feature_volumes across calls, infer.py:113,184-193) ---------
  * The tensor-core heads consume fp16 / hi-lo split copies of the LEFT volumes.  Without this call
  * they are rebuilt from d_bank on every heads call; ovn_bank_prepare builds them once for rows

@@ -31,8 +31,13 @@ SYMBOLS = [
     'ovn_shard_create', 'ovn_shard_open', 'ovn_shard_close', 'ovn_gather_rows',
     'ovn_set_train_stop', 'ovn_train_stage_size', 'ovn_copy_train_stage',
     'ovn_rows_topk', 'ovn_heads_prefix_topk',
+    'ovn_mcl_set_map', 'ovn_mcl_init', 'ovn_mcl_predict', 'ovn_mcl_update', 'ovn_mcl_copy_particles',
+    'ovn_mcl_copy_stage', 'ovn_mcl_philox',
 ]
 TOPK_MAX = 32     # ovn_rows_topk / ovn_heads_prefix_topk: k in [1, TOPK_MAX]
+MCL_INIT_MODES = {'global': 0, 'pose': 1}     # ovn_mcl_init_mode
+MCL_STAGES = {'motion': 0, 'lookup': 1, 'loglik': 2, 'weights': 3, 'prefix': 4, 'ancestors': 5}     # ovn_mcl_stage
+MCL_MAX_PARTICLES = 1 << 24
 IPC_HANDLE_BYTES = 64     # ovn_shard_create / ovn_shard_open
 HEADS_STAGES = {'o1': 0, 'x3': 1, 'dense': 2, 'centres': 3}     # ovn_heads_stage
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
@@ -58,6 +63,12 @@ class OvnConfig(C.Structure):
   ]
 
 
+class McEstimate(C.Structure):
+  """ovn_mcl_estimate"""
+  _fields_ = [('x', C.c_double), ('y', C.c_double), ('theta', C.c_double), ('ess', C.c_double),
+              ('n_touched', C.c_int32), ('resampled', C.c_int32), ('step', C.c_int64)]
+
+
 class OvnError(Exception):
   """Raised for any non-zero ovn_status (plain Exception subclass, like the reference's errors)."""
 
@@ -75,6 +86,7 @@ def lib():
                    '(there is no CPU fallback for the CUDA path)')
   L = C.CDLL(LIB_PATH)
   vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
+  u64, f64 = C.c_uint64, C.c_double
   L.ovn_default_config.argtypes = [C.POINTER(OvnConfig)]
   L.ovn_default_config.restype = None
   L.ovn_create.argtypes = [C.POINTER(OvnConfig), C.POINTER(vp)]
@@ -109,6 +121,13 @@ def lib():
   L.ovn_heads_rows_vs_bank.argtypes = [vp, vp, i64, i64, i64, vp, vp, vp]
   L.ovn_rows_topk.argtypes = [vp, vp, vp, i64, i64, vp, i32, vp, vp, vp, vp]
   L.ovn_heads_prefix_topk.argtypes = [vp, vp, i64, i64, i64, vp, i32, vp, vp, vp, vp]
+  L.ovn_mcl_set_map.argtypes = [vp, vp, i32, vp, i32, i32, f64, f64, f64]
+  L.ovn_mcl_init.argtypes = [vp, i32, i32, u64, vp, vp, f64, vp]
+  L.ovn_mcl_predict.argtypes = [vp, vp, vp, vp, C.POINTER(i32), vp]
+  L.ovn_mcl_update.argtypes = [vp, vp, vp, i32, f64, f64, f64, C.POINTER(McEstimate), vp]
+  L.ovn_mcl_copy_particles.argtypes = [vp, vp, vp]
+  L.ovn_mcl_copy_stage.argtypes = [vp, i32, vp, vp]
+  L.ovn_mcl_philox.argtypes = [vp, u64, vp, i32, vp, vp]
   L.ovn_bank_release.argtypes = [vp, vp]
   L.ovn_check.argtypes = [vp, vp]
   L.ovn_set_feature_center.argtypes = [vp, vp]

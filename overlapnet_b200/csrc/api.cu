@@ -772,6 +772,125 @@ int ovn_heads_prefix_topk(ovn_handle* h, const float* d_bank, int64_t bank_size,
   return reduce_fill();
 }
 
+// ---- Monte Carlo localization -------------------------------------------------------------------------------
+static bool finite_nonneg(const double* v, int n) {
+  for (int i = 0; i < n; ++i)
+    if (!(v[i] >= 0.0 && v[i] < INFINITY)) return false;
+  return true;
+}
+
+int ovn_mcl_set_map(ovn_handle* h, const double* h_keyframes, int32_t n_keyframes, const int32_t* h_raster,
+                    int32_t rows, int32_t cols, double x0, double y0, double cell) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, h_keyframes && h_raster, "NULL pointer");
+  REQUIRE(h, n_keyframes >= 1 && n_keyframes <= kMcMaxKeyframes, "n_keyframes must be in [1, 2^24]");
+  REQUIRE(h, rows >= 1 && cols >= 1 && (int64_t)rows * cols <= kMcMaxCells, "rows, cols >= 1 and rows cols <= 2^28");
+  REQUIRE(h, cell > 0.0 && cell < INFINITY && std::isfinite(x0) && std::isfinite(y0), "cell > 0 and finite origin");
+  for (int64_t i = 0; i < (int64_t)n_keyframes * 3; ++i)
+    if (!std::isfinite(h_keyframes[i])) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_mcl_set_map: keyframe value %lld is not finite", (long long)i);
+  for (int64_t i = 0; i < (int64_t)rows * cols; ++i)
+    if (h_raster[i] < -1 || h_raster[i] >= n_keyframes)
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_mcl_set_map: raster cell %lld = %d is outside [-1, %d)", (long long)i,
+                  h_raster[i], n_keyframes);
+  McState& m = h->mcl;
+  m.n = 0;                                   // the set referred to the old map
+  m.pending = -1;
+  m.stages = 0;
+  OVN_CUDA(h, cudaDeviceSynchronize());      // no queued kernel still reads the old map
+  int rc;
+  m.map = McMap{};
+  if ((rc = m.kf.ensure(h, (size_t)n_keyframes * 3 * sizeof(double))) != OVN_OK ||
+      (rc = m.raster.ensure(h, (size_t)rows * cols * sizeof(int32_t))) != OVN_OK ||
+      (rc = m.flags.ensure(h, (size_t)n_keyframes * sizeof(int32_t))) != OVN_OK ||
+      (rc = m.slot.ensure(h, (size_t)n_keyframes * sizeof(int32_t))) != OVN_OK)
+    return rc;
+  OVN_CUDA(h, cudaMemcpy(m.kf, h_keyframes, (size_t)n_keyframes * 3 * sizeof(double), cudaMemcpyHostToDevice));
+  OVN_CUDA(h, cudaMemcpy(m.raster, h_raster, (size_t)rows * cols * sizeof(int32_t), cudaMemcpyHostToDevice));
+  m.map.K = n_keyframes;
+  m.map.rows = rows;
+  m.map.cols = cols;
+  m.map.x0 = x0;
+  m.map.y0 = y0;
+  m.map.cell = cell;
+  return OVN_OK;
+}
+
+int ovn_mcl_init(ovn_handle* h, int32_t mode, int32_t n, uint64_t seed, const double* h_pose, const double* h_sigma,
+                 double init_radius, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, h->mcl.map.K > 0, "no map: call ovn_mcl_set_map first");
+  REQUIRE(h, n >= 1 && n <= kMcMaxParticles, "n must be in [1, 2^24]");
+  if (mode == OVN_MCL_INIT_GLOBAL) {
+    REQUIRE(h, init_radius >= 0.0 && init_radius < INFINITY, "init_radius must be finite and >= 0");
+  } else if (mode == OVN_MCL_INIT_POSE) {
+    REQUIRE(h, h_pose && h_sigma, "NULL pointer");
+    REQUIRE(h, std::isfinite(h_pose[0]) && std::isfinite(h_pose[1]) && std::isfinite(h_pose[2]), "pose not finite");
+    REQUIRE(h, finite_nonneg(h_sigma, 3), "sigma must be finite and >= 0");
+  } else {
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_mcl_init: mode %d is not an ovn_mcl_init_mode", mode);
+  }
+  return mcl_init(h, mode, n, seed, mode == OVN_MCL_INIT_POSE ? h_pose : nullptr,
+                  mode == OVN_MCL_INIT_POSE ? h_sigma : nullptr, init_radius, (cudaStream_t)stream);
+}
+
+int ovn_mcl_predict(ovn_handle* h, const double* h_odom, const double* h_sigma, int32_t* d_touched,
+                    int32_t* h_n_touched, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, h->mcl.n > 0, "no particles: call ovn_mcl_init first");
+  REQUIRE(h, h_odom && h_sigma && d_touched && h_n_touched, "NULL pointer");
+  REQUIRE(h, std::isfinite(h_odom[0]) && std::isfinite(h_odom[1]) && std::isfinite(h_odom[2]), "odometry not finite");
+  REQUIRE(h, finite_nonneg(h_sigma, 3), "sigma must be finite and >= 0");
+  return mcl_predict(h, h_odom, h_sigma, d_touched, h_n_touched, (cudaStream_t)stream);
+}
+
+int ovn_mcl_update(ovn_handle* h, const float* d_overlap, const int32_t* d_yaw, int32_t n, double sigma_overlap,
+                   double sigma_yaw, double rho, ovn_mcl_estimate* h_est, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, h->mcl.n > 0, "no particles: call ovn_mcl_init first");
+  REQUIRE(h, h->mcl.pending >= 0, "no predict awaits an update");
+  if (n != h->mcl.pending)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_mcl_update: n = %d, but the last predict touched %d keyframes", n,
+                h->mcl.pending);
+  REQUIRE(h, h_est && (n == 0 || (d_overlap && d_yaw)), "NULL pointer");
+  REQUIRE(h, sigma_overlap > 0.0 && sigma_overlap < INFINITY && sigma_yaw > 0.0 && sigma_yaw < INFINITY,
+          "sigma_overlap and sigma_yaw must be finite and > 0");
+  REQUIRE(h, rho >= 0.0 && rho <= 1.0, "rho must be in [0, 1]");
+  return mcl_update(h, d_overlap, d_yaw, sigma_overlap, sigma_yaw, rho, h_est, (cudaStream_t)stream);
+}
+
+int ovn_mcl_copy_particles(ovn_handle* h, double* d_out, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, h->mcl.n > 0, "no particles: call ovn_mcl_init first");
+  REQUIRE(h, d_out, "NULL pointer");
+  return mcl_copy_particles(h, d_out, (cudaStream_t)stream);
+}
+
+int ovn_mcl_copy_stage(ovn_handle* h, int32_t stage, void* d_out, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, stage >= OVN_MCL_STAGE_MOTION && stage <= OVN_MCL_STAGE_ANCESTORS, "stage is not an ovn_mcl_stage");
+  REQUIRE(h, d_out, "NULL pointer");
+  const int need = stage <= OVN_MCL_STAGE_LOOKUP ? kMcHeldPredict
+                   : stage <= OVN_MCL_STAGE_WEIGHTS ? kMcHeldUpdate : kMcHeldResample;
+  if (!(h->mcl.stages & need))
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_mcl_copy_stage: stage %d is not held (no %s since the last init)", stage,
+                need == kMcHeldPredict ? "predict" : need == kMcHeldUpdate ? "update" : "update that resampled");
+  return mcl_copy_stage(h, stage, d_out, (cudaStream_t)stream);
+}
+
+int ovn_mcl_philox(ovn_handle* h, uint64_t seed, const uint32_t* d_ctr, int32_t n, uint32_t* d_out, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, n >= 0, "n must be >= 0");
+  REQUIRE(h, n == 0 || (d_ctr && d_out), "NULL pointer");
+  return mcl_philox(h, seed, d_ctr, n, d_out, (cudaStream_t)stream);
+}
+
 // ---- training precision ---------------------------------------------------------------------------
 int ovn_set_train_precision(ovn_handle* h, int32_t train_precision) {
   if (!h) return OVN_ERR_INVALID_ARG;

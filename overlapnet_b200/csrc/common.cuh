@@ -173,6 +173,45 @@ inline bool train_stop_here(TrainState& t, int stage, int layer, const float* li
   }
   return t.stopped;
 }
+
+// Monte Carlo localization (ovn_mcl_*, mcl.cu).  The map: K keyframes' planar poses and the raster of the nearest
+// keyframe per cell; the particles: two structure-of-arrays float64 buffers of 4 cap values (x, y, theta, log-weight).
+struct McMap {
+  int K = 0, rows = 0, cols = 0;
+  double x0 = 0.0, y0 = 0.0, cell = 0.0;
+};
+struct McParticles {
+  double *x, *y, *th, *lw;
+};
+// the device scalars of one update: k_mcl_final writes them, the host reads [0, kScTouched)
+enum McScalar { kScMax = 0, kScExpSum, kScEss, kScX, kScY, kScTheta, kScResample, kScU0, kScTouched, kScCount };
+constexpr int kMcPartialStride = 8;      // doubles per block partial
+constexpr int kMcMaxParticles = 1 << 24;
+constexpr int kMcMaxKeyframes = 1 << 24;
+constexpr int64_t kMcMaxCells = int64_t(1) << 28;
+enum McHeld { kMcHeldPredict = 1, kMcHeldUpdate = 2, kMcHeldResample = 4 };   // the stages McState holds
+struct McState {
+  McMap map;
+  Buffer<double> kf;             // [K][3] x, y, theta of the keyframes
+  Buffer<int32_t> raster;        // [rows][cols] keyframe index or -1
+  Buffer<int32_t> flags;         // [K] touched by the last predict
+  Buffer<int32_t> slot;          // [K] position in the last predict's touched list, or -1
+  Buffer<double> part[2];        // particle buffers, [4][cap]
+  Buffer<int32_t> kidx;          // [cap] the last lookup
+  Buffer<double> ll, w, cdf;     // [cap] log-likelihood, normalised weights, inclusive prefix sum of the weights
+  Buffer<int32_t> anc;           // [cap] the last resampling's ancestors
+  Buffer<double> tiles;          // prefix sum: one total per tile
+  Buffer<double> partial;        // [kMclRedBlocks][kMcPartialStride] per-block partials of a reduction
+  Buffer<double> scal;           // [kScCount] McScalar
+  PinnedBuffer<double> host;     // [kScCount] their host copy
+  int cap = 0;                   // particles the buffers hold
+  int n = 0;                     // particles of the set, 0 before ovn_mcl_init
+  int cur = 0, pred_buf = 0;     // the buffer of the current set; the one the last predict moved
+  uint64_t seed = 0;
+  int64_t step = 0;              // predicts since ovn_mcl_init
+  int pending = -1;              // n_touched of a predict that awaits its update, else -1
+  int stages = 0;                // McHeld bits
+};
 }  // namespace ovn
 
 struct ovn_handle {
@@ -232,6 +271,7 @@ struct ovn_handle {
   // mapped.  Declared in this order so that the mappings are closed before the own shards are freed.
   std::vector<ovn::Buffer<uint8_t>> own_shards;
   std::vector<ovn::IpcMapping> open_shards;
+  ovn::McState mcl;                          // ovn_mcl_*: map and particles, allocated by ovn_mcl_set_map / ovn_mcl_init
   cudaStream_t own_stream = nullptr;
   // per-kernel profiling (ovn_profile_enable / ovn_profile_read)
   bool profiling = false;
@@ -430,6 +470,17 @@ constexpr int64_t kTopkRowsPerLaunch = 65536;
 constexpr int64_t kTopkScratchPairs = int64_t(1) << 21;   // ovn_heads_prefix_topk's scratch: 16 MiB
 int rows_topk(ovn_handle* h, const float* d_ov, const int32_t* d_yaw, const int64_t* h_off, const int32_t* h_len,
               int64_t rows, int k, float* d_top_ov, int32_t* d_top_idx, int32_t* d_top_yaw, cudaStream_t s);
+
+// Monte Carlo localization (mcl.cu); the caller has checked every argument and the handle's state
+int mcl_init(ovn_handle* h, int mode, int n, uint64_t seed, const double* pose, const double* sigma, double radius,
+             cudaStream_t s);
+int mcl_predict(ovn_handle* h, const double* odom, const double* sigma, int32_t* d_touched, int32_t* n_touched,
+                cudaStream_t s);
+int mcl_update(ovn_handle* h, const float* d_ov, const int32_t* d_yaw, double s_o, double s_psi, double rho,
+               ovn_mcl_estimate* est, cudaStream_t s);
+int mcl_copy_particles(ovn_handle* h, double* d_out, cudaStream_t s);
+int mcl_copy_stage(ovn_handle* h, int stage, void* d_out, cudaStream_t s);
+int mcl_philox(ovn_handle* h, uint64_t seed, const uint32_t* d_ctr, int n, uint32_t* d_out, cudaStream_t s);
 
 int corr_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* left,
                       const int32_t* right, int np, int32_t* d_yaw, float* d_corr, cudaStream_t s);

@@ -477,6 +477,77 @@ class Engine:
                                                self._stream()), 'ovn_heads_prefix_topk')
     return out
 
+  # ---- Monte Carlo localization (ovn_mcl_*, overlapnet_b200.mcl) -----------------------------------------------
+  def mcl_set_map(self, keyframes, raster, x0, y0, cell):
+    """ovn_mcl_set_map: ``keyframes`` (K, 3) x, y, theta; ``raster`` (rows, cols) keyframe index or -1.  Drops the
+    particle set."""
+    kf = np.ascontiguousarray(keyframes, np.float64).reshape(-1, 3)
+    ras = np.ascontiguousarray(raster, np.int32)
+    assert ras.ndim == 2
+    check(self._h, lib().ovn_mcl_set_map(self._h, kf.ctypes.data_as(C.c_void_p), kf.shape[0],
+                                         ras.ctypes.data_as(C.c_void_p), ras.shape[0], ras.shape[1], float(x0),
+                                         float(y0), float(cell)), 'ovn_mcl_set_map')
+    self._mcl_k = kf.shape[0]
+    self._mcl_n = 0
+
+  def mcl_init(self, mode, n, seed, pose=None, sigma=None, init_radius=0.0):
+    """ovn_mcl_init: ``mode`` 'global' (uniform in init_radius around a random keyframe, theta uniform) or 'pose'
+    (Gaussian around ``pose`` (x, y, theta) with standard deviations ``sigma``)."""
+    pose = np.ascontiguousarray(pose if pose is not None else np.zeros(3), np.float64).reshape(3)
+    sigma = np.ascontiguousarray(sigma if sigma is not None else np.zeros(3), np.float64).reshape(3)
+    check(self._h, lib().ovn_mcl_init(self._h, _cabi.MCL_INIT_MODES[mode], int(n), int(seed) & (2 ** 64 - 1),
+                                      pose.ctypes.data_as(C.c_void_p), sigma.ctypes.data_as(C.c_void_p),
+                                      float(init_radius), self._stream()), 'ovn_mcl_init')
+    self._mcl_n = int(n)
+
+  def mcl_predict(self, odom, sigma):
+    """ovn_mcl_predict: (touched int32 cuda [K], n_touched); the first n_touched entries are the touched keyframes,
+    ascending."""
+    odom = np.ascontiguousarray(odom, np.float64).reshape(3)
+    sigma = np.ascontiguousarray(sigma, np.float64).reshape(3)
+    touched = torch.empty((getattr(self, '_mcl_k', 0),), dtype=torch.int32, device=self.device)
+    n = C.c_int32(0)
+    check(self._h, lib().ovn_mcl_predict(self._h, odom.ctypes.data_as(C.c_void_p), sigma.ctypes.data_as(C.c_void_p),
+                                         _ptr(touched), C.byref(n), self._stream()), 'ovn_mcl_predict')
+    return touched, int(n.value)
+
+  def mcl_update(self, overlap, yaw, n, sigma_overlap, sigma_yaw, rho=0.5):
+    """ovn_mcl_update with the heads' overlap f32 / yaw i32 cuda tensors [n] of the last predict's touched keyframes
+    (None when n = 0).  Returns the estimate: dict of x, y, theta, ess, n_touched, resampled, step."""
+    for t, dtype in ((overlap, torch.float32), (yaw, torch.int32)):   # the library refuses NULL with n > 0
+      if t is not None:
+        assert t.dtype == dtype and t.is_contiguous() and t.numel() >= n
+    est = _cabi.McEstimate()
+    check(self._h, lib().ovn_mcl_update(self._h, _ptr(overlap), _ptr(yaw), int(n), float(sigma_overlap),
+                                        float(sigma_yaw), float(rho), C.byref(est), self._stream()), 'ovn_mcl_update')
+    return {'x': est.x, 'y': est.y, 'theta': est.theta, 'ess': est.ess, 'n_touched': int(est.n_touched),
+            'resampled': bool(est.resampled), 'step': int(est.step)}
+
+  def mcl_particles(self):
+    """ovn_mcl_copy_particles: [4, N] float64 cuda tensor x, y, theta, log-weight."""
+    out = torch.empty((4, self._mcl_n), dtype=torch.float64, device=self.device)
+    check(self._h, lib().ovn_mcl_copy_particles(self._h, _ptr(out), self._stream()), 'ovn_mcl_copy_particles')
+    return out
+
+  def mcl_stage(self, stage):
+    """ovn_mcl_copy_stage: 'motion' [3, N] f64, 'lookup' [N] i32, 'loglik' / 'weights' / 'prefix' [N] f64,
+    'ancestors' [N] i32."""
+    n = self._mcl_n
+    shape, dtype = {'motion': ((3, n), torch.float64), 'lookup': ((n,), torch.int32),
+                    'ancestors': ((n,), torch.int32)}.get(stage, ((n,), torch.float64))
+    out = torch.empty(shape, dtype=dtype, device=self.device)
+    check(self._h, lib().ovn_mcl_copy_stage(self._h, _cabi.MCL_STAGES[stage], _ptr(out), self._stream()),
+          'ovn_mcl_copy_stage')
+    return out
+
+  def mcl_philox(self, seed, counters):
+    """ovn_mcl_philox: the Philox4x32-10 words [n, 4] (int32 cuda, the uint32 bits) of ``counters`` [n, 4]."""
+    ctr = torch.as_tensor(np.ascontiguousarray(counters, np.uint32).view(np.int32)).to(self.device).contiguous()
+    out = torch.empty_like(ctr)
+    check(self._h, lib().ovn_mcl_philox(self._h, int(seed) & (2 ** 64 - 1), _ptr(ctr), int(ctr.shape[0]), _ptr(out),
+                                        self._stream()), 'ovn_mcl_philox')
+    return out
+
   def bank_prepare(self, bank, first=0, count=None):
     """Keep the tensor-core operand copies of bank rows [first, first+count) resident: later heads
     calls on this same tensor skip the per-call conversion (ovn_bank_prepare)."""
