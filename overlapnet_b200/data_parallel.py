@@ -7,6 +7,8 @@ rank applies g = sum_r (n_r / n) g_r (``Engine.adagrad_step_sum``).  The losses 
 so that sum is the gradient of the whole batch up to the order of the float32 sums, and every rank ends a step
 with the same weights and accumulators bit for bit.
 """
+import collections
+
 import numpy as np
 import torch
 import torch.distributed as dist
@@ -35,6 +37,22 @@ def chunk_plan(n, n_chunks, world, rank):
   bounds, weights = shares(n, n_chunks)
   c0, c1 = shard_range(n_chunks, rank, world)
   return bounds, weights, (c0, c1), (bounds[c0][0], bounds[c1 - 1][1])
+
+
+StepPlan = collections.namedtuple('StepPlan', 'lo hi offsets weights counts')
+
+
+def step_plan(n, world, rank, gradient_chunks=None):
+  """What ``rank`` of ``world`` trains in a step on a batch of n pairs: its pairs [lo, hi) of the batch; with
+  gradient_chunks K the offsets of its chunks within them, relative to lo (None without chunks); the weights of the
+  parts the Adagrad step sums, the chunks' n_k / n or the ranks' n_r / n; and how many of those parts each rank
+  computes, in rank order (its chunk count, or 1)."""
+  if gradient_chunks is None:
+    bounds, weights = shares(n, world)
+    return StepPlan(bounds[rank][0], bounds[rank][1], None, weights, [1] * world)
+  bounds, weights, (c0, c1), (lo, hi) = chunk_plan(n, gradient_chunks, world, rank)
+  offsets = [bounds[c][0] - lo for c in range(c0, c1)] + [hi - lo]
+  return StepPlan(lo, hi, offsets, weights, [d1 - d0 for d0, d1 in shares(gradient_chunks, world)[0]])
 
 
 def chunk_rows(n_chunks, world):

@@ -36,13 +36,11 @@ def image_bytes(eng):
 
 
 def share_pairs(n_pairs, world, gradient_chunks=None):
-  """The largest share of an n_pairs batch that one of ``world`` data-parallel ranks trains; with gradient_chunks K
-  the largest sum of the chunks of one rank's chunk range (data_parallel.chunk_plan).  A full batch has the
-  largest chunks: a shorter one only makes some of them smaller."""
-  if gradient_chunks is None:
-    bounds, _ = data_parallel.shares(n_pairs, world)
-    return max(hi - lo for lo, hi in bounds)
-  return max(b - a for a, b in (data_parallel.chunk_plan(n_pairs, gradient_chunks, world, r)[3] for r in range(world)))
+  """The most pairs of an n_pairs batch that one of ``world`` data-parallel ranks trains in a step
+  (data_parallel.step_plan), with or without gradient_chunks K.  A full batch has the largest shares: a shorter one
+  only makes some of them smaller."""
+  plans = (data_parallel.step_plan(n_pairs, world, r, gradient_chunks) for r in range(world))
+  return max(p.hi - p.lo for p in plans)
 
 
 def parts_bytes(eng, whole_network, world, gradient_chunks=None):
@@ -119,6 +117,41 @@ def plan_rows(*row_lists):
   return uniq[order], out
 
 
+def bank_rows(keys):
+  """{key: row} of the distinct (dir, scan) keys: by directory, then by scan name."""
+  rows = {}
+  for d in sorted({k[0] for k in keys}):
+    for name in sorted(k[1] for k in keys if k[0] == d):
+      rows[(d, name)] = len(rows)
+  return rows
+
+
+def fill_image_bank(infer, rows, bank, chunk=256):
+  """bank[rows[key]] = the packed network input of each key, through Infer's cue loader (one sequence directory
+  at a time, ``chunk`` scans per load).  ``bank``: a device tensor or a host NumPy array [n, H, W, C]."""
+  keys = list(rows)
+  for d in sorted({k[0] for k in keys}):
+    names = sorted(k[1] for k in keys if k[0] == d)
+    infer.seq = d
+    for s in range(0, len(names), chunk):
+      x = infer._prepare_inputs(names[s:s + chunk])
+      r0 = rows[(d, names[s])]
+      if isinstance(bank, np.ndarray):
+        bank[r0:r0 + len(x)] = x
+      else:
+        bank[r0:r0 + len(x)] = torch.from_numpy(x).to(bank.device)
+
+
+def load_image_bank(infer, keys, chunk=256):
+  """Packed network inputs of the distinct (dir, scan) keys, through Infer's cue loader (one sequence
+  directory at a time), in one device tensor [n, H, W, C].  Returns it and {key: row}."""
+  eng = infer._engine
+  rows = bank_rows(keys)
+  bank = torch.empty((len(rows), eng.H, eng.W, eng.C), dtype=torch.float32, device=eng.device)
+  fill_image_bank(infer, rows, bank, chunk)
+  return bank, rows
+
+
 class HostBank:
   """The images [n, H, W, C] float32 in one page-locked host block, pinned through the handle
   (Engine.host_register), which releases it on close() or when the handle closes."""
@@ -163,7 +196,6 @@ class ShardedImageBank:
   peer's, every rank closes what it made and raises ShardOpenError with the reasons.  So is ``close``."""
 
   def __init__(self, infer, rows, dp):
-    from .training_leg import fill_image_bank
     self.eng = eng = infer._engine
     self.dp = dp
     world, rank = (1, 0) if dp is None else (dp.world, dp.rank)
@@ -326,7 +358,6 @@ def open_bank(infer, keys, image_bank, b_share, whole_network, gathered, feature
   rank, choose_rank_placement), 'device', 'host' or 'sharded' forces it.  Returns (placement, the device tensor,
   HostBank or ShardedImageBank, {key: row}).  ``what`` names the bank in the log.  A chosen sharded bank that some
   rank cannot set up falls back to the host bank on every rank; a forced one raises."""
-  from .training_leg import bank_rows, fill_image_bank, load_image_bank
   eng = infer._engine
   if image_bank not in (None,) + PLACEMENTS:
     raise ValueError('image_bank %r: use None, %s' % (image_bank, ' or '.join(repr(p) for p in PLACEMENTS)))

@@ -175,15 +175,11 @@ def orientation_rms(overlap, argmax, gt_orientation, width):
 
 def _encode_bank(infer, keys):
   """Feature volumes of the distinct (dir, scan) keys with the frozen leg, through Infer's cue loader
-  (one sequence directory at a time).  Returns the bank [n, Wf, 128] and {key: row}."""
-  rows, parts, n = {}, [], 0
-  for d in sorted({k[0] for k in keys}):
-    names = sorted(k[1] for k in keys if k[0] == d)
+  (one sequence directory at a time).  Returns the bank [n, Wf, 128] and {key: row} (image_bank.bank_rows)."""
+  rows, parts = _image_bank.bank_rows(keys), []
+  for d in sorted({k[0] for k in rows}):
     infer.seq = d
-    parts.append(infer._create_feature_volumes_device(names))
-    for i, name in enumerate(names):
-      rows[(d, name)] = n + i
-    n += len(names)
+    parts.append(infer._create_feature_volumes_device([name for dd, name in rows if dd == d]))
   return torch.cat(parts).contiguous(), rows
 
 
@@ -533,22 +529,7 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None, made=N
     right_h = np.asarray([steps.image_rows[k] for k in zip(t_d2, t_f2)], np.int64)
     left_h = np.asarray([steps.image_rows[k] for k in zip(t_d1, t_f1)], np.int64) if steps.whole_network else None
     t_rows_h = (left_h, right_h, right_h if yaw_augmentation else None)
-  if gradient_chunks is not None:
-    m = data_parallel.chunk_rows(gradient_chunks, world)
-    size = eng.gradient_size(steps.whole_network)
-    parts = torch.empty((world * m, size), dtype=torch.float32, device=dev)
-    local = parts if dp is None else torch.empty((m, size), dtype=torch.float32, device=dev)
-    ranges = data_parallel.shares(gradient_chunks, world)[0]
-    logger.info('  gradient chunks: %d per batch, summed in chunk order; chunk ranges by rank: %s', gradient_chunks,
-                ', '.join('%d: [%d, %d)' % (r, c0, c1) for r, (c0, c1) in enumerate(ranges)))
-    if dp is not None:
-      logger.info('  data-parallel over %d ranks: each step all-gathers %d x %d gradients per rank', world, m, size)
-  elif dp is not None:
-    whole = steps.whole_network
-    grad = torch.zeros((eng.gradient_size(whole),), dtype=torch.float32, device=dev)
-    parts = torch.empty((dp.world, grad.numel()), dtype=torch.float32, device=dev)
-    logger.info('  data-parallel over %d ranks: each step all-gathers %d gradients per rank', dp.world,
-                grad.numel())
+  local, parts = _step_buffers(dp, steps, eng, gradient_chunks)
   history = {'epoch_loss': [], 'batch_losses': [], 'validation': [], 'weights_filename': weights_filename}
   first_epoch = 0
   if resumed is not None:
@@ -572,34 +553,18 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None, made=N
       shifts_d = torch.from_numpy(shifts).to(dev)
       rot_d = torch.from_numpy(augment.rotation(shifts, W)).to(dev)
       t_or_epoch = augment.move_labels(t_or_d, shifts_d, W, width)
-    if staged:                                                     # this rank's pairs of each step, in order
-      spans = []
-      for b in perm:
-        s0, s1 = b * batch_size, min(n, (b + 1) * batch_size)
-        if gradient_chunks is not None:
-          lo, hi = data_parallel.chunk_plan(s1 - s0, gradient_chunks, world, rank)[3]
-        else:
-          lo, hi = (0, s1 - s0) if dp is None else data_parallel.shares(s1 - s0, dp.world)[0][dp.rank]
-        if hi > lo:
-          spans.append((s0 + lo, s0 + hi))
-      steps.begin_epoch(spans, *t_rows_h)
+      rotate = (t_right_img, shifts_d, rot_d)
+    batches = []                                                   # (first pair, pairs, this rank's plan) per step
     for b in perm:
       s0, s1 = b * batch_size, min(n, (b + 1) * batch_size)
-      if gradient_chunks is not None:
-        loss = _chunked_step(dp, steps, eng, gradient_chunks, parts, local, s0, s1, t_left, t_right, t_ov_d,
-                             t_or_epoch, min_overlap_for_angle, lr,
-                             (t_right_img, shifts_d, rot_d) if yaw_augmentation else None)
-      elif dp is not None:
-        loss = _data_parallel_step(dp, steps, eng, grad, parts, s0, s1, t_left, t_right, t_ov_d, t_or_epoch,
-                                   min_overlap_for_angle, lr,
-                                   (t_right_img, shifts_d, rot_d) if yaw_augmentation else None)
-      else:
-        if yaw_augmentation:
-          rotate = (t_right_img[s0:s1], shifts_d[s0:s1], rot_d[s0:s1])
-        loss = steps.step(t_left[s0:s1], t_right[s0:s1], t_ov_d[s0:s1], t_or_epoch[s0:s1], min_overlap_for_angle,
-                          lr, rotate)
+      batches.append((s0, s1 - s0, data_parallel.step_plan(s1 - s0, world, rank, gradient_chunks)))
+    if staged:                                                     # this rank's pairs of each step, in order
+      steps.begin_epoch([(s0 + p.lo, s0 + p.hi) for s0, _, p in batches if p.hi > p.lo], *t_rows_h)
+    for s0, size, plan in batches:
+      loss = _step(dp, steps, eng, plan, local, parts, s0, t_left, t_right, t_ov_d, t_or_epoch, min_overlap_for_angle,
+                   lr, rotate)
       losses.append(loss)
-      sizes.append(s1 - s0)
+      sizes.append(size)
       logger.info('  epoch %d batch %d: loss %.6f (overlap %.6f, orientation %.6f)', epoch + 1, len(losses),
                   loss[0], loss[1], loss[2])
     epoch_loss = float(np.average([l[0] for l in losses], weights=sizes))
@@ -647,58 +612,62 @@ def _train(config, model, imgpath, out_dir, device, Infer, flow, dp=None, made=N
   return history
 
 
-def _data_parallel_step(dp, steps, eng, grad, parts, s0, s1, t_left, t_right, t_ov, t_or, min_overlap_for_angle,
-                        lr, rotate):
-  """One step of the global batch [s0, s1): this rank's share's gradients, all-gathered, and the same weighted
-  Adagrad step on every rank.  ``rotate`` = (RIGHT image rows, shifts, rotations) of every training pair, or
-  None.  Returns the batch loss sum_r w_r loss_r (float64, rank order)."""
-  bounds, weights = data_parallel.shares(s1 - s0, dp.world)
-  a, b = s0 + bounds[dp.rank][0], s0 + bounds[dp.rank][1]
-  loss = (0.0, 0.0, 0.0)
-  if b > a:
-    share_rotate = None if rotate is None else tuple(t[a:b] for t in rotate)
-    loss = steps.gradients(t_left[a:b], t_right[a:b], t_ov[a:b], t_or[a:b], min_overlap_for_angle, share_rotate)
-    eng.copy_gradients(steps.whole_network, out=grad)
-  else:                                                            # weight 0: skipped by the sum
-    grad.zero_()
-  dp.gather_flat(grad, parts)
-  eng.adagrad_step_sum(parts, weights, lr, steps.whole_network)
-  all_losses = dp.gather_rows(np.asarray([loss], np.float64), [1] * dp.world)
-  return tuple(float(sum(w * l[k] for w, l in zip(weights, all_losses))) for k in range(3))
+def _step_buffers(dp, steps, eng, gradient_chunks):
+  """The gradient parts of the flow ``steps`` for the steps that sum them (_step): (local, parts), this rank's parts
+  [m, n] and every rank's all-gathered [world m, n] (one tensor on one process), with m = ceil(K / world) for
+  gradient_chunks K and m = 1 without; (None, None) on one process without chunks, whose step is the flow's own."""
+  if dp is None and gradient_chunks is None:
+    return None, None
+  world = 1 if dp is None else dp.world
+  m = 1 if gradient_chunks is None else data_parallel.chunk_rows(gradient_chunks, world)
+  size = eng.gradient_size(steps.whole_network)
+  if gradient_chunks is not None:
+    ranges = data_parallel.shares(gradient_chunks, world)[0]
+    logger.info('  gradient chunks: %d per batch, summed in chunk order; chunk ranges by rank: %s', gradient_chunks,
+                ', '.join('%d: [%d, %d)' % (r, c0, c1) for r, (c0, c1) in enumerate(ranges)))
+  if dp is not None:
+    logger.info('  data-parallel over %d ranks: each step all-gathers %s gradients per rank', world,
+                '%d' % size if gradient_chunks is None else '%d x %d' % (m, size))
+  parts = torch.empty((world * m, size), dtype=torch.float32, device=eng.device)
+  return (parts if dp is None else torch.empty((m, size), dtype=torch.float32, device=eng.device)), parts
 
 
-def _chunked_step(dp, steps, eng, n_chunks, parts, local, s0, s1, t_left, t_right, t_ov, t_or, min_overlap_for_angle,
-                  lr, rotate):
-  """One step of the global batch [s0, s1) cut into n_chunks chunks (``gradient_chunks``), on one process or on
-  every rank of ``dp``: this rank's chunk range in one gradient call into ``local`` [ceil(K / world), n]; with
-  several ranks the parts all-gathered into ``parts`` [world ceil(K / world), n] and moved into chunk order; then
-  the Adagrad step of g = sum_k (n_k / n) g_k over parts[:K].  Each g_k is what a call on chunk k alone computes, so
-  the step does not depend on how the chunks are spread over ranks.  Returns the batch loss sum_k (n_k / n) loss_k
-  (float64, chunk order)."""
-  world, rank = (1, 0) if dp is None else (dp.world, dp.rank)
-  bounds, weights, (c0, c1), (a, b) = data_parallel.chunk_plan(s1 - s0, n_chunks, world, rank)
-  a, b = s0 + a, s0 + b
-  mine = local[:c1 - c0]
-  losses = [(0.0, 0.0, 0.0)] * (c1 - c0)
-  if b > a:
-    offsets = [bounds[c][0] - bounds[c0][0] for c in range(c0, c1)] + [b - a]
-    chunk_rotate = None if rotate is None else tuple(t[a:b] for t in rotate)
-    losses = steps.gradients(t_left[a:b], t_right[a:b], t_ov[a:b], t_or[a:b], min_overlap_for_angle, chunk_rotate,
-                             chunks=(offsets, mine))
-  else:                                                            # every chunk empty: weight 0, skipped by the sum
-    mine.zero_()
-  losses = np.asarray(losses, np.float64).reshape(c1 - c0, 3)
+def _step(dp, steps, eng, plan, local, parts, s0, t_left, t_right, t_ov, t_or, min_overlap_for_angle, lr, rotate):
+  """One step of the batch whose first training pair is s0, under this rank's ``plan`` (data_parallel.step_plan):
+  the pairs [s0 + lo, s0 + hi) of ``t_*`` and of ``rotate`` (the RIGHT image rows, shifts and rotations of every
+  training pair, or None).  On one process without chunks that is the flow's own step.  Otherwise this rank's parts
+  -- its share's gradients, or its chunks' in one gradient call -- go to ``local`` (_step_buffers); with several ranks
+  they are all-gathered into ``parts`` and moved into chunk order; then every rank applies the Adagrad step of
+  g = sum_k w_k g_k over the plan's weights.  Each part is what a call on its pairs alone computes, so a chunked step
+  does not depend on how the chunks are spread over ranks.  Returns the flow's loss on one process without chunks,
+  else the batch loss sum_k w_k loss_k (float64, in the parts' order)."""
+  a, b = s0 + plan.lo, s0 + plan.hi
+  pairs = [t[a:b] for t in (t_left, t_right, t_ov, t_or)]
+  rotate = None if rotate is None else tuple(t[a:b] for t in rotate)
+  if local is None:
+    return steps.step(*pairs, min_overlap_for_angle, lr, rotate)
+  k = 1 if plan.offsets is None else len(plan.offsets) - 1        # the parts this rank computes
+  losses = [(0.0, 0.0, 0.0)] * k
+  if b == a:                                                       # no pairs: weight 0, skipped by the sum
+    local[:k].zero_()
+  elif plan.offsets is None:
+    losses = [steps.gradients(*pairs, min_overlap_for_angle, rotate)]
+    eng.copy_gradients(steps.whole_network, out=local[0])
+  else:
+    losses = steps.gradients(*pairs, min_overlap_for_angle, rotate, chunks=(plan.offsets, local[:k]))
+  losses = np.asarray(losses, np.float64).reshape(k, 3)
   if dp is not None:
     m = local.shape[0]
-    dp.gather_flat(local.reshape(-1), parts.view(world, -1))
-    ranges = data_parallel.shares(n_chunks, world)[0]
-    for r, (d0, d1) in enumerate(ranges):          # rank r's rows [r m, r m + d1 - d0) to chunks [d0, d1)
-      for j in range(d1 - d0):                     # d0 <= r m: a row never lands on one still to be read
+    dp.gather_flat(local.reshape(-1), parts.view(dp.world, -1))
+    d0 = 0
+    for r, c in enumerate(plan.counts):            # rank r's rows [r m, r m + c) to parts [d0, d0 + c)
+      for j in range(c):                           # d0 <= r m: a row never lands on one still to be read
         if d0 + j != r * m + j:
           parts[d0 + j].copy_(parts[r * m + j])
-    losses = dp.gather_rows(losses, [d1 - d0 for d0, d1 in ranges])
-  eng.adagrad_step_sum(parts[:n_chunks], weights, lr, steps.whole_network)
-  return tuple(float(sum(w * l[k] for w, l in zip(weights, losses))) for k in range(3))
+      d0 += c
+    losses = dp.gather_rows(losses, plan.counts)
+  eng.adagrad_step_sum(parts[:len(plan.weights)], plan.weights, lr, steps.whole_network)
+  return tuple(float(sum(w * l[i] for w, l in zip(plan.weights, losses))) for i in range(3))
 
 
 def main(argv=None):

@@ -17,13 +17,13 @@ Not supported (an Exception says so): ``rotate_training_data`` -- the reference 
 moving its yaw label (ImagePairOverlapOrientationSequence.py:112,209-212) -- and TensorBoard output.
 ``yaw_augmentation: True`` is the geometric version (overlapnet_b200.training, overlapnet_b200.augment).
 """
-import numpy as np
 import torch
 
 from . import data_parallel
 from . import image_bank as _image_bank
 from . import training
 from .engine import FEAT_C
+from .image_bank import bank_rows  # noqa: F401 -- the row order of this flow's image bank, public here as well
 from .training import logger
 
 
@@ -38,41 +38,6 @@ def check_config(config):
   training.check_unsupported_options(config)
   training.check_yaw_augmentation(config)
   training.check_training_precision(config)
-
-
-def bank_rows(keys):
-  """{key: row} of the distinct (dir, scan) keys: by directory, then by scan name."""
-  rows = {}
-  for d in sorted({k[0] for k in keys}):
-    for name in sorted(k[1] for k in keys if k[0] == d):
-      rows[(d, name)] = len(rows)
-  return rows
-
-
-def fill_image_bank(infer, rows, bank, chunk=256):
-  """bank[rows[key]] = the packed network input of each key, through Infer's cue loader (one sequence directory
-  at a time, ``chunk`` scans per load).  ``bank``: a device tensor or a host NumPy array [n, H, W, C]."""
-  keys = list(rows)
-  for d in sorted({k[0] for k in keys}):
-    names = sorted(k[1] for k in keys if k[0] == d)
-    infer.seq = d
-    for s in range(0, len(names), chunk):
-      x = infer._prepare_inputs(names[s:s + chunk])
-      r0 = rows[(d, names[s])]
-      if isinstance(bank, np.ndarray):
-        bank[r0:r0 + len(x)] = x
-      else:
-        bank[r0:r0 + len(x)] = torch.from_numpy(x).to(bank.device)
-
-
-def load_image_bank(infer, keys, chunk=256):
-  """Packed network inputs of the distinct (dir, scan) keys, through Infer's cue loader (one sequence
-  directory at a time), in one device tensor [n, H, W, C].  Returns it and {key: row}."""
-  eng = infer._engine
-  rows = bank_rows(keys)
-  bank = torch.empty((len(rows), eng.H, eng.W, eng.C), dtype=torch.float32, device=eng.device)
-  fill_image_bank(infer, rows, bank, chunk)
-  return bank, rows
 
 
 class WholeNetwork:

@@ -142,7 +142,7 @@ def _gather_worker(rank, world, port, out):
   res = {}
   try:
     from overlapnet_b200 import data_parallel
-    from overlapnet_b200.training_leg import bank_rows
+    from overlapnet_b200.image_bank import bank_rows
     eng = _engine(4)
     infer = _PatternInfer(eng)
     keys = {('00', '%06d' % i) for i in range(3)} | {('01', '%06d' % i) for i in range(2)}

@@ -3,7 +3,7 @@ without a GPU: the placement rule over several ranks and the shard plan."""
 import pytest
 
 from overlapnet_b200 import _cabi, image_bank
-from overlapnet_b200.training_leg import bank_rows
+from overlapnet_b200.image_bank import bank_rows
 
 
 @pytest.mark.parametrize('bank,budget', [(10, 100), (10, 10), (11, 10), (0, 0), (100, 1)])

@@ -121,7 +121,8 @@ def test_one_process_step_sums_the_chunks_in_order():
   steps, eng = _Steps(), _StepEng()
   left = torch.arange(100, 116, dtype=torch.int32)
   parts = torch.full((3, 2), -1.0)
-  loss = training._chunked_step(None, steps, eng, 3, parts, parts, 0, 16, left, left, left, left, 0.7, 1e-3, None)
+  loss = training._step(None, steps, eng, data_parallel.step_plan(16, 1, 0, 3), parts, parts, 0, left, left, left, left,
+                        0.7, 1e-3, None)
   assert steps.calls == [(list(range(100, 116)), [0, 6, 11, 16])]
   (got, weights), = eng.steps
   assert weights == [6 / 16, 5 / 16, 5 / 16]
@@ -131,6 +132,6 @@ def test_one_process_step_sums_the_chunks_in_order():
   assert loss[0] == expect and loss[1] == float(sum(w * 0.1 for w in weights))
   # a short last batch: chunks of 1, 1, 0; the empty chunk has weight 0
   eng.steps.clear()
-  training._chunked_step(None, steps, eng, 3, parts, parts, 16, 18, torch.arange(18, dtype=torch.int32),
-                         left, left, left, 0.7, 1e-3, None)
+  training._step(None, steps, eng, data_parallel.step_plan(2, 1, 0, 3), parts, parts, 16,
+                 torch.arange(18, dtype=torch.int32), left, left, left, 0.7, 1e-3, None)
   assert steps.calls[-1] == ([16, 17], [0, 1, 2, 2]) and eng.steps[0][1] == [0.5, 0.5, 0.0]
