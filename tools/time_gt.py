@@ -18,7 +18,6 @@ Prints, as one JSON line:
 import argparse
 import json
 import os
-import subprocess
 import sys
 import threading
 import time
@@ -27,27 +26,21 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 
+import gpu_timing
 from overlapnet_b200 import gt, synth
 
 
-def nvsmi(fields):
-  try:
-    return subprocess.run(['nvidia-smi', '--query-gpu=' + fields, '--format=csv,noheader', '-i',
-                           str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
-  except Exception as e:                       # nvidia-smi missing: say so rather than guess
-    return 'unknown (%s)' % e
-
-
 class ClockSampler:
-  """SM clock (MHz) every 0.5 s inside the ``with`` block; the thread ends when the block does."""
+  """SM clock (MHz) of the current device every 0.5 s inside the ``with`` block; the thread ends when the block
+  does."""
 
   def __init__(self):
-    self.samples, self._stop = [], threading.Event()
+    self.samples, self._stop, self._device = [], threading.Event(), torch.cuda.current_device()
     self._t = threading.Thread(target=self._run, daemon=True)
 
   def _run(self):
     while not self._stop.is_set():
-      v = nvsmi('clocks.sm').split()
+      v = gpu_timing.nvidia_smi(('clocks.sm',), self._device)[0].split()
       if v and v[0].isdigit():
         self.samples.append(int(v[0]))
       self._stop.wait(0.5)
@@ -79,6 +72,7 @@ def main():
   ap.add_argument('--points', type=int, default=synth.KITTI_POINTS)
   ap.add_argument('--per-frame', type=int, default=3)
   args = ap.parse_args()
+  gpu_timing.require_cuda('time_gt.py')
   torch.cuda.set_device(0)
   n = args.scans
   clouds = [synth.kitti_like_cloud(i, n_points=args.points) for i in range(n)]
@@ -135,7 +129,7 @@ def main():
     identical &= bool(np.array_equal(m, rows[f * n:(f + 1) * n]))
   pairs = n * n
   out = {
-      'card': nvsmi('name,power.limit'), 'sm_clock_mhz_sampled': [min(clk.samples, default=0), max(clk.samples, default=0)],
+      'card': gpu_timing.card(), 'sm_clock_mhz_sampled': [min(clk.samples, default=0), max(clk.samples, default=0)],
       'scans': n, 'points_per_scan': args.points, 'pairs': pairs,
       'pruned_fraction': round(res.n_pruned / pairs, 4), 'pairs_with_overlap': int(np.count_nonzero(res.counts)),
       'all_pairs_s': round(t_all, 3), 'all_pairs_pairs_per_s': round(pairs / t_all),

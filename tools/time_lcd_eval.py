@@ -9,7 +9,6 @@ the card's name and power limit beside the numbers."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -17,6 +16,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
+import gpu_timing                                                 # noqa: E402
 from oracle import network as N                                   # noqa: E402
 from overlapnet_b200 import synth                                 # noqa: E402
 from overlapnet_b200.engine import Engine                         # noqa: E402
@@ -36,16 +36,6 @@ def rolled_bank(fv_src, n, dev):
   return fv_src[src[:, None], rows].contiguous()
 
 
-def card():
-  try:
-    out = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
-                         capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    name, limit = [s.strip() for s in out.split(',')]
-    return name, limit
-  except Exception as e:                                           # the numbers still stand; say what is missing
-    return torch.cuda.get_device_name(), 'unknown (%r)' % e
-
-
 def main():
   p = argparse.ArgumentParser()
   p.add_argument('--precision', default='f16_tc', choices=('f16_tc', 'fp32'))
@@ -54,8 +44,7 @@ def main():
   p.add_argument('--sample-rows', type=int, default=64)
   p.add_argument('--out')
   a = p.parse_args()
-  if not torch.cuda.is_available():
-    raise SystemExit('time_lcd_eval needs a CUDA device')
+  gpu_timing.require_cuda('time_lcd_eval.py')
   dev = torch.device('cuda', 0)
   eng = Engine(model=MODEL, precision=a.precision, max_batch_scans=N_SRC, max_batch_pairs=1101)
   eng.load_weights(N.glorot_weights(4, MODEL, seed=0))
@@ -107,9 +96,8 @@ def main():
     t_rows.append(ms)
   eng.check()
   agree = bool(np.array_equal(rec[1][:, 0].cpu().numpy(), best))
-  name, limit = card()
   res = {
-      'card': name, 'power_limit': limit, 'precision': a.precision, 'k': a.k,
+      'card': gpu_timing.card(), 'precision': a.precision, 'k': a.k,
       'bank': N_BANK, 'exclude_frames': EXCLUDE, 'pairs': pairs,
       'prefix_topk_all_rows_ms': full_ms, 'prefix_topk_pairs_per_s': pairs / (min(full_ms) * 1e-3),
       'rows_topk_ms_profiled': topk_ms, 'rows_topk_launches': topk_launches, 'profiled_run_ms': prof_ms,

@@ -12,7 +12,6 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -20,6 +19,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
+import gpu_timing                                                 # noqa: E402
 from overlapnet_b200 import mcl, synth                            # noqa: E402
 from overlapnet_b200.engine import Engine                         # noqa: E402
 from overlapnet_b200.infer import Infer                           # noqa: E402
@@ -47,16 +47,6 @@ def step_bytes(n, resampled):
   return b
 
 
-def card():
-  try:
-    out = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
-                         capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    name, limit = [s.strip() for s in out.split(',')]
-    return name, limit
-  except Exception as e:
-    return torch.cuda.get_device_name(), 'unknown (%r)' % e
-
-
 def timed(fn, reps):
   s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
   torch.cuda.synchronize()
@@ -74,9 +64,7 @@ def main():
   p.add_argument('--steps', type=int, default=50)
   p.add_argument('--out')
   a = p.parse_args()
-  if not torch.cuda.is_available():
-    raise SystemExit('time_mcl needs a CUDA device')
-  name, limit = card()
+  gpu_timing.require_cuda('time_mcl.py')
   K = a.keyframes
   kf = np.stack([2.0 * np.arange(K), np.zeros(K), np.zeros(K)], 1)
   idx = mcl.MapIndex(kf[:, :2], 0.5, 5.0)
@@ -85,7 +73,7 @@ def main():
   rng = np.random.default_rng(0)
   ov_all = torch.as_tensor(rng.random(K).astype(np.float32)).cuda()
   yaw_all = torch.as_tensor(rng.integers(-180, 180, K).astype(np.int32)).cuda()
-  result = {'card': name, 'power_limit': limit, 'keyframes': K, 'filter': []}
+  result = {'card': gpu_timing.card(), 'keyframes': K, 'filter': []}
   for n in (10 ** 4, 10 ** 5, 10 ** 6):
     for rho, label in ((0.0, 'no_resampling'), (1.0, 'resampling')):
       eng.mcl_init('global', n, 1, init_radius=2.0)

@@ -15,7 +15,6 @@ name and power limit; ``--out`` also writes it to a file.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -23,6 +22,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 
+import gpu_timing
 from oracle import network as N
 from overlapnet_b200 import synth
 from overlapnet_b200.engine import Engine
@@ -33,25 +33,8 @@ N_POINTS = 124668
 N_CAND = 1101
 
 
-def card():
-  q = subprocess.run(['nvidia-smi', '-i', str(torch.cuda.current_device()), '--query-gpu=power.limit,clocks.max.sm',
-                      '--format=csv,noheader'], capture_output=True, text=True)
-  return {'name': torch.cuda.get_device_name(), 'power_limit_and_max_sm_clock': q.stdout.strip() or q.stderr.strip()}
-
-
 def event_median_ms(fn, reps, warm):
-  for _ in range(warm):
-    fn()
-  torch.cuda.synchronize()
-  times = []
-  for _ in range(reps):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    fn()
-    b.record()
-    b.synchronize()
-    times.append(a.elapsed_time(b))
-  return float(np.median(times))
+  return float(np.median(gpu_timing.step_ms(lambda _: fn(), range(warm + reps), warm)))
 
 
 def host_median_ms(fn, reps, warm):
@@ -80,14 +63,13 @@ def main():
   ap.add_argument('--warmup', type=int, default=5)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
-  if not torch.cuda.is_available():
-    raise SystemExit('time_semantic_raw: no CUDA device')
+  gpu_timing.require_cuda('time_semantic_raw.py')
   eng = Engine(use=USE, model=MODEL, precision='f16_tc', max_batch_scans=32, max_batch_pairs=N_CAND)
   assert eng.C == 25
   eng.load_weights(N.glorot_weights(25, MODEL, seed=0))
   clouds = [synth.kitti_like_cloud(s, n_points=N_POINTS) for s in range(32)]
   probs = [synth.random_probs(1000 + s, N_POINTS) for s in range(32)]
-  res = {'card': card(), 'C': eng.C, 'n_points': N_POINTS, 'reps': args.reps}
+  res = {'card': gpu_timing.card(), 'C': eng.C, 'n_points': N_POINTS, 'reps': args.reps}
 
   for n in (1, 32):
     batch = eng.upload_clouds(clouds[:n])
