@@ -301,6 +301,60 @@ int ovn_mcl_copy_particles(ovn_handle* h, double* d_out, void* stream);
 int ovn_mcl_copy_stage(ovn_handle* h, int32_t stage, void* d_out, void* stream);
 int ovn_mcl_philox(ovn_handle* h, uint64_t seed, const uint32_t* d_ctr, int32_t n, uint32_t* d_out, void* stream);
 
+/* ---- point-to-plane ICP of loop-closure pairs on range images (overlapnet_b200/registration.py, DESIGN.md
+ * sections 4 and 7).  Reference: none (the paper's ICP verification of loop candidates, seeded by the yaw head).
+ * Pair i registers the source scan d_src[i] (RIGHT) to the target scan d_dst[i] (LEFT): it estimates the row-major
+ * float64 pose T = T_LEFT^-1 T_RIGHT that takes the source's vertices into the target's frame, starting from the
+ * first three rows of d_init[i] ([np][16]).  The images are what ovn_project_batch / ovn_normals_batch write at the
+ * handle's geometry: d_vertex [n_scans][H][W][4] (w = 1 where valid) and d_normal [n_scans][H][W][3] ((-1, -1, -1)
+ * where absent).  Per iteration k, with d_k = max(d_end, d_start gamma^k): a valid source pixel is moved by T in
+ * float64 and binned by the ground-truth generator's float64 range_projection (dropped outside (0, max_range)); it
+ * is an inlier when that target pixel is valid, ||p - q|| <= d_k and n_t . (R n_s) >= cos_normal.  The 29 float64
+ * sums of H = sum J^T J (upper triangle, row by row), g = sum J e, the inliers and sum e^2, with e = n_t . (p - q)
+ * and J = [p x n_t, n_t], give the update H delta = -g (Cholesky) applied on the left, T <- [R(omega) | v] T.  A pair
+ * ends CONVERGED once d_k = d_end and ||omega|| < eps_rot and ||v|| < eps_trans, DEGENERATE at a pivot <= 1e-12
+ * trace(H), TOO_FEW_INLIERS below min_inliers, else MAX_ITERATIONS.  One CTA runs every iteration of a pair and sums
+ * in a fixed order, so a pair's result has the same bits in any batch, position, call or handle.
+ *   d_out [np]: the pose, rms = sqrt(sum e^2 / inliers), inliers and the sums of the last iteration run, the valid
+ *               source pixels, the iterations run and the status.
+ *   d_assoc [np][H][W] (optional, NULL to skip): the inlier target pixel by * W + bx of each source pixel, or -1, in
+ *               the last iteration run.  d_system [np][29] (optional): that iteration's sums before its solve.  With
+ *               iterations = 1 both are exactly one step from d_init.
+ * NULL pointers, np < 0, n_scans < 1 with np > 0, iterations outside [1, 200], min_inliers < 0, a parameter that is
+ * not finite, d_end <= 0, d_end > d_start, gamma outside (0, 1], cos_normal outside [0, 1], eps_* < 0 and a d_init
+ * value that is not finite (read back synchronously) are OVN_ERR_INVALID_ARG with nothing launched; np = 0 is a
+ * no-op.  An index outside [0, n_scans) raises the device flag (ovn_check), and only its pair is poisoned: NaN pose
+ * and rms, status OVN_ICP_BAD_INDEX, d_assoc -1, d_system NaN. */
+#define OVN_ICP_SYSTEM_SIZE 29
+#define OVN_ICP_MAX_ITERATIONS_LIMIT 200
+typedef enum ovn_icp_status {
+  OVN_ICP_CONVERGED = 0,
+  OVN_ICP_MAX_ITERATIONS = 1,
+  OVN_ICP_DEGENERATE = 2,
+  OVN_ICP_TOO_FEW_INLIERS = 3,
+  OVN_ICP_BAD_INDEX = 4
+} ovn_icp_status;
+typedef struct ovn_icp_params {
+  double d_start, d_end, gamma;   /* association distance schedule, metres: d_k = max(d_end, d_start gamma^k) */
+  double cos_normal;              /* the least cosine between the target normal and the moved source normal */
+  double eps_rot, eps_trans;      /* convergence: the update's rotation (rad) and translation (m) */
+  int32_t iterations;             /* the most iterations, 1 .. 200 */
+  int32_t min_inliers;
+} ovn_icp_params;
+typedef struct ovn_icp_result {
+  double pose[16];                /* row-major T_LEFT^-1 T_RIGHT */
+  double rms;                     /* of the last iteration's inlier residuals, metres */
+  int32_t inliers;                /* of the last iteration */
+  int32_t valid;                  /* valid source pixels (vertex and normal) */
+  int32_t iterations;             /* iterations run */
+  int32_t status;                 /* ovn_icp_status */
+} ovn_icp_result;
+/* defaults: 2 m -> 0.3 m, gamma 0.8, cos 30 deg, 1e-6 rad, 1e-5 m, 30 iterations, 100 inliers (not tuned on KITTI) */
+void ovn_icp_default_params(ovn_icp_params* p);
+int ovn_icp_pairs(ovn_handle* h, const float* d_vertex, const float* d_normal, int32_t n_scans, const int32_t* d_src,
+                  const int32_t* d_dst, const double* d_init, int32_t np, const ovn_icp_params* params,
+                  ovn_icp_result* d_out, int32_t* d_assoc, double* d_system, void* stream);
+
 /* ---- resident bank (Infer keeps self.feature_volumes across calls, infer.py:113,184-193) ---------
  * The tensor-core heads consume fp16 / hi-lo split copies of the LEFT volumes.  Without this call
  * they are rebuilt from d_bank on every heads call; ovn_bank_prepare builds them once for rows

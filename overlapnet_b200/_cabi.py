@@ -32,12 +32,14 @@ SYMBOLS = [
     'ovn_set_train_stop', 'ovn_train_stage_size', 'ovn_copy_train_stage',
     'ovn_rows_topk', 'ovn_heads_prefix_topk',
     'ovn_mcl_set_map', 'ovn_mcl_init', 'ovn_mcl_predict', 'ovn_mcl_update', 'ovn_mcl_copy_particles',
-    'ovn_mcl_copy_stage', 'ovn_mcl_philox',
+    'ovn_mcl_copy_stage', 'ovn_mcl_philox', 'ovn_icp_default_params', 'ovn_icp_pairs',
 ]
 TOPK_MAX = 32     # ovn_rows_topk / ovn_heads_prefix_topk: k in [1, TOPK_MAX]
 MCL_INIT_MODES = {'global': 0, 'pose': 1}     # ovn_mcl_init_mode
 MCL_STAGES = {'motion': 0, 'lookup': 1, 'loglik': 2, 'weights': 3, 'prefix': 4, 'ancestors': 5}     # ovn_mcl_stage
 MCL_MAX_PARTICLES = 1 << 24
+ICP_SYSTEM_SIZE = 29      # ovn_icp_pairs: d_system [np][ICP_SYSTEM_SIZE]
+ICP_STATUS = {'converged': 0, 'max_iterations': 1, 'degenerate': 2, 'too_few_inliers': 3, 'bad_index': 4}     # ovn_icp_status
 IPC_HANDLE_BYTES = 64     # ovn_shard_create / ovn_shard_open
 HEADS_STAGES = {'o1': 0, 'x3': 1, 'dense': 2, 'centres': 3}     # ovn_heads_stage
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
@@ -67,6 +69,15 @@ class McEstimate(C.Structure):
   """ovn_mcl_estimate"""
   _fields_ = [('x', C.c_double), ('y', C.c_double), ('theta', C.c_double), ('ess', C.c_double),
               ('n_touched', C.c_int32), ('resampled', C.c_int32), ('step', C.c_int64)]
+
+
+class IcpParams(C.Structure):
+  """ovn_icp_params"""
+  _fields_ = [('d_start', C.c_double), ('d_end', C.c_double), ('gamma', C.c_double), ('cos_normal', C.c_double),
+              ('eps_rot', C.c_double), ('eps_trans', C.c_double), ('iterations', C.c_int32), ('min_inliers', C.c_int32)]
+
+
+ICP_RESULT_BYTES = 152    # sizeof(ovn_icp_result): pose double[16], rms double, inliers, valid, iterations, status int32
 
 
 class OvnError(Exception):
@@ -128,6 +139,9 @@ def lib():
   L.ovn_mcl_copy_particles.argtypes = [vp, vp, vp]
   L.ovn_mcl_copy_stage.argtypes = [vp, i32, vp, vp]
   L.ovn_mcl_philox.argtypes = [vp, u64, vp, i32, vp, vp]
+  L.ovn_icp_default_params.argtypes = [C.POINTER(IcpParams)]
+  L.ovn_icp_default_params.restype = None
+  L.ovn_icp_pairs.argtypes = [vp, vp, vp, i32, vp, vp, vp, i32, C.POINTER(IcpParams), vp, vp, vp, vp]
   L.ovn_bank_release.argtypes = [vp, vp]
   L.ovn_check.argtypes = [vp, vp]
   L.ovn_set_feature_center.argtypes = [vp, vp]

@@ -99,6 +99,9 @@ int check_device_error(ovn_handle* h, cudaStream_t s) {
   const char* ring = nullptr;          // a ring wait timed out: producer codes are 1xx, consumer codes 2xx / 4xx
   switch (e) {
     case kErrBadIndex: OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "a pair / candidate index is outside [0, bank_size)");
+    case kErrIcpBadIndex:
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_icp_pairs: a scan index is outside [0, n_scans) (that pair's outputs "
+                  "are poisoned: NaN pose, status OVN_ICP_BAD_INDEX)");
     case kErrRowNotPrepared:
       OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "resident bank: an indexed row was never passed to ovn_bank_prepare");
     case kErrNonFiniteOperand:
@@ -889,6 +892,50 @@ int ovn_mcl_philox(ovn_handle* h, uint64_t seed, const uint32_t* d_ctr, int32_t 
   REQUIRE(h, n >= 0, "n must be >= 0");
   REQUIRE(h, n == 0 || (d_ctr && d_out), "NULL pointer");
   return mcl_philox(h, seed, d_ctr, n, d_out, (cudaStream_t)stream);
+}
+
+// ---- point-to-plane ICP of loop-closure pairs ----------------------------------------------------------------
+void ovn_icp_default_params(ovn_icp_params* p) {
+  if (!p) return;
+  p->d_start = 2.0;
+  p->d_end = 0.3;
+  p->gamma = 0.8;
+  p->cos_normal = 0.86602540378443865;      // cos 30 deg
+  p->eps_rot = 1e-6;
+  p->eps_trans = 1e-5;
+  p->iterations = 30;
+  p->min_inliers = 100;
+}
+
+int ovn_icp_pairs(ovn_handle* h, const float* d_vertex, const float* d_normal, int32_t n_scans, const int32_t* d_src,
+                  const int32_t* d_dst, const double* d_init, int32_t np, const ovn_icp_params* params,
+                  ovn_icp_result* d_out, int32_t* d_assoc, double* d_system, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, params, "NULL pointer");
+  REQUIRE(h, np >= 0, "np must be >= 0");
+  const ovn_icp_params& p = *params;
+  REQUIRE(h, p.iterations >= 1 && p.iterations <= OVN_ICP_MAX_ITERATIONS_LIMIT, "iterations must be in [1, 200]");
+  REQUIRE(h, p.min_inliers >= 0, "min_inliers must be >= 0");
+  REQUIRE(h, std::isfinite(p.d_start) && std::isfinite(p.d_end) && std::isfinite(p.gamma) &&
+                 std::isfinite(p.cos_normal) && std::isfinite(p.eps_rot) && std::isfinite(p.eps_trans),
+          "every ICP parameter must be finite");
+  REQUIRE(h, p.d_end > 0.0 && p.d_end <= p.d_start, "0 < d_end <= d_start");
+  REQUIRE(h, p.gamma > 0.0 && p.gamma <= 1.0, "gamma must be in (0, 1]");
+  REQUIRE(h, p.cos_normal >= 0.0 && p.cos_normal <= 1.0, "cos_normal must be in [0, 1]");
+  REQUIRE(h, p.eps_rot >= 0.0 && p.eps_trans >= 0.0, "eps_rot and eps_trans must be >= 0");
+  if (np == 0) return OVN_OK;
+  REQUIRE(h, d_vertex && d_normal && d_src && d_dst && d_init && d_out, "NULL pointer");
+  REQUIRE(h, n_scans >= 1, "n_scans must be >= 1");
+  cudaStream_t s = (cudaStream_t)stream;
+  std::vector<double> init((size_t)np * 16);
+  OVN_CUDA(h, cudaMemcpyAsync(init.data(), d_init, init.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  OVN_CUDA(h, cudaStreamSynchronize(s));
+  for (size_t i = 0; i < init.size(); ++i)
+    if (!std::isfinite(init[i]))
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_icp_pairs: d_init[%lld][%lld] is not finite", (long long)(i / 16),
+                  (long long)(i % 16));
+  return icp_pairs(h, d_vertex, d_normal, n_scans, d_src, d_dst, d_init, np, p, d_out, d_assoc, d_system, s);
 }
 
 // ---- training precision ---------------------------------------------------------------------------

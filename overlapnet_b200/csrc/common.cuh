@@ -362,6 +362,7 @@ enum DeviceError : int {
   kErrInjectedFault = 501,        // k_conv2_wgmma under OVN_DEBUG_FAULT (the error-path test hook)
   kErrBadIndex = 900,             // a pair / candidate index outside [0, bank_size)
   kErrRowNotPrepared = 901,       // resident bank: the row was never passed to ovn_bank_prepare
+  kErrIcpBadIndex = 902,          // ovn_icp_pairs: a scan index outside [0, n_scans)
   kErrNonFiniteOperand = 910,     // an fp16 operand of the tensor-core heads or leg is not finite (NaN, inf, > 65504)
   kErrPeerWait = 950,             // ovn_peer_wait: a peer rank never signalled
 };
@@ -481,6 +482,11 @@ int mcl_update(ovn_handle* h, const float* d_ov, const int32_t* d_yaw, double s_
 int mcl_copy_particles(ovn_handle* h, double* d_out, cudaStream_t s);
 int mcl_copy_stage(ovn_handle* h, int stage, void* d_out, cudaStream_t s);
 int mcl_philox(ovn_handle* h, uint64_t seed, const uint32_t* d_ctr, int n, uint32_t* d_out, cudaStream_t s);
+
+// point-to-plane ICP of np pairs (icp.cu), one k_icp_pairs launch; the caller has checked every argument
+int icp_pairs(ovn_handle* h, const float* d_vertex, const float* d_normal, int n_scans, const int32_t* d_src,
+              const int32_t* d_dst, const double* d_init, int np, const ovn_icp_params& prm, ovn_icp_result* d_out,
+              int32_t* d_assoc, double* d_system, cudaStream_t s);
 
 int corr_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* left,
                       const int32_t* right, int np, int32_t* d_yaw, float* d_corr, cudaStream_t s);

@@ -8,14 +8,9 @@
 // like integers; only the range image is needed, so no point index travels with the key); a second
 // kernel rounds the winners to float32 (the image dtype, utils.py:120) and a third counts pixels.
 // HBM-bound byte work: 16 B read per point, 8 B atomic per valid point into an L2-resident key image.
-#include "common.cuh"
+#include "range_bin.cuh"
 
 namespace ovn {
-
-struct GtParams {
-  int H, W;
-  double pi, abs_fov_down, fov, max_range;
-};
 
 constexpr unsigned long long kGtEmpty = 0xFFFFFFFFFFFFFFFFull;
 
@@ -31,20 +26,13 @@ __device__ __forceinline__ void mat4_apply(const double* __restrict__ M, double&
   x = r[0]; y = r[1]; z = r[2]; w = r[3];
 }
 
-// range_projection of one transformed point in float64 (utils.py:75-104) and the atomic-min of its
+// range_projection of one transformed point in float64 (utils.py:75-104, range_bin) and the atomic-min of its
 // depth into the key image `keys` [H][W]; points outside (0, max_range) are dropped
 __device__ __forceinline__ void gt_scatter_point(double x, double y, double z, const GtParams& P,
                                                  unsigned long long* __restrict__ keys) {
-  const double depth = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)));   // utils.py:75
-  if (!(depth > 0.0 && depth < P.max_range)) return;                                                     // :76-77
-  const double yaw = -atan2(y, x);                                                                       // :86
-  const double pitch = asin(__ddiv_rn(z, depth));                                                        // :87
-  double px = __dmul_rn(0.5, __dadd_rn(__ddiv_rn(yaw, P.pi), 1.0));                                      // :90
-  double py = __dsub_rn(1.0, __ddiv_rn(__dadd_rn(pitch, P.abs_fov_down), P.fov));                        // :91
-  px = floor(__dmul_rn(px, (double)P.W));                                                                // :94,98
-  py = floor(__dmul_rn(py, (double)P.H));
-  const int bx = (int)fmax(0.0, fmin((double)(P.W - 1), px));                                            // :99-104
-  const int by = (int)fmax(0.0, fmin((double)(P.H - 1), py));
+  double depth;
+  int bx, by;
+  if (!range_bin(x, y, z, P, depth, bx, by)) return;
   atomicMin(keys + (size_t)by * P.W + bx, (unsigned long long)__double_as_longlong(depth));
 }
 
@@ -99,17 +87,6 @@ k_gt_overlap_count(const float* __restrict__ ref, const float* __restrict__ cur,
     for (int k = 0; k < 8; ++k) t += s[k];
     if (t) atomicAdd(counts + b, t);
   }
-}
-
-static GtParams gt_params(const ovn_handle* h, float max_range) {
-  GtParams P;
-  P.H = h->cfg.proj_H; P.W = h->cfg.proj_W;
-  P.pi = 3.14159265358979323846;
-  const double fu = (double)h->cfg.fov_up_deg / 180.0 * P.pi, fd = (double)h->cfg.fov_down_deg / 180.0 * P.pi;   // utils.py:70-71
-  P.abs_fov_down = fabs(fd);
-  P.fov = fabs(fd) + fabs(fu);                                                                                     // :72
-  P.max_range = max_range < 0 ? (double)h->cfg.max_range : (double)max_range;
-  return P;
 }
 
 int gt_range_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans, int64_t n_total,

@@ -548,6 +548,41 @@ class Engine:
                                         self._stream()), 'ovn_mcl_philox')
     return out
 
+  def icp(self, vertex, normal, src, dst, init, params=None, want_stage=False):
+    """ovn_icp_pairs: point-to-plane ICP of the pairs (source scan src[i] = RIGHT, target scan dst[i] = LEFT) of the
+    images ``vertex`` [n, H, W, 4] and ``normal`` [n, H, W, 3] (Engine.project / Engine.normals), from ``init``
+    [np, 4, 4] float64.  ``params``: a dict overriding icp_default_params().  Returns a dict of cuda tensors: pose
+    [np, 4, 4] f64, rms [np] f64, inliers / valid / iterations / status [np] i32, and with ``want_stage`` assoc
+    [np, H, W] i32 and system [np, 29] f64 of the last iteration run.  Index errors surface at the next check()."""
+    prm = _cabi.IcpParams()
+    lib().ovn_icp_default_params(C.byref(prm))
+    for key, value in (params or {}).items():
+      if key not in dict(prm._fields_):
+        raise KeyError('unknown ICP parameter %r' % key)
+      setattr(prm, key, value)
+    dev = self.device
+    src = torch.as_tensor(src, dtype=torch.int32).reshape(-1).to(dev).contiguous()
+    dst = torch.as_tensor(dst, dtype=torch.int32).reshape(-1).to(dev).contiguous()
+    n_pairs = int(src.numel())
+    init = torch.as_tensor(init, dtype=torch.float64).reshape(n_pairs, 16).to(dev).contiguous()
+    assert dst.numel() == n_pairs
+    assert vertex.dtype == torch.float32 and normal.dtype == torch.float32 and vertex.is_contiguous() \
+        and normal.is_contiguous()
+    n = int(vertex.shape[0])
+    assert tuple(vertex.shape) == (n, self.H, self.W, 4) and tuple(normal.shape) == (n, self.H, self.W, 3)
+    raw = torch.empty((n_pairs, _cabi.ICP_RESULT_BYTES // 8), dtype=torch.float64, device=dev)
+    assoc = torch.empty((n_pairs, self.H, self.W), dtype=torch.int32, device=dev) if want_stage else None
+    system = torch.empty((n_pairs, _cabi.ICP_SYSTEM_SIZE), dtype=torch.float64, device=dev) if want_stage else None
+    check(self._h, lib().ovn_icp_pairs(self._h, _ptr(vertex), _ptr(normal), n, _ptr(src), _ptr(dst), _ptr(init),
+                                       n_pairs, C.byref(prm), _ptr(raw), _ptr(assoc), _ptr(system), self._stream()),
+          'ovn_icp_pairs')
+    ints = raw[:, 17:].view(torch.int32)
+    out = {'pose': raw[:, :16].reshape(n_pairs, 4, 4), 'rms': raw[:, 16], 'inliers': ints[:, 0], 'valid': ints[:, 1],
+           'iterations': ints[:, 2], 'status': ints[:, 3]}
+    if want_stage:
+      out.update(assoc=assoc, system=system)
+    return out
+
   def bank_prepare(self, bank, first=0, count=None):
     """Keep the tensor-core operand copies of bank rows [first, first+count) resident: later heads
     calls on this same tensor skip the per-call conversion (ovn_bank_prepare)."""

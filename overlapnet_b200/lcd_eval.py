@@ -2,7 +2,7 @@
 paper, with the candidate rules of the reference's demo 3 (demo/demo3_lcd.py).
 
   python -m overlapnet_b200.lcd_eval [config/demo.yml] [--top-k K] [--exclude-frames 100] [--exclude-distance 50]
-                                     [--gt-overlap 0.3]
+                                     [--gt-overlap 0.3] [--register [--min-inlier-fraction 0.3]]
   torchrun --nproc_per_node G -m overlapnet_b200.lcd_eval ...            (the rows split over G GPUs)
 
 The protocol (DESIGN.md section 7):
@@ -18,6 +18,9 @@ The protocol (DESIGN.md section 7):
               query i is positive when max_{j < c_i} g[i, j] > gt_overlap, and correct when g[i, j*_i] > gt_overlap
               for its top record j*_i.  Queries are the rows with c_i > 0.
   curve       for every distinct top score t, the queries with s_i >= t are declared (``metrics``).
+  register    (opt-in) each top record is registered by point-to-plane ICP on the GPU (registration.register),
+              LEFT = j*_i, RIGHT = i, once from the heads' yaw seed and once from the identity, against the
+              ground-truth pose T_j*^-1 T_i; a success is a translation error < 0.5 m and a rotation error < 2 deg.
 
 Scans are encoded from the raw ``.bin`` files (Infer.encode_clouds); configs with class probabilities are
 refused, since they would need a ``.label`` file per scan.  Results go to ``<experiments_path>/<testname>`` of
@@ -36,6 +39,9 @@ from ._cabi import TOPK_MAX
 logger = logging.getLogger('overlapnet_b200.lcd_eval')
 
 OPERATING_POINT = 0.3          # demo3_lcd.py:119 declares a loop when max overlap > 0.3 (strict)
+SUCCESS_TRANSLATION = 0.5      # metres: a registration within this and SUCCESS_ROTATION of the ground truth succeeds
+SUCCESS_ROTATION = 2.0         # degrees
+SEEDS = ('yaw', 'identity')    # the seed axis of the registration_* arrays
 
 
 # ---- the candidate prefix ---------------------------------------------------------------------------------
@@ -187,6 +193,72 @@ def yaw_errors(engine, bank, rows, cand, gt_bin, width=360):
   return np.minimum(a, width - a)                                  # evaluate.error_statistics' circular rule
 
 
+# ---- registration of the top records --------------------------------------------------------------------------
+def register_records(engine, clouds, poses, rows, top_index, top_yaw, params=None):
+  """Register the top record of each of ``rows`` (LEFT = top_index[r, 0], RIGHT = rows[r]) twice in one call, from
+  the yaw seed of top_yaw[r, 0] and from the identity.  Returns a dict of arrays over the rows, the seed axis in
+  SEEDS order: pose [rows, 2, 4, 4], gt_pose [rows, 4, 4] (T_j*^-1 T_i), error [rows, 2, 2] (metres, degrees),
+  inlier_fraction [rows, 2] (inliers over valid source pixels), rms [rows, 2], status / iterations [rows, 2] int32.
+  A row without a record holds NaN, status -1 and 0 iterations."""
+  from .evaluate import yaw_to_argmax
+  from .registration import pose_error, register, seed_pose
+  rows = np.asarray(rows, np.int64)
+  n = rows.size
+  out = {'pose': np.full((n, 2, 4, 4), np.nan), 'gt_pose': np.full((n, 4, 4), np.nan),
+         'error': np.full((n, 2, 2), np.nan), 'inlier_fraction': np.full((n, 2), np.nan),
+         'rms': np.full((n, 2), np.nan), 'status': np.full((n, 2), -1, np.int32),
+         'iterations': np.zeros((n, 2), np.int32)}
+  live = np.flatnonzero(np.asarray(top_index)[:, 0] >= 0) if n else np.zeros(0, np.int64)
+  if live.size:
+    left = np.asarray(top_index)[live, 0].astype(np.int64)
+    right = rows[live]
+    init = np.concatenate([seed_pose(yaw_to_argmax(np.asarray(top_yaw)[live, 0]), engine.Wf),
+                           np.broadcast_to(np.eye(4), (live.size, 4, 4))])
+    res = register(engine, clouds, np.concatenate([left, left]), np.concatenate([right, right]), init, params)
+    gt = np.linalg.solve(poses[left], poses[right])
+    m = live.size
+    pose = np.stack([res['pose'][:m], res['pose'][m:]], 1)
+    t_err, r_err = pose_error(pose, gt[:, None])
+    out['pose'][live] = pose
+    out['gt_pose'][live] = gt
+    out['error'][live] = np.stack([t_err, np.rad2deg(r_err)], -1)
+    for key in ('rms', 'status', 'iterations'):
+      out[key][live] = np.stack([res[key][:m], res[key][m:]], 1)
+    frac = res['inliers'] / np.maximum(res['valid'], 1).astype(np.float64)
+    out['inlier_fraction'][live] = np.stack([frac[:m], frac[m:]], 1)
+  return out
+
+
+def registration_summary(top_overlap, top_index, gt_top_overlap, gt_best, tp_rows, error, inlier_fraction,
+                         gt_overlap=0.3, min_inlier_fraction=0.3, operating_point=OPERATING_POINT):
+  """The ``registration`` section of the summary: over the true positives ``tp_rows`` at F1max, the success rate
+  from each seed and the yaw seed's median / max errors; and precision / recall at the operating point when a
+  declared loop must also reach ``min_inlier_fraction`` from the yaw seed (``error`` [rows, 2, 2] and
+  ``inlier_fraction`` [rows, 2] as register_records gives them)."""
+  error = np.asarray(error, np.float64)
+  tp_rows = np.asarray(tp_rows, np.int64)
+  e = error[tp_rows]
+  ok = (e[..., 0] < SUCCESS_TRANSLATION) & (e[..., 1] < SUCCESS_ROTATION)
+  out = {'success_translation_m': SUCCESS_TRANSLATION, 'success_rotation_deg': SUCCESS_ROTATION,
+         'min_inlier_fraction': min_inlier_fraction, 'true_positives': int(tp_rows.size)}
+  for k, seed in enumerate(SEEDS):
+    out['success_rate_' + seed] = float(ok[:, k].mean()) if tp_rows.size else float('nan')
+  for k, what in enumerate(('translation_m', 'rotation_deg')):
+    v = e[:, 0, k]
+    out['median_error_%s_yaw' % what] = float(np.median(v)) if v.size else float('nan')
+    out['max_error_%s_yaw' % what] = float(np.max(v)) if v.size else float('nan')
+  top_index = np.asarray(top_index)
+  query = top_index[:, 0] >= 0
+  s = np.asarray(top_overlap, np.float64)[:, 0]
+  correct = query & (np.asarray(gt_top_overlap, np.float64)[:, 0] > gt_overlap)
+  n_pos = int((query & (np.asarray(gt_best, np.float64) > gt_overlap)).sum())
+  declared = query & (s > operating_point) & (np.asarray(inlier_fraction, np.float64)[:, 0] >= min_inlier_fraction)
+  tp = int((declared & correct).sum())
+  out['precision_at_operating_point_verified'] = tp / int(declared.sum()) if declared.any() else 1.0
+  out['recall_at_operating_point_verified'] = tp / n_pos if n_pos else float('nan')
+  return out
+
+
 # ---- the driver ---------------------------------------------------------------------------------------------
 def _dist():
   dist = torch.distributed
@@ -238,13 +310,16 @@ def save_npz(path, arrays):
 
 
 def evaluate_clouds(infer, clouds, poses, top_k=5, exclude_frames=100, exclude_distance=50, gt_overlap=0.3,
-                    out_dir=None):
+                    out_dir=None, register=False, min_inlier_fraction=0.3):
   """Evaluate loop closure over a sequence: ``clouds`` (N, 4) float32 arrays or zero-argument callables returning
   one, ``poses`` (n, 4, 4) LiDAR-frame poses, ``infer`` an overlapnet_b200.Infer.  In a process group every rank
   encodes a contiguous share of the scans, the bank is all-gathered, every rank scores and labels the rows of an
   equal share of the pairs, and rank 0 gathers them; the results do not depend on the world size.  Returns on
   rank 0 (summary dict, results dict of arrays), None elsewhere; rank 0 writes lcd_results.npz and
-  lcd_summary.json to ``out_dir`` when given."""
+  lcd_summary.json to ``out_dir`` when given.  With ``register`` each rank also registers its rows' top records
+  (register_records) and the results gain the registration_* arrays and a ``registration`` summary section
+  (registration_summary, with ``min_inlier_fraction``); without it nothing differs from an evaluation without
+  registration."""
   if not 1 <= int(top_k) <= TOPK_MAX:
     raise ValueError('top_k must be in [1, %d], got %r' % (TOPK_MAX, top_k))
   top_k = int(top_k)
@@ -266,13 +341,17 @@ def evaluate_clouds(infer, clouds, poses, top_k=5, exclude_frames=100, exclude_d
   top_ov, top_idx, top_yaw = search(eng, bank, c, top_k, r_lo, r_hi)
   truth = ground_truth(clouds, poses, np.arange(r_lo, r_hi), c[r_lo:r_hi], top_idx, eng.Wf, local=world > 1)
   part = (top_ov, top_idx, top_yaw, truth['best'], truth['top_overlap'], truth['top_yaw_bin'])
+  if register:
+    reg = register_records(eng, clouds, poses, np.arange(r_lo, r_hi), top_idx, top_yaw)
+    reg_keys = sorted(reg)
+    part += tuple(reg[key] for key in reg_keys)
   if world > 1:
     parts = [None] * world if rank == 0 else None
     dist.gather_object(part, parts, dst=0)
     if rank != 0:
       return None
     part = tuple(np.concatenate([p[f] for p in parts]) for f in range(len(part)))
-  top_ov, top_idx, top_yaw, gt_best, gt_top, gt_bin = part
+  top_ov, top_idx, top_yaw, gt_best, gt_top, gt_bin = part[:6]
   summary, curve = metrics(top_ov, top_idx, gt_top, gt_best, gt_overlap)
   t = summary['f1_max_threshold']
   tp_rows = true_positives_at(top_ov, top_idx, gt_top, t, gt_overlap) if np.isfinite(t) else np.zeros(0, np.int64)
@@ -287,6 +366,11 @@ def evaluate_clouds(infer, clouds, poses, top_k=5, exclude_frames=100, exclude_d
              'gt_top_yaw_bin': gt_bin, 'gt_best': gt_best, 'positive': gt_best > gt_overlap,
              'true_positive_rows': tp_rows, 'yaw_error': d_yaw}
   results.update({'curve_' + key: v for key, v in curve.items()})
+  if register:
+    reg = dict(zip(reg_keys, part[6:]))
+    results.update({'registration_' + key: v for key, v in reg.items()})
+    summary['registration'] = registration_summary(top_ov, top_idx, gt_top, gt_best, tp_rows, reg['error'],
+                                                   reg['inlier_fraction'], gt_overlap, min_inlier_fraction)
   if out_dir is not None:
     os.makedirs(out_dir, exist_ok=True)
     save_npz(os.path.join(out_dir, 'lcd_results.npz'), results)
@@ -305,9 +389,15 @@ def parse_args(argv):
   p.add_argument('--exclude-distance', type=float, default=50.0, help='metres of travel skipped (default 50)')
   p.add_argument('--gt-overlap', type=float, default=0.3, help='ground-truth overlap of a true loop (default 0.3)')
   p.add_argument('--precision', default='f16_tc', choices=('f16_tc', 'fp32'))
+  p.add_argument('--register', action='store_true',
+                 help='register each top record by ICP on the GPU, from the yaw seed and from the identity')
+  p.add_argument('--min-inlier-fraction', type=float, default=0.3,
+                 help='with --register: the inlier fraction a verified loop reaches (default 0.3)')
   args = p.parse_args(argv)
   if not 1 <= args.top_k <= TOPK_MAX:
     p.error('--top-k must be in [1, %d], got %d' % (TOPK_MAX, args.top_k))
+  if not 0.0 <= args.min_inlier_fraction <= 1.0:
+    p.error('--min-inlier-fraction must be in [0, 1], got %g' % args.min_inlier_fraction)
   return args
 
 
@@ -348,7 +438,7 @@ def main(argv=None):
   infer = Infer(net, precision=args.precision)
   out_dir = os.path.join(net.get('experiments_path', '/tmp'), net.get('testname', 'experiment_test'))
   res = evaluate_clouds(infer, clouds, poses, args.top_k, args.exclude_frames, args.exclude_distance,
-                        args.gt_overlap, out_dir)
+                        args.gt_overlap, out_dir, args.register, args.min_inlier_fraction)
   if res is not None:
     s = res[0]
     logger.info('Loop closure over %d scans, %d queries, %d positive (ground-truth overlap > %g), %d pairs scored',
@@ -360,6 +450,15 @@ def main(argv=None):
     logger.info('  recall@1 / recall@%d:            %f / %f', s['k'], s['recall_at_1'], s['recall_at_k'])
     logger.info('  yaw error of the %d true positives at F1max: mean %f, max %f, RMS %f bins',
                 s['true_positives_at_f1_max'], s['yaw_error_mean'], s['yaw_error_max'], s['yaw_error_rms'])
+    if 'registration' in s:
+      r = s['registration']
+      logger.info('  registration of the %d true positives: success %f from the yaw seed, %f from the identity '
+                  '(< %g m, < %g deg); yaw seed median %f m / %f deg', r['true_positives'], r['success_rate_yaw'],
+                  r['success_rate_identity'], r['success_translation_m'], r['success_rotation_deg'],
+                  r['median_error_translation_m_yaw'], r['median_error_rotation_deg_yaw'])
+      logger.info('  precision / recall at > %g with inlier fraction >= %g: %f / %f', s['operating_point'],
+                  r['min_inlier_fraction'], r['precision_at_operating_point_verified'],
+                  r['recall_at_operating_point_verified'])
     logger.info('  written to %s', out_dir)
   if world > 1:
     torch.distributed.barrier()

@@ -62,3 +62,130 @@ def feature_volumes(seed, n, width=360, channels=128, sparsity=0.5, scale=1.0):
   v = rng.standard_normal((n, 1, width, channels)).astype(np.float32) * np.float32(scale)
   v = np.maximum(v + np.float32(scale * (0.0 if sparsity == 0.5 else 0.3)), 0)
   return np.ascontiguousarray(v, dtype=np.float32)
+
+
+# ---- an analytic street scene, ray-cast from any pose -----------------------------------------------------------
+HDL64_PITCH_DEG = (-24.8, 2.0)     # the 64 beams' elevations span this range evenly
+STREET_CELL = 40.0                 # roads run along x = 40 i and y = 40 j
+STREET_HALF_WIDTH = 7.0
+
+
+def _street_cell_objects(seed, i, j):
+  """Boxes [(x0, x1, y0, y1, z1)] and poles [(x, y, radius, height)] of the city block whose corner is (40 i, 40 j):
+  two or three buildings set back from the roads, parked boxes and poles along its kerbs.  Seeded by (seed, i, j)
+  only, so a block is the same from every pose."""
+  rng = np.random.default_rng([int(seed) & 0xFFFFFFFF, int(i) & 0xFFFFFFFF, int(j) & 0xFFFFFFFF])
+  x0, y0 = STREET_CELL * i, STREET_CELL * j
+  lo, hi = STREET_HALF_WIDTH + 2.0 + rng.uniform(0, 2, 2), STREET_CELL - STREET_HALF_WIDTH - 2.0 - rng.uniform(0, 2, 2)
+  boxes, poles = [], []
+  cuts = np.sort(rng.uniform(lo[0] + 6, hi[0] - 6, rng.integers(1, 3)))
+  edges = np.concatenate([[lo[0]], cuts, [hi[0]]])
+  for a, b in zip(edges[:-1], edges[1:]):          # buildings side by side, a 1.5 m gap between neighbours
+    boxes.append((x0 + a, x0 + b - 1.5, y0 + lo[1], y0 + hi[1], rng.uniform(6.0, 20.0)))
+  for side in range(4):                            # kerbside boxes (parked cars, kiosks) and poles
+    for _ in range(rng.integers(1, 4)):
+      s = rng.uniform(4.0, STREET_CELL - 8.0)
+      w, l, h = rng.uniform(1.6, 2.2), rng.uniform(3.5, 5.0), rng.uniform(1.4, 2.5)
+      off = STREET_HALF_WIDTH - 2.0 - w
+      if side == 0: boxes.append((x0 + s, x0 + s + l, y0 + off, y0 + off + w, h))
+      elif side == 1: boxes.append((x0 + off, x0 + off + w, y0 + s, y0 + s + l, h))
+      elif side == 2: boxes.append((x0 + s, x0 + s + l, y0 + STREET_CELL - off - w, y0 + STREET_CELL - off, h))
+      else: boxes.append((x0 + STREET_CELL - off - w, x0 + STREET_CELL - off, y0 + s, y0 + s + l, h))
+    for _ in range(rng.integers(1, 3)):
+      s = rng.uniform(2.0, STREET_CELL - 2.0)
+      r = STREET_HALF_WIDTH - 0.5
+      xy = [(x0 + s, y0 + r), (x0 + r, y0 + s), (x0 + s, y0 + STREET_CELL - r), (x0 + STREET_CELL - r, y0 + s)][side]
+      poles.append((xy[0], xy[1], rng.uniform(0.1, 0.25), rng.uniform(4.0, 8.0)))
+  return boxes, poles
+
+
+def street_scene_cloud(pose, seed=0, noise=0.0, n_azimuth=1800, max_hit=80.0, ground_only=False):
+  """A HDL-64-like scan of a seeded street scene from the LiDAR pose ``pose`` (4x4 float64, world from sensor): a
+  ground plane z = 0, blocks of buildings between roads along x = 40 i and y = 40 j (14 m wide), parked boxes and
+  poles along the kerbs.  64 beams span -24.8 .. +2 degrees, ``n_azimuth`` columns per turn; a ray keeps its nearest
+  hit closer than ``max_hit`` metres, plus N(0, ``noise``) metres along the ray.  Ground hits sit at z = 0 exactly
+  in the world, so a level scan's ground points share one float32 z.  Returns (N, 4) float32 x, y, z, intensity
+  in the sensor frame.  Sensors ride at about 1.73 m (KITTI's mounting height)."""
+  T = np.asarray(pose, np.float64).reshape(4, 4)
+  R, o = T[:3, :3], T[:3, 3]
+  pitch = np.deg2rad(np.linspace(HDL64_PITCH_DEG[0], HDL64_PITCH_DEG[1], 64))
+  az = (np.arange(n_azimuth) + 0.5) * (2 * np.pi / n_azimuth)
+  pp, aa = np.meshgrid(pitch, az, indexing='ij')
+  d_local = np.stack([np.cos(pp) * np.cos(aa), np.cos(pp) * np.sin(aa), np.sin(pp)], -1).reshape(-1, 3)
+  d = d_local @ R.T
+  t = np.full(d.shape[0], np.inf)
+  with np.errstate(divide='ignore', invalid='ignore'):
+    tg = np.where(d[:, 2] < 0, -o[2] / d[:, 2], np.inf)
+  ground = tg < t
+  t = np.where(ground, tg, t)
+  if not ground_only:
+    t = t.reshape(64, n_azimuth)
+    ground = ground.reshape(64, n_azimuth)
+    dd = d.reshape(64, n_azimuth, 3)
+    level = abs(R[2, 2] - 1.0) < 1e-12
+    heading = np.arctan2(R[1, 0], R[0, 0])
+    step = 2 * np.pi / n_azimuth
+
+    def columns(xy, half=0.0):
+      """The columns whose rays can reach points xy (k, 2) widened by the angle `half`; every column unless level."""
+      if not level:
+        return slice(None)
+      rel = np.arctan2(xy[:, 1] - o[1], xy[:, 0] - o[0]) - heading
+      c = np.angle(np.exp(1j * rel).mean())                  # the points lie within a half turn of their mean
+      dev = np.angle(np.exp(1j * (rel - c)))
+      lo, hi = c + dev.min() - half - 2 * step, c + dev.max() + half + 2 * step
+      k0, k1 = int(np.floor(lo / step)), int(np.ceil(hi / step))
+      return np.arange(k0, k1 + 1) % n_azimuth
+
+    reach = max_hit + STREET_CELL
+    i0, i1 = int(np.floor((o[0] - reach) / STREET_CELL)), int(np.floor((o[0] + reach) / STREET_CELL))
+    j0, j1 = int(np.floor((o[1] - reach) / STREET_CELL)), int(np.floor((o[1] + reach) / STREET_CELL))
+    with np.errstate(invalid='ignore', divide='ignore'):
+      for i in range(i0, i1 + 1):
+        for j in range(j0, j1 + 1):
+          boxes, poles = _street_cell_objects(seed, i, j)
+          for (bx0, bx1, by0, by1, bz1) in boxes:          # slab test of an axis-aligned box on the ground
+            near = np.hypot(max(bx0 - o[0], 0, o[0] - bx1), max(by0 - o[1], 0, o[1] - by1))
+            if near >= max_hit:
+              continue
+            inside = bx0 <= o[0] <= bx1 and by0 <= o[1] <= by1
+            cols = slice(None) if inside else columns(np.array([[bx0, by0], [bx0, by1], [bx1, by0], [bx1, by1]]))
+            dc = dd[:, cols]
+            inv = 1.0 / dc
+            ta = (np.array([bx0, by0, 0.0]) - o) * inv
+            tb = (np.array([bx1, by1, bz1]) - o) * inv
+            tn = np.nanmax(np.minimum(ta, tb), -1)
+            tf = np.nanmin(np.maximum(ta, tb), -1)
+            tc = t[:, cols]
+            hit = (tn <= tf) & (tn > 0) & (tn < tc)
+            t[:, cols] = np.where(hit, tn, tc)
+            ground[:, cols] &= ~hit
+          for (cx, cy, r, h) in poles:                     # vertical cylinder, entry point only
+            dist = np.hypot(cx - o[0], cy - o[1])
+            if dist - r >= max_hit or dist <= r:
+              continue
+            cols = columns(np.array([[cx, cy]]), np.arcsin(r / dist))
+            dc = dd[:, cols]
+            a = dc[..., 0] ** 2 + dc[..., 1] ** 2
+            b = 2 * (dc[..., 0] * (o[0] - cx) + dc[..., 1] * (o[1] - cy))
+            c = (o[0] - cx) ** 2 + (o[1] - cy) ** 2 - r * r
+            disc = b * b - 4 * a * c
+            tq = (-b - np.sqrt(np.maximum(disc, 0))) / (2 * np.where(a > 0, a, 1))
+            z = o[2] + tq * dc[..., 2]
+            tc = t[:, cols]
+            hit = (disc > 0) & (a > 0) & (tq > 0) & (tq < tc) & (z >= 0) & (z <= h)
+            t[:, cols] = np.where(hit, tq, tc)
+            ground[:, cols] &= ~hit
+    t = t.reshape(-1)
+    ground = ground.reshape(-1)
+  keep = t < max_hit
+  if noise > 0:
+    t = t + np.random.default_rng(int(seed) + 1).normal(0.0, noise, t.shape)
+    keep &= t > 0.1
+  pw = o + t[keep, None] * d[keep]
+  pw[ground[keep] & (noise <= 0), 2] = 0.0
+  local = (pw - o) @ R                                     # R^T (p - o), row by row
+  out = np.empty((local.shape[0], 4), np.float32)
+  out[:, :3] = local
+  out[:, 3] = 0.5
+  return out
