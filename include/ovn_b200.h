@@ -97,7 +97,7 @@ int64_t     ovn_launch_count(const ovn_handle* h);
  * on the launching stream while enabled.  ovn_profile_read synchronises the device, returns the
  * accumulated milliseconds / launch count since the last read and resets them.  Names:
  * "delta_conv1", "conv2", "conv3", "corr", "project_scatter", "project_gather", "leg", "gather_rows",
- * "rows_topk". */
+ * "rows_topk", "pgo_graphs". */
 int ovn_profile_enable(ovn_handle* h, int on);
 int ovn_profile_read(ovn_handle* h, const char* kernel, double* total_ms, int64_t* launches);
 
@@ -354,6 +354,72 @@ void ovn_icp_default_params(ovn_icp_params* p);
 int ovn_icp_pairs(ovn_handle* h, const float* d_vertex, const float* d_normal, int32_t n_scans, const int32_t* d_src,
                   const int32_t* d_dst, const double* d_init, int32_t np, const ovn_icp_params* params,
                   ovn_icp_result* d_out, int32_t* d_assoc, double* d_system, void* stream);
+
+/* ---- robust pose-graph optimization of a batch of graphs (overlapnet_b200/pose_graph.py, DESIGN.md sections 4 and
+ * 7, "Pose-graph optimization").  Reference: none; the model is DESIGN section 7's.
+ * Graph g has the nodes [node_offset[g], node_offset[g + 1]) (n >= 2 of them) and the edges [edge_offset[g],
+ * edge_offset[g + 1]); edge node indices are local to the graph.  Its first n - 1 edges are the odometry chain
+ * (k, k + 1) in order; every later edge is a loop edge (a, b), a != b.  A node is a row-major float64 4x4 pose; node
+ * 0 is fixed.  Edge k measures Z_k ~ T_a^-1 T_b with the weights w_k ((omega, v) order, > 0): its residual is
+ * e = (Log(R_E), t_E) of E = Z^-1 T_a^-1 T_b, chi2 = e^T diag(w) e, and the cost is F = 1/2 sum rho(chi2) with
+ * rho(x) = x on the chain and the Geman-McClure rho(x) = phi x / (phi + x) on loops (phi = +inf: rho(x) = x).
+ * Levenberg-Marquardt on (H + lambda diag(H)) delta = -g over nodes 1 .. n-1, solved by conjugate gradients
+ * preconditioned with the exact block Cholesky factor of the damped block-diagonal plus the chain's off-diagonal
+ * blocks; each node moves as T <- [R(omega) | v] T.  One CTA runs every iteration of one graph and sums in a fixed
+ * order, so a graph's outputs have the same bits in any batch, position, call or handle.
+ * All buffers are host memory; the call copies in, runs one k_pgo_graphs launch on `stream` and copies out
+ * synchronously; the launch is profiled as "pgo_graphs".  Outputs:
+ *   out_poses [N][16]      the poses at the last accepted state
+ *   out_result [n_graphs]  status, iterations (every LM trial), accepted trials, CG iterations, F at the input and
+ *                          at the end, the final lambda and max |g| over nodes 1 .. n-1 at the end
+ *   out_chi2, out_scale [E]  chi2 and s = phi / (phi + chi2) of each edge at the end (s = 1 on the chain)
+ *   out_gradient [N][6]    (optional, NULL to skip) g of every node at the end, node 0 included
+ *   out_trace [n_graphs][max_iterations] (optional) each trial's F, lambda, accepted flag and CG iterations;
+ *                          slots past the graph's last trial hold NaN, NaN, -1, -1
+ * With max_iterations = 0 the call only evaluates F, chi2, s and g at the input.
+ * Refused with OVN_ERR_INVALID_ARG and nothing launched or written: NULL required pointers, n_graphs outside
+ * [1, OVN_PGO_MAX_GRAPHS], offsets not starting at 0 or not increasing, a graph with n < 2, more than
+ * OVN_PGO_MAX_NODES nodes or OVN_PGO_MAX_EDGES edges or fewer than n - 1 edges, a chain edge other than (k, k + 1),
+ * a node index out of range or a == b, a pose or measurement that is not finite or whose bottom row is not
+ * 0 0 0 1, a weight that is not finite or <= 0, and parameters out of their ranges (phi > 0, may be +inf;
+ * 0 < lambda_min <= lambda0 <= lambda_max, finite; tolerances finite and >= 0; max_iterations in
+ * [0, OVN_PGO_MAX_ITERATIONS_LIMIT]; max_cg_iterations in [1, OVN_PGO_MAX_CG_ITERATIONS_LIMIT]). */
+#define OVN_PGO_MAX_GRAPHS 65535
+#define OVN_PGO_MAX_NODES (1 << 20)
+#define OVN_PGO_MAX_EDGES (1 << 22)
+#define OVN_PGO_MAX_ITERATIONS_LIMIT 1000
+#define OVN_PGO_MAX_CG_ITERATIONS_LIMIT 10000
+typedef enum ovn_pgo_status {
+  OVN_PGO_CONVERGED = 0,
+  OVN_PGO_MAX_ITERATIONS = 1,
+  OVN_PGO_STALLED = 2,          /* lambda > lambda_max */
+  OVN_PGO_FAILED = 3            /* a non-positive preconditioner pivot or p^T (H + lambda D) p <= 0 */
+} ovn_pgo_status;
+typedef struct ovn_pgo_params {
+  double phi;                     /* Geman-McClure scale of the loop edges; +inf: plain least squares */
+  double lambda0, lambda_min, lambda_max;   /* LM damping, relative to diag(H) */
+  double rel_cost_tol;            /* converged: an accepted step lowers F by at most rel_cost_tol F */
+  double step_tol;                /* converged: max |delta| <= step_tol */
+  double cg_tol;                  /* CG stops at ||r|| <= cg_tol ||g|| */
+  int32_t max_iterations;         /* LM trials, 0 .. 1000 */
+  int32_t max_cg_iterations;      /* per trial, 1 .. 10000 */
+} ovn_pgo_params;
+typedef struct ovn_pgo_result {
+  double initial_cost, final_cost, lambda, max_gradient;
+  int32_t status, iterations, accepted, cg_iterations;
+} ovn_pgo_result;
+typedef struct ovn_pgo_trial {
+  double cost, lambda;            /* the trial's F and the lambda it was solved with */
+  int32_t accepted, cg_iterations;
+} ovn_pgo_trial;
+/* defaults: phi 25, lambda 1e-6 in [1e-12, 1e12], rel_cost_tol 1e-10, step_tol 1e-10, cg_tol 1e-12, 50 iterations,
+ * 2000 CG iterations (none tuned on KITTI) */
+void ovn_pgo_default_params(ovn_pgo_params* p);
+int ovn_pgo_optimize_host(ovn_handle* h, int32_t n_graphs, const int64_t* node_offset, const int64_t* edge_offset,
+                          const double* poses, const int32_t* edge_nodes, const double* edge_pose,
+                          const double* edge_weight, const ovn_pgo_params* params, double* out_poses,
+                          ovn_pgo_result* out_result, double* out_chi2, double* out_scale, double* out_gradient,
+                          ovn_pgo_trial* out_trace, void* stream);
 
 /* ---- resident bank (Infer keeps self.feature_volumes across calls, infer.py:113,184-193) ---------
  * The tensor-core heads consume fp16 / hi-lo split copies of the LEFT volumes.  Without this call

@@ -33,6 +33,7 @@ SYMBOLS = [
     'ovn_rows_topk', 'ovn_heads_prefix_topk',
     'ovn_mcl_set_map', 'ovn_mcl_init', 'ovn_mcl_predict', 'ovn_mcl_update', 'ovn_mcl_copy_particles',
     'ovn_mcl_copy_stage', 'ovn_mcl_philox', 'ovn_icp_default_params', 'ovn_icp_pairs',
+    'ovn_pgo_default_params', 'ovn_pgo_optimize_host',
 ]
 TOPK_MAX = 32     # ovn_rows_topk / ovn_heads_prefix_topk: k in [1, TOPK_MAX]
 MCL_INIT_MODES = {'global': 0, 'pose': 1}     # ovn_mcl_init_mode
@@ -40,6 +41,12 @@ MCL_STAGES = {'motion': 0, 'lookup': 1, 'loglik': 2, 'weights': 3, 'prefix': 4, 
 MCL_MAX_PARTICLES = 1 << 24
 ICP_SYSTEM_SIZE = 29      # ovn_icp_pairs: d_system [np][ICP_SYSTEM_SIZE]
 ICP_STATUS = {'converged': 0, 'max_iterations': 1, 'degenerate': 2, 'too_few_inliers': 3, 'bad_index': 4}     # ovn_icp_status
+PGO_STATUS = {'converged': 0, 'max_iterations': 1, 'stalled': 2, 'failed': 3}     # ovn_pgo_status
+PGO_MAX_GRAPHS = 65535
+PGO_MAX_NODES = 1 << 20
+PGO_MAX_EDGES = 1 << 22
+PGO_MAX_ITERATIONS = 1000
+PGO_MAX_CG_ITERATIONS = 10000
 IPC_HANDLE_BYTES = 64     # ovn_shard_create / ovn_shard_open
 HEADS_STAGES = {'o1': 0, 'x3': 1, 'dense': 2, 'centres': 3}     # ovn_heads_stage
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
@@ -75,6 +82,25 @@ class IcpParams(C.Structure):
   """ovn_icp_params"""
   _fields_ = [('d_start', C.c_double), ('d_end', C.c_double), ('gamma', C.c_double), ('cos_normal', C.c_double),
               ('eps_rot', C.c_double), ('eps_trans', C.c_double), ('iterations', C.c_int32), ('min_inliers', C.c_int32)]
+
+
+class PgoParams(C.Structure):
+  """ovn_pgo_params"""
+  _fields_ = [('phi', C.c_double), ('lambda0', C.c_double), ('lambda_min', C.c_double), ('lambda_max', C.c_double),
+              ('rel_cost_tol', C.c_double), ('step_tol', C.c_double), ('cg_tol', C.c_double),
+              ('max_iterations', C.c_int32), ('max_cg_iterations', C.c_int32)]
+
+
+class PgoResult(C.Structure):
+  """ovn_pgo_result"""
+  _fields_ = [('initial_cost', C.c_double), ('final_cost', C.c_double), ('lambda_', C.c_double),
+              ('max_gradient', C.c_double), ('status', C.c_int32), ('iterations', C.c_int32), ('accepted', C.c_int32),
+              ('cg_iterations', C.c_int32)]
+
+
+class PgoTrial(C.Structure):
+  """ovn_pgo_trial"""
+  _fields_ = [('cost', C.c_double), ('lambda_', C.c_double), ('accepted', C.c_int32), ('cg_iterations', C.c_int32)]
 
 
 ICP_RESULT_BYTES = 152    # sizeof(ovn_icp_result): pose double[16], rms double, inliers, valid, iterations, status int32
@@ -142,6 +168,10 @@ def lib():
   L.ovn_icp_default_params.argtypes = [C.POINTER(IcpParams)]
   L.ovn_icp_default_params.restype = None
   L.ovn_icp_pairs.argtypes = [vp, vp, vp, i32, vp, vp, vp, i32, C.POINTER(IcpParams), vp, vp, vp, vp]
+  L.ovn_pgo_default_params.argtypes = [C.POINTER(PgoParams)]
+  L.ovn_pgo_default_params.restype = None
+  L.ovn_pgo_optimize_host.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, C.POINTER(PgoParams), vp, vp, vp, vp, vp, vp,
+                                      vp]
   L.ovn_bank_release.argtypes = [vp, vp]
   L.ovn_check.argtypes = [vp, vp]
   L.ovn_set_feature_center.argtypes = [vp, vp]

@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libovn_b200.so')
 SOURCES = ['api.cu', 'projection.cu', 'gt_overlap.cu', 'network_fp32.cu', 'network_tc.cu', 'bank_shard.cu', 'rows_topk.cu',
-           'mcl.cu', 'icp.cu']
+           'mcl.cu', 'icp.cu', 'pose_graph.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC'] + os.environ.get('OVN_NVCC_EXTRA', '').split()
 

@@ -342,7 +342,7 @@ int ovn_profile_read(ovn_handle* h, const char* kernel, double* total_ms, int64_
   DeviceGuard guard(h);
   if (!kernel || !total_ms || !launches) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_profile_read: NULL argument");
   static const char* names[kProfKinds] = {"delta_conv1", "conv2", "conv3", "corr", "project_scatter",
-                                          "project_gather", "leg", "gather_rows", "rows_topk"};
+                                          "project_gather", "leg", "gather_rows", "rows_topk", "pgo_graphs"};
   int kind = -1;
   for (int i = 0; i < kProfKinds; ++i) if (strcmp(kernel, names[i]) == 0) kind = i;
   if (kind < 0) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_profile_read: unknown kernel '%s'", kernel);
@@ -936,6 +936,84 @@ int ovn_icp_pairs(ovn_handle* h, const float* d_vertex, const float* d_normal, i
       OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_icp_pairs: d_init[%lld][%lld] is not finite", (long long)(i / 16),
                   (long long)(i % 16));
   return icp_pairs(h, d_vertex, d_normal, n_scans, d_src, d_dst, d_init, np, p, d_out, d_assoc, d_system, s);
+}
+
+// ---- robust pose-graph optimization (DESIGN section 7, "Pose-graph optimization") -------------------------------
+void ovn_pgo_default_params(ovn_pgo_params* p) {
+  if (!p) return;
+  p->phi = 25.0;
+  p->lambda0 = 1e-6;
+  p->lambda_min = 1e-12;
+  p->lambda_max = 1e12;
+  p->rel_cost_tol = 1e-10;
+  p->step_tol = 1e-10;
+  p->cg_tol = 1e-12;
+  p->max_iterations = 50;
+  p->max_cg_iterations = 2000;
+}
+
+// a finite row-major 4x4 whose bottom row is 0 0 0 1
+static bool rigid_rows(const double* T) {
+  for (int i = 0; i < 16; ++i)
+    if (!std::isfinite(T[i])) return false;
+  return T[12] == 0.0 && T[13] == 0.0 && T[14] == 0.0 && T[15] == 1.0;
+}
+
+int ovn_pgo_optimize_host(ovn_handle* h, int32_t n_graphs, const int64_t* node_offset, const int64_t* edge_offset,
+                          const double* poses, const int32_t* edge_nodes, const double* edge_pose,
+                          const double* edge_weight, const ovn_pgo_params* params, double* out_poses,
+                          ovn_pgo_result* out_result, double* out_chi2, double* out_scale, double* out_gradient,
+                          ovn_pgo_trial* out_trace, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, params && node_offset && edge_offset && poses && edge_nodes && edge_pose && edge_weight && out_poses &&
+                 out_result && out_chi2 && out_scale, "NULL pointer");
+  REQUIRE(h, n_graphs >= 1 && n_graphs <= OVN_PGO_MAX_GRAPHS, "n_graphs must be in [1, 65535]");
+  const ovn_pgo_params& p = *params;
+  REQUIRE(h, p.phi > 0.0 && !std::isnan(p.phi), "phi must be > 0 (+inf: plain least squares)");
+  REQUIRE(h, std::isfinite(p.lambda0) && std::isfinite(p.lambda_min) && std::isfinite(p.lambda_max) &&
+                 p.lambda_min > 0.0 && p.lambda_min <= p.lambda0 && p.lambda0 <= p.lambda_max,
+          "0 < lambda_min <= lambda0 <= lambda_max, all finite");
+  REQUIRE(h, std::isfinite(p.rel_cost_tol) && std::isfinite(p.step_tol) && std::isfinite(p.cg_tol) &&
+                 p.rel_cost_tol >= 0.0 && p.step_tol >= 0.0 && p.cg_tol >= 0.0,
+          "rel_cost_tol, step_tol and cg_tol must be finite and >= 0");
+  REQUIRE(h, p.max_iterations >= 0 && p.max_iterations <= OVN_PGO_MAX_ITERATIONS_LIMIT,
+          "max_iterations must be in [0, 1000]");
+  REQUIRE(h, p.max_cg_iterations >= 1 && p.max_cg_iterations <= OVN_PGO_MAX_CG_ITERATIONS_LIMIT,
+          "max_cg_iterations must be in [1, 10000]");
+  REQUIRE(h, node_offset[0] == 0 && edge_offset[0] == 0, "node_offset[0] and edge_offset[0] must be 0");
+  for (int g = 0; g < n_graphs; ++g) {
+    const int64_t n = node_offset[g + 1] - node_offset[g], ne = edge_offset[g + 1] - edge_offset[g];
+    if (n < 2 || n > OVN_PGO_MAX_NODES)
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_pgo_optimize_host: graph %d has %lld nodes (2 .. %d)", g, (long long)n,
+                  OVN_PGO_MAX_NODES);
+    if (ne < n - 1 || ne > OVN_PGO_MAX_EDGES)
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_pgo_optimize_host: graph %d has %lld edges (n - 1 .. %d)", g,
+                  (long long)ne, OVN_PGO_MAX_EDGES);
+    for (int64_t i = node_offset[g]; i < node_offset[g + 1]; ++i)
+      if (!rigid_rows(poses + 16 * i))
+        OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_pgo_optimize_host: pose %lld of graph %d is not finite or its bottom "
+                    "row is not 0 0 0 1", (long long)(i - node_offset[g]), g);
+    for (int64_t k = edge_offset[g]; k < edge_offset[g + 1]; ++k) {
+      const int64_t l = k - edge_offset[g];
+      const int32_t a = edge_nodes[2 * k], b = edge_nodes[2 * k + 1];
+      if (l < n - 1 && (a != l || b != l + 1))
+        OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_pgo_optimize_host: edge %lld of graph %d is (%d, %d), but the first "
+                    "n - 1 edges are the chain (k, k + 1)", (long long)l, g, a, b);
+      if (a < 0 || a >= n || b < 0 || b >= n || a == b)
+        OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_pgo_optimize_host: edge %lld of graph %d is (%d, %d): a node is "
+                    "outside [0, %lld) or a == b", (long long)l, g, a, b, (long long)n);
+      if (!rigid_rows(edge_pose + 16 * k))
+        OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_pgo_optimize_host: the measurement of edge %lld of graph %d is not "
+                    "finite or its bottom row is not 0 0 0 1", (long long)l, g);
+      for (int t = 0; t < 6; ++t)
+        if (!(std::isfinite(edge_weight[6 * k + t]) && edge_weight[6 * k + t] > 0.0))
+          OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_pgo_optimize_host: weight %d of edge %lld of graph %d is not finite "
+                      "and > 0", t, (long long)l, g);
+    }
+  }
+  return pgo_graphs(h, n_graphs, node_offset, edge_offset, poses, edge_nodes, edge_pose, edge_weight, p, out_poses,
+                    out_result, out_chi2, out_scale, out_gradient, out_trace, (cudaStream_t)stream);
 }
 
 // ---- training precision ---------------------------------------------------------------------------

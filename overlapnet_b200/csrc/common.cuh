@@ -69,7 +69,7 @@ static_assert(sizeof(float) == sizeof(int32_t), "the three staging arrays are 4 
 constexpr int kFeatC = 128;           // leg output channels (generateNet.py:214)
 constexpr int kMaxLegLayers = 12;
 enum ProfKind { PROF_DELTA = 0, PROF_CONV2, PROF_CONV3, PROF_CORR, PROF_SCATTER, PROF_GATHER, PROF_LEG, PROF_GATHER_ROWS,
-                PROF_ROWS_TOPK, kProfKinds };
+                PROF_ROWS_TOPK, PROF_PGO, kProfKinds };
 
 // The one owner of another process's shard mapped by ovn_shard_open (cudaIpcOpenMemHandle); unmaps it on
 // destruction.  Move-only, like Buffer.
@@ -272,6 +272,7 @@ struct ovn_handle {
   std::vector<ovn::Buffer<uint8_t>> own_shards;
   std::vector<ovn::IpcMapping> open_shards;
   ovn::McState mcl;                          // ovn_mcl_*: map and particles, allocated by ovn_mcl_set_map / ovn_mcl_init
+  ovn::Buffer<uint8_t> d_pgo;                // ovn_pgo_optimize_host: one call's inputs and workspace, grown on use
   cudaStream_t own_stream = nullptr;
   // per-kernel profiling (ovn_profile_enable / ovn_profile_read)
   bool profiling = false;
@@ -487,6 +488,13 @@ int mcl_philox(ovn_handle* h, uint64_t seed, const uint32_t* d_ctr, int n, uint3
 int icp_pairs(ovn_handle* h, const float* d_vertex, const float* d_normal, int n_scans, const int32_t* d_src,
               const int32_t* d_dst, const double* d_init, int np, const ovn_icp_params& prm, ovn_icp_result* d_out,
               int32_t* d_assoc, double* d_system, cudaStream_t s);
+
+// pose-graph optimization of n_graphs graphs (pose_graph.cu), one k_pgo_graphs launch between the host copies; the
+// caller has checked every argument
+int pgo_graphs(ovn_handle* h, int n_graphs, const int64_t* node_off, const int64_t* edge_off, const double* poses,
+               const int32_t* edge_nodes, const double* edge_pose, const double* edge_weight,
+               const ovn_pgo_params& prm, double* out_poses, ovn_pgo_result* out_result, double* out_chi2,
+               double* out_scale, double* out_gradient, ovn_pgo_trial* out_trace, cudaStream_t s);
 
 int corr_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* left,
                       const int32_t* right, int np, int32_t* d_yaw, float* d_corr, cudaStream_t s);

@@ -6,6 +6,7 @@
 // pair's position in it or the launch, so a pair's result has the same bits in any call.  The association uses the
 // ground-truth generator's float64 bin (range_bin.cuh), so a point lands in the pixel the float64 oracle gives it.
 #include "range_bin.cuh"
+#include "se3.cuh"
 #include <math.h>
 #include <math_constants.h>
 
@@ -64,23 +65,8 @@ __device__ int icp_solve_update(const double* S, double* T, double dk, const ovn
     for (int k = i + 1; k < 6; ++k) t -= L[k][i] * d[k];
     d[i] = t / L[i][i];
   }
-  // R(omega) = I + sin(th) K + (1 - cos(th)) K^2, K the cross-product matrix of the unit axis
+  left_update(d, T);                                   // Rodrigues and T <- [R(omega) | v] T (se3.cuh)
   const double th = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-  double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-  if (th > 0.0) {
-    const double kx = d[0] / th, ky = d[1] / th, kz = d[2] / th, s = sin(th), c1 = 1.0 - cos(th);
-    const double K[9] = {0, -kz, ky, kz, 0, -kx, -ky, kx, 0};
-    for (int i = 0; i < 3; ++i)
-      for (int j = 0; j < 3; ++j) {
-        const double kk = K[3 * i] * K[j] + K[3 * i + 1] * K[3 + j] + K[3 * i + 2] * K[6 + j];
-        R[3 * i + j] += s * K[3 * i + j] + c1 * kk;
-      }
-  }
-  double N[12];
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 4; ++j)
-      N[4 * i + j] = R[3 * i] * T[j] + R[3 * i + 1] * T[4 + j] + R[3 * i + 2] * T[8 + j] + (j == 3 ? d[3 + i] : 0.0);
-  for (int i = 0; i < 12; ++i) T[i] = N[i];
   const double tn = sqrt(d[3] * d[3] + d[4] * d[4] + d[5] * d[5]);
   if (dk == prm.d_end && th < prm.eps_rot && tn < prm.eps_trans) return OVN_ICP_CONVERGED;
   return -1;

@@ -583,6 +583,67 @@ class Engine:
       out.update(assoc=assoc, system=system)
     return out
 
+  def pose_graph(self, graphs, params=None, want_gradient=False, want_trace=False):
+    """ovn_pgo_optimize_host: robust pose-graph optimization of ``graphs`` in one launch (one CTA per graph).  Each
+    graph is a dict of poses [n, 4, 4], edges [E, 2] (the chain (k, k + 1) first, then the loops), measurements
+    [E, 4, 4] (Z ~ T_a^-1 T_b) and weights [E, 6] ((omega, v) order), as pose_graph.chain_graph builds it; every
+    graph is checked by pose_graph.check_graph first.  ``params``: a dict overriding pgo_default_params().  Returns
+    one dict of host arrays per graph: poses, chi2 and scale per edge, status (ovn_pgo_status), iterations,
+    accepted, cg_iterations, initial_cost, final_cost, lambda, max_gradient, and with ``want_gradient`` gradient
+    [n, 6], with ``want_trace`` trace (cost, lambda, accepted, cg_iterations of each trial run)."""
+    from .pose_graph import check_graph, default_params
+    prm = default_params(params)
+    graphs = [check_graph(g) for g in graphs]
+    if not 1 <= len(graphs) <= _cabi.PGO_MAX_GRAPHS:
+      raise ValueError('pose_graph: 1 .. %d graphs per call, got %d' % (_cabi.PGO_MAX_GRAPHS, len(graphs)))
+    node_off = np.concatenate([[0], np.cumsum([g['poses'].shape[0] for g in graphs])]).astype(np.int64)
+    edge_off = np.concatenate([[0], np.cumsum([g['edges'].shape[0] for g in graphs])]).astype(np.int64)
+    out = self.pose_graph_raw(node_off, edge_off, np.concatenate([g['poses'] for g in graphs]),
+                              np.concatenate([g['edges'] for g in graphs]),
+                              np.concatenate([g['measurements'] for g in graphs]),
+                              np.concatenate([g['weights'] for g in graphs]), prm, want_gradient, want_trace)
+    check(self._h, out.pop('rc'), 'ovn_pgo_optimize_host')
+    res = []
+    for g in range(len(graphs)):
+      n0, n1, e0, e1 = node_off[g], node_off[g + 1], edge_off[g], edge_off[g + 1]
+      r = out['result'][g]
+      d = {'poses': out['poses'][n0:n1], 'chi2': out['chi2'][e0:e1], 'scale': out['scale'][e0:e1],
+           'status': int(r['status']), 'iterations': int(r['iterations']), 'accepted': int(r['accepted']),
+           'cg_iterations': int(r['cg_iterations']), 'initial_cost': float(r['initial_cost']),
+           'final_cost': float(r['final_cost']), 'lambda': float(r['lambda']), 'max_gradient': float(r['max_gradient'])}
+      if want_gradient:
+        d['gradient'] = out['gradient'][n0:n1]
+      if want_trace:
+        t = out['trace'][g, :d['iterations']]
+        d['trace'] = {k: t[k].copy() for k in ('cost', 'lambda', 'accepted', 'cg_iterations')}
+      res.append(d)
+    return res
+
+  def pose_graph_raw(self, node_off, edge_off, poses, edges, measurements, weights, params, want_gradient=False,
+                     want_trace=False, outputs=None):
+    """One ovn_pgo_optimize_host call on packed host arrays, unchecked (the library checks them).  ``params``: a
+    PgoParams.  ``outputs``: preallocated output arrays to write into (a dict as returned).  Returns the output
+    arrays and the status code ``rc``; nothing raises here."""
+    node_off = np.ascontiguousarray(node_off, np.int64)
+    edge_off = np.ascontiguousarray(edge_off, np.int64)
+    poses = np.ascontiguousarray(poses, np.float64).reshape(-1, 4, 4)
+    edges = np.ascontiguousarray(edges, np.int32).reshape(-1, 2)
+    measurements = np.ascontiguousarray(measurements, np.float64).reshape(-1, 4, 4)
+    weights = np.ascontiguousarray(weights, np.float64).reshape(-1, 6)
+    G, N, E = node_off.size - 1, poses.shape[0], edges.shape[0]
+    res_dt = np.dtype([('initial_cost', 'f8'), ('final_cost', 'f8'), ('lambda', 'f8'), ('max_gradient', 'f8'),
+                       ('status', 'i4'), ('iterations', 'i4'), ('accepted', 'i4'), ('cg_iterations', 'i4')])
+    tr_dt = np.dtype([('cost', 'f8'), ('lambda', 'f8'), ('accepted', 'i4'), ('cg_iterations', 'i4')])
+    out = outputs if outputs is not None else {
+        'poses': np.empty((N, 4, 4)), 'result': np.zeros(max(G, 0), res_dt), 'chi2': np.empty(E),
+        'scale': np.empty(E), 'gradient': np.empty((N, 6)) if want_gradient else None,
+        'trace': np.empty((max(G, 0), params.max_iterations), tr_dt) if want_trace else None}
+    p = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else C.c_void_p(0)  # noqa: E731
+    rc = lib().ovn_pgo_optimize_host(self._h, G, p(node_off), p(edge_off), p(poses), p(edges), p(measurements),
+                                     p(weights), C.byref(params), p(out['poses']), p(out['result']), p(out['chi2']),
+                                     p(out['scale']), p(out['gradient']), p(out['trace']), self._stream())
+    return dict(out, rc=rc)
+
   def bank_prepare(self, bank, first=0, count=None):
     """Keep the tensor-core operand copies of bank rows [first, first+count) resident: later heads
     calls on this same tensor skip the per-call conversion (ovn_bank_prepare)."""

@@ -2,7 +2,7 @@
 paper, with the candidate rules of the reference's demo 3 (demo/demo3_lcd.py).
 
   python -m overlapnet_b200.lcd_eval [config/demo.yml] [--top-k K] [--exclude-frames 100] [--exclude-distance 50]
-                                     [--gt-overlap 0.3] [--register [--min-inlier-fraction 0.3]]
+                                     [--gt-overlap 0.3] [--register [--min-inlier-fraction 0.3]] [--close-loops]
   torchrun --nproc_per_node G -m overlapnet_b200.lcd_eval ...            (the rows split over G GPUs)
 
 The protocol (DESIGN.md section 7):
@@ -21,6 +21,11 @@ The protocol (DESIGN.md section 7):
   register    (opt-in) each top record is registered by point-to-plane ICP on the GPU (registration.register),
               LEFT = j*_i, RIGHT = i, once from the heads' yaw seed and once from the identity, against the
               ground-truth pose T_j*^-1 T_i; a success is a translation error < 0.5 m and a rotation error < 2 deg.
+  close loops (opt-in, implies register) the odometry steps (i - 1, i) are registered by ICP from the identity, and
+              five pose graphs over them (PGO_GRAPHS: no loops, verified, s >= F1max threshold, every top record,
+              the correct records) are optimized in one launch (pose_graph.py); ground-truth poses only select the
+              correct records and score the trajectories.  Untested on KITTI; scans about 1 m apart fit ICP's 2 m
+              start distance.
 
 Scans are encoded from the raw ``.bin`` files (Infer.encode_clouds); configs with class probabilities are
 refused, since they would need a ``.label`` file per scan.  Results go to ``<experiments_path>/<testname>`` of
@@ -259,6 +264,114 @@ def registration_summary(top_overlap, top_index, gt_top_overlap, gt_best, tp_row
   return out
 
 
+# ---- closing the loops: ICP odometry and pose graphs ------------------------------------------------------------
+PGO_GRAPHS = ('odometry', 'verified', 'f1_max', 'all_records', 'true_loops')   # the graph axis of the pgo_* arrays
+VERIFIED_SCORE = 0.3           # a verified loop: s_i > VERIFIED_SCORE and the yaw seed's inlier fraction is high enough
+
+
+def register_odometry(engine, clouds, poses, rows, params=None):
+  """The odometry steps of ``rows``: each row i >= 1 registers (LEFT = i - 1, RIGHT = i) from the identity, in one
+  registration.register call.  Returns pose [rows, 4, 4] (T_{i-1}^-1 T_i estimated), status [rows] int32 and error
+  [rows, 2] (metres, degrees against the ground-truth step); row 0 holds NaN and status -1."""
+  from .registration import pose_error, register
+  rows = np.asarray(rows, np.int64)
+  out = {'pose': np.full((rows.size, 4, 4), np.nan), 'status': np.full(rows.size, -1, np.int32),
+         'error': np.full((rows.size, 2), np.nan)}
+  live = np.flatnonzero(rows >= 1)
+  if live.size:
+    i = rows[live]
+    res = register(engine, clouds, i - 1, i, np.broadcast_to(np.eye(4), (live.size, 4, 4)), params)
+    t, r = pose_error(res['pose'], np.linalg.solve(poses[i - 1], poses[i]))
+    out['pose'][live] = res['pose']
+    out['status'][live] = res['status']
+    out['error'][live] = np.stack([t, np.degrees(r)], -1)
+  return out
+
+
+def loop_sets(top_overlap, top_index, gt_top_overlap, inlier_fraction, f1_threshold, gt_overlap=0.3,
+              min_inlier_fraction=0.3):
+  """The loop edges of each graph of PGO_GRAPHS, as bool masks over the rows (a row's loop is its top record):
+  none; verified (s_i > 0.3 and the yaw seed's inlier fraction >= min_inlier_fraction); s_i >= the F1max threshold;
+  every top record; the correct records by ground truth (the upper bound)."""
+  top_index = np.asarray(top_index)
+  has = top_index[:, 0] >= 0
+  s = np.asarray(top_overlap, np.float64)[:, 0]
+  f1 = has & (s >= f1_threshold) if np.isfinite(f1_threshold) else np.zeros_like(has)
+  return {'odometry': np.zeros_like(has),
+          'verified': has & (s > VERIFIED_SCORE) & (np.asarray(inlier_fraction, np.float64)[:, 0] >= min_inlier_fraction),
+          'f1_max': f1, 'all_records': has,
+          'true_loops': has & (np.asarray(gt_top_overlap, np.float64)[:, 0] > gt_overlap)}
+
+
+def loop_graphs(odometry_pose, top_index, loop_pose, masks):
+  """One pose graph per mask (PGO_GRAPHS order) over every scan: the chain measures odometry_pose[1:], the loops
+  (j*_i, i) of the masked rows measure loop_pose[i] (the yaw-seeded registration), with the default weights.  The
+  initial poses compose the odometry from the identity; no ground-truth pose enters a graph."""
+  from .pose_graph import chain_graph
+  rows_all = np.arange(len(top_index))
+  graphs = []
+  for name in PGO_GRAPHS:
+    rows = rows_all[masks[name]]
+    edges = np.stack([np.asarray(top_index)[rows, 0], rows], 1)
+    graphs.append(chain_graph(odometry_pose[1:], (edges, loop_pose[rows])))
+  return graphs
+
+
+def close_loops_graphs(engine, odometry_pose, top_index, loop_pose, masks):
+  """Optimize the loop_graphs of ``masks`` in one Engine.pose_graph call.  Returns the pgo_* arrays: poses [G, n, 4, 4],
+  loop_mask / loop_scale / loop_chi2 [G, rows] (NaN off-graph), status / iterations [G], cost [G, 2] (F before
+  and after)."""
+  from .pose_graph import optimize
+  graphs = loop_graphs(odometry_pose, top_index, loop_pose, masks)
+  res = optimize(engine, graphs)
+  n = odometry_pose.shape[0]
+  G = len(graphs)
+  out = {'poses': np.stack([r['poses'] for r in res]), 'loop_mask': np.stack([masks[k] for k in PGO_GRAPHS]),
+         'loop_scale': np.full((G, n), np.nan), 'loop_chi2': np.full((G, n), np.nan),
+         'status': np.array([r['status'] for r in res], np.int32),
+         'iterations': np.array([r['iterations'] for r in res], np.int32),
+         'cost': np.array([[r['initial_cost'], r['final_cost']] for r in res])}
+  for g, r in enumerate(res):
+    rows = np.flatnonzero(out['loop_mask'][g])
+    out['loop_scale'][g, rows] = r['scale'][n - 1:]
+    out['loop_chi2'][g, rows] = r['chi2'][n - 1:]
+  return out
+
+
+def pose_graph_summary(pgo, odometry, poses, gt_top_overlap, gt_overlap=0.3):
+  """The ``pose_graph`` section of the summary: the odometry steps' errors and end states, and per graph the loops
+  (correct ones), the kept loops (s >= 1/2) split into correct and incorrect, the trajectory error before (the
+  composed odometry) and after, its status and iterations."""
+  from ._cabi import ICP_STATUS, PGO_STATUS
+  from .pose_graph import KEEP_SCALE, trajectory_error
+  steps = odometry['status'] >= 0
+  e = odometry['error'][steps]
+  st = odometry['status'][steps]
+  n = poses.shape[0]
+  before = np.empty((n, 4, 4))
+  before[0] = np.eye(4)
+  for k in range(1, n):
+    before[k] = before[k - 1] @ odometry['pose'][k]
+  correct = np.asarray(gt_top_overlap, np.float64)[:, 0] > gt_overlap
+  names = {v: k for k, v in PGO_STATUS.items()}
+  out = {'odometry': {'steps': int(steps.sum()),
+                      'median_error_translation_m': float(np.median(e[:, 0])) if e.size else float('nan'),
+                      'max_error_translation_m': float(np.max(e[:, 0])) if e.size else float('nan'),
+                      'median_error_rotation_deg': float(np.median(e[:, 1])) if e.size else float('nan'),
+                      'max_error_rotation_deg': float(np.max(e[:, 1])) if e.size else float('nan'),
+                      'degenerate': int((st == ICP_STATUS['degenerate']).sum()),
+                      'too_few_inliers': int((st == ICP_STATUS['too_few_inliers']).sum())},
+         'error_before': trajectory_error(before, poses), 'keep_scale': KEEP_SCALE, 'graphs': {}}
+  for g, name in enumerate(PGO_GRAPHS):
+    m = pgo['loop_mask'][g]
+    kept = m & (pgo['loop_scale'][g] >= KEEP_SCALE)
+    out['graphs'][name] = {'loops': int(m.sum()), 'correct_loops': int((m & correct).sum()),
+                           'kept_correct': int((kept & correct).sum()), 'kept_incorrect': int((kept & ~correct).sum()),
+                           'error_after': trajectory_error(pgo['poses'][g], poses),
+                           'status': names[int(pgo['status'][g])], 'iterations': int(pgo['iterations'][g])}
+  return out
+
+
 # ---- the driver ---------------------------------------------------------------------------------------------
 def _dist():
   dist = torch.distributed
@@ -310,7 +423,7 @@ def save_npz(path, arrays):
 
 
 def evaluate_clouds(infer, clouds, poses, top_k=5, exclude_frames=100, exclude_distance=50, gt_overlap=0.3,
-                    out_dir=None, register=False, min_inlier_fraction=0.3):
+                    out_dir=None, register=False, min_inlier_fraction=0.3, close_loops=False):
   """Evaluate loop closure over a sequence: ``clouds`` (N, 4) float32 arrays or zero-argument callables returning
   one, ``poses`` (n, 4, 4) LiDAR-frame poses, ``infer`` an overlapnet_b200.Infer.  In a process group every rank
   encodes a contiguous share of the scans, the bank is all-gathered, every rank scores and labels the rows of an
@@ -319,7 +432,9 @@ def evaluate_clouds(infer, clouds, poses, top_k=5, exclude_frames=100, exclude_d
   lcd_summary.json to ``out_dir`` when given.  With ``register`` each rank also registers its rows' top records
   (register_records) and the results gain the registration_* arrays and a ``registration`` summary section
   (registration_summary, with ``min_inlier_fraction``); without it nothing differs from an evaluation without
-  registration."""
+  registration.  ``close_loops`` implies ``register``: each rank also registers the odometry steps (i - 1, i) of its
+  rows (register_odometry), and rank 0 optimizes the five loop_graphs in one pose-graph call (close_loops_graphs);
+  the results gain the odometry_* and pgo_* arrays and a ``pose_graph`` summary section (pose_graph_summary)."""
   if not 1 <= int(top_k) <= TOPK_MAX:
     raise ValueError('top_k must be in [1, %d], got %r' % (TOPK_MAX, top_k))
   top_k = int(top_k)
@@ -327,6 +442,7 @@ def evaluate_clouds(infer, clouds, poses, top_k=5, exclude_frames=100, exclude_d
   n = len(clouds)
   if poses.shape != (n, 4, 4):
     raise ValueError('poses has shape %s, expected (%d, 4, 4)' % (poses.shape, n))
+  register = register or close_loops
   dist, rank, world = _dist()
   eng = infer._engine
   c = past_prefix(poses[:, :2, 3], exclude_frames, exclude_distance)
@@ -345,6 +461,10 @@ def evaluate_clouds(infer, clouds, poses, top_k=5, exclude_frames=100, exclude_d
     reg = register_records(eng, clouds, poses, np.arange(r_lo, r_hi), top_idx, top_yaw)
     reg_keys = sorted(reg)
     part += tuple(reg[key] for key in reg_keys)
+  if close_loops:
+    odo = register_odometry(eng, clouds, poses, np.arange(r_lo, r_hi))
+    odo_keys = sorted(odo)
+    part += tuple(odo[key] for key in odo_keys)
   if world > 1:
     parts = [None] * world if rank == 0 else None
     dist.gather_object(part, parts, dst=0)
@@ -367,10 +487,17 @@ def evaluate_clouds(infer, clouds, poses, top_k=5, exclude_frames=100, exclude_d
              'true_positive_rows': tp_rows, 'yaw_error': d_yaw}
   results.update({'curve_' + key: v for key, v in curve.items()})
   if register:
-    reg = dict(zip(reg_keys, part[6:]))
+    reg = dict(zip(reg_keys, part[6:6 + len(reg_keys)]))
     results.update({'registration_' + key: v for key, v in reg.items()})
     summary['registration'] = registration_summary(top_ov, top_idx, gt_top, gt_best, tp_rows, reg['error'],
                                                    reg['inlier_fraction'], gt_overlap, min_inlier_fraction)
+  if close_loops:
+    odo = dict(zip(odo_keys, part[6 + len(reg_keys):]))
+    results.update({'odometry_' + key: v for key, v in odo.items()})
+    masks = loop_sets(top_ov, top_idx, gt_top, reg['inlier_fraction'], t, gt_overlap, min_inlier_fraction)
+    pgo = close_loops_graphs(eng, odo['pose'], top_idx, reg['pose'][:, 0], masks)
+    results.update({'pgo_' + key: v for key, v in pgo.items()})
+    summary['pose_graph'] = pose_graph_summary(pgo, odo, poses, gt_top, gt_overlap)
   if out_dir is not None:
     os.makedirs(out_dir, exist_ok=True)
     save_npz(os.path.join(out_dir, 'lcd_results.npz'), results)
@@ -391,6 +518,9 @@ def parse_args(argv):
   p.add_argument('--precision', default='f16_tc', choices=('f16_tc', 'fp32'))
   p.add_argument('--register', action='store_true',
                  help='register each top record by ICP on the GPU, from the yaw seed and from the identity')
+  p.add_argument('--close-loops', action='store_true',
+                 help='also register the odometry by ICP and optimize pose graphs over five loop sets (implies '
+                      '--register)')
   p.add_argument('--min-inlier-fraction', type=float, default=0.3,
                  help='with --register: the inlier fraction a verified loop reaches (default 0.3)')
   args = p.parse_args(argv)
@@ -398,6 +528,7 @@ def parse_args(argv):
     p.error('--top-k must be in [1, %d], got %d' % (TOPK_MAX, args.top_k))
   if not 0.0 <= args.min_inlier_fraction <= 1.0:
     p.error('--min-inlier-fraction must be in [0, 1], got %g' % args.min_inlier_fraction)
+  args.register = args.register or args.close_loops
   return args
 
 
@@ -438,7 +569,7 @@ def main(argv=None):
   infer = Infer(net, precision=args.precision)
   out_dir = os.path.join(net.get('experiments_path', '/tmp'), net.get('testname', 'experiment_test'))
   res = evaluate_clouds(infer, clouds, poses, args.top_k, args.exclude_frames, args.exclude_distance,
-                        args.gt_overlap, out_dir, args.register, args.min_inlier_fraction)
+                        args.gt_overlap, out_dir, args.register, args.min_inlier_fraction, args.close_loops)
   if res is not None:
     s = res[0]
     logger.info('Loop closure over %d scans, %d queries, %d positive (ground-truth overlap > %g), %d pairs scored',
@@ -459,6 +590,21 @@ def main(argv=None):
       logger.info('  precision / recall at > %g with inlier fraction >= %g: %f / %f', s['operating_point'],
                   r['min_inlier_fraction'], r['precision_at_operating_point_verified'],
                   r['recall_at_operating_point_verified'])
+    if 'pose_graph' in s:
+      pgs = s['pose_graph']
+      o = pgs['odometry']
+      logger.info('  odometry: %d ICP steps, median error %f m / %f deg, max %f m / %f deg, %d degenerate, %d with '
+                  'too few inliers', o['steps'], o['median_error_translation_m'], o['median_error_rotation_deg'],
+                  o['max_error_translation_m'], o['max_error_rotation_deg'], o['degenerate'], o['too_few_inliers'])
+      b = pgs['error_before']
+      logger.info('  trajectory error of the odometry: RMSE %f m / %f deg, max %f m / %f deg',
+                  b['translation_rmse_m'], b['rotation_rmse_deg'], b['translation_max_m'], b['rotation_max_deg'])
+      for name, gs in pgs['graphs'].items():
+        a = gs['error_after']
+        logger.info('  pose graph %-11s %4d loops (%d correct), kept %d correct / %d incorrect: RMSE %f m / %f deg, '
+                    'max %f m / %f deg, %s after %d iterations', name, gs['loops'], gs['correct_loops'],
+                    gs['kept_correct'], gs['kept_incorrect'], a['translation_rmse_m'], a['rotation_rmse_deg'],
+                    a['translation_max_m'], a['rotation_max_deg'], gs['status'], gs['iterations'])
     logger.info('  written to %s', out_dir)
   if world > 1:
     torch.distributed.barrier()

@@ -189,3 +189,53 @@ def street_scene_cloud(pose, seed=0, noise=0.0, n_azimuth=1800, max_hit=80.0, gr
   out[:, :3] = local
   out[:, 3] = 0.5
   return out
+
+
+def _rotation(axis_angle):
+  w = np.asarray(axis_angle, np.float64)
+  th = np.linalg.norm(w)
+  if th == 0:
+    return np.eye(3)
+  k = w / th
+  K = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
+  return np.eye(3) + np.sin(th) * K + (1 - np.cos(th)) * K @ K
+
+
+def pose_graph_scene(n, n_loops, seed=0, n_false=0, step=1.0, init_noise=(0.02, 0.005), min_gap=10):
+  """A seeded pose graph of a random drive: ground-truth poses [n, 4, 4] (mostly yaw turns, ``step`` metres per
+  node), exact odometry T_k^-1 T_{k+1}, ``n_loops`` exact loop edges (a, b) with |a - b| >= ``min_gap``, then
+  ``n_false`` false loops with random measurements (any rotation, up to 20 m).  The initial poses compose the
+  odometry with increments perturbed by N(0, init_noise) (degrees, metres) per axis.  Returns (graph, gt) with the
+  graph as pose_graph.chain_graph builds it (default weights) and its initial poses replaced."""
+  from .pose_graph import chain_graph
+  rng = np.random.default_rng(seed)
+  gt = np.empty((n, 4, 4))
+  gt[0] = np.eye(4)
+  for k in range(1, n):
+    D = np.eye(4)
+    D[:3, :3] = _rotation([rng.normal(0, 0.002), rng.normal(0, 0.002), rng.normal(0, 0.05)])
+    D[:3, 3] = [step, rng.normal(0, 0.02), rng.normal(0, 0.01)]
+    gt[k] = gt[k - 1] @ D
+  odo = np.linalg.solve(gt[:-1], gt[1:])
+  pairs = []
+  while len(pairs) < n_loops + n_false:
+    a, b = sorted(rng.integers(0, n, 2))
+    if b - a >= min_gap:
+      pairs.append((a, b))
+  pairs = np.array(pairs, np.int64).reshape(-1, 2)
+  Z = np.linalg.solve(gt[pairs[:, 0]], gt[pairs[:, 1]]) if len(pairs) else np.zeros((0, 4, 4))
+  for m in range(n_loops, n_loops + n_false):
+    Z[m] = np.eye(4)
+    Z[m, :3, :3] = _rotation(rng.normal(0, 1, 3) / np.sqrt(3) * rng.uniform(0, np.pi))
+    Z[m, :3, 3] = rng.uniform(-20, 20, 3)
+  g = chain_graph(odo, (pairs, Z))
+  T = np.empty((n, 4, 4))
+  T[0] = gt[0]
+  r, t = np.deg2rad(init_noise[0]), init_noise[1]
+  for k in range(n - 1):
+    D = np.eye(4)
+    D[:3, :3] = _rotation(rng.normal(0, r, 3))
+    D[:3, 3] = rng.normal(0, t, 3)
+    T[k + 1] = T[k] @ odo[k] @ D
+  g['poses'] = T
+  return g, gt
