@@ -97,7 +97,7 @@ int64_t     ovn_launch_count(const ovn_handle* h);
  * on the launching stream while enabled.  ovn_profile_read synchronises the device, returns the
  * accumulated milliseconds / launch count since the last read and resets them.  Names:
  * "delta_conv1", "conv2", "conv3", "corr", "project_scatter", "project_gather", "leg", "gather_rows",
- * "rows_topk", "pgo_graphs". */
+ * "rows_topk", "pgo_graphs", "render_scatter", "render_gather". */
 int ovn_profile_enable(ovn_handle* h, int on);
 int ovn_profile_read(ovn_handle* h, const char* kernel, double* total_ms, int64_t* launches);
 
@@ -190,6 +190,38 @@ int ovn_preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* d_
 int ovn_preprocess_cues_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets,
                               int32_t n_scans, int64_t n_points_total, const float* d_probs,
                               float* d_input, void* stream);
+
+/* ---- stage 1e: virtual scans rendered from resident clouds (DESIGN.md sections 4 and 7) -------------
+ * n_virtual images, each from a list of entries: image v takes the entries [h_entry_offsets[v],
+ * h_entry_offsets[v+1]) (h_entry_offsets[0] = 0).  Entry e is the resident cloud h_entry_cloud[e], the points
+ * [h_offsets[c], h_offsets[c+1]) of d_points ([n][4] float32 back to back, as for ovn_project_batch; h_offsets
+ * is read on the host), moved by the row-major float64 pose h_entry_pose[e] ([16], bottom row 0 0 0 1; callers
+ * compose it as T_v^-1 T_k).  Each point becomes q = fl32(M (x, y, z, 1)): every coordinate is
+ * ((M_i0 x + M_i1 y) + M_i2 z) + M_i3 in float64, each product and sum rounded once (no FMA), then rounded to
+ * float32; the intensity is kept.  Image v is then, bit for bit, what ovn_project_batch gives for the cloud that
+ * concatenates the entries' transformed clouds in entry order, at the handle's geometry and max_range (< 0: the
+ * handle's): the nearest point wins, the lower concatenated index on exact ties.  d_winner [n][H][W] int32 is
+ * the winner's index in that concatenated cloud (not in the filtered one, unlike d_idx), -1 where empty; an
+ * image with no entries is all -1.  Outputs may be NULL.
+ * Caveat: with M = I a coordinate -0 becomes +0 (-0 + 0 = +0), and a point with y = -0 and x < 0 moves from
+ * column W-1 to column 0; so an identity entry equals ovn_project_batch only for clouds without negative zeros.
+ * The host tables are read and checked before anything is launched: decreasing offsets, h_entry_offsets[0] != 0,
+ * a cloud index outside [0, n_clouds), a pose that is not finite or whose bottom row is not 0 0 0 1, and an
+ * image whose concatenated points reach 2^32 (the key's index field; d_winner holds the index's low 32 bits)
+ * are OVN_ERR_INVALID_ARG, with the handle still usable.  n_virtual > max_batch_scans is OVN_ERR_CAPACITY.
+ * The entry table goes through a handle-owned device buffer, grown on use.  Profiled as "render_scatter" and
+ * "render_gather". */
+int ovn_render_batch(ovn_handle* h, const float* d_points, const int64_t* h_offsets /* [n_clouds+1] */,
+                     int32_t n_clouds, int32_t n_virtual, const int64_t* h_entry_offsets /* [n_virtual+1] */,
+                     const int32_t* h_entry_cloud /* [n_entries] */, const double* h_entry_pose /* [n_entries][16] */,
+                     float max_range, float* d_range, float* d_vertex, float* d_intensity,
+                     int32_t* d_winner /* [n][H][W] */, void* stream);
+
+/* The render packed as ovn_preprocess_batch packs a projection: d_input [n_virtual][H][W][C] at the handle's
+ * max_range.  OVN_ERR_BAD_CONFIG on a handle with probability channels: renders carry none. */
+int ovn_render_preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int32_t n_clouds,
+                                int32_t n_virtual, const int64_t* h_entry_offsets, const int32_t* h_entry_cloud,
+                                const double* h_entry_pose, float* d_input, void* stream);
 
 /* Pack separately computed cue images into the NHWC network input (same channel order). */
 int ovn_pack_input(ovn_handle* h, const float* d_depth, const float* d_normal, const float* d_prob,

@@ -16,7 +16,8 @@ SYMBOLS = [
     'ovn_abi_version', 'ovn_input_channels', 'ovn_feature_width', 'ovn_feature_channels',
     'ovn_launch_count', 'ovn_profile_enable', 'ovn_profile_read', 'ovn_set_weights', 'ovn_finalize_weights', 'ovn_project_batch',
     'ovn_normals_batch', 'ovn_semantic_batch', 'ovn_gt_range_batch', 'ovn_gt_overlap_count', 'ovn_gt_scan_radius',
-    'ovn_gt_pairs_count', 'ovn_preprocess_batch', 'ovn_preprocess_cues_batch',
+    'ovn_gt_pairs_count', 'ovn_preprocess_batch', 'ovn_preprocess_cues_batch', 'ovn_render_batch',
+    'ovn_render_preprocess_batch',
     'ovn_pack_input',
     'ovn_leg_forward', 'ovn_heads_forward', 'ovn_heads_1vsN', 'ovn_bank_prepare', 'ovn_bank_release', 'ovn_encode_clouds_host',
     'ovn_query_cloud_vs_bank_host', 'ovn_check', 'ovn_set_feature_center', 'ovn_get_feature_center',
@@ -150,6 +151,8 @@ def lib():
   L.ovn_semantic_batch.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp]
   L.ovn_preprocess_batch.argtypes = [vp, vp, vp, i32, i64, vp, vp, vp]
   L.ovn_preprocess_cues_batch.argtypes = [vp, vp, vp, i32, i64, vp, vp, vp]
+  L.ovn_render_batch.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, f32, vp, vp, vp, vp, vp]
+  L.ovn_render_preprocess_batch.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp]
   L.ovn_pack_input.argtypes = [vp, vp, vp, vp, vp, i32, vp, vp]
   L.ovn_leg_forward.argtypes = [vp, vp, i32, vp, vp]
   L.ovn_heads_forward.argtypes = [vp, vp, i64, vp, vp, i32, vp, vp, vp, vp]

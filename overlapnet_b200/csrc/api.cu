@@ -342,7 +342,8 @@ int ovn_profile_read(ovn_handle* h, const char* kernel, double* total_ms, int64_
   DeviceGuard guard(h);
   if (!kernel || !total_ms || !launches) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_profile_read: NULL argument");
   static const char* names[kProfKinds] = {"delta_conv1", "conv2", "conv3", "corr", "project_scatter",
-                                          "project_gather", "leg", "gather_rows", "rows_topk", "pgo_graphs"};
+                                          "project_gather", "leg", "gather_rows", "rows_topk", "pgo_graphs",
+                                          "render_scatter", "render_gather"};
   int kind = -1;
   for (int i = 0; i < kProfKinds; ++i) if (strcmp(kernel, names[i]) == 0) kind = i;
   if (kind < 0) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_profile_read: unknown kernel '%s'", kernel);
@@ -584,6 +585,31 @@ int ovn_preprocess_cues_batch(ovn_handle* h, const float* d_points, const int64_
   REQUIRE(h, n_scans >= 0 && n_total >= 0, "negative size");
   REQUIRE(h, n_scans == 0 || (d_offsets && d_input), "NULL pointer");
   return preprocess_cues_batch(h, d_points, d_offsets, n_scans, n_total, d_probs, d_input, (cudaStream_t)stream);
+}
+
+int ovn_render_batch(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int32_t n_clouds,
+                     int32_t n_virtual, const int64_t* h_entry_offsets, const int32_t* h_entry_cloud,
+                     const double* h_entry_pose, float max_range, float* d_range, float* d_vertex, float* d_intensity,
+                     int32_t* d_winner, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, n_clouds >= 0 && n_virtual >= 0, "negative size");
+  REQUIRE(h, n_virtual == 0 || (h_offsets && h_entry_offsets), "NULL pointer");
+  REQUIRE(h, n_virtual == 0 || h_entry_offsets[n_virtual] == 0 || (h_entry_cloud && h_entry_pose), "NULL pointer");
+  return render_batch(h, d_points, h_offsets, n_clouds, n_virtual, h_entry_offsets, h_entry_cloud, h_entry_pose,
+                      max_range, d_range, d_vertex, d_intensity, d_winner, (cudaStream_t)stream);
+}
+
+int ovn_render_preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int32_t n_clouds,
+                                int32_t n_virtual, const int64_t* h_entry_offsets, const int32_t* h_entry_cloud,
+                                const double* h_entry_pose, float* d_input, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, n_clouds >= 0 && n_virtual >= 0, "negative size");
+  REQUIRE(h, n_virtual == 0 || (h_offsets && h_entry_offsets && d_input), "NULL pointer");
+  REQUIRE(h, n_virtual == 0 || h_entry_offsets[n_virtual] == 0 || (h_entry_cloud && h_entry_pose), "NULL pointer");
+  return render_preprocess_batch(h, d_points, h_offsets, n_clouds, n_virtual, h_entry_offsets, h_entry_cloud,
+                                 h_entry_pose, d_input, (cudaStream_t)stream);
 }
 
 int ovn_pack_input(ovn_handle* h, const float* d_depth, const float* d_normal, const float* d_prob,

@@ -69,7 +69,7 @@ static_assert(sizeof(float) == sizeof(int32_t), "the three staging arrays are 4 
 constexpr int kFeatC = 128;           // leg output channels (generateNet.py:214)
 constexpr int kMaxLegLayers = 12;
 enum ProfKind { PROF_DELTA = 0, PROF_CONV2, PROF_CONV3, PROF_CORR, PROF_SCATTER, PROF_GATHER, PROF_LEG, PROF_GATHER_ROWS,
-                PROF_ROWS_TOPK, PROF_PGO, kProfKinds };
+                PROF_ROWS_TOPK, PROF_PGO, PROF_RENDER_SCATTER, PROF_RENDER_GATHER, kProfKinds };
 
 // The one owner of another process's shard mapped by ovn_shard_open (cudaIpcOpenMemHandle); unmaps it on
 // destruction.  Move-only, like Buffer.
@@ -273,6 +273,7 @@ struct ovn_handle {
   std::vector<ovn::IpcMapping> open_shards;
   ovn::McState mcl;                          // ovn_mcl_*: map and particles, allocated by ovn_mcl_set_map / ovn_mcl_init
   ovn::Buffer<uint8_t> d_pgo;                // ovn_pgo_optimize_host: one call's inputs and workspace, grown on use
+  ovn::Buffer<uint8_t> d_render;             // ovn_render_*: one call's entry table, grown on use
   cudaStream_t own_stream = nullptr;
   // per-kernel profiling (ovn_profile_enable / ovn_profile_read)
   bool profiling = false;
@@ -411,6 +412,14 @@ int gt_pairs_count(ovn_handle* h, const float* d_points, const int64_t* h_offset
                    const double* d_radius, const float* d_cur_range, const double* d_pose_cur_inv, int n_cur,
                    float max_range, int tile_cur, int tile_ref, int32_t* d_counts, int64_t ld_counts,
                    int64_t* d_n_pruned, cudaStream_t s);
+// the render (projection.cu): checks the host tables itself, before anything is launched
+int render_batch(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int n_clouds, int n_virtual,
+                 const int64_t* h_entry_offsets, const int32_t* h_entry_cloud, const double* h_entry_pose,
+                 float max_range, float* d_range, float* d_vertex, float* d_intensity, int32_t* d_winner,
+                 cudaStream_t s);
+int render_preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int n_clouds,
+                            int n_virtual, const int64_t* h_entry_offsets, const int32_t* h_entry_cloud,
+                            const double* h_entry_pose, float* d_input, cudaStream_t s);
 int pack_input(ovn_handle* h, const float* d_depth, const float* d_normal, const float* d_prob,
                const float* d_intensity, int n_scans, float* d_input, cudaStream_t s);
 

@@ -9,22 +9,11 @@
 // kernel rounds the winners to float32 (the image dtype, utils.py:120) and a third counts pixels.
 // HBM-bound byte work: 16 B read per point, 8 B atomic per valid point into an L2-resident key image.
 #include "range_bin.cuh"
+#include "se3.cuh"
 
 namespace ovn {
 
 constexpr unsigned long long kGtEmpty = 0xFFFFFFFFFFFFFFFFull;
-
-// row-major 4x4 times (x, y, z, w): left-to-right sums of separately rounded products, which is
-// what a reference BLAS without FMA contraction produces; FMA vs non-FMA differences (<= 1 ulp of a
-// coordinate) move a point across a bin edge or the |dr| < 1 threshold with probability ~1e-12.
-__device__ __forceinline__ void mat4_apply(const double* __restrict__ M, double& x, double& y, double& z, double& w) {
-  double r[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-    r[i] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(M[4 * i + 0], x), __dmul_rn(M[4 * i + 1], y)),
-                               __dmul_rn(M[4 * i + 2], z)), __dmul_rn(M[4 * i + 3], w));
-  x = r[0]; y = r[1]; z = r[2]; w = r[3];
-}
 
 // range_projection of one transformed point in float64 (utils.py:75-104, range_bin) and the atomic-min of its
 // depth into the key image `keys` [H][W]; points outside (0, max_range) are dropped

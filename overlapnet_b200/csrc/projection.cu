@@ -22,6 +22,10 @@
 //                its floor when it is further from a bin edge than a margin derived from H, W and the
 //                fov (make_params); otherwise the float64 function is evaluated (see K1).
 #include "common.cuh"
+#include "se3.cuh"
+
+#include <cmath>
+#include <cstring>
 
 namespace ovn {
 
@@ -124,17 +128,122 @@ __device__ __forceinline__ int find_scan(const int64_t* __restrict__ offsets, in
 }
 
 // ------------------------------------------------------------------------------------------
-// K1: scatter.  grid = ceil(n_total / 256), block = 256.
-// kCues (ovn_preprocess_cues_batch): two key images per call, keys = A [n_scans][H*W] then B [n_scans][H*W].  A takes
-// the points of the configured filter (0 < depth < max_range, utils.py:76-77), B those of the semantic cue's
-// (0 < depth < inf, gen_semantic_data.py:39; NaN fails both).  The bins are computed once per point, and the
-// validity bits (the ranks) follow B's filter: the probability gather indexes with B's filtered index.
+// Point sources of the scatter and the gather.  The scatter runs one thread per g in [seg[0], seg[n_seg]) and
+// finds the segment s with seg[s] <= g < seg[s + 1]; the source gives the point of g, the image it lands in and
+// the index its key carries (from g and seg[s]).  Image b's points are g = base(b) + key index, from which the gather recomputes a
+// winner's point.
 // ------------------------------------------------------------------------------------------
-template <bool kCues>
+// Raw clouds (ovn_project_batch and the preprocess calls): segment b is scan b and image b, seg the caller's
+// point offsets; the key carries the point's index in its scan.
+struct RawPoints {
+  static constexpr bool kRanked = true;      // d_idx is the winner's index in the FILTERED cloud
+  const float4* __restrict__ pts;
+  const int64_t* __restrict__ offsets;
+  __device__ __forceinline__ float4 point(int b, int64_t g) const { return __ldg(pts + g); }
+  __device__ __forceinline__ int image(int b) const { return b; }
+  __device__ __forceinline__ uint32_t key_index(int b, int64_t g, int64_t seg_start) const {
+    return (uint32_t)(g - seg_start);
+  }
+  __device__ __forceinline__ int64_t base(int b) const { return __ldg(offsets + b); }
+  __device__ __forceinline__ float4 winner(int b, int64_t base, uint32_t k) const { return __ldg(pts + base + k); }
+};
+
+// One render entry (ovn_render_batch): a resident cloud moved by a float64 pose into a virtual frame.
+struct RenderEntry {
+  double M[16];          // row-major 4x4, bottom row 0 0 0 1
+  int64_t cloud_start;   // the cloud's first point in d_points
+  int64_t image_base;    // seg[] of the image's first entry: the key carries g - image_base, the concatenated index
+  int32_t image;
+  int32_t pad;
+};
+static_assert(sizeof(RenderEntry) == 152, "RenderEntry layout");
+
+// Posed entries: segment e is entry e, seg the prefix of the entries' point counts over the call, so an image's
+// entries are consecutive segments and g - image_base is the point's index in the image's concatenated cloud.
+struct PosedPoints {
+  static constexpr bool kRanked = false;     // d_idx (d_winner) is the concatenated index itself
+  const float4* __restrict__ pts;
+  const RenderEntry* __restrict__ ent;       // [n_entries]
+  const int64_t* __restrict__ seg;           // [n_entries + 1]
+  const int64_t* __restrict__ first;         // [n_images + 1] first entry of each image
+  // q = fl32(M (x, y, z, 1)) in float64 without contraction (mat4_apply), intensity kept
+  __device__ __forceinline__ float4 load(int e, int64_t local) const {
+    const float4 p = __ldg(pts + ent[e].cloud_start + local);
+    double x = (double)p.x, y = (double)p.y, z = (double)p.z, w = 1.0;
+    mat4_apply(ent[e].M, x, y, z, w);
+    return make_float4(__double2float_rn(x), __double2float_rn(y), __double2float_rn(z), p.w);
+  }
+  __device__ __forceinline__ float4 point(int e, int64_t g) const { return load(e, g - seg[e]); }
+  __device__ __forceinline__ int image(int e) const { return ent[e].image; }
+  __device__ __forceinline__ uint32_t key_index(int e, int64_t g, int64_t seg_start) const {
+    return (uint32_t)(g - ent[e].image_base);
+  }
+  __device__ __forceinline__ int64_t base(int b) const { return seg[first[b]]; }
+  __device__ __forceinline__ float4 winner(int b, int64_t base, uint32_t k) const {
+    const int64_t e0 = first[b], g = base + k;
+    const int e = (int)e0 + find_scan(seg + e0, (int)(first[b + 1] - e0), g);
+    return point(e, g);
+  }
+};
+
+// utils.py:75  np.linalg.norm(xyz, 2, axis=1): sqrt((x*x + y*y) + z*z), float32, no FMA
+__device__ __forceinline__ float point_depth(const float4 p) {
+  return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(p.x, p.x), __fmul_rn(p.y, p.y)), __fmul_rn(p.z, p.z)));
+}
+
+// utils.py:86-104: the pixel of a point of float32 depth `depth` > 0
+__device__ __forceinline__ void point_bins(const float4 p, const float depth, const ProjParams& P, int& bx, int& by) {
+  // Bins: the exact answer is floor(P(fl32(angle))) with P the reference's float32 pipeline (bin_x /
+  // bin_y, monotone) and fl32 the correctly rounded float32 angle.  Fast path: ONE fused estimate
+  // t = angle * scale + offset of the pre-floor value; all error sources together (atan2f <= 3 ulp,
+  // asinf <= 2 ulp, the pipeline's roundings, the estimate's own) stay below bound_x / bound_y bins
+  // (2.8e-4 / 4.2e-5 at 64 x 900 and the default fov), so whenever t is further than P.mx (P.my, at
+  // least twice the bound) from an integer -- and inside the image -- floor(t) IS the reference's bin.
+  // Otherwise (0.2 % of the points at 64 x 900) the float64 function is rounded once and pushed through
+  // the exact pipeline.  The first version ran the exact pipeline on
+  // both ends of an error bracket for every point: 4 correctly rounded divisions, 295 instructions per
+  // point, issue-bound.
+  // ---- yaw bin (utils.py:86,90,94,98-100)
+  {
+    const float yaw_f = -atan2f(p.y, p.x);
+    const float t = fmaf(yaw_f, P.kx, P.cx);
+    const float fl = floorf(t);
+    const float fr = t - fl;
+    if (fr > P.mx && fr < 1.0f - P.mx && t > P.mx && t < P.W32 - P.mx) {
+      bx = (int)fl;
+    } else {
+      const float yaw_cr = __double2float_rn(-atan2((double)p.y, (double)p.x));
+      bx = bin_x(yaw_cr, P);
+    }
+  }
+  // ---- pitch bin (utils.py:87,91,95,102-104); q must be the reference's correctly rounded z / depth
+  {
+    const float q = __fdiv_rn(p.z, depth);
+    const float pit_f = asinf(q);
+    const float t = fmaf(pit_f, P.ky, P.cy);
+    const float fl = floorf(t);
+    const float fr = t - fl;
+    if (fr > P.my && fr < 1.0f - P.my && t > P.my && t < P.H32 - P.my) {
+      by = (int)fl;
+    } else {
+      const float pit_cr = __double2float_rn(asin((double)q));
+      by = bin_y(pit_cr, P);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// K1: scatter.  grid = ceil(n_total / 256), block = 256; one thread per g of the source's segments.
+// kCues (ovn_preprocess_cues_batch, raw points only): two key images per call, keys = A [n_scans][H*W] then
+// B [n_scans][H*W].  A takes the points of the configured filter (0 < depth < max_range, utils.py:76-77), B those
+// of the semantic cue's (0 < depth < inf, gen_semantic_data.py:39; NaN fails both).  The bins are computed once per
+// point, and the validity bits (the ranks) follow B's filter: the probability gather indexes with B's filtered
+// index.
+// ------------------------------------------------------------------------------------------
+template <bool kCues, class Src>
 __global__ void __launch_bounds__(256)
-k_project_scatter(const float4* __restrict__ pts, const int64_t* __restrict__ offsets, int n_scans,
-                  int64_t n_total, ProjParams P, unsigned long long* __restrict__ keys,
-                  uint32_t* __restrict__ valid_words) {
+k_project_scatter(const Src src, const int64_t* __restrict__ offsets, int n_scans, int64_t n_total, ProjParams P,
+                  unsigned long long* __restrict__ keys, uint32_t* __restrict__ valid_words) {
   __shared__ int s_first_scan;
   const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (threadIdx.x == 0) {
@@ -146,55 +255,16 @@ k_project_scatter(const float4* __restrict__ pts, const int64_t* __restrict__ of
   if (g < n_total && g >= offsets[0] && g < offsets[n_scans]) {
     int b = s_first_scan;
     while (b + 1 < n_scans && g >= offsets[b + 1]) ++b;   // a block rarely spans > 2 scans
-    const float4 p = __ldg(pts + g);
-    // utils.py:75  np.linalg.norm(xyz, 2, axis=1): sqrt((x*x + y*y) + z*z), float32, no FMA
-    const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(p.x, p.x), __fmul_rn(p.y, p.y)), __fmul_rn(p.z, p.z));
-    const float depth = __fsqrt_rn(d2);
+    const float4 p = src.point(b, g);
+    const float depth = point_depth(p);
     const bool in_a = (depth > 0.0f) && (depth < P.max_range);   // utils.py:76-77
     valid = kCues ? (depth > 0.0f) && (depth < __int_as_float(0x7f800000)) : in_a;
     if (valid) {
-      // Bins: the exact answer is floor(P(fl32(angle))) with P the reference's float32 pipeline (bin_x /
-      // bin_y, monotone) and fl32 the correctly rounded float32 angle.  Fast path: ONE fused estimate
-      // t = angle * scale + offset of the pre-floor value; all error sources together (atan2f <= 3 ulp,
-      // asinf <= 2 ulp, the pipeline's roundings, the estimate's own) stay below bound_x / bound_y bins
-      // (2.8e-4 / 4.2e-5 at 64 x 900 and the default fov), so whenever t is further than P.mx (P.my, at
-      // least twice the bound) from an integer -- and inside the image -- floor(t) IS the reference's bin.
-      // Otherwise (0.2 % of the points at 64 x 900) the float64 function is rounded once and pushed through
-      // the exact pipeline.  The first version ran the exact pipeline on
-      // both ends of an error bracket for every point: 4 correctly rounded divisions, 295 instructions per
-      // point, issue-bound.
-      // ---- yaw bin (utils.py:86,90,94,98-100)
-      int bx;
-      {
-        const float yaw_f = -atan2f(p.y, p.x);
-        const float t = fmaf(yaw_f, P.kx, P.cx);
-        const float fl = floorf(t);
-        const float fr = t - fl;
-        if (fr > P.mx && fr < 1.0f - P.mx && t > P.mx && t < P.W32 - P.mx) {
-          bx = (int)fl;
-        } else {
-          const float yaw_cr = __double2float_rn(-atan2((double)p.y, (double)p.x));
-          bx = bin_x(yaw_cr, P);
-        }
-      }
-      // ---- pitch bin (utils.py:87,91,95,102-104); q must be the reference's correctly rounded z / depth
-      int by;
-      {
-        const float q = __fdiv_rn(p.z, depth);
-        const float pit_f = asinf(q);
-        const float t = fmaf(pit_f, P.ky, P.cy);
-        const float fl = floorf(t);
-        const float fr = t - fl;
-        if (fr > P.my && fr < 1.0f - P.my && t > P.my && t < P.H32 - P.my) {
-          by = (int)fl;
-        } else {
-          const float pit_cr = __double2float_rn(asin((double)q));
-          by = bin_y(pit_cr, P);
-        }
-      }
-      const uint32_t local = (uint32_t)(g - offsets[b]);
+      int bx, by;
+      point_bins(p, depth, P, bx, by);
+      const uint32_t local = src.key_index(b, g, offsets[b]);
       const unsigned long long key = ((unsigned long long)__float_as_uint(depth) << 32) | local;
-      const size_t pix = (size_t)b * P.H * P.W + (size_t)by * P.W + bx;
+      const size_t pix = (size_t)src.image(b) * P.H * P.W + (size_t)by * P.W + bx;
       if (!kCues || in_a) atomicMin(keys + pix, key);
       if (kCues) atomicMin(keys + (size_t)n_scans * P.H * P.W + pix, key);
     }
@@ -336,17 +406,17 @@ constexpr int TILE_R = 8, TILE_C = 32;
 
 // kCues: keys holds A then B (k_project_scatter<true>); depth, normals and intensity come from A's winners, the
 // probabilities from B's, indexed with B's rank (the validity bits are B's filter); out.idx is not written.
-template <bool kCues>
+// Src::kRanked: out.idx is the winner's index in the filtered cloud (raw points); else the key's index.
+template <bool kCues, class Src>
 __global__ void __launch_bounds__(256)
-k_project_gather(const float4* __restrict__ pts, const int64_t* __restrict__ offsets, ProjParams P,
-                 const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ valid_words,
-                 const uint32_t* __restrict__ word_prefix, GatherOut out) {
+k_project_gather(const Src src, ProjParams P, const unsigned long long* __restrict__ keys,
+                 const uint32_t* __restrict__ valid_words, const uint32_t* __restrict__ word_prefix, GatherOut out) {
   __shared__ float4 s_pt[TILE_R + 1][TILE_C + 1];
   __shared__ float s_depth[TILE_R + 1][TILE_C + 1];
   __shared__ uint32_t s_local[TILE_R + 1][TILE_C + 1];
   const int b = blockIdx.z;
   const int x0 = blockIdx.x * TILE_C, y0 = blockIdx.y * TILE_R;
-  const int64_t off = offsets[b];
+  const int64_t off = src.base(b);
   const unsigned long long* kb = keys + (size_t)b * P.H * P.W;
   for (int c = threadIdx.x; c < (TILE_R + 1) * (TILE_C + 1); c += blockDim.x) {
     const int ry = c / (TILE_C + 1), rx = c % (TILE_C + 1);
@@ -361,7 +431,7 @@ k_project_gather(const float4* __restrict__ pts, const int64_t* __restrict__ off
       if (k != kEmptyKey) {
         depth = __uint_as_float((uint32_t)(k >> 32));
         local = (uint32_t)(k & 0xFFFFFFFFull);
-        p = __ldg(pts + off + local);
+        p = src.winner(b, off, local);
       }
     }
     s_pt[ry][rx] = p;
@@ -379,9 +449,13 @@ k_project_gather(const float4* __restrict__ pts, const int64_t* __restrict__ off
 
   int32_t fidx = -1;
   if (!kCues && has && (out.idx != nullptr || out.n_prob > 0)) {
-    // index into the FILTERED cloud (utils.py:76,117-118)
-    fidx = (int32_t)(valid_before(valid_words, word_prefix, off + s_local[ty][tx]) -
-                     valid_before(valid_words, word_prefix, off));
+    if constexpr (Src::kRanked) {
+      // index into the FILTERED cloud (utils.py:76,117-118)
+      fidx = (int32_t)(valid_before(valid_words, word_prefix, off + s_local[ty][tx]) -
+                       valid_before(valid_words, word_prefix, off));
+    } else {
+      fidx = (int32_t)s_local[ty][tx];
+    }
   }
   float nrm[3] = {-1.f, -1.f, -1.f};
   if ((out.normal != nullptr || out.c_normal >= 0) && has && y < P.H - 1 &&
@@ -531,20 +605,18 @@ static int ensure_point_capacity(ovn_handle* h, int64_t n_total) {
   return h->d_scan_tmp.ensure(h, (need / 1024 + 2) * sizeof(uint32_t), (words / 1024 + 2) * sizeof(uint32_t));
 }
 
+// One projection of n_images images from the source's n_seg segments of g in [offsets[0], offsets[n_seg]).
 // cues: the two key images of ovn_preprocess_cues_batch (k_project_scatter<true>); the handle's d_keys holds them
-// only when it has probability channels (ovn_create)
-static int run_projection(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans,
-                          int64_t n_total, float max_range, const GatherOut& out_in, cudaStream_t s,
-                          bool cues = false) {
-  if (n_scans <= 0) return OVN_OK;
-  if (n_scans > h->cfg.max_batch_scans)
-    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "n_scans=%d exceeds max_batch_scans=%d", n_scans, h->cfg.max_batch_scans);
-  GatherOut out = out_in;
+// only when it has probability channels (ovn_create).
+template <class Src>
+static int launch_projection(ovn_handle* h, const Src& src, const int64_t* d_offsets, int n_seg, int n_images,
+                             int64_t n_total, float max_range, const GatherOut& out, cudaStream_t s, bool cues,
+                             int prof_scatter, int prof_gather) {
   const ProjParams P = make_params(h, max_range);
-  const bool need_rank = cues || out.idx != nullptr || out.n_prob > 0;
+  const bool need_rank = Src::kRanked && (cues || out.idx != nullptr || out.n_prob > 0);
   const size_t HW = (size_t)P.H * P.W;
-  const size_t n_images = cues ? 2 : 1;
-  OVN_CUDA(h, cudaMemsetAsync(h->d_keys, 0xFF, n_images * n_scans * HW * sizeof(unsigned long long), s));
+  const size_t n_key_images = cues ? 2 : 1;
+  OVN_CUDA(h, cudaMemsetAsync(h->d_keys, 0xFF, n_key_images * n_images * HW * sizeof(unsigned long long), s));
   int64_t n_words = (n_total + 31) / 32;
   if (need_rank) {
     int rc = ensure_point_capacity(h, n_total);
@@ -552,11 +624,12 @@ static int run_projection(ovn_handle* h, const float* d_points, const int64_t* d
   }
   if (n_total > 0) {
     const int64_t blocks = (n_total + 255) / 256;
-    prof_mark(h, PROF_SCATTER, s);
-    auto scatter = cues ? k_project_scatter<true> : k_project_scatter<false>;
-    scatter<<<(unsigned)blocks, 256, 0, s>>>(reinterpret_cast<const float4*>(d_points), d_offsets, n_scans, n_total,
-                                             P, h->d_keys, need_rank ? h->d_valid_words.get() : nullptr);
-    prof_mark(h, PROF_SCATTER, s);
+    prof_mark(h, prof_scatter, s);
+    auto scatter = k_project_scatter<false, Src>;
+    if constexpr (Src::kRanked) if (cues) scatter = k_project_scatter<true, Src>;
+    scatter<<<(unsigned)blocks, 256, 0, s>>>(src, d_offsets, n_seg, n_total, P, h->d_keys,
+                                             need_rank ? h->d_valid_words.get() : nullptr);
+    prof_mark(h, prof_scatter, s);
     OVN_LAUNCH_CHECK(h);
     if (need_rank) {
       const int nb = (int)((n_words + 1023) / 1024);
@@ -568,14 +641,25 @@ static int run_projection(ovn_handle* h, const float* d_points, const int64_t* d
       OVN_LAUNCH_CHECK(h);
     }
   }
-  dim3 grid((P.W + TILE_C - 1) / TILE_C, (P.H + TILE_R - 1) / TILE_R, n_scans);
-  prof_mark(h, PROF_GATHER, s);
-  auto gather = cues ? k_project_gather<true> : k_project_gather<false>;
-  gather<<<grid, 256, 0, s>>>(reinterpret_cast<const float4*>(d_points), d_offsets, P, h->d_keys, h->d_valid_words,
-                              h->d_word_prefix, out);
-  prof_mark(h, PROF_GATHER, s);
+  dim3 grid((P.W + TILE_C - 1) / TILE_C, (P.H + TILE_R - 1) / TILE_R, n_images);
+  prof_mark(h, prof_gather, s);
+  auto gather = k_project_gather<false, Src>;
+  if constexpr (Src::kRanked) if (cues) gather = k_project_gather<true, Src>;
+  gather<<<grid, 256, 0, s>>>(src, P, h->d_keys, h->d_valid_words, h->d_word_prefix, out);
+  prof_mark(h, prof_gather, s);
   OVN_LAUNCH_CHECK(h);
   return OVN_OK;
+}
+
+static int run_projection(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans,
+                          int64_t n_total, float max_range, const GatherOut& out, cudaStream_t s,
+                          bool cues = false) {
+  if (n_scans <= 0) return OVN_OK;
+  if (n_scans > h->cfg.max_batch_scans)
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "n_scans=%d exceeds max_batch_scans=%d", n_scans, h->cfg.max_batch_scans);
+  const RawPoints src = {reinterpret_cast<const float4*>(d_points), d_offsets};
+  return launch_projection(h, src, d_offsets, n_scans, n_scans, n_total, max_range, out, s, cues, PROF_SCATTER,
+                           PROF_GATHER);
 }
 
 int project_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans,
@@ -630,6 +714,100 @@ int preprocess_cues_batch(ovn_handle* h, const float* d_points, const int64_t* d
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "d_probs is NULL but n_prob_channels=%d", h->cfg.n_prob_channels);
   return run_projection(h, d_points, d_offsets, n_scans, n_total, h->cfg.max_range,
                         packed_channels(h, d_probs, d_input), s, true);
+}
+
+// ---- the render: range images of resident clouds moved into virtual frames ----------------------------------
+// Reads and checks the host tables (nothing is launched on a refusal), uploads the entry table to d_render and
+// projects each image from its entries' transformed points in entry order (PosedPoints).
+static int render(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int n_clouds, int n_virtual,
+                  const int64_t* h_entry_offsets, const int32_t* h_entry_cloud, const double* h_entry_pose,
+                  float max_range, const GatherOut& out, cudaStream_t s) {
+  if (n_virtual > h->cfg.max_batch_scans)
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "n_virtual=%d exceeds max_batch_scans=%d", n_virtual, h->cfg.max_batch_scans);
+  if (n_virtual <= 0) return OVN_OK;
+  if (h_offsets[0] < 0) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render: h_offsets[0] < 0");
+  for (int c = 0; c < n_clouds; ++c)
+    if (h_offsets[c + 1] < h_offsets[c])
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render: h_offsets decreases at cloud %d", c);
+  if (h_entry_offsets[0] != 0) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render: h_entry_offsets[0] must be 0");
+  for (int v = 0; v < n_virtual; ++v)
+    if (h_entry_offsets[v + 1] < h_entry_offsets[v])
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render: h_entry_offsets decreases at image %d", v);
+  const int64_t n_entries = h_entry_offsets[n_virtual];
+  if (n_entries >= INT32_MAX) OVN_SET_ERR(h, OVN_ERR_CAPACITY, "render: %lld entries", (long long)n_entries);
+  std::vector<RenderEntry> ent((size_t)n_entries);
+  std::vector<int64_t> seg((size_t)n_entries + 1), first(h_entry_offsets, h_entry_offsets + n_virtual + 1);
+  seg[0] = 0;
+  for (int v = 0; v < n_virtual; ++v) {
+    for (int64_t e = h_entry_offsets[v]; e < h_entry_offsets[v + 1]; ++e) {
+      const int32_t c = h_entry_cloud[e];
+      if (c < 0 || c >= n_clouds)
+        OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render: entry %lld names cloud %d, outside [0, %d)", (long long)e, c,
+                    n_clouds);
+      const double* M = h_entry_pose + 16 * e;
+      for (int i = 0; i < 16; ++i)
+        if (!std::isfinite(M[i])) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render: the pose of entry %lld is not finite",
+                                              (long long)e);
+      if (M[12] != 0.0 || M[13] != 0.0 || M[14] != 0.0 || M[15] != 1.0)
+        OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render: the pose of entry %lld does not end in the row 0 0 0 1",
+                    (long long)e);
+      RenderEntry& E = ent[(size_t)e];
+      memcpy(E.M, M, sizeof(E.M));
+      E.cloud_start = h_offsets[c];
+      E.image_base = seg[(size_t)h_entry_offsets[v]];
+      E.image = v;
+      E.pad = 0;
+      seg[(size_t)e + 1] = seg[(size_t)e] + (h_offsets[c + 1] - h_offsets[c]);
+    }
+    // the key's index field holds the concatenated index
+    const int64_t n_image = seg[(size_t)h_entry_offsets[v + 1]] - seg[(size_t)h_entry_offsets[v]];
+    if (n_image >= (int64_t(1) << 32))
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render: image %d concatenates %lld points, 2^32 or more", v,
+                  (long long)n_image);
+  }
+  const int64_t n_total = seg[(size_t)n_entries];
+  if (n_total > (int64_t)INT32_MAX * 256)
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "render: %lld points in one call exceed the scatter grid", (long long)n_total);
+  if (n_total > 0 && d_points == nullptr) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render: d_points is NULL");
+  const size_t b_ent = ent.size() * sizeof(RenderEntry), b_seg = seg.size() * sizeof(int64_t);
+  const size_t b_first = first.size() * sizeof(int64_t);
+  std::vector<uint8_t> table(b_ent + b_seg + b_first);
+  if (b_ent) memcpy(table.data(), ent.data(), b_ent);
+  memcpy(table.data() + b_ent, seg.data(), b_seg);
+  memcpy(table.data() + b_ent + b_seg, first.data(), b_first);
+  int rc = h->d_render.ensure(h, table.size());
+  if (rc != OVN_OK) return rc;
+  // pageable source: the copy is staged before the call returns, after the stream's earlier work
+  OVN_CUDA(h, cudaMemcpyAsync(h->d_render, table.data(), table.size(), cudaMemcpyHostToDevice, s));
+  const uint8_t* base = h->d_render;
+  PosedPoints src;
+  src.pts = reinterpret_cast<const float4*>(d_points);
+  src.ent = reinterpret_cast<const RenderEntry*>(base);
+  src.seg = reinterpret_cast<const int64_t*>(base + b_ent);
+  src.first = reinterpret_cast<const int64_t*>(base + b_ent + b_seg);
+  return launch_projection(h, src, src.seg, (int)n_entries, n_virtual, n_total,
+                           max_range < 0 ? h->cfg.max_range : max_range, out, s, false, PROF_RENDER_SCATTER,
+                           PROF_RENDER_GATHER);
+}
+
+int render_batch(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int n_clouds, int n_virtual,
+                 const int64_t* h_entry_offsets, const int32_t* h_entry_cloud, const double* h_entry_pose,
+                 float max_range, float* d_range, float* d_vertex, float* d_intensity, int32_t* d_winner,
+                 cudaStream_t s) {
+  GatherOut out = {};
+  out.range = d_range; out.vertex = d_vertex; out.intensity = d_intensity; out.idx = d_winner;
+  out.c_depth = out.c_normal = out.c_prob = out.c_intensity = -1;
+  return render(h, d_points, h_offsets, n_clouds, n_virtual, h_entry_offsets, h_entry_cloud, h_entry_pose, max_range,
+                out, s);
+}
+
+int render_preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int n_clouds,
+                            int n_virtual, const int64_t* h_entry_offsets, const int32_t* h_entry_cloud,
+                            const double* h_entry_pose, float* d_input, cudaStream_t s) {
+  if (h->cfg.n_prob_channels > 0)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "render_preprocess: the handle has probability channels, which renders lack");
+  return render(h, d_points, h_offsets, n_clouds, n_virtual, h_entry_offsets, h_entry_cloud, h_entry_pose,
+                h->cfg.max_range, packed_channels(h, nullptr, d_input), s);
 }
 
 int normals_batch(ovn_handle* h, const float* d_range, const float* d_vertex, int n_scans,

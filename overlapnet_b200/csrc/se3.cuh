@@ -1,10 +1,23 @@
-// se3.cuh -- the pose update shared by ICP (icp.cu) and the pose-graph optimizer (pose_graph.cu), DESIGN.md section 7.
+// se3.cuh -- the pose update shared by ICP (icp.cu) and the pose-graph optimizer (pose_graph.cu), DESIGN.md section 7,
+// and the float64 point transform shared by the ground-truth generator (gt_overlap.cu) and the render (projection.cu).
 // A pose is the first three rows of a row-major 4x4; an update xi = (omega, v) moves it on the left,
 // T <- [R(omega) | v] T, with R by Rodrigues.
 #pragma once
 #include <math.h>
 
 namespace ovn {
+
+// row-major 4x4 times (x, y, z, w): left-to-right sums of separately rounded products, which is
+// what a reference BLAS without FMA contraction produces; FMA vs non-FMA differences (<= 1 ulp of a
+// coordinate) move a point across a bin edge or the |dr| < 1 threshold with probability ~1e-12.
+__device__ __forceinline__ void mat4_apply(const double* __restrict__ M, double& x, double& y, double& z, double& w) {
+  double r[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    r[i] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(M[4 * i + 0], x), __dmul_rn(M[4 * i + 1], y)),
+                               __dmul_rn(M[4 * i + 2], z)), __dmul_rn(M[4 * i + 3], w));
+  x = r[0]; y = r[1]; z = r[2]; w = r[3];
+}
 
 // R(omega) = I + sin(th) K + (1 - cos(th)) K^2, K the cross-product matrix of the unit axis (row-major 3x3)
 __device__ __forceinline__ void rodrigues(const double* d, double R[9]) {

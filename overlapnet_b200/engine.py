@@ -318,6 +318,64 @@ class Engine:
                                                  _ptr(out[s0:s1]), self._stream()), 'ovn_preprocess_cues_batch')
     return out
 
+  def _render_chunks(self, batch, entry_offsets, entry_cloud, entry_pose):
+    """Host tables of the render, cut into calls of at most max_batch_scans virtual frames: yields (v0, v1,
+    offsets, clouds, poses) with the chunk's entry offsets starting at 0."""
+    eo = np.ascontiguousarray(entry_offsets, np.int64).reshape(-1)
+    ec = np.ascontiguousarray(entry_cloud, np.int32).reshape(-1)
+    ep = np.ascontiguousarray(entry_pose, np.float64).reshape(-1, 16)
+    if eo.size < 1 or eo[0] != 0 or eo[-1] != ec.size or ep.shape[0] != ec.size:
+      raise ValueError('render: entry_offsets [n_virtual + 1] must run from 0 to the number of entries, with one '
+                       'cloud and one 4x4 pose per entry')
+    n = eo.size - 1
+    for v0 in range(0, n, self.max_batch_scans):
+      v1 = min(n, v0 + self.max_batch_scans)
+      e0, e1 = int(eo[v0]), int(eo[v1])
+      yield v0, v1, np.ascontiguousarray(eo[v0:v1 + 1] - e0), np.ascontiguousarray(ec[e0:e1]), \
+          np.ascontiguousarray(ep[e0:e1])
+
+  @staticmethod
+  def _hp(a):
+    return a.ctypes.data_as(C.c_void_p)
+
+  def render(self, batch, entry_offsets, entry_cloud, entry_pose, max_range=-1.0,
+             want=('range', 'vertex', 'intensity', 'winner')):
+    """ovn_render_batch: range images of virtual frames rendered from the clouds of a CloudBatch.  Virtual frame v
+    concatenates, in entry order, the entries [entry_offsets[v], entry_offsets[v + 1]): cloud entry_cloud[e] moved
+    by the float64 pose entry_pose[e] (4x4, T_v^-1 T_k).  ``winner`` is the int32 index of each pixel's point in
+    that concatenated cloud, -1 where empty.  Calls of max_batch_scans frames."""
+    n = int(np.asarray(entry_offsets).reshape(-1).shape[0]) - 1
+    dev = self.device
+    out = {}
+    if 'range' in want: out['range'] = torch.empty((n, self.H, self.W), dtype=torch.float32, device=dev)
+    if 'vertex' in want: out['vertex'] = torch.empty((n, self.H, self.W, 4), dtype=torch.float32, device=dev)
+    if 'intensity' in want: out['intensity'] = torch.empty((n, self.H, self.W), dtype=torch.float32, device=dev)
+    if 'winner' in want: out['winner'] = torch.empty((n, self.H, self.W), dtype=torch.int32, device=dev)
+    offs = np.ascontiguousarray(batch.offsets_host, np.int64)
+    L = lib()
+    for v0, v1, eo, ec, ep in self._render_chunks(batch, entry_offsets, entry_cloud, entry_pose):
+      sl = {k: v[v0:v1] for k, v in out.items()}
+      check(self._h, L.ovn_render_batch(
+          self._h, _ptr(batch.points), self._hp(offs), batch.n, v1 - v0, self._hp(eo), self._hp(ec), self._hp(ep),
+          float(max_range), _ptr(sl.get('range')), _ptr(sl.get('vertex')), _ptr(sl.get('intensity')),
+          _ptr(sl.get('winner')), self._stream()), 'ovn_render_batch')
+    return out
+
+  def render_preprocess(self, batch, entry_offsets, entry_cloud, entry_pose, out=None):
+    """ovn_render_preprocess_batch: the render's packed NHWC network input [n_virtual, H, W, C], as preprocess packs
+    a projection (``out``: an optional float32 tensor of that shape to write)."""
+    n = int(np.asarray(entry_offsets).reshape(-1).shape[0]) - 1
+    if out is None:
+      out = torch.empty((n, self.H, self.W, self.C), dtype=torch.float32, device=self.device)
+    assert out.dtype == torch.float32 and tuple(out.shape) == (n, self.H, self.W, self.C) and out.is_contiguous()
+    offs = np.ascontiguousarray(batch.offsets_host, np.int64)
+    L = lib()
+    for v0, v1, eo, ec, ep in self._render_chunks(batch, entry_offsets, entry_cloud, entry_pose):
+      check(self._h, L.ovn_render_preprocess_batch(
+          self._h, _ptr(batch.points), self._hp(offs), batch.n, v1 - v0, self._hp(eo), self._hp(ec), self._hp(ep),
+          _ptr(out[v0:v1]), self._stream()), 'ovn_render_preprocess_batch')
+    return out
+
   def pack_input(self, depth=None, normal=None, prob=None, intensity=None):
     first = next(t for t in (depth, normal, prob, intensity) if t is not None)
     n = first.shape[0]

@@ -3,13 +3,17 @@ network's overlap and yaw as the observation model and the particle filter on th
 
   python -m overlapnet_b200.mcl [config/demo.yml] [--keyframe-stride S] [--particles N] [--runs R]
                                 [--sigma-overlap 0.1] [--sigma-yaw-deg 10] [--cell 0.5] [--max-distance 5]
-                                [--converged-m 2]
+                                [--converged-m 2] [--virtual-spacing G [--render-sources 8] [--render-radius R]]
 
 The model:
   map         K keyframes, each a scan encoded once (Infer.encode_clouds), calibrated on keyframe 0 and kept
               resident, with its planar pose (x_k, y_k, theta_k = atan2(R10, R00)).  ``MapIndex`` rasterises the
               keyframes' bounding box grown by max_distance: each cell holds the keyframe nearest to its centre
               within max_distance (ties to the lowest index), else -1.
+  virtual     with a virtual spacing G, the map frames are instead the points of a G-metre lattice within
+              max_distance of the keyframes (virtual_map.lattice), each rendered on the GPU from its M nearest
+              keyframe clouds within the render radius and encoded; the raster holds the nearest lattice frame
+              within G of each cell centre.
   particles   (x, y, theta) with a log-weight, float64, on the device (Engine.mcl_*).
   step        predict (odometry + noise, raster lookup, the touched keyframes listed on the device), the heads on
               LEFT = touched keyframes, RIGHT = the query (ovn_heads_1vsN), update (likelihood, normalisation,
@@ -33,8 +37,11 @@ import torch
 
 logger = logging.getLogger('overlapnet_b200.mcl')
 
+# None of these is tuned on KITTI.  render_sources = 8 comes from the synthetic street-scene study of DESIGN.md
+# section 7.
 DEFAULTS = dict(cell=0.5, max_distance=5.0, sigma_overlap=0.1, sigma_yaw_deg=10.0, rho=0.5, init_radius=1.0,
-                motion_sigma=(0.1, 0.1, math.radians(1.0)))
+                motion_sigma=(0.1, 0.1, math.radians(1.0)), render_sources=8)
+MAX_RENDER_SOURCES = 64
 
 
 # ---- geometry -----------------------------------------------------------------------------------------------
@@ -117,21 +124,41 @@ class MapIndex:
 class OverlapMCL:
   """Localize a scan stream in the map of ``map_clouds`` ((N, 4) float32 arrays or callables returning one) at the
   LiDAR-frame ``map_poses`` (K, 4, 4), with ``infer``'s network (an overlapnet_b200.Infer).  The map's volumes become
-  ``infer``'s resident bank; the particle set lives in its engine."""
+  ``infer``'s resident bank; the particle set lives in its engine.
+
+  With ``virtual_spacing`` G, the map frames are the lattice frames of virtual_map.lattice(map_poses, G,
+  max_distance), rendered from their ``render_sources`` nearest keyframe clouds within ``render_radius`` (default:
+  the handle's max_range); the raster is MapIndex(lattice xy, cell, max_distance=G).  ``keyframes`` holds the map
+  frames' planar poses either way."""
 
   def __init__(self, infer, map_clouds, map_poses, cell=DEFAULTS['cell'], max_distance=DEFAULTS['max_distance'],
                sigma_overlap=DEFAULTS['sigma_overlap'], sigma_yaw=math.radians(DEFAULTS['sigma_yaw_deg']),
-               rho=DEFAULTS['rho'], motion_sigma=DEFAULTS['motion_sigma']):
+               rho=DEFAULTS['rho'], motion_sigma=DEFAULTS['motion_sigma'], virtual_spacing=None,
+               render_sources=DEFAULTS['render_sources'], render_radius=None):
     from .lcd_eval import encode_share
     self.infer = infer
     self.engine = infer._engine
-    self.keyframes = planar(map_poses)
-    if len(map_clouds) != self.keyframes.shape[0]:
-      raise ValueError('%d map clouds for %d map poses' % (len(map_clouds), self.keyframes.shape[0]))
-    self.index = MapIndex(self.keyframes[:, :2], cell, max_distance)
+    map_poses = np.asarray(map_poses, np.float64)
+    if len(map_clouds) != map_poses.shape[0]:
+      raise ValueError('%d map clouds for %d map poses' % (len(map_clouds), map_poses.shape[0]))
+    self.max_distance = float(max_distance)
+    self.virtual_spacing = None if virtual_spacing is None else float(virtual_spacing)
     self.sigma_overlap, self.sigma_yaw, self.rho = float(sigma_overlap), float(sigma_yaw), float(rho)
     self.motion_sigma = tuple(float(s) for s in motion_sigma)
-    bank, _ = encode_share(infer, map_clouds)
+    if self.virtual_spacing is None:
+      self.keyframes = planar(map_poses)
+      self.index = MapIndex(self.keyframes[:, :2], cell, max_distance)
+      bank, _ = encode_share(infer, map_clouds)
+    else:
+      from . import virtual_map
+      if not 1 <= int(render_sources) <= MAX_RENDER_SOURCES:
+        raise ValueError('render_sources must be in [1, %d], got %s' % (MAX_RENDER_SOURCES, render_sources))
+      self.render_sources = int(render_sources)
+      self.render_radius = float(self.engine.cfg.max_range if render_radius is None else render_radius)
+      frames = virtual_map.lattice(map_poses, self.virtual_spacing, max_distance)
+      self.keyframes = planar(frames)
+      self.index = MapIndex(self.keyframes[:, :2], cell, self.virtual_spacing)
+      bank = virtual_map.encode(infer, map_clouds, map_poses, frames, self.render_sources, self.render_radius)
     # the tensor-core heads' numeric centres from keyframe 0, before the operand copies are built (as lcd_eval)
     self.engine.calibrate(bank[0])
     infer._set_bank(bank)
@@ -234,11 +261,15 @@ def evaluate_sequence(infer, clouds, poses, keyframe_stride=5, particles=100000,
   conv = np.array([convergence_step(pos_err[r], converged_m) for r in range(runs)], np.int64)
   summary = summarize(pos_err, yaw_err, conv, converged_m)
   summary.update(frames=len(clouds), keyframes=int(kf.size), queries=int(T), keyframe_stride=int(keyframe_stride),
-                 particles=int(particles), cell=mcl.index.cell, max_distance=mcl.index.max_distance,
+                 particles=int(particles), cell=mcl.index.cell, max_distance=mcl.max_distance,
                  sigma_overlap=mcl.sigma_overlap, sigma_yaw_deg=math.degrees(mcl.sigma_yaw), rho=mcl.rho)
   results = {'keyframes': kf, 'queries': q, 'truth': truth, 'odometry': odom, 'estimate': est,
              'position_error': pos_err, 'yaw_error': yaw_err, 'ess': ess, 'n_touched': n_touched,
              'resampled': resampled, 'convergence_step': conv}
+  if mcl.virtual_spacing is not None:
+    summary.update(virtual_spacing=mcl.virtual_spacing, render_sources=mcl.render_sources,
+                   render_radius=mcl.render_radius, map_frames=int(mcl.keyframes.shape[0]))
+    results['map_frames'] = mcl.keyframes
   if out_dir is not None:
     os.makedirs(out_dir, exist_ok=True)
     save_npz(os.path.join(out_dir, 'mcl_results.npz'), results)
@@ -262,6 +293,14 @@ def parse_args(argv):
                  help='metres from a keyframe a cell may be (default 5)')
   p.add_argument('--converged-m', type=float, default=2.0, help='position error of a converged run (default 2)')
   p.add_argument('--precision', default='f16_tc', choices=('f16_tc', 'fp32'))
+  p.add_argument('--virtual-spacing', type=float, default=None,
+                 help='localize in a map of virtual scans rendered on a lattice of this spacing in metres '
+                      '(default: the keyframe scans themselves)')
+  p.add_argument('--render-sources', type=int, default=DEFAULTS['render_sources'],
+                 help='keyframe clouds rendered into each virtual scan, 1..%d (default %d)'
+                      % (MAX_RENDER_SOURCES, DEFAULTS['render_sources']))
+  p.add_argument('--render-radius', type=float, default=None,
+                 help='metres from a virtual frame a rendered keyframe may be (default: the max_range)')
   args = p.parse_args(argv)
   if args.keyframe_stride < 2:
     p.error('--keyframe-stride must be at least 2, got %d' % args.keyframe_stride)
@@ -274,7 +313,21 @@ def parse_args(argv):
       p.error('--%s must be > 0' % name.replace('_', '-'))
   if not args.max_distance >= 0:
     p.error('--max-distance must be >= 0')
+  if args.virtual_spacing is not None and not (args.virtual_spacing > 0 and math.isfinite(args.virtual_spacing)):
+    p.error('--virtual-spacing must be > 0')
+  if not 1 <= args.render_sources <= MAX_RENDER_SOURCES:
+    p.error('--render-sources must be in [1, %d], got %d' % (MAX_RENDER_SOURCES, args.render_sources))
+  if args.render_radius is not None and not (args.render_radius > 0 and math.isfinite(args.render_radius)):
+    p.error('--render-radius must be > 0')
   return args
+
+
+def virtual_args(args):
+  """OverlapMCL's virtual-map arguments of the parsed command line: none without --virtual-spacing."""
+  if args.virtual_spacing is None:
+    return {}
+  return dict(virtual_spacing=args.virtual_spacing, render_sources=args.render_sources,
+              render_radius=args.render_radius)
 
 
 def network_config(config):
@@ -310,7 +363,7 @@ def main(argv=None):
   out_dir = os.path.join(net.get('experiments_path', '/tmp'), net.get('testname', 'experiment_test'))
   s, _ = evaluate_sequence(infer, clouds, poses, args.keyframe_stride, args.particles, args.runs, args.converged_m,
                            out_dir, cell=args.cell, max_distance=args.max_distance, sigma_overlap=args.sigma_overlap,
-                           sigma_yaw=math.radians(args.sigma_yaw_deg))
+                           sigma_yaw=math.radians(args.sigma_yaw_deg), **virtual_args(args))
   logger.info('MCL over %d frames: %d keyframes, %d queries, %d particles, %d runs', s['frames'], s['keyframes'],
               s['queries'], s['particles'], s['runs'])
   logger.info('  success rate (position error < %g m to the end): %f', s['converged_m'], s['success_rate'])
