@@ -452,6 +452,29 @@ int ovn_pgo_optimize_host(ovn_handle* h, int32_t n_graphs, const int64_t* node_o
                           const double* edge_weight, const ovn_pgo_params* params, double* out_poses,
                           ovn_pgo_result* out_result, double* out_chi2, double* out_scale, double* out_gradient,
                           ovn_pgo_trial* out_trace, void* stream);
+/* ovn_pgo_copy_workspace: h_out = one array of graph `graph` of the last successful ovn_pgo_optimize_host call,
+ * synchronously, as the kernel left it (DESIGN.md section 2, "Pose-graph stages").  n and E are the graph's nodes and
+ * edges; every array is float64, per node or per edge, in the graph's local order:
+ *   T, Tt [n][16]      the poses of the last accepted state and the last trial's poses
+ *   M [E][36], q [E][6]  each edge's rho' A^T W A and rho' A^T W e at T
+ *   Hd [n][36], gn [n][6]  each node's diagonal block and gradient at T
+ *   Ld, Ls, Lk [n][36]  the preconditioner's Cholesky blocks of the last factor: Ld of nodes 1 .. n-1; Ls (the block
+ *                      below node j) of the segment nodes that are not the last node n - 1; Lk (the spike to the left
+ *                      separator, or of separator q >= 2 the block to separator q - 1) of the nodes of segments 1 .. Q
+ *                      and of separators 2 .. Q
+ *   x, r, z, p, Ap [n][6]  the last trial's CG vectors, y [n][6] its last forward substitution, nodes 1 .. n-1
+ * Positions not listed (node 0 of Ld / Ls / Lk and of the vectors, Ls of the separators and of node n - 1, Lk of
+ * segment 0 and of the first separator) are never written and hold data of earlier calls; so does every array but
+ * T, M, q, Hd and gn after a call with max_iterations = 0 or whose trials all had g = 0.  After a trial is accepted
+ * M, q, Hd and gn are those of the new T, while the factor and the vectors stay those of the trial.
+ * Refused with OVN_ERR_INVALID_ARG: no successful call since the handle was created or since the last call that
+ * returned an error, `graph` or `array` out of range, or h_out NULL. */
+typedef enum ovn_pgo_array {
+  OVN_PGO_T = 0, OVN_PGO_TT = 1, OVN_PGO_M = 2, OVN_PGO_Q = 3, OVN_PGO_HD = 4, OVN_PGO_GN = 5, OVN_PGO_LD = 6,
+  OVN_PGO_LS = 7, OVN_PGO_LK = 8, OVN_PGO_X = 9, OVN_PGO_R = 10, OVN_PGO_Z = 11, OVN_PGO_P = 12, OVN_PGO_AP = 13,
+  OVN_PGO_Y = 14
+} ovn_pgo_array;
+int ovn_pgo_copy_workspace(ovn_handle* h, int32_t array, int32_t graph, double* h_out);
 
 /* ---- resident bank (Infer keeps self.feature_volumes across calls, infer.py:113,184-193) ---------
  * The tensor-core heads consume fp16 / hi-lo split copies of the LEFT volumes.  Without this call

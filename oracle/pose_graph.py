@@ -3,7 +3,8 @@
 and Levenberg-Marquardt with an exact sparse solve and the library's stopping rules.  Test infrastructure only.
 
 A graph is a dict of poses [n, 4, 4], edges [E, 2] (chain (k, k + 1) first), measurements [E, 4, 4] and weights
-[E, 6], as overlapnet_b200.pose_graph.chain_graph builds it."""
+[E, 6], as overlapnet_b200.pose_graph.chain_graph builds it.  The geometry (hat to jacobian, rho) keeps np.longdouble
+inputs in long double, so that oracle/pgo_stages.py can take it as an exact reference for the kernel's float64."""
 import numpy as np
 import scipy.sparse as sp
 import scipy.sparse.linalg as spla
@@ -15,9 +16,26 @@ DEFAULTS = dict(phi=25.0, lambda0=1e-6, lambda_min=1e-12, lambda_max=1e12, rel_c
 STATUS = ('converged', 'max_iterations', 'stalled', 'failed')
 
 
+def _f(x):
+  """x as float64, or as long double when it is long double"""
+  x = np.asarray(x)
+  return x if x.dtype == np.longdouble else x.astype(np.float64)
+
+
+def inv_rigid(T):
+  """[R | t]^-1 = [R^T | -R^T t], as the kernel inverts a pose or a measurement"""
+  T = _f(T)
+  out = np.zeros_like(T)
+  Rt = np.swapaxes(T[..., :3, :3], -1, -2)
+  out[..., :3, :3] = Rt
+  out[..., :3, 3] = -np.einsum('...ij,...j->...i', Rt, T[..., :3, 3])
+  out[..., 3, 3] = 1.0
+  return out
+
+
 def hat(v):
-  v = np.asarray(v, np.float64)
-  K = np.zeros(v.shape[:-1] + (3, 3))
+  v = _f(v)
+  K = np.zeros(v.shape[:-1] + (3, 3), v.dtype)
   K[..., 0, 1], K[..., 0, 2], K[..., 1, 2] = -v[..., 2], v[..., 1], -v[..., 0]
   K[..., 1, 0], K[..., 2, 0], K[..., 2, 1] = v[..., 2], -v[..., 1], v[..., 0]
   return K
@@ -25,8 +43,8 @@ def hat(v):
 
 def rodrigues(w):
   """R(omega) [..., 3, 3] = I + sin(th) K + (1 - cos(th)) K^2, K the cross-product matrix of the unit axis."""
-  w = np.asarray(w, np.float64)
-  th = np.linalg.norm(w, axis=-1)
+  w = _f(w)
+  th = np.sqrt(np.sum(w * w, -1))
   safe = np.where(th > 0, th, 1.0)
   K = hat(w / safe[..., None])
   s, c1 = np.sin(th)[..., None, None], (1 - np.cos(th))[..., None, None]
@@ -36,20 +54,20 @@ def rodrigues(w):
 
 def update(T, xi):
   """T <- [R(omega) | v] T of xi = (omega, v) [..., 6]."""
-  xi = np.asarray(xi, np.float64)
-  U = np.zeros(xi.shape[:-1] + (4, 4))
+  xi = _f(xi)
+  U = np.zeros(xi.shape[:-1] + (4, 4), xi.dtype)
   U[..., :3, :3] = rodrigues(xi[..., :3])
   U[..., :3, 3] = xi[..., 3:]
   U[..., 3, 3] = 1.0
-  return U @ np.asarray(T, np.float64)
+  return U @ _f(T)
 
 
 def log_so3(R):
   """phi [..., 3] of R [..., 3, 3]: the angle atan2(|axis| / 2, (tr R - 1) / 2) (registration.pose_error's), the axis
   from the antisymmetric part, or from the symmetric part above pi - PI_BRANCH."""
-  R = np.asarray(R, np.float64)
+  R = _f(R)
   ax = np.stack([R[..., 2, 1] - R[..., 1, 2], R[..., 0, 2] - R[..., 2, 0], R[..., 1, 0] - R[..., 0, 1]], -1)
-  sn = np.linalg.norm(ax, axis=-1)
+  sn = np.sqrt(np.sum(ax * ax, -1))
   cs = 0.5 * (np.trace(R, axis1=-2, axis2=-1) - 1.0)
   th = np.arctan2(0.5 * sn, cs)
   phi = np.where((sn > 0)[..., None], (th / np.where(sn > 0, sn, 1.0))[..., None] * ax, 0.0)
@@ -58,10 +76,10 @@ def log_so3(R):
     Rn, csn, thn, axn = R[near], cs[near], th[near], ax[near]
     d = np.diagonal(Rn, axis1=-2, axis2=-1)
     i = np.argmax(d, -1)
-    out = np.empty((Rn.shape[0], 3))
+    out = np.empty((Rn.shape[0], 3), R.dtype)
     for m in range(Rn.shape[0]):
       oc = 1.0 - csn[m]
-      k = np.empty(3)
+      k = np.empty(3, R.dtype)
       k[i[m]] = np.sqrt(max((Rn[m, i[m], i[m]] - csn[m]) / oc, 0.0))
       for j in range(3):
         if j != i[m]:
@@ -73,7 +91,7 @@ def log_so3(R):
 
 def jl_inv(phi):
   """J_l^-1(phi) = I - K / 2 + c K^2, c = 1 / th^2 - (1 + cos th) / (2 th sin th) (a series below SERIES_BELOW)."""
-  phi = np.asarray(phi, np.float64)
+  phi = _f(phi)
   t2 = np.sum(phi * phi, -1)
   th = np.sqrt(t2)
   with np.errstate(divide='ignore', invalid='ignore'):
@@ -89,7 +107,7 @@ def exp_so3(phi):
 
 def residual(Ta, Tb, Z):
   """e [..., 6] = (Log(R_E), t_E) of E = Z^-1 T_a^-1 T_b, and C = Z^-1 T_a^-1 [..., 4, 4]."""
-  C = np.linalg.inv(Z) @ np.linalg.inv(Ta)
+  C = inv_rigid(Z) @ inv_rigid(Ta)
   E = C @ Tb
   return np.concatenate([log_so3(E[..., :3, :3]), E[..., :3, 3]], -1), C
 
@@ -98,7 +116,7 @@ def jacobian(Ta, Tb, Z):
   """(e, A) with A = J_E Ad_C [..., 6, 6]: de/dxi_b = A and de/dxi_a = -A."""
   e, C = residual(Ta, Tb, Z)
   RC, tC = C[..., :3, :3], C[..., :3, 3]
-  A = np.zeros(e.shape[:-1] + (6, 6))
+  A = np.zeros(e.shape[:-1] + (6, 6), e.dtype)
   A[..., :3, :3] = jl_inv(e[..., :3]) @ RC
   A[..., 3:, :3] = hat(tC - e[..., 3:]) @ RC
   A[..., 3:, 3:] = RC
@@ -107,7 +125,7 @@ def jacobian(Ta, Tb, Z):
 
 def rho(x, loop, phi):
   """(rho(chi2), s): least squares on the chain (and for phi = inf), Geman-McClure on loops."""
-  x = np.asarray(x, np.float64)
+  x = _f(x)
   if np.isinf(phi):
     return x.copy(), np.ones_like(x)
   s = np.where(loop, phi / (phi + x), 1.0)

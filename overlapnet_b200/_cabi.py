@@ -34,7 +34,7 @@ SYMBOLS = [
     'ovn_rows_topk', 'ovn_heads_prefix_topk',
     'ovn_mcl_set_map', 'ovn_mcl_init', 'ovn_mcl_predict', 'ovn_mcl_update', 'ovn_mcl_copy_particles',
     'ovn_mcl_copy_stage', 'ovn_mcl_philox', 'ovn_icp_default_params', 'ovn_icp_pairs',
-    'ovn_pgo_default_params', 'ovn_pgo_optimize_host',
+    'ovn_pgo_default_params', 'ovn_pgo_optimize_host', 'ovn_pgo_copy_workspace',
 ]
 TOPK_MAX = 32     # ovn_rows_topk / ovn_heads_prefix_topk: k in [1, TOPK_MAX]
 MCL_INIT_MODES = {'global': 0, 'pose': 1}     # ovn_mcl_init_mode
@@ -48,6 +48,11 @@ PGO_MAX_NODES = 1 << 20
 PGO_MAX_EDGES = 1 << 22
 PGO_MAX_ITERATIONS = 1000
 PGO_MAX_CG_ITERATIONS = 10000
+# ovn_pgo_array: name -> (value, doubles per node or edge, per edge)
+PGO_ARRAYS = {'T': (0, 16, False), 'Tt': (1, 16, False), 'M': (2, 36, True), 'q': (3, 6, True), 'Hd': (4, 36, False),
+              'gn': (5, 6, False), 'Ld': (6, 36, False), 'Ls': (7, 36, False), 'Lk': (8, 36, False),
+              'x': (9, 6, False), 'r': (10, 6, False), 'z': (11, 6, False), 'p': (12, 6, False), 'Ap': (13, 6, False),
+              'y': (14, 6, False)}
 IPC_HANDLE_BYTES = 64     # ovn_shard_create / ovn_shard_open
 HEADS_STAGES = {'o1': 0, 'x3': 1, 'dense': 2, 'centres': 3}     # ovn_heads_stage
 TRAIN_PRECISIONS = {'fp32': 0, 'tf32x3': 1}     # ovn_train_precision
@@ -175,6 +180,7 @@ def lib():
   L.ovn_pgo_default_params.restype = None
   L.ovn_pgo_optimize_host.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, C.POINTER(PgoParams), vp, vp, vp, vp, vp, vp,
                                       vp]
+  L.ovn_pgo_copy_workspace.argtypes = [vp, i32, i32, vp]
   L.ovn_bank_release.argtypes = [vp, vp]
   L.ovn_check.argtypes = [vp, vp]
   L.ovn_set_feature_center.argtypes = [vp, vp]

@@ -991,6 +991,7 @@ int ovn_pgo_optimize_host(ovn_handle* h, int32_t n_graphs, const int64_t* node_o
                           ovn_pgo_result* out_result, double* out_chi2, double* out_scale, double* out_gradient,
                           ovn_pgo_trial* out_trace, void* stream) {
   if (!h) return OVN_ERR_INVALID_ARG;
+  h->pgo_node_off.clear();      // pgo_graphs records the call again when it succeeds
   DeviceGuard guard(h);
   REQUIRE(h, params && node_offset && edge_offset && poses && edge_nodes && edge_pose && edge_weight && out_poses &&
                  out_result && out_chi2 && out_scale, "NULL pointer");
@@ -1040,6 +1041,16 @@ int ovn_pgo_optimize_host(ovn_handle* h, int32_t n_graphs, const int64_t* node_o
   }
   return pgo_graphs(h, n_graphs, node_offset, edge_offset, poses, edge_nodes, edge_pose, edge_weight, p, out_poses,
                     out_result, out_chi2, out_scale, out_gradient, out_trace, (cudaStream_t)stream);
+}
+
+int ovn_pgo_copy_workspace(ovn_handle* h, int32_t array, int32_t graph, double* h_out) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  REQUIRE(h, !h->pgo_node_off.empty(), "no successful ovn_pgo_optimize_host call since the last refused or failed one");
+  REQUIRE(h, array >= OVN_PGO_T && array <= OVN_PGO_Y, "array is not an ovn_pgo_array");
+  REQUIRE(h, graph >= 0 && graph + 1 < (int64_t)h->pgo_node_off.size(), "graph is not a graph of the last call");
+  REQUIRE(h, h_out, "NULL pointer");
+  return pgo_copy_workspace(h, array, graph, h_out);
 }
 
 // ---- training precision ---------------------------------------------------------------------------

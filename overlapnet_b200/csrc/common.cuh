@@ -273,6 +273,10 @@ struct ovn_handle {
   std::vector<ovn::IpcMapping> open_shards;
   ovn::McState mcl;                          // ovn_mcl_*: map and particles, allocated by ovn_mcl_set_map / ovn_mcl_init
   ovn::Buffer<uint8_t> d_pgo;                // ovn_pgo_optimize_host: one call's inputs and workspace, grown on use
+  // where the last successful ovn_pgo_optimize_host call put its graphs and its arrays (ovn_pgo_array order) in
+  // d_pgo, for ovn_pgo_copy_workspace; pgo_node_off is empty when there is no such call
+  std::vector<int64_t> pgo_node_off, pgo_edge_off;
+  size_t pgo_array_off[15] = {};
   ovn::Buffer<uint8_t> d_render;             // ovn_render_*: one call's entry table, grown on use
   cudaStream_t own_stream = nullptr;
   // per-kernel profiling (ovn_profile_enable / ovn_profile_read)
@@ -504,6 +508,8 @@ int pgo_graphs(ovn_handle* h, int n_graphs, const int64_t* node_off, const int64
                const int32_t* edge_nodes, const double* edge_pose, const double* edge_weight,
                const ovn_pgo_params& prm, double* out_poses, ovn_pgo_result* out_result, double* out_chi2,
                double* out_scale, double* out_gradient, ovn_pgo_trial* out_trace, cudaStream_t s);
+// h_out = array `array` of graph `graph` of the call pgo_graphs recorded; the caller has checked both
+int pgo_copy_workspace(ovn_handle* h, int array, int graph, double* h_out);
 
 int corr_forward_fp32(ovn_handle* h, const float* d_bank, const float* d_query, const int32_t* left,
                       const int32_t* right, int np, int32_t* d_yaw, float* d_corr, cudaStream_t s);

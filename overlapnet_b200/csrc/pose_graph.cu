@@ -759,6 +759,22 @@ int pgo_graphs(ovn_handle* h, int n_graphs, const int64_t* node_off, const int64
   if (out_gradient) OVN_CUDA(h, down(out_gradient, p_gn));
   if (a.trace) OVN_CUDA(h, down(out_trace, p_tr));
   OVN_CUDA(h, cudaStreamSynchronize(s));
+  const Part* arrays[15] = {&p_T, &p_Tt, &p_M, &p_q, &p_Hd, &p_gn, &p_Ld, &p_Ls, &p_Lk,
+                            &p_vec[0], &p_vec[1], &p_vec[2], &p_vec[3], &p_vec[4], &p_vec[5]};
+  for (int v = 0; v < 15; ++v) h->pgo_array_off[v] = arrays[v]->off;
+  h->pgo_node_off.assign(node_off, node_off + n_graphs + 1);
+  h->pgo_edge_off.assign(edge_off, edge_off + n_graphs + 1);
+  return OVN_OK;
+}
+
+int pgo_copy_workspace(ovn_handle* h, int array, int graph, double* h_out) {
+  // doubles per node or per edge of each ovn_pgo_array, and whether it is per edge
+  static const int width[15] = {16, 16, 36, 6, 36, 6, 36, 36, 36, 6, 6, 6, 6, 6, 6};
+  const bool per_edge = array == OVN_PGO_M || array == OVN_PGO_Q;
+  const std::vector<int64_t>& off = per_edge ? h->pgo_edge_off : h->pgo_node_off;
+  const size_t first = (size_t)off[graph] * width[array], count = (size_t)(off[graph + 1] - off[graph]) * width[array];
+  const double* src = reinterpret_cast<const double*>(h->d_pgo.get() + h->pgo_array_off[array]) + first;
+  OVN_CUDA(h, cudaMemcpy(h_out, src, count * sizeof(double), cudaMemcpyDeviceToHost));
   return OVN_OK;
 }
 

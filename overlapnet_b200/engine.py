@@ -107,6 +107,7 @@ class Engine:
     self.Wf = L.ovn_feature_width(self._h)
     self.max_batch_scans = int(max_batch_scans)
     self.max_batch_pairs = int(max_batch_pairs)
+    self._pgo_sizes = []      # (n, E) of each graph of the last successful pose_graph call
 
   def close(self):
     if getattr(self, '_h', None) is not None and self._h.value:
@@ -700,7 +701,25 @@ class Engine:
     rc = lib().ovn_pgo_optimize_host(self._h, G, p(node_off), p(edge_off), p(poses), p(edges), p(measurements),
                                      p(weights), C.byref(params), p(out['poses']), p(out['result']), p(out['chi2']),
                                      p(out['scale']), p(out['gradient']), p(out['trace']), self._stream())
+    self._pgo_sizes = list(zip(np.diff(node_off).tolist(), np.diff(edge_off).tolist())) if rc == 0 else []
     return dict(out, rc=rc)
+
+  def pose_graph_workspace(self, name, graph=0):
+    """ovn_pgo_copy_workspace: array ``name`` ('T', 'Tt', 'M', 'q', 'Hd', 'gn', 'Ld', 'Ls', 'Lk', 'x', 'r', 'z', 'p',
+    'Ap' or 'y') of graph ``graph`` of the last successful pose_graph call, as a float64 host array: [n, 4, 4] for
+    T and Tt, [E, 6, 6] for M, [E, 6] for q, [n, 6, 6] for Hd, Ld, Ls and Lk, [n, 6] for the others.  Which positions
+    are defined is in include/ovn_b200.h.  Raises OvnError when there is no such call or graph."""
+    code, width, per_edge = _cabi.PGO_ARRAYS[name]
+    L = lib()
+    if not self._pgo_sizes or not 0 <= graph < len(self._pgo_sizes):
+      # the library refuses the copy and says why
+      check(self._h, L.ovn_pgo_copy_workspace(self._h, code, int(graph), None), 'ovn_pgo_copy_workspace')
+    count = self._pgo_sizes[graph][1 if per_edge else 0]
+    shape = {16: (count, 4, 4), 36: (count, 6, 6), 6: (count, 6)}[width]
+    out = np.empty(shape, np.float64)
+    check(self._h, L.ovn_pgo_copy_workspace(self._h, code, int(graph), out.ctypes.data_as(C.c_void_p)),
+          'ovn_pgo_copy_workspace')
+    return out
 
   def bank_prepare(self, bank, first=0, count=None):
     """Keep the tensor-core operand copies of bank rows [first, first+count) resident: later heads

@@ -164,6 +164,15 @@ def _runs(frames, positions):
 
 
 def _all_pairs_local(clouds, poses, frames, leg_output_width, device_budget_bytes, tile_cur, tile_ref):
+  try:
+    return _all_pairs_blocks(clouds, poses, frames, leg_output_width, device_budget_bytes, tile_cur, tile_ref)
+  finally:
+    # the scan staging buffer is half the free device memory by default: hand it back to the driver rather than
+    # leave it in torch's cache, where the library's own allocations (a new handle, its workspaces) cannot reach it
+    torch.cuda.empty_cache()
+
+
+def _all_pairs_blocks(clouds, poses, frames, leg_output_width, device_budget_bytes, tile_cur, tile_ref):
   eng = _engine(3.0, -25.0, 64, 900, 50)
   dev = eng.device
   n, F = len(clouds), len(frames)
