@@ -9,6 +9,8 @@ with the GPU's except where ``atan2`` / ``asin`` round differently at a bin edge
 """
 import numpy as np
 
+from . import gt as G
+
 F64 = np.float64
 
 DEFAULTS = dict(d_start=2.0, d_end=0.3, gamma=0.8, cos_normal=float(np.cos(np.deg2rad(30.0))), eps_rot=1e-6,
@@ -19,24 +21,14 @@ PIVOT = 1e-12
 
 def geometry(H=64, W=900, fov_up=3.0, fov_down=-25.0, max_range=50.0):
   """A handle's projection geometry; the angles and the range are float32 config values, as the handle stores them."""
-  return dict(H=int(H), W=int(W), fov_up=F64(np.float32(fov_up)), fov_down=F64(np.float32(fov_down)),
-              max_range=F64(np.float32(max_range)))
+  return G.geometry(H, W, fov_up, fov_down, max_range)
 
 
 def bins_f64(x, y, z, g):
-  """(keep, bx, by) of float64 points under range_projection (utils.py:75-104), as oracle/gt.range_image_f64 bins."""
-  up = g['fov_up'] / 180.0 * np.pi
-  down = g['fov_down'] / 180.0 * np.pi
-  fov = abs(down) + abs(up)
-  depth = np.sqrt((x * x + y * y) + z * z)
-  keep = (depth > 0) & (depth < g['max_range'])
-  with np.errstate(invalid='ignore', divide='ignore'):
-    yaw = -np.arctan2(y, x)
-    pitch = np.arcsin(np.where(keep, z / np.where(keep, depth, 1.0), 0.0))
-  px = np.floor((0.5 * (yaw / np.pi + 1.0)) * g['W'])
-  py = np.floor((1.0 - (pitch + abs(down)) / fov) * g['H'])
-  bx = np.maximum(0, np.minimum(g['W'] - 1, px)).astype(np.int64)
-  by = np.maximum(0, np.minimum(g['H'] - 1, py)).astype(np.int64)
+  """(keep, bx, by) of float64 points under range_projection (utils.py:75-104), the expression of
+  oracle/gt.range_image_f64 (oracle/gt.range_angles and angle_bins)."""
+  _, keep, yaw, pitch = G.range_angles(x, y, z, g)
+  bx, by = G.angle_bins(yaw, pitch, g)
   return keep, bx, by
 
 

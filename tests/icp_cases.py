@@ -49,3 +49,24 @@ def street_pair(k, seed=7, noise=0.0):
   from overlapnet_b200.synth import street_scene_cloud
   TL, TR = street_pose(*STREET_LEFT), street_pose(*STREET_RIGHT[k])
   return (street_scene_cloud(TL, seed, noise), street_scene_cloud(TR, seed, noise), np.linalg.solve(TL, TR))
+
+
+def pixel_centre_image(g, depth=10.0, nz=True, seed=3):
+  """(vertex [H, W, 4], normal [H, W, 3]) float32: every vertex on its own pixel's centre ray, a random unit normal
+  (with n_z = 0 when not ``nz``: no point constrains z, so H has rank 5)."""
+  H, W = g['H'], g['W']
+  down = abs(g['fov_down'] / 180.0 * np.pi)
+  fov = down + abs(g['fov_up'] / 180.0 * np.pi)
+  r, c = np.meshgrid(np.arange(H) + 0.5, np.arange(W) + 0.5, indexing='ij')
+  yaw = np.pi * (2.0 * c / W - 1.0)
+  pitch = (1.0 - r / H) * fov - down
+  v = np.ones((H, W, 4), np.float32)
+  v[..., 0] = depth * np.cos(pitch) * np.cos(-yaw)
+  v[..., 1] = depth * np.cos(pitch) * np.sin(-yaw)
+  v[..., 2] = depth * np.sin(pitch)
+  rng = np.random.default_rng(seed)
+  n = rng.normal(size=(H, W, 3))
+  if not nz:
+    n[..., 2] = 0.0
+  n /= np.linalg.norm(n, axis=-1, keepdims=True)
+  return v, n.astype(np.float32)
