@@ -294,11 +294,16 @@ int ovn_heads_prefix_topk(ovn_handle* h, const float* d_bank, int64_t bank_size,
  *                    RIGHT = the query; n must be the last predict's count (the pointers may be NULL when it is 0).
  *                    Adds each particle's log-likelihood, normalises, and resamples systematically when the ESS falls
  *                    below rho N.  sigma_overlap, sigma_yaw > 0 (radians), rho in [0, 1].  Synchronous: *h_est.
+ *                    An observed overlap that is not finite, or an update after which no particle has a finite
+ *                    log-weight, is OVN_ERR_INVALID_ARG (the message names which): the particle set and *h_est are
+ *                    unchanged, the predict still awaits its update and only its stages are held.
  *   ovn_mcl_copy_particles: d_out [4][N] float64 x, y, theta, log-weight of the current set, asynchronous.
  *   ovn_mcl_copy_stage: d_out = a stage of the last step, asynchronous: MOTION [3][N] f64 (x, y, theta after the last
  *                    predict), LOOKUP [N] i32 (the keyframe of each particle after it, -1 outside), LOGLIK [N] f64,
  *                    WEIGHTS [N] f64 (the normalised weights), PREFIX [N] f64 (their inclusive prefix sum) and
- *                    ANCESTORS [N] i32 of the last update; the last two only when it resampled.
+ *                    ANCESTORS [N] i32 of the last update, the last two only when it resampled; SCALARS [8] f64 of the
+ *                    last update: the max m of the updated log-weights, S = sum exp(lw - m), the ESS, x, y, theta,
+ *                    the resampling decision (1 or 0) and the resampling offset u0.
  *   ovn_mcl_philox:  d_out [n][4] = the Philox4x32-10 words of the counters d_ctr [n][4] under the seed (tests).
  * Invalid arguments, a call before ovn_mcl_set_map / ovn_mcl_init, an update without a predict and a stage the handle
  * does not hold are OVN_ERR_INVALID_ARG with nothing launched; the handle stays usable. */
@@ -312,7 +317,8 @@ typedef enum ovn_mcl_stage {
   OVN_MCL_STAGE_LOGLIK = 2,
   OVN_MCL_STAGE_WEIGHTS = 3,
   OVN_MCL_STAGE_PREFIX = 4,
-  OVN_MCL_STAGE_ANCESTORS = 5
+  OVN_MCL_STAGE_ANCESTORS = 5,
+  OVN_MCL_STAGE_SCALARS = 6
 } ovn_mcl_stage;
 typedef struct ovn_mcl_estimate {
   double x, y, theta;             /* weighted means; theta = atan2(sum w sin, sum w cos) */

@@ -38,7 +38,8 @@ SYMBOLS = [
 ]
 TOPK_MAX = 32     # ovn_rows_topk / ovn_heads_prefix_topk: k in [1, TOPK_MAX]
 MCL_INIT_MODES = {'global': 0, 'pose': 1}     # ovn_mcl_init_mode
-MCL_STAGES = {'motion': 0, 'lookup': 1, 'loglik': 2, 'weights': 3, 'prefix': 4, 'ancestors': 5}     # ovn_mcl_stage
+MCL_STAGES = {'motion': 0, 'lookup': 1, 'loglik': 2, 'weights': 3, 'prefix': 4, 'ancestors': 5,
+              'scalars': 6}                                                                      # ovn_mcl_stage
 MCL_MAX_PARTICLES = 1 << 24
 ICP_SYSTEM_SIZE = 29      # ovn_icp_pairs: d_system [np][ICP_SYSTEM_SIZE]
 ICP_STATUS = {'converged': 0, 'max_iterations': 1, 'degenerate': 2, 'too_few_inliers': 3, 'bad_index': 4}     # ovn_icp_status

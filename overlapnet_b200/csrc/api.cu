@@ -902,10 +902,11 @@ int ovn_mcl_copy_particles(ovn_handle* h, double* d_out, void* stream) {
 int ovn_mcl_copy_stage(ovn_handle* h, int32_t stage, void* d_out, void* stream) {
   if (!h) return OVN_ERR_INVALID_ARG;
   DeviceGuard guard(h);
-  REQUIRE(h, stage >= OVN_MCL_STAGE_MOTION && stage <= OVN_MCL_STAGE_ANCESTORS, "stage is not an ovn_mcl_stage");
+  REQUIRE(h, stage >= OVN_MCL_STAGE_MOTION && stage <= OVN_MCL_STAGE_SCALARS, "stage is not an ovn_mcl_stage");
   REQUIRE(h, d_out, "NULL pointer");
   const int need = stage <= OVN_MCL_STAGE_LOOKUP ? kMcHeldPredict
-                   : stage <= OVN_MCL_STAGE_WEIGHTS ? kMcHeldUpdate : kMcHeldResample;
+                   : stage <= OVN_MCL_STAGE_WEIGHTS || stage == OVN_MCL_STAGE_SCALARS ? kMcHeldUpdate
+                                                                                      : kMcHeldResample;
   if (!(h->mcl.stages & need))
     OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_mcl_copy_stage: stage %d is not held (no %s since the last init)", stage,
                 need == kMcHeldPredict ? "predict" : need == kMcHeldUpdate ? "update" : "update that resampled");

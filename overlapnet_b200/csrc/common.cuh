@@ -183,8 +183,10 @@ struct McMap {
 struct McParticles {
   double *x, *y, *th, *lw;
 };
-// the device scalars of one update: k_mcl_final writes them, the host reads [0, kScTouched)
-enum McScalar { kScMax = 0, kScExpSum, kScEss, kScX, kScY, kScTheta, kScResample, kScU0, kScTouched, kScCount };
+// the device scalars of one update: k_mcl_final writes them, the host reads [0, kScTouched); OVN_MCL_STAGE_SCALARS
+// copies [kScMax, kScU0]
+enum McScalar { kScMax = 0, kScExpSum, kScEss, kScX, kScY, kScTheta, kScResample, kScU0, kScRefused, kScTouched,
+                kScCount };
 constexpr int kMcPartialStride = 8;      // doubles per block partial
 constexpr int kMcMaxParticles = 1 << 24;
 constexpr int kMcMaxKeyframes = 1 << 24;

@@ -176,12 +176,14 @@ static __device__ __forceinline__ void block_reduce(double (&v)[V], double* __re
   }
 }
 
-// log l_i = -1/2 ((1 - O) / s_o)^2 - 1/2 (D / s_psi)^2; log-weights += log l; per-block max of the new log-weights
+// log l_i = -1/2 ((1 - O) / s_o)^2 - 1/2 (D / s_psi)^2 into ll_out; per-block max of the updated log-weights
+// lw + log l, and whether a touched overlap is not finite.  The log-weights themselves are left as they are: the
+// update writes them in k_mcl_normalize, once k_mcl_final has accepted the observations.
 static __global__ void __launch_bounds__(kMclThreads)
 k_mcl_loglik(McParticles p, int n, const int32_t* __restrict__ kidx, const int32_t* __restrict__ slot,
              const double* __restrict__ kf, const float* __restrict__ ov, const int32_t* __restrict__ yaw, int Wf,
              double s_o, double s_psi, double* __restrict__ ll_out, double* __restrict__ partial) {
-  double v[1] = {-INFINITY};
+  double v[2] = {-INFINITY, 0.0};
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const int k = kidx[i];
     double O = 0.0, D = kPi;
@@ -195,34 +197,37 @@ k_mcl_loglik(McParticles p, int n, const int32_t* __restrict__ kidx, const int32
       int64_t d = ((a - (int64_t)e) % Wf + Wf) % Wf;
       d = min(d, (int64_t)Wf - d);
       D = __dmul_rn((double)d, kTwoPi / (double)Wf);
+      if (!isfinite(O)) v[1] = 1.0;
     }
     const double t1 = (1.0 - O) / s_o, t2 = D / s_psi;
     const double ll = -0.5 * (t1 * t1) - 0.5 * (t2 * t2);
-    const double lw = p.lw[i] + ll;
     ll_out[i] = ll;
-    p.lw[i] = lw;
-    v[0] = fmax(v[0], lw);
+    v[0] = fmax(v[0], p.lw[i] + ll);
   }
-  block_reduce<1, true>(v, partial);
+  block_reduce<2, true>(v, partial);
 }
 
-// per-block sums of exp(lw - m), m = scal[kScMax]
+// per-block sums of exp(lw + ll - m), m = scal[kScMax]
 static __global__ void __launch_bounds__(kMclThreads)
-k_mcl_expsum(const double* __restrict__ lw, int n, const double* __restrict__ scal, double* __restrict__ partial) {
+k_mcl_expsum(const double* __restrict__ lw, const double* __restrict__ ll, int n, const double* __restrict__ scal,
+             double* __restrict__ partial) {
+  if (scal[kScRefused] != 0.0) return;
   const double m = scal[kScMax];
   double v[1] = {0.0};
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) v[0] += exp(lw[i] - m);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    v[0] += exp(lw[i] + ll[i] - m);
   block_reduce<1, false>(v, partial);
 }
 
-// lw -= m + log s; w = exp(lw); per-block sums of w, w^2, w x, w y, w sin theta, w cos theta
+// lw = lw + ll - (m + log s); w = exp(lw); per-block sums of w, w^2, w x, w y, w sin theta, w cos theta
 static __global__ void __launch_bounds__(kMclThreads)
-k_mcl_normalize(McParticles p, int n, const double* __restrict__ scal, double* __restrict__ w_out,
-                double* __restrict__ partial) {
+k_mcl_normalize(McParticles p, const double* __restrict__ ll, int n, const double* __restrict__ scal,
+                double* __restrict__ w_out, double* __restrict__ partial) {
+  if (scal[kScRefused] != 0.0) return;
   const double L = scal[kScMax] + log(scal[kScExpSum]);
   double v[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double lw = p.lw[i] - L;
+    const double lw = (p.lw[i] + ll[i]) - L;
     const double w = exp(lw);
     const double th = p.th[i];
     p.lw[i] = lw;
@@ -238,14 +243,17 @@ k_mcl_normalize(McParticles p, int n, const double* __restrict__ scal, double* _
 }
 
 // One block of kMclRedBlocks threads reduces the partials with a fixed tree, then finishes the stage:
-// mode 0: scal[kScMax] = max; mode 1: scal[kScExpSum] = sum; mode 2: the six sums, the ESS, the estimate, the
-// resampling decision and its offset u0.
+// mode 0: scal[kScMax] = max, scal[kScRefused] = 1 when a touched overlap is not finite, else 2 when no updated
+// log-weight is finite (the max is -inf), else 0, and no resampling until mode 2 decides; mode 1: scal[kScExpSum] =
+// sum; mode 2: the six sums, the ESS, the estimate, the resampling decision and its offset u0.  Modes 1 and 2 do
+// nothing once mode 0 has refused the update.
 static __global__ void __launch_bounds__(kMclRedBlocks)
 k_mcl_final(const double* __restrict__ partial, int n_parts, int mode, int n, double rho, uint64_t seed,
             uint32_t step, double* __restrict__ scal) {
   constexpr int V = 6;
   __shared__ double sm[V][kMclRedBlocks];
-  const int nv = mode == 2 ? V : 1;
+  if (mode != 0 && scal[kScRefused] != 0.0) return;
+  const int nv = mode == 2 ? V : mode == 0 ? 2 : 1;
   const bool is_max = mode == 0;
   for (int j = 0; j < nv; ++j)
     sm[j][threadIdx.x] = threadIdx.x < n_parts ? partial[threadIdx.x * kMcPartialStride + j] : (is_max ? -INFINITY : 0.0);
@@ -259,6 +267,8 @@ k_mcl_final(const double* __restrict__ partial, int n_parts, int mode, int n, do
   if (threadIdx.x != 0) return;
   if (mode == 0) {
     scal[kScMax] = sm[0][0];
+    scal[kScRefused] = sm[1][0] != 0.0 ? 1.0 : sm[0][0] == -INFINITY ? 2.0 : 0.0;
+    scal[kScResample] = 0.0;
   } else if (mode == 1) {
     scal[kScExpSum] = sm[0][0];
   } else {
@@ -443,15 +453,16 @@ int mcl_update(ovn_handle* h, const float* d_ov, const int32_t* d_yaw, double s_
   OVN_LAUNCH_CHECK(h);
   k_mcl_final<<<1, kMclRedBlocks, 0, s>>>(m.partial, G, 0, n, rho, m.seed, (uint32_t)m.step, scal);
   OVN_LAUNCH_CHECK(h);
-  k_mcl_expsum<<<G, kMclThreads, 0, s>>>(p.lw, n, scal, m.partial);
+  k_mcl_expsum<<<G, kMclThreads, 0, s>>>(p.lw, m.ll, n, scal, m.partial);
   OVN_LAUNCH_CHECK(h);
   k_mcl_final<<<1, kMclRedBlocks, 0, s>>>(m.partial, G, 1, n, rho, m.seed, (uint32_t)m.step, scal);
   OVN_LAUNCH_CHECK(h);
-  k_mcl_normalize<<<G, kMclThreads, 0, s>>>(p, n, scal, m.w, m.partial);
+  k_mcl_normalize<<<G, kMclThreads, 0, s>>>(p, m.ll, n, scal, m.w, m.partial);
   OVN_LAUNCH_CHECK(h);
   k_mcl_final<<<1, kMclRedBlocks, 0, s>>>(m.partial, G, 2, n, rho, m.seed, (uint32_t)m.step, scal);
   OVN_LAUNCH_CHECK(h);
-  // the resampling kernels read the decision on the device and return at once when there is none
+  // the resampling kernels read the decision on the device and return at once when there is none (k_mcl_final
+  // clears it when it refuses the update)
   k_mcl_tile_sums<<<n_tiles, kMclThreads, 0, s>>>(m.w, n, scal, m.tiles);
   OVN_LAUNCH_CHECK(h);
   k_mcl_tile_offsets<<<1, 32, 0, s>>>(m.tiles, n_tiles, scal);
@@ -464,6 +475,12 @@ int mcl_update(ovn_handle* h, const float* d_ov, const int32_t* d_yaw, double s_
   double* hs = m.host.get();
   OVN_CUDA(h, cudaMemcpyAsync(hs, scal, kScTouched * sizeof(double), cudaMemcpyDeviceToHost, s));
   OVN_CUDA(h, cudaStreamSynchronize(s));
+  // a refused update has written nothing to the particle set: the predict still awaits its update
+  if (hs[kScRefused] == 1.0)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_mcl_update: an observed overlap is not finite; the particles are unchanged");
+  if (hs[kScRefused] != 0.0)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG,
+                "ovn_mcl_update: no particle has a finite log-weight after the update; the particles are unchanged");
   est->x = hs[kScX];
   est->y = hs[kScY];
   est->theta = hs[kScTheta];
@@ -498,6 +515,11 @@ int mcl_copy_stage(ovn_handle* h, int stage, void* d_out, cudaStream_t s) {
     for (int j = 0; j < 3; ++j)
       OVN_CUDA(h, cudaMemcpyAsync(static_cast<double*>(d_out) + j * n, src[j], n * sizeof(double),
                                   cudaMemcpyDeviceToDevice, s));
+    return OVN_OK;
+  }
+  if (stage == OVN_MCL_STAGE_SCALARS) {
+    OVN_CUDA(h, cudaMemcpyAsync(d_out, m.scal.get() + kScMax, (kScU0 + 1 - kScMax) * sizeof(double),
+                                cudaMemcpyDeviceToDevice, s));
     return OVN_OK;
   }
   const void* src = stage == OVN_MCL_STAGE_LOOKUP ? (const void*)m.kidx.get()

@@ -590,10 +590,10 @@ class Engine:
 
   def mcl_stage(self, stage):
     """ovn_mcl_copy_stage: 'motion' [3, N] f64, 'lookup' [N] i32, 'loglik' / 'weights' / 'prefix' [N] f64,
-    'ancestors' [N] i32."""
+    'ancestors' [N] i32, 'scalars' [8] f64 (m, S, ess, x, y, theta, resampled, u0 of the last update)."""
     n = self._mcl_n
     shape, dtype = {'motion': ((3, n), torch.float64), 'lookup': ((n,), torch.int32),
-                    'ancestors': ((n,), torch.int32)}.get(stage, ((n,), torch.float64))
+                    'ancestors': ((n,), torch.int32), 'scalars': ((8,), torch.float64)}.get(stage, ((n,), torch.float64))
     out = torch.empty(shape, dtype=dtype, device=self.device)
     check(self._h, lib().ovn_mcl_copy_stage(self._h, _cabi.MCL_STAGES[stage], _ptr(out), self._stream()),
           'ovn_mcl_copy_stage')

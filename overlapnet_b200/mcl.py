@@ -35,6 +35,8 @@ import sys
 import numpy as np
 import torch
 
+from ._cabi import OvnError
+
 logger = logging.getLogger('overlapnet_b200.mcl')
 
 # None of these is tuned on KITTI.  render_sources = 8 comes from the synthetic street-scene study of DESIGN.md
@@ -186,7 +188,16 @@ class OverlapMCL:
     def observe(ids):
       ov, yaw, _ = eng.heads_1vsN(bank, query, cand_idx=ids)
       return ov, yaw
-    return self.step_observed(odom, observe)
+    try:
+      return self.step_observed(odom, observe)
+    except OvnError as refused:
+      # The tensor-core heads poison every output while a device error (a non-finite operand) is flagged, until
+      # ovn_check reports and clears it: check here, so that the next step's heads are clean again.
+      try:
+        eng.check()
+      except OvnError as flagged:
+        raise OvnError('%s; the heads flagged: %s' % (refused, flagged)) from refused
+      raise
 
   def step_observed(self, odom, observe):
     """One step with ``observe(ids)`` -> (overlap [n], yaw [n]) in place of the heads: ``ids`` is the int32 cuda

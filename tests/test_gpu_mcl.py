@@ -1,6 +1,6 @@
-"""Monte Carlo localization on the GPU: every stage of the filter modelled by oracle/mcl.py from the GPU's own input to
-it, determinism across handles, the network path against its host composition, convergence with a sensor that knows
-the true pose, and the refusals."""
+"""Monte Carlo localization on the GPU: the Philox words, determinism across handles, the network path against its host
+composition, convergence with a sensor that knows the true pose, and the refusals.  Every stage against its float64
+model is tests/test_gpu_mcl_stages.py."""
 import copy
 import math
 
@@ -38,10 +38,6 @@ def holey_map(seed, K=40):
   return kf, raster, idx
 
 
-def fake_observation(rng, n):
-  return rng.random(n).astype(np.float32), rng.integers(-180, 540, n).astype(np.int32)
-
-
 def _np(t):
   return t.cpu().numpy()
 
@@ -54,89 +50,6 @@ def test_philox_words_are_bit_exact(seed):
   ctr[:3] = [[0, 0, 0, 0], [2 ** 32 - 1] * 4, [1, 2, 3, 4]]
   got = _np(eng.mcl_philox(seed, ctr)).view(np.uint32)
   assert np.array_equal(got, om.philox(seed, ctr))
-  eng.close()
-
-
-@pytest.mark.parametrize('n', [1, 31, 1000, 65537, 10 ** 6])
-def test_every_stage_against_the_oracle(n):
-  eng = _engine()
-  kf, raster, idx = holey_map(n)
-  eng.mcl_set_map(kf, raster, idx.x0, idx.y0, idx.cell)
-  seed = 1234 + n
-  eng.mcl_init('global', n, seed, init_radius=6.0)
-  p = _np(eng.mcl_particles())
-  want = om.init_global(n, seed, kf, 6.0)
-  np.testing.assert_allclose(p, want, rtol=1e-12, atol=1e-12 * 100)
-  rng = np.random.default_rng(n)
-  excluded = 0
-  resampled_seen = 0
-  steps = 2 if n >= 10 ** 6 else 4
-  for step in range(1, steps + 1):
-    odom = (rng.uniform(-2, 2), rng.uniform(-1, 1), rng.uniform(-0.3, 0.3))
-    touched, nt = eng.mcl_predict(odom, SIGMA)
-    # motion from the particles before the predict
-    mo = _np(eng.mcl_stage('motion'))
-    x, y, th = om.motion(p[0], p[1], p[2], seed, step, odom, SIGMA)
-    np.testing.assert_allclose(mo[0], x, rtol=1e-12, atol=1e-12 * 100)
-    np.testing.assert_allclose(mo[1], y, rtol=1e-12, atol=1e-12 * 100)
-    np.testing.assert_allclose(mo[2], th, rtol=1e-12, atol=1e-12)
-    # lookup and the touched list from the GPU's motion output: exact
-    k = _np(eng.mcl_stage('lookup'))
-    assert np.array_equal(k, om.lookup(mo[0], mo[1], raster, idx.x0, idx.y0, idx.cell))
-    ids = om.touched(k, kf.shape[0])
-    assert nt == ids.size and np.array_equal(_np(touched[:nt]), ids)
-    if n >= 1000:
-      assert (k < 0).any() and (k >= 0).any()                # particles outside the raster and in its holes
-    # likelihood from the GPU's lookup and headings
-    ov, yaw = fake_observation(rng, nt)
-    if nt:
-      ov[0] = 1.0
-      yaw[-1] = 180 - om.expected_bin(om.wrap_pi(mo[2][k == ids[-1]][0] - kf[ids[-1], 2]), WIDTH)
-    rho = 1.0 if step % 2 else 0.0
-    est = eng.mcl_update(torch.as_tensor(ov).cuda() if nt else None, torch.as_tensor(yaw).cuda() if nt else None, nt,
-                         0.2, math.radians(15), rho)
-    ll = _np(eng.mcl_stage('loglik'))
-    np.testing.assert_allclose(ll, om.loglik(k, mo[2], kf[:, 2], ids, ov, yaw, WIDTH, 0.2, math.radians(15)),
-                               rtol=1e-12, atol=1e-12)
-    w = _np(eng.mcl_stage('weights'))
-    lw_want, w_want = om.normalize(p[3] + ll)
-    np.testing.assert_allclose(w, w_want, rtol=1e-12, atol=1e-12)
-    e = om.estimate(w, mo[0], mo[1], mo[2])
-    for key in ('x', 'y', 'theta'):
-      assert abs(est[key] - e[key]) <= 1e-9 * max(1.0, abs(e[key])), (key, est[key], e[key])
-    assert abs(est['ess'] - e['ess']) <= 1e-9 * e['ess']
-    assert est['n_touched'] == nt and est['step'] == step
-    assert est['resampled'] == (est['ess'] < rho * n)
-    p = _np(eng.mcl_particles())
-    if est['resampled']:
-      resampled_seen += 1
-      cdf = _np(eng.mcl_stage('prefix'))
-      np.testing.assert_allclose(cdf, np.cumsum(w), rtol=0, atol=1e-12)
-      anc = _np(eng.mcl_stage('ancestors'))
-      u0 = om.resample_u0(seed, step)
-      assert np.array_equal(anc, om.systematic(cdf, u0))      # from the GPU's own prefix sum: exact
-      host = om.systematic(np.cumsum(w), u0)                  # from the oracle's: exact away from near-ties
-      t = (np.arange(n) + u0) / n
-      near = np.abs(np.cumsum(w)[np.minimum(host, n - 1)] - t) <= 1e-12
-      near |= np.abs(np.cumsum(w)[np.maximum(np.minimum(host, n - 1) - 1, 0)] - t) <= 1e-12
-      excluded += int(np.count_nonzero(near & (anc != host)))
-      assert np.array_equal(anc[~near], host[~near])
-      assert np.array_equal(p[:3], mo[:, anc]) and np.all(p[3] == -np.log(n))
-    else:
-      assert np.array_equal(p[:3], mo)
-      np.testing.assert_allclose(p[3], lw_want, rtol=1e-12, atol=1e-12 * np.abs(lw_want).max())
-  print('n = %d: %d resampling steps, %d ancestors excluded as near-ties' % (n, resampled_seen, excluded))
-  assert resampled_seen >= 1 or n == 1
-  eng.close()
-
-
-def test_pose_init_against_the_oracle():
-  eng = _engine()
-  kf, raster, idx = holey_map(5)
-  eng.mcl_set_map(kf, raster, idx.x0, idx.y0, idx.cell)
-  eng.mcl_init('pose', 4097, 99, pose=(20.0, 10.0, 3.1), sigma=(1.0, 2.0, 0.5))
-  np.testing.assert_allclose(_np(eng.mcl_particles()), om.init_pose(4097, 99, (20.0, 10.0, 3.1), (1.0, 2.0, 0.5)),
-                             rtol=1e-12, atol=1e-12 * 100)
   eng.close()
 
 
@@ -255,7 +168,7 @@ def test_invalid_arguments_are_refused_and_the_handle_stays_usable():
   _refused(lambda: eng.mcl_init('global', 10, 1, init_radius=-1.0))
   _refused(lambda: eng.mcl_init('pose', 10, 1, pose=(0, 0, 0), sigma=(1, -1, 1)))
   eng.mcl_init('global', 1000, 1, init_radius=5.0)
-  for stage in ('motion', 'lookup', 'loglik', 'weights', 'prefix', 'ancestors'):
+  for stage in ('motion', 'lookup', 'loglik', 'weights', 'prefix', 'ancestors', 'scalars'):
     _refused(lambda: eng.mcl_stage(stage))                                             # nothing held yet
   _refused(lambda: eng.mcl_update(None, None, 0, 0.1, 0.1, 0.5))                         # update before predict
   _refused(lambda: eng.mcl_predict((1, 0, 0), (0.1, -0.1, 0.1)))                         # sigma < 0

@@ -35,13 +35,13 @@ def step_bytes(n, resampled):
   """DRAM bytes one predict + update moves for n particles (float64 x, y, theta, log-weight; int32 lookup), from the
   kernels' loads and stores; the map, touched list and partials are negligible.
     motion      reads x, y, theta (24), writes them (24) and the lookup (4)
-    loglik      reads lookup, theta, log-weight (20), writes log-weight and log-likelihood (16)
-    expsum      reads log-weight (8)
-    normalize   reads log-weight, x, y, theta (32), writes log-weight and weight (16)
+    loglik      reads lookup, theta, log-weight (20), writes the log-likelihood (8)
+    expsum      reads log-weight and log-likelihood (16)
+    normalize   reads log-weight, log-likelihood, x, y, theta (40), writes log-weight and weight (16)
     resampling  tile sums read the weights (8); the prefix reads them again and writes C (16); the resampling reads
                 each particle's ancestor (32) and C on its binary search (~8), writes the new set (32) and the
                 ancestor (4)"""
-  b = n * (24 + 24 + 4 + 20 + 16 + 8 + 32 + 16)
+  b = n * (24 + 24 + 4 + 20 + 8 + 16 + 40 + 16)
   if resampled:
     b += n * (8 + 16 + 32 + 8 + 32 + 4)
   return b
