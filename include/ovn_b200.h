@@ -97,7 +97,8 @@ int64_t     ovn_launch_count(const ovn_handle* h);
  * on the launching stream while enabled.  ovn_profile_read synchronises the device, returns the
  * accumulated milliseconds / launch count since the last read and resets them.  Names:
  * "delta_conv1", "conv2", "conv3", "corr", "project_scatter", "project_gather", "leg", "gather_rows",
- * "rows_topk", "pgo_graphs", "render_scatter", "render_gather". */
+ * "rows_topk", "pgo_graphs", "render_scatter", "render_gather", "surfel_build", "surfel_scatter",
+ * "surfel_gather". */
 int ovn_profile_enable(ovn_handle* h, int on);
 int ovn_profile_read(ovn_handle* h, const char* kernel, double* total_ms, int64_t* launches);
 
@@ -222,6 +223,51 @@ int ovn_render_batch(ovn_handle* h, const float* d_points, const int64_t* h_offs
 int ovn_render_preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int32_t n_clouds,
                                 int32_t n_virtual, const int64_t* h_entry_offsets, const int32_t* h_entry_cloud,
                                 const double* h_entry_pose, float* d_input, void* stream);
+
+/* ---- stage 1f: virtual scans rendered from surfels (DESIGN.md sections 4 and 7, "Surfel renders") -------------
+ * A keyframe's surfels are its projection's pixels (the handle's geometry and max_range): slot y W + x of its
+ * [H][W][8] float32 bank holds (cx, cy, cz, r, nx, ny, nz, intensity), c the pixel's vertex, n its normal (the
+ * sensor-facing -c / |c| where gen_normal_map leaves the (-1, -1, -1) fill) and r = fl32(((kappa d) delta) /
+ * max(|n.c| / d, c_min)) in float64, d the pixel's range and delta = max(2 pi / W, fov / H).  An empty pixel is an
+ * all-zero slot (r = 0, never drawn).  The defaults (kappa 1, c_min 0.5, max_splat 8) come from a synthetic street
+ * study, not from KITTI. */
+#define OVN_SURFEL_MAX_SPLAT_LIMIT 32
+typedef struct ovn_surfel_params {
+  double kappa;           /* radius scale, > 0 */
+  double c_min;           /* the least |cos| between a normal and its pixel's ray in the radius, (0, 1] */
+  int32_t max_splat;      /* a surfel is tested on the pixels within max_splat rows and columns of its centre, 0 .. 32 */
+} ovn_surfel_params;
+void ovn_surfel_default_params(ovn_surfel_params* p);
+/* The surfel banks of n_clouds clouds (d_points / d_offsets as for ovn_project_batch), d_surfels [n][H][W][8].
+ * Profiled as "project_scatter", "project_gather" and "surfel_build".  n_clouds > max_batch_scans is
+ * OVN_ERR_CAPACITY. */
+int ovn_surfels_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int32_t n_clouds,
+                      int64_t n_points_total, const ovn_surfel_params* params, float* d_surfels, void* stream);
+/* n_virtual images z-buffered from surfel banks, with the entry tables of ovn_render_batch (entry e: bank
+ * h_entry_cloud[e] of d_surfels [n_clouds][H][W][8], moved by h_entry_pose[e]).  d_rays [H][W][3] float64: the
+ * unit directions of the pixel centres (virtual_map.pixel_rays).  Per surfel, q = M (c, 1) in mat4_apply's order and
+ * m = R n, in float64 without contraction; it is culled when |q| - r >= max_range or fl32(q) has depth 0, and tested
+ * on the pixels within max_splat rows (clipped) and columns (circular) of fl32(q)'s projection pixel.  At pixel ray u:
+ * t = (m.q) / (m.u), drawn when |m.u| > 1e-6, t > 0, fl32(t) < max_range and |t u - q|^2 <= r^2.  The key is
+ * float_bits(fl32(t)) << 32 | (entry ordinal in the image * H W + slot), so the nearest hit wins, then the lowest
+ * entry, then the lowest slot.  The gather gives range fl32(t), vertex fl32(t u), the surfel's intensity, and
+ * d_winner = the key's index (its low 32 bits as int32), -1 where empty.  So each image is what the projection gives
+ * for a scan whose points are the hit points.  max_range < 0 selects the handle's.  The host tables get
+ * ovn_render_batch's checks and codes; an image of 2^32 / (H W) entries or more, a NULL d_surfels or d_rays with
+ * entries, and bad parameters (kappa <= 0, a non-finite value, c_min outside (0, 1], max_splat outside [0, 32]) are
+ * OVN_ERR_INVALID_ARG; n_virtual > max_batch_scans is OVN_ERR_CAPACITY.  Profiled as "surfel_scatter" and
+ * "surfel_gather". */
+int ovn_render_surfels_batch(ovn_handle* h, const float* d_surfels, int32_t n_clouds, const double* d_rays,
+                             int32_t n_virtual, const int64_t* h_entry_offsets /* [n_virtual+1] */,
+                             const int32_t* h_entry_cloud, const double* h_entry_pose /* [n_entries][16] */,
+                             const ovn_surfel_params* params, float max_range, float* d_range, float* d_vertex,
+                             float* d_intensity, int32_t* d_winner, void* stream);
+/* The surfel render packed as ovn_preprocess_batch packs a projection: d_input [n_virtual][H][W][C] at the handle's
+ * max_range.  OVN_ERR_BAD_CONFIG on a handle with probability channels: renders carry none. */
+int ovn_render_surfels_preprocess_batch(ovn_handle* h, const float* d_surfels, int32_t n_clouds, const double* d_rays,
+                                        int32_t n_virtual, const int64_t* h_entry_offsets,
+                                        const int32_t* h_entry_cloud, const double* h_entry_pose,
+                                        const ovn_surfel_params* params, float* d_input, void* stream);
 
 /* Pack separately computed cue images into the NHWC network input (same channel order). */
 int ovn_pack_input(ovn_handle* h, const float* d_depth, const float* d_normal, const float* d_prob,

@@ -17,7 +17,8 @@ SYMBOLS = [
     'ovn_launch_count', 'ovn_profile_enable', 'ovn_profile_read', 'ovn_set_weights', 'ovn_finalize_weights', 'ovn_project_batch',
     'ovn_normals_batch', 'ovn_semantic_batch', 'ovn_gt_range_batch', 'ovn_gt_overlap_count', 'ovn_gt_scan_radius',
     'ovn_gt_pairs_count', 'ovn_preprocess_batch', 'ovn_preprocess_cues_batch', 'ovn_render_batch',
-    'ovn_render_preprocess_batch',
+    'ovn_render_preprocess_batch', 'ovn_surfel_default_params', 'ovn_surfels_batch', 'ovn_render_surfels_batch',
+    'ovn_render_surfels_preprocess_batch',
     'ovn_pack_input',
     'ovn_leg_forward', 'ovn_heads_forward', 'ovn_heads_1vsN', 'ovn_bank_prepare', 'ovn_bank_release', 'ovn_encode_clouds_host',
     'ovn_query_cloud_vs_bank_host', 'ovn_check', 'ovn_set_feature_center', 'ovn_get_feature_center',
@@ -110,6 +111,13 @@ class PgoTrial(C.Structure):
   _fields_ = [('cost', C.c_double), ('lambda_', C.c_double), ('accepted', C.c_int32), ('cg_iterations', C.c_int32)]
 
 
+class SurfelParams(C.Structure):
+  """ovn_surfel_params"""
+  _fields_ = [('kappa', C.c_double), ('c_min', C.c_double), ('max_splat', C.c_int32)]
+
+
+SURFEL_MAX_SPLAT = 32     # ovn_surfel_params.max_splat in [0, SURFEL_MAX_SPLAT]
+SURFEL_FLOATS = 8         # ovn_surfels_batch: d_surfels [n][H][W][SURFEL_FLOATS]
 ICP_RESULT_BYTES = 152    # sizeof(ovn_icp_result): pose double[16], rms double, inliers, valid, iterations, status int32
 
 
@@ -159,6 +167,12 @@ def lib():
   L.ovn_preprocess_cues_batch.argtypes = [vp, vp, vp, i32, i64, vp, vp, vp]
   L.ovn_render_batch.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, f32, vp, vp, vp, vp, vp]
   L.ovn_render_preprocess_batch.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp]
+  L.ovn_surfel_default_params.argtypes = [C.POINTER(SurfelParams)]
+  L.ovn_surfel_default_params.restype = None
+  L.ovn_surfels_batch.argtypes = [vp, vp, vp, i32, i64, C.POINTER(SurfelParams), vp, vp]
+  L.ovn_render_surfels_batch.argtypes = [vp, vp, i32, vp, i32, vp, vp, vp, C.POINTER(SurfelParams), f32, vp, vp, vp,
+                                         vp, vp]
+  L.ovn_render_surfels_preprocess_batch.argtypes = [vp, vp, i32, vp, i32, vp, vp, vp, C.POINTER(SurfelParams), vp, vp]
   L.ovn_pack_input.argtypes = [vp, vp, vp, vp, vp, i32, vp, vp]
   L.ovn_leg_forward.argtypes = [vp, vp, i32, vp, vp]
   L.ovn_heads_forward.argtypes = [vp, vp, i64, vp, vp, i32, vp, vp, vp, vp]

@@ -343,7 +343,8 @@ int ovn_profile_read(ovn_handle* h, const char* kernel, double* total_ms, int64_
   if (!kernel || !total_ms || !launches) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_profile_read: NULL argument");
   static const char* names[kProfKinds] = {"delta_conv1", "conv2", "conv3", "corr", "project_scatter",
                                           "project_gather", "leg", "gather_rows", "rows_topk", "pgo_graphs",
-                                          "render_scatter", "render_gather"};
+                                          "render_scatter", "render_gather", "surfel_build", "surfel_scatter",
+                                          "surfel_gather"};
   int kind = -1;
   for (int i = 0; i < kProfKinds; ++i) if (strcmp(kernel, names[i]) == 0) kind = i;
   if (kind < 0) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "ovn_profile_read: unknown kernel '%s'", kernel);
@@ -610,6 +611,67 @@ int ovn_render_preprocess_batch(ovn_handle* h, const float* d_points, const int6
   REQUIRE(h, n_virtual == 0 || h_entry_offsets[n_virtual] == 0 || (h_entry_cloud && h_entry_pose), "NULL pointer");
   return render_preprocess_batch(h, d_points, h_offsets, n_clouds, n_virtual, h_entry_offsets, h_entry_cloud,
                                  h_entry_pose, d_input, (cudaStream_t)stream);
+}
+
+void ovn_surfel_default_params(ovn_surfel_params* p) {
+  if (!p) return;
+  p->kappa = 1.0;
+  p->c_min = 0.5;
+  p->max_splat = 8;
+}
+
+static int check_surfel_params(ovn_handle* h, const ovn_surfel_params* p, const char* fn) {
+  if (!p) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: NULL surfel parameters", fn);
+  if (!(std::isfinite(p->kappa) && std::isfinite(p->c_min)))
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: kappa and c_min must be finite", fn);
+  if (!(p->kappa > 0.0)) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: kappa must be > 0", fn);
+  if (!(p->c_min > 0.0 && p->c_min <= 1.0)) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: c_min must be in (0, 1]", fn);
+  if (p->max_splat < 0 || p->max_splat > OVN_SURFEL_MAX_SPLAT_LIMIT)
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "%s: max_splat must be in [0, %d]", fn, OVN_SURFEL_MAX_SPLAT_LIMIT);
+  return OVN_OK;
+}
+
+int ovn_surfels_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int32_t n_clouds,
+                      int64_t n_total, const ovn_surfel_params* params, float* d_surfels, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  int rc = check_surfel_params(h, params, __func__);
+  if (rc != OVN_OK) return rc;
+  REQUIRE(h, n_clouds >= 0 && n_total >= 0, "negative size");
+  REQUIRE(h, n_clouds == 0 || (d_offsets && d_surfels), "NULL pointer");
+  REQUIRE(h, n_total == 0 || d_points, "NULL pointer");
+  return surfels_batch(h, d_points, d_offsets, n_clouds, n_total, *params, d_surfels, (cudaStream_t)stream);
+}
+
+int ovn_render_surfels_batch(ovn_handle* h, const float* d_surfels, int32_t n_clouds, const double* d_rays,
+                             int32_t n_virtual, const int64_t* h_entry_offsets, const int32_t* h_entry_cloud,
+                             const double* h_entry_pose, const ovn_surfel_params* params, float max_range,
+                             float* d_range, float* d_vertex, float* d_intensity, int32_t* d_winner, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  int rc = check_surfel_params(h, params, __func__);
+  if (rc != OVN_OK) return rc;
+  REQUIRE(h, n_clouds >= 0 && n_virtual >= 0, "negative size");
+  REQUIRE(h, n_virtual == 0 || h_entry_offsets, "NULL pointer");
+  REQUIRE(h, n_virtual == 0 || h_entry_offsets[n_virtual] == 0 || (h_entry_cloud && h_entry_pose), "NULL pointer");
+  return render_surfels_batch(h, d_surfels, n_clouds, d_rays, n_virtual, h_entry_offsets, h_entry_cloud,
+                              h_entry_pose, *params, max_range, d_range, d_vertex, d_intensity, d_winner,
+                              (cudaStream_t)stream);
+}
+
+int ovn_render_surfels_preprocess_batch(ovn_handle* h, const float* d_surfels, int32_t n_clouds, const double* d_rays,
+                                        int32_t n_virtual, const int64_t* h_entry_offsets,
+                                        const int32_t* h_entry_cloud, const double* h_entry_pose,
+                                        const ovn_surfel_params* params, float* d_input, void* stream) {
+  if (!h) return OVN_ERR_INVALID_ARG;
+  DeviceGuard guard(h);
+  int rc = check_surfel_params(h, params, __func__);
+  if (rc != OVN_OK) return rc;
+  REQUIRE(h, n_clouds >= 0 && n_virtual >= 0, "negative size");
+  REQUIRE(h, n_virtual == 0 || (h_entry_offsets && d_input), "NULL pointer");
+  REQUIRE(h, n_virtual == 0 || h_entry_offsets[n_virtual] == 0 || (h_entry_cloud && h_entry_pose), "NULL pointer");
+  return render_surfels_preprocess_batch(h, d_surfels, n_clouds, d_rays, n_virtual, h_entry_offsets, h_entry_cloud,
+                                         h_entry_pose, *params, d_input, (cudaStream_t)stream);
 }
 
 int ovn_pack_input(ovn_handle* h, const float* d_depth, const float* d_normal, const float* d_prob,

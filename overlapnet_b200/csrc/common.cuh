@@ -69,7 +69,8 @@ static_assert(sizeof(float) == sizeof(int32_t), "the three staging arrays are 4 
 constexpr int kFeatC = 128;           // leg output channels (generateNet.py:214)
 constexpr int kMaxLegLayers = 12;
 enum ProfKind { PROF_DELTA = 0, PROF_CONV2, PROF_CONV3, PROF_CORR, PROF_SCATTER, PROF_GATHER, PROF_LEG, PROF_GATHER_ROWS,
-                PROF_ROWS_TOPK, PROF_PGO, PROF_RENDER_SCATTER, PROF_RENDER_GATHER, kProfKinds };
+                PROF_ROWS_TOPK, PROF_PGO, PROF_RENDER_SCATTER, PROF_RENDER_GATHER, PROF_SURFEL_BUILD, PROF_SURFEL_SCATTER,
+                PROF_SURFEL_GATHER, kProfKinds };
 
 // The one owner of another process's shard mapped by ovn_shard_open (cudaIpcOpenMemHandle); unmaps it on
 // destruction.  Move-only, like Buffer.
@@ -280,6 +281,7 @@ struct ovn_handle {
   std::vector<int64_t> pgo_node_off, pgo_edge_off;
   size_t pgo_array_off[15] = {};
   ovn::Buffer<uint8_t> d_render;             // ovn_render_*: one call's entry table, grown on use
+  ovn::Buffer<uint8_t> d_surfel;             // ovn_surfels_batch: one call's projection images, grown on use
   cudaStream_t own_stream = nullptr;
   // per-kernel profiling (ovn_profile_enable / ovn_profile_read)
   bool profiling = false;
@@ -426,6 +428,17 @@ int render_batch(ovn_handle* h, const float* d_points, const int64_t* h_offsets,
 int render_preprocess_batch(ovn_handle* h, const float* d_points, const int64_t* h_offsets, int n_clouds,
                             int n_virtual, const int64_t* h_entry_offsets, const int32_t* h_entry_cloud,
                             const double* h_entry_pose, float* d_input, cudaStream_t s);
+// surfels and their renders (projection.cu); the parameters are checked by the entry points
+int surfels_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans, int64_t n_total,
+                  const ovn_surfel_params& prm, float* d_surfels, cudaStream_t s);
+int render_surfels_batch(ovn_handle* h, const float* d_surfels, int n_clouds, const double* d_rays, int n_virtual,
+                         const int64_t* h_entry_offsets, const int32_t* h_entry_cloud, const double* h_entry_pose,
+                         const ovn_surfel_params& prm, float max_range, float* d_range, float* d_vertex,
+                         float* d_intensity, int32_t* d_winner, cudaStream_t s);
+int render_surfels_preprocess_batch(ovn_handle* h, const float* d_surfels, int n_clouds, const double* d_rays,
+                                    int n_virtual, const int64_t* h_entry_offsets, const int32_t* h_entry_cloud,
+                                    const double* h_entry_pose, const ovn_surfel_params& prm, float* d_input,
+                                    cudaStream_t s);
 int pack_input(ovn_handle* h, const float* d_depth, const float* d_normal, const float* d_prob,
                const float* d_intensity, int n_scans, float* d_input, cudaStream_t s);
 

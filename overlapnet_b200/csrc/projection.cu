@@ -145,7 +145,9 @@ struct RawPoints {
     return (uint32_t)(g - seg_start);
   }
   __device__ __forceinline__ int64_t base(int b) const { return __ldg(offsets + b); }
-  __device__ __forceinline__ float4 winner(int b, int64_t base, uint32_t k) const { return __ldg(pts + base + k); }
+  __device__ __forceinline__ float4 winner(int b, int64_t base, uint32_t k, int, int) const {
+    return __ldg(pts + base + k);
+  }
 };
 
 // One render entry (ovn_render_batch): a resident cloud moved by a float64 pose into a virtual frame.
@@ -179,7 +181,7 @@ struct PosedPoints {
     return (uint32_t)(g - ent[e].image_base);
   }
   __device__ __forceinline__ int64_t base(int b) const { return seg[first[b]]; }
-  __device__ __forceinline__ float4 winner(int b, int64_t base, uint32_t k) const {
+  __device__ __forceinline__ float4 winner(int b, int64_t base, uint32_t k, int, int) const {
     const int64_t e0 = first[b], g = base + k;
     const int e = (int)e0 + find_scan(seg + e0, (int)(first[b + 1] - e0), g);
     return point(e, g);
@@ -431,7 +433,7 @@ k_project_gather(const Src src, ProjParams P, const unsigned long long* __restri
       if (k != kEmptyKey) {
         depth = __uint_as_float((uint32_t)(k >> 32));
         local = (uint32_t)(k & 0xFFFFFFFFull);
-        p = src.winner(b, off, local);
+        p = src.winner(b, off, local, y, x);
       }
     }
     s_pt[ry][rx] = p;
@@ -808,6 +810,345 @@ int render_preprocess_batch(ovn_handle* h, const float* d_points, const int64_t*
     OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG, "render_preprocess: the handle has probability channels, which renders lack");
   return render(h, d_points, h_offsets, n_clouds, n_virtual, h_entry_offsets, h_entry_cloud, h_entry_pose,
                 h->cfg.max_range, packed_channels(h, nullptr, d_input), s);
+}
+
+// ---- surfel renders: oriented disks from the keyframes' range images (DESIGN.md section 7, "Surfel renders") ------
+// A keyframe's surfels are its projection's pixels: slot y W + x of its [H][W] bank holds two float4, (cx, cy, cz, r)
+// and (nx, ny, nz, intensity); an empty pixel is an all-zero slot (r = 0, never drawn).
+struct SurfelBuild {
+  double kappa, c_min, delta;   // r = fl32(((kappa d) delta) / max(|n.c| / d, c_min)), delta = max(2 pi / W, fov / H)
+};
+
+// One thread per pixel of the projection's outputs.  Every float64 operation is rounded once (no contraction).
+__global__ void __launch_bounds__(256)
+k_surfel_build(const float* __restrict__ range, const float4* __restrict__ vertex, const float* __restrict__ intensity,
+               const float* __restrict__ normal, size_t n_pix, SurfelBuild B, float4* __restrict__ out) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_pix) return;
+  const float d = range[i];
+  if (!(d > 0.0f)) {
+    out[2 * i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    out[2 * i + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
+    return;
+  }
+  const float4 c = vertex[i];
+  const double cx = c.x, cy = c.y, cz = c.z;
+  float n0 = normal[3 * i], n1 = normal[3 * i + 1], n2 = normal[3 * i + 2];
+  if (n0 == -1.f && n1 == -1.f && n2 == -1.f) {   // gen_normal_map's fill: the sensor-facing unit vector -c / |c|
+    const double nc = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(cx, cx), __dmul_rn(cy, cy)), __dmul_rn(cz, cz)));
+    n0 = __double2float_rn(__ddiv_rn(-cx, nc));
+    n1 = __double2float_rn(__ddiv_rn(-cy, nc));
+    n2 = __double2float_rn(__ddiv_rn(-cz, nc));
+  }
+  const double dot = __dadd_rn(__dadd_rn(__dmul_rn((double)n0, cx), __dmul_rn((double)n1, cy)),
+                               __dmul_rn((double)n2, cz));
+  const double den = fmax(__ddiv_rn(fabs(dot), (double)d), B.c_min);
+  const float r = __double2float_rn(__ddiv_rn(__dmul_rn(__dmul_rn(B.kappa, (double)d), B.delta), den));
+  out[2 * i] = make_float4(c.x, c.y, c.z, r);
+  out[2 * i + 1] = make_float4(n0, n1, n2, intensity[i]);
+}
+
+// The entries of a surfel render (RenderEntry: M, cloud_start = the first slot of its keyframe's bank, image_base =
+// the first entry of its image, image) with the banks, the pixel rays and the window's scales.
+struct SurfelRender {
+  const float4* __restrict__ surfels;   // [n_clouds][H][W][2]
+  const RenderEntry* __restrict__ ent;  // [n_entries]
+  const int64_t* __restrict__ first;    // [n_images + 1] first entry of each image
+  const double* __restrict__ rays;      // [H][W][3] unit directions of the pixel centres
+  double rows_per_rad, cols_per_rad;    // H / fov, W / (2 pi)
+  int S;                                // max_splat
+};
+
+// q = M (c, 1) in mat4_apply's order, m = R n: float64, every product and sum rounded once
+__device__ __forceinline__ void surfel_pose(const double* __restrict__ M, const float4 a, const float4 b, double q[3],
+                                            double m[3]) {
+  const double cx = a.x, cy = a.y, cz = a.z, nx = b.x, ny = b.y, nz = b.z;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    q[i] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(M[4 * i], cx), __dmul_rn(M[4 * i + 1], cy)),
+                               __dmul_rn(M[4 * i + 2], cz)), M[4 * i + 3]);
+    m[i] = __dadd_rn(__dadd_rn(__dmul_rn(M[4 * i], nx), __dmul_rn(M[4 * i + 1], ny)), __dmul_rn(M[4 * i + 2], nz));
+  }
+}
+
+__device__ __forceinline__ double dot3_rn(const double a[3], const double* b) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(a[0], b[0]), __dmul_rn(a[1], b[1])), __dmul_rn(a[2], b[2]));
+}
+
+// The ray u meets the plane (q, m) at t = (m.q) / (m.u); the pixel is drawn when |m.u| > 1e-6, t > 0,
+// fl32(t) < max_range and |t u - q|^2 <= r^2.
+__device__ __forceinline__ bool surfel_hit(const double q[3], const double m[3], double r2, const double* u,
+                                           float max_range, double& t) {
+  const double uu[3] = {__ldg(u), __ldg(u + 1), __ldg(u + 2)};
+  const double den = dot3_rn(m, uu), num = dot3_rn(m, q);
+  if (!(fabs(den) > 1e-6)) return false;
+  t = __ddiv_rn(num, den);
+  if (!(t > 0.0) || !(__double2float_rn(t) < max_range)) return false;
+  const double d0 = __dsub_rn(__dmul_rn(t, uu[0]), q[0]), d1 = __dsub_rn(__dmul_rn(t, uu[1]), q[1]);
+  const double d2 = __dsub_rn(__dmul_rn(t, uu[2]), q[2]);
+  return __dadd_rn(__dadd_rn(__dmul_rn(d0, d0), __dmul_rn(d1, d1)), __dmul_rn(d2, d2)) <= r2;
+}
+
+// Half-widths (rows hy, columns hx) of the box around the centre pixel that holds every pixel the surfel can draw,
+// at most S.  A drawn ray lies within a = asin(r / |q|) of q (r < |q|), so its pitch differs from q's by at most a
+// and its azimuth by at most 2 asin(sin(a / 2) / cos(|pitch_q| + a)) (haversine); in pixels that is at most
+// a H / fov + 1/2 rows and that azimuth W / (2 pi) + 1/2 columns from the centre pixel.  ceil(.) + 1 adds at least
+// 1/2 pixel more than that, which covers libm's errors here and the float32 bins of the centre many times over
+// (DESIGN.md section 7).  NaN anywhere gives the full window.
+__device__ __forceinline__ void surfel_window(double qz, double nq, double r, const SurfelRender& R, int& hy,
+                                             int& hx) {
+  hy = hx = R.S;
+  if (!(r < nq)) return;
+  const double a = asin(r / nq);
+  hy = (int)fmin((double)R.S, ceil(a * R.rows_per_rad) + 1.0);
+  const double p = fabs(asin(qz / nq)) + a;
+  if (p < 1.5707963267948966) {
+    const double s = sin(0.5 * a) / cos(p);
+    if (s < 1.0) hx = (int)fmin((double)R.S, ceil(2.0 * asin(s) * R.cols_per_rad) + 1.0);
+  }
+}
+
+// One lane's surfel in the scatter's flattened pixel loop.
+struct SurfelLane {
+  double q[3], m[3], r2;
+  int y0, x0, ncols, image;   // box rows y0 .., columns x0 .. x0 + ncols - 1 (mod W)
+  uint32_t key;               // the entry's ordinal in its image * H W + slot
+};
+
+// K1 of the surfel render.  grid = ceil(n_entries H W / 256), block = 256; thread i takes (entry, slot) = (i / HW,
+// i % HW).  Each lane moves its surfel, culls it and forms its box; a warp prefix over the box areas flattens the
+// warp's (surfel, pixel) list, and the 32 lanes stride over it, so a warp's lanes stay busy whatever the boxes'
+// sizes (0 to (2S + 1)^2 pixels).  Key: float_bits(fl32(t)) << 32 | key, 64-bit atomicMin.
+__global__ void __launch_bounds__(256)
+k_surfel_scatter(const SurfelRender R, int64_t n_items, ProjParams P, unsigned long long* __restrict__ keys) {
+  __shared__ SurfelLane s_lane[8][32];
+  __shared__ int s_start[8][32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int HW = P.H * P.W;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  int area = 0;
+  if (i < n_items) {
+    const int64_t e = i / HW;
+    const int slot = (int)(i - e * HW);
+    const RenderEntry& E = R.ent[e];
+    const float4* rec = R.surfels + 2 * (E.cloud_start + slot);
+    const float4 a = __ldg(rec);
+    if (a.w > 0.0f) {
+      SurfelLane& L = s_lane[wid][lane];
+      surfel_pose(E.M, a, __ldg(rec + 1), L.q, L.m);
+      const double nq = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(L.q[0], L.q[0]), __dmul_rn(L.q[1], L.q[1])),
+                                             __dmul_rn(L.q[2], L.q[2])));
+      const double r = (double)a.w;
+      if (nq > 0.0 && __dsub_rn(nq, r) < (double)P.max_range) {
+        const float4 c = make_float4(__double2float_rn(L.q[0]), __double2float_rn(L.q[1]), __double2float_rn(L.q[2]),
+                                     0.f);
+        const float depth = point_depth(c);
+        if (depth > 0.0f) {
+          int bx, by, hy, hx;
+          point_bins(c, depth, P, bx, by);
+          surfel_window(L.q[2], nq, r, R, hy, hx);
+          const int y0 = max(0, by - hy), y1 = min(P.H - 1, by + hy);
+          L.r2 = __dmul_rn(r, r);
+          L.y0 = y0;
+          L.x0 = bx - hx;
+          L.ncols = 2 * hx + 1;
+          L.image = E.image;
+          L.key = (uint32_t)((e - E.image_base) * HW + slot);
+          area = (y1 - y0 + 1) * L.ncols;
+        }
+      }
+    }
+  }
+  int incl = area;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  s_start[wid][lane] = incl - area;
+  const int total = __shfl_sync(0xffffffffu, incl, 31);
+  __syncwarp();
+  for (int k = lane; k < total; k += 32) {
+    // the owner: the last lane whose box starts at or before k (a lane with an empty box shares its start with the
+    // next lane, so the last such lane has a box)
+    int o = 0;
+#pragma unroll
+    for (int step = 16; step > 0; step >>= 1)
+      if (s_start[wid][o + step] <= k) o += step;
+    const SurfelLane& L = s_lane[wid][o];
+    const int local = k - s_start[wid][o];
+    const int row = local / L.ncols;
+    const int y = L.y0 + row;
+    int x = (L.x0 + (local - row * L.ncols)) % P.W;
+    if (x < 0) x += P.W;
+    double t;
+    if (surfel_hit(L.q, L.m, L.r2, R.rays + 3 * ((size_t)y * P.W + x), P.max_range, t)) {
+      const unsigned long long key = ((unsigned long long)__float_as_uint(__double2float_rn(t)) << 32) | L.key;
+      atomicMin(keys + (size_t)L.image * HW + (size_t)y * P.W + x, key);
+    }
+  }
+}
+
+// The gather's source of a surfel render: image b's key index k is (entry ordinal) H W + slot; the winner's point is
+// its hit on the pixel's ray, recomputed as the scatter computed it: (fl32(t u), intensity).
+struct SurfelHits {
+  static constexpr bool kRanked = false;     // d_winner is the key's index itself
+  SurfelRender R;
+  int HW, W;
+  __device__ __forceinline__ int64_t base(int b) const { return R.first[b]; }
+  __device__ __forceinline__ float4 winner(int b, int64_t base, uint32_t k, int y, int x) const {
+    const int64_t e = base + k / (uint32_t)HW;
+    const int slot = (int)(k % (uint32_t)HW);
+    const RenderEntry& E = R.ent[e];
+    const float4* rec = R.surfels + 2 * (E.cloud_start + slot);
+    const float4 b1 = __ldg(rec + 1);
+    double q[3], m[3];
+    surfel_pose(E.M, __ldg(rec), b1, q, m);
+    const double* u = R.rays + 3 * ((size_t)y * W + x);
+    const double uu[3] = {__ldg(u), __ldg(u + 1), __ldg(u + 2)};
+    const double t = __ddiv_rn(dot3_rn(m, q), dot3_rn(m, uu));
+    return make_float4(__double2float_rn(__dmul_rn(t, uu[0])), __double2float_rn(__dmul_rn(t, uu[1])),
+                       __double2float_rn(__dmul_rn(t, uu[2])), b1.w);
+  }
+};
+
+static double surfel_delta(const ovn_handle* h) {
+  const double pi = 3.14159265358979323846;
+  const double fu = (double)h->cfg.fov_up_deg / 180.0 * pi, fd = (double)h->cfg.fov_down_deg / 180.0 * pi;
+  return fmax(2.0 * pi / h->cfg.proj_W, (fabs(fd) + fabs(fu)) / h->cfg.proj_H);
+}
+
+int surfels_batch(ovn_handle* h, const float* d_points, const int64_t* d_offsets, int n_scans, int64_t n_total,
+                  const ovn_surfel_params& prm, float* d_surfels, cudaStream_t s) {
+  if (n_scans <= 0) return OVN_OK;
+  if (n_scans > h->cfg.max_batch_scans)
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "n_scans=%d exceeds max_batch_scans=%d", n_scans, h->cfg.max_batch_scans);
+  const size_t n_pix = (size_t)n_scans * h->cfg.proj_H * h->cfg.proj_W;
+  // the projection's outputs: vertex (16 B), range, intensity (4 B) and normal (12 B) per pixel
+  int rc = h->d_surfel.ensure(h, n_pix * 36);
+  if (rc != OVN_OK) return rc;
+  GatherOut out = {};
+  out.vertex = reinterpret_cast<float*>(h->d_surfel.get());
+  out.range = out.vertex + 4 * n_pix;
+  out.intensity = out.range + n_pix;
+  out.normal = out.intensity + n_pix;
+  out.c_depth = out.c_normal = out.c_prob = out.c_intensity = -1;
+  rc = run_projection(h, d_points, d_offsets, n_scans, n_total, h->cfg.max_range, out, s);
+  if (rc != OVN_OK) return rc;
+  const SurfelBuild B = {prm.kappa, prm.c_min, surfel_delta(h)};
+  prof_mark(h, PROF_SURFEL_BUILD, s);
+  k_surfel_build<<<(unsigned)((n_pix + 255) / 256), 256, 0, s>>>(out.range, reinterpret_cast<const float4*>(out.vertex),
+                                                                 out.intensity, out.normal, n_pix, B,
+                                                                 reinterpret_cast<float4*>(d_surfels));
+  prof_mark(h, PROF_SURFEL_BUILD, s);
+  OVN_LAUNCH_CHECK(h);
+  return OVN_OK;
+}
+
+// Reads and checks the host tables (nothing is launched on a refusal), uploads the entry table to d_render, and
+// z-buffers each image's entries' surfels (k_surfel_scatter) before the projection's gather reads the winners.
+static int render_surfels(ovn_handle* h, const float* d_surfels, int n_clouds, const double* d_rays, int n_virtual,
+                          const int64_t* h_entry_offsets, const int32_t* h_entry_cloud, const double* h_entry_pose,
+                          int max_splat, float max_range, const GatherOut& out, cudaStream_t s) {
+  if (n_virtual > h->cfg.max_batch_scans)
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "n_virtual=%d exceeds max_batch_scans=%d", n_virtual, h->cfg.max_batch_scans);
+  if (n_virtual <= 0) return OVN_OK;
+  const int64_t HW = (int64_t)h->cfg.proj_H * h->cfg.proj_W;
+  if (h_entry_offsets[0] != 0) OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render_surfels: h_entry_offsets[0] must be 0");
+  for (int v = 0; v < n_virtual; ++v) {
+    if (h_entry_offsets[v + 1] < h_entry_offsets[v])
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render_surfels: h_entry_offsets decreases at image %d", v);
+    // the key's index field holds (entry ordinal) H W + slot
+    if ((h_entry_offsets[v + 1] - h_entry_offsets[v]) * HW >= (int64_t(1) << 32))
+      OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render_surfels: image %d has %lld entries, 2^32 / (H W) or more", v,
+                  (long long)(h_entry_offsets[v + 1] - h_entry_offsets[v]));
+  }
+  const int64_t n_entries = h_entry_offsets[n_virtual];
+  if (n_entries >= INT32_MAX) OVN_SET_ERR(h, OVN_ERR_CAPACITY, "render_surfels: %lld entries", (long long)n_entries);
+  const int64_t n_items = n_entries * HW;
+  if (n_items > (int64_t)INT32_MAX * 256)
+    OVN_SET_ERR(h, OVN_ERR_CAPACITY, "render_surfels: %lld surfel slots in one call exceed the scatter grid",
+                (long long)n_items);
+  std::vector<RenderEntry> ent((size_t)n_entries);
+  for (int v = 0; v < n_virtual; ++v) {
+    for (int64_t e = h_entry_offsets[v]; e < h_entry_offsets[v + 1]; ++e) {
+      const int32_t c = h_entry_cloud[e];
+      if (c < 0 || c >= n_clouds)
+        OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render_surfels: entry %lld names cloud %d, outside [0, %d)", (long long)e,
+                    c, n_clouds);
+      const double* M = h_entry_pose + 16 * e;
+      for (int i = 0; i < 16; ++i)
+        if (!std::isfinite(M[i]))
+          OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render_surfels: the pose of entry %lld is not finite", (long long)e);
+      if (M[12] != 0.0 || M[13] != 0.0 || M[14] != 0.0 || M[15] != 1.0)
+        OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render_surfels: the pose of entry %lld does not end in the row 0 0 0 1",
+                    (long long)e);
+      RenderEntry& E = ent[(size_t)e];
+      memcpy(E.M, M, sizeof(E.M));
+      E.cloud_start = (int64_t)c * HW;
+      E.image_base = h_entry_offsets[v];
+      E.image = v;
+      E.pad = 0;
+    }
+  }
+  if (n_entries > 0 && (d_surfels == nullptr || d_rays == nullptr))
+    OVN_SET_ERR(h, OVN_ERR_INVALID_ARG, "render_surfels: d_surfels or d_rays is NULL");
+  const size_t b_ent = ent.size() * sizeof(RenderEntry), b_first = (size_t)(n_virtual + 1) * sizeof(int64_t);
+  std::vector<uint8_t> table(b_ent + b_first);
+  if (b_ent) memcpy(table.data(), ent.data(), b_ent);
+  memcpy(table.data() + b_ent, h_entry_offsets, b_first);
+  int rc = h->d_render.ensure(h, table.size());
+  if (rc != OVN_OK) return rc;
+  // pageable source: the copy is staged before the call returns, after the stream's earlier work
+  OVN_CUDA(h, cudaMemcpyAsync(h->d_render, table.data(), table.size(), cudaMemcpyHostToDevice, s));
+  const ProjParams P = make_params(h, max_range < 0 ? h->cfg.max_range : max_range);
+  const double pi = 3.14159265358979323846;
+  const double fov = fabs((double)h->cfg.fov_down_deg / 180.0 * pi) + fabs((double)h->cfg.fov_up_deg / 180.0 * pi);
+  SurfelHits src;
+  src.R.surfels = reinterpret_cast<const float4*>(d_surfels);
+  src.R.ent = reinterpret_cast<const RenderEntry*>(h->d_render.get());
+  src.R.first = reinterpret_cast<const int64_t*>(h->d_render.get() + b_ent);
+  src.R.rays = d_rays;
+  src.R.rows_per_rad = P.H / fov;
+  src.R.cols_per_rad = P.W / (2.0 * pi);
+  src.R.S = max_splat;
+  src.HW = (int)HW;
+  src.W = P.W;
+  OVN_CUDA(h, cudaMemsetAsync(h->d_keys, 0xFF, (size_t)n_virtual * HW * sizeof(unsigned long long), s));
+  if (n_items > 0) {
+    prof_mark(h, PROF_SURFEL_SCATTER, s);
+    k_surfel_scatter<<<(unsigned)((n_items + 255) / 256), 256, 0, s>>>(src.R, n_items, P, h->d_keys);
+    prof_mark(h, PROF_SURFEL_SCATTER, s);
+    OVN_LAUNCH_CHECK(h);
+  }
+  dim3 grid((P.W + TILE_C - 1) / TILE_C, (P.H + TILE_R - 1) / TILE_R, n_virtual);
+  prof_mark(h, PROF_SURFEL_GATHER, s);
+  k_project_gather<false, SurfelHits><<<grid, 256, 0, s>>>(src, P, h->d_keys, nullptr, nullptr, out);
+  prof_mark(h, PROF_SURFEL_GATHER, s);
+  OVN_LAUNCH_CHECK(h);
+  return OVN_OK;
+}
+
+int render_surfels_batch(ovn_handle* h, const float* d_surfels, int n_clouds, const double* d_rays, int n_virtual,
+                         const int64_t* h_entry_offsets, const int32_t* h_entry_cloud, const double* h_entry_pose,
+                         const ovn_surfel_params& prm, float max_range, float* d_range, float* d_vertex,
+                         float* d_intensity, int32_t* d_winner, cudaStream_t s) {
+  GatherOut out = {};
+  out.range = d_range; out.vertex = d_vertex; out.intensity = d_intensity; out.idx = d_winner;
+  out.c_depth = out.c_normal = out.c_prob = out.c_intensity = -1;
+  return render_surfels(h, d_surfels, n_clouds, d_rays, n_virtual, h_entry_offsets, h_entry_cloud, h_entry_pose,
+                        prm.max_splat, max_range, out, s);
+}
+
+int render_surfels_preprocess_batch(ovn_handle* h, const float* d_surfels, int n_clouds, const double* d_rays,
+                                    int n_virtual, const int64_t* h_entry_offsets, const int32_t* h_entry_cloud,
+                                    const double* h_entry_pose, const ovn_surfel_params& prm, float* d_input,
+                                    cudaStream_t s) {
+  if (h->cfg.n_prob_channels > 0)
+    OVN_SET_ERR(h, OVN_ERR_BAD_CONFIG,
+                "render_surfels_preprocess: the handle has probability channels, which renders lack");
+  return render_surfels(h, d_surfels, n_clouds, d_rays, n_virtual, h_entry_offsets, h_entry_cloud, h_entry_pose,
+                        prm.max_splat, h->cfg.max_range, packed_channels(h, nullptr, d_input), s);
 }
 
 int normals_batch(ovn_handle* h, const float* d_range, const float* d_vertex, int n_scans,

@@ -377,6 +377,88 @@ class Engine:
           _ptr(out[v0:v1]), self._stream()), 'ovn_render_preprocess_batch')
     return out
 
+  def surfel_params(self, params=None):
+    """ovn_surfel_params: ovn_surfel_default_params (kappa 1, c_min 0.5, max_splat 8, from a synthetic study and not
+    tuned on KITTI) with the keys of the ``params`` dict overriding them."""
+    prm = _cabi.SurfelParams()
+    lib().ovn_surfel_default_params(C.byref(prm))
+    for k, v in dict(params or {}).items():
+      if k not in ('kappa', 'c_min', 'max_splat'):
+        raise ValueError('unknown surfel parameter %r (kappa, c_min, max_splat)' % (k,))
+      setattr(prm, k, int(v) if k == 'max_splat' else float(v))
+    return prm
+
+  def pixel_rays(self):
+    """The float64 unit directions [H, W, 3] of the pixel centres at the handle's geometry (virtual_map.pixel_rays), on
+    the device; built once per engine."""
+    if getattr(self, '_rays', None) is None:
+      from .virtual_map import pixel_rays
+      self._rays = torch.from_numpy(pixel_rays(self.H, self.W, self.cfg.fov_up_deg, self.cfg.fov_down_deg)).to(
+          self.device)
+    return self._rays
+
+  def surfels(self, batch, params=None, out=None):
+    """ovn_surfels_batch: the surfel banks [n, H, W, 8] float32 of the clouds of a CloudBatch, one slot per pixel of
+    their projections: (cx, cy, cz, r, nx, ny, nz, intensity), all zero where the pixel is empty.  Calls of
+    max_batch_scans clouds; ``out``: an optional float32 tensor of that shape to write."""
+    if out is None:
+      out = torch.empty((batch.n, self.H, self.W, _cabi.SURFEL_FLOATS), dtype=torch.float32, device=self.device)
+    assert out.dtype == torch.float32 and tuple(out.shape) == (batch.n, self.H, self.W, _cabi.SURFEL_FLOATS) \
+        and out.is_contiguous()
+    prm = self.surfel_params(params)
+    L = lib()
+    for s0, s1, p0, p1, pts, offs in self._chunks(batch):
+      check(self._h, L.ovn_surfels_batch(self._h, _ptr(pts), _ptr(offs), s1 - s0, p1 - p0, C.byref(prm),
+                                         _ptr(out[s0:s1]), self._stream()), 'ovn_surfels_batch')
+    return out
+
+  def _surfel_bank(self, surfels):
+    assert surfels.dtype == torch.float32 and surfels.is_contiguous() and \
+        tuple(surfels.shape[1:]) == (self.H, self.W, _cabi.SURFEL_FLOATS), 'surfels: [n, H, W, 8] float32 expected'
+    return int(surfels.shape[0])
+
+  def render_surfels(self, surfels, entry_offsets, entry_cloud, entry_pose, params=None, max_range=-1.0,
+                     want=('range', 'vertex', 'intensity', 'winner')):
+    """ovn_render_surfels_batch: range images of virtual frames z-buffered from surfel banks (``surfels`` [n, H, W, 8],
+    Engine.surfels), with render's entry tables: entry e is bank entry_cloud[e] moved by entry_pose[e].  ``winner`` is
+    each pixel's (entry ordinal in its frame) H W + slot, -1 where empty.  ``params``: as surfel_params (only
+    max_splat is read here).  Calls of max_batch_scans frames."""
+    n = int(np.asarray(entry_offsets).reshape(-1).shape[0]) - 1
+    n_clouds = self._surfel_bank(surfels)
+    dev = self.device
+    out = {}
+    if 'range' in want: out['range'] = torch.empty((n, self.H, self.W), dtype=torch.float32, device=dev)
+    if 'vertex' in want: out['vertex'] = torch.empty((n, self.H, self.W, 4), dtype=torch.float32, device=dev)
+    if 'intensity' in want: out['intensity'] = torch.empty((n, self.H, self.W), dtype=torch.float32, device=dev)
+    if 'winner' in want: out['winner'] = torch.empty((n, self.H, self.W), dtype=torch.int32, device=dev)
+    prm = self.surfel_params(params)
+    rays = self.pixel_rays()
+    L = lib()
+    for v0, v1, eo, ec, ep in self._render_chunks(None, entry_offsets, entry_cloud, entry_pose):
+      sl = {k: v[v0:v1] for k, v in out.items()}
+      check(self._h, L.ovn_render_surfels_batch(
+          self._h, _ptr(surfels), n_clouds, _ptr(rays), v1 - v0, self._hp(eo), self._hp(ec), self._hp(ep),
+          C.byref(prm), float(max_range), _ptr(sl.get('range')), _ptr(sl.get('vertex')), _ptr(sl.get('intensity')),
+          _ptr(sl.get('winner')), self._stream()), 'ovn_render_surfels_batch')
+    return out
+
+  def render_surfels_preprocess(self, surfels, entry_offsets, entry_cloud, entry_pose, params=None, out=None):
+    """ovn_render_surfels_preprocess_batch: the surfel render's packed NHWC network input [n_virtual, H, W, C], as
+    preprocess packs a projection (``out``: an optional float32 tensor of that shape to write)."""
+    n = int(np.asarray(entry_offsets).reshape(-1).shape[0]) - 1
+    n_clouds = self._surfel_bank(surfels)
+    if out is None:
+      out = torch.empty((n, self.H, self.W, self.C), dtype=torch.float32, device=self.device)
+    assert out.dtype == torch.float32 and tuple(out.shape) == (n, self.H, self.W, self.C) and out.is_contiguous()
+    prm = self.surfel_params(params)
+    rays = self.pixel_rays()
+    L = lib()
+    for v0, v1, eo, ec, ep in self._render_chunks(None, entry_offsets, entry_cloud, entry_pose):
+      check(self._h, L.ovn_render_surfels_preprocess_batch(
+          self._h, _ptr(surfels), n_clouds, _ptr(rays), v1 - v0, self._hp(eo), self._hp(ec), self._hp(ep),
+          C.byref(prm), _ptr(out[v0:v1]), self._stream()), 'ovn_render_surfels_preprocess_batch')
+    return out
+
   def pack_input(self, depth=None, normal=None, prob=None, intensity=None):
     first = next(t for t in (depth, normal, prob, intensity) if t is not None)
     n = first.shape[0]

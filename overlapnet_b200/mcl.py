@@ -3,7 +3,8 @@ network's overlap and yaw as the observation model and the particle filter on th
 
   python -m overlapnet_b200.mcl [config/demo.yml] [--keyframe-stride S] [--particles N] [--runs R]
                                 [--sigma-overlap 0.1] [--sigma-yaw-deg 10] [--cell 0.5] [--max-distance 5]
-                                [--converged-m 2] [--virtual-spacing G [--render-sources 8] [--render-radius R]]
+                                [--converged-m 2] [--virtual-spacing G [--render-sources 8] [--render-radius R]
+                                [--render surfels [--surfel-kappa 1] [--max-splat 8]]]
 
 The model:
   map         K keyframes, each a scan encoded once (Infer.encode_clouds), calibrated on keyframe 0 and kept
@@ -13,7 +14,8 @@ The model:
   virtual     with a virtual spacing G, the map frames are instead the points of a G-metre lattice within
               max_distance of the keyframes (virtual_map.lattice), each rendered on the GPU from its M nearest
               keyframe clouds within the render radius and encoded; the raster holds the nearest lattice frame
-              within G of each cell centre.
+              within G of each cell centre.  ``--render surfels`` renders them from the keyframes' surfels (oriented
+              disks, DESIGN.md section 7, "Surfel renders") instead of their points.
   particles   (x, y, theta) with a log-weight, float64, on the device (Engine.mcl_*).
   step        predict (odometry + noise, raster lookup, the touched keyframes listed on the device), the heads on
               LEFT = touched keyframes, RIGHT = the query (ovn_heads_1vsN), update (likelihood, normalisation,
@@ -35,7 +37,7 @@ import sys
 import numpy as np
 import torch
 
-from ._cabi import OvnError
+from ._cabi import SURFEL_MAX_SPLAT, OvnError
 
 logger = logging.getLogger('overlapnet_b200.mcl')
 
@@ -130,13 +132,14 @@ class OverlapMCL:
 
   With ``virtual_spacing`` G, the map frames are the lattice frames of virtual_map.lattice(map_poses, G,
   max_distance), rendered from their ``render_sources`` nearest keyframe clouds within ``render_radius`` (default:
-  the handle's max_range); the raster is MapIndex(lattice xy, cell, max_distance=G).  ``keyframes`` holds the map
-  frames' planar poses either way."""
+  the handle's max_range); the raster is MapIndex(lattice xy, cell, max_distance=G).  ``render`` 'surfels' renders
+  the lattice frames from the keyframes' surfels, with ``surfel_params`` (a dict overriding Engine.surfel_params's
+  defaults).  ``keyframes`` holds the map frames' planar poses either way."""
 
   def __init__(self, infer, map_clouds, map_poses, cell=DEFAULTS['cell'], max_distance=DEFAULTS['max_distance'],
                sigma_overlap=DEFAULTS['sigma_overlap'], sigma_yaw=math.radians(DEFAULTS['sigma_yaw_deg']),
                rho=DEFAULTS['rho'], motion_sigma=DEFAULTS['motion_sigma'], virtual_spacing=None,
-               render_sources=DEFAULTS['render_sources'], render_radius=None):
+               render_sources=DEFAULTS['render_sources'], render_radius=None, render='points', surfel_params=None):
     from .lcd_eval import encode_share
     self.infer = infer
     self.engine = infer._engine
@@ -147,6 +150,11 @@ class OverlapMCL:
     self.virtual_spacing = None if virtual_spacing is None else float(virtual_spacing)
     self.sigma_overlap, self.sigma_yaw, self.rho = float(sigma_overlap), float(sigma_yaw), float(rho)
     self.motion_sigma = tuple(float(s) for s in motion_sigma)
+    if render not in ('points', 'surfels'):
+      raise ValueError("render must be 'points' or 'surfels', got %r" % (render,))
+    if render == 'surfels' and self.virtual_spacing is None:
+      raise ValueError("render='surfels' needs a virtual_spacing: keyframe maps are not rendered")
+    self.render = render
     if self.virtual_spacing is None:
       self.keyframes = planar(map_poses)
       self.index = MapIndex(self.keyframes[:, :2], cell, max_distance)
@@ -160,7 +168,13 @@ class OverlapMCL:
       frames = virtual_map.lattice(map_poses, self.virtual_spacing, max_distance)
       self.keyframes = planar(frames)
       self.index = MapIndex(self.keyframes[:, :2], cell, self.virtual_spacing)
-      bank = virtual_map.encode(infer, map_clouds, map_poses, frames, self.render_sources, self.render_radius)
+      surfels = None
+      if render == 'surfels':
+        prm = self.engine.surfel_params(surfel_params)
+        self.surfel_params = dict(kappa=prm.kappa, c_min=prm.c_min, max_splat=prm.max_splat)
+        surfels = self.surfel_params
+      bank = virtual_map.encode(infer, map_clouds, map_poses, frames, self.render_sources, self.render_radius,
+                                surfels=surfels)
     # the tensor-core heads' numeric centres from keyframe 0, before the operand copies are built (as lcd_eval)
     self.engine.calibrate(bank[0])
     infer._set_bank(bank)
@@ -280,6 +294,9 @@ def evaluate_sequence(infer, clouds, poses, keyframe_stride=5, particles=100000,
   if mcl.virtual_spacing is not None:
     summary.update(virtual_spacing=mcl.virtual_spacing, render_sources=mcl.render_sources,
                    render_radius=mcl.render_radius, map_frames=int(mcl.keyframes.shape[0]))
+    if mcl.render == 'surfels':
+      summary.update(render='surfels', surfel_kappa=mcl.surfel_params['kappa'],
+                     surfel_c_min=mcl.surfel_params['c_min'], surfel_max_splat=mcl.surfel_params['max_splat'])
     results['map_frames'] = mcl.keyframes
   if out_dir is not None:
     os.makedirs(out_dir, exist_ok=True)
@@ -312,6 +329,13 @@ def parse_args(argv):
                       % (MAX_RENDER_SOURCES, DEFAULTS['render_sources']))
   p.add_argument('--render-radius', type=float, default=None,
                  help='metres from a virtual frame a rendered keyframe may be (default: the max_range)')
+  p.add_argument('--render', default='points', choices=('points', 'surfels'),
+                 help='render the virtual scans from the keyframes\' points or surfels (default points; needs '
+                      '--virtual-spacing)')
+  p.add_argument('--surfel-kappa', type=float, default=None,
+                 help='surfel radius scale, > 0 (default 1, from a synthetic study; not tuned on KITTI)')
+  p.add_argument('--max-splat', type=int, default=None,
+                 help='pixels a surfel may cover on each side of its centre, 0..%d (default 8)' % SURFEL_MAX_SPLAT)
   args = p.parse_args(argv)
   if args.keyframe_stride < 2:
     p.error('--keyframe-stride must be at least 2, got %d' % args.keyframe_stride)
@@ -330,6 +354,14 @@ def parse_args(argv):
     p.error('--render-sources must be in [1, %d], got %d' % (MAX_RENDER_SOURCES, args.render_sources))
   if args.render_radius is not None and not (args.render_radius > 0 and math.isfinite(args.render_radius)):
     p.error('--render-radius must be > 0')
+  if args.render == 'surfels' and args.virtual_spacing is None:
+    p.error('--render surfels needs --virtual-spacing')
+  if (args.surfel_kappa is not None or args.max_splat is not None) and args.render != 'surfels':
+    p.error('--surfel-kappa and --max-splat need --render surfels')
+  if args.surfel_kappa is not None and not (args.surfel_kappa > 0 and math.isfinite(args.surfel_kappa)):
+    p.error('--surfel-kappa must be > 0')
+  if args.max_splat is not None and not 0 <= args.max_splat <= SURFEL_MAX_SPLAT:
+    p.error('--max-splat must be in [0, %d], got %d' % (SURFEL_MAX_SPLAT, args.max_splat))
   return args
 
 
@@ -337,8 +369,12 @@ def virtual_args(args):
   """OverlapMCL's virtual-map arguments of the parsed command line: none without --virtual-spacing."""
   if args.virtual_spacing is None:
     return {}
-  return dict(virtual_spacing=args.virtual_spacing, render_sources=args.render_sources,
-              render_radius=args.render_radius)
+  out = dict(virtual_spacing=args.virtual_spacing, render_sources=args.render_sources,
+             render_radius=args.render_radius)
+  if args.render == 'surfels':
+    prm = {k: v for k, v in (('kappa', args.surfel_kappa), ('max_splat', args.max_splat)) if v is not None}
+    out.update(render='surfels', surfel_params=prm)
+  return out
 
 
 def network_config(config):

@@ -6,7 +6,12 @@ clouds around each point, and encoded by the leg into a resident bank (DESIGN.md
   entries   for each virtual frame, its m nearest keyframes within radius (by ascending planar distance, then index),
             each moved into the frame by inv(T_v) T_k, composed in NumPy float64.
   encode    the keyframe clouds uploaded once; ovn_render_preprocess_batch and the leg in chunks of max_batch_scans
-            frames, giving the device bank [V, 360, 128]."""
+            frames, giving the device bank [V, 360, 128].  With ``surfels``, the keyframes' surfel banks are built
+            in chunks of max_batch_scans keyframes and the frames rendered from them
+            (ovn_render_surfels_preprocess_batch, DESIGN.md section 7, "Surfel renders").
+  pixel_rays  the float64 unit directions of the pixel centres that the surfel render intersects."""
+import math
+
 import numpy as np
 import torch
 
@@ -86,32 +91,65 @@ def entries(virtual_poses, keyframe_poses, m, radius):
           np.asarray(poses, np.float64).reshape(-1, 4, 4))
 
 
-def bank_bytes(engine, n):
+def pixel_rays(H, W, fov_up, fov_down):
+  """[H, W, 3] float64: u[y][x] the unit direction whose projection's pre-floor values (utils.py:86-95) are
+  (x + 1/2, y + 1/2): azimuth pi (1 - 2 (x + 1/2) / W), pitch (1 - (y + 1/2) / H) fov - |fov_down|, u = (cos p cos a,
+  cos p sin a, sin p).  Built with math.sin / math.cos (libm), one value at a time, so that every caller gets the same
+  table."""
+  fu = float(fov_up) / 180.0 * math.pi
+  fd = float(fov_down) / 180.0 * math.pi
+  fov = abs(fd) + abs(fu)
+  az = [math.pi * (1.0 - 2.0 * (x + 0.5) / W) for x in range(W)]
+  ca, sa = [math.cos(a) for a in az], [math.sin(a) for a in az]
+  out = np.empty((H, W, 3), np.float64)
+  for y in range(H):
+    p = (1.0 - (y + 0.5) / H) * fov - abs(fd)
+    cp, sp = math.cos(p), math.sin(p)
+    out[y, :, 0] = [cp * c for c in ca]
+    out[y, :, 1] = [cp * s for s in sa]
+    out[y, :, 2] = sp
+  return out
+
+
+def bank_bytes(engine, n, n_surfel_banks=0):
   """Device bytes of a resident bank of ``n`` volumes: float32 [n, 360, 128], and on a tensor-core handle the
-  operand copies ovn_bank_prepare keeps per row (an fp16 [360][128] copy, six 32 KB correlation tiles, a flag)."""
+  operand copies ovn_bank_prepare keeps per row (an fp16 [360][128] copy, six 32 KB correlation tiles, a flag); plus
+  ``n_surfel_banks`` keyframe surfel banks of [H, W, 8] float32 (1.84 MB at 64 x 900)."""
   row = engine.Wf * FEAT_C * 4
   if engine.precision == 'f16_tc':
     row += engine.Wf * FEAT_C * 2 + 6 * 32768 + 4
-  return int(n) * row
+  return int(n) * row + int(n_surfel_banks) * engine.H * engine.W * 8 * 4
 
 
-def encode(infer, clouds, keyframe_poses, virtual_poses, m, radius):
+def encode(infer, clouds, keyframe_poses, virtual_poses, m, radius, surfels=None):
   """The feature volumes [V, 360, 128] (device) of the virtual frames at ``virtual_poses``, rendered from their m
-  nearest keyframe clouds within ``radius`` (``clouds``: (N, 4) float32 arrays or callables returning one).  Refused
-  before anything is rendered when the bank and its tensor-core copies do not fit in the device's free memory."""
+  nearest keyframe clouds within ``radius`` (``clouds``: (N, 4) float32 arrays or callables returning one).  With
+  ``surfels`` (a dict of surfel parameters, Engine.surfel_params; {} for the defaults) the frames are rendered from
+  the keyframes' surfels instead of their points.  Refused before anything is rendered when the bank, its
+  tensor-core copies and the keyframes' surfel banks do not fit in the device's free memory."""
   eng = infer._engine
   vp = np.asarray(virtual_poses, np.float64).reshape(-1, 4, 4)
   kp = np.asarray(keyframe_poses, np.float64).reshape(-1, 4, 4)
   if len(clouds) != kp.shape[0]:
     raise ValueError('%d keyframe clouds for %d keyframe poses' % (len(clouds), kp.shape[0]))
   V = vp.shape[0]
-  need = bank_bytes(eng, V)
+  if surfels is not None:
+    eng.surfel_params(surfels)                                   # unknown keys are refused before anything runs
+  need = bank_bytes(eng, V, 0 if surfels is None else kp.shape[0])
   free, _ = torch.cuda.mem_get_info(eng.device)
   if need > free:
-    raise MemoryError('virtual map: the bank of %d frames needs %d bytes (float32 and tensor-core copies), but the '
-                      'device has %d bytes free' % (V, need, free))
+    raise MemoryError('virtual map: the bank of %d frames needs %d bytes (float32 and tensor-core copies%s), but the '
+                      'device has %d bytes free' % (V, need, '' if surfels is None else ', keyframe surfels', free))
   eo, ec, ep = entries(vp, kp, m, radius)
-  batch = eng.upload_clouds([np.ascontiguousarray(c() if callable(c) else c, np.float32) for c in clouds])
+  load = lambda c: np.ascontiguousarray(c() if callable(c) else c, np.float32)
+  if surfels is None:
+    batch = eng.upload_clouds([load(c) for c in clouds])
+  else:
+    # the surfel banks from max_batch_scans keyframe clouds at a time: no more clouds on the device at once
+    src = torch.empty((kp.shape[0], eng.H, eng.W, 8), dtype=torch.float32, device=eng.device)
+    for k0 in range(0, kp.shape[0], eng.max_batch_scans):
+      k1 = min(kp.shape[0], k0 + eng.max_batch_scans)
+      eng.surfels(eng.upload_clouds([load(c) for c in clouds[k0:k1]]), surfels, out=src[k0:k1])
   bank = torch.empty((V, eng.Wf, FEAT_C), dtype=torch.float32, device=eng.device)
   x = None
   for v0 in range(0, V, eng.max_batch_scans):
@@ -119,6 +157,9 @@ def encode(infer, clouds, keyframe_poses, virtual_poses, m, radius):
     e0, e1 = int(eo[v0]), int(eo[v1])
     if x is None or x.shape[0] != v1 - v0:
       x = torch.empty((v1 - v0, eng.H, eng.W, eng.C), dtype=torch.float32, device=eng.device)
-    eng.render_preprocess(batch, eo[v0:v1 + 1] - e0, ec[e0:e1], ep[e0:e1], out=x)
+    if surfels is None:
+      eng.render_preprocess(batch, eo[v0:v1 + 1] - e0, ec[e0:e1], ep[e0:e1], out=x)
+    else:
+      eng.render_surfels_preprocess(src, eo[v0:v1 + 1] - e0, ec[e0:e1], ep[e0:e1], surfels, out=x)
     eng.leg(x, out=bank[v0:v1])
   return bank
